@@ -16,8 +16,8 @@ Other named configs, one JSON line each, same timing rules (`--workload`):
   value : samples/s with the step's inputs already resident in HBM (CUDA-event timed, max over ranks)
   e2e   : the same through the public module API with HOST (pinned) inputs: H2D of ids/masks/features and a
           D2H read of the loss inside the timed region
-  roofline     : dominant kernel (the tcgen05 GEMM at the workload's FFN-up shape) timed alone with CUDA events,
-                 algorithmic FLOPs / duration vs MEASURED_PEAKS.json bf16 peak; `traffic` from the kept ncu capture
+  roofline     : dominant kernel (the wgmma GEMM at the workload's FFN-up shape) timed alone with CUDA events,
+                 algorithmic FLOPs / duration vs MEASURED_PEAKS.json bf16 peak, else the H100 SXM data sheet
   roofline_hbm : the largest HBM-bound kernel (fused LayerNorm backward) timed alone, algorithmic bytes / duration vs the
                  measured copy bandwidth
   parity       : before timing, the model in eval mode on a small batch against the CPU arm with the SAME weights
@@ -540,7 +540,7 @@ def _init_ref(m):
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle sampling during the timed region (B200_PROFILING.md)"""
+    """nvidia-smi clock / throttle sampling during the timed region (read-only queries)"""
 
     def __init__(self, index):
         self.rows, self.proc, self.index = [], None, index
@@ -586,8 +586,9 @@ def peaks():
     if os.path.exists(path):
         with open(path) as fh:
             d = json.load(fh)
-        return d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured"
-    return 1590.0, 1400.0, 6650.0, "fallback"
+        return d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured"
+    # H100 SXM data sheet (dense bf16, HBM3) at 700 W: upper bounds, not rates this card has been measured to reach
+    return 989.0, 989.0, 3350.0, "H100 SXM data sheet"
 
 
 def usable_cores():
@@ -683,19 +684,29 @@ def _forward_outputs(wl, model, batch):
     raise RuntimeError("no output hook for %s" % wl.name)
 
 
-def kept_traffic(wl_name, B):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel from the kept `ncu --set full` capture
-    (profiles/dominant_traffic.json, written by tools/ncu_traffic.py from the .ncu-rep): only for the batch it was taken at"""
-    path = os.path.join(ROOT, "profiles", "dominant_traffic.json")
-    try:
-        with open(path) as fh:
-            d = json.load(fh)
-        e = d.get(wl_name)
-        if e and int(e.get("batch", -1)) == int(B):
-            return float(e["dram_bytes_read"]) + float(e["dram_bytes_write"]), e.get("source")
-    except Exception:
-        pass
-    return None, None
+def dump_outputs(out_dir, model, loss, per_tensor=8192, max_bytes=64 << 20):
+    """The step's results as a caller receives them: the loss (float64) and every parameter gradient (float32).  A gradient
+    larger than `per_tensor` elements is sampled at the sorted indices torch.randint(0, numel, (per_tensor,)) draws from a
+    CPU generator seeded with zlib.crc32(<parameter name>), so two dumps hold the same elements; at most `max_bytes` in
+    all (parameters past the cap are left out, in a fixed order)."""
+    import zlib
+
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss.detach().double())], dtype=np.float64))
+    total = 8
+    for name, p in model.named_parameters():
+        if p.grad is None:
+            continue
+        flat = p.grad.detach().reshape(-1).float().cpu()
+        if flat.numel() > per_tensor:
+            gen = torch.Generator().manual_seed(zlib.crc32(name.encode()))
+            flat = flat[torch.randint(0, flat.numel(), (per_tensor,), generator=gen).sort().values]
+        if total + 4 * flat.numel() > max_bytes:
+            break
+        total += 4 * flat.numel()
+        np.save(os.path.join(out_dir, "grad." + name + ".npy"), flat.numpy().astype(np.float32))
 
 
 def main():
@@ -721,12 +732,16 @@ def main():
     ap.add_argument("--graph", dest="graph", action="store_true", default=None,
                     help="replay the step (forward + backward) as ONE CUDA graph (mmf_b200.graphs.GraphedStep): the same C-ABI "
                          "launches recorded by stream capture.  Default: on for a single GPU and the workloads it has been "
-                         "validated with (visual_bert, mmbt, vilbert) - ~430 launches of ~45 us host time each are 19 ms per "
-                         "step, which a slow host CPU cannot hide behind a 26 ms step (seen as e2e 5530 against value 6323 on "
-                         "one lease); single GPU only")
+                         "validated with (visual_bert, mmbt, vilbert): hundreds of launches per step cost tens of "
+                         "microseconds of host time each, which a slow host CPU cannot hide; single GPU only")
     ap.add_argument("--no-graph", dest="graph", action="store_false", help="launch every kernel of the step eagerly")
-    ap.add_argument("--profile", action="store_true", help="device-resident steps only (for ncu launch lists)")
+    ap.add_argument("--profile", action="store_true", help="device-resident steps only (timed steps without the extras)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (its loss and a fixed, seeded "
+                         "sample of every parameter gradient) as DIR/<name>.npy, so that two builds can be compared")
     args = ap.parse_args()
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs at least one timed step (--steps >= 1)")
 
     wl = WORKLOADS[args.workload]()
     if args.graph is None:
@@ -742,12 +757,12 @@ def main():
     config = {"workload": wl.describe(), "workload_key": wl.name, "batch_per_gpu": B, "global_batch": B * max(world, 1),
               "seq_len": S, "dropout": args.dropout, "parallelism": "dp%d" % max(world, 1),
               "gflop_per_sample_fwd_bwd": step_flops / 1e9,
-              "l2_policy": "activations + weights touched per step exceed the 126 MB L2 at this batch"
+              "l2_policy": "activations + weights touched per step exceed the 50 MB L2 at this batch"
                            if B * S >= 8192 else "small batch: the working set fits L2; a 160 MB buffer is zeroed between "
                                                  "timed steps (L2 flush)"}
     if wl.name == "visual_bert":
-        config["batch_choice"] = ("166 samples x 228 tokens = 147.8 -> 148 pair tiles of 256 rows: every GEMM of the block is "
-                                  "an exact number of waves on 148 SMs (sweep in profiles/README.md)")
+        config["batch_choice"] = ("166 samples x 228 tokens = 37848 rows = 296 row tiles of 128: the FFN GEMMs (12 or 3 column "
+                                  "tiles of 256) fill 27 and 7 waves of 132 SMs almost exactly")
 
     if args.impl == "reference":
         if rank != 0:
@@ -837,7 +852,7 @@ def main():
     launches0 = lib.launch_count()
     barrier()
     if args.profile:
-        torch.cuda.profiler.start()    # ncu --profile-from-start off: capture exactly the timed steps
+        torch.cuda.profiler.start()    # an external profiler started with capture off records exactly the timed steps
     if small:
         # per-step events so that the L2 flush between steps stays outside the timed intervals
         evs = []
@@ -845,7 +860,7 @@ def main():
             flush.zero_()
             a, b_ = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
-            step(dev_batch)
+            last_loss = step(dev_batch)
             b_.record()
             evs.append((a, b_))
         barrier()
@@ -854,12 +869,14 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(args.steps):
-            step(dev_batch)
+            last_loss = step(dev_batch)
         e1.record()
         barrier()
         ms_total = e0.elapsed_time(e1)
     if args.profile:
         torch.cuda.profiler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, last_loss)
     launches = lib.launch_count() - launches0
     if args.graph:
         launches = graph_launches * args.steps      # replays do not pass through the C ABI: kernels recorded at capture x steps
@@ -957,7 +974,7 @@ def main():
                 if i >= skip:
                     ts.append(g0.elapsed_time(g1))
             return statistics.mean(ts)
-        # dominant kernel alone: the tcgen05 GEMM at the FFN-up shape [B*S, H] x [I, H]^T (+bias+GELU epilogue)
+        # dominant kernel alone: the wgmma GEMM at the FFN-up shape [B*S, H] x [I, H]^T (+bias+GELU epilogue)
         M, HID, INTER = B * S, wl.hidden, wl.inter
         a = torch.randn(M, HID, device=dev).to(torch.bfloat16)
         w = (torch.randn(INTER, HID, device=dev) * 0.02).to(torch.bfloat16)
@@ -967,11 +984,9 @@ def main():
         k_ms = time_alone(lambda: F.gemm(a, w, epi=lib.EPI_BIAS_GELU, bias=bias, out=o1, out2=o2))
         k_flops = 2.0 * M * HID * INTER
         achieved = k_flops / (k_ms * 1e-3) / 1e12
-        traffic, traffic_src = kept_traffic(wl.name, B)
         roofline = {"bound": "tensor", "kernel": "gemm_kernel<256,K-major,K-major,BIAS_GELU> FFN-up [%d,%d]x[%d,%d]^T" % (M, HID, INTER, HID),
                     "achieved": achieved, "peak": burst, "unit": "TFLOP/s", "frac": achieved / burst,
                     "peak_source": "%s bf16_tflops (burst: kernel timed alone)" % how,
-                    "traffic": traffic, "traffic_source": traffic_src,
                     "kernel_ms": k_ms, "flops_per_launch": k_flops,
                     "step_tflops": step_flops * value / 1e12 / world,
                     "step_frac_of_sustained": step_flops * value / 1e12 / world / sustained}
@@ -987,7 +1002,7 @@ def main():
         l_bytes = M * (8.0 * HID + HID / 8.0 + 8.0)
         roofline_hbm = {"bound": "hbm", "kernel": "layernorm_bwd (+dropout bwd, dgamma/dbeta/dbias) [%d,%d]" % (M, HID),
                         "achieved": l_bytes / (l_ms * 1e-3) / 1e9, "peak": hbm, "unit": "GB/s",
-                        "frac": l_bytes / (l_ms * 1e-3) / 1e9 / hbm, "peak_source": "%s hbm_gbs" % how, "traffic": None,
+                        "frac": l_bytes / (l_ms * 1e-3) / 1e9 / hbm, "peak_source": "%s hbm_gbs" % how,
                         "kernel_ms": l_ms, "bytes_per_launch": l_bytes}
         # fused AdamW over a flat fp32 buffer of this model's size: reads p, g, m, v and writes p, m, v (28 B / parameter)
         n_par = (sum(p_.numel() for p_ in model.parameters()) + 7) // 8 * 8

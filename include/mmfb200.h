@@ -1,4 +1,4 @@
-/* mmfb200.h - C ABI of the B200-native multimodal-fusion block (libmmfb200.so).
+/* mmfb200.h - C ABI of the H100-native (sm_90a) multimodal-fusion block (libmmfb200.so).
  *
  * The reference (facebookresearch/mmf) has no FFI for this path: the boundary is the Python-level
  * module contract of
@@ -17,7 +17,7 @@
  *     workspace); functions never allocate, never synchronise, enqueue on `stream` only
  *   - return value: 0 = ok, otherwise an mmfb_status; mmfb_last_error() gives the message of the
  *     last failure on the calling thread; no C++ exception crosses the ABI
- *   - there is no CPU fallback: without an sm_100 device every compute entry point fails
+ *   - there is no CPU fallback: without an sm_90 device every compute entry point fails
  */
 #ifndef MMFB200_H_
 #define MMFB200_H_
@@ -35,7 +35,7 @@ typedef enum {
   MMFB_OK = 0,
   MMFB_ERR_ARG = 1,     /* bad shape / alignment / null pointer  -> ValueError in the binding */
   MMFB_ERR_CUDA = 2,    /* CUDA runtime / driver failure         -> RuntimeError */
-  MMFB_ERR_DEVICE = 3   /* no sm_100 device                      -> RuntimeError */
+  MMFB_ERR_DEVICE = 3   /* no sm_90 device                       -> RuntimeError */
 } mmfb_status;
 
 /* epilogues of mmfb_gemm */
@@ -63,7 +63,7 @@ typedef struct {
   int epi;
   int splits;                    /* split-K factor, MMFB_EPI_ATOMIC_F32 only (0/1 = none) */
   int block_n;                   /* 0 = auto, else 128 or 256 */
-  int cluster;                   /* 0 = library default, 1 = single CTA, 2 = 2-CTA cluster sharing the B tile by TMA multicast */
+  int cluster;                   /* 0, 1 or 2; kept for ABI compatibility: every GEMM runs as single-CTA tiles */
 } mmfb_gemm_args;
 
 int mmfb_gemm(const mmfb_gemm_args* args, mmfb_stream stream);
@@ -222,7 +222,7 @@ int mmfb_adamw(const mmfb_adamw_args* args, mmfb_stream stream);
 /* library / diagnostics */
 const char* mmfb_last_error(void);
 int mmfb_version(void);
-int mmfb_device_ok(void);          /* 1 if the current device is sm_100 */
+int mmfb_device_ok(void);          /* 1 if the current device is sm_90 */
 int64_t mmfb_launch_count(void);   /* number of kernels this library has launched in this process */
 
 #ifdef __cplusplus

@@ -1,4 +1,4 @@
-"""mmf_b200 - B200-native (sm_100a) fusion block for MMF-style multimodal transformers.
+"""mmf_b200 - H100-native (sm_90a) fusion block for MMF-style multimodal transformers.
 
 Importing the package loads libmmfb200.so (building it in-tree with nvcc if missing) and fails loudly if that is
 impossible; there is no CPU fallback for any compute path.  See DESIGN.md / INTEGRATION.md.

@@ -1,26 +1,26 @@
-// Fused multi-head (self / cross) attention for the fusion block, forward and backward (sm_100a).
+// Fused multi-head (self / cross) attention for the fusion block, forward and backward (sm_90a).
 //
 // Reference semantics (mmf/modules/hf_layers.py:182-210; mmf/models/vilbert.py:81-103, 421-461):
 //     scores = Q K^T / sqrt(d) + M        M = additive mask [B, Skv] (0 / -10000), NOT -inf
 //     probs  = dropout(softmax(scores))   a fully masked row becomes uniform, never NaN
 //     ctx    = probs V, heads merged back to [B, Sq, h*d]
 //
-// Forward: one CTA per (128-query tile, head, batch).  TMA stages Q, K, V head slices straight out of
-// the fused [tokens, 3*H] projection buffer (3-D tensor maps: sequence tails are zero-filled, never read
-// from the next sample).  The whole score row block S = Q K^T [128 x Skv] lives in TMEM (Skv <= 384),
-// so softmax is a single exact pass: thread r owns TMEM lane r == query row r (no shuffles), exp2 with
-// the 1/sqrt(d) scale folded into log2(e).  P is written to shared memory as the K-major A operand of
-// the second tcgen05 contraction O = P V (V is consumed MN-major from the same TMA tile), P reusing the
-// bytes of Q and K.  Row log-sum-exp (log2 domain) is saved for the backward.
+// Every kernel works on 64-row tiles of one (batch, head): four warps, each owning 16 rows of the resident tile, and a
+// loop over 64-row blocks of the other sequence.  TMA stages the head slices straight out of the fused [tokens, 3*H]
+// projection buffers (3-D tensor maps: sequence tails are zero-filled, never read from the next sample) into
+// 128-byte-swizzled shared memory; the looped blocks go through a two-stage ring signalled by mbarriers, so the load of
+// block i+2 overlaps the math of block i+1.  The products run on the tensor cores with mma.sync m16n8k16 (bf16 in,
+// fp32 accumulate): operand fragments come from shared memory through ldmatrix (.trans for the operands that are
+// consumed along their rows), and a probability / gradient tile computed in registers is reused directly as the A
+// operand of the next product - the accumulator layout of two adjacent n8 tiles is the A layout of one k16 step.
 //
-// Backward: the probabilities are recomputed from Q, K and the saved row statistics (nothing of size
-// S x S ever touches HBM).  Two launches of ONE templated kernel:
-//   ROWS_ARE_Q = true : CTA owns 128 query rows, loops over key blocks,   dQ  = scale * dS K
-//   ROWS_ARE_Q = false: CTA owns 128 key rows,   loops over query blocks, dK^T-free formulation
-//                       S'^T = K Q^T, dP'^T = V dO^T,  dV = P^T dO,  dK = scale * dS^T Q
-// In both, thread r owns row r of the 128x128 S'/dP' tiles in TMEM, writes P'/dS' (bf16) to shared
-// memory as K-major A operands and the looped operand tile is re-read MN-major as the B operand of
-// the accumulation MMA - no transposes, no atomics, deterministic.
+// Forward: online softmax over the key blocks in the log2 domain (the 1/sqrt(d) scale folded into log2(e)); the row
+// log-sum-exp is saved for the backward.
+// Backward: the probabilities are recomputed from Q, K and the saved row statistics (nothing of size S x S ever touches
+// HBM).  Two kernels, no atomics, deterministic:
+//   dq kernel : CTA owns 64 query rows, loops over key blocks:    dQ = scale * dS K
+//   dkv kernel: CTA owns 64 key rows, loops over query blocks:    dV = P^T dO,  dK = scale * dS^T Q
+//               (computed as S^T = K Q^T and dP^T = V dO^T, so the key rows stay the rows of every register tile)
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -29,6 +29,68 @@
 namespace mmfb {
 
 constexpr float LOG2E = 1.4426950408889634f;
+constexpr int AT_ROWS = 64;       // rows of every staged tile
+constexpr int AT_THREADS = 128;   // four warps x 16 rows
+
+// byte offset of the 16-byte chunk holding column c (a multiple of 8) of row r in a staged tile: 64-column panels of
+// ROWS x 128 B, SWIZZLE_128B (chunk index XOR row % 8), as written by a TMA box {64, ROWS}
+template <int ROWS>
+__device__ __forceinline__ uint32_t tile_off(int r, int c) {
+  return (c >> 6) * (ROWS * 128) + r * 128 + ((((c >> 3) & 7) ^ (r & 7)) << 4);
+}
+
+// TMA of one [ROWS x D] head slice (D/64 boxes) into `dst`, credited to `bar`
+template <int D, int ROWS>
+__device__ __forceinline__ void load_tile(uint8_t* dst, const CUtensorMap* m, uint64_t* bar, int col0, int row0, int b) {
+#pragma unroll
+  for (int c = 0; c < D / 64; ++c) tma_load_3d(dst + c * ROWS * 128, m, bar, col0 + c * 64, row0, b);
+}
+
+// acc[16 x 8 NT] (+)= A[16 rows from r0 of tile a, D] * B[8 NT rows of tile b, D]^T   (both tiles K-major along D)
+template <int D, int NT, int AROWS, int BROWS>
+__device__ __forceinline__ void mma_abt(float (&acc)[NT][4], uint32_t a, int r0, uint32_t b, int lane) {
+  const int mi = lane >> 3, lr = lane & 7;
+#pragma unroll
+  for (int ks = 0; ks < D / 16; ++ks) {
+    uint32_t af[4];
+    ldsm_x4(af, a + tile_off<AROWS>(r0 + (mi & 1) * 8 + lr, ks * 16 + (mi >> 1) * 8));
+#pragma unroll
+    for (int np = 0; np < NT / 2; ++np) {
+      uint32_t bf[4];
+      ldsm_x4(bf, b + tile_off<BROWS>(np * 16 + (mi >> 1) * 8 + lr, ks * 16 + (mi & 1) * 8));
+      mma_bf16_16816(acc[2 * np], af, bf[0], bf[1]);
+      mma_bf16_16816(acc[2 * np + 1], af, bf[2], bf[3]);
+    }
+  }
+}
+
+// acc[16 x D] += P[16 x 16 KS] * B[16 KS rows of tile b, D]   (P: bf16 A fragments in registers, B consumed along rows)
+template <int D, int KS, int BROWS>
+__device__ __forceinline__ void mma_pb(float (&acc)[D / 8][4], const uint32_t (&pf)[KS][4], uint32_t b, int lane) {
+  const int mi = lane >> 3, lr = lane & 7;
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+#pragma unroll
+    for (int dp = 0; dp < D / 16; ++dp) {
+      uint32_t bf[4];
+      ldsm_x4_t(bf, b + tile_off<BROWS>(ks * 16 + (mi & 1) * 8 + lr, dp * 16 + (mi >> 1) * 8));
+      mma_bf16_16816(acc[2 * dp], pf[ks], bf[0], bf[1]);
+      mma_bf16_16816(acc[2 * dp + 1], pf[ks], bf[2], bf[3]);
+    }
+  }
+}
+
+// accumulator tile [16 x 8 NT] (fp32) -> bf16 A fragments of NT/2 k16 steps
+template <int NT>
+__device__ __forceinline__ void acc_to_a(const float (&c)[NT][4], uint32_t (&pf)[NT / 2][4]) {
+#pragma unroll
+  for (int k = 0; k < NT / 2; ++k) {
+    pf[k][0] = pack_bf16x2(c[2 * k][0], c[2 * k][1]);
+    pf[k][1] = pack_bf16x2(c[2 * k][2], c[2 * k][3]);
+    pf[k][2] = pack_bf16x2(c[2 * k + 1][0], c[2 * k + 1][1]);
+    pf[k][3] = pack_bf16x2(c[2 * k + 1][2], c[2 * k + 1][3]);
+  }
+}
 
 // ----------------------------------------------------------------------------------------------
 // forward
@@ -40,7 +102,7 @@ struct AttnFwdDev {
   int64_t ldo;
   bf16* ctx_lo;           // optional [B*Sq, H*D] (training): bf16(O - float(ctx)), the part of O the bf16 output drops.
                           // The backward's delta = rowsum(dO * (ctx + ctx_lo)): with the bf16 O alone every dS of a row
-                          // inherits the same rounding error (round 1: 4.5e-2 on q/k weight gradients of a 10-token case)
+                          // inherits the same rounding error
   float* lse2;            // [B, H, Sq]  log2-domain log-sum-exp of the scaled+masked scores
   const uint32_t* dmask;  // keep bits [B, H, Sq, W] (bit kv%32 of word kv/32) or null
   int W;
@@ -48,2148 +110,412 @@ struct AttnFwdDev {
   float scale2;           // log2(e)/sqrt(d)
 };
 
-// 288 threads: warps 0..7 = softmax / epilogue (TWO threads per query row: warp w owns TMEM lane quarter w & 3 and the
-// 32-column chunks of parity w >> 2; row max / sum are exchanged through shared memory), warp 8 = TMA + MMA issue.
+// grid (query tiles, heads, batch); smem: Q tile, two stages of (K block, V block), the key mask (log2 domain)
 template <int D>
-__global__ void __launch_bounds__(288, 2)
+__global__ void __launch_bounds__(AT_THREADS)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, AttnFwdDev p) {
-  griddep_launch();
-  griddep_wait();
-  constexpr int DC = D / 64;
+  constexpr int TB = D / 64 * AT_ROWS * 128;   // bytes of one staged tile
+  constexpr int DT = D / 8;                    // n8 tiles of the output
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
-  const int SK = (p.Skv + 63) & ~63;
-  const int NB = SK / 64;
-  const int r0_bytes = max(NB * 16384, DC * 16384 + DC * SK * 128);
-  uint8_t* sQ = smem;                      // DC x [128 x 128B]
-  uint8_t* sK = smem + DC * 16384;         // DC x [SK x 128B]
-  uint8_t* sP = smem;                      // NB x [128 x 128B]   (aliases Q and K once S is complete)
-  uint8_t* sV = smem + r0_bytes;           // DC x [SK x 128B]
-  float* sMask = reinterpret_cast<float*>(sV + DC * SK * 128);  // [SK]
-  float* sRed = sMask + SK;                                     // [2 stats][2 halves][128 rows]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sRed + 512);
-  uint64_t* qk_full = bars;
-  uint64_t* v_full = bars + 1;
-  uint64_t* s_ready = bars + 2;
-  uint64_t* p_ready = bars + 3;
-  uint64_t* o_ready = bars + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5);
+  uint8_t* sQ = smem;
+  uint8_t* sKV = smem + TB;                    // stage s: K at sKV + 2 s TB, V at sKV + (2 s + 1) TB
+  const int NKB = (p.Skv + AT_ROWS - 1) / AT_ROWS;
+  float* sMask = reinterpret_cast<float*>(sKV + 4 * TB);   // [NKB * 64]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sMask + NKB * AT_ROWS);   // [0] Q, [1..2] K/V stages
 
+  griddep_launch();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int q0 = qt * 128;
-  const int need_cols = SK > D ? SK : D;  // S occupies SK columns, O later reuses columns [0, D)
-  const uint32_t tmem_cols = need_cols <= 64 ? 64 : (need_cols <= 128 ? 128 : (need_cols <= 256 ? 256 : 512));
-
-  if (warp == 8) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmQ);
-      tma_prefetch_desc(&tmK);
-      tma_prefetch_desc(&tmV);
-      mbar_init(qk_full, 1);
-      mbar_init(v_full, 1);
-      mbar_init(s_ready, 1);
-      mbar_init(p_ready, 256);
-      mbar_init(o_ready, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, tmem_cols);
-    tmem_relinquish();
-  } else {
-    // additive mask in the log2 domain; padded key columns get -inf so that exp2 yields exactly 0 without any
-    // per-element bounds test in the softmax loops
-    for (int i = threadIdx.x; i < SK; i += 256)
-      sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + i] * LOG2E : 0.0f) : -INFINITY;
+  const int q0 = blockIdx.x * AT_ROWS, h = blockIdx.y, b = blockIdx.z;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  griddep_wait();
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(&bars[0], TB);
+    load_tile<D, AT_ROWS>(sQ, &tmQ, &bars[0], h * D, q0, b);
+    for (int kb = 0; kb < 2 && kb < NKB; ++kb) {
+      mbar_expect_tx(&bars[1 + kb], 2 * TB);
+      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, kb * AT_ROWS, b);
+      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, kb * AT_ROWS, b);
+    }
+  }
+  // additive mask in the log2 domain; padded key columns get -inf so that exp2 yields exactly 0
+  for (int i = threadIdx.x; i < NKB * AT_ROWS; i += AT_THREADS)
+    sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + i] * LOG2E : 0.0f) : -INFINITY;
+  __syncthreads();
 
-  if (warp == 8) {
-    if (lane == 0) {
-      // ---- loads ----
-      mbar_expect_tx(qk_full, DC * 16384 + DC * SK * 128);
-      for (int c = 0; c < DC; ++c) tma_load_3d(sQ + c * 16384, &tmQ, qk_full, h * D + c * 64, q0, b);
-      for (int c = 0; c < DC; ++c)
-        for (int rb = 0; rb < NB; ++rb)
-          tma_load_3d(sK + c * SK * 128 + rb * 8192, &tmK, qk_full, h * D + c * 64, rb * 64, b);
-      mbar_expect_tx(v_full, DC * SK * 128);
-      for (int c = 0; c < DC; ++c)
-        for (int rb = 0; rb < NB; ++rb)
-          tma_load_3d(sV + c * SK * 128 + rb * 8192, &tmV, v_full, h * D + c * 64, rb * 64, b);
-      // ---- S = Q K^T ----
-      mbar_wait(qk_full, 0);
-      tc_fence_after();
-      for (int n0 = 0; n0 < SK; n0 += 256) {
-        const int nn = min(256, SK - n0);
-        const uint32_t idesc = umma_idesc_bf16(128, nn, false, false);
+  const int g = lane >> 2, t4 = lane & 3;
+  const int r0 = warp * 16;                    // this warp's rows of the tile
+  float o[DT][4];
 #pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint64_t da = umma_desc_sw128(smem_u32(sQ) + (kk >> 2) * 16384 + (kk & 3) * 32, 16, 1024);
-          const uint64_t db =
-              umma_desc_sw128(smem_u32(sK) + (kk >> 2) * SK * 128 + n0 * 128 + (kk & 3) * 32, 16, 1024);
-          umma_bf16(tmem_base + n0, da, db, idesc, kk > 0 ? 1u : 0u);
-        }
-      }
-      umma_commit(s_ready);
-      // ---- O = P V ----
-      mbar_wait(p_ready, 0);
-      mbar_wait(v_full, 0);
-      tc_fence_after();
-      const uint32_t idesc_o = umma_idesc_bf16(128, D, false, true);
-      const int ksteps = (p.Skv + 15) / 16;
-      for (int kk = 0; kk < ksteps; ++kk) {
-        const uint64_t da = umma_desc_sw128(smem_u32(sP) + (kk >> 2) * 16384 + (kk & 3) * 32, 16, 1024);
-        const uint64_t db = umma_desc_sw128(smem_u32(sV) + kk * 2048, SK * 128, 1024);
-        umma_bf16(tmem_base, da, db, idesc_o, kk > 0 ? 1u : 0u);
-      }
-      umma_commit(o_ready);
-    }
-  } else {
-    // ------------------------------ softmax + epilogue (thread == query row) ------------------------------
-    const int quarter = warp & 3, half = warp >> 2;
-    const int row = quarter * 32 + lane;
-    const int q = q0 + row;
-    const bool valid = q < p.Sq;
-    const uint32_t trow = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    const int nch = (p.Skv + 31) / 32;
-    const int nk1 = (nch - half + 1) / 2;      // this thread's chunks with data: c = half + 2k, k < nk1
-    const int nk2 = SK / 64;                   // this thread's chunks of the padded row: c = half + 2k, k < nk2
-    mbar_wait(s_ready, 0);
-    tc_fence_after();
-    float mx = -INFINITY;
-    const float4* sMask4 = reinterpret_cast<const float4*>(sMask);
-    // pass 1 (row max): TMEM loads are software-pipelined - chunk c+1 is in flight while chunk c is reduced
-    auto max_chunk = [&](const uint32_t (&r)[32], int c) {
-#if MMFB_F32X2
-      const uint64_t sc2 = pk2(p.scale2, p.scale2);
+  for (int i = 0; i < DT; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.0f;
+  float mrow[2] = {-INFINITY, -INFINITY}, lrow[2] = {0.0f, 0.0f};
+  const uint32_t* dm[2] = {nullptr, nullptr};
 #pragma unroll
-      for (int q4 = 0; q4 < 8; ++q4) {
-        const float4 m = sMask4[c * 8 + q4];
-        float a0, a1, a2, a3;
-        upk2(fma2(pk2(__uint_as_float(r[q4 * 4 + 0]), __uint_as_float(r[q4 * 4 + 1])), sc2, pk2(m.x, m.y)), a0, a1);
-        upk2(fma2(pk2(__uint_as_float(r[q4 * 4 + 2]), __uint_as_float(r[q4 * 4 + 3])), sc2, pk2(m.z, m.w)), a2, a3);
-        mx = fmaxf(fmaxf(mx, a0), a1);      // one 3-input FMNMX per pair
-        mx = fmaxf(fmaxf(mx, a2), a3);
-      }
-#else
+  for (int hr = 0; hr < 2; ++hr) {
+    const int q = q0 + r0 + g + hr * 8;
+    if (p.dmask != nullptr && q < p.Sq) dm[hr] = p.dmask + (static_cast<int64_t>(b * p.H + h) * p.Sq + q) * p.W;
+  }
+  mbar_wait(&bars[0], 0);
+  const uint32_t uQ = smem_u32(sQ);
+
+  for (int kb = 0; kb < NKB; ++kb) {
+    const int st = kb & 1;
+    mbar_wait(&bars[1 + st], (kb >> 1) & 1);
+    const uint32_t uK = smem_u32(sKV + 2 * st * TB), uV = uK + TB;
+    float s[8][4];
 #pragma unroll
-      for (int q4 = 0; q4 < 8; ++q4) {
-        const float4 m = sMask4[c * 8 + q4];
-        mx = fmaxf(mx, fmaf(__uint_as_float(r[q4 * 4 + 0]), p.scale2, m.x));
-        mx = fmaxf(mx, fmaf(__uint_as_float(r[q4 * 4 + 1]), p.scale2, m.y));
-        mx = fmaxf(mx, fmaf(__uint_as_float(r[q4 * 4 + 2]), p.scale2, m.z));
-        mx = fmaxf(mx, fmaf(__uint_as_float(r[q4 * 4 + 3]), p.scale2, m.w));
-      }
-#endif
-    };
-    {
-      uint32_t ra[32], rb[32];
-      if (nk1 > 0) tmem_ld32(trow + half * 32, ra);
-#pragma unroll 1
-      for (int k = 0; k < nk1; k += 2) {
-        tmem_ld_wait();
-        if (k + 1 < nk1) tmem_ld32(trow + (half + 2 * (k + 1)) * 32, rb);
-        max_chunk(ra, half + 2 * k);
-        if (k + 1 < nk1) {
-          tmem_ld_wait();
-          if (k + 2 < nk1) tmem_ld32(trow + (half + 2 * (k + 2)) * 32, ra);
-          max_chunk(rb, half + 2 * (k + 1));
-        }
+    for (int i = 0; i < 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.0f;
+    mma_abt<D, 8, AT_ROWS, AT_ROWS>(s, uQ, r0, uK, lane);
+    // scale + mask, block row max (the four threads of a quad share a row)
+    float bmax[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      const float2 mk = *reinterpret_cast<const float2*>(sMask + kb * AT_ROWS + nt * 8 + 2 * t4);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        s[nt][e] = fmaf(s[nt][e], p.scale2, (e & 1) ? mk.y : mk.x);
+        bmax[e >> 1] = fmaxf(bmax[e >> 1], s[nt][e]);
       }
     }
-    sRed[half * 128 + row] = mx;
-    asm volatile("bar.sync 2, 256;" ::: "memory");
-    mx = fmaxf(sRed[row], sRed[128 + row]);
-    float sum = 0.0f;
-#if MMFB_F32X2
-    uint64_t sum2 = pk2(0.0f, 0.0f);
-#endif
-    const uint32_t* dm = (p.dmask != nullptr && valid)
-                             ? p.dmask + (static_cast<int64_t>(b * p.H + h) * p.Sq + q) * p.W
-                             : nullptr;
-    uint8_t* prow = sP + row * 128;
-    auto exp_chunk = [&](const uint32_t (&r)[32], int c) {
-      float e[32];
-      if (c < nch) {
-        const uint32_t bits = dm ? __ldg(dm + c) : 0xFFFFFFFFu;
-#if MMFB_F32X2
-        // the same arithmetic two lanes at a time (FFMA2 / FADD2); the row sum is kept as two interleaved partial sums
-        const uint64_t sc2 = pk2(p.scale2, p.scale2), nmx2 = pk2(-mx, -mx);
+    float corr[2];
 #pragma unroll
-        for (int q4 = 0; q4 < 8; ++q4) {
-          const float4 m = sMask4[c * 8 + q4];
-          const float mm[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-          for (int k = 0; k < 4; k += 2) {
-            const int j = q4 * 4 + k;
-            float a0, a1;
-            upk2(add2(fma2(pk2(__uint_as_float(r[j]), __uint_as_float(r[j + 1])), sc2, pk2(mm[k], mm[k + 1])), nmx2), a0, a1);
-            const float e0 = ex2_approx(a0), e1 = ex2_approx(a1);      // 0 for padded columns
-            sum2 = add2(sum2, pk2(e0, e1));
-            e[j] = ((bits >> j) & 1u) ? e0 : 0.0f;
-            e[j + 1] = ((bits >> (j + 1)) & 1u) ? e1 : 0.0f;
-          }
-        }
-#else
-#pragma unroll
-        for (int q4 = 0; q4 < 8; ++q4) {
-          const float4 m = sMask4[c * 8 + q4];
-          const float mm[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int j = q4 * 4 + k;
-            const float ev = ex2_approx(fmaf(__uint_as_float(r[j]), p.scale2, mm[k]) - mx);   // 0 for padded columns
-            sum += ev;
-            e[j] = ((bits >> j) & 1u) ? ev : 0.0f;
-          }
-        }
-#endif
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) e[j] = 0.0f;
-      }
-      uint8_t* chunk_base = prow + (c >> 1) * 16384;
-#pragma unroll
-      for (int qd = 0; qd < 4; ++qd) {
-        const int chunk = ((c & 1) * 4 + qd) ^ (row & 7);
-        uint4 o;
-        o.x = pack_bf16x2(e[qd * 8 + 0], e[qd * 8 + 1]);
-        o.y = pack_bf16x2(e[qd * 8 + 2], e[qd * 8 + 3]);
-        o.z = pack_bf16x2(e[qd * 8 + 4], e[qd * 8 + 5]);
-        o.w = pack_bf16x2(e[qd * 8 + 6], e[qd * 8 + 7]);
-        *reinterpret_cast<uint4*>(chunk_base + chunk * 16) = o;
-      }
-    };
-    // (pass 2 keeps a single TMEM buffer: with 288 threads and two CTAs per SM the budget is 112 registers)
-#pragma unroll 1
-    for (int k = 0; k < nk2; ++k) {
-      const int c = half + 2 * k;
-      uint32_t r[32];
-      if (c < nch) {
-        tmem_ld32(trow + c * 32, r);
-        tmem_ld_wait();
-      }
-      exp_chunk(r, c);
+    for (int hr = 0; hr < 2; ++hr) {
+      bmax[hr] = fmaxf(bmax[hr], __shfl_xor_sync(0xffffffffu, bmax[hr], 1));
+      bmax[hr] = fmaxf(bmax[hr], __shfl_xor_sync(0xffffffffu, bmax[hr], 2));
+      const float mn = fmaxf(mrow[hr], bmax[hr]);   // finite: every key block holds at least one real key
+      corr[hr] = ex2_approx(mrow[hr] - mn);         // 0 on the first block
+      mrow[hr] = mn;
+      lrow[hr] *= corr[hr];
     }
-#if MMFB_F32X2
-    {
-      float s0, s1;
-      upk2(sum2, s0, s1);
-      sum = s0 + s1;
+#pragma unroll
+    for (int i = 0; i < DT; ++i) {
+      o[i][0] *= corr[0]; o[i][1] *= corr[0];
+      o[i][2] *= corr[1]; o[i][3] *= corr[1];
     }
-#endif
-    sRed[256 + half * 128 + row] = sum;
+    uint32_t bits[2] = {0xFFFFFFFFu, 0xFFFFFFFFu}, bits2[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      if (dm[hr] != nullptr) {
+        const int w0 = kb * 2;
+        bits[hr] = __ldg(dm[hr] + w0);
+        if (w0 + 1 < p.W) bits2[hr] = __ldg(dm[hr] + w0 + 1);
+      }
+    }
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int hr = e >> 1;
+        const float pe = ex2_approx(s[nt][e] - mrow[hr]);   // 0 for padded columns
+        lrow[hr] += pe;
+        const int col = nt * 8 + 2 * t4 + (e & 1);          // key within the block
+        const uint32_t w = col < 32 ? bits[hr] : bits2[hr];
+        s[nt][e] = ((w >> (col & 31)) & 1u) ? pe : 0.0f;
+      }
+    }
+    uint32_t pf[4][4];
+    acc_to_a<8>(s, pf);
+    mma_pb<D, 4, AT_ROWS>(o, pf, uV, lane);
+    // every warp is done with this stage: its ldmatrix reads (generic proxy) are ordered before the TMA refill (async
+    // proxy) that thread 0 issues next; a barrier alone does not order the two proxies
     fence_proxy_async();
-    tc_fence_before();
-    mbar_arrive(p_ready);
-    asm volatile("bar.sync 2, 256;" ::: "memory");
-    sum = sRed[256 + row] + sRed[256 + 128 + row];
-    if (valid && half == 0) p.lse2[static_cast<int64_t>(b * p.H + h) * p.Sq + q] = mx + log2f(sum);
-    const float inv = p.dscale / sum;
-    mbar_wait(o_ready, 0);
-    tc_fence_after();
-#pragma unroll
-    for (int c = half; c < D / 32; c += 2) {
-      uint32_t r[32];
-      tmem_ld32(trow + c * 32, r);
-      tmem_ld_wait();
-      if (valid) {
-        uint4* dst = reinterpret_cast<uint4*>(p.ctx + (static_cast<int64_t>(b) * p.Sq + q) * p.ldo + h * D + c * 32);
-#pragma unroll
-        for (int qd = 0; qd < 4; ++qd) {
-          uint4 o;
-          o.x = pack_bf16x2(__uint_as_float(r[qd * 8 + 0]) * inv, __uint_as_float(r[qd * 8 + 1]) * inv);
-          o.y = pack_bf16x2(__uint_as_float(r[qd * 8 + 2]) * inv, __uint_as_float(r[qd * 8 + 3]) * inv);
-          o.z = pack_bf16x2(__uint_as_float(r[qd * 8 + 4]) * inv, __uint_as_float(r[qd * 8 + 5]) * inv);
-          o.w = pack_bf16x2(__uint_as_float(r[qd * 8 + 6]) * inv, __uint_as_float(r[qd * 8 + 7]) * inv);
-          dst[qd] = o;
-        }
-        if (p.ctx_lo != nullptr) {
-          uint4* dlo = reinterpret_cast<uint4*>(p.ctx_lo + (static_cast<int64_t>(b) * p.Sq + q) * (p.H * D) + h * D + c * 32);
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd) {
-            uint32_t w[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float o0 = __uint_as_float(r[qd * 8 + 2 * e]) * inv, o1 = __uint_as_float(r[qd * 8 + 2 * e + 1]) * inv;
-              const float2 hi = unpack_bf16x2(pack_bf16x2(o0, o1));
-              w[e] = pack_bf16x2(o0 - hi.x, o1 - hi.y);
-            }
-            dlo[qd] = make_uint4(w[0], w[1], w[2], w[3]);
-          }
-        }
-      }
+    __syncthreads();
+    if (threadIdx.x == 0 && kb + 2 < NKB) {
+      mbar_expect_tx(&bars[1 + st], 2 * TB);
+      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, (kb + 2) * AT_ROWS, b);
+      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, (kb + 2) * AT_ROWS, b);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
+
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    float l = lrow[hr];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const int q = q0 + r0 + g + hr * 8;
+    if (q >= p.Sq) continue;
+    if (t4 == 0) p.lse2[static_cast<int64_t>(b * p.H + h) * p.Sq + q] = mrow[hr] + log2f(l);
+    const float inv = p.dscale / l;
+    bf16* dst = p.ctx + (static_cast<int64_t>(b) * p.Sq + q) * p.ldo + h * D;
+    bf16* dlo = p.ctx_lo != nullptr ? p.ctx_lo + (static_cast<int64_t>(b) * p.Sq + q) * (p.H * D) + h * D : nullptr;
+#pragma unroll
+    for (int i = 0; i < DT; ++i) {
+      const int c = i * 8 + 2 * t4;
+      const float v0 = o[i][hr * 2] * inv, v1 = o[i][hr * 2 + 1] * inv;
+      const uint32_t hi = pack_bf16x2(v0, v1);
+      *reinterpret_cast<uint32_t*>(dst + c) = hi;
+      if (dlo != nullptr) {
+        const float2 hf = unpack_bf16x2(hi);
+        *reinterpret_cast<uint32_t*>(dlo + c) = pack_bf16x2(v0 - hf.x, v1 - hf.y);
+      }
+    }
   }
 }
-
-// ----------------------------------------------------------------------------------------------
-// forward, paired-tile persistent kernel (head size 64, Sq, Skv <= 256): the default for the VisualBERT / MMBT shapes
-//
-// One persistent CTA per SM walks over (batch, head) PAIRS of 128-query tiles.  Round-2 ncu view of attn_fwd_kernel (one
-// CTA per tile, 2 CTAs per SM): tensor pipe 8.7 % active, IPC 1.4 of 4, 27 % of the issued instructions in barrier spin
-// loops, K and V fetched once per query tile, P through 64 KB of shared memory - a serial chain TMA -> S -> softmax -> P ->
-// O per CTA.  Here:
-//   * K, V of a (batch, head) are loaded ONCE for both query tiles, into a two-stage ring (2 x 96 KB: Q0 Q1 K V), so the
-//     next pair streams in while this one computes;
-//   * each tile owns 256 TMEM columns and one softmax group of 8 warps (2 threads per query row, 128 score columns
-//     each): the S MMA of one tile and the softmax of the other overlap (ping-pong), nobody waits for a load;
-//   * P never touches shared memory: it is written over the score columns that have already been consumed
-//     (tcgen05.st, bf16 pairs in K order) and O = P V reads its A operand from tensor memory;
-//     region map per tile:  S [0,256)  ->  P(keys 0..127) [0,64) | O [64,128) | P(keys 128..255) [128,192).
-// 608 threads: warps 0..7 = softmax group of tile 0, warps 8..15 = tile 1, warp 16 = MMA issue, warp 17 = TMA loads + mask
-// rows + item counter, warp 18 = bulk tensor stores of the output tiles.
-// Barriers (phase = pair parity unless noted): qk_full / v_full / mask_full / stage_free per ring stage, and per tile
-// s_ready (S committed), p_ready (256 arrivals: P complete), o_ready (O committed), o_read (256 arrivals: O copied out).
-// ----------------------------------------------------------------------------------------------
-// Timeline tracing for kernel development (-DMMFB_TRACE=1 builds only, python tools/ab.py build trace -DMMFB_TRACE=1):
-// CTA 0 stamps clock64() at fixed points of its first 64 items; tools/trace_attn.py prints the phase durations.
-#ifdef MMFB_TRACE
-__device__ long long mmfb_trace_buf[4 * 64 * 16];
-#define MMFB_TR(role, n, slot)                                                                                        \
-  do {                                                                                                                \
-    if (blockIdx.x == 0 && (n) < 64) mmfb_trace_buf[((role) * 64 + (n)) * 16 + (slot)] = clock64();                   \
-  } while (0)
-#else
-#define MMFB_TR(role, n, slot) do { } while (0)
-#endif
-
-__device__ __forceinline__ void fwd_chunk_max(const uint32_t (&r)[32], const float4* m4, float scale2, float& mx) {
-#if MMFB_F32X2
-  const uint64_t sc2 = pk2(scale2, scale2);
-#pragma unroll
-  for (int q4 = 0; q4 < 8; ++q4) {
-    const float4 m = m4[q4];
-    float a0, a1, a2, a3;
-    upk2(fma2(pk2(__uint_as_float(r[q4 * 4 + 0]), __uint_as_float(r[q4 * 4 + 1])), sc2, pk2(m.x, m.y)), a0, a1);
-    upk2(fma2(pk2(__uint_as_float(r[q4 * 4 + 2]), __uint_as_float(r[q4 * 4 + 3])), sc2, pk2(m.z, m.w)), a2, a3);
-    mx = fmaxf(fmaxf(mx, a0), a1);
-    mx = fmaxf(fmaxf(mx, a2), a3);
-  }
-#else
-#pragma unroll
-  for (int q4 = 0; q4 < 8; ++q4) {
-    const float4 m = m4[q4];
-    mx = fmaxf(mx, fmaf(__uint_as_float(r[q4 * 4 + 0]), scale2, m.x));
-    mx = fmaxf(mx, fmaf(__uint_as_float(r[q4 * 4 + 1]), scale2, m.y));
-    mx = fmaxf(mx, fmaf(__uint_as_float(r[q4 * 4 + 2]), scale2, m.z));
-    mx = fmaxf(mx, fmaf(__uint_as_float(r[q4 * 4 + 3]), scale2, m.w));
-  }
-#endif
-}
-// exp2(s*scale2 + mask - mx) of one 32-column chunk -> 16 packed bf16 pairs (dropout applied), row sum accumulated
-// (measured and dropped: dropout as an AND of the packed pair with a mask looked up per 8 keep-bits, as the LayerNorm
-//  backward does - 115 us against 111.5 us for the bit tests below: the look-ups queue behind the mask-row loads)
-__device__ __forceinline__ void fwd_chunk_exp(const uint32_t (&r)[32], const float4* m4, float scale2, float mx,
-                                              uint32_t bits, float& sum, uint32_t (&pk)[16]) {
-#if MMFB_F32X2
-  const uint64_t sc2 = pk2(scale2, scale2), nmx2 = pk2(-mx, -mx);
-  uint64_t sum2 = pk2(sum, 0.0f);
-#endif
-#pragma unroll
-  for (int q4 = 0; q4 < 8; ++q4) {
-    const float4 m = m4[q4];
-    const float mm[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-    for (int k = 0; k < 4; k += 2) {
-      const int j = q4 * 4 + k;
-#if MMFB_F32X2
-      float a0, a1;
-      upk2(add2(fma2(pk2(__uint_as_float(r[j]), __uint_as_float(r[j + 1])), sc2, pk2(mm[k], mm[k + 1])), nmx2), a0, a1);
-      const float e0 = ex2_approx(a0), e1 = ex2_approx(a1);
-      sum2 = add2(sum2, pk2(e0, e1));
-#else
-      const float e0 = ex2_approx(fmaf(__uint_as_float(r[j]), scale2, mm[k]) - mx);
-      const float e1 = ex2_approx(fmaf(__uint_as_float(r[j + 1]), scale2, mm[k + 1]) - mx);
-      sum += e0;
-      sum += e1;
-#endif
-      pk[j >> 1] = pack_bf16x2(((bits >> j) & 1u) ? e0 : 0.0f, ((bits >> (j + 1)) & 1u) ? e1 : 0.0f);
-    }
-  }
-#if MMFB_F32X2
-  float s0, s1;
-  upk2(sum2, s0, s1);
-  sum = s0 + s1;
-#endif
-}
-
-constexpr int FWD_PAIR_THREADS = 608;       // 16 softmax warps + MMA-issue warp + loader warp + store warp
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-// 18 warps put 5 on one scheduler partition (16 K registers each): at most 96 registers per thread can launch
-__global__ void __launch_bounds__(FWD_PAIR_THREADS, 1)
-attn_fwd_pair_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmO,
-                     const __grid_constant__ CUtensorMap tmOlo, AttnFwdDev p, int n_pairs, int* sched) {
-  griddep_launch();
-  griddep_wait();
-  constexpr int D = 64;
-  constexpr int TILE = 16384;                        // [128 x 128 B]
-  constexpr int STAGE = 6 * TILE;                    // Q0 | Q1 | K0 K1 | V0 V1
-  // region map per tile (256 columns): S [0,256) -> O [0,64) | P(keys 0..127) [64,128) | - | P(keys 128..255) [192,256):
-  // pass 2 walks a thread's chunks from the last to the first, so chunk k's probabilities (16 columns) land on score
-  // columns of chunks >= k that have been consumed, and the two chunks pass 1 read last are still in registers.
-  constexpr uint32_t REG = 256, COL_O = 0, COL_PLO = 64, COL_PHI = 192;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_align1024(smem_raw);
-  float* sMask = reinterpret_cast<float*>(smem + 2 * STAGE);      // [2 stages][256]
-  float* sMax = sMask + 512;                                      // [2 tiles][2 halves][128 rows]
-  float* sSum = sMax + 512;                                       // [2 tiles][2 halves][128 rows]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sSum + 512);
-  uint64_t* qk_full = bars;          // [2]
-  uint64_t* v_full = bars + 2;       // [2]
-  uint64_t* mask_full = bars + 4;    // [2]
-  uint64_t* stage_free = bars + 6;   // [2]  per tile: one commit of the MMA thread + one arrival of the store warp
-  uint64_t* s_ready = bars + 8;      // [2 tiles]
-  uint64_t* p_ready = bars + 10;     // [2 tiles]
-  uint64_t* o_ready = bars + 12;     // [2 tiles]
-  uint64_t* o_read = bars + 14;      // [2 tiles]
-  // [2 tiles][2 stages] 256 arrivals: the output tile is in shared memory.  Per STAGE: a group may run a whole item ahead of
-  // the other one, and the store warp serves the tiles in order - with one barrier per tile its phase could complete twice
-  // before the store warp looked at it once (seen as a rare hang under ragged padding); two items ahead is impossible, the
-  // ring stage is not refilled before the store warp has released it.
-  uint64_t* o_staged = bars + 16;
-  uint64_t* k_free = bars + 20;      // [2 stages] both tiles' score MMAs of the stage have completed: the K slots are free
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 22);
-  uint32_t* sAct = tmem_slot + 1;    // [2 stages] bit c: 32-key chunk c has at least one key that is not masked out
-  int* sItem = reinterpret_cast<int*>(sAct + 2);   // [2 stages] (batch, head) item of the stage, -1 = no more work
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nt = (p.Sq + 127) / 128;                 // query tiles per pair (1 or 2)
-  const int nkt = (p.Skv + 127) / 128;               // key tiles (1 or 2)
-  const int SKP = nkt * 128;                         // padded key count: N of the score MMA
-
-  if (warp == 17) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmQ);
-      tma_prefetch_desc(&tmK);
-      tma_prefetch_desc(&tmV);
-      for (int s = 0; s < 2; ++s) {
-        mbar_init(&qk_full[s], 1);
-        mbar_init(&v_full[s], 1);
-        mbar_init(&mask_full[s], 32);
-        mbar_init(&stage_free[s], 2 * nt);
-        mbar_init(&o_staged[s], 256);
-        mbar_init(&o_staged[2 + s], 256);
-        mbar_init(&k_free[s], nt);
-        mbar_init(&s_ready[s], 1);
-        mbar_init(&p_ready[s], 256);
-        mbar_init(&o_ready[s], 1);
-        mbar_init(&o_read[s], 256);
-      }
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 17) {
-    // ------------------------------------ loader: TMA tiles + mask rows, two pairs ahead ------------------------------------
-    // Items are handed out by an atomic counter (sched[0]), not by a fixed stride: their cost varies with the padding of the
-    // sample (masked chunks are skipped), and with 13.5 items per CTA a static split leaves the slowest CTA ~10 % behind.
-    // The item of ring stage s travels with its mask row: sItem[s], sAct[s], sMask[s] are published by mask_full[s].
-    auto load_pair = [&](int n, int it) {  // lane 0: Q tiles + K into qk_full, V into v_full of ring stage n & 1
-      const int h = it % p.H, b = it / p.H;
-      const int s = n & 1;
-      uint8_t* st = smem + s * STAGE;
-      mbar_expect_tx(&qk_full[s], (nt + nkt) * TILE);
-      for (int t = 0; t < nt; ++t) tma_load_3d(st + t * TILE, &tmQ, &qk_full[s], h * D, t * 128, b);
-      for (int j = 0; j < nkt; ++j) tma_load_3d(st + (2 + j) * TILE, &tmK, &qk_full[s], h * D, j * 128, b);
-      mbar_expect_tx(&v_full[s], nkt * TILE);
-      for (int j = 0; j < nkt; ++j) tma_load_3d(st + (4 + j) * TILE, &tmV, &v_full[s], h * D, j * 128, b);
-    };
-    auto load_mask = [&](int n, int it) {  // whole warp: log2-domain additive mask, -inf on the padded key columns
-      float* dst = sMask + (n & 1) * 256;
-      // Chunks whose 32 keys are ALL masked out (additive -10000, or beyond Skv) contribute exp2(-14427 + ...) = 0 exactly:
-      // they are skipped in both softmax passes and in the P V contraction (identical results; a quarter of the chunks at
-      // the padding rates of the reference's text / region batches).  A sample without any attendable key keeps them all:
-      // its softmax is uniform over the masked keys (hf_layers.py:191-196 semantics).
-      uint32_t act = 0;
-      if (it >= 0) {
-        const int b = it / p.H;
-        float mv[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int i = lane + 32 * j;
-          mv[j] = (i < p.Skv) ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + i] * LOG2E : 0.0f) : -INFINITY;
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          dst[lane + 32 * j] = mv[j];
-          if (__any_sync(0xffffffffu, mv[j] > -5000.0f)) act |= 1u << j;
-        }
-        if (act == 0) act = (1u << ((p.Skv + 31) / 32)) - 1u;
-      }
-      if (lane == 0) { sAct[n & 1] = act; sItem[n & 1] = it; }
-      __syncwarp();
-      mbar_arrive(&mask_full[n & 1]);
-    };
-    for (int n = 0;; ++n) {
-      // ring stage n & 1 (tiles, mask row, item) is refilled once every MMA of the item that used it has completed
-      if (n >= 2) mbar_wait(&stage_free[n & 1], ((n - 2) >> 1) & 1);
-      int it = 0;
-      if (lane == 0) it = atomicAdd(sched, 1);
-      it = __shfl_sync(0xffffffffu, it, 0);
-      if (it >= n_pairs) it = -1;
-      if (lane == 0) MMFB_TR(3, n, 0);
-      if (lane == 0 && it >= 0) load_pair(n, it);
-      load_mask(n, it);
-      if (lane == 0) MMFB_TR(3, n, 1);
-      if (it < 0) break;
-    }
-  } else if (warp == 16) {
-    // ------------------------------------ MMA issue: one thread, both tiles, never blocked on one of them ------------------------------------
-    if (lane == 0) {
-      auto issue_s = [&](int n, int t) {   // S_t = Q_t K^T over all (padded) keys
-        const uint32_t st = smem_u32(smem + (n & 1) * STAGE);
-        const uint32_t aQ = st + t * TILE, aK = st + 2 * TILE;
-        const uint32_t idesc = umma_idesc_bf16(128, SKP, false, false);
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk)
-          umma_bf16(tmem_base + t * REG, umma_desc_sw128(aQ + kk * 32, 16, 1024), umma_desc_sw128(aK + kk * 32, 16, 1024), idesc,
-                    kk > 0 ? 1u : 0u);
-        umma_commit(&s_ready[t]);
-        umma_commit(&k_free[n & 1]);
-      };
-      auto issue_o = [&](int n, int t) {   // O_t = P V, A = P from tensor memory (8 columns per 16 keys)
-        const uint32_t aV = smem_u32(smem + (n & 1) * STAGE + 4 * TILE);
-        const uint32_t idesc = umma_idesc_bf16(128, D, false, true);
-        const int ksteps = (p.Skv + 15) / 16;
-        const uint32_t act = sAct[n & 1];
-        bool first = true;
-        for (int kk = 0; kk < ksteps; ++kk) {
-          if (!((act >> (kk >> 1)) & 1u)) continue;            // P is exactly zero over this chunk
-          const uint32_t a_tm = tmem_base + t * REG + (kk < 8 ? COL_PLO + kk * 8 : COL_PHI + (kk - 8) * 8);
-          // V tile j = kk / 8 (128 keys each), 16 keys per step: 2048 B per step inside the tile, MN-major
-          umma_bf16_ts(tmem_base + t * REG + COL_O, a_tm, umma_desc_sw128(aV + (kk >> 3) * TILE + (kk & 7) * 2048, TILE, 1024), idesc,
-                       first ? 0u : 1u);
-          first = false;
-        }
-        umma_commit(&o_ready[t]);
-      };
-      // Per tile: [wait P_t(n)] -> O_t(n) -> [wait O_t(n) copied out, item n+1 published] -> S_t(n+1) -> ...  The two chains
-      // are independent; the barriers are PROBED (mbarrier.test_wait) in turn, so whichever softmax group gets there first is
-      // served first and the groups settle half a period apart: the tensor core work of one hides behind the arithmetic of
-      // the other.  An idle probe round sleeps ~50 ns: a spinning warp would take issue slots from the softmax warps of
-      // its scheduler partition.
-      int pn[2] = {0, 0};                  // item index (per CTA) the tile is in
-      int ph[2] = {0, 0};                  // 0: O_t(pn) is next, 1: S_t(pn + 1) is next, 2: done
-      int live = nt;
-      if (nt < 2) ph[1] = 2;
-      mbar_wait(&mask_full[0], 0);
-      if (sItem[0] < 0) live = 0;
-      else {
-        mbar_wait(&qk_full[0], 0);
-        tc_fence_after();
-        for (int t = 0; t < nt; ++t) issue_s(0, t);
-      }
-      uint32_t spins = 0;
-      long long t0 = 0;
-      while (live > 0) {
-        bool progressed = false;
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-          const int n = pn[t];
-          if (ph[t] == 0) {
-            if (mbar_test(&p_ready[t], n & 1) && mbar_test(&v_full[n & 1], (n >> 1) & 1)) {
-              tc_fence_after();
-              MMFB_TR(2, n, 2 * t);
-              issue_o(n, t);
-              umma_commit(&stage_free[n & 1]);                 // every MMA of this tile that reads the ring stage has been issued
-              ph[t] = 1;
-              progressed = true;
-            }
-          } else if (ph[t] == 1) {
-            if (mbar_test(&o_read[t], n & 1) && mbar_test(&mask_full[(n + 1) & 1], ((n + 1) >> 1) & 1)) {
-              if (sItem[(n + 1) & 1] < 0) {                    // no further item
-                ph[t] = 2;
-                --live;
-                progressed = true;
-              } else if (mbar_test(&qk_full[(n + 1) & 1], ((n + 1) >> 1) & 1)) {
-                tc_fence_after();
-                MMFB_TR(2, n, 2 * t + 1);
-                issue_s(n + 1, t);
-                pn[t] = n + 1;
-                ph[t] = 0;
-                progressed = true;
-              }
-            }
-          }
-        }
-        if (progressed) { spins = 0; t0 = 0; }
-        else {
-          __nanosleep(40);
-          if (((++spins) & 0xFFFFu) == 0) {                    // watchdog: a protocol bug traps instead of hanging the GPU
-            const long long now = clock64();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 8000000000LL) { printf("mmfb: attention forward issue loop timeout (block %d)\n", (int)blockIdx.x); __trap(); }
-          }
-        }
-      }
-    }
-  } else if (warp == 18) {
-    // ------------------------------------ store warp: one bulk tensor store per output tile ------------------------------------
-    // rows beyond Sq are clipped by the tensor map ([B][Sq][heads * d]); the ring stage is released to the loader only after
-    // the stores have finished READING shared memory
-    for (int n = 0;; ++n) {
-      mbar_wait(&mask_full[n & 1], (n >> 1) & 1);
-      const int it = sItem[n & 1];
-      if (it < 0) break;
-      const int h = it % p.H, b = it / p.H;
-      uint8_t* stage_base = smem + (n & 1) * STAGE;
-      for (int t = 0; t < nt; ++t) {
-        mbar_wait(&o_staged[t * 2 + (n & 1)], (n >> 1) & 1);
-        if (lane == 0) {
-          tma_store_3d(&tmO, stage_base + t * TILE, h * D, t * 128, b);
-          if (p.ctx_lo != nullptr) tma_store_3d(&tmOlo, stage_base + (2 + t) * TILE, h * D, t * 128, b);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-          mbar_arrive(&stage_free[n & 1]);
-        }
-        __syncwarp();
-      }
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // writes complete before the CTA exits
-  } else {
-    // ------------------------------------ softmax groups ------------------------------------
-    const int t = warp >> 3;                                  // tile / group
-    if (t < nt) {
-      const int quarter = warp & 3, half = (warp >> 2) & 1;
-      const int row = quarter * 32 + lane;
-      const uint32_t treg = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + t * REG;
-      const int nch = (p.Skv + 31) / 32;
-      const int c0 = half * 4;                                // this thread's chunks: c0 .. c0+3 (keys 128*half ..)
-      const bool have = half < nkt;                           // this half of the key range exists
-      float* gMax = sMax + t * 256;
-      float* gSum = sSum + t * 256;
-      const int bar_id = 1 + t;
-      const uint32_t pcol = half == 0 ? COL_PLO : COL_PHI;
-      // (Measured and dropped: serialising the two groups' exponential passes with named barriers so that they settle half
-      // a period apart - 185 k cycles per 14 items with and without it: the pass is bound by the issue slots of the group's
-      // own 8 warps, not by the SM's 16 MUFU lanes, so running both groups' passes together costs nothing extra.)
-      for (int n = 0;; ++n) {
-        const bool tr = (threadIdx.x & 255) == 0;
-        if (tr) MMFB_TR(t, n, 0);
-        mbar_wait(&mask_full[n & 1], (n >> 1) & 1);
-        if (tr) MMFB_TR(t, n, 1);
-        const int it = sItem[n & 1];
-        if (it < 0) break;
-        const int h = it % p.H, b = it / p.H;
-        const int q = t * 128 + row;
-        const bool valid = q < p.Sq;
-        const float4* m4 = reinterpret_cast<const float4*>(sMask + (n & 1) * 256) + c0 * 8;
-        // keep-bit words of this thread's chunks: fetched before the score barrier
-        uint32_t bits[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
-        if (p.dmask != nullptr && valid) {
-          const uint32_t* dm = p.dmask + (static_cast<int64_t>(b * p.H + h) * p.Sq + q) * p.W;
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (c0 + k < nch) bits[k] = __ldg(dm + c0 + k);
-        }
-        const uint32_t act = have ? (sAct[n & 1] >> c0) & 0xFu : 0u;   // bit k: chunk k of this thread has an attendable key
-        const bool on0 = act & 1u, on1 = act & 2u, on2 = act & 4u, on3 = act & 8u;
-        mbar_wait(&s_ready[t], n & 1);
-        tc_fence_after();
-        if (tr) MMFB_TR(t, n, 2);
-        // ---- pass 1: row maximum; the load of the next chunk is in flight while this one is reduced ----
-        uint32_t ra[32], rb[32];
-        float mx = -INFINITY;
-        if (on0) tmem_ld32(treg + (c0 + 0) * 32, ra);
-        tmem_ld_wait();
-        if (on1) tmem_ld32(treg + (c0 + 1) * 32, rb);
-        if (on0) fwd_chunk_max(ra, m4 + 0, p.scale2, mx);
-        tmem_ld_wait();
-        if (on2) tmem_ld32(treg + (c0 + 2) * 32, ra);
-        if (on1) fwd_chunk_max(rb, m4 + 8, p.scale2, mx);
-        tmem_ld_wait();
-        if (on3) tmem_ld32(treg + (c0 + 3) * 32, rb);
-        if (on2) fwd_chunk_max(ra, m4 + 16, p.scale2, mx);
-        tmem_ld_wait();
-        if (on3) fwd_chunk_max(rb, m4 + 24, p.scale2, mx);
-        gMax[half * 128 + row] = mx;
-        if (tr) MMFB_TR(t, n, 3);
-        asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");
-        if (tr) MMFB_TR(t, n, 4);
-        mx = fmaxf(gMax[row], gMax[128 + row]);
-        // ---- pass 2, last chunk first (chunks 3 and 2 are still in rb / ra): probabilities -> tensor memory ----
-        float sum = 0.0f;
-        uint32_t pk[16];
-        if (on3) {
-          fwd_chunk_exp(rb, m4 + 24, p.scale2, mx, bits[3], sum, pk);
-          tmem_st16(treg + pcol + 48, pk);
-        }
-        if (on1) tmem_ld32(treg + (c0 + 1) * 32, rb);
-        if (on2) {
-          fwd_chunk_exp(ra, m4 + 16, p.scale2, mx, bits[2], sum, pk);
-          tmem_st16(treg + pcol + 32, pk);
-        }
-        tmem_ld_wait();
-        if (on0) tmem_ld32(treg + (c0 + 0) * 32, ra);
-        if (on1) {
-          fwd_chunk_exp(rb, m4 + 8, p.scale2, mx, bits[1], sum, pk);
-          tmem_st16(treg + pcol + 16, pk);
-        }
-        tmem_ld_wait();
-        if (on0) {
-          fwd_chunk_exp(ra, m4 + 0, p.scale2, mx, bits[0], sum, pk);
-          tmem_st16(treg + pcol + 0, pk);
-        }
-        gSum[half * 128 + row] = sum;
-        if (tr) MMFB_TR(t, n, 5);
-        tmem_st_wait();
-        tc_fence_before();
-        mbar_arrive(&p_ready[t]);
-        if (tr) MMFB_TR(t, n, 6);
-        asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");
-        if (tr) MMFB_TR(t, n, 7);
-        sum = gSum[row] + gSum[128 + row];
-        // ---- O_t: 32 of the 64 columns per thread ----
-        mbar_wait(&o_ready[t], n & 1);
-        tc_fence_after();
-        if (tr) MMFB_TR(t, n, 8);
-        tmem_ld32(treg + COL_O + half * 32, ra);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(&o_read[t]);
-        if (tr) MMFB_TR(t, n, 9);
-        // ---- the tile goes out through shared memory and ONE bulk tensor store per tile: 16-byte stores of a warp to 32
-        //      different rows cost 32 LSU passes each (round-2 trace: 47 % of an item's time in these stores) ----
-        {
-          const float inv = p.dscale / sum;
-          if (valid && half == 0) p.lse2[static_cast<int64_t>(b * p.H + h) * p.Sq + q] = mx + log2f(sum);
-          uint8_t* stage_base = smem + (n & 1) * STAGE;
-          uint8_t* orow = stage_base + t * TILE + row * 128;            // the Q_t slot: free since S_t completed
-          uint8_t* lrow = stage_base + (2 + t) * TILE + row * 128;      // the K_t slot: free once BOTH tiles' S completed
-          const bool want_lo = p.ctx_lo != nullptr;
-          if (want_lo) mbar_wait(&k_free[n & 1], (n >> 1) & 1);
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd) {
-            uint32_t wh[4], wl[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float o0 = __uint_as_float(ra[qd * 8 + 2 * e]) * inv, o1 = __uint_as_float(ra[qd * 8 + 2 * e + 1]) * inv;
-              wh[e] = pack_bf16x2(o0, o1);
-              const float2 hi = unpack_bf16x2(wh[e]);
-              wl[e] = pack_bf16x2(o0 - hi.x, o1 - hi.y);
-            }
-            const int chunk = ((half * 4 + qd) ^ (row & 7)) * 16;
-            *reinterpret_cast<uint4*>(orow + chunk) = make_uint4(wh[0], wh[1], wh[2], wh[3]);
-            if (want_lo) *reinterpret_cast<uint4*>(lrow + chunk) = make_uint4(wl[0], wl[1], wl[2], wl[3]);
-          }
-          fence_proxy_async();
-          mbar_arrive(&o_staged[t * 2 + (n & 1)]);
-        }
-        if (tr) MMFB_TR(t, n, 10);
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 17) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-  // the last CTA to finish re-arms the item counter for the next launch (launches of one stream are serialised)
-  if (threadIdx.x == 0 && atomicAdd(sched + 1, 1) == static_cast<int>(gridDim.x) - 1) {
-    atomicExch(sched, 0);
-    atomicExch(sched + 1, 0);
-  }
-}
-
-// (Measured and removed in round 2: a key-BLOCK form of the paired kernel - two blocks of 128 keys with their own statistics,
-// each thread's 64 score columns read from tensor memory once and kept in registers, combined in the epilogue.  At 96
-// registers per thread ptxas spilled 0.5-0.9 KB per thread whichever way the block code was arranged (inlined, looped,
-// out of line), and the kernel ran at 255 us against 112 us for the two-pass form above; profiles/r2_trace_fwd_key_blocks.txt.)
 
 // ----------------------------------------------------------------------------------------------
 // backward
 // ----------------------------------------------------------------------------------------------
 struct AttnBwdDev {
   int B, H, Sq, Skv;
-  const float* mask;      // [B, Skv] additive or null
-  const float* lse2;      // [B, H, Sq]
-  const float* delta;     // [B, H, Sq]  rowsum(dO * O)
-  const uint32_t* dmask;  // [B, H, Sq, W] or null
-  int W;
-  float dscale, scale2, scale;
-  bf16* out0;             // ROWS_ARE_Q: dQ ; else dK      [B*S_rows, ld0], head at col h*D
-  int64_t ld0;
-  bf16* out1;             // else-mode only: dV
-  int64_t ld1;
-};
-
-// rows: the operand pair that stays resident (R, Rg); cols: the looped pair (C, Cg)
-//   ROWS_ARE_Q :  R = Q_i, Rg = dO_i ; C = K_j, Cg = V_j ;  out0 = dQ_i = scale * sum_j dS' C
-//   !ROWS_ARE_Q:  R = K_j, Rg = V_j  ; C = Q_i, Cg = dO_i;  out0 = dK_j = scale * sum_i dS' C ; out1 = dV_j = sum_i P' Cg
-// CB = width of the looped block (keys for dQ, queries for dK/dV).  CB = 64 keeps the CTA at 256 TMEM columns and
-// ~80 KB of shared memory for d = 64, so two CTAs share an SM and hide each other's TMA / MMA / barrier latencies.
-template <int D, bool ROWS_ARE_Q, bool DROP, int CB>
-__global__ void __launch_bounds__(160, (CB == 64) ? 2 : 1)
-attn_bwd_kernel(const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmRg,
-                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmCg, AttnBwdDev p) {
-  griddep_launch();
-  griddep_wait();
-  constexpr int DC = D / 64;
-  constexpr int TILE = DC * 16384;   // one [128 x D] bf16 resident-operand tile
-  constexpr int CTILE = DC * CB * 128;  // one [CB x D] bf16 looped-operand tile
-  constexpr int PBYTES = 128 * CB * 2;  // P' / dS' [128 x CB] bf16
-  constexpr int NCBUF = (CB == 64) ? 2 : 1;   // prefetch the next looped tiles while this iteration computes
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_align1024(smem_raw);
-  uint8_t* sR = smem;
-  uint8_t* sRg = sR + TILE;
-  uint8_t* sC = sRg + TILE;
-  uint8_t* sCg = sC + NCBUF * CTILE;   // looped tiles are double-buffered when NCBUF == 2: [buf][tile]
-  uint8_t* sP = sCg + NCBUF * CTILE;   // [128 x CB] bf16, CB/64 chunks of [128 x 128B]
-  uint8_t* sDS = sP + PBYTES;
-  float* sCol = reinterpret_cast<float*>(sDS + PBYTES);   // [2 buffers][2 stats][128] per-column statistics
-  uint32_t* sBits = reinterpret_cast<uint32_t*>(sCol + 512);  // [2 buffers][128 cols][4 words] dropout keep bits
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sBits + 1024);
-  uint64_t* r_full = bars;
-  uint64_t* c_full = bars + 1;    // [2]
-  uint64_t* s_ready = bars + 3;
-  uint64_t* p_ready = bars + 4;
-  uint64_t* acc_done = bars + 5;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int rt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int row0 = rt * 128;
-  const int S_rows = ROWS_ARE_Q ? p.Sq : p.Skv;
-  const int S_cols = ROWS_ARE_Q ? p.Skv : p.Sq;
-  const int n_it = (S_cols + CB - 1) / CB;
-  constexpr uint32_t TMEM_COLS = (2 * CB + (ROWS_ARE_Q ? D : 2 * D)) <= 256 ? 256 : 512;
-  constexpr uint32_t COL_S = 0, COL_DP = CB, COL_O0 = 2 * CB, COL_O1 = 2 * CB + D;
-
-  if (warp == 4) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmR);
-      tma_prefetch_desc(&tmRg);
-      tma_prefetch_desc(&tmC);
-      tma_prefetch_desc(&tmCg);
-      mbar_init(r_full, 1);
-      mbar_init(&c_full[0], 1);
-      mbar_init(&c_full[1], 1);
-      mbar_init(s_ready, 1);
-      mbar_init(p_ready, 128);
-      mbar_init(acc_done, 1);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 4) {
-    if (lane == 0) {
-      mbar_expect_tx(r_full, 2 * TILE);
-      for (int c = 0; c < DC; ++c) {
-        tma_load_3d(sR + c * 16384, &tmR, r_full, h * D + c * 64, row0, b);
-        tma_load_3d(sRg + c * 16384, &tmRg, r_full, h * D + c * 64, row0, b);
-      }
-      const uint32_t idesc_s = umma_idesc_bf16(128, CB, false, false);
-      const uint32_t idesc_o = umma_idesc_bf16(128, D, false, true);
-      auto load_c = [&](int it_, int buf) {
-        mbar_expect_tx(&c_full[buf], 2 * CTILE);
-        for (int c = 0; c < DC; ++c) {
-          tma_load_3d(sC + buf * CTILE + c * CB * 128, &tmC, &c_full[buf], h * D + c * 64, it_ * CB, b);
-          tma_load_3d(sCg + buf * CTILE + c * CB * 128, &tmCg, &c_full[buf], h * D + c * 64, it_ * CB, b);
-        }
-      };
-      if (NCBUF == 2) load_c(0, 0);
-      for (int it = 0; it < n_it; ++it) {
-        const int cb = (NCBUF == 2) ? (it & 1) : 0;
-        const uint32_t sCb = smem_u32(sC + cb * CTILE), sCgb = smem_u32(sCg + cb * CTILE);
-        if (NCBUF == 1) {
-          if (it > 0) mbar_wait(acc_done, (it - 1) & 1);  // previous accumulation MMAs have consumed C/Cg and P/dS
-          load_c(it, 0);
-        }
-        if (it == 0) mbar_wait(r_full, 0);
-        mbar_wait(&c_full[cb], (NCBUF == 2) ? ((it >> 1) & 1) : (it & 1));
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
-          const uint32_t coff = (kk >> 2) * CB * 128 + (kk & 3) * 32;
-          umma_bf16(tmem_base + COL_S, umma_desc_sw128(smem_u32(sR) + off, 16, 1024),
-                    umma_desc_sw128(sCb + coff, 16, 1024), idesc_s, kk > 0 ? 1u : 0u);
-        }
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
-          const uint32_t coff = (kk >> 2) * CB * 128 + (kk & 3) * 32;
-          umma_bf16(tmem_base + COL_DP, umma_desc_sw128(smem_u32(sRg) + off, 16, 1024),
-                    umma_desc_sw128(sCgb + coff, 16, 1024), idesc_s, kk > 0 ? 1u : 0u);
-        }
-        umma_commit(s_ready);
-        if (NCBUF == 2) {
-          // the other buffer was last read by the accumulation MMAs of iteration it-1 (issued before the S'/dP' MMAs of
-          // this iteration, so normally long complete): once they are done, stream the next tiles into it
-          if (it > 0) mbar_wait(acc_done, (it - 1) & 1);
-          if (it + 1 < n_it) load_c(it + 1, cb ^ 1);
-        }
-        mbar_wait(p_ready, it & 1);
-        tc_fence_after();
-        // accumulate over the CB looped positions (K dimension of these MMAs), B operands MN-major
-#pragma unroll
-        for (int kk = 0; kk < CB / 16; ++kk) {
-          const uint32_t aoff = (kk >> 2) * 16384 + (kk & 3) * 32;
-          umma_bf16(tmem_base + COL_O0, umma_desc_sw128(smem_u32(sDS) + aoff, 16, 1024),
-                    umma_desc_sw128(sCb + kk * 2048, CB * 128, 1024), idesc_o, (it > 0 || kk > 0) ? 1u : 0u);
-        }
-        if (!ROWS_ARE_Q) {
-#pragma unroll
-          for (int kk = 0; kk < CB / 16; ++kk) {
-            const uint32_t aoff = (kk >> 2) * 16384 + (kk & 3) * 32;
-            umma_bf16(tmem_base + COL_O1, umma_desc_sw128(smem_u32(sP) + aoff, 16, 1024),
-                      umma_desc_sw128(sCgb + kk * 2048, CB * 128, 1024), idesc_o,
-                      (it > 0 || kk > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(acc_done);
-      }
-    }
-  } else {
-    const int row = threadIdx.x;
-    const int ridx = row0 + row;              // q (ROWS_ARE_Q) or kv index
-    const bool rvalid = ridx < S_rows;
-    const uint32_t trow = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-    const int64_t bh = static_cast<int64_t>(b) * p.H + h;
-    // per-row scalars
-    // validity is folded into the statistics so the inner loop needs no bounds tests: an invalid query gets
-    // lse = +inf, an invalid key gets mask = -inf; either way exp2(t - lse) = 0 exactly
-    float rowA, rowB = 0.0f;
-    if (ROWS_ARE_Q) {
-      rowA = INFINITY;
-      if (rvalid) { rowA = p.lse2[bh * p.Sq + ridx]; rowB = p.delta[bh * p.Sq + ridx]; }
-    } else {
-      rowA = rvalid ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + ridx] * LOG2E : 0.0f) : -INFINITY;
-    }
-#pragma unroll 1
-    for (int it = 0; it < n_it; ++it) {
-      const int col0 = it * CB;
-      // per-column stats for this block; double-buffered: a thread can run at most one iteration ahead of the
-      // slowest (the bar.sync below), so buffer it&1 is never rewritten while still being read
-      float* sColA = sCol + (it & 1) * 256;
-      float* sColB = sColA + 128;
-      {
-        const int cidx = col0 + row;
-        float a = ROWS_ARE_Q ? -INFINITY : INFINITY, bb = 0.0f;
-        if (row < CB && cidx < S_cols) {
-          if (ROWS_ARE_Q) {
-            a = (p.mask != nullptr) ? p.mask[static_cast<int64_t>(b) * p.Skv + cidx] * LOG2E : 0.0f;
-          } else {
-            a = p.lse2[bh * p.Sq + cidx];
-            bb = p.delta[bh * p.Sq + cidx];
-          }
-        }
-        sColA[row] = a;
-        sColB[row] = bb;
-        if (!ROWS_ARE_Q && DROP) {
-          // keys-as-rows orientation: this CTA needs, for every query column of the block, the 4 words covering its
-          // 128 key rows; staged once per block (coalesced 16-byte reads) instead of one global load per element
-          uint32_t* dst = sBits + (it & 1) * 512 + row * 4;
-#pragma unroll
-          for (int w = 0; w < 4; ++w) {
-            const int wi = (row0 >> 5) + w;
-            dst[w] = (row < CB && cidx < S_cols && wi < p.W) ? __ldg(p.dmask + (bh * p.Sq + cidx) * p.W + wi) : 0u;
-          }
-        }
-      }
-      const uint32_t* sBitsCur = sBits + (it & 1) * 512;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (it > 0) mbar_wait(acc_done, (it - 1) & 1);  // P/dS smem free again
-      mbar_wait(s_ready, it & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < CB / 32; ++c) {
-        uint32_t rs[32], rd[32];
-        tmem_ld32(trow + COL_S + c * 32, rs);
-        tmem_ld32(trow + COL_DP + c * 32, rd);
-        tmem_ld_wait();
-        float pv[32], ds[32];
-        uint32_t bits = 0xFFFFFFFFu;
-        if (ROWS_ARE_Q && DROP && rvalid) {
-          const int w = (col0 >> 5) + c;
-          if (w < p.W) bits = __ldg(p.dmask + (bh * p.Sq + ridx) * p.W + w);
-        }
-        const float4* cA4 = reinterpret_cast<const float4*>(sColA) + c * 8;
-        const float4* cB4 = reinterpret_cast<const float4*>(sColB) + c * 8;
-#pragma unroll
-        for (int q4 = 0; q4 < 8; ++q4) {
-          const float4 ca = cA4[q4];
-          const float ca_[4] = {ca.x, ca.y, ca.z, ca.w};
-          float cb_[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-          if (!ROWS_ARE_Q) {
-            const float4 cb = cB4[q4];
-            cb_[0] = cb.x; cb_[1] = cb.y; cb_[2] = cb.z; cb_[3] = cb.w;
-          }
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int j = q4 * 4 + k;
-            const int cl = c * 32 + j;
-            float pr, dl;
-            if (ROWS_ARE_Q) {
-              pr = ex2_approx(fmaf(__uint_as_float(rs[j]), p.scale2, ca_[k]) - rowA);
-              dl = rowB;
-            } else {
-              pr = ex2_approx(fmaf(__uint_as_float(rs[j]), p.scale2, rowA) - ca_[k]);
-              dl = cb_[k];
-            }
-            float dp = __uint_as_float(rd[j]);
-            float pk = pr;
-            if (DROP) {
-              bool kp;
-              if (ROWS_ARE_Q) kp = (bits >> j) & 1u;
-              else kp = (sBitsCur[cl * 4 + (row >> 5)] >> (row & 31)) & 1u;   // warp-uniform address: broadcast
-              dp = kp ? dp * p.dscale : 0.0f;
-              pk = kp ? pr * p.dscale : 0.0f;
-            }
-            ds[j] = pr * (dp - dl);
-            pv[j] = pk;
-          }
-        }
-        uint8_t* dsrow = sDS + (c >> 1) * 16384 + row * 128;
-        uint8_t* prow = sP + (c >> 1) * 16384 + row * 128;
-#pragma unroll
-        for (int qd = 0; qd < 4; ++qd) {
-          const int chunk = ((c & 1) * 4 + qd) ^ (row & 7);
-          uint4 o;
-          o.x = pack_bf16x2(ds[qd * 8 + 0], ds[qd * 8 + 1]);
-          o.y = pack_bf16x2(ds[qd * 8 + 2], ds[qd * 8 + 3]);
-          o.z = pack_bf16x2(ds[qd * 8 + 4], ds[qd * 8 + 5]);
-          o.w = pack_bf16x2(ds[qd * 8 + 6], ds[qd * 8 + 7]);
-          *reinterpret_cast<uint4*>(dsrow + chunk * 16) = o;
-          if (!ROWS_ARE_Q) {
-            o.x = pack_bf16x2(pv[qd * 8 + 0], pv[qd * 8 + 1]);
-            o.y = pack_bf16x2(pv[qd * 8 + 2], pv[qd * 8 + 3]);
-            o.z = pack_bf16x2(pv[qd * 8 + 4], pv[qd * 8 + 5]);
-            o.w = pack_bf16x2(pv[qd * 8 + 6], pv[qd * 8 + 7]);
-            *reinterpret_cast<uint4*>(prow + chunk * 16) = o;
-          }
-        }
-      }
-      fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive(p_ready);
-    }
-    // ---- epilogue ----
-    mbar_wait(acc_done, (n_it - 1) & 1);
-    tc_fence_after();
-#pragma unroll
-    for (int o = 0; o < (ROWS_ARE_Q ? 1 : 2); ++o) {
-      bf16* outp = (o == 0) ? p.out0 : p.out1;
-      const int64_t ld = (o == 0) ? p.ld0 : p.ld1;
-      const float mul = (o == 0) ? p.scale : 1.0f;
-#pragma unroll
-      for (int c = 0; c < D / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld32(trow + (o == 0 ? COL_O0 : COL_O1) + c * 32, r);
-        tmem_ld_wait();
-        if (rvalid) {
-          uint4* dst = reinterpret_cast<uint4*>(outp + (static_cast<int64_t>(b) * S_rows + ridx) * ld + h * D + c * 32);
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd) {
-            uint4 v;
-            v.x = pack_bf16x2(__uint_as_float(r[qd * 8 + 0]) * mul, __uint_as_float(r[qd * 8 + 1]) * mul);
-            v.y = pack_bf16x2(__uint_as_float(r[qd * 8 + 2]) * mul, __uint_as_float(r[qd * 8 + 3]) * mul);
-            v.z = pack_bf16x2(__uint_as_float(r[qd * 8 + 4]) * mul, __uint_as_float(r[qd * 8 + 5]) * mul);
-            v.w = pack_bf16x2(__uint_as_float(r[qd * 8 + 6]) * mul, __uint_as_float(r[qd * 8 + 7]) * mul);
-            dst[qd] = v;
-          }
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// ----------------------------------------------------------------------------------------------
-// fused backward (d = 64, Sq, Skv <= 256): one CTA per (batch, head)
-//
-// Q, dO, K, V of the head stay resident in shared memory (8 tiles of [128 x 64]).  For every 128x128 block pair
-// (query block i, key block j) the scores S = Q_i K_j^T and dP = dO_i V_j^T are computed ONCE (the two-kernel path
-// recomputes them, and the exp / dropout / dS arithmetic, in both launches); thread == query row turns them into
-// P' and dS' (bf16, K-major [q][kv] in smem) and three accumulations consume the same two buffers:
-//     dQ_i += dS' K_j        A = dS' K-major  (M = q),   B = K_j  MN-major
-//     dK_j += dS'^T Q_i      A = dS' MN-major (M = kv),  B = Q_i  MN-major      (transposed view, no data movement)
-//     dV_j += P'^T dO_i      A = P'  MN-major (M = kv),  B = dO_i MN-major
-// TMEM (512 columns): S 128 | dP 128 | dQ_0 64 | dQ_1 64 | dK_j 64 | dV_j 64.
-// 288 threads: warps 0..7 compute (two threads per row, alternate 32-column chunks), warp 8 = TMA + MMA issue.
-// ----------------------------------------------------------------------------------------------
-struct AttnBwdFusedDev {
-  int B, H, Sq, Skv;
   const float* mask;
-  const float* lse2;
-  const float* delta;
+  const float* lse2;      // [B, H, Sq]
+  const float* delta;     // [B, H, Sq]
   const uint32_t* dmask;
   int W;
-  float dscale, scale2, scale;
-  bf16* dq; int64_t ld_dq;
-  bf16* dk; int64_t ld_dk;
-  bf16* dv; int64_t ld_dv;
+  float dscale, scale, scale2;
+  bf16* out0; int64_t ld0;   // dq (dq kernel) / dk (dkv kernel)
+  bf16* out1; int64_t ld1;   // dv (dkv kernel)
 };
 
-template <bool DROP>
-__global__ void __launch_bounds__(288, 1)
-attn_bwd_fused_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
-                      const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                      AttnBwdFusedDev p) {
-  griddep_launch();
-  griddep_wait();
-  constexpr int D = 64;
-  constexpr int TILE = 16384;
+// dQ for 64 query rows.  smem: Q, dO tiles; two stages of (K block, V block)
+template <int D, bool DROP>
+__global__ void __launch_bounds__(AT_THREADS)
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
+                   const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, AttnBwdDev p) {
+  constexpr int TB = D / 64 * AT_ROWS * 128;
+  constexpr int DT = D / 8;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
-  uint8_t* sQ = smem;                 // [2][128 x 128B]
-  uint8_t* sdO = sQ + 2 * TILE;
-  uint8_t* sK = sdO + 2 * TILE;
-  uint8_t* sV = sK + 2 * TILE;
-  uint8_t* sP = sV + 2 * TILE;        // [128 q x 128 kv] bf16 = 2 chunks of [128 x 128B]
-  uint8_t* sDS = sP + 2 * TILE;
-  float* sLse = reinterpret_cast<float*>(sDS + 2 * TILE);   // [256] per query: lse (log2 domain), +inf if invalid
-  float* sDel = sLse + 256;                                 // [256] per query: delta
-  float* sMsk = sDel + 256;                                 // [256] per key: additive mask * log2e, -inf if invalid
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sMsk + 256);
-  uint64_t* r_full = bars;
-  uint64_t* s_ready = bars + 1;
-  uint64_t* p_ready = bars + 2;
-  uint64_t* acc_done = bars + 3;
-  uint64_t* kv_read = bars + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5);
-  constexpr uint32_t COL_S = 0, COL_DP = 128, COL_DQ = 256, COL_DK = 384, COL_DV = 448;
+  uint8_t* sQ = smem;
+  uint8_t* sdO = smem + TB;
+  uint8_t* sKV = smem + 2 * TB;
+  const int NKB = (p.Skv + AT_ROWS - 1) / AT_ROWS;
+  float* sMask = reinterpret_cast<float*>(sKV + 4 * TB);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sMask + NKB * AT_ROWS);
 
+  griddep_launch();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int h = blockIdx.x, b = blockIdx.y;
-  const int ni = (p.Sq + 127) / 128, nj = (p.Skv + 127) / 128;
+  const int q0 = blockIdx.x * AT_ROWS, h = blockIdx.y, b = blockIdx.z;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmdO);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  griddep_wait();
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(&bars[0], 2 * TB);
+    load_tile<D, AT_ROWS>(sQ, &tmQ, &bars[0], h * D, q0, b);
+    load_tile<D, AT_ROWS>(sdO, &tmdO, &bars[0], h * D, q0, b);
+    for (int kb = 0; kb < 2 && kb < NKB; ++kb) {
+      mbar_expect_tx(&bars[1 + kb], 2 * TB);
+      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, kb * AT_ROWS, b);
+      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, kb * AT_ROWS, b);
+    }
+  }
+  for (int i = threadIdx.x; i < NKB * AT_ROWS; i += AT_THREADS)
+    sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + i] * LOG2E : 0.0f) : -INFINITY;
+  __syncthreads();
+
+  const int g = lane >> 2, t4 = lane & 3;
+  const int r0 = warp * 16;
   const int64_t bh = static_cast<int64_t>(b) * p.H + h;
+  float lse[2], dlt[2];
+  const uint32_t* dm[2] = {nullptr, nullptr};
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int q = q0 + r0 + g + hr * 8;
+    const bool ok = q < p.Sq;
+    lse[hr] = ok ? p.lse2[bh * p.Sq + q] : INFINITY;      // rows past the sequence: P = 0
+    dlt[hr] = ok ? p.delta[bh * p.Sq + q] : 0.0f;
+    if (DROP && ok) dm[hr] = p.dmask + (bh * p.Sq + q) * p.W;
+  }
+  float dq[DT][4];
+#pragma unroll
+  for (int i = 0; i < DT; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.0f;
+  mbar_wait(&bars[0], 0);
+  const uint32_t uQ = smem_u32(sQ), udO = smem_u32(sdO);
 
-  if (warp == 8) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-      mbar_init(r_full, 1);
-      mbar_init(s_ready, 1);
-      mbar_init(p_ready, 256);
-      mbar_init(acc_done, 1);
-      mbar_init(kv_read, 256);
-      fence_barrier_init();
+  for (int kb = 0; kb < NKB; ++kb) {
+    const int st = kb & 1;
+    mbar_wait(&bars[1 + st], (kb >> 1) & 1);
+    const uint32_t uK = smem_u32(sKV + 2 * st * TB), uV = uK + TB;
+    float s[8][4], dp[8][4];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.0f;
+      dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.0f;
     }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  } else {
-    for (int i = threadIdx.x; i < 256; i += 256) {
-      const bool qv = i < p.Sq, kv = i < p.Skv;
-      sLse[i] = qv ? p.lse2[bh * p.Sq + i] : INFINITY;
-      sDel[i] = qv ? p.delta[bh * p.Sq + i] : 0.0f;
-      sMsk[i] = kv ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + i] * LOG2E : 0.0f) : -INFINITY;
+    mma_abt<D, 8, AT_ROWS, AT_ROWS>(s, uQ, r0, uK, lane);
+    mma_abt<D, 8, AT_ROWS, AT_ROWS>(dp, udO, r0, uV, lane);
+    uint32_t bits[2][2] = {{0xFFFFFFFFu, 0xFFFFFFFFu}, {0xFFFFFFFFu, 0xFFFFFFFFu}};
+    if (DROP) {
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        if (dm[hr] != nullptr) {
+          bits[hr][0] = __ldg(dm[hr] + kb * 2);
+          if (kb * 2 + 1 < p.W) bits[hr][1] = __ldg(dm[hr] + kb * 2 + 1);
+        }
+      }
+    }
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      const float2 mk = *reinterpret_cast<const float2*>(sMask + kb * AT_ROWS + nt * 8 + 2 * t4);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int hr = e >> 1;
+        const float pe = ex2_approx(fmaf(s[nt][e], p.scale2, (e & 1) ? mk.y : mk.x) - lse[hr]);
+        float dpe = dp[nt][e];
+        if (DROP) {
+          const int col = nt * 8 + 2 * t4 + (e & 1);
+          dpe = ((bits[hr][col >> 5] >> (col & 31)) & 1u) ? dpe * p.dscale : 0.0f;
+        }
+        s[nt][e] = pe * (dpe - dlt[hr]);                    // dS
+      }
+    }
+    uint32_t sf[4][4];
+    acc_to_a<8>(s, sf);
+    mma_pb<D, 4, AT_ROWS>(dq, sf, uK, lane);
+    fence_proxy_async();
+    __syncthreads();
+    if (threadIdx.x == 0 && kb + 2 < NKB) {
+      mbar_expect_tx(&bars[1 + st], 2 * TB);
+      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, (kb + 2) * AT_ROWS, b);
+      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, (kb + 2) * AT_ROWS, b);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 8) {
-    if (lane == 0) {
-      mbar_expect_tx(r_full, (2 * ni + 2 * nj) * TILE);
-      for (int i = 0; i < ni; ++i) {
-        tma_load_3d(sQ + i * TILE, &tmQ, r_full, h * D, i * 128, b);
-        tma_load_3d(sdO + i * TILE, &tmdO, r_full, h * D, i * 128, b);
-      }
-      for (int j = 0; j < nj; ++j) {
-        tma_load_3d(sK + j * TILE, &tmK, r_full, h * D, j * 128, b);
-        tma_load_3d(sV + j * TILE, &tmV, r_full, h * D, j * 128, b);
-      }
-      const uint32_t idesc_s = umma_idesc_bf16(128, 128, false, false);
-      const uint32_t idesc_q = umma_idesc_bf16(128, D, false, true);   // A K-major,  B MN-major
-      const uint32_t idesc_t = umma_idesc_bf16(128, D, true, true);    // A MN-major, B MN-major
-      mbar_wait(r_full, 0);
-      auto issue_scores = [&](int i, int j) {      // S = Q_i K_j^T, dP = dO_i V_j^T
-        const uint32_t aQ_ = smem_u32(sQ + i * TILE), adO_ = smem_u32(sdO + i * TILE);
-        const uint32_t aK_ = smem_u32(sK + j * TILE), aV_ = smem_u32(sV + j * TILE);
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          umma_bf16(tmem_base + COL_S, umma_desc_sw128(aQ_ + kk * 32, 16, 1024), umma_desc_sw128(aK_ + kk * 32, 16, 1024),
-                    idesc_s, kk > 0 ? 1u : 0u);
+  for (int hr = 0; hr < 2; ++hr) {
+    const int q = q0 + r0 + g + hr * 8;
+    if (q >= p.Sq) continue;
+    bf16* dst = p.out0 + (static_cast<int64_t>(b) * p.Sq + q) * p.ld0 + h * D;
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          umma_bf16(tmem_base + COL_DP, umma_desc_sw128(adO_ + kk * 32, 16, 1024), umma_desc_sw128(aV_ + kk * 32, 16, 1024),
-                    idesc_s, kk > 0 ? 1u : 0u);
-        umma_commit(s_ready);
-      };
-      int pair = 0;
-      for (int j = 0; j < nj; ++j) {
-        for (int i = 0; i < ni; ++i, ++pair) {
-          tc_fence_after();
-          const uint32_t aQ = smem_u32(sQ + i * TILE), adO = smem_u32(sdO + i * TILE);
-          const uint32_t aK = smem_u32(sK + j * TILE);
-          issue_scores(i, j);
-          mbar_wait(p_ready, pair & 1);
-          // dK_j / dV_j of the previous key block must have been read out before the first pair of this block overwrites them
-          if (i == 0 && j > 0) mbar_wait(kv_read, (j - 1) & 1);
-          tc_fence_after();
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {   // K dimension = the 128 keys of block j
-            const uint32_t aoff = (kk >> 2) * TILE + (kk & 3) * 32;
-            umma_bf16(tmem_base + COL_DQ + i * D, umma_desc_sw128(smem_u32(sDS) + aoff, 16, 1024),
-                      umma_desc_sw128(aK + kk * 2048, TILE, 1024), idesc_q, (j > 0 || kk > 0) ? 1u : 0u);
-          }
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {   // K dimension = the 128 queries of block i; A = transposed views
-            umma_bf16(tmem_base + COL_DK, umma_desc_sw128(smem_u32(sDS) + kk * 2048, TILE, 1024),
-                      umma_desc_sw128(aQ + kk * 2048, TILE, 1024), idesc_t, (i > 0 || kk > 0) ? 1u : 0u);
-            umma_bf16(tmem_base + COL_DV, umma_desc_sw128(smem_u32(sP) + kk * 2048, TILE, 1024),
-                      umma_desc_sw128(adO + kk * 2048, TILE, 1024), idesc_t, (i > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(acc_done);
-        }
-      }
-    }
-  } else {
-    const int quarter = warp & 3, half = warp >> 2;
-    const int row = quarter * 32 + lane;
-    const uint32_t trow = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    int pair = 0;
-    for (int j = 0; j < nj; ++j) {
-      for (int i = 0; i < ni; ++i, ++pair) {
-        const int q = i * 128 + row;
-        const float l2 = sLse[q], dl = sDel[q];
-        if (pair > 0) mbar_wait(acc_done, (pair - 1) & 1);   // P'/dS' buffers are free again
-        mbar_wait(s_ready, pair & 1);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = half; c < 4; c += 2) {
-          uint32_t rs[32], rd[32];
-          tmem_ld32(trow + COL_S + c * 32, rs);
-          tmem_ld32(trow + COL_DP + c * 32, rd);
-          tmem_ld_wait();
-          uint32_t bits = 0xFFFFFFFFu;
-          if (DROP && q < p.Sq) {
-            const int w = j * 4 + c;
-            if (w < p.W) bits = __ldg(p.dmask + (bh * p.Sq + q) * p.W + w);
-          }
-          const float4* m4 = reinterpret_cast<const float4*>(sMsk + j * 128 + c * 32);
-          float pv[32], ds[32];
-#if MMFB_F32X2
-          // two lanes per FMA-pipe slot; dropout enters as the factor kf = keep ? 1/(1-p) : 0, so that
-          // dS' = P (dP kf - delta) is one FFMA2 + one FMUL2 and P' = P kf one FMUL2 per pair
-          const uint64_t sc2 = pk2(p.scale2, p.scale2), nl2 = pk2(-l2, -l2), ndl2 = pk2(-dl, -dl);
-#pragma unroll
-          for (int q4 = 0; q4 < 8; ++q4) {
-            const float4 m = m4[q4];
-            const float mm[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-            for (int k = 0; k < 4; k += 2) {
-              const int jx = q4 * 4 + k;
-              float a0, a1;
-              upk2(add2(fma2(pk2(__uint_as_float(rs[jx]), __uint_as_float(rs[jx + 1])), sc2, pk2(mm[k], mm[k + 1])), nl2), a0, a1);
-              const uint64_t pr = pk2(ex2_approx(a0), ex2_approx(a1));
-              const uint64_t dp = pk2(__uint_as_float(rd[jx]), __uint_as_float(rd[jx + 1]));
-              if (DROP) {
-                const uint64_t kf = pk2(((bits >> jx) & 1u) ? p.dscale : 0.0f, ((bits >> (jx + 1)) & 1u) ? p.dscale : 0.0f);
-                upk2(mul2(pr, fma2(dp, kf, ndl2)), ds[jx], ds[jx + 1]);
-                upk2(mul2(pr, kf), pv[jx], pv[jx + 1]);
-              } else {
-                upk2(mul2(pr, add2(dp, ndl2)), ds[jx], ds[jx + 1]);
-                upk2(pr, pv[jx], pv[jx + 1]);
-              }
-            }
-          }
-#else
-#pragma unroll
-          for (int q4 = 0; q4 < 8; ++q4) {
-            const float4 m = m4[q4];
-            const float mm[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int jx = q4 * 4 + k;
-              const float pr = ex2_approx(fmaf(__uint_as_float(rs[jx]), p.scale2, mm[k]) - l2);
-              float dp = __uint_as_float(rd[jx]);
-              float pk = pr;
-              if (DROP) {
-                const bool kp = (bits >> jx) & 1u;
-                dp = kp ? dp * p.dscale : 0.0f;
-                pk = kp ? pr * p.dscale : 0.0f;
-              }
-              ds[jx] = pr * (dp - dl);
-              pv[jx] = pk;
-            }
-          }
-#endif
-          uint8_t* dsrow = sDS + (c >> 1) * TILE + row * 128;
-          uint8_t* prow = sP + (c >> 1) * TILE + row * 128;
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd) {
-            const int chunk = ((c & 1) * 4 + qd) ^ (row & 7);
-            uint4 o;
-            o.x = pack_bf16x2(ds[qd * 8 + 0], ds[qd * 8 + 1]);
-            o.y = pack_bf16x2(ds[qd * 8 + 2], ds[qd * 8 + 3]);
-            o.z = pack_bf16x2(ds[qd * 8 + 4], ds[qd * 8 + 5]);
-            o.w = pack_bf16x2(ds[qd * 8 + 6], ds[qd * 8 + 7]);
-            *reinterpret_cast<uint4*>(dsrow + chunk * 16) = o;
-            o.x = pack_bf16x2(pv[qd * 8 + 0], pv[qd * 8 + 1]);
-            o.y = pack_bf16x2(pv[qd * 8 + 2], pv[qd * 8 + 3]);
-            o.z = pack_bf16x2(pv[qd * 8 + 4], pv[qd * 8 + 5]);
-            o.w = pack_bf16x2(pv[qd * 8 + 6], pv[qd * 8 + 7]);
-            *reinterpret_cast<uint4*>(prow + chunk * 16) = o;
-          }
-        }
-        fence_proxy_async();
-        tc_fence_before();
-        mbar_arrive(p_ready);
-      }
-      // ---- dK_j, dV_j are complete: rows = keys of block j; this thread stores 32 of the 64 columns of each ----
-      mbar_wait(acc_done, (pair - 1) & 1);
-      tc_fence_after();
-      {
-        const int kvr = j * 128 + row;
-        uint32_t rk[32], rv[32];
-        tmem_ld32(trow + COL_DK + half * 32, rk);
-        tmem_ld32(trow + COL_DV + half * 32, rv);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(kv_read);
-        if (kvr < p.Skv) {
-          uint4* dk4 = reinterpret_cast<uint4*>(p.dk + (static_cast<int64_t>(b) * p.Skv + kvr) * p.ld_dk + h * D + half * 32);
-          uint4* dv4 = reinterpret_cast<uint4*>(p.dv + (static_cast<int64_t>(b) * p.Skv + kvr) * p.ld_dv + h * D + half * 32);
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd) {
-            uint4 o;
-            o.x = pack_bf16x2(__uint_as_float(rk[qd * 8 + 0]) * p.scale, __uint_as_float(rk[qd * 8 + 1]) * p.scale);
-            o.y = pack_bf16x2(__uint_as_float(rk[qd * 8 + 2]) * p.scale, __uint_as_float(rk[qd * 8 + 3]) * p.scale);
-            o.z = pack_bf16x2(__uint_as_float(rk[qd * 8 + 4]) * p.scale, __uint_as_float(rk[qd * 8 + 5]) * p.scale);
-            o.w = pack_bf16x2(__uint_as_float(rk[qd * 8 + 6]) * p.scale, __uint_as_float(rk[qd * 8 + 7]) * p.scale);
-            dk4[qd] = o;
-            o.x = pack_bf16x2(__uint_as_float(rv[qd * 8 + 0]), __uint_as_float(rv[qd * 8 + 1]));
-            o.y = pack_bf16x2(__uint_as_float(rv[qd * 8 + 2]), __uint_as_float(rv[qd * 8 + 3]));
-            o.z = pack_bf16x2(__uint_as_float(rv[qd * 8 + 4]), __uint_as_float(rv[qd * 8 + 5]));
-            o.w = pack_bf16x2(__uint_as_float(rv[qd * 8 + 6]), __uint_as_float(rv[qd * 8 + 7]));
-            dv4[qd] = o;
-          }
-        }
-      }
-    }
-    // ---- dQ_i: rows = queries ----
-    for (int i = 0; i < ni; ++i) {
-      const int q = i * 128 + row;
-      uint32_t rq[32];
-      tmem_ld32(trow + COL_DQ + i * D + half * 32, rq);
-      tmem_ld_wait();
-      if (q < p.Sq) {
-        uint4* dq4 = reinterpret_cast<uint4*>(p.dq + (static_cast<int64_t>(b) * p.Sq + q) * p.ld_dq + h * D + half * 32);
-#pragma unroll
-        for (int qd = 0; qd < 4; ++qd) {
-          uint4 o;
-          o.x = pack_bf16x2(__uint_as_float(rq[qd * 8 + 0]) * p.scale, __uint_as_float(rq[qd * 8 + 1]) * p.scale);
-          o.y = pack_bf16x2(__uint_as_float(rq[qd * 8 + 2]) * p.scale, __uint_as_float(rq[qd * 8 + 3]) * p.scale);
-          o.z = pack_bf16x2(__uint_as_float(rq[qd * 8 + 4]) * p.scale, __uint_as_float(rq[qd * 8 + 5]) * p.scale);
-          o.w = pack_bf16x2(__uint_as_float(rq[qd * 8 + 6]) * p.scale, __uint_as_float(rq[qd * 8 + 7]) * p.scale);
-          dq4[qd] = o;
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    for (int i = 0; i < DT; ++i)
+      *reinterpret_cast<uint32_t*>(dst + i * 8 + 2 * t4) = pack_bf16x2(dq[i][hr * 2] * p.scale, dq[i][hr * 2 + 1] * p.scale);
   }
 }
 
-// ----------------------------------------------------------------------------------------------
-// fused backward, 16 compute warps (d = 64, Sq, Skv <= 256)
-//
-// Same data flow, TMEM map and MMAs as attn_bwd_fused_kernel, re-balanced after its ncu capture (IPC ~0.3 per scheduler
-// with 2 compute warps each, every pair a serial chain  scores -> exp/dS arithmetic -> 24 accumulation MMAs):
-//   * FOUR threads per query row (warp w: TMEM lane quarter w & 3, 32-column chunk w >> 2 of the 128-wide key block):
-//     4 warps per scheduler hide the MUFU / TMEM-load latencies; a thread handles its chunk as two 16-column halves so the
-//     kernel fits the 120 registers that 544 threads leave.
-//   * overlapped issue order: S/dP of pair k+1 are issued as soon as pair k's have been read, BEFORE the accumulations of
-//     pair k; the compute threads wait for those accumulations only right before they overwrite P'/dS'.
-//   * the operand tiles arrive on four barriers in order of first use (K_0,V_0 | Q_0,dO_0 | Q_1,dO_1 | K_1,V_1): the first
-//     pair starts after 64 KB instead of 128 KB; the dropout word of a chunk is fetched before the score barrier.
-// Accumulation order is that of attn_bwd_fused_kernel, so the results are bit-identical to it.
-// ----------------------------------------------------------------------------------------------
-template <bool DROP>
-__global__ void __launch_bounds__(544, 1)
-attn_bwd_fused16_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
-                        const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                        AttnBwdFusedDev p) {
-  griddep_launch();
-  griddep_wait();
-  constexpr int D = 64;
-  constexpr int TILE = 16384;
+// dK, dV for 64 key rows.  smem: K, V tiles; two stages of (Q block, dO block) of QB query rows.  The register tiles are
+// transposed products (rows = keys, columns = queries).
+template <int D, bool DROP, int QB>
+__global__ void __launch_bounds__(AT_THREADS)
+attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                    const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO, AttnBwdDev p) {
+  constexpr int TB = D / 64 * AT_ROWS * 128;    // resident key tile
+  constexpr int QTB = D / 64 * QB * 128;        // streamed query block
+  constexpr int DT = D / 8, NT = QB / 8;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
-  uint8_t* sQ = smem;                 // [2][128 x 128B]
-  uint8_t* sdO = sQ + 2 * TILE;
-  uint8_t* sK = sdO + 2 * TILE;
-  uint8_t* sV = sK + 2 * TILE;
-  uint8_t* sP = sV + 2 * TILE;        // [128 q x 128 kv] bf16 = 2 chunks of [128 x 128B]
-  uint8_t* sDS = sP + 2 * TILE;
-  float* sLse = reinterpret_cast<float*>(sDS + 2 * TILE);
-  float* sDel = sLse + 256;
-  float* sMsk = sDel + 256;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sMsk + 256);
-  uint64_t* q_full = bars;            // [2]  Q_i + dO_i
-  uint64_t* kv_full = bars + 2;       // [2]  K_j + V_j
-  uint64_t* s_ready = bars + 4;
-  uint64_t* p_ready = bars + 5;
-  uint64_t* acc_done = bars + 6;
-  uint64_t* kv_read = bars + 7;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-  constexpr uint32_t COL_S = 0, COL_DP = 128, COL_DQ = 256, COL_DK = 384, COL_DV = 448;
+  uint8_t* sK = smem;
+  uint8_t* sV = smem + TB;
+  uint8_t* sQd = smem + 2 * TB;                 // stage s: Q at sQd + 2 s QTB, dO at sQd + (2 s + 1) QTB
+  float* sMask = reinterpret_cast<float*>(sQd + 4 * QTB);   // [64] this tile's keys
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sMask + AT_ROWS);
 
+  griddep_launch();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int h = blockIdx.x, b = blockIdx.y;
-  const int ni = (p.Sq + 127) / 128, nj = (p.Skv + 127) / 128;
+  const int k0 = blockIdx.x * AT_ROWS, h = blockIdx.y, b = blockIdx.z;
+  const int NQB = (p.Sq + QB - 1) / QB;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmdO);
+    for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  griddep_wait();
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(&bars[0], 2 * TB);
+    load_tile<D, AT_ROWS>(sK, &tmK, &bars[0], h * D, k0, b);
+    load_tile<D, AT_ROWS>(sV, &tmV, &bars[0], h * D, k0, b);
+    for (int qb = 0; qb < 2 && qb < NQB; ++qb) {
+      mbar_expect_tx(&bars[1 + qb], 2 * QTB);
+      load_tile<D, QB>(sQd + 2 * qb * QTB, &tmQ, &bars[1 + qb], h * D, qb * QB, b);
+      load_tile<D, QB>(sQd + (2 * qb + 1) * QTB, &tmdO, &bars[1 + qb], h * D, qb * QB, b);
+    }
+  }
+  for (int i = threadIdx.x; i < AT_ROWS; i += AT_THREADS) {
+    const int kv = k0 + i;
+    sMask[i] = (kv < p.Skv) ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + kv] * LOG2E : 0.0f) : -INFINITY;
+  }
+  __syncthreads();
+
+  const int g = lane >> 2, t4 = lane & 3;
+  const int r0 = warp * 16;
   const int64_t bh = static_cast<int64_t>(b) * p.H + h;
+  const float mk[2] = {sMask[r0 + g], sMask[r0 + g + 8]};
+  // keys r0 + g and r0 + g + 8 share one keep-bit word (16-aligned group of keys)
+  const int kw = (k0 + r0) >> 5, ksh0 = (k0 + r0 + g) & 31;
+  float dk[DT][4], dv[DT][4];
+#pragma unroll
+  for (int i = 0; i < DT; ++i) {
+    dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = 0.0f;
+    dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.0f;
+  }
+  mbar_wait(&bars[0], 0);
+  const uint32_t uK = smem_u32(sK), uV = smem_u32(sV);
 
-  if (warp == 16) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-      mbar_init(&q_full[0], 1); mbar_init(&q_full[1], 1);
-      mbar_init(&kv_full[0], 1); mbar_init(&kv_full[1], 1);
-      mbar_init(s_ready, 1);
-      mbar_init(p_ready, 512);
-      mbar_init(acc_done, 1);
-      mbar_init(kv_read, 512);
-      fence_barrier_init();
-      // operand tiles in order of first use; nothing here depends on the barrier below
-      auto load_kv = [&](int j) {
-        mbar_expect_tx(&kv_full[j], 2 * TILE);
-        tma_load_3d(sK + j * TILE, &tmK, &kv_full[j], h * D, j * 128, b);
-        tma_load_3d(sV + j * TILE, &tmV, &kv_full[j], h * D, j * 128, b);
-      };
-      auto load_q = [&](int i) {
-        mbar_expect_tx(&q_full[i], 2 * TILE);
-        tma_load_3d(sQ + i * TILE, &tmQ, &q_full[i], h * D, i * 128, b);
-        tma_load_3d(sdO + i * TILE, &tmdO, &q_full[i], h * D, i * 128, b);
-      };
-      load_kv(0);
-      for (int i = 0; i < ni; ++i) load_q(i);
-      for (int j = 1; j < nj; ++j) load_kv(j);
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  } else {
-    if (threadIdx.x < 256) {
-      const int i = threadIdx.x;
-      const bool qv = i < p.Sq, kv = i < p.Skv;
-      sLse[i] = qv ? p.lse2[bh * p.Sq + i] : INFINITY;
-      sDel[i] = qv ? p.delta[bh * p.Sq + i] : 0.0f;
-      sMsk[i] = kv ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + i] * LOG2E : 0.0f) : -INFINITY;
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // 32-key chunks whose keys are ALL masked out (additive -10000 or beyond Skv) have P = exp2(-14427 + ...) = 0 and dS = 0
-  // exactly: their arithmetic is skipped (zeros are stored).  A sample without any attendable key keeps every chunk.
-  uint32_t my_act = 0;            // bit j: this thread's chunk (warp >> 2) of key block j has an attendable key
-  if (warp < 16) {
-    const int cc = warp >> 2;
+  for (int qb = 0; qb < NQB; ++qb) {
+    const int st = qb & 1;
+    mbar_wait(&bars[1 + st], (qb >> 1) & 1);
+    const uint32_t uQ = smem_u32(sQd + 2 * st * QTB), udO = uQ + QTB;
+    float s[NT][4], dp[NT][4];
 #pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const float4* m4 = reinterpret_cast<const float4*>(sMsk + j * 128 + cc * 32);
-      bool any = false;
+    for (int i = 0; i < NT; ++i) {
+      s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.0f;
+      dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.0f;
+    }
+    mma_abt<D, NT, AT_ROWS, QB>(s, uK, r0, uQ, lane);      // S^T  [keys x queries]
+    mma_abt<D, NT, AT_ROWS, QB>(dp, uV, r0, udO, lane);    // dP^T
+    float pd[NT][4];                                        // dropped probabilities P^T * keep * dscale
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float4 m = m4[i];
-        any = any || m.x > -5000.0f || m.y > -5000.0f || m.z > -5000.0f || m.w > -5000.0f;
+    for (int nt = 0; nt < NT; ++nt) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int q = qb * QB + nt * 8 + 2 * t4 + j;
+        const bool ok = q < p.Sq;
+        const float lse = ok ? __ldg(p.lse2 + bh * p.Sq + q) : INFINITY;
+        const float dlt = ok ? __ldg(p.delta + bh * p.Sq + q) : 0.0f;
+        uint32_t w = 0xFFFFFFFFu;
+        if (DROP && ok && k0 + r0 < p.Skv) w = __ldg(p.dmask + (bh * p.Sq + q) * p.W + kw);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int e = hr * 2 + j;
+          const float pe = ex2_approx(fmaf(s[nt][e], p.scale2, mk[hr]) - lse);
+          const bool keep = !DROP || ((w >> (ksh0 + hr * 8)) & 1u);
+          const float dpe = keep ? dp[nt][e] * p.dscale : 0.0f;
+          pd[nt][e] = keep ? pe * p.dscale : 0.0f;
+          s[nt][e] = pe * (dpe - dlt);                      // dS^T
+        }
       }
-      if (any) my_act |= 1u << j;
+    }
+    uint32_t pf[NT / 2][4], sf[NT / 2][4];
+    acc_to_a<NT>(pd, pf);
+    acc_to_a<NT>(s, sf);
+    mma_pb<D, NT / 2, QB>(dv, pf, udO, lane);
+    mma_pb<D, NT / 2, QB>(dk, sf, uQ, lane);
+    fence_proxy_async();
+    __syncthreads();
+    if (threadIdx.x == 0 && qb + 2 < NQB) {
+      mbar_expect_tx(&bars[1 + st], 2 * QTB);
+      load_tile<D, QB>(sQd + 2 * st * QTB, &tmQ, &bars[1 + st], h * D, (qb + 2) * QB, b);
+      load_tile<D, QB>(sQd + (2 * st + 1) * QTB, &tmdO, &bars[1 + st], h * D, (qb + 2) * QB, b);
     }
   }
-  if (!__syncthreads_or(my_act != 0)) my_act = 3u;
-
-  if (warp == 16) {
-    if (lane == 0) {
-      const uint32_t idesc_s = umma_idesc_bf16(128, 128, false, false);
-      const uint32_t idesc_q = umma_idesc_bf16(128, D, false, true);   // A K-major,  B MN-major
-      const uint32_t idesc_t = umma_idesc_bf16(128, D, true, true);    // A MN-major, B MN-major
-      auto issue_scores = [&](int i, int j) {      // S = Q_i K_j^T, dP = dO_i V_j^T
-        mbar_wait(&q_full[i], 0);
-        mbar_wait(&kv_full[j], 0);
-        tc_fence_after();
-        const uint32_t aQ_ = smem_u32(sQ + i * TILE), adO_ = smem_u32(sdO + i * TILE);
-        const uint32_t aK_ = smem_u32(sK + j * TILE), aV_ = smem_u32(sV + j * TILE);
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          umma_bf16(tmem_base + COL_S, umma_desc_sw128(aQ_ + kk * 32, 16, 1024), umma_desc_sw128(aK_ + kk * 32, 16, 1024),
-                    idesc_s, kk > 0 ? 1u : 0u);
+  for (int hr = 0; hr < 2; ++hr) {
+    const int kv = k0 + r0 + g + hr * 8;
+    if (kv >= p.Skv) continue;
+    bf16* dK = p.out0 + (static_cast<int64_t>(b) * p.Skv + kv) * p.ld0 + h * D;
+    bf16* dV = p.out1 + (static_cast<int64_t>(b) * p.Skv + kv) * p.ld1 + h * D;
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          umma_bf16(tmem_base + COL_DP, umma_desc_sw128(adO_ + kk * 32, 16, 1024), umma_desc_sw128(aV_ + kk * 32, 16, 1024),
-                    idesc_s, kk > 0 ? 1u : 0u);
-        umma_commit(s_ready);
-      };
-      int pair = 0;
-      issue_scores(0, 0);
-      for (int j = 0; j < nj; ++j) {
-        for (int i = 0; i < ni; ++i, ++pair) {
-          const uint32_t aQ = smem_u32(sQ + i * TILE), adO = smem_u32(sdO + i * TILE);
-          const uint32_t aK = smem_u32(sK + j * TILE);
-          mbar_wait(p_ready, pair & 1);            // S/dP of this pair have been read, P'/dS' are in shared memory
-          const int i2 = (i + 1 < ni) ? i + 1 : 0, j2 = (i + 1 < ni) ? j : j + 1;
-          if (j2 < nj) issue_scores(i2, j2);
-          // dK_j / dV_j of the previous key block must have been read out before the first pair of this block overwrites them
-          if (i == 0 && j > 0) mbar_wait(kv_read, (j - 1) & 1);
-          tc_fence_after();
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {   // K dimension = the 128 keys of block j
-            const uint32_t aoff = (kk >> 2) * TILE + (kk & 3) * 32;
-            umma_bf16(tmem_base + COL_DQ + i * D, umma_desc_sw128(smem_u32(sDS) + aoff, 16, 1024),
-                      umma_desc_sw128(aK + kk * 2048, TILE, 1024), idesc_q, (j > 0 || kk > 0) ? 1u : 0u);
-          }
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {   // K dimension = the 128 queries of block i; A = transposed views
-            umma_bf16(tmem_base + COL_DK, umma_desc_sw128(smem_u32(sDS) + kk * 2048, TILE, 1024),
-                      umma_desc_sw128(aQ + kk * 2048, TILE, 1024), idesc_t, (i > 0 || kk > 0) ? 1u : 0u);
-            umma_bf16(tmem_base + COL_DV, umma_desc_sw128(smem_u32(sP) + kk * 2048, TILE, 1024),
-                      umma_desc_sw128(adO + kk * 2048, TILE, 1024), idesc_t, (i > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(acc_done);
-        }
-      }
+    for (int i = 0; i < DT; ++i) {
+      *reinterpret_cast<uint32_t*>(dK + i * 8 + 2 * t4) = pack_bf16x2(dk[i][hr * 2] * p.scale, dk[i][hr * 2 + 1] * p.scale);
+      *reinterpret_cast<uint32_t*>(dV + i * 8 + 2 * t4) = pack_bf16x2(dv[i][hr * 2], dv[i][hr * 2 + 1]);
     }
-  } else {
-    const int quarter = warp & 3, c = warp >> 2;          // c: this thread's 32-column chunk of the key block
-    const int row = quarter * 32 + lane;
-    const uint32_t trow = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    int pair = 0;
-    for (int j = 0; j < nj; ++j) {
-      for (int i = 0; i < ni; ++i, ++pair) {
-        const int q = i * 128 + row;
-        const float l2 = sLse[q], dl = sDel[q];
-        uint32_t bits = 0xFFFFFFFFu;
-        if (DROP && q < p.Sq) {
-          const int w = j * 4 + c;
-          if (w < p.W) bits = __ldg(p.dmask + (bh * p.Sq + q) * p.W + w);
-        }
-        const float4* m4 = reinterpret_cast<const float4*>(sMsk + j * 128 + c * 32);
-        uint32_t wds[16], wp[16];                           // packed bf16 pairs of dS' and P' for this thread's 32 columns
-        mbar_wait(s_ready, pair & 1);
-        tc_fence_after();
-        const bool chunk_on = (my_act >> j) & 1u;
-        if (!chunk_on) {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) { wds[e] = 0u; wp[e] = 0u; }
-        }
-#pragma unroll
-        for (int hh = 0; hh < 2 && chunk_on; ++hh) {
-          uint32_t rs[16], rd[16];
-          tmem_ld16(trow + COL_S + c * 32 + hh * 16, rs);
-          tmem_ld16(trow + COL_DP + c * 32 + hh * 16, rd);
-          tmem_ld_wait();
-#if MMFB_F32X2
-          const uint64_t sc2 = pk2(p.scale2, p.scale2), nl2 = pk2(-l2, -l2), ndl2 = pk2(-dl, -dl);
-#endif
-#pragma unroll
-          for (int q4 = 0; q4 < 4; ++q4) {
-            const float4 m = m4[hh * 4 + q4];
-            const float mm[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-            for (int k = 0; k < 4; k += 2) {
-              const int jx = q4 * 4 + k;                    // column inside the 16-column half
-              const int bx = hh * 16 + jx;                  // bit index inside the 32-column chunk
-              float ds0, ds1, pv0, pv1;
-#if MMFB_F32X2
-              float a0, a1;
-              upk2(add2(fma2(pk2(__uint_as_float(rs[jx]), __uint_as_float(rs[jx + 1])), sc2, pk2(mm[k], mm[k + 1])), nl2), a0, a1);
-              const uint64_t pr = pk2(ex2_approx(a0), ex2_approx(a1));
-              const uint64_t dp = pk2(__uint_as_float(rd[jx]), __uint_as_float(rd[jx + 1]));
-              if (DROP) {
-                const uint64_t kf = pk2(((bits >> bx) & 1u) ? p.dscale : 0.0f, ((bits >> (bx + 1)) & 1u) ? p.dscale : 0.0f);
-                upk2(mul2(pr, fma2(dp, kf, ndl2)), ds0, ds1);
-                upk2(mul2(pr, kf), pv0, pv1);
-              } else {
-                upk2(mul2(pr, add2(dp, ndl2)), ds0, ds1);
-                upk2(pr, pv0, pv1);
-              }
-#else
-              const float pr0 = ex2_approx(fmaf(__uint_as_float(rs[jx]), p.scale2, mm[k]) - l2);
-              const float pr1 = ex2_approx(fmaf(__uint_as_float(rs[jx + 1]), p.scale2, mm[k + 1]) - l2);
-              float dp0 = __uint_as_float(rd[jx]), dp1 = __uint_as_float(rd[jx + 1]);
-              pv0 = pr0; pv1 = pr1;
-              if (DROP) {
-                const bool k0 = (bits >> bx) & 1u, k1 = (bits >> (bx + 1)) & 1u;
-                dp0 = k0 ? dp0 * p.dscale : 0.0f;  pv0 = k0 ? pr0 * p.dscale : 0.0f;
-                dp1 = k1 ? dp1 * p.dscale : 0.0f;  pv1 = k1 ? pr1 * p.dscale : 0.0f;
-              }
-              ds0 = pr0 * (dp0 - dl);
-              ds1 = pr1 * (dp1 - dl);
-#endif
-              wds[hh * 8 + (jx >> 1)] = pack_bf16x2(ds0, ds1);
-              wp[hh * 8 + (jx >> 1)] = pack_bf16x2(pv0, pv1);
-            }
-          }
-        }
-        // the accumulations of the previous pair still read P'/dS' while the arithmetic above ran
-        if (pair > 0) mbar_wait(acc_done, (pair - 1) & 1);
-        uint8_t* dsrow = sDS + (c >> 1) * TILE + row * 128;
-        uint8_t* prow = sP + (c >> 1) * TILE + row * 128;
-#pragma unroll
-        for (int qd = 0; qd < 4; ++qd) {
-          const int chunk = ((c & 1) * 4 + qd) ^ (row & 7);
-          *reinterpret_cast<uint4*>(dsrow + chunk * 16) = make_uint4(wds[qd * 4], wds[qd * 4 + 1], wds[qd * 4 + 2], wds[qd * 4 + 3]);
-          *reinterpret_cast<uint4*>(prow + chunk * 16) = make_uint4(wp[qd * 4], wp[qd * 4 + 1], wp[qd * 4 + 2], wp[qd * 4 + 3]);
-        }
-        fence_proxy_async();
-        tc_fence_before();
-        mbar_arrive(p_ready);
-      }
-      // ---- dK_j, dV_j are complete: rows = keys of block j; this thread stores 16 of the 64 columns of each ----
-      mbar_wait(acc_done, (pair - 1) & 1);
-      tc_fence_after();
-      {
-        const int kvr = j * 128 + row;
-        uint32_t rk[16], rv[16];
-        tmem_ld16(trow + COL_DK + c * 16, rk);
-        tmem_ld16(trow + COL_DV + c * 16, rv);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(kv_read);
-        if (kvr < p.Skv) {
-          uint4* dk4 = reinterpret_cast<uint4*>(p.dk + (static_cast<int64_t>(b) * p.Skv + kvr) * p.ld_dk + h * D + c * 16);
-          uint4* dv4 = reinterpret_cast<uint4*>(p.dv + (static_cast<int64_t>(b) * p.Skv + kvr) * p.ld_dv + h * D + c * 16);
-#pragma unroll
-          for (int qd = 0; qd < 2; ++qd) {
-            uint4 o;
-            o.x = pack_bf16x2(__uint_as_float(rk[qd * 8 + 0]) * p.scale, __uint_as_float(rk[qd * 8 + 1]) * p.scale);
-            o.y = pack_bf16x2(__uint_as_float(rk[qd * 8 + 2]) * p.scale, __uint_as_float(rk[qd * 8 + 3]) * p.scale);
-            o.z = pack_bf16x2(__uint_as_float(rk[qd * 8 + 4]) * p.scale, __uint_as_float(rk[qd * 8 + 5]) * p.scale);
-            o.w = pack_bf16x2(__uint_as_float(rk[qd * 8 + 6]) * p.scale, __uint_as_float(rk[qd * 8 + 7]) * p.scale);
-            dk4[qd] = o;
-            o.x = pack_bf16x2(__uint_as_float(rv[qd * 8 + 0]), __uint_as_float(rv[qd * 8 + 1]));
-            o.y = pack_bf16x2(__uint_as_float(rv[qd * 8 + 2]), __uint_as_float(rv[qd * 8 + 3]));
-            o.z = pack_bf16x2(__uint_as_float(rv[qd * 8 + 4]), __uint_as_float(rv[qd * 8 + 5]));
-            o.w = pack_bf16x2(__uint_as_float(rv[qd * 8 + 6]), __uint_as_float(rv[qd * 8 + 7]));
-            dv4[qd] = o;
-          }
-        }
-      }
-    }
-    // ---- dQ_i: rows = queries (all accumulations are complete: acc_done of the last pair was waited for above) ----
-    for (int i = 0; i < ni; ++i) {
-      const int q = i * 128 + row;
-      uint32_t rq[16];
-      tmem_ld16(trow + COL_DQ + i * D + c * 16, rq);
-      tmem_ld_wait();
-      if (q < p.Sq) {
-        uint4* dq4 = reinterpret_cast<uint4*>(p.dq + (static_cast<int64_t>(b) * p.Sq + q) * p.ld_dq + h * D + c * 16);
-#pragma unroll
-        for (int qd = 0; qd < 2; ++qd) {
-          uint4 o;
-          o.x = pack_bf16x2(__uint_as_float(rq[qd * 8 + 0]) * p.scale, __uint_as_float(rq[qd * 8 + 1]) * p.scale);
-          o.y = pack_bf16x2(__uint_as_float(rq[qd * 8 + 2]) * p.scale, __uint_as_float(rq[qd * 8 + 3]) * p.scale);
-          o.z = pack_bf16x2(__uint_as_float(rq[qd * 8 + 4]) * p.scale, __uint_as_float(rq[qd * 8 + 5]) * p.scale);
-          o.w = pack_bf16x2(__uint_as_float(rq[qd * 8 + 6]) * p.scale, __uint_as_float(rq[qd * 8 + 7]) * p.scale);
-          dq4[qd] = o;
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 16) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-// ----------------------------------------------------------------------------------------------
-// fused backward, persistent (d = 64, Sq, Skv <= 256) - the default
-//
-// attn_bwd_fused16_kernel is launched once per (batch, head): 13.5 waves of CTAs that each pay the tensor-memory
-// allocation, barrier set-up, the (exposed) loads of the row statistics, the first 64 KB of operand tiles and, at the end,
-// the drain of dK / dV / dQ - about a third of the ~18 us a CTA lives (ncu round 2: 50 % of the stall samples on loads and
-// barriers, tensor pipe 15 % active).  This kernel keeps ONE CTA per SM alive over its share of the (batch, head) items:
-//   * same arithmetic, tensor-memory map, MMAs and accumulation order as the 16-warp kernel (bit-identical results);
-//   * warp 17 is a loader: the four operand slot groups (K_0 V_0 | Q_0 dO_0 | Q_1 dO_1 | K_1 V_1) are refilled for the NEXT
-//     item as soon as the last accumulation that reads them has completed (tile_free barriers committed by the MMA
-//     thread), and the row statistics / mask row / active-chunk bits of the next item are staged in a second buffer;
-//   * the score MMAs of the next item's first block pair are issued right after the last pair's probabilities have been
-//     read, so the tensor core and the TMA engine work through the epilogue stores of the previous item.
-// 576 threads: warps 0..15 compute (thread = query row x 32-column chunk), warp 16 = MMA issue, warp 17 = loader.
-// ----------------------------------------------------------------------------------------------
-constexpr int BWD_PERS_THREADS = 608;       // 16 compute warps + MMA-issue warp + loader warp + store warp
-template <bool DROP>
-__global__ void __launch_bounds__(BWD_PERS_THREADS, 1)
-attn_bwd_pers_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
-                     const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                     const __grid_constant__ CUtensorMap tmdQ, const __grid_constant__ CUtensorMap tmdK,
-                     const __grid_constant__ CUtensorMap tmdV, AttnBwdFusedDev p, int n_items, int* sched) {
-  griddep_launch();
-  griddep_wait();
-  constexpr int D = 64;
-  constexpr int TILE = 16384;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_align1024(smem_raw);
-  uint8_t* sQ = smem;                 // [2][128 x 128B]
-  uint8_t* sdO = sQ + 2 * TILE;
-  uint8_t* sK = sdO + 2 * TILE;
-  uint8_t* sV = sK + 2 * TILE;
-  uint8_t* sP = sV + 2 * TILE;        // [128 q x 128 kv] bf16 = 2 chunks of [128 x 128B]
-  uint8_t* sDS = sP + 2 * TILE;
-  float* sStat = reinterpret_cast<float*>(sDS + 2 * TILE);   // [2 buffers][lse 256 | delta 256 | mask 256]
-  // keep-factor masks: entry b (8 keep-bits) -> eight words, all ones where the bit is set: kf = dscale & mask replaces a
-  // shift / test / select per element of the exp / dS arithmetic
-  uint32_t* sKf = reinterpret_cast<uint32_t*>(sStat + 2 * 768);         // [256][8]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sKf + 256 * 8);
-  uint64_t* q_full = bars;            // [2]  Q_i + dO_i          (phase = item parity)
-  uint64_t* kv_full = bars + 2;       // [2]  K_j + V_j           (phase = item parity)
-  uint64_t* tile_free = bars + 4;     // [4]  K0V0 | Q0dO0 | Q1dO1 | K1V1: last reader of this item has completed
-  uint64_t* stat_full = bars + 8;     // [2 buffers] 32 arrivals
-  uint64_t* s_ready = bars + 10;      // phase = pair counter parity
-  uint64_t* p_ready = bars + 11;      // 512 arrivals
-  uint64_t* acc_done = bars + 12;
-  uint64_t* kv_read = bars + 13;      // 512 arrivals, phase = key-block counter parity
-  uint64_t* dq_read = bars + 14;      // 512 arrivals, phase = item parity
-  uint64_t* sdp_read = bars + 15;     // 512 arrivals: S / dP of the pair are in registers, the score columns are free
-  uint64_t* kv_staged = bars + 16;    // [2] 512 arrivals: dK_j / dV_j are in the K_j / V_j slots; alternating by key-block counter so
-                                      // that two read-outs may be outstanding before the store warp has looked at the first
-  uint64_t* dq_staged = bars + 18;    // 512 arrivals: dQ_i are in the P' buffer (phase = item parity)
-  uint64_t* stg_free = bars + 19;     // the dQ store has finished reading the P' buffer (phase = item parity)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 20);
-  uint32_t* sAct = tmem_slot + 1;     // [2 buffers] bit c: 32-key chunk c has an attendable key
-  int* sItem = reinterpret_cast<int*>(sAct + 2);    // [2 buffers] (batch, head) item, -1 = no more work; published by stat_full
-  constexpr uint32_t COL_S = 0, COL_DP = 128, COL_DQ = 256, COL_DK = 384, COL_DV = 448;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ni = (p.Sq + 127) / 128, nj = (p.Skv + 127) / 128;
-  const int np = ni * nj;
-
-  if (DROP)
-    for (int e = threadIdx.x; e < 256 * 8; e += BWD_PERS_THREADS) sKf[e] = (((e >> 3) >> (e & 7)) & 1) ? 0xFFFFFFFFu : 0u;
-  if (warp == 17) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmdO); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-      for (int x = 0; x < 2; ++x) { mbar_init(&q_full[x], 1); mbar_init(&kv_full[x], 1); mbar_init(&stat_full[x], 32); }
-      // K_j / V_j slots double as staging for dK_j / dV_j: released by the MMA thread's commit AND the store warp
-      mbar_init(&tile_free[0], 2); mbar_init(&tile_free[1], 1); mbar_init(&tile_free[2], 1); mbar_init(&tile_free[3], 2);
-      mbar_init(sdp_read, 512); mbar_init(&kv_staged[0], 512); mbar_init(&kv_staged[1], 512); mbar_init(dq_staged, 512); mbar_init(stg_free, 1);
-      mbar_init(s_ready, 1);
-      mbar_init(p_ready, 512);
-      mbar_init(acc_done, 1);
-      mbar_init(kv_read, 512);
-      mbar_init(dq_read, 512);
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 17) {
-    // ------------------------------------ loader ------------------------------------
-    // Items come from an atomic counter (sched[0]), not a fixed stride: their cost varies with the padding of the sample
-    // (masked chunks are skipped) and a static split leaves the slowest of 148 CTAs ~10 % behind the mean.
-    auto fetch = [&]() -> int {
-      int it = 0;
-      if (lane == 0) it = atomicAdd(sched, 1);
-      it = __shfl_sync(0xffffffffu, it, 0);
-      return it < n_items ? it : -1;
-    };
-    auto load_kv = [&](int it, int j) {    // lane 0
-      const int h = it % p.H, b = it / p.H;
-      mbar_expect_tx(&kv_full[j], 2 * TILE);
-      tma_load_3d(sK + j * TILE, &tmK, &kv_full[j], h * D, j * 128, b);
-      tma_load_3d(sV + j * TILE, &tmV, &kv_full[j], h * D, j * 128, b);
-    };
-    auto load_q = [&](int it, int i) {     // lane 0
-      const int h = it % p.H, b = it / p.H;
-      mbar_expect_tx(&q_full[i], 2 * TILE);
-      tma_load_3d(sQ + i * TILE, &tmQ, &q_full[i], h * D, i * 128, b);
-      tma_load_3d(sdO + i * TILE, &tmdO, &q_full[i], h * D, i * 128, b);
-    };
-    auto load_stats = [&](int n, int it) { // whole warp: lse2, delta, log2-domain mask row, active-chunk bits, the item itself
-      float* st = sStat + (n & 1) * 768;
-      uint32_t act = 0;
-      if (it >= 0) {
-        const int h = it % p.H, b = it / p.H;
-        const int64_t bh = static_cast<int64_t>(b) * p.H + h;
-        float lv[8], dv[8], mv[8];
-#pragma unroll
-        for (int x = 0; x < 8; ++x) {
-          const int i = lane + 32 * x;
-          const bool qv = i < p.Sq, kv = i < p.Skv;
-          lv[x] = qv ? p.lse2[bh * p.Sq + i] : INFINITY;
-          dv[x] = qv ? p.delta[bh * p.Sq + i] : 0.0f;
-          mv[x] = kv ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + i] * LOG2E : 0.0f) : -INFINITY;
-        }
-        // 32-key chunks whose keys are ALL masked out (additive -10000 or beyond Skv) have P = 0 and dS = 0 exactly: their
-        // arithmetic is skipped (zeros are stored).  A sample without any attendable key keeps every chunk.
-#pragma unroll
-        for (int x = 0; x < 8; ++x) {
-          const int i = lane + 32 * x;
-          st[i] = lv[x];
-          st[256 + i] = dv[x];
-          st[512 + i] = mv[x];
-          if (__any_sync(0xffffffffu, mv[x] > -5000.0f)) act |= 1u << x;
-        }
-        if (act == 0) act = 0xFFu;
-      }
-      if (lane == 0) { sAct[n & 1] = act; sItem[n & 1] = it; }
-      __syncwarp();
-      mbar_arrive(&stat_full[n & 1]);
-    };
-    int it_cur = fetch();
-    if (lane == 0 && it_cur >= 0) {
-      load_kv(it_cur, 0);
-      for (int i = 0; i < ni; ++i) load_q(it_cur, i);
-      for (int j = 1; j < nj; ++j) load_kv(it_cur, j);
-    }
-    load_stats(0, it_cur);
-    for (int n = 0; it_cur >= 0; ++n) {
-      // statistics of item n+1 go to the buffer item n-1 used: every compute thread has left item n-1 (dq_read)
-      if (n >= 1) mbar_wait(dq_read, (n - 1) & 1);
-      const int it_next = fetch();
-      load_stats(n + 1, it_next);
-      if (it_next >= 0) {
-        // operand slots in the order in which item n releases them (pair index of the last reader, j outer / i inner)
-        for (int pidx = 0; pidx < np; ++pidx) {
-          for (int j = 0; j < nj; ++j)
-            if (pidx == j * ni + ni - 1) {
-              mbar_wait(&tile_free[j == 0 ? 0 : 3], n & 1);
-              if (lane == 0) load_kv(it_next, j);
-            }
-          for (int i = 0; i < ni; ++i)
-            if (pidx == (nj - 1) * ni + i) {
-              mbar_wait(&tile_free[1 + i], n & 1);
-              if (lane == 0) load_q(it_next, i);
-            }
-        }
-      }
-      it_cur = it_next;
-    }
-  } else if (warp == 16) {
-    // ------------------------------------ MMA issue ------------------------------------
-    if (lane == 0) {
-      const uint32_t idesc_s = umma_idesc_bf16(128, 128, false, false);
-      const uint32_t idesc_q = umma_idesc_bf16(128, D, false, true);   // A K-major,  B MN-major
-      const uint32_t idesc_t = umma_idesc_bf16(128, D, true, true);    // A MN-major, B MN-major
-      auto issue_scores = [&](int n, int i, int j) {      // S = Q_i K_j^T, dP = dO_i V_j^T of item n
-        mbar_wait(&q_full[i], n & 1);
-        mbar_wait(&kv_full[j], n & 1);
-        tc_fence_after();
-        const uint32_t aQ_ = smem_u32(sQ + i * TILE), adO_ = smem_u32(sdO + i * TILE);
-        const uint32_t aK_ = smem_u32(sK + j * TILE), aV_ = smem_u32(sV + j * TILE);
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          umma_bf16(tmem_base + COL_S, umma_desc_sw128(aQ_ + kk * 32, 16, 1024), umma_desc_sw128(aK_ + kk * 32, 16, 1024),
-                    idesc_s, kk > 0 ? 1u : 0u);
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          umma_bf16(tmem_base + COL_DP, umma_desc_sw128(adO_ + kk * 32, 16, 1024), umma_desc_sw128(aV_ + kk * 32, 16, 1024),
-                    idesc_s, kk > 0 ? 1u : 0u);
-        umma_commit(s_ready);
-      };
-      uint32_t g = 0;                    // pair counter over all items
-      uint32_t kb = 0;                   // key-block counter over all items
-      mbar_wait(&stat_full[0], 0);
-      bool more = sItem[0] >= 0;
-      if (more) issue_scores(0, 0, 0);
-      for (int n = 0; more; ++n) {
-        for (int j = 0; j < nj; ++j, ++kb) {
-          for (int i = 0; i < ni; ++i, ++g) {
-            const int pidx = j * ni + i;
-            const uint32_t aQ = smem_u32(sQ + i * TILE), adO = smem_u32(sdO + i * TILE);
-            const uint32_t aK = smem_u32(sK + j * TILE);
-            const bool last_pair = pidx == np - 1;
-            // the next pair's scores go out as soon as every thread holds S / dP of this one in registers: the tensor core
-            // computes them while the threads are still in the exp / dS arithmetic (the round-2 trace showed ~1000 idle
-            // cycles per pair between "P'/dS' stored" and "next scores ready")
-            mbar_wait(sdp_read, g & 1);
-            if (!last_pair) {
-              const int i2 = (i + 1 < ni) ? i + 1 : 0, j2 = (i + 1 < ni) ? j : j + 1;
-              tc_fence_after();
-              issue_scores(n, i2, j2);               // next pair of this item: its tiles are resident
-            }
-            mbar_wait(p_ready, g & 1);               // P'/dS' of this pair are in shared memory
-            MMFB_TR(1, n, 2 * pidx);
-            // accumulators that are overwritten (not accumulated) must have been read out by the compute threads
-            if (i == 0 && kb > 0) mbar_wait(kv_read, (kb - 1) & 1);
-            if (pidx == 0 && n > 0) mbar_wait(dq_read, (n - 1) & 1);
-            tc_fence_after();
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk) {   // K dimension = the 128 keys of block j
-              const uint32_t aoff = (kk >> 2) * TILE + (kk & 3) * 32;
-              umma_bf16(tmem_base + COL_DQ + i * D, umma_desc_sw128(smem_u32(sDS) + aoff, 16, 1024),
-                        umma_desc_sw128(aK + kk * 2048, TILE, 1024), idesc_q, (j > 0 || kk > 0) ? 1u : 0u);
-            }
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk) {   // K dimension = the 128 queries of block i; A = transposed views
-              umma_bf16(tmem_base + COL_DK, umma_desc_sw128(smem_u32(sDS) + kk * 2048, TILE, 1024),
-                        umma_desc_sw128(aQ + kk * 2048, TILE, 1024), idesc_t, (i > 0 || kk > 0) ? 1u : 0u);
-              umma_bf16(tmem_base + COL_DV, umma_desc_sw128(smem_u32(sP) + kk * 2048, TILE, 1024),
-                        umma_desc_sw128(adO + kk * 2048, TILE, 1024), idesc_t, (i > 0 || kk > 0) ? 1u : 0u);
-            }
-            umma_commit(acc_done);
-            MMFB_TR(1, n, 2 * pidx + 1);
-            // operand slots whose last reader this pair was
-            if (i == ni - 1) umma_commit(&tile_free[j == 0 ? 0 : 3]);
-            if (j == nj - 1) umma_commit(&tile_free[1 + i]);
-            // first pair of the next item AFTER the accumulations: its tiles may still be in flight
-            if (last_pair) {
-              mbar_wait(&stat_full[(n + 1) & 1], ((n + 1) >> 1) & 1);      // published while item n was running
-              more = sItem[(n + 1) & 1] >= 0;
-              if (more) issue_scores(n + 1, 0, 0);
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 18) {
-    // ------------------------------------ store warp: bulk tensor stores of dK_j, dV_j, dQ_i ------------------------------------
-    // (16-byte register stores of a warp to 32 different rows cost 32 LSU passes each; rows beyond Sq / Skv are clipped by
-    // the tensor maps)
-    uint32_t kbs = 0;
-    for (int n = 0;; ++n) {
-      mbar_wait(&stat_full[n & 1], (n >> 1) & 1);
-      const int it = sItem[n & 1];
-      if (it < 0) break;
-      const int h = it % p.H, b = it / p.H;
-      for (int j = 0; j < nj; ++j, ++kbs) {
-        mbar_wait(&kv_staged[kbs & 1], (kbs >> 1) & 1);
-        if (lane == 0) {
-          tma_store_3d(&tmdK, sK + j * TILE, h * D, j * 128, b);
-          tma_store_3d(&tmdV, sV + j * TILE, h * D, j * 128, b);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-          mbar_arrive(&tile_free[j == 0 ? 0 : 3]);
-        }
-        __syncwarp();
-      }
-      mbar_wait(dq_staged, n & 1);
-      if (lane == 0) {
-        for (int i = 0; i < ni; ++i) tma_store_3d(&tmdQ, sP + i * TILE, h * D, i * 128, b);
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        mbar_arrive(stg_free);
-      }
-      __syncwarp();
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // writes complete before the CTA exits
-  } else {
-    // ------------------------------------ compute ------------------------------------
-    const int quarter = warp & 3, c = warp >> 2;          // c: this thread's 32-column chunk of the key block
-    const int row = quarter * 32 + lane;
-    const uint32_t trow = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    uint32_t g = 0, kb = 0, ro = 0;       // pair, key-block and read-out counters over all items
-    int h = 0, b = 0;
-    // dK_j, dV_j (rows = keys of block j, 16 of the 64 columns of each per thread) -> K_j / V_j slots (their last readers, the
-    // accumulations of the block's last pair, have completed) -> one bulk tensor store per tile by the store warp
-    auto readout_kv = [&](int jb) {
-      uint32_t rk[16], rv[16];
-      tc_fence_after();
-      tmem_ld16(trow + COL_DK + c * 16, rk);
-      tmem_ld16(trow + COL_DV + c * 16, rv);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(kv_read);
-      uint8_t* krow = sK + jb * TILE + row * 128;
-      uint8_t* vrow = sV + jb * TILE + row * 128;
-#pragma unroll
-      for (int qd = 0; qd < 2; ++qd) {
-        uint4 o;
-        o.x = pack_bf16x2(__uint_as_float(rk[qd * 8 + 0]) * p.scale, __uint_as_float(rk[qd * 8 + 1]) * p.scale);
-        o.y = pack_bf16x2(__uint_as_float(rk[qd * 8 + 2]) * p.scale, __uint_as_float(rk[qd * 8 + 3]) * p.scale);
-        o.z = pack_bf16x2(__uint_as_float(rk[qd * 8 + 4]) * p.scale, __uint_as_float(rk[qd * 8 + 5]) * p.scale);
-        o.w = pack_bf16x2(__uint_as_float(rk[qd * 8 + 6]) * p.scale, __uint_as_float(rk[qd * 8 + 7]) * p.scale);
-        const int chunk = ((c * 2 + qd) ^ (row & 7)) * 16;
-        *reinterpret_cast<uint4*>(krow + chunk) = o;
-        o.x = pack_bf16x2(__uint_as_float(rv[qd * 8 + 0]), __uint_as_float(rv[qd * 8 + 1]));
-        o.y = pack_bf16x2(__uint_as_float(rv[qd * 8 + 2]), __uint_as_float(rv[qd * 8 + 3]));
-        o.z = pack_bf16x2(__uint_as_float(rv[qd * 8 + 4]), __uint_as_float(rv[qd * 8 + 5]));
-        o.w = pack_bf16x2(__uint_as_float(rv[qd * 8 + 6]), __uint_as_float(rv[qd * 8 + 7]));
-        *reinterpret_cast<uint4*>(vrow + chunk) = o;
-      }
-      fence_proxy_async();
-      mbar_arrive(&kv_staged[ro & 1]);
-      ++ro;
-    };
-    for (int n = 0;; ++n) {
-      mbar_wait(&stat_full[n & 1], (n >> 1) & 1);
-      const int it = sItem[n & 1];
-      if (it < 0) break;
-      h = it % p.H;
-      b = it / p.H;
-      const int64_t bh = static_cast<int64_t>(b) * p.H + h;
-      const float* sLse = sStat + (n & 1) * 768;
-      const float* sDel = sLse + 256;
-      const float* sMsk = sLse + 512;
-      const bool tr = threadIdx.x == 0;
-      if (tr) MMFB_TR(0, n, 14);
-      const uint32_t act = sAct[n & 1];
-      for (int j = 0; j < nj; ++j, ++kb) {
-        for (int i = 0; i < ni; ++i, ++g) {
-          const int q = i * 128 + row;
-          const float l2 = sLse[q], dl = sDel[q];
-          uint32_t bits = 0xFFFFFFFFu;
-          if (DROP && q < p.Sq) {
-            const int w = j * 4 + c;
-            if (w < p.W) bits = __ldg(p.dmask + (bh * p.Sq + q) * p.W + w);
-          }
-          const float4* m4 = reinterpret_cast<const float4*>(sMsk + j * 128 + c * 32);
-          uint32_t wds[16], wp[16];                           // packed bf16 pairs of dS' and P' for this thread's 32 columns
-          mbar_wait(s_ready, g & 1);
-          tc_fence_after();
-          if (tr) MMFB_TR(0, n, 3 * (j * ni + i));
-          const bool chunk_on = (act >> (j * 4 + c)) & 1u;
-          if (!chunk_on) {
-#pragma unroll
-            for (int e = 0; e < 16; ++e) { wds[e] = 0u; wp[e] = 0u; }
-            tc_fence_before();
-            mbar_arrive(sdp_read);
-          }
-#pragma unroll
-          for (int hh = 0; hh < 2 && chunk_on; ++hh) {
-            uint32_t rs[16], rd[16];
-            tmem_ld16(trow + COL_S + c * 32 + hh * 16, rs);
-            tmem_ld16(trow + COL_DP + c * 32 + hh * 16, rd);
-            tmem_ld_wait();
-            if (hh == 1) {                                    // both halves are in registers: the score columns are free
-              tc_fence_before();
-              mbar_arrive(sdp_read);
-            }
-            const uint64_t sc2 = pk2(p.scale2, p.scale2), nl2 = pk2(-l2, -l2), ndl2 = pk2(-dl, -dl);
-            uint32_t km[16];
-            if (DROP) {
-              const uint32_t dsb = __float_as_uint(p.dscale);
-              const uint4* L0 = reinterpret_cast<const uint4*>(sKf + ((bits >> (16 * hh)) & 0xFFu) * 8);
-              const uint4* L1 = reinterpret_cast<const uint4*>(sKf + ((bits >> (16 * hh + 8)) & 0xFFu) * 8);
-              const uint4 k0 = L0[0], k1 = L0[1], k2 = L1[0], k3 = L1[1];
-              km[0] = k0.x & dsb; km[1] = k0.y & dsb; km[2] = k0.z & dsb; km[3] = k0.w & dsb;
-              km[4] = k1.x & dsb; km[5] = k1.y & dsb; km[6] = k1.z & dsb; km[7] = k1.w & dsb;
-              km[8] = k2.x & dsb; km[9] = k2.y & dsb; km[10] = k2.z & dsb; km[11] = k2.w & dsb;
-              km[12] = k3.x & dsb; km[13] = k3.y & dsb; km[14] = k3.z & dsb; km[15] = k3.w & dsb;
-            }
-#pragma unroll
-            for (int q4 = 0; q4 < 4; ++q4) {
-              const float4 m = m4[hh * 4 + q4];
-              const float mm[4] = {m.x, m.y, m.z, m.w};
-#pragma unroll
-              for (int k = 0; k < 4; k += 2) {
-                const int jx = q4 * 4 + k;                    // column inside the 16-column half
-                float ds0, ds1, pv0, pv1, a0, a1;
-                upk2(add2(fma2(pk2(__uint_as_float(rs[jx]), __uint_as_float(rs[jx + 1])), sc2, pk2(mm[k], mm[k + 1])), nl2), a0, a1);
-                const uint64_t pr = pk2(ex2_approx(a0), ex2_approx(a1));
-                const uint64_t dp = pk2(__uint_as_float(rd[jx]), __uint_as_float(rd[jx + 1]));
-                if (DROP) {
-                  const uint64_t kf = pk2(__uint_as_float(km[jx]), __uint_as_float(km[jx + 1]));
-                  upk2(mul2(pr, fma2(dp, kf, ndl2)), ds0, ds1);
-                  upk2(mul2(pr, kf), pv0, pv1);
-                } else {
-                  upk2(mul2(pr, add2(dp, ndl2)), ds0, ds1);
-                  upk2(pr, pv0, pv1);
-                }
-                wds[hh * 8 + (jx >> 1)] = pack_bf16x2(ds0, ds1);
-                wp[hh * 8 + (jx >> 1)] = pack_bf16x2(pv0, pv1);
-              }
-            }
-          }
-          // the accumulations of the previous pair still read P'/dS' while the arithmetic above ran
-          if (tr) MMFB_TR(0, n, 3 * (j * ni + i) + 1);
-          if (g > 0) mbar_wait(acc_done, (g - 1) & 1);
-          if (j == 0 && i == 0 && n > 0) mbar_wait(stg_free, (n - 1) & 1);   // the previous item's dQ store has read the P' buffer
-          uint8_t* dsrow = sDS + (c >> 1) * TILE + row * 128;
-          uint8_t* prow = sP + (c >> 1) * TILE + row * 128;
-#pragma unroll
-          for (int qd = 0; qd < 4; ++qd) {
-            const int chunk = ((c & 1) * 4 + qd) ^ (row & 7);
-            *reinterpret_cast<uint4*>(dsrow + chunk * 16) = make_uint4(wds[qd * 4], wds[qd * 4 + 1], wds[qd * 4 + 2], wds[qd * 4 + 3]);
-            *reinterpret_cast<uint4*>(prow + chunk * 16) = make_uint4(wp[qd * 4], wp[qd * 4 + 1], wp[qd * 4 + 2], wp[qd * 4 + 3]);
-          }
-          fence_proxy_async();
-          tc_fence_before();
-          mbar_arrive(p_ready);
-          if (tr) MMFB_TR(0, n, 3 * (j * ni + i) + 2);
-          // the previous key block's dK / dV leave AFTER this pair's arithmetic: their accumulations (waited for above)
-          // completed while it ran, instead of 512 threads idling through them at the block boundary
-          if (i == 0 && j > 0) readout_kv(j - 1);
-        }
-      }
-      // ---- item end: the last key block's dK / dV, then dQ (every accumulation of the item is complete) ----
-      mbar_wait(acc_done, (g - 1) & 1);
-      readout_kv(nj - 1);
-      {
-        uint32_t rq[2][16];
-        tc_fence_after();
-#pragma unroll
-        for (int i = 0; i < 2; ++i)
-          if (i < ni) tmem_ld16(trow + COL_DQ + i * D + c * 16, rq[i]);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(dq_read);
-        if (tr) MMFB_TR(0, n, 12);
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          if (i < ni) {
-            uint8_t* qrow = sP + i * TILE + row * 128;           // P' buffer: free since the last accumulation completed
-#pragma unroll
-            for (int qd = 0; qd < 2; ++qd) {
-              uint4 o;
-              o.x = pack_bf16x2(__uint_as_float(rq[i][qd * 8 + 0]) * p.scale, __uint_as_float(rq[i][qd * 8 + 1]) * p.scale);
-              o.y = pack_bf16x2(__uint_as_float(rq[i][qd * 8 + 2]) * p.scale, __uint_as_float(rq[i][qd * 8 + 3]) * p.scale);
-              o.z = pack_bf16x2(__uint_as_float(rq[i][qd * 8 + 4]) * p.scale, __uint_as_float(rq[i][qd * 8 + 5]) * p.scale);
-              o.w = pack_bf16x2(__uint_as_float(rq[i][qd * 8 + 6]) * p.scale, __uint_as_float(rq[i][qd * 8 + 7]) * p.scale);
-              *reinterpret_cast<uint4*>(qrow + (((c * 2 + qd) ^ (row & 7)) * 16)) = o;
-            }
-          }
-        }
-        fence_proxy_async();
-        mbar_arrive(dq_staged);
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 17) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-  // the last CTA to finish re-arms the item counter for the next launch
-  if (threadIdx.x == 0 && atomicAdd(sched + 1, 1) == static_cast<int>(gridDim.x) - 1) {
-    atomicExch(sched, 0);
-    atomicExch(sched + 1, 0);
   }
 }
 
@@ -2257,20 +583,10 @@ static int check_attn_common(const mmfb_attn_args& a, const char* who) {
   return MMFB_OK;
 }
 
-// Work counters of the persistent attention kernels ([0..1] forward: next item / finished CTAs, [4..5] backward): device
-// memory owned by the library, zero between launches (the last CTA of a launch re-arms them).  One set per device: the
-// kernels of ONE stream are serialised; concurrent attention launches on different streams of a device are not supported.
-static int* sched_counters() {
-  static int* buf[64] = {nullptr};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-  if (buf[dev] == nullptr) {
-    int* b = nullptr;
-    if (cudaMalloc(&b, 8 * sizeof(int)) != cudaSuccess) return nullptr;
-    if (cudaMemset(b, 0, 8 * sizeof(int)) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) return nullptr;
-    buf[dev] = b;
-  }
-  return buf[dev];
+static int set_smem(const void* kern, int bytes, const char* who) {
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "%s smem attr (%d B): %s", who, bytes, cudaGetErrorString(e));
+  return MMFB_OK;
 }
 
 template <int D>
@@ -2278,18 +594,11 @@ static int attn_fwd_launch(const mmfb_attn_args& a, cudaStream_t stream) {
   const int W = a.heads * D;
   CUtensorMap tmQ, tmK, tmV;
   int rc;
-  if ((rc = make_tmap_3d(&tmQ, a.q, W, a.Sq, a.B, a.ldq, a.ldq * a.Sq, 64, 128))) return rc;
-  if ((rc = make_tmap_3d(&tmK, a.k, W, a.Skv, a.B, a.ldk, a.ldk * a.Skv, 64, 64))) return rc;
-  if ((rc = make_tmap_3d(&tmV, a.v, W, a.Skv, a.B, a.ldv, a.ldv * a.Skv, 64, 64))) return rc;
-  CUtensorMap tmK128 = tmK, tmV128 = tmV;      // 128-key boxes for the paired-tile kernel
-  if (D == 64 && a.Sq <= 256 && a.Skv <= 256) {
-    if ((rc = make_tmap_3d(&tmK128, a.k, W, a.Skv, a.B, a.ldk, a.ldk * a.Skv, 64, 128))) return rc;
-    if ((rc = make_tmap_3d(&tmV128, a.v, W, a.Skv, a.B, a.ldv, a.ldv * a.Skv, 64, 128))) return rc;
-  }
-  constexpr int DC = D / 64;
-  const int SK = (a.Skv + 63) & ~63, NB = SK / 64;
-  const int r0 = NB * 16384 > DC * 16384 + DC * SK * 128 ? NB * 16384 : DC * 16384 + DC * SK * 128;
-  const int smem = r0 + DC * SK * 128 + SK * 4 + 2048 + 128 + 1024;
+  if ((rc = make_tmap_3d(&tmQ, a.q, W, a.Sq, a.B, a.ldq, a.ldq * a.Sq, 64, AT_ROWS))) return rc;
+  if ((rc = make_tmap_3d(&tmK, a.k, W, a.Skv, a.B, a.ldk, a.ldk * a.Skv, 64, AT_ROWS))) return rc;
+  if ((rc = make_tmap_3d(&tmV, a.v, W, a.Skv, a.B, a.ldv, a.ldv * a.Skv, 64, AT_ROWS))) return rc;
+  const int NKB = (a.Skv + AT_ROWS - 1) / AT_ROWS;
+  const int smem = 5 * (D / 64) * AT_ROWS * 128 + NKB * AT_ROWS * 4 + 64 + 1024;
   AttnFwdDev p;
   p.B = a.B; p.H = a.heads; p.Sq = a.Sq; p.Skv = a.Skv;
   p.mask = a.mask;
@@ -2298,40 +607,14 @@ static int attn_fwd_launch(const mmfb_attn_args& a, cudaStream_t stream) {
   p.ctx_lo = reinterpret_cast<bf16*>(a.ctx_lo);
   p.dmask = a.drop_mask; p.W = (a.Skv + 31) / 32; p.dscale = a.drop_mask ? a.drop_scale : 1.0f;
   p.scale2 = LOG2E / sqrtf(static_cast<float>(D));
-  if (D == 64 && a.Sq <= 256 && a.Skv <= 256) {
-    // default for head size 64 and sequences within two 128-row tiles; MMFB_ATTN_FWD=1 (read per call) selects the
-    // one-CTA-per-tile kernel below for A/B runs
-    const char* f_env = getenv("MMFB_ATTN_FWD");
-    if (f_env == nullptr || f_env[0] != '1') {
-      const int smem_p = 2 * 6 * 16384 + (512 + 512 + 512) * 4 + 256 + 1024;
-      static bool attr_p = false;
-      if (!attr_p) {
-        cudaError_t e2 = cudaFuncSetAttribute(attn_fwd_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_p);
-        if (e2 != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_fwd_pair smem attr (%d B): %s", smem_p, cudaGetErrorString(e2));
-        attr_p = true;
-      }
-      const int n_pairs = a.heads * a.B;
-      const int grid_p = n_pairs < num_sms() ? n_pairs : num_sms();
-      int* sched = sched_counters();
-      if (sched == nullptr) return set_error(MMFB_ERR_CUDA, "attn_fwd: scheduler counters");
-      CUtensorMap tmO, tmOlo;
-      if ((rc = make_tmap_3d(&tmO, a.ctx, W, a.Sq, a.B, a.ldo, a.ldo * a.Sq, 64, 128))) return rc;
-      tmOlo = tmO;
-      if (a.ctx_lo != nullptr && (rc = make_tmap_3d(&tmOlo, a.ctx_lo, W, a.Sq, a.B, W, static_cast<int64_t>(W) * a.Sq, 64, 128))) return rc;
-      MMFB_LAUNCH(attn_fwd_pair_kernel, grid_p, FWD_PAIR_THREADS, smem_p, stream, tmQ, tmK128, tmV128, tmO, tmOlo, p, n_pairs, sched);
-      count_launch();
-      return MMFB_OK;
-    }
-  }
   auto kern = attn_fwd_kernel<D>;
   static int smem_set = 0;
   if (smem > smem_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_fwd smem attr (%d B): %s", smem, cudaGetErrorString(e));
+    if ((rc = set_smem(reinterpret_cast<const void*>(kern), smem, "attn_fwd"))) return rc;
     smem_set = smem;
   }
-  dim3 grid((a.Sq + 127) / 128, a.heads, a.B);
-  MMFB_LAUNCH(kern, grid, 288, smem, stream, tmQ, tmK, tmV, p);
+  dim3 grid((a.Sq + AT_ROWS - 1) / AT_ROWS, a.heads, a.B);
+  MMFB_LAUNCH(kern, grid, AT_THREADS, smem, stream, tmQ, tmK, tmV, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_fwd launch: %s", cudaGetErrorString(e));
   count_launch();
@@ -2345,136 +628,70 @@ int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream) {
   return a.head_dim == 64 ? attn_fwd_launch<64>(a, stream) : attn_fwd_launch<128>(a, stream);
 }
 
+template <int D, bool DROP>
+static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, cudaStream_t stream) {
+  constexpr int QB = (D == 64) ? 64 : 32;   // query block of the dK/dV kernel: d = 128 keeps its tiles in registers
+  const int W = a.heads * D;
+  CUtensorMap tmQ, tmK, tmV, tmdO, tmQc, tmdOc;
+  int rc;
+  if ((rc = make_tmap_3d(&tmQ, a.q, W, a.Sq, a.B, a.ldq, a.ldq * a.Sq, 64, AT_ROWS))) return rc;
+  if ((rc = make_tmap_3d(&tmdO, a.dctx, W, a.Sq, a.B, a.ld_dctx, a.ld_dctx * a.Sq, 64, AT_ROWS))) return rc;
+  if ((rc = make_tmap_3d(&tmK, a.k, W, a.Skv, a.B, a.ldk, a.ldk * a.Skv, 64, AT_ROWS))) return rc;
+  if ((rc = make_tmap_3d(&tmV, a.v, W, a.Skv, a.B, a.ldv, a.ldv * a.Skv, 64, AT_ROWS))) return rc;
+  tmQc = tmQ;
+  tmdOc = tmdO;
+  if (QB != AT_ROWS) {
+    if ((rc = make_tmap_3d(&tmQc, a.q, W, a.Sq, a.B, a.ldq, a.ldq * a.Sq, 64, QB))) return rc;
+    if ((rc = make_tmap_3d(&tmdOc, a.dctx, W, a.Sq, a.B, a.ld_dctx, a.ld_dctx * a.Sq, 64, QB))) return rc;
+  }
+  const int TB = (D / 64) * AT_ROWS * 128;
+  const int NKB = (a.Skv + AT_ROWS - 1) / AT_ROWS;
+  const int smem_q = 6 * TB + NKB * AT_ROWS * 4 + 64 + 1024;
+  const int smem_kv = 2 * TB + 4 * (D / 64) * QB * 128 + AT_ROWS * 4 + 64 + 1024;
+  static int set_q = 0;
+  static bool set_kv = false;
+  if (smem_q > set_q) {
+    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel<D, DROP>), smem_q, "attn_bwd_dq"))) return rc;
+    set_q = smem_q;
+  }
+  if (!set_kv) {
+    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dkv_kernel<D, DROP, QB>), smem_kv, "attn_bwd_dkv"))) return rc;
+    set_kv = true;
+  }
+  AttnBwdDev p = base;
+  p.out0 = reinterpret_cast<bf16*>(a.dq); p.ld0 = a.ld_dq; p.out1 = nullptr; p.ld1 = 0;
+  MMFB_LAUNCH((attn_bwd_dq_kernel<D, DROP>), dim3((a.Sq + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS, smem_q, stream,
+              tmQ, tmdO, tmK, tmV, p);
+  count_launch();
+  p.out0 = reinterpret_cast<bf16*>(a.dk); p.ld0 = a.ld_dk;
+  p.out1 = reinterpret_cast<bf16*>(a.dv); p.ld1 = a.ld_dv;
+  MMFB_LAUNCH((attn_bwd_dkv_kernel<D, DROP, QB>), dim3((a.Skv + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS, smem_kv,
+              stream, tmK, tmV, tmQc, tmdOc, p);
+  count_launch();
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_bwd launch: %s", cudaGetErrorString(e));
+  return MMFB_OK;
+}
+
 template <int D>
 static int attn_bwd_launch(const mmfb_attn_args& a, cudaStream_t stream) {
-  const int W = a.heads * D;
-  CUtensorMap tmQ, tmK, tmV, tmdO;
-  int rc;
-  if ((rc = make_tmap_3d(&tmQ, a.q, W, a.Sq, a.B, a.ldq, a.ldq * a.Sq, 64, 128))) return rc;
-  if ((rc = make_tmap_3d(&tmdO, a.dctx, W, a.Sq, a.B, a.ld_dctx, a.ld_dctx * a.Sq, 64, 128))) return rc;
-  if ((rc = make_tmap_3d(&tmK, a.k, W, a.Skv, a.B, a.ldk, a.ldk * a.Skv, 64, 128))) return rc;
-  if ((rc = make_tmap_3d(&tmV, a.v, W, a.Skv, a.B, a.ldv, a.ldv * a.Skv, 64, 128))) return rc;
-  // the looped operand is fetched in [CB x 64] boxes, the resident one in [128 x 64] boxes
-  constexpr int CBH = (D == 64) ? 64 : 128;
-  CUtensorMap tmQc = tmQ, tmdOc = tmdO, tmKc = tmK, tmVc = tmV;
-  if (CBH != 128) {
-    if ((rc = make_tmap_3d(&tmQc, a.q, W, a.Sq, a.B, a.ldq, a.ldq * a.Sq, 64, CBH))) return rc;
-    if ((rc = make_tmap_3d(&tmdOc, a.dctx, W, a.Sq, a.B, a.ld_dctx, a.ld_dctx * a.Sq, 64, CBH))) return rc;
-    if ((rc = make_tmap_3d(&tmKc, a.k, W, a.Skv, a.B, a.ldk, a.ldk * a.Skv, 64, CBH))) return rc;
-    if ((rc = make_tmap_3d(&tmVc, a.v, W, a.Skv, a.B, a.ldv, a.ldv * a.Skv, 64, CBH))) return rc;
-  }
   // delta = rowsum(dO * O)
   {
     const int64_t warps = static_cast<int64_t>(a.B) * a.Sq;
     const int threads = 256;
     const int64_t blocks = (warps * 32 + threads - 1) / threads;
-    MMFB_LAUNCH(attn_delta_kernel, static_cast<unsigned>(blocks), threads, 0, stream, 
+    MMFB_LAUNCH(attn_delta_kernel, static_cast<unsigned>(blocks), threads, 0, stream,
         reinterpret_cast<const bf16*>(a.dctx), a.ld_dctx, reinterpret_cast<const bf16*>(a.ctx), a.ldo, reinterpret_cast<const bf16*>(a.ctx_lo), a.delta,
         a.B, a.heads, a.Sq, D);
     count_launch();
   }
-  // d = 64 and both sequences within two 128-row blocks: single fused kernel, S/dP/exp computed once per block pair
-  static int use_fused = -1;
-  if (use_fused < 0) {
-    const char* e = getenv("MMFB_ATTN_FUSED_BWD");
-    use_fused = (e == nullptr) ? 1 : (e[0] != '0');
-  }
-  if (D == 64 && use_fused && a.Sq <= 256 && a.Skv <= 256) {
-    const int smem = 12 * 16384 + 3 * 1024 + 128 + 1024;
-    AttnBwdFusedDev f;
-    f.B = a.B; f.H = a.heads; f.Sq = a.Sq; f.Skv = a.Skv;
-    f.mask = a.mask; f.lse2 = a.lse2; f.delta = a.delta;
-    f.dmask = a.drop_mask; f.W = (a.Skv + 31) / 32; f.dscale = a.drop_mask ? a.drop_scale : 1.0f;
-    f.scale = 1.0f / sqrtf(static_cast<float>(D));
-    f.scale2 = LOG2E * f.scale;
-    f.dq = reinterpret_cast<bf16*>(a.dq); f.ld_dq = a.ld_dq;
-    f.dk = reinterpret_cast<bf16*>(a.dk); f.ld_dk = a.ld_dk;
-    f.dv = reinterpret_cast<bf16*>(a.dv); f.ld_dv = a.ld_dv;
-    static bool fset = false;
-    if (!fset) {
-      cudaError_t e = cudaFuncSetAttribute(attn_bwd_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_bwd_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-      if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_bwd_fused smem attr: %s", cudaGetErrorString(e));
-      fset = true;
-    }
-    dim3 grid(a.heads, a.B);
-    // default: the 16-warp kernel (measured 307 us against 336 us per layer at the bench shape, profiles/r2_kbench_before.json);
-    // MMFB_ATTN_BWD=8 (read per call) selects the 8-warp kernel for A/B runs
-    const char* w_env = getenv("MMFB_ATTN_BWD");
-    if (w_env == nullptr || w_env[0] == 'p') {
-      // default: the persistent kernel (one CTA per SM over its share of the (batch, head) items); MMFB_ATTN_BWD=16 / 8
-      // (read per call) select the one-CTA-per-item kernels for A/B runs
-      const int smem_p = 12 * 16384 + 2 * 768 * 4 + 256 * 8 * 4 + 256 + 1024;
-      static bool pers_attr = false;
-      if (!pers_attr) {
-        cudaError_t e = cudaFuncSetAttribute(attn_bwd_pers_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_p);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_bwd_pers_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_p);
-        if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_bwd(persistent) smem attr: %s", cudaGetErrorString(e));
-        pers_attr = true;
-      }
-      const int n_items = a.heads * a.B;
-      const int grid_p = n_items < num_sms() ? n_items : num_sms();
-      int* sched = sched_counters();
-      if (sched == nullptr) return set_error(MMFB_ERR_CUDA, "attn_bwd: scheduler counters");
-      CUtensorMap tmdQ, tmdK, tmdV;
-      if ((rc = make_tmap_3d(&tmdQ, a.dq, W, a.Sq, a.B, a.ld_dq, a.ld_dq * a.Sq, 64, 128))) return rc;
-      if ((rc = make_tmap_3d(&tmdK, a.dk, W, a.Skv, a.B, a.ld_dk, a.ld_dk * a.Skv, 64, 128))) return rc;
-      if ((rc = make_tmap_3d(&tmdV, a.dv, W, a.Skv, a.B, a.ld_dv, a.ld_dv * a.Skv, 64, 128))) return rc;
-      if (f.dmask != nullptr) MMFB_LAUNCH(attn_bwd_pers_kernel<true>, grid_p, BWD_PERS_THREADS, smem_p, stream, tmQ, tmdO, tmK, tmV, tmdQ, tmdK, tmdV, f, n_items, sched + 4);
-      else MMFB_LAUNCH(attn_bwd_pers_kernel<false>, grid_p, BWD_PERS_THREADS, smem_p, stream, tmQ, tmdO, tmK, tmV, tmdQ, tmdK, tmdV, f, n_items, sched + 4);
-    } else if (w_env[0] != '8') {
-      static bool w16_attr = false;
-      if (!w16_attr) {
-        cudaError_t e = cudaFuncSetAttribute(attn_bwd_fused16_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_bwd_fused16_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_bwd(fused16) smem attr: %s", cudaGetErrorString(e));
-        w16_attr = true;
-      }
-      if (f.dmask != nullptr) MMFB_LAUNCH(attn_bwd_fused16_kernel<true>, grid, 544, smem, stream, tmQ, tmdO, tmK, tmV, f);
-      else MMFB_LAUNCH(attn_bwd_fused16_kernel<false>, grid, 544, smem, stream, tmQ, tmdO, tmK, tmV, f);
-    } else if (f.dmask != nullptr) MMFB_LAUNCH(attn_bwd_fused_kernel<true>, grid, 288, smem, stream, tmQ, tmdO, tmK, tmV, f);
-    else MMFB_LAUNCH(attn_bwd_fused_kernel<false>, grid, 288, smem, stream, tmQ, tmdO, tmK, tmV, f);
-    count_launch();
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_bwd_fused launch: %s", cudaGetErrorString(e));
-    return MMFB_OK;
-  }
-  constexpr int DC = D / 64;
-  constexpr int CB = (D == 64) ? 64 : 128;   // d = 64: 64-wide looped blocks -> 256 TMEM columns, 2 CTAs per SM
-  const int smem = 2 * DC * 16384 + (CB == 64 ? 2 : 1) * 2 * DC * CB * 128 + 2 * (128 * CB * 2) + 2048 + 4096 + 128 + 1024;
   AttnBwdDev p;
   p.B = a.B; p.H = a.heads; p.Sq = a.Sq; p.Skv = a.Skv;
   p.mask = a.mask; p.lse2 = a.lse2; p.delta = a.delta;
   p.dmask = a.drop_mask; p.W = (a.Skv + 31) / 32; p.dscale = a.drop_mask ? a.drop_scale : 1.0f;
   p.scale = 1.0f / sqrtf(static_cast<float>(D));
   p.scale2 = LOG2E * p.scale;
-  static bool set = false;
-  if (!set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel<D, true, true, CB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_bwd_kernel<D, true, false, CB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_bwd_kernel<D, false, true, CB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(attn_bwd_kernel<D, false, false, CB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_bwd smem attr: %s", cudaGetErrorString(e));
-    set = true;
-  }
-  {
-    p.out0 = reinterpret_cast<bf16*>(a.dq); p.ld0 = a.ld_dq; p.out1 = nullptr; p.ld1 = 0;
-    dim3 grid((a.Sq + 127) / 128, a.heads, a.B);
-    if (p.dmask != nullptr) MMFB_LAUNCH((attn_bwd_kernel<D, true, true, CB>), grid, 160, smem, stream, tmQ, tmdO, tmKc, tmVc, p);
-    else MMFB_LAUNCH((attn_bwd_kernel<D, true, false, CB>), grid, 160, smem, stream, tmQ, tmdO, tmKc, tmVc, p);
-    count_launch();
-  }
-  {
-    p.out0 = reinterpret_cast<bf16*>(a.dk); p.ld0 = a.ld_dk;
-    p.out1 = reinterpret_cast<bf16*>(a.dv); p.ld1 = a.ld_dv;
-    dim3 grid((a.Skv + 127) / 128, a.heads, a.B);
-    if (p.dmask != nullptr) MMFB_LAUNCH((attn_bwd_kernel<D, false, true, CB>), grid, 160, smem, stream, tmK, tmV, tmQc, tmdOc, p);
-    else MMFB_LAUNCH((attn_bwd_kernel<D, false, false, CB>), grid, 160, smem, stream, tmK, tmV, tmQc, tmdOc, p);
-    count_launch();
-  }
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_bwd launch: %s", cudaGetErrorString(e));
-  return MMFB_OK;
+  return a.drop_mask != nullptr ? attn_bwd_kernels<D, true>(a, p, stream) : attn_bwd_kernels<D, false>(a, p, stream);
 }
 
 int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
@@ -2486,16 +703,3 @@ int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
 }
 
 }  // namespace mmfb
-
-#ifdef MMFB_TRACE
-// development builds only: copies the trace stamps of CTA 0 to the host (see MMFB_TR above, tools/trace_attn.py)
-extern "C" int mmfb_trace_read(long long* host, int n) {
-  if (n > 4 * 64 * 16) n = 4 * 64 * 16;
-  cudaDeviceSynchronize();
-  return cudaMemcpyFromSymbol(host, mmfb::mmfb_trace_buf, sizeof(long long) * n) == cudaSuccess ? 0 : 1;
-}
-extern "C" int mmfb_trace_clear(void) {
-  static long long zeros[4 * 64 * 16];
-  return cudaMemcpyToSymbol(mmfb::mmfb_trace_buf, zeros, sizeof(zeros)) == cudaSuccess ? 0 : 1;
-}
-#endif

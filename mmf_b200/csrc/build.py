@@ -1,11 +1,11 @@
-"""Builds libmmfb200.so (sm_100a only) in-tree with nvcc.
+"""Builds libmmfb200.so (sm_90a only) in-tree with nvcc.
 
     python -m mmf_b200.csrc.build [--force] [--verbose]
     python -m mmf_b200.csrc.build --variant NAME -DFLAG=1 ...   # libmmfb200_NAME.so with extra defines, for A/B runs
                                                                 # (select it at run time with MMFB_LIB=<path>)
 
-The built library lives next to the sources (git-ignored, but it travels to the GPU box with
-the gpurun snapshot).  There is exactly one target architecture: compute_100a / sm_100a.
+The built library lives next to the sources (git-ignored).  There is exactly one target architecture:
+compute_90a / sm_90a (H100).
 """
 import hashlib
 import os
@@ -19,7 +19,7 @@ LIB = os.path.join(HERE, "libmmfb200.so")
 STAMP = os.path.join(HERE, ".build_stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -80,7 +80,7 @@ def build(force=False, verbose=False, variant=None, defines=()):
                     sys.stderr.write("[%s] %s\n" % (src, line))
     if failed:
         raise RuntimeError("building libmmfb200.so failed")
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("linking libmmfb200.so failed:\n" + r.stdout)
@@ -105,7 +105,7 @@ def _build_variant(name, defines, verbose):
         for line in o.splitlines():
             if verbose or ("spill" in line and "0 bytes spill stores, 0 bytes spill loads" not in line):
                 sys.stderr.write("[%s %s] %s\n" % (name, src, line))
-    r = subprocess.run([nvcc, "-shared", "-o", out] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
+    r = subprocess.run([nvcc, "-shared", "-o", out] + objs + ["-gencode", "arch=compute_90a,code=sm_90a",
                                                              "-cudart", "static"],
                        stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:

@@ -39,7 +39,7 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -107,7 +107,7 @@ static int check_device() {
       cudaGetLastError();
       return 0;  // not cached: a device may appear later (e.g. after CUDA_VISIBLE_DEVICES changes)
     }
-    ok = (major == 10) ? 1 : 0;
+    ok = (major == 9) ? 1 : 0;
   }
   return ok;
 }
@@ -119,7 +119,7 @@ using namespace mmfb;
 #define MMFB_REQUIRE_DEVICE()                                                                              \
   do {                                                                                                     \
     if (!check_device())                                                                                   \
-      return set_error(MMFB_ERR_DEVICE, "libmmfb200 needs an sm_100 (B200) device; there is no CPU fallback"); \
+      return set_error(MMFB_ERR_DEVICE, "libmmfb200 needs an sm_90 (H100) device; there is no CPU fallback"); \
   } while (0)
 
 extern "C" {

@@ -1,4 +1,4 @@
-// Cross-entropy over vocabulary-sized rows, forward AND backward in one pass over each row (sm_100a).
+// Cross-entropy over vocabulary-sized rows, forward AND backward in one pass over each row (sm_90a).
 //
 //   loss_i  = logsumexp(z_i) - z_i[label_i]                      (rows with label == ignore_index contribute nothing)
 //   dz_i    = (softmax(z_i) - onehot(label_i)) * grad_scale      written IN PLACE over the logits (bf16)

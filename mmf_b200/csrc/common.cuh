@@ -1,7 +1,7 @@
-// Shared device-side primitives for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM
-// wrappers (inline PTX), UMMA descriptor builders, Philox dropout, small math helpers.
+// Shared device-side primitives for the sm_90a kernels: mbarrier, TMA, wgmma / mma.sync wrappers (inline PTX),
+// wgmma descriptor builders, Philox dropout, small math helpers.
 //
-// Everything in csrc/ is written for sm_100a only (B200); there is no other code path.
+// Everything in csrc/ is written for sm_90a only (H100); there is no other code path.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -27,22 +27,10 @@ __device__ __forceinline__ uint8_t* smem_align1024(uint8_t* raw) {
   return raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
 }
 
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // --------------------------------------------------------------------------------------
 // programmatic dependent launch: every kernel of the library lets the NEXT kernel of the stream start launching as soon
 // as all of its own CTAs have started (griddep_launch at the top), and waits for the PREVIOUS kernel to have completed and
-// flushed its memory before it touches global data (griddep_wait after its own set-up: barrier init, TMEM allocation,
+// flushed its memory before it touches global data (griddep_wait after its own set-up: barrier init,
 // descriptor prefetch).  The launch latency and the prologue of kernel n+1 overlap the tail of kernel n; both
 // instructions are no-ops when the kernel was launched without the attribute (MMFB_PDL=0).
 // --------------------------------------------------------------------------------------
@@ -58,7 +46,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// make generic-proxy smem writes visible to the async proxy (TMA / tcgen05 operand reads)
+// make generic-proxy smem writes visible to the async proxy (TMA stores / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -82,25 +70,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// non-blocking probe (mbarrier.test_wait returns at once; try_wait may suspend the thread for a hardware time slice)
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 // Wait with a watchdog: a protocol bug must abort the kernel (trap) instead of hanging the GPU.
 // The spin loop is kept to three instructions per failed probe (try_wait itself suspends the warp in hardware for a
-// while before it returns false): the clock is read only every 2^16 probes.  The round-1 loop read the clock on every
-// probe, and ncu showed 27 % of the attention forward's issued warp-instructions in it (CS2R / ISETP / BRA), taken from
-// the second CTA on the SM.
+// while before it returns false): the clock is read only every 2^16 probes, so that a waiting warp takes few issue
+// slots from the other warps of its SM.  No function call (printf) in it: the GEMM consumers wait between wgmma commit
+// and wgmma wait, and a call there makes ptxas serialise every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = 0;
@@ -109,10 +83,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if ((spins & 0xFFFFu) == 0) {
       const long long now = clock64();
       if (t0 == 0) t0 = now;
-      else if (now - t0 > 8000000000LL) {  // ~4 s at 2 GHz
-        printf("mmfb: mbarrier wait timeout (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x);
-        __trap();
-      }
+      else if (now - t0 > 8000000000LL) __trap();  // ~4 s at 2 GHz
     }
   }
 }
@@ -138,202 +109,83 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// multicast variant: the box lands at the same CTA-relative smem offset in every CTA of `mask`, and each destination
-// CTA's mbarrier (same CTA-relative address) receives the complete_tx bytes
-__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                               uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
-      "%4}], [%2], %5;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
 // --------------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// --------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate, issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// ---- cta_group::2 (CTA pair) variants --------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[128 rows in each CTA's smem] * B[N/2 rows in each CTA's smem]; issued by the leader only
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-// TMA load into THIS CTA's smem whose completion bytes are credited to the mbarrier at the same offset in the pair's
-// leader CTA (peer bit of the shared::cluster address cleared)
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
-}
-// arrive on the mbarrier at this CTA-relative address in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(rank)
-      : "memory");
-}
-// same, arriving on the barrier at this CTA-relative address in every CTA of `mask` (cluster pipelines)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 columns of fp32: thread t of the warp receives lane (row) t, columns [c, c+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]),
-        "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-        "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-// registers -> TMEM, 32 lanes x 16 columns (thread t of the warp writes lane t)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand is read from tensor memory (K-major only: lane = row, 16-bit elements
-// packed two per 32-bit column in K order, so one K=16 step spans 8 columns).  Issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// --------------------------------------------------------------------------------------
-// UMMA shared-memory matrix descriptors (SWIZZLE_128B canonical layouts, bf16)
+// wgmma (warpgroup MMA, sm_90a): D[64 x N] (+)= A[64 x 16] * B[16 x N]^T, bf16 operands from shared memory,
+// fp32 accumulators in registers, issued by all 128 threads of a warpgroup.
 //
+// Shared-memory matrix descriptors, SWIZZLE_128B canonical layouts (bf16):
 // K-major operand tile  [rows][64 k]  : each row is one 128-byte line (64 bf16 along K), lines of 8
 //   consecutive rows form a 1024-byte swizzle atom (exactly what a TMA box {64, rows} with
-//   CU_TENSOR_MAP_SWIZZLE_128B writes).  SBO = 1024 B (next 8 rows). One UMMA (K=16) reads 32 bytes
-//   of each line, so the k-th UMMA of the tile starts 32*k bytes further.
+//   CU_TENSOR_MAP_SWIZZLE_128B writes).  SBO = 1024 B (next 8 rows).  One wgmma (K=16) reads 32 bytes
+//   of each line, so the k-th wgmma of the tile starts 32*k bytes further.
 // MN-major operand tile [64 k][64 mn] per 8 KB panel: each line is one k, 64 bf16 along M/N (TMA box
-//   {64 mn, 64 k}); SBO = 1024 B (next 8 k), LBO = bytes between 64-wide mn panels.  One UMMA (K=16)
+//   {64 mn, 64 k}); SBO = 1024 B (next 8 k), LBO = bytes between 64-wide mn panels.  One wgmma (K=16)
 //   reads 16 lines = 2048 bytes.
-// Descriptor bits: [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, [46,48) version=1, [61,64) layout=2.
+// Descriptor bits: [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, [62,64) layout (1 = 128-byte swizzle).
+//
+// Accumulator layout of m64nNk16 (f32): thread t of warp w of the warpgroup holds d[i], i < N/2, at
+//   row 16 w + t/4 + 8 ((i/2) & 1), column 8 (i/4) + 2 (t%4) + (i & 1).
 // --------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// instruction descriptor, kind::f16, A/B = bf16, D = fp32
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4)                              // D format: F32
-         | (1u << 7)                            // A format: BF16
-         | (1u << 10)                           // B format: BF16
-         | ((a_mn_major ? 1u : 0u) << 15)       // A major
-         | ((b_mn_major ? 1u : 0u) << 16)       // B major
-         | (static_cast<uint32_t>(N >> 3) << 17)  // N
-         | (static_cast<uint32_t>(M >> 4) << 24); // M
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// TA / TB = 1: the A / B operand is MN-major (transposed) in shared memory
+#define MMFB_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                   "+f"(d[i + 6]), "+f"(d[i + 7])
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}\n"
+      : MMFB_F8(0), MMFB_F8(8), MMFB_F8(16), MMFB_F8(24),
+        MMFB_F8(32), MMFB_F8(40), MMFB_F8(48), MMFB_F8(56)
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, %131, %132;\n\t}\n"
+      : MMFB_F8(0), MMFB_F8(8), MMFB_F8(16), MMFB_F8(24),
+        MMFB_F8(32), MMFB_F8(40), MMFB_F8(48), MMFB_F8(56),
+        MMFB_F8(64), MMFB_F8(72), MMFB_F8(80), MMFB_F8(88),
+        MMFB_F8(96), MMFB_F8(104), MMFB_F8(112), MMFB_F8(120)
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+}
+#undef MMFB_F8
+
+// --------------------------------------------------------------------------------------
+// mma.sync (m16n8k16, bf16 -> fp32) and ldmatrix, for the attention kernels whose operands are register tiles
+// --------------------------------------------------------------------------------------
+__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr));
+}
+__device__ __forceinline__ void ldsm_x4_t(uint32_t (&r)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr));
 }
 
 // --------------------------------------------------------------------------------------
@@ -397,14 +249,9 @@ __device__ __forceinline__ float gelu_erf_grad(float x) {
   const float cdf = gelu_phi_parts(x, e);
   return fmaf(x * 0.3989422804014327f, e, cdf);
 }
-// ---- packed fp32 pairs (sm_100 FFMA2 / FMUL2 / FADD2: two IEEE fp32 lanes per FMA-pipe issue slot) ----
-// Lane results are bit-identical to the scalar fmaf / * / + (round-to-nearest, no ftz), so a packed epilogue is a pure
-// issue-slot optimisation.  On by default since round 2 (isolated timings, profiles/r2_kbench_before*.json: FFN-up GEMM
-// + GELU 165 -> 152 us, GELU' dgrad 177 -> 154 us, fused attention backward 307 -> 296 us); -DMMFB_F32X2=0 builds the
-// scalar variant for A/B runs.  See gelu_erf2 / gelu_erf_grad_mul2.
-#ifndef MMFB_F32X2
-#define MMFB_F32X2 1
-#endif
+// ---- fp32 pairs carried in one 64-bit value ----
+// The row kernels keep pairs of fp32 lanes together (two bf16 of a packed word).  Hopper has no packed fp32 arithmetic,
+// so each helper is two scalar IEEE operations (round-to-nearest, no ftz): the results equal fmaf / * / + per lane.
 __device__ __forceinline__ uint64_t pk2(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -414,53 +261,19 @@ __device__ __forceinline__ void upk2(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  upk2(a, a0, a1); upk2(b, b0, b1); upk2(c, c0, c1);
+  return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1); upk2(b, b0, b1);
+  return pk2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// Phi(x) and exp(-x^2/2) for the pair (x0, x1): the arithmetic of gelu_phi_parts, two lanes at a time (the negated
-// polynomial coefficients give -(poly) exactly, so -poly*t needs no separate negation)
-__device__ __forceinline__ uint64_t gelu_phi_parts2(float x0, float x1, uint64_t x, uint64_t& e) {
-  const uint64_t den = fma2(pk2(fabsf(x0), fabsf(x1)), pk2(0.3275911f * 0.70710678118654752f, 0.3275911f * 0.70710678118654752f),
-                            pk2(1.0f, 1.0f));
-  float d0, d1;
-  upk2(den, d0, d1);
-  const uint64_t t = pk2(rcp_approx(d0), rcp_approx(d1));
-  const uint64_t arg = mul2(mul2(x, x), pk2(-0.5f * 1.4426950408889634f, -0.5f * 1.4426950408889634f));
-  float a0, a1;
-  upk2(arg, a0, a1);
-  e = pk2(ex2_approx(a0), ex2_approx(a1));
-  uint64_t np = fma2(pk2(-1.061405429f, -1.061405429f), t, pk2(1.453152027f, 1.453152027f));
-  np = fma2(np, t, pk2(-1.421413741f, -1.421413741f));
-  np = fma2(np, t, pk2(0.284496736f, 0.284496736f));
-  np = fma2(np, t, pk2(-0.254829592f, -0.254829592f));
-  const uint64_t erf_abs = fma2(mul2(np, t), e, pk2(1.0f, 1.0f));
-  float r0, r1;
-  upk2(erf_abs, r0, r1);
-  return fma2(pk2(0.5f, 0.5f), pk2(copysignf(r0, x0), copysignf(r1, x1)), pk2(0.5f, 0.5f));
-}
-__device__ __forceinline__ void gelu_erf2(float x0, float x1, float& y0, float& y1) {
-  const uint64_t x = pk2(x0, x1);
-  uint64_t e;
-  upk2(mul2(x, gelu_phi_parts2(x0, x1, x, e)), y0, y1);
-}
-// (v0, v1) *= GELU'(x0), GELU'(x1)
-__device__ __forceinline__ void gelu_erf_grad_mul2(float x0, float x1, float& v0, float& v1) {
-  const uint64_t x = pk2(x0, x1);
-  uint64_t e;
-  const uint64_t cdf = gelu_phi_parts2(x0, x1, x, e);
-  const uint64_t g = fma2(mul2(x, pk2(0.3989422804014327f, 0.3989422804014327f)), e, cdf);
-  upk2(mul2(pk2(v0, v1), g), v0, v1);
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1); upk2(b, b0, b1);
+  return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   __nv_bfloat162 v = __floats2bfloat162_rn(a, b);

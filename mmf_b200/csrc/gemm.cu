@@ -1,30 +1,24 @@
-// tcgen05 GEMM family for the fusion block (sm_100a).
+// wgmma GEMM family for the fusion block (sm_90a).
 //
-//   C[M,N] = epilogue( A[M,K] * B[N,K]^T )       bf16 operands, fp32 accumulation in TMEM
+//   C[M,N] = epilogue( A[M,K] * B[N,K]^T )       bf16 operands, fp32 accumulation in registers
 //
-// One persistent CTA per SM, 192 threads:
-//   warp 0     : TMA producer (one elected thread) - fills a STAGES-deep smem ring of 128x64 A tiles
-//                and BNx64 B tiles (SWIZZLE_128B), signalling `full[s]` with complete_tx bytes
-//   warp 1     : TMEM allocator + MMA issuer (one thread) - tcgen05.mma cta_group::1 kind::f16,
-//                128 x BN x 16 per instruction, accumulating into one of two TMEM stages;
-//                tcgen05.commit releases smem slots (`empty[s]`) and publishes the accumulator
-//                (`tmem_full[a]`)
-//   warps 2..9 : epilogue - two sets of four warps (one warp per TMEM lane quarter) that take alternate
-//                64-column slices of the accumulator: tcgen05.ld (thread == accumulator row), fused
-//                elementwise epilogue, bf16 results staged in swizzled smem and written with TMA stores
-//                (or fp32 vector reductions for the split-K weight-gradient GEMM).  Eight warps because the
-//                GELU / GELU' epilogues are ALU-bound: two warps per scheduler hide each other's latency.
-// Double-buffered accumulators let the epilogue of tile i overlap the MMAs of tile i+1.
+// One CTA per (128 x BN output tile, K split), 384 threads = three warpgroups:
+//   warpgroup 0    : TMA producer (one thread) - fills a STAGES-deep smem ring of 128x64 A tiles and BNx64 B tiles
+//                    (SWIZZLE_128B), signalling `full[s]` with complete_tx bytes
+//   warpgroups 1,2 : consumers - each owns 64 rows of the tile and issues wgmma m64nBNk16 straight from the smem
+//                    ring (one k-block in flight while the previous one retires and its slot is released through
+//                    `empty[s]`), then runs the fused elementwise epilogue from its accumulator registers and writes
+//                    bf16 pairs (or fp32 vector reductions for the split-K weight-gradient GEMM) to global memory.
 //
 // Operand layouts: each of A and B may be K-major (row-major [rows, K]) or MN-major (row-major
 // [K, rows]); the latter is what the backward pass needs (dgrad reads W[out,in] as B[N=in,K=out],
 // wgrad reads dY[tokens,out] as A[M=out,K=tokens] and X[tokens,in] as B[N=in,K=tokens]) without
-// ever materialising a transpose in HBM.
+// ever materialising a transpose in HBM: wgmma reads MN-major bf16 tiles directly (transpose bits).
 //
-// Reference ops this replaces (mmf = /root/reference): the nn.Linear calls in
-// mmf/modules/hf_layers.py:169-180 (Q,K,V), HF BertSelfOutput/BertIntermediate/BertOutput invoked at
-// hf_layers.py:248,289-290, mmf/models/vilbert.py:77-79,127,144-145,396-412,504-509 and their
-// autograd backward (mmf/trainers/core/training_loop.py:211-213).
+// Reference ops this replaces (mmf): the nn.Linear calls in mmf/modules/hf_layers.py:169-180 (Q,K,V),
+// HF BertSelfOutput/BertIntermediate/BertOutput invoked at hf_layers.py:248,289-290,
+// mmf/models/vilbert.py:77-79,127,144-145,396-412,504-509 and their autograd backward
+// (mmf/trainers/core/training_loop.py:211-213).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -34,14 +28,15 @@ namespace mmfb {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int NUM_THREADS = 320;
-constexpr int STG_BYTES = 128 * 64 * 2;  // one 128-row x 64-col bf16 staging slice (SW128)
+constexpr int NUM_THREADS = 384;
 
 struct GemmDev {
   int M, N, K;
   int splits;
+  bf16* c;               // bf16 destination [M, ldc]
+  bf16* c2;              // second bf16 destination (EPI_BIAS_GELU)
   float* c32;            // EPI_ATOMIC_F32 destination
-  int64_t ldc32;
+  int64_t ldc;
   const bf16* bias;      // [N] or null
   const bf16* aux;       // residual / pre-activation, [M, ldaux]
   int64_t ldaux;
@@ -50,460 +45,185 @@ struct GemmDev {
   float dscale;          // 1/(1-p)
 };
 
-// internal epilogue id: EPI_BIAS_DROP_RESID with the residual tile staged by TMA (chosen by the dispatcher for short-K
-// GEMMs, where the mainloop is too short to hide the epilogue's strided global loads of the residual)
-constexpr int EPI_BIAS_DROP_RESID_T = 32;
-constexpr bool is_drop_resid(int epi) { return epi == EPI_BIAS_DROP_RESID || epi == EPI_BIAS_DROP_RESID_T; }
-constexpr bool epi_uses_aux(int epi) { return is_drop_resid(epi) || epi == EPI_GELU_BWD || epi == EPI_ADD_AUX; }
-
-template <int BN, bool MC = false, int EPI = EPI_BIAS>
+template <int BN>
 struct Cfg {
-  // AUX_TMA: the residual / pre-activation tile the epilogue needs is prefetched by TMA into swizzled smem slices
-  // (2 sets x 2 buffers x 16 KB) one slice ahead, instead of strided global loads in the epilogue's critical path.
-  // Only in the CTA-pair mode, whose 32 KB stages leave room for it.
-  // Measured (profiles/README.md): a clear win for the GELU' dgrad (K = hidden: short mainloop, heavy epilogue: 107 -> 79 us);
-  // for the residual epilogues of the K = 3072 / 2304 GEMMs the ring shrinking from 6 to 4 stages costs more than
-  // the staging saves, so those keep the direct 16-byte global loads.
-  // Round 2 (ncu source view of the attention out-projection, K = N = 768: 51 % of the stall samples on the first use of the
-  // residual's LDG.128 / the mask word, tensor pipe 40 % active): the short-K residual epilogue stages its tile the same
-  // way (EPI_BIAS_DROP_RESID_T); 4 stages are plenty for 12 k-blocks.
-  static constexpr bool AUX_TMA = MC && (EPI == EPI_GELU_BWD || EPI == EPI_BIAS_DROP_RESID_T);
-  static constexpr int AUX_BYTES = AUX_TMA ? 4 * STG_BYTES : 0;
-  // MC (CTA pair, 2-SM MMA): each CTA stages only half of the B tile -> 32 KB per stage, deeper ring
-  static constexpr int STAGES = MC ? (AUX_TMA ? ((BN == 256) ? 4 : 5) : ((BN == 256) ? 6 : 8)) : ((BN == 256) ? 4 : 6);
+  // 192 KB of operand ring either way: 6 stages of 32 KB (BN = 128) or 4 stages of 48 KB (BN = 256)
+  static constexpr int STAGES = (BN == 256) ? 4 : 6;
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = (MC ? BN / 2 : BN) * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int TMEM_COLS = 2 * BN;  // 512 or 256 (power of two)
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * STG_BYTES + AUX_BYTES + 256 + 1024;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
 };
 
-__device__ __forceinline__ void named_bar_sync(int id, int n) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_tile(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (BN == 256) wgmma_n256<TA, TB>(acc, da, db, accumulate);
+  else wgmma_n128<TA, TB>(acc, da, db, accumulate);
 }
 
-template <int BN, bool A_MN, bool B_MN, int EPI, bool MC>
+template <int BN, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
-            const __grid_constant__ CUtensorMap tmAux, GemmDev p) {
-  using C = Cfg<BN, MC, EPI>;
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmDev p) {
+  using C = Cfg<BN>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
-  uint8_t* stg = smem + STAGES * C::STAGE_BYTES;
-  uint8_t* auxs = stg + 2 * STG_BYTES;     // [2 sets][2 buffers] 16 KB aux slices (AUX_TMA only)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(auxs + C::AUX_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * C::STAGE_BYTES);
   uint64_t* full = bars;                  // [STAGES]
   uint64_t* empty = bars + STAGES;        // [STAGES]
-  uint64_t* tfull = bars + 2 * STAGES;    // [2]
-  uint64_t* tempty = bars + 2 * STAGES + 2;  // [2]
-  uint64_t* auxfull = bars + 2 * STAGES + 4;  // [2 sets][2 buffers]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 8);
 
   griddep_launch();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles_m = (p.M + BM - 1) / BM, tiles_n = (p.N + BN - 1) / BN;
+  const int wg = threadIdx.x >> 7;
+  const int tiles_n = (p.N + BN - 1) / BN;
   const int kb_total = (p.K + BK - 1) / BK;
   const int kb_per_split = (kb_total + p.splits - 1) / p.splits;
-  // MC: a CTA pair (cluster of two, one TPC) computes a 256 x BN tile with the 2-SM MMA (tcgen05 cta_group::2):
-  // each CTA stages its 128 rows of A and HALF of the B tile, the leader issues the MMAs, each CTA's TMEM receives
-  // its own 128 accumulator rows.  Halves the per-SM shared-memory traffic of the B operand.  Work units are pairs.
-  const int crank = MC ? static_cast<int>(cluster_ctarank()) : 0;
-  const int units = (MC ? (tiles_m + 1) / 2 : tiles_m) * tiles_n * p.splits;
-  const int u_first = MC ? (blockIdx.x >> 1) : blockIdx.x;
-  const int u_step = MC ? (gridDim.x >> 1) : gridDim.x;
+  const int split = blockIdx.x % p.splits;
+  const int t = blockIdx.x / p.splits;
+  const int m0 = (t / tiles_n) * BM, n0 = (t % tiles_n) * BN;
+  const int kb0 = split * kb_per_split;
+  const int kb1 = min(kb_total, kb0 + kb_per_split);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (EPI != EPI_ATOMIC_F32) tma_prefetch_desc(&tmC);
-    if (C::AUX_TMA) tma_prefetch_desc(&tmAux);
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full[s], MC ? 2 : 1);    // MC (leader's barrier): own producer (+expect_tx of both CTAs' bytes) + peer producer
-      mbar_init(&empty[s], 1);            // MC: released by the leader's multicast tcgen05.commit
-    }
-    for (int a = 0; a < 4; ++a) mbar_init(&auxfull[a], 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull[a], 1);
-      mbar_init(&tempty[a], MC ? 512 : 256);   // MC (leader's barrier): both CTAs' epilogue threads
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 256);          // every consumer thread releases the slot after its wgmma retired
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if (MC) { tmem_alloc_2sm(tmem_slot, C::TMEM_COLS); tmem_relinquish_2sm(); }
-    else { tmem_alloc(tmem_slot, C::TMEM_COLS); tmem_relinquish(); }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (MC) cluster_sync_all();   // peer barriers are initialised before any multicast / remote arrive targets them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_wait();        // operands / aux / bias of this GEMM may come from the kernel that is still finishing
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       int s = 0;
       uint32_t ph = 0;
-      for (int u = u_first; u < units; u += u_step) {
-        const int split = u % p.splits;
-        const int t = u / p.splits;
-        const int m0 = (MC ? 2 * (t / tiles_n) + crank : (t / tiles_n)) * BM, n0 = (t % tiles_n) * BN;
-        const int kb0 = split * kb_per_split;
-        const int kb1 = min(kb_total, kb0 + kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty[s], ph ^ 1);
-          uint8_t* sa = smem + s * C::STAGE_BYTES;
-          uint8_t* sb = sa + C::A_BYTES;
-          if (MC) {
-            // both CTAs' loads credit the LEADER's full barrier; the leader arms it for the pair's total bytes
-            if (crank == 0) mbar_expect_tx(&full[s], 2 * C::STAGE_BYTES);
-            else mbar_arrive_remote(&full[s], 0);
-            if (!A_MN) {
-              tma_load_2d_2sm(sa, &tmA, &full[s], kb * BK, m0);
-            } else {
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&empty[s], ph ^ 1);
+        uint8_t* sa = smem + s * C::STAGE_BYTES;
+        uint8_t* sb = sa + C::A_BYTES;
+        mbar_expect_tx(&full[s], C::STAGE_BYTES);
+        if (!A_MN) {
+          tma_load_2d(sa, &tmA, &full[s], kb * BK, m0);
+        } else {
 #pragma unroll
-              for (int pnl = 0; pnl < BM / 64; ++pnl) tma_load_2d_2sm(sa + pnl * 8192, &tmA, &full[s], m0 + pnl * 64, kb * BK);
-            }
-            if (!B_MN) {
-              tma_load_2d_2sm(sb, &tmB, &full[s], kb * BK, n0 + crank * (BN / 2));
-            } else {
-#pragma unroll
-              for (int pnl = 0; pnl < BN / 128; ++pnl)
-                tma_load_2d_2sm(sb + pnl * 8192, &tmB, &full[s], n0 + (crank * (BN / 128) + pnl) * 64, kb * BK);
-            }
-            if (++s == STAGES) { s = 0; ph ^= 1; }
-            continue;
-          }
-          mbar_expect_tx(&full[s], C::STAGE_BYTES);
-          if (!A_MN) {
-            tma_load_2d(sa, &tmA, &full[s], kb * BK, m0);
-          } else {
-#pragma unroll
-            for (int pnl = 0; pnl < BM / 64; ++pnl) tma_load_2d(sa + pnl * 8192, &tmA, &full[s], m0 + pnl * 64, kb * BK);
-          }
-          if (!B_MN) {
-            tma_load_2d(sb, &tmB, &full[s], kb * BK, n0);
-          } else {
-#pragma unroll
-            for (int pnl = 0; pnl < BN / 64; ++pnl) tma_load_2d(sb + pnl * 8192, &tmB, &full[s], n0 + pnl * 64, kb * BK);
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+          for (int pnl = 0; pnl < BM / 64; ++pnl) tma_load_2d(sa + pnl * 8192, &tmA, &full[s], m0 + pnl * 64, kb * BK);
         }
+        if (!B_MN) {
+          tma_load_2d(sb, &tmB, &full[s], kb * BK, n0);
+        } else {
+#pragma unroll
+          for (int pnl = 0; pnl < BN / 64; ++pnl) tma_load_2d(sb + pnl * 8192, &tmB, &full[s], n0 + pnl * 64, kb * BK);
+        }
+        if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer --------------------------------
-    if (lane == 0 && (!MC || crank == 0)) {
-      constexpr uint32_t idesc = umma_idesc_bf16(MC ? 2 * BM : BM, BN, A_MN, B_MN);
-      int s = 0;
-      uint32_t ph = 0;
-      int as = 0;
-      uint32_t aph = 0;
-      for (int u = u_first; u < units; u += u_step) {
-        const int split = u % p.splits;
-        const int kb0 = split * kb_per_split;
-        const int kb1 = min(kb_total, kb0 + kb_per_split);
-        mbar_wait(&tempty[as], aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * C::STAGE_BYTES);
-          const uint32_t sb = sa + C::A_BYTES;
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint64_t da = A_MN ? umma_desc_sw128(sa + kk * 2048, 8192, 1024) : umma_desc_sw128(sa + kk * 32, 16, 1024);
-            const uint64_t db = B_MN ? umma_desc_sw128(sb + kk * 2048, 8192, 1024) : umma_desc_sw128(sb + kk * 32, 16, 1024);
-            if (MC) umma_bf16_2sm(d_tmem, da, db, idesc, (kb > kb0 || kk > 0) ? 1u : 0u);
-            else umma_bf16(d_tmem, da, db, idesc, (kb > kb0 || kk > 0) ? 1u : 0u);
-          }
-          if (MC) umma_commit_2sm_mc(&empty[s], 3); else umma_commit(&empty[s]);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-        if (MC) umma_commit_2sm_mc(&tfull[as], 3); else umma_commit(&tfull[as]);
-        if (++as == 2) { as = 0; aph ^= 1; }
-      }
-    }
-  } else {
-    // ------------------------------ epilogue ----------------------------------
-    const int quarter = warp & 3;           // TMEM lane quarter this warp may access (hardware rule: warp id % 4)
-    const int set = (warp - 2) >> 2;        // 0: warps 2..5, 1: warps 6..9
-    const int row = quarter * 32 + lane;    // accumulator row inside the tile
-    const bool store_thread = (threadIdx.x == 64 + set * 128);
-    const int bar_id = 1 + set;
-    uint8_t* stg_set = stg + set * STG_BYTES;   // one staging slice per warp set
-    constexpr int NSL = BN / 64;            // 64-column slices per tile; this set owns slices sl with (sl & 1) == set
-    constexpr int SPT = NSL / 2;            // slices per tile for one set
-    int as = 0;
-    uint32_t aph = 0;
-    int gslice = 0;                         // running index of the slices this set has processed (aux double buffer)
-    // coordinates of this set's k-th slice, false past the end of the schedule
-    auto slice_coords = [&](int k, int& am0, int& an) -> bool {
-      const int u2 = u_first + (k / SPT) * u_step;
-      if (u2 >= units) return false;
-      const int t2 = u2 / p.splits;
-      am0 = (MC ? 2 * (t2 / tiles_n) + crank : (t2 / tiles_n)) * BM;
-      an = (t2 % tiles_n) * BN + (set + 2 * (k % SPT)) * 64;
-      return true;
-    };
-    auto aux_prefetch = [&](int k) {        // store_thread only
-      int am0, an;
-      if (slice_coords(k, am0, an)) {
-        uint64_t* bar = &auxfull[set * 2 + (k & 1)];
-        mbar_expect_tx(bar, STG_BYTES);
-        tma_load_2d(auxs + (set * 2 + (k & 1)) * STG_BYTES, &tmAux, bar, an, am0);
-      }
-    };
-    if (C::AUX_TMA && store_thread) aux_prefetch(0);
-    for (int u = u_first; u < units; u += u_step) {
-      const int t = u / p.splits;
-      const int m0 = (MC ? 2 * (t / tiles_n) + crank : (t / tiles_n)) * BM, n0 = (t % tiles_n) * BN;
-      const int m = m0 + row;
-      const bool row_ok = m < p.M;
-      mbar_wait(&tfull[as], aph);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + as * BN;
-
-      if (EPI == EPI_ATOMIC_F32) {
-#pragma unroll 1
-        for (int c = set; c < BN / 32; c += 2) {
-          uint32_t r[32];
-          tmem_ld32(t_row + c * 32, r);
-          tmem_ld_wait();
-          const int n = n0 + c * 32;
-          if (row_ok) {
-            float* dst = p.c32 + static_cast<int64_t>(m) * p.ldc32 + n;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              if (n + j < p.N) {
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j),
-                             "f"(__uint_as_float(r[j])), "f"(__uint_as_float(r[j + 1])),
-                             "f"(__uint_as_float(r[j + 2])), "f"(__uint_as_float(r[j + 3]))
-                             : "memory");
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        if (MC && crank != 0) mbar_arrive_remote(&tempty[as], 0); else mbar_arrive(&tempty[as]);
-      } else {
-#pragma unroll 1
-        for (int sl = set; sl < NSL; sl += 2) {  // 64-column slices of this warp set
-          // 1) everything that does not need the staging buffer: TMEM -> registers, fused math, bf16 packing.
-          //    The previous slice's TMA store drains the (single) staging buffer meanwhile.
-          uint32_t pk[32];                       // this thread's 64 output columns, packed bf16 pairs
-          uint32_t hk[EPI == EPI_BIAS_GELU ? 32 : 1];
-          const uint8_t* auxrow = nullptr;
-          uint32_t mbits[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
-          if (is_drop_resid(EPI) && p.dmask != nullptr && row_ok) {
-            // the two keep-bit words of this slice are fetched before the accumulator loads, not in the middle of the math
-            const int ns = n0 + sl * 64;
-            const uint32_t* mp = p.dmask + static_cast<int64_t>(m) * p.ldmask + (ns >> 5);
-            if (ns < p.N) mbits[0] = __ldg(mp);
-            if (ns + 32 < p.N) mbits[1] = __ldg(mp + 1);
-          }
-          if (C::AUX_TMA) {
-            // the slice after this one starts streaming in now (its buffer was last read two slices ago, and every
-            // thread of the set has passed that slice's staging barriers since)
-            if (store_thread) aux_prefetch(gslice + 1);
-            mbar_wait(&auxfull[set * 2 + (gslice & 1)], (gslice >> 1) & 1);
-            auxrow = auxs + (set * 2 + (gslice & 1)) * STG_BYTES + row * 128;
-          }
-          // both 32-column halves of the slice are requested up front: the second load is in flight while the first half
-          // goes through the fused math (the epilogue warps - two per scheduler partition - were stalled on this wait)
-#ifndef MMFB_EPI_PREFETCH
-#define MMFB_EPI_PREFETCH 1
-#endif
-          uint32_t rr[2][32];
-          tmem_ld32(t_row + sl * 64, rr[0]);
-          tmem_ld_wait();
-          if (MMFB_EPI_PREFETCH) tmem_ld32(t_row + sl * 64 + 32, rr[1]);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint32_t (&r)[32] = rr[h];
-            if (h == 1) {
-              if (!MMFB_EPI_PREFETCH) tmem_ld32(t_row + sl * 64 + 32, rr[1]);
-              tmem_ld_wait();
-            }
-            if (sl + 2 >= NSL && h == 1) {
-              // this thread has drained its share of the accumulator: hand the TMEM stage back to the MMA warp
-              tc_fence_before();
-              if (MC && crank != 0) mbar_arrive_remote(&tempty[as], 0); else mbar_arrive(&tempty[as]);
-            }
-            const int n = n0 + sl * 64 + h * 32;
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-            if (EPI == EPI_BIAS || EPI == EPI_BIAS_GELU || is_drop_resid(EPI) || EPI == EPI_BIAS_RELU) {
-              if (p.bias != nullptr && n < p.N) {
-                const uint4* bp = reinterpret_cast<const uint4*>(p.bias + n);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  if (n + q * 8 < p.N) {
-                    uint4 b = __ldg(bp + q);
-                    float2 f;
-                    f = unpack_bf16x2(b.x); v[q * 8 + 0] += f.x; v[q * 8 + 1] += f.y;
-                    f = unpack_bf16x2(b.y); v[q * 8 + 2] += f.x; v[q * 8 + 3] += f.y;
-                    f = unpack_bf16x2(b.z); v[q * 8 + 4] += f.x; v[q * 8 + 5] += f.y;
-                    f = unpack_bf16x2(b.w); v[q * 8 + 6] += f.x; v[q * 8 + 7] += f.y;
-                  }
-                }
-              }
-            }
-            if (EPI == EPI_BIAS_RELU) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.0f);
-            }
-            if (is_drop_resid(EPI)) {
-              if (p.dmask != nullptr && row_ok && n < p.N) {
-                const uint32_t bits = mbits[h];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = ((bits >> j) & 1u) ? v[j] * p.dscale : 0.0f;
-              }
-            }
-            if (is_drop_resid(EPI) || EPI == EPI_GELU_BWD || EPI == EPI_ADD_AUX) {
-              if (C::AUX_TMA || (p.aux != nullptr && row_ok && n < p.N)) {
-                uint4 a4[4];
-                if (C::AUX_TMA) {
-                  // swizzled smem slice written by TMA (out-of-range rows / columns arrive as zeros)
-#pragma unroll
-                  for (int q = 0; q < 4; ++q)
-                    a4[q] = *reinterpret_cast<const uint4*>(auxrow + (((h * 4 + q) ^ (row & 7)) * 16));
-                } else {
-                  const uint4* ap = reinterpret_cast<const uint4*>(p.aux + static_cast<int64_t>(m) * p.ldaux + n);
-#pragma unroll
-                  for (int q = 0; q < 4; ++q) a4[q] = (n + q * 8 < p.N) ? __ldg(ap + q) : make_uint4(0, 0, 0, 0);
-                }
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  float x[8];
-                  float2 f;
-                  f = unpack_bf16x2(a4[q].x); x[0] = f.x; x[1] = f.y;
-                  f = unpack_bf16x2(a4[q].y); x[2] = f.x; x[3] = f.y;
-                  f = unpack_bf16x2(a4[q].z); x[4] = f.x; x[5] = f.y;
-                  f = unpack_bf16x2(a4[q].w); x[6] = f.x; x[7] = f.y;
-#if MMFB_F32X2
-                  if (EPI == EPI_GELU_BWD) {
-#pragma unroll
-                    for (int e = 0; e < 8; e += 2) gelu_erf_grad_mul2(x[e], x[e + 1], v[q * 8 + e], v[q * 8 + e + 1]);
-                  } else {
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) v[q * 8 + e] += x[e];
-                  }
-#else
-#pragma unroll
-                  for (int e = 0; e < 8; ++e) {
-                    if (EPI == EPI_GELU_BWD) v[q * 8 + e] *= gelu_erf_grad(x[e]);
-                    else v[q * 8 + e] += x[e];
-                  }
-#endif
-                }
-              }
-            }
-#pragma unroll
-            for (int j = 0; j < 16; ++j) pk[h * 16 + j] = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-            if (EPI == EPI_BIAS_GELU) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-#if MMFB_F32X2
-                float g0, g1;
-                gelu_erf2(v[2 * j], v[2 * j + 1], g0, g1);
-                hk[h * 16 + j] = pack_bf16x2(g0, g1);
-#else
-                hk[h * 16 + j] = pack_bf16x2(gelu_erf(v[2 * j]), gelu_erf(v[2 * j + 1]));
-#endif
-              }
-            }
-          }
-          // 2) stage + TMA store (C, then C2 for the GELU epilogue through the same buffer)
-#pragma unroll
-          for (int o = 0; o < (EPI == EPI_BIAS_GELU ? 2 : 1); ++o) {
-            if (store_thread) tma_store_wait_read<0>();   // the buffer's previous TMA store has finished reading it
-            named_bar_sync(bar_id, 128);
-            uint8_t* rowp = stg_set + row * 128;
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const int chunk = q ^ (row & 7);
-              uint4 w4;
-              if (o == 0) w4 = make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]);
-              else w4 = make_uint4(hk[(q * 4) % (EPI == EPI_BIAS_GELU ? 32 : 1)], hk[(q * 4 + 1) % (EPI == EPI_BIAS_GELU ? 32 : 1)],
-                                   hk[(q * 4 + 2) % (EPI == EPI_BIAS_GELU ? 32 : 1)], hk[(q * 4 + 3) % (EPI == EPI_BIAS_GELU ? 32 : 1)]);
-              *reinterpret_cast<uint4*>(rowp + chunk * 16) = w4;
-            }
-            fence_proxy_async();
-            named_bar_sync(bar_id, 128);
-            if (store_thread) {
-              const int nn = n0 + sl * 64;
-              if (nn < p.N) tma_store_2d(o == 0 ? &tmC : &tmC2, stg_set, nn, m0);
-              tma_store_commit();
-            }
-          }
-          ++gslice;
-        }
-      }
-      if (++as == 2) { as = 0; aph ^= 1; }
-    }
-    if (store_thread) tma_store_wait_read<0>();
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (MC) cluster_sync_all();   // the peer may still multicast-commit onto this CTA's barriers until it is done too
-  if (warp == 1) {
-    tc_fence_after();
-    if (MC) tmem_dealloc_2sm(tmem_base, C::TMEM_COLS); else tmem_dealloc(tmem_base, C::TMEM_COLS);
+  // ------------------------------ consumers ------------------------------
+  const int half = wg - 1;                       // rows [64 half, 64 half + 64) of the tile
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+  {
+    int s = 0, prev = -1;
+    uint32_t ph = 0;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full[s], ph);
+      const uint32_t sa = smem_u32(smem + s * C::STAGE_BYTES) + half * 8192;   // K-major: 64 rows x 128 B; MN-major: panel
+      const uint32_t sb = smem_u32(smem + s * C::STAGE_BYTES) + C::A_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BK / 16; ++kk) {
+        const uint64_t da = A_MN ? gmma_desc_sw128(sa + kk * 2048, 8192, 1024) : gmma_desc_sw128(sa + kk * 32, 16, 1024);
+        const uint64_t db = B_MN ? gmma_desc_sw128(sb + kk * 2048, 8192, 1024) : gmma_desc_sw128(sb + kk * 32, 16, 1024);
+        wgmma_tile<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (kb > kb0 || kk > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                   // the previous k-block's wgmmas have retired: its slot may be refilled
+      if (prev >= 0) mbar_arrive(&empty[prev]);
+      prev = s;
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+    }
+    wgmma_wait<0>();
+  }
+
+  // ------------------------------ epilogue (registers -> global) ------------------------------
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int rh = 0; rh < 2; ++rh) {
+    const int m = m0 + half * 64 + warp * 16 + (lane >> 2) + rh * 8;
+    if (m >= p.M) continue;
+    const uint32_t* mrow = (EPI == EPI_BIAS_DROP_RESID && p.dmask != nullptr) ? p.dmask + static_cast<int64_t>(m) * p.ldmask
+                                                                               : nullptr;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int n = n0 + j * 8 + (lane & 3) * 2;
+      if (n >= p.N) continue;                    // N % 8 == 0: n < N implies n + 1 < N
+      float v0 = acc[j * 4 + rh * 2], v1 = acc[j * 4 + rh * 2 + 1];
+      if (EPI == EPI_ATOMIC_F32) {
+        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p.c32 + static_cast<int64_t>(m) * p.ldc + n), "f"(v0),
+                     "f"(v1)
+                     : "memory");
+        continue;
+      }
+      if (EPI == EPI_BIAS || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_DROP_RESID || EPI == EPI_BIAS_RELU) {
+        if (p.bias != nullptr) {
+          const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
+          v0 += b.x;
+          v1 += b.y;
+        }
+      }
+      if (EPI == EPI_BIAS_RELU) {
+        v0 = fmaxf(v0, 0.0f);
+        v1 = fmaxf(v1, 0.0f);
+      }
+      if (EPI == EPI_BIAS_DROP_RESID && mrow != nullptr) {
+        const uint32_t bits = __ldg(mrow + (n >> 5)) >> (n & 31);
+        v0 = (bits & 1u) ? v0 * p.dscale : 0.0f;
+        v1 = (bits & 2u) ? v1 * p.dscale : 0.0f;
+      }
+      if ((EPI == EPI_BIAS_DROP_RESID || EPI == EPI_GELU_BWD || EPI == EPI_ADD_AUX) && p.aux != nullptr) {
+        const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.aux + static_cast<int64_t>(m) * p.ldaux + n)));
+        if (EPI == EPI_GELU_BWD) {
+          v0 *= gelu_erf_grad(x.x);
+          v1 *= gelu_erf_grad(x.y);
+        } else {
+          v0 += x.x;
+          v1 += x.y;
+        }
+      }
+      const int64_t off = static_cast<int64_t>(m) * p.ldc + n;
+      *reinterpret_cast<uint32_t*>(p.c + off) = pack_bf16x2(v0, v1);
+      if (EPI == EPI_BIAS_GELU) *reinterpret_cast<uint32_t*>(p.c2 + off) = pack_bf16x2(gelu_erf(v0), gelu_erf(v1));
+    }
   }
 }
 
 // ----------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------
-template <int BN, bool A_MN, bool B_MN, int EPI, bool MC>
+template <int BN, bool A_MN, bool B_MN, int EPI>
 static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
-  using C = Cfg<BN, MC, EPI>;
-  CUtensorMap tmA, tmB, tmC, tmC2, tmAux;
+  using C = Cfg<BN>;
+  CUtensorMap tmA, tmB;
   // operand maps: K-major -> tensor [rows, K] (inner = K), box {64, rows_per_tile}
   //               MN-major -> tensor [K, rows] (inner = rows), box {64, 64}
   int rc;
   if (!A_MN) rc = make_tmap_2d(&tmA, a.A, a.K, a.M, a.lda, 64, BM);
   else rc = make_tmap_2d(&tmA, a.A, a.M, a.K, a.lda, 64, 64);
   if (rc) return rc;
-  if (!B_MN) rc = make_tmap_2d(&tmB, a.B, a.K, a.N, a.ldb, 64, MC ? BN / 2 : BN);   // MC: each CTA loads half the rows
+  if (!B_MN) rc = make_tmap_2d(&tmB, a.B, a.K, a.N, a.ldb, 64, BN);
   else rc = make_tmap_2d(&tmB, a.B, a.N, a.K, a.ldb, 64, 64);
   if (rc) return rc;
-  if (EPI != EPI_ATOMIC_F32) {
-    rc = make_tmap_2d(&tmC, a.C, a.N, a.M, a.ldc, 64, BM);
-    if (rc) return rc;
-    if (EPI == EPI_BIAS_GELU) {
-      rc = make_tmap_2d(&tmC2, a.C2, a.N, a.M, a.ldc, 64, BM);
-      if (rc) return rc;
-    } else {
-      tmC2 = tmC;
-    }
-  } else {
-    tmC = tmA;
-    tmC2 = tmA;
-  }
-  tmAux = tmA;
-  if (C::AUX_TMA) {
-    if (a.aux == nullptr) return set_error(MMFB_ERR_ARG, "gemm: this epilogue needs the aux operand");
-    rc = make_tmap_2d(&tmAux, a.aux, a.N, a.M, a.ldaux, 64, BM);
-    if (rc) return rc;
-  }
+  if (EPI == EPI_BIAS_GELU && a.C2 == nullptr) return set_error(MMFB_ERR_ARG, "gemm: this epilogue needs the C2 output");
+  if (((reinterpret_cast<uintptr_t>(a.C) | reinterpret_cast<uintptr_t>(a.C2) | reinterpret_cast<uintptr_t>(a.bias) |
+        reinterpret_cast<uintptr_t>(a.aux)) & 3) ||
+      (a.aux != nullptr && (a.ldaux % 2)))
+    return set_error(MMFB_ERR_ARG, "gemm: C / C2 / bias / aux must be 4-byte aligned");
   GemmDev p;
   p.M = a.M; p.N = a.N; p.K = a.K;
   p.splits = (EPI == EPI_ATOMIC_F32 && a.splits > 0) ? a.splits : 1;
@@ -511,8 +231,10 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
   if (p.splits > kb_total) p.splits = kb_total;
   // every split must own at least one k-block
   while (p.splits > 1 && ((kb_total + p.splits - 1) / p.splits) * (p.splits - 1) >= kb_total) --p.splits;
+  p.c = reinterpret_cast<bf16*>(a.C);
+  p.c2 = reinterpret_cast<bf16*>(a.C2);
   p.c32 = reinterpret_cast<float*>(a.C);
-  p.ldc32 = a.ldc;
+  p.ldc = a.ldc;
   p.bias = reinterpret_cast<const bf16*>(a.bias);
   p.aux = reinterpret_cast<const bf16*>(a.aux);
   p.ldaux = a.ldaux;
@@ -520,61 +242,39 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
   p.ldmask = a.ldmask;
   p.dscale = a.drop_scale;
 
-  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, MC>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "cudaFuncSetAttribute(gemm): %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  const int tiles_m = (a.M + BM - 1) / BM;
-  cudaError_t e;
-  if (MC) {
-    const int pairs = ((tiles_m + 1) / 2) * ((a.N + BN - 1) / BN) * p.splits;
-    const int max_clusters = num_sms() / 2;
-    const int clusters = pairs < max_clusters ? pairs : max_clusters;
-    e = launch_k(kern, dim3(2 * clusters), dim3(NUM_THREADS), static_cast<size_t>(C::SMEM_BYTES), stream, 2, tmA, tmB, tmC, tmC2,
-                 tmAux, p);
-  } else {
-    const int tiles = tiles_m * ((a.N + BN - 1) / BN) * p.splits;
-    const int grid = tiles < num_sms() ? tiles : num_sms();
-    MMFB_LAUNCH(kern, grid, NUM_THREADS, C::SMEM_BYTES, stream, tmA, tmB, tmC, tmC2, tmAux, p);
-    e = cudaGetLastError();
-  }
+  const int tiles = ((a.M + BM - 1) / BM) * ((a.N + BN - 1) / BN) * p.splits;
+  MMFB_LAUNCH(kern, tiles, NUM_THREADS, C::SMEM_BYTES, stream, tmA, tmB, p);
+  cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "gemm launch: %s", cudaGetErrorString(e));
   count_launch();
   return MMFB_OK;
 }
 
-template <int BN, bool MC>
+template <int BN>
 static int dispatch(const mmfb_gemm_args& a, cudaStream_t s) {
   const int key = (a.a_mn ? 100 : 0) + (a.b_mn ? 10 : 0) + a.epi;
   switch (key) {
-    case 0 + EPI_BIAS: return launch<BN, false, false, EPI_BIAS, MC>(a, s);
-    case 0 + EPI_BIAS_GELU: return launch<BN, false, false, EPI_BIAS_GELU, MC>(a, s);
-    case 0 + EPI_BIAS_DROP_RESID:
-      if (MC && a.K <= 1024 && a.aux != nullptr) return launch<BN, false, false, EPI_BIAS_DROP_RESID_T, MC>(a, s);
-      return launch<BN, false, false, EPI_BIAS_DROP_RESID, MC>(a, s);
-    case 0 + EPI_BIAS_RELU: return launch<BN, false, false, EPI_BIAS_RELU, MC>(a, s);
-    case 10 + EPI_BIAS: return launch<BN, false, true, EPI_BIAS, MC>(a, s);
-    case 10 + EPI_GELU_BWD: return launch<BN, false, true, EPI_GELU_BWD, MC>(a, s);
-    case 10 + EPI_ADD_AUX: return launch<BN, false, true, EPI_ADD_AUX, MC>(a, s);
-    case 110 + EPI_ATOMIC_F32: return launch<BN, true, true, EPI_ATOMIC_F32, MC>(a, s);
+    case 0 + EPI_BIAS: return launch<BN, false, false, EPI_BIAS>(a, s);
+    case 0 + EPI_BIAS_GELU: return launch<BN, false, false, EPI_BIAS_GELU>(a, s);
+    case 0 + EPI_BIAS_DROP_RESID: return launch<BN, false, false, EPI_BIAS_DROP_RESID>(a, s);
+    case 0 + EPI_BIAS_RELU: return launch<BN, false, false, EPI_BIAS_RELU>(a, s);
+    case 10 + EPI_BIAS: return launch<BN, false, true, EPI_BIAS>(a, s);
+    case 10 + EPI_GELU_BWD: return launch<BN, false, true, EPI_GELU_BWD>(a, s);
+    case 10 + EPI_ADD_AUX: return launch<BN, false, true, EPI_ADD_AUX>(a, s);
+    case 110 + EPI_ATOMIC_F32: return launch<BN, true, true, EPI_ATOMIC_F32>(a, s);
     // test-only layout combinations (kept small: plain store epilogue)
-    case 100 + EPI_BIAS: return launch<BN, true, false, EPI_BIAS, MC>(a, s);
-    case 110 + EPI_BIAS: return launch<BN, true, true, EPI_BIAS, MC>(a, s);
+    case 100 + EPI_BIAS: return launch<BN, true, false, EPI_BIAS>(a, s);
+    case 110 + EPI_BIAS: return launch<BN, true, true, EPI_BIAS>(a, s);
     default:
       return set_error(MMFB_ERR_ARG, "gemm: unsupported (a_mn=%d, b_mn=%d, epi=%d)", a.a_mn, a.b_mn, a.epi);
   }
-}
-
-static bool cluster_default() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MMFB_GEMM_CLUSTER");   // default: CTA pairs (2-SM MMA); MMFB_GEMM_CLUSTER=0 forces single-CTA
-    v = (e == nullptr) ? 1 : (e[0] != '0');
-  }
-  return v != 0;
 }
 
 int gemm(const mmfb_gemm_args& a, cudaStream_t stream) {
@@ -588,11 +288,8 @@ int gemm(const mmfb_gemm_args& a, cudaStream_t stream) {
   if ((a.lda % 8) || (a.ldb % 8) || (a.epi != EPI_ATOMIC_F32 && (a.ldc % 8)))
     return set_error(MMFB_ERR_ARG, "gemm: leading dimensions must be multiples of 8 elements");
   const int bn = a.block_n > 0 ? a.block_n : (a.N >= 256 ? 256 : 128);
-  // cluster: 0 = library default (env MMFB_GEMM_CLUSTER), 1 = single-CTA MMA, 2 = CTA pair with the 2-SM MMA
-  bool mc = a.cluster == 2 || (a.cluster == 0 && cluster_default());
-  if ((a.M + BM - 1) / BM < 2 || num_sms() < 2) mc = false;
-  if (bn == 256) return mc ? dispatch<256, true>(a, stream) : dispatch<256, false>(a, stream);
-  if (bn == 128) return mc ? dispatch<128, true>(a, stream) : dispatch<128, false>(a, stream);
+  if (bn == 256) return dispatch<256>(a, stream);
+  if (bn == 128) return dispatch<128>(a, stream);
   return set_error(MMFB_ERR_ARG, "gemm: block_n must be 128 or 256");
 }
 

@@ -363,13 +363,12 @@ ln_bwd_lean_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __rest
   }
 }
 
-// Single-pass LayerNorm backward, streaming variant (MMFB_LN_BWD=stream).  ncu of the kernel above (round 2, call 6): issue
-// slots 39 % used, 49 % of the stall samples on the global loads of the row a warp is about to process - a warp loads,
-// computes, stores, and only the other 15 warps of the SM cover its load latency.  Here every warp owns a private ring of
+// Single-pass LayerNorm backward, streaming variant (MMFB_LN_BWD=stream).  In the kernel above a warp loads, computes and
+// stores a row, and only the other warps of the SM cover its load latency.  Here every warp owns a private ring of
 // ST row slots in shared memory that its lane 0 fills with bulk async copies (cp.async.bulk, one per tensor row,
 // completion on a per-slot mbarrier) ST rows ahead, so ST x 16 warps x 3 KB are in flight per SM whatever the warps are
-// doing, the row lives in shared memory across the two phases (no row registers), and the arithmetic is the packed-fp32
-// form of the lean kernel.  Rows are read from HBM once; dy / dz are stored straight from registers.
+// doing, the row lives in shared memory across the two phases (no row registers), and the arithmetic is the fp32-pair
+// form of the lean kernel (common.cuh: pk2 / fma2).  Rows are read from HBM once; dy / dz are stored straight from registers.
 __device__ __forceinline__ void bulk_load_1d(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(dst_smem)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
@@ -1130,9 +1129,7 @@ int ln_bwd(const mmfb_ln_args& a, cudaStream_t s) {
   if (a.drop_mask && !a.dz) return set_error(MMFB_ERR_ARG, "layernorm_bwd: dropout mask given without dz");
   const int nv_ = (a.H + 255) / 256;
   // read per call (not cached) so that one test process can run the variants back to back.
-  // default: the streaming single-pass kernel (58 us at [37848, 768] against 66 us for "lean", 80 us for "tile" and 100 us
-  // for the rows + cols "pair", profiles/r2_kbench_persistent_attn_stream_ln.json); MMFB_LN_BWD=lean / tile / pair select
-  // the others for A/B runs
+  // default: the streaming single-pass kernel; MMFB_LN_BWD=lean / tile / pair select the others for A/B runs
   const char* lean_env = getenv("MMFB_LN_BWD");
   const bool lean = lean_env != nullptr && lean_env[0] == 'l';
   const bool tile = lean_env != nullptr && lean_env[0] == 't';
@@ -1204,9 +1201,7 @@ int ln_bwd(const mmfb_ln_args& a, cudaStream_t s) {
     return launch_ok("layernorm_bwd(lean)");
   }
   if (nv_ <= 4) {
-    // two kernels: a light row kernel (dy, dz) at high occupancy, then coalesced column statistics.  (Measured
-    // alternatives: one fused kernel with register accumulators - 188 registers, one block per SM, 51 us; one fused
-    // kernel with red.shared column partials - 72 shared reductions per lane per row, slower end to end.  The pair: 23 + 22 us.)
+    // two kernels: a light row kernel (dy, dz) at high occupancy, then coalesced column statistics
     const bool need_dz_buf = (a.drop_mask != nullptr) || (a.dz != nullptr && a.dz != a.dy);
     const int rgrid = (a.M + ROW_WARPS - 1) / ROW_WARPS;
 #define LN_ROWS(NV)                                                                                              \

@@ -3,7 +3,7 @@
   B200VisioLinguisticEmbeddings  <->  BertVisioLinguisticEmbeddings   mmf/modules/embeddings.py:309-459
   B200ImageFeatureEmbeddings     <->  BertImageFeatureEmbeddings      mmf/models/vilbert.py:891-913
 
-Data flow (all on device): region features -> tcgen05 projection GEMM (bias epilogue) -> one row-composer
+Data flow (all on device): region features -> wgmma projection GEMM (bias epilogue) -> one row-composer
 kernel that gathers word / position / type rows (or the projected region row + visual type / position rows),
 sums them in fp32 and writes the pre-LN row -> LayerNorm (+dropout) kernel.  All embedding tables of a module
 are adjacent in its flat parameter pack and are addressed as ONE table with row offsets, so the composer and

@@ -31,7 +31,7 @@ def _idx_len(idx, M, name):
 
 def gemm(a, b, *, a_mn=False, b_mn=False, epi=lib.EPI_BIAS, bias=None, aux=None, drop_mask=None,
          drop_scale=1.0, out=None, out2=None, splits=1, block_n=0, cluster=0):
-    """C[M,N] = epi(A[M,K] @ B[N,K]^T) on the tcgen05 GEMM.
+    """C[M,N] = epi(A[M,K] @ B[N,K]^T) on the wgmma GEMM.
 
     a: [M,K] (a_mn=False) or [K,M] (a_mn=True); b: [N,K] (b_mn=False) or [K,N] (b_mn=True); bf16.
     Returns C (and C2 for EPI_BIAS_GELU).  For EPI_ATOMIC_F32 `out` (fp32 [M,N]) is accumulated into.

@@ -12,7 +12,7 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
     `.grad` are views of them afterwards - an optimizer sees fresh gradients after every replay;
   * inputs: static device tensors, refreshed by `copy_` on the replay stream (shapes are fixed at capture).
 The reference has no counterpart (its trainer launches eagerly, mmf/trainers/core/training_loop.py:185-213); this is the
-B200 answer to SURVEY.md 8a's "at T = R = 36 everything is launch-bound"."""
+answer to SURVEY.md 8a's "at T = R = 36 everything is launch-bound"."""
 import torch
 
 from . import functional as F

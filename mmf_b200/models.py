@@ -320,7 +320,7 @@ def build_model(config):
 # heads shared by the three models
 # ------------------------------------------------------------------------------------------------------
 class B200Linear(nn.Linear):
-    """nn.Linear parameters (`weight`, `bias`), forward on the tcgen05 GEMM (any feature counts, ops.linear_any)"""
+    """nn.Linear parameters (`weight`, `bias`), forward on the wgmma GEMM (any feature counts, ops.linear_any)"""
 
     def forward(self, x):
         shape = x.shape

@@ -24,9 +24,9 @@ from . import lib
 def _require_cuda(t, what):
     if not t.is_cuda:
         raise RuntimeError(
-            "%s is on %s: the B200 fusion path has no CPU fallback (move the model and inputs to a B200)" % (what, t.device))
+            "%s is on %s: the fusion path has no CPU fallback (move the model and inputs to an H100)" % (what, t.device))
     if not lib.device_ok():
-        raise RuntimeError("libmmfb200 needs an sm_100 (B200) device: " + lib.last_error())
+        raise RuntimeError("libmmfb200 needs an sm_90 (H100) device: " + lib.last_error())
 
 
 def _check_erf_gelu(layer):
@@ -52,8 +52,7 @@ _SEED_COUNTER = [0]
 
 def _fresh_dropout_state(prefetchable=False):
     """One Philox stream per forward, derived from torch's seed so `torch.manual_seed` makes runs repeatable.
-    (A side-stream generator that drew the next layer's bits ahead was measured in round 2 and dropped: +0.2 %, i.e. noise -
-    the persistent GEMMs leave no SM resources for a concurrent kernel; profiles/r2_ab_sweep_first.txt.)"""
+    (The bits are drawn on the compute stream: the GEMMs a side-stream generator would overlap occupy every SM.)"""
     _SEED_COUNTER[0] += 1
     seed = torch.initial_seed() * 1000003 + _SEED_COUNTER[0]
     return E.DropoutState(seed)

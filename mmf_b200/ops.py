@@ -17,7 +17,7 @@ def _bf16(t):
 
 
 class _Linear(torch.autograd.Function):
-    """y = x W^T + b on the tcgen05 GEMM; backward: dgrad (MN-major W), split-K wgrad, column-sum bias gradient."""
+    """y = x W^T + b on the wgmma GEMM; backward: dgrad (MN-major W), split-K wgrad, column-sum bias gradient."""
 
     @staticmethod
     def forward(ctx, x, weight, bias):

@@ -15,7 +15,7 @@ from .modules import B200BertEncoder, B200BertLayer, EncoderRunner, _init_bert_w
 
 
 class BertPooler(nn.Module):
-    """HF BertPooler: tanh(dense(h[:, 0])) (visual_bert.py:146): the [B, H] x [H, H]^T product on the tcgen05 GEMM, tanh as
+    """HF BertPooler: tanh(dense(h[:, 0])) (visual_bert.py:146): the [B, H] x [H, H]^T product on the wgmma GEMM, tanh as
     a torch elementwise op on the [B, H] result."""
 
     def __init__(self, hidden):

@@ -1,9 +1,9 @@
 """TEST / BASELINE INFRASTRUCTURE - recipe that stages the reference's OWN hot-path source files under oracle/_ref/.
 
-    python -m oracle.build_ref            (run by __graft_entry__.build() wherever /root/reference exists)
+    python -m oracle.build_ref            (run by __graft_entry__.build() wherever the reference tree exists)
 
-oracle/_ref/ is git-ignored (reference sources never enter this repository's history) but it travels to the GPU box with
-the gpurun snapshot, where /root/reference does not exist.  There `bench.py --impl reference` / `cpu_baseline` execute
+oracle/_ref/ is git-ignored (reference sources never enter this repository's history); a tree built where the reference
+exists keeps it, so it also serves where the reference tree is absent.  There `bench.py --impl reference` / `cpu_baseline` execute
 these files, UNMODIFIED, through oracle/ref_loader.py (MMF_REFERENCE_ROOT=oracle/_ref) - the reference's own
 `VisualBERTBase` (BertVisioLinguisticEmbeddings + BertEncoderJit), i.e. `cpu_baseline.kind = "reference"`.
 Nothing in the product (mmf_b200/) imports from here.

@@ -1,9 +1,9 @@
 """TEST INFRASTRUCTURE - generates tests/golden/*.pt by running the REFERENCE's own source files.
 
-Runs only in the build container (needs /root/reference):   python -m oracle.make_golden
+Needs the reference tree (MMF_REFERENCE_ROOT, see oracle/ref_loader.py):   python -m oracle.make_golden
 Each fixture holds seeded weights (reference state_dict key names), inputs, the reference's outputs
 and the gradients of a fixed random-projection loss  (out * W_rand).sum()  (SURVEY.md 8d: out.sum()
-is degenerate after a final LayerNorm).  Shapes are tiny so the fixtures are a few hundred KB.
+is degenerate after a final LayerNorm).  Shapes are tiny and _save keeps every fixture under 1 MB.
 All modules run in eval mode (dropout off): the reference's RNG stream is not reproducible elsewhere.
 """
 import os
@@ -14,22 +14,30 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from oracle import golden_format as GF  # noqa: E402
 from oracle import ref_loader as R  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 
 
+def _q8(x, base):
+    """x rounded to base + k / 1024 with |k| <= 127: exactly what oracle/golden_format.Q8 stores as one int8 per element, so
+    the weights of a fixture are stored exactly in a quarter of the fp32 bytes"""
+    return torch.round((x - base) * 1024.0).clamp(-127, 127) / 1024.0 + base
+
+
 def _perturb(module, seed):
-    """reference init (normal 0.02, zero bias, LN 1/0) + small perturbation of biases / LN so they matter"""
+    """reference init (normal 0.02, zero bias, LN 1/0) + small perturbation of biases / LN so they matter; every value on
+    the int8 grid of _q8"""
     g = torch.Generator().manual_seed(seed)
     with torch.no_grad():
         for n, p in module.named_parameters():
             if p.dim() >= 2:
-                p.copy_(torch.randn(p.shape, generator=g) * 0.02)
+                p.copy_(_q8(torch.randn(p.shape, generator=g) * 0.02, 0.0))
             elif "LayerNorm.weight" in n or n.endswith("layer_norms.0.weight") or n.endswith(".1.weight"):
-                p.copy_(1.0 + torch.randn(p.shape, generator=g) * 0.02)
+                p.copy_(_q8(1.0 + torch.randn(p.shape, generator=g) * 0.02, 1.0))
             else:
-                p.copy_(torch.randn(p.shape, generator=g) * 0.02)
+                p.copy_(_q8(torch.randn(p.shape, generator=g) * 0.02, 0.0))
 
 
 def _grads(module, names):
@@ -37,11 +45,72 @@ def _grads(module, names):
     return {n: sd[n].grad.detach().clone() for n in names if sd[n].grad is not None}
 
 
+GRAD_SAMPLE = 256      # elements kept of a larger gradient (plus its first row), see _encode
+MAX_BYTES = 1 << 20    # no fixture file may exceed 1 MB
+
+
+def _encode(obj, key=None, name=""):
+    """Compact storage (oracle/golden_format.py; torch.load expands it): fp32 tensors on the _q8 grid as int8 (exact); each
+    gradient under a "grads" key with more than GRAD_SAMPLE elements as a fixed seeded sample of GRAD_SAMPLE elements plus
+    its first row (the tests compare relative L2 errors over the stored elements)."""
+    if isinstance(obj, dict):
+        return {k: _encode(v, k if key != "grads" else "grads", name + "/" + str(k)) for k, v in obj.items()}
+    if isinstance(obj, (list, tuple)):
+        return type(obj)(_encode(v, None, name + "/%d" % i) for i, v in enumerate(obj))
+    if not torch.is_tensor(obj) or obj.dtype != torch.float32:
+        return obj
+    t = obj.detach().contiguous()
+    if key == "grads" and t.numel() > GRAD_SAMPLE:
+        import zlib
+        g = torch.Generator().manual_seed(zlib.crc32(name.encode()))
+        first = t.shape[-1] if t.dim() >= 2 else 0
+        idx = torch.unique(torch.cat([torch.arange(first), torch.randperm(t.numel(), generator=g)[:GRAD_SAMPLE]]))
+        return GF.Sampled(tuple(t.shape), idx.to(torch.int32), t.reshape(-1)[idx])
+    for base in (0.0, 1.0):
+        k = torch.round((t - base) * 1024.0)
+        if k.abs().max() <= 127 and torch.equal(k.clamp(-127, 127) / 1024.0 + base, t):
+            return GF.Q8(k.to(torch.int8), base)
+    return t
+
+
+def _perturb_values(sd, seed):
+    """the values the pre-int8 _perturb drew for the float entries of `sd`, in key order (the decoder of the "replay"
+    format in oracle/golden_format.py draws the same way)"""
+    g = torch.Generator().manual_seed(seed)
+    out = {}
+    for n, p in sd.items():
+        if not p.dtype.is_floating_point:
+            continue
+        lnw = "LayerNorm.weight" in n or n.endswith("layer_norms.0.weight") or n.endswith(".1.weight")
+        out[n] = (1.0 if (p.dim() < 2 and lnw) else 0.0) + torch.randn(p.shape, generator=g) * 0.02
+    return out
+
+
+def compact_legacy(name, seeds):
+    """Rewrites fixture `name` (plain torch.save of fp32 tensors, from before the int8 weights) in the compact format:
+    each state_dict by its _perturb seed (entries the replay does not reproduce bit for bit are kept as they are),
+    gradients sampled like _encode.  For fixtures whose reference code no longer runs with the installed libraries
+    (lxmert: seed 91; models: seeds by entry)."""
+    path = os.path.join(OUT, name + ".pt")
+    obj = torch.load(path, weights_only=False)
+    entries = obj if name == "models" else {None: obj}
+    for key, fx in entries.items():
+        if isinstance(fx, dict) and "state_dict" in fx:
+            sd = fx["state_dict"]
+            vals = _perturb_values(sd, seeds[key])
+            fx["state_dict"] = GF.Replay(seeds[key], [(k, tuple(v.shape), v.dtype) for k, v in sd.items()],
+                                         {k: v for k, v in sd.items() if k not in vals or not torch.equal(vals[k], v)})
+    _save(name, obj)
+
+
 def _save(name, obj):
     os.makedirs(OUT, exist_ok=True)
     path = os.path.join(OUT, name + ".pt")
-    torch.save(obj, path)
-    print("wrote %s (%.1f KB)" % (path, os.path.getsize(path) / 1024))
+    torch.save(_encode(obj), path)
+    size = os.path.getsize(path)
+    print("wrote %s (%.1f KB)" % (path, size / 1024))
+    if size > MAX_BYTES:
+        raise RuntimeError("%s is %d bytes: fixtures must stay under 1 MB" % (path, size))
 
 
 def golden_bert_encoder():
@@ -702,6 +771,38 @@ def golden_models():
     _save("models", out)
 
 
+def golden_model_config_defaults():
+    """model_config.<name> of the reference's configs/models/<name>/defaults.yaml (read and resolved with the product's
+    own YAML loader), and the keys tests check of three configs that include them -> tests/golden/model_config_defaults.json"""
+    import json
+
+    import mmf_b200.mmft  # noqa: F401  (registers the mmf_transformer defaults)
+    import mmf_b200.models as MD
+    mmf_root = os.path.join(R.REF_ROOT, "mmf")
+    out = {"defaults": {}, "configs": {}}
+    for name in ("visual_bert", "vilbert", "mmbt", "mmf_transformer"):
+        doc = MD.read_yaml_with_includes(os.path.join(mmf_root, "configs/models/%s/defaults.yaml" % name), mmf_root)
+        out["defaults"][name] = MD._resolve_interpolations(doc["model_config"][name], doc)
+    c = MD.load_model_config("visual_bert", yaml_path="configs/models/visual_bert/classification.yaml", mmf_root=mmf_root)
+    out["configs"]["visual_bert/classification"] = {"training_head_type": c.training_head_type,
+                                                     "visual_embedding_dim": c.visual_embedding_dim}
+    c = MD.load_model_config("mmbt", yaml_path="configs/models/mmbt/classification.yaml", mmf_root=mmf_root)
+    out["configs"]["mmbt/classification"] = {"training_head_type": c.training_head_type, "loss0_type": c.losses[0]["type"]}
+    c = MD.load_model_config("mmbt", yaml_path="configs/models/mmbt/with_features.yaml", mmf_root=mmf_root)
+    out["configs"]["mmbt/with_features"] = {"direct_features_input": c.direct_features_input,
+                                            "modal_encoder_type": c.modal_encoder.type}
+
+    def plain(x):
+        if isinstance(x, dict):
+            return {k: plain(v) for k, v in x.items()}
+        if isinstance(x, (list, tuple)):
+            return [plain(v) for v in x]
+        return x
+    with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden",
+                           "model_config_defaults.json"), "w") as fh:
+        fh.write(json.dumps(plain(out), sort_keys=True, separators=(",", ":")) + "\n")
+
+
 def main():
     torch.manual_seed(0)
     torch.set_num_threads(4)
@@ -719,6 +820,7 @@ def main():
     golden_models()
     golden_vit()
     golden_vinvl()
+    golden_model_config_defaults()
 
 
 if __name__ == "__main__":

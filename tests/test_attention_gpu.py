@@ -1,4 +1,4 @@
-"""Fused tcgen05 attention (fwd + recompute bwd) vs the oracle's attention_core on the same bf16 inputs.
+"""Fused attention (fwd + recompute bwd) vs the oracle's attention_core on the same bf16 inputs.
 Tolerance: 1e-2 relative L2 (bf16 bar of BASELINE.md 5); the oracle runs in fp32 on the GPU."""
 import pytest
 import torch
@@ -91,17 +91,15 @@ def test_attention_dropout_explicit_mask(S, d):
 @pytest.mark.parametrize("B,heads,Sq,Skv,p_drop", [(40, 12, 228, 228, 0.1), (70, 8, 100, 256, 0.0), (64, 6, 256, 36, 0.1),
                                                    (13, 12, 128, 128, 0.0)])
 def test_attention_many_items_per_cta(B, heads, Sq, Skv, p_drop):
-    """d = 64, both sequences <= 256: the persistent kernels (one CTA per SM) walk several (batch, head) items each - ring
-    stages, statistics buffers, barrier phases and accumulator hand-over across items (1, 2 and 3+ items per CTA, one and
-    two 128-row blocks per side), with ragged key padding and one sample without any attendable key"""
+    """d = 64, many (batch, head) items of 64-row tiles: one to four blocks per side through the two-stage ring (odd and
+    even counts), with ragged key padding and one sample without any attendable key"""
     errs = _case(B, heads, Sq, Skv, 64, p_drop=p_drop, seed=11, full_mask_row=True)
     assert max(errs.values()) < 1e-2
 
 
 def test_attention_repeated_launches_are_identical_under_ragged_padding():
-    """Race / hang regression for the persistent kernels (work counter, ring stages, staged-output barriers): 25 forward +
-    backward launches over 1152 items with ragged key padding, the kind of input under which one softmax group gets a whole
-    item ahead of the other.  Every repetition must reproduce the first one bit for bit, and none may trap."""
+    """Race / hang regression for the staged rings (stage refills, barrier phases): 25 forward + backward launches over 1152
+    items with ragged key padding.  Every repetition must reproduce the first one bit for bit, and none may trap."""
     from mmf_b200 import functional as F
     g = torch.Generator(device="cuda").manual_seed(21)
     B, heads, S, d = 96, 12, 228, 64

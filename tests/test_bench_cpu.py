@@ -41,10 +41,3 @@ def test_reference_arm_and_multi_gpu_runs_are_eager(bench, monkeypatch):
     src = open(os.path.join(ROOT, "bench.py")).read()
     assert 'args.workload in ("visual_bert", "mmbt", "vilbert")' in src and 'not args.profile and args.impl == "b200"' in src
     assert isinstance(argparse.ArgumentParser(), argparse.ArgumentParser)
-
-
-def test_kept_traffic_is_reported_only_for_the_batch_it_was_captured_at(bench):
-    tr, src = bench.kept_traffic("visual_bert", 166)
-    assert tr is not None and tr > 4e8 and "ncu" in src            # profiles/dominant_traffic.json: 63 MB read + 406 MB written
-    assert bench.kept_traffic("visual_bert", 64) == (None, None)
-    assert bench.kept_traffic("no_such_workload", 166) == (None, None)

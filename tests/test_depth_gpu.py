@@ -6,7 +6,7 @@
   layers / 1024): end to end the product must be no worse than the REFERENCE ARITHMETIC ITSELF run in bf16 (the oracle with
   bf16 weights and activations on the same device): error(product vs fp32 oracle) <= 1.5 x error(bf16 oracle vs fp32 oracle),
   with an absolute ceiling of 2.5e-2 on the outputs.
-Every measured error is printed (pytest -rP keeps it; the GPU log of the round is copied to profiles/)."""
+Every measured error is printed (pytest -rP keeps it)."""
 import types
 
 import pytest

@@ -10,12 +10,14 @@ import pytest
 import torch
 
 from oracle import fusion_oracle as O
+from oracle.golden_format import kept  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
 
 def rel(a, b, floor=1e-3):
+    a, b = kept(a, b)        # a sampled golden gradient: compare the elements it stores
     fl = floor * (b.numel() ** 0.5)
     return ((a.double().cpu() - b.double().cpu()).norm() / b.double().norm().clamp_min(fl)).item()
 
@@ -141,7 +143,6 @@ def test_bert_encoder_vs_oracle_config_shapes(B, S, H, heads, I, L):
     o_out, o_dx, o_g = _oracle_run(sd, x.to(torch.bfloat16).float(), add, L, heads, w_rand)
     e_out, e_dx = rel(out, o_out), rel(xg.grad, o_dx)
     print("B%d S%d H%d L%d: out %.2e dx %.2e" % (B, S, H, L, e_out, e_dx))
-    # measured (profiles/r2_parity_errors.txt): L=1 out 3.4e-3 / dx 3.8e-3 / worst dW 5.3e-3; L=2 4.8e-3 / 5.2e-3 / 7.5e-3
     assert e_out < 1e-2 and e_dx < 1e-2
     worst, worst_n = check_param_grads(enc.named_parameters(), o_g, 1e-2 if L == 1 else 1.5e-2)
     print("   worst dW %.2e (%s)" % (worst, worst_n))

@@ -127,7 +127,7 @@ def test_bad_head_split_raises_like_reference():
 
 def test_best_splits_prefers_full_waves():
     from mmf_b200.engine import best_splits
-    assert best_splits(768, 768, 14592) >= 4      # 18 tiles -> needs split-K to fill 148 SMs
+    assert best_splits(768, 768, 14592) >= 4      # 18 tiles -> needs split-K to fill 132 SMs
     assert best_splits(3072, 768, 14592) >= 2
     assert best_splits(128, 256, 64) == 1         # a single k-block cannot be split
 

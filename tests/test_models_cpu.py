@@ -11,12 +11,13 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import fake_kernels as FK  # noqa: E402
+from oracle.golden_format import kept  # noqa: E402
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
-REF = "/root/reference/mmf"
 
 
 def rel(a, b):
+    a, b = kept(a, b)        # a sampled golden gradient: compare the elements it stores
     a, b = a.detach().double(), b.detach().double()
     return ((a - b).norm() / b.norm().clamp_min(1e-12)).item()
 
@@ -175,21 +176,39 @@ def test_mmbt_registered_model_classification_runs_and_matches_oracle(cpu_models
     assert rel(out["scores"], ref) < 3e-2
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present (GPU box)")
 def test_restated_defaults_equal_the_reference_yaml(cpu_models):
-    """MODEL_DEFAULTS is a restatement: pin it to the YAML files it cites, read with the module's own YAML loader"""
+    """MODEL_DEFAULTS is a restatement: pin it to the reference's YAML files it cites (model_config.<name> of
+    configs/models/<name>/defaults.yaml, read with the module's own YAML loader and stored in
+    tests/golden/model_config_defaults.json by oracle/make_golden.py::golden_model_config_defaults)"""
+    import json
     MD = cpu_models
     import mmf_b200.mmft  # noqa: F401  (adds the mmf_transformer defaults)
-    for name, rel_path in (("visual_bert", "configs/models/visual_bert/defaults.yaml"),
-                           ("vilbert", "configs/models/vilbert/defaults.yaml"), ("mmbt", "configs/models/mmbt/defaults.yaml"),
-                           ("mmf_transformer", "configs/models/mmf_transformer/defaults.yaml")):
-        doc = MD.read_yaml_with_includes(os.path.join(REF, rel_path), REF)
-        block = MD._resolve_interpolations(doc["model_config"][name], doc)
-        assert dict(MD.ConfigNode(MD.MODEL_DEFAULTS[name])) == dict(MD.ConfigNode(block)), name
-    # `includes:` + override order: classification.yaml = defaults + training_head_type
-    c = MD.load_model_config("visual_bert", yaml_path="configs/models/visual_bert/classification.yaml", mmf_root=REF)
-    assert c.training_head_type == "classification" and c.visual_embedding_dim == 2048
-    c = MD.load_model_config("mmbt", yaml_path="configs/models/mmbt/classification.yaml", mmf_root=REF)
-    assert c.training_head_type == "classification" and c.losses[0]["type"] == "cross_entropy"
-    c = MD.load_model_config("mmbt", yaml_path="configs/models/mmbt/with_features.yaml", mmf_root=REF)
-    assert c.direct_features_input is True and c.modal_encoder.type == "finetune_faster_rcnn_fpn_fc7"
+    with open(os.path.join(GOLD, "model_config_defaults.json")) as fh:
+        g = json.load(fh)
+    for name in ("visual_bert", "vilbert", "mmbt", "mmf_transformer"):
+        assert dict(MD.ConfigNode(MD.MODEL_DEFAULTS[name])) == dict(MD.ConfigNode(g["defaults"][name])), name
+    # what the reference's classification / with_features YAMLs resolve to (defaults + their own keys)
+    assert g["configs"]["visual_bert/classification"] == {"training_head_type": "classification", "visual_embedding_dim": 2048}
+    assert g["configs"]["mmbt/classification"] == {"training_head_type": "classification", "loss0_type": "cross_entropy"}
+    assert g["configs"]["mmbt/with_features"] == {"direct_features_input": True,
+                                                  "modal_encoder_type": "finetune_faster_rcnn_fpn_fc7"}
+
+
+def test_yaml_includes_and_override_order(cpu_models, tmp_path):
+    """`includes:` (relative to the mmf root or to the including file) merge first, the including file overrides them,
+    interpolations resolve against the merged document, and the registry name is stamped last"""
+    MD = cpu_models
+    d = tmp_path / "configs" / "models" / "visual_bert"
+    d.mkdir(parents=True)
+    (tmp_path / "configs" / "common.yaml").write_text("shared:\n  dim: 2048\n")
+    (d / "defaults.yaml").write_text("includes:\n- configs/common.yaml\nmodel_config:\n  visual_bert:\n"
+                                     "    training_head_type: pretraining\n    visual_embedding_dim: ${shared.dim}\n"
+                                     "    num_labels: 2\n")
+    (d / "classification.yaml").write_text("includes:\n- ./defaults.yaml\nmodel_config:\n  visual_bert:\n"
+                                           "    training_head_type: classification\n    model: bert\n")
+    c = MD.load_model_config("visual_bert", yaml_path="configs/models/visual_bert/classification.yaml", mmf_root=str(tmp_path))
+    assert c.training_head_type == "classification" and c.visual_embedding_dim == 2048 and c.num_labels == 2
+    assert c.model == "visual_bert"
+    c = MD.load_model_config("visual_bert", yaml_path="configs/models/visual_bert/classification.yaml", mmf_root=str(tmp_path),
+                             overrides={"num_labels": 3129})
+    assert c.num_labels == 3129

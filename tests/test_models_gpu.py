@@ -1,16 +1,18 @@
-"""Registered model plugins on the B200 (through the C ABI): `forward(SampleList) -> scores / losses` of visual_bert and
+"""Registered model plugins on the H100 (through the C ABI): `forward(SampleList) -> scores / losses` of visual_bert and
 vilbert against the outputs of the REFERENCE's own registered model classes (tests/golden/models.pt), integer tensors with
 torch.equal, gradients of the heads and of trunk weights against the reference's autograd."""
 import os
 
 import pytest
 import torch
+from oracle.golden_format import kept  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def rel(a, b):
+    a, b = kept(a, b)        # a sampled golden gradient: compare the elements it stores
     a, b = a.detach().double().cpu(), b.detach().double().cpu()
     return ((a - b).norm() / b.norm().clamp_min(1e-12)).item()
 

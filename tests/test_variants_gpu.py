@@ -1,4 +1,4 @@
-"""The kernels the product library does NOT run by default but keeps for A/B timing (MMFB_LN_BWD=pair|tile, MMFB_ATTN_BWD=8)
+"""The kernels the product library does NOT run by default but keeps for A/B timing (MMFB_LN_BWD=pair|tile|stream|lean)
 against the default ones, in one process (the switches are read per call).  Part of the default `-m gpu` suite: a variant
 that is kept must stay correct."""
 import os
@@ -45,83 +45,3 @@ def test_layernorm_backward_variants_match_the_default(variant, M, H):
                     assert (r - t).abs().max() <= 4e-3 * r.abs().max().clamp_min(1.0)
     finally:
         os.environ.pop("MMFB_LN_BWD", None)
-
-
-@pytest.mark.parametrize("variant", ["8", "16"])
-@pytest.mark.parametrize("Sq,Skv,drop", [(228, 228, True), (256, 130, False), (100, 256, True), (36, 36, True), (128, 128, False)])
-def test_one_cta_per_item_attention_backward_matches_the_default(Sq, Skv, drop, variant):
-    """MMFB_ATTN_BWD=8 (two threads per query row, serial issue order) and =16 (four threads per row, overlapped issue order,
-    one CTA per (batch, head)) against the default persistent kernel: same MMAs in the same accumulation order, same
-    arithmetic.  B * heads = 12 items are fewer than the SMs; the many-items-per-CTA case is the 37848-token encoder test
-    and tests/test_attention_gpu.py::test_attention_many_items_per_cta."""
-    from mmf_b200 import functional as F
-    torch.manual_seed(Sq * 5 + Skv)
-    B, heads, d = 4, 3, 64
-    W = heads * d
-    q = torch.randn(B * Sq, W, device="cuda").to(torch.bfloat16)
-    k = torch.randn(B * Skv, W, device="cuda").to(torch.bfloat16)
-    v = torch.randn(B * Skv, W, device="cuda").to(torch.bfloat16)
-    dctx = torch.randn(B * Sq, W, device="cuda").to(torch.bfloat16)
-    mask = torch.zeros(B, Skv, device="cuda")
-    mask[1, Skv // 3:] = -10000.0
-    mask[2, :] = -10000.0
-    bits = F.dropout_bits((B, heads, Sq), Skv, 0.1, 9, 0, "cuda") if drop else None
-    scale = 1.0 / 0.9 if drop else 1.0
-    ctx, lse2, c32 = F.attention_fwd(q, k, v, B, heads, Sq, Skv, mask, bits, scale, save_lo=True)
-
-    def run(flag):
-        if flag:
-            os.environ["MMFB_ATTN_BWD"] = variant
-        else:
-            os.environ.pop("MMFB_ATTN_BWD", None)
-        out = F.attention_bwd(dctx, q, k, v, ctx, lse2, B, heads, Sq, Skv, mask, bits, scale, ctx_lo=c32)
-        torch.cuda.synchronize()
-        return [t.clone() for t in out]
-    try:
-        ref, got = run(False), run(True)
-    finally:
-        os.environ.pop("MMFB_ATTN_BWD", None)
-    for name, r, t in zip(("dq", "dk", "dv"), ref, got):
-        r, t = r.float(), t.float()
-        assert (r - t).abs().max() <= 1e-2 * r.abs().max(), name
-        assert (r != t).float().mean() < 0.01, (name, (r != t).float().mean().item())
-
-
-@pytest.mark.parametrize("variant", ["1"])
-@pytest.mark.parametrize("Sq,Skv,drop", [(228, 228, True), (128, 256, False), (100, 36, True), (256, 17, False), (36, 130, True)])
-def test_other_attention_forwards_match_the_default(Sq, Skv, drop, variant):
-    """MMFB_ATTN_FWD=1 (one CTA per 128-query tile, P through shared memory) against the default (paired tiles, persistent,
-    P in tensor memory, outputs through bulk tensor stores): the same arithmetic per element"""
-    from mmf_b200 import functional as F
-    torch.manual_seed(Sq + Skv)
-    B, heads, d = 7, 3, 64
-    W = heads * d
-    q = torch.randn(B * Sq, W, device="cuda").to(torch.bfloat16)
-    k = torch.randn(B * Skv, W, device="cuda").to(torch.bfloat16)
-    v = torch.randn(B * Skv, W, device="cuda").to(torch.bfloat16)
-    mask = torch.zeros(B, Skv, device="cuda")
-    mask[1, Skv // 2:] = -10000.0
-    mask[2, :] = -10000.0                                   # fully masked sample: uniform softmax
-    bits = F.dropout_bits((B, heads, Sq), Skv, 0.1, 5, 0, "cuda") if drop else None
-    scale = 1.0 / 0.9 if drop else 1.0
-
-    def run(flag):
-        if flag:
-            os.environ["MMFB_ATTN_FWD"] = variant
-        else:
-            os.environ.pop("MMFB_ATTN_FWD", None)
-        out = F.attention_fwd(q, k, v, B, heads, Sq, Skv, mask, bits, scale, save_lo=True)
-        torch.cuda.synchronize()
-        return [t.clone() for t in out]
-    try:
-        ref, got = run(True), run(False)
-    finally:
-        os.environ.pop("MMFB_ATTN_FWD", None)
-    # the low part alone is a rounding residual (a last-bit difference of O flips it): compare ctx, lse2 and ctx + ctx_lo
-    ref = [ref[0], ref[1], ref[0].float() + ref[2].float()]
-    got = [got[0], got[1], got[0].float() + got[2].float()]
-    for name, r, t in zip(("ctx", "lse2", "ctx + ctx_lo"), ref, got):
-        r, t = r.float(), t.float()
-        assert torch.isfinite(t).all(), name
-        assert (r - t).abs().max() <= 2e-2 * r.abs().max(), (name, (r - t).abs().max().item())
-        assert ((r - t).norm() / r.norm()).item() < 3e-3, name

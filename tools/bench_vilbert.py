@@ -62,7 +62,7 @@ def main():
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench_vilbert needs a B200: the fusion path has no CPU fallback")
+        raise SystemExit("bench_vilbert needs an H100: the fusion path has no CPU fallback")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:

@@ -105,15 +105,13 @@ def main():
         f_fwd, f_bwd = 4.0 * B * heads * S * S * d, 10.0 * B * heads * S * S * d
         b_fwd = M * 3 * H * 2 + M * H * 2 + M * H * 4 + bits.numel() * 4
         b_bwd = M * 3 * H * 2 * 2 + M * H * 2 + bits.numel() * 4
-        for tag, env in (("default paired tiles", {}), ("MMFB_ATTN_FWD=1", {"MMFB_ATTN_FWD": "1"})):
-            timeit("attention_fwd [%s]" % tag, lambda: F.attention_fwd(q, k, v, B, heads, S, S, mask, bits, 1 / 0.9, save_lo=True),
-                   f_fwd, b_fwd, env)
+        timeit("attention_fwd", lambda: F.attention_fwd(q, k, v, B, heads, S, S, mask, bits, 1 / 0.9, save_lo=True),
+               f_fwd, b_fwd, {})
         ctx, lse2, c32 = F.attention_fwd(q, k, v, B, heads, S, S, mask, bits, 1 / 0.9, save_lo=True)
         dq = torch.empty_like(qkv)
-        for tag, env in (("default persistent", {}), ("MMFB_ATTN_BWD=16", {"MMFB_ATTN_BWD": "16"}), ("MMFB_ATTN_BWD=8", {"MMFB_ATTN_BWD": "8"})):
-            timeit("attention_bwd (+delta) [%s]" % tag,
-                   lambda: F.attention_bwd(dctx, q, k, v, ctx, lse2, B, heads, S, S, mask, bits, 1 / 0.9, dq=dq[:, :H],
-                                           dk=dq[:, H:2 * H], dv=dq[:, 2 * H:], ctx_lo=c32), f_bwd, b_bwd, env)
+        timeit("attention_bwd (+delta)",
+               lambda: F.attention_bwd(dctx, q, k, v, ctx, lse2, B, heads, S, S, mask, bits, 1 / 0.9, dq=dq[:, :H],
+                                       dk=dq[:, H:2 * H], dv=dq[:, 2 * H:], ctx_lo=c32), f_bwd, b_bwd, {})
         timeit("dropout_bits attention [B,h,S,S]", lambda: F.dropout_bits((B, heads, S), S, 0.1, 7, 0, dev), None, bits.numel() * 4)
         del qkv, dctx, dq, ctx, c32
 
