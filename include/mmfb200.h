@@ -101,7 +101,10 @@ int mmfb_attention_bwd(const mmfb_attn_args* args, mmfb_stream stream);
 /* LayerNorm over the last dimension (eps 1e-12 on this path), one warp per row.
  * fwd: x = LN(y)*gamma + beta, optional dropout on x (embeddings), saves mean / rstd (fp32 [M]).
  * bwd: dy = dLN(dx (+dx2)); dz = dropout-backward(dy) for the dense branch that fed y = dropout(dense)+resid;
- *      dgamma/dbeta/dbias (fp32 [H]) are ACCUMULATED (+=).  dz may equal dy (no dropout) or be NULL. */
+ *      dgamma/dbeta/dbias (fp32 [H]) are ACCUMULATED (+=).  dz may equal dy (no dropout) or be NULL.
+ * Limits (MMFB_ERR_ARG otherwise): H a multiple of 8 and <= 2048; rows are read and written as 16-byte vectors, so every
+ * row tensor the call uses starts 16-byte aligned and, when M > 1, has a leading dimension that is a multiple of 8;
+ * gamma and beta are 16-byte aligned in the forward, gamma in the backward when H > 1024. */
 typedef struct {
   const void* y; int64_t ldy;        /* bf16 [M,H] pre-LN input */
   const void* gamma; const void* beta; /* bf16 [H] */

@@ -1,8 +1,6 @@
 """Builds libmmfb200.so (sm_90a only) in-tree with nvcc.
 
     python -m mmf_b200.csrc.build [--force] [--verbose]
-    python -m mmf_b200.csrc.build --variant NAME -DFLAG=1 ...   # libmmfb200_NAME.so with extra defines, for A/B runs
-                                                                # (select it at run time with MMFB_LIB=<path>)
 
 The built library lives next to the sources (git-ignored).  There is exactly one target architecture:
 compute_90a / sm_90a (H100).
@@ -48,11 +46,8 @@ def _digest():
     return h.hexdigest()
 
 
-def build(force=False, verbose=False, variant=None, defines=()):
-    """Compile every .cu into objects (parallel) and link the shared library. Returns its path.
-    `variant` + `defines`: an experimental build next to the product library (never loaded unless MMFB_LIB names it)."""
-    if variant:
-        return _build_variant(variant, list(defines), verbose)
+def build(force=False, verbose=False):
+    """Compile every .cu into objects (parallel) and link the shared library. Returns its path."""
     digest = _digest()
     if not force and os.path.exists(LIB) and os.path.exists(STAMP):
         with open(STAMP) as fh:
@@ -89,34 +84,6 @@ def build(force=False, verbose=False, variant=None, defines=()):
     return LIB
 
 
-def _build_variant(name, defines, verbose):
-    nvcc = _nvcc()
-    out = os.path.join(HERE, "libmmfb200_%s.so" % name)
-    objs, procs = [], []
-    for src in _sources():
-        obj = os.path.join(HERE, src.replace(".cu", ".%s.o" % name))
-        objs.append(obj)
-        cmd = [nvcc] + NVCC_FLAGS + defines + ["-c", os.path.join(HERE, src), "-o", obj]
-        procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
-    for src, p in procs:
-        o, _ = p.communicate()
-        if p.returncode != 0:
-            raise RuntimeError("nvcc failed for %s (%s):\n%s" % (src, name, o))
-        for line in o.splitlines():
-            if verbose or ("spill" in line and "0 bytes spill stores, 0 bytes spill loads" not in line):
-                sys.stderr.write("[%s %s] %s\n" % (name, src, line))
-    r = subprocess.run([nvcc, "-shared", "-o", out] + objs + ["-gencode", "arch=compute_90a,code=sm_90a",
-                                                             "-cudart", "static"],
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    if r.returncode != 0:
-        raise RuntimeError("linking %s failed:\n%s" % (out, r.stdout))
-    for o in objs:
-        os.remove(o)
-    return out
-
-
 if __name__ == "__main__":
-    variant = sys.argv[sys.argv.index("--variant") + 1] if "--variant" in sys.argv else None
-    path = build(force="--force" in sys.argv, verbose="--verbose" in sys.argv, variant=variant,
-                 defines=[a for a in sys.argv[1:] if a.startswith("-D")])
+    path = build(force="--force" in sys.argv, verbose="--verbose" in sys.argv)
     print(path)

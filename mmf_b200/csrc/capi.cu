@@ -5,8 +5,6 @@
 
 #include <atomic>
 
-#include <stdlib.h>
-
 #include "mmfb_internal.h"
 
 namespace mmfb {
@@ -23,15 +21,6 @@ int set_error(int code, const char* fmt, ...) {
 }
 
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-
-bool pdl_enabled() {
-  static int v = -1;      // benign race: every thread computes the same value
-  if (v < 0) {
-    const char* e = getenv("MMFB_PDL");
-    v = (e == nullptr) ? 1 : (e[0] != '0');
-  }
-  return v != 0;
-}
 
 int num_sms() {
   static int n = 0;

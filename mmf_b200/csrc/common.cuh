@@ -31,8 +31,8 @@ __device__ __forceinline__ uint8_t* smem_align1024(uint8_t* raw) {
 // programmatic dependent launch: every kernel of the library lets the NEXT kernel of the stream start launching as soon
 // as all of its own CTAs have started (griddep_launch at the top), and waits for the PREVIOUS kernel to have completed and
 // flushed its memory before it touches global data (griddep_wait after its own set-up: barrier init,
-// descriptor prefetch).  The launch latency and the prologue of kernel n+1 overlap the tail of kernel n; both
-// instructions are no-ops when the kernel was launched without the attribute (MMFB_PDL=0).
+// descriptor prefetch).  The launch latency and the prologue of kernel n+1 overlap the tail of kernel n.  launch_k
+// (mmfb_internal.h) sets the launch attribute that enables this on every kernel of the library.
 // --------------------------------------------------------------------------------------
 __device__ __forceinline__ void griddep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -204,13 +204,6 @@ __device__ __forceinline__ uint4 philox4x32(uint64_t seed, uint64_t ctr) {
     k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
   }
   return make_uint4(c0, c1, c2, c3);
-}
-// keep-mask for the 4 consecutive elements [4*quad, 4*quad+4): bit i set = keep element i.
-// thresh = floor(p * 2^32); element kept iff rnd >= thresh.
-__device__ __forceinline__ uint32_t dropout_keep4(uint64_t seed, uint64_t quad, uint32_t thresh) {
-  uint4 r = philox4x32(seed, quad);
-  return (r.x >= thresh ? 1u : 0u) | (r.y >= thresh ? 2u : 0u) | (r.z >= thresh ? 4u : 0u) |
-         (r.w >= thresh ? 8u : 0u);
 }
 
 // --------------------------------------------------------------------------------------

@@ -31,37 +31,23 @@ int make_tmap_2d(CUtensorMap* map, const void* ptr, int64_t inner, int64_t outer
 int make_tmap_3d(CUtensorMap* map, const void* ptr, int64_t inner, int64_t d1, int64_t d2, int64_t ld1,
                  int64_t ld2, int box_inner, int box_d1);
 
-// Launch with the programmatic-stream-serialization attribute (common.cuh: griddep_launch / griddep_wait), optionally as
-// clusters of `cluster` CTAs.  MMFB_PDL=0 (read once) launches plainly - the A/B switch.
-bool pdl_enabled();
+// Launch with the programmatic-stream-serialization attribute (common.cuh: griddep_launch / griddep_wait).
 template <typename... KArgs, typename... Args>
-cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, int cluster,
-                     Args&&... args) {
+cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int n = 0;
-  if (cluster > 1) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = cluster;
-    attr[n].val.clusterDim.y = 1;
-    attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  if (pdl_enabled()) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = n;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 #define MMFB_LAUNCH(kern, grid, block, smem, stream, ...) \
-  (void)::mmfb::launch_k(kern, dim3(grid), dim3(block), static_cast<size_t>(smem), stream, 1, __VA_ARGS__)
+  (void)::mmfb::launch_k(kern, dim3(grid), dim3(block), static_cast<size_t>(smem), stream, __VA_ARGS__)
 
 int gemm(const mmfb_gemm_args& a, cudaStream_t stream);
 int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream);

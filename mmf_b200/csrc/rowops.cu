@@ -11,6 +11,8 @@
 #include "common.cuh"
 #include "mmfb_internal.h"
 
+#include <initializer_list>
+
 namespace mmfb {
 
 constexpr int MAXV = 8;         // per-lane 8-element vectors: rows up to 8*256 = 2048 columns
@@ -98,8 +100,10 @@ ln_fwd_kernel(const bf16* __restrict__ y, int64_t ldy, const bf16* __restrict__ 
 //   dgamma += sum_rows dx * xhat ; dbeta += sum_rows dx ; dbias += sum_rows dz
 // dx_in may carry an extra additive term dx2 (the residual gradient arriving from a later consumer).
 // A persistent grid (grid-stride over row groups) keeps the number of fp32 atomics at 3*H per block.
+// Two kernels, chosen by H: ln_bwd_stream_kernel for H <= 1024, ln_bwd_kernel for 1024 < H <= 2048.
 // ----------------------------------------------------------------------------------------------
-template <int NV>
+// Rows of up to MAXV * 256 columns: a warp loads, computes and stores a row held in registers, and only the other warps
+// of the SM cover its load latency.
 __global__ void __launch_bounds__(ROW_WARPS * 32)
 ln_bwd_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict__ dx2, int64_t lddx2,
               const bf16* __restrict__ y, int64_t ldy, const float* __restrict__ mean,
@@ -110,19 +114,19 @@ ln_bwd_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict_
   griddep_wait();
   __shared__ float red[ROW_WARPS][256];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  float ag[NV][8], ab[NV][8], az[NV][8];
+  float ag[MAXV][8], ab[MAXV][8], az[MAXV][8];
 #pragma unroll
-  for (int i = 0; i < NV; ++i)
+  for (int i = 0; i < MAXV; ++i)
 #pragma unroll
     for (int e = 0; e < 8; ++e) { ag[i][e] = 0.0f; ab[i][e] = 0.0f; az[i][e] = 0.0f; }
 
   for (int64_t row = static_cast<int64_t>(blockIdx.x) * ROW_WARPS + warp; row < M;
        row += static_cast<int64_t>(gridDim.x) * ROW_WARPS) {
     const float mu = mean[row], rs = rstd[row];
-    float g[NV][8], d[NV][8], xh[NV][8];
+    float g[MAXV][8], d[MAXV][8], xh[MAXV][8];
     float s1 = 0.0f, s2 = 0.0f;
 #pragma unroll
-    for (int i = 0; i < NV; ++i) {
+    for (int i = 0; i < MAXV; ++i) {
       const int col = i * 256 + lane * 8;
       if (col < H) {
         float yy[8];
@@ -149,7 +153,7 @@ ln_bwd_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict_
     s1 = warp_sum(s1) / H;
     s2 = warp_sum(s2) / H;
 #pragma unroll
-    for (int i = 0; i < NV; ++i) {
+    for (int i = 0; i < MAXV; ++i) {
       const int col = i * 256 + lane * 8;
       if (col < H) {
         float o[8];
@@ -176,7 +180,7 @@ ln_bwd_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict_
     float* dst = which == 0 ? dgamma : (which == 1 ? dbeta : dbias);
     if (dst == nullptr) continue;
 #pragma unroll
-    for (int i = 0; i < NV; ++i) {
+    for (int i = 0; i < MAXV; ++i) {
       if (i * 256 >= H) break;
       __syncthreads();
 #pragma unroll
@@ -191,18 +195,6 @@ ln_bwd_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict_
   }
 }
 
-// Single-pass LayerNorm backward, lean variant (staged: selected with MMFB_LN_BWD=lean, not the default until it is
-// measured).  Same results as ln_bwd_kernel, built for two 256-thread blocks per SM: the row is held as the PACKED
-// bf16 words that were loaded (d, y: 8 registers per 256-column slab instead of 16 floats) and unpacked again in the
-// second phase; gamma is re-read from L1 per row.  Only the three column-sum sets stay in registers across rows, so
-// the row tensors are read from HBM once (the rows + cols pair reads d and y twice and dz once more).
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  float2 t;
-  t = unpack_bf16x2(u.x); f[0] = t.x; f[1] = t.y;
-  t = unpack_bf16x2(u.y); f[2] = t.x; f[3] = t.y;
-  t = unpack_bf16x2(u.z); f[4] = t.x; f[5] = t.y;
-  t = unpack_bf16x2(u.w); f[6] = t.x; f[7] = t.y;
-}
 // bf16x2 word -> the two values as a packed fp32 pair (exact: a bf16 is the top half of an fp32)
 __device__ __forceinline__ uint64_t unpack2(uint32_t w) {
   return pk2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
@@ -212,163 +204,17 @@ __device__ __forceinline__ uint32_t pack2(uint64_t v) {
   upk2(v, lo, hi);
   return pack_bf16x2(lo, hi);
 }
-// Instruction diet (the first version issued ~42 instructions per element and was issue-bound at 0.48 of the HBM peak):
-// all arithmetic on packed fp32 pairs (FFMA2 / FMUL2 / FADD2), xhat as ONE fma (y * rstd - mean * rstd), the output as
+
+// Single-pass streaming LayerNorm backward for rows of up to 4 * 256 columns.  Every warp owns a private ring of ST row
+// slots in shared memory that its lane 0 fills with bulk async copies (cp.async.bulk, one per tensor row, completion on a
+// per-slot mbarrier) ST rows ahead, so ST x 16 warps x 3 KB are in flight per SM whatever the warps are doing, and the
+// row lives in shared memory across the two phases (no row registers).  Rows are read from HBM once; dy / dz are stored
+// straight from registers.
+// Instruction diet (a first version issued ~42 instructions per element and was issue-bound at 0.48 of the HBM peak):
+// all arithmetic on packed fp32 pairs (common.cuh: pk2 / fma2), xhat as ONE fma (y * rstd - mean * rstd), the output as
 // two (d * (gamma * rstd) - rstd * m1, then - rstd * m2 * xhat), gamma as fp32 in shared memory (LDS.128, no unpack),
 // dropout applied to the PACKED bf16 result with an AND mask looked up per 8 keep-bits (256 x 16 B table in shared
 // memory) instead of eight bit tests + selects; dbias sums the bf16 values that are stored (what the consumer reads).
-template <int NV, bool HAS_DX2>
-__global__ void __launch_bounds__(ROW_WARPS * 32, 2)
-ln_bwd_lean_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict__ dx2, int64_t lddx2,
-                   const bf16* __restrict__ y, int64_t ldy, const float* __restrict__ mean,
-                   const float* __restrict__ rstd, const bf16* __restrict__ gamma, bf16* __restrict__ dy, int64_t lddy,
-                   bf16* __restrict__ dz, int64_t lddz, const uint32_t* __restrict__ dmask, int64_t ldmask, float dscale,
-                   float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M, int H) {
-  griddep_launch();
-  griddep_wait();
-  __shared__ float red[ROW_WARPS][256];
-  __shared__ __align__(16) float sG[NV * 256];
-  __shared__ __align__(16) uint32_t sKeep[256][4];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int c = threadIdx.x; c < NV * 256; c += ROW_WARPS * 32) sG[c] = c < H ? __bfloat162float(gamma[c]) : 0.0f;
-  {
-    const uint32_t b = threadIdx.x;          // 256 threads <-> the 256 patterns of 8 keep-bits
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      sKeep[b][k] = (((b >> (2 * k)) & 1u) ? 0x0000ffffu : 0u) | (((b >> (2 * k + 1)) & 1u) ? 0xffff0000u : 0u);
-  }
-  __syncthreads();
-  uint64_t ag[NV][4], ab[NV][4], az[NV][4];
-#pragma unroll
-  for (int i = 0; i < NV; ++i)
-#pragma unroll
-    for (int k = 0; k < 4; ++k) { ag[i][k] = 0ull; ab[i][k] = 0ull; az[i][k] = 0ull; }
-  const float invH = 1.0f / static_cast<float>(H);
-  const uint64_t ds2 = pk2(dscale, dscale);
-
-  for (int64_t row = static_cast<int64_t>(blockIdx.x) * ROW_WARPS + warp; row < M;
-       row += static_cast<int64_t>(gridDim.x) * ROW_WARPS) {
-    const float mu = mean[row], rs = rstd[row];
-    const float nmr = -mu * rs;
-    const uint64_t rs2 = pk2(rs, rs), nmr2 = pk2(nmr, nmr);
-    uint4 dw[NV], yw[NV];      // packed bf16 rows of dx and y, kept across the two phases
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int col = i * 256 + lane * 8;
-      dw[i] = make_uint4(0u, 0u, 0u, 0u);
-      yw[i] = make_uint4(0u, 0u, 0u, 0u);
-      if (col < H) {
-        dw[i] = *reinterpret_cast<const uint4*>(dx + row * lddx + col);
-        yw[i] = *reinterpret_cast<const uint4*>(y + row * ldy + col);
-      }
-    }
-    uint64_t s1 = 0ull, s2 = 0ull;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int col = i * 256 + lane * 8;
-      if (col < H) {
-        const uint32_t da[4] = {dw[i].x, dw[i].y, dw[i].z, dw[i].w};
-        const uint32_t ya[4] = {yw[i].x, yw[i].y, yw[i].z, yw[i].w};
-        uint32_t xa[4] = {0u, 0u, 0u, 0u};
-        if (HAS_DX2) {
-          // d = dx + dx2 is formed in fp32; re-packing the sum to bf16 would change the result, so the second
-          // stream is not kept but re-read in phase 2 (an L1 hit)
-          const uint4 t = *reinterpret_cast<const uint4*>(dx2 + row * lddx2 + col);
-          xa[0] = t.x; xa[1] = t.y; xa[2] = t.z; xa[3] = t.w;
-        }
-        const float4 ga = *reinterpret_cast<const float4*>(sG + col), gb = *reinterpret_cast<const float4*>(sG + col + 4);
-        const uint64_t g2[4] = {pk2(ga.x, ga.y), pk2(ga.z, ga.w), pk2(gb.x, gb.y), pk2(gb.z, gb.w)};
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          uint64_t d2 = unpack2(da[k]);
-          if (HAS_DX2) d2 = add2(d2, unpack2(xa[k]));
-          const uint64_t xh2 = fma2(unpack2(ya[k]), rs2, nmr2);
-          const uint64_t dg2 = mul2(d2, g2[k]);
-          s1 = add2(s1, dg2);
-          s2 = fma2(dg2, xh2, s2);
-          ag[i][k] = fma2(d2, xh2, ag[i][k]);
-          ab[i][k] = add2(ab[i][k], d2);
-        }
-      }
-    }
-    float s1a, s1b, s2a, s2b;
-    upk2(s1, s1a, s1b);
-    upk2(s2, s2a, s2b);
-    const float m1 = warp_sum(s1a + s1b) * invH, m2 = warp_sum(s2a + s2b) * invH;
-    const uint64_t nA2 = pk2(-rs * m1, -rs * m1), nB2 = pk2(-rs * m2, -rs * m2);
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      const int col = i * 256 + lane * 8;
-      if (col < H) {
-        const uint32_t da[4] = {dw[i].x, dw[i].y, dw[i].z, dw[i].w};
-        const uint32_t ya[4] = {yw[i].x, yw[i].y, yw[i].z, yw[i].w};
-        uint32_t xa[4] = {0u, 0u, 0u, 0u};
-        if (HAS_DX2) {
-          const uint4 t = *reinterpret_cast<const uint4*>(dx2 + row * lddx2 + col);
-          xa[0] = t.x; xa[1] = t.y; xa[2] = t.z; xa[3] = t.w;
-        }
-        const float4 ga = *reinterpret_cast<const float4*>(sG + col), gb = *reinterpret_cast<const float4*>(sG + col + 4);
-        const uint64_t g2[4] = {pk2(ga.x, ga.y), pk2(ga.z, ga.w), pk2(gb.x, gb.y), pk2(gb.z, gb.w)};
-        uint32_t keep[4] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu};
-        if (dmask != nullptr) {
-          const uint32_t w = __ldg(dmask + row * ldmask + (col >> 5));
-          const uint4 kk = *reinterpret_cast<const uint4*>(sKeep[(w >> (col & 31)) & 0xFFu]);
-          keep[0] = kk.x; keep[1] = kk.y; keep[2] = kk.z; keep[3] = kk.w;
-        }
-        uint32_t ow[4], zw[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          uint64_t d2 = unpack2(da[k]);
-          if (HAS_DX2) d2 = add2(d2, unpack2(xa[k]));
-          const uint64_t xh2 = fma2(unpack2(ya[k]), rs2, nmr2);
-          const uint64_t o2 = fma2(nB2, xh2, fma2(d2, mul2(g2[k], rs2), nA2));
-          ow[k] = pack2(o2);
-          if (dmask != nullptr) {
-            zw[k] = pack2(mul2(o2, ds2)) & keep[k];
-            az[i][k] = add2(az[i][k], unpack2(zw[k]));
-          } else {
-            zw[k] = ow[k];
-            az[i][k] = add2(az[i][k], o2);
-          }
-        }
-        if (dy != nullptr) *reinterpret_cast<uint4*>(dy + row * lddy + col) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-        if (dz != nullptr && (dmask != nullptr || dz != dy))
-          *reinterpret_cast<uint4*>(dz + row * lddz + col) = make_uint4(zw[0], zw[1], zw[2], zw[3]);
-      }
-    }
-  }
-  // block reduction of the three column-sum sets, 256 columns at a time, then one atomic per column
-#pragma unroll
-  for (int which = 0; which < 3; ++which) {
-    float* dst = which == 0 ? dgamma : (which == 1 ? dbeta : dbias);
-    if (dst == nullptr) continue;
-#pragma unroll
-    for (int i = 0; i < NV; ++i) {
-      if (i * 256 >= H) break;
-      __syncthreads();
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        float lo, hi;
-        upk2(which == 0 ? ag[i][k] : (which == 1 ? ab[i][k] : az[i][k]), lo, hi);
-        red[warp][lane * 8 + 2 * k] = lo;
-        red[warp][lane * 8 + 2 * k + 1] = hi;
-      }
-      __syncthreads();
-      const int c = threadIdx.x;  // 256 threads <-> 256 columns
-      float t = 0.0f;
-#pragma unroll
-      for (int w = 0; w < ROW_WARPS; ++w) t += red[w][c];
-      if (i * 256 + c < H) atomicAdd(dst + i * 256 + c, t);
-    }
-  }
-}
-
-// Single-pass LayerNorm backward, streaming variant (MMFB_LN_BWD=stream).  In the kernel above a warp loads, computes and
-// stores a row, and only the other warps of the SM cover its load latency.  Here every warp owns a private ring of
-// ST row slots in shared memory that its lane 0 fills with bulk async copies (cp.async.bulk, one per tensor row,
-// completion on a per-slot mbarrier) ST rows ahead, so ST x 16 warps x 3 KB are in flight per SM whatever the warps are
-// doing, the row lives in shared memory across the two phases (no row registers), and the arithmetic is the fp32-pair
-// form of the lean kernel (common.cuh: pk2 / fma2).  Rows are read from HBM once; dy / dz are stored straight from registers.
 __device__ __forceinline__ void bulk_load_1d(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(dst_smem)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
@@ -549,256 +395,6 @@ ln_bwd_stream_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __re
       for (int w = 0; w < ROW_WARPS; ++w) t += red[w * 256 + c];
       if (i * 256 + c < H) atomicAdd(dst + i * 256 + c, t);
     }
-  }
-}
-
-// Single-pass LayerNorm backward, tile variant (staged: MMFB_LN_BWD=tile).  A row is spread over WPR warps (each lane
-// owns ONE 8-column slab for all rows it visits), so the three column-sum sets cost 24 registers per thread instead of
-// 24 x (H / 256), gamma is loop-invariant, and a group of WPR warps processes RB rows per step: 2 x RB 16-byte loads in
-// flight per lane and one named barrier per RB rows (row statistics of the WPR warps exchanged through shared memory,
-// double-buffered by step parity).  dx, y, keep-bits are read once, dy / dz written once: traffic = the algorithmic bytes.
-template <int WPR, int G, bool HAS_DX2>
-__global__ void __launch_bounds__(WPR * G * 32, 1)
-ln_bwd_tile_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict__ dx2, int64_t lddx2,
-                   const bf16* __restrict__ y, int64_t ldy, const float* __restrict__ mean,
-                   const float* __restrict__ rstd, const bf16* __restrict__ gamma, bf16* __restrict__ dy, int64_t lddy,
-                   bf16* __restrict__ dz, int64_t lddz, const uint32_t* __restrict__ dmask, int64_t ldmask, float dscale,
-                   float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M, int H) {
-  griddep_launch();
-  griddep_wait();
-  constexpr int RB = 4;
-  __shared__ float sStat[2][G][WPR][RB][2];
-  __shared__ float sRed[G][WPR * 256];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int grp = warp / WPR, wig = warp % WPR;
-  const int col = (wig * 32 + lane) * 8;
-  const bool cok = col < H;
-  float g[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) g[e] = 0.0f;
-  if (cok) ld8(gamma + col, g);
-  float ag[8], ab[8], az[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) { ag[e] = 0.0f; ab[e] = 0.0f; az[e] = 0.0f; }
-  const float invH = 1.0f / static_cast<float>(H);
-  const int64_t n_steps = (static_cast<int64_t>(M) + RB - 1) / RB;
-  int par = 0;
-  const int64_t g_first = static_cast<int64_t>(blockIdx.x) * G + grp, g_stride = static_cast<int64_t>(gridDim.x) * G;
-  for (int64_t st = g_first; st < n_steps; st += g_stride, par ^= 1) {
-    const int64_t row0 = st * RB;
-    uint4 dw[RB], yw[RB];          // the rows as the packed bf16 words that were loaded; unpacked in both phases
-    float mu[RB], rs[RB], s1[RB], s2[RB];
-#pragma unroll
-    for (int r = 0; r < RB; ++r) {
-      const int64_t row = row0 + r;
-      dw[r] = make_uint4(0, 0, 0, 0);
-      yw[r] = make_uint4(0, 0, 0, 0);
-      if (cok && row < M) {
-        dw[r] = *reinterpret_cast<const uint4*>(dx + row * lddx + col);
-        yw[r] = *reinterpret_cast<const uint4*>(y + row * ldy + col);
-      }
-      mu[r] = row < M ? mean[row] : 0.0f;
-      rs[r] = row < M ? rstd[row] : 0.0f;
-    }
-#pragma unroll
-    for (int r = 0; r < RB; ++r) {
-      float d[8], yy[8];
-      unpack8(dw[r], d);
-      if (HAS_DX2 && cok && row0 + r < M) {
-        // d = dx + dx2 in fp32; the second stream is re-read in phase 2 (an L1 hit) rather than kept
-        float t[8];
-        ld8(dx2 + (row0 + r) * lddx2 + col, t);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) d[e] += t[e];
-      }
-      unpack8(yw[r], yy);
-      float a1 = 0.0f, a2 = 0.0f;
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float xh = (yy[e] - mu[r]) * rs[r];
-        const float dg = d[e] * g[e];
-        a1 += dg;
-        a2 += dg * xh;
-        ag[e] += d[e] * xh;
-        ab[e] += d[e];
-      }
-      s1[r] = warp_sum(a1);
-      s2[r] = warp_sum(a2);
-    }
-    if (WPR > 1) {
-      if (lane == 0) {
-#pragma unroll
-        for (int r = 0; r < RB; ++r) { sStat[par][grp][wig][r][0] = s1[r]; sStat[par][grp][wig][r][1] = s2[r]; }
-      }
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(WPR * 32) : "memory");
-#pragma unroll
-      for (int r = 0; r < RB; ++r) {
-        float t1 = 0.0f, t2 = 0.0f;
-#pragma unroll
-        for (int w = 0; w < WPR; ++w) { t1 += sStat[par][grp][w][r][0]; t2 += sStat[par][grp][w][r][1]; }
-        s1[r] = t1; s2[r] = t2;
-      }
-    }
-#pragma unroll
-    for (int r = 0; r < RB; ++r) {
-      const int64_t row = row0 + r;
-      if (!(cok && row < M)) continue;
-      float d[8], yy[8], o[8];
-      unpack8(dw[r], d);
-      if (HAS_DX2) {
-        float t[8];
-        ld8(dx2 + row * lddx2 + col, t);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) d[e] += t[e];
-      }
-      unpack8(yw[r], yy);
-      const float m1 = s1[r] * invH, m2 = s2[r] * invH;
-#pragma unroll
-      for (int e = 0; e < 8; ++e) o[e] = rs[r] * (d[e] * g[e] - m1 - ((yy[e] - mu[r]) * rs[r]) * m2);
-      if (dy != nullptr) st8(dy + row * lddy + col, o);
-      if (dmask != nullptr) {
-        const uint32_t w = __ldg(dmask + row * ldmask + (col >> 5));
-        const uint32_t bits = (w >> (col & 31)) & 0xFFu;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) o[e] = ((bits >> e) & 1u) ? o[e] * dscale : 0.0f;
-        st8(dz + row * lddz + col, o);
-      } else if (dz != nullptr && dz != dy) {
-        st8(dz + row * lddz + col, o);
-      }
-#pragma unroll
-      for (int e = 0; e < 8; ++e) az[e] += o[e];
-    }
-  }
-  // block reduction over the G groups, then one atomic per column and statistic
-#pragma unroll
-  for (int which = 0; which < 3; ++which) {
-    float* dst = which == 0 ? dgamma : (which == 1 ? dbeta : dbias);
-    if (dst == nullptr) continue;
-    __syncthreads();
-#pragma unroll
-    for (int e = 0; e < 8; ++e) sRed[grp][(wig * 32 + lane) * 8 + e] = which == 0 ? ag[e] : (which == 1 ? ab[e] : az[e]);
-    __syncthreads();
-    for (int c = threadIdx.x; c < WPR * 256; c += WPR * G * 32) {
-      float t = 0.0f;
-#pragma unroll
-      for (int gg = 0; gg < G; ++gg) t += sRed[gg][c];
-      if (c < H) atomicAdd(dst + c, t);
-    }
-  }
-}
-
-// Row-only LayerNorm backward (no column statistics): few registers, high occupancy.  dy, dz as above.
-template <int NV>
-__global__ void __launch_bounds__(ROW_WARPS * 32)
-ln_bwd_rows_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict__ dx2, int64_t lddx2,
-                   const bf16* __restrict__ y, int64_t ldy, const float* __restrict__ mean,
-                   const float* __restrict__ rstd, const bf16* __restrict__ gamma, bf16* __restrict__ dy, int64_t lddy,
-                   bf16* __restrict__ dz, int64_t lddz, const uint32_t* __restrict__ dmask, int64_t ldmask, float dscale,
-                   int M, int H) {
-  griddep_launch();
-  griddep_wait();
-  const int lane = threadIdx.x & 31;
-  const int64_t row = static_cast<int64_t>(blockIdx.x) * ROW_WARPS + (threadIdx.x >> 5);
-  if (row >= M) return;
-  const float mu = mean[row], rs = rstd[row];
-  float dg[NV][8], xh[NV][8];
-  float s1 = 0.0f, s2 = 0.0f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int col = i * 256 + lane * 8;
-    if (col < H) {
-      float d[8], yy[8], g[8];
-      ld8(dx + row * lddx + col, d);
-      if (dx2 != nullptr) {
-        float t[8];
-        ld8(dx2 + row * lddx2 + col, t);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) d[e] += t[e];
-      }
-      ld8(y + row * ldy + col, yy);
-      ld8(gamma + col, g);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        xh[i][e] = (yy[e] - mu) * rs;
-        dg[i][e] = d[e] * g[e];
-        s1 += dg[i][e];
-        s2 += dg[i][e] * xh[i][e];
-      }
-    }
-  }
-  s1 = warp_sum(s1) / H;
-  s2 = warp_sum(s2) / H;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const int col = i * 256 + lane * 8;
-    if (col < H) {
-      float o[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) o[e] = rs * (dg[i][e] - s1 - xh[i][e] * s2);
-      if (dy != nullptr) st8(dy + row * lddy + col, o);
-      if (dmask != nullptr) {
-        const uint32_t w = __ldg(dmask + row * ldmask + (col >> 5));
-        const uint32_t bits = (w >> (col & 31)) & 0xFFu;
-#pragma unroll
-        for (int e = 0; e < 8; ++e) o[e] = ((bits >> e) & 1u) ? o[e] * dscale : 0.0f;
-        st8(dz + row * lddz + col, o);
-      } else if (dz != nullptr && dz != dy) {
-        st8(dz + row * lddz + col, o);
-      }
-    }
-  }
-}
-
-// Column statistics of the LayerNorm backward: dgamma += sum_r d*xhat, dbeta += sum_r d, dbias += sum_r dz, with
-// d = dx (+dx2).  Same access pattern as colsum: each thread owns 8 columns for a strided set of rows.
-__global__ void __launch_bounds__(256)
-ln_bwd_cols_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict__ dx2, int64_t lddx2,
-                   const bf16* __restrict__ y, int64_t ldy, const float* __restrict__ mean,
-                   const float* __restrict__ rstd, const bf16* __restrict__ dz, int64_t lddz,
-                   float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M, int H) {
-  griddep_launch();
-  griddep_wait();
-  __shared__ float red[8][256];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int col = blockIdx.x * 256 + lane * 8;
-  float ag[8], ab[8], az[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) { ag[e] = 0.0f; ab[e] = 0.0f; az[e] = 0.0f; }
-  if (col < H) {
-    for (int64_t row = static_cast<int64_t>(blockIdx.y) * 8 + warp; row < M; row += static_cast<int64_t>(gridDim.y) * 8) {
-      const float mu = mean[row], rs = rstd[row];
-      float d[8], yy[8];
-      ld8(dx + row * lddx + col, d);
-      if (dx2 != nullptr) {
-        float t[8];
-        ld8(dx2 + row * lddx2 + col, t);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) d[e] += t[e];
-      }
-      ld8(y + row * ldy + col, yy);
-#pragma unroll
-      for (int e = 0; e < 8; ++e) { ag[e] += d[e] * (yy[e] - mu) * rs; ab[e] += d[e]; }
-      if (dbias != nullptr) {
-        float z[8];
-        ld8(dz + row * lddz + col, z);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) az[e] += z[e];
-      }
-    }
-  }
-#pragma unroll
-  for (int which = 0; which < 3; ++which) {
-    float* dst = which == 0 ? dgamma : (which == 1 ? dbeta : dbias);
-    if (dst == nullptr) continue;
-    __syncthreads();
-#pragma unroll
-    for (int e = 0; e < 8; ++e) red[warp][lane * 8 + e] = which == 0 ? ag[e] : (which == 1 ? ab[e] : az[e]);
-    __syncthreads();
-    float t = 0.0f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) t += red[w][threadIdx.x];
-    const int c = blockIdx.x * 256 + threadIdx.x;
-    if (c < H) atomicAdd(dst + c, t);
   }
 }
 
@@ -1108,10 +704,30 @@ static int launch_ok(const char* who) {
   return MMFB_OK;
 }
 
+// The LayerNorm kernels move rows as 16-byte vectors (the streaming backward with cp.async.bulk), so every row a kernel
+// reads or writes must start on a 16-byte boundary: the base pointer aligned and, when there is more than one row, the
+// leading dimension a multiple of 8 elements.  Null tensors are not used by the call and are skipped.
+struct RowTensor {
+  const void* p;
+  int64_t ld;        // 0 for the [H] vectors
+  const char* name;
+};
+static int check_aligned(const char* who, int M, std::initializer_list<RowTensor> ts) {
+  for (const RowTensor& t : ts) {
+    if (t.p == nullptr) continue;
+    if (reinterpret_cast<uintptr_t>(t.p) & 15) return set_error(MMFB_ERR_ARG, "%s: %s must be 16-byte aligned", who, t.name);
+    if (M > 1 && t.ld % 8)
+      return set_error(MMFB_ERR_ARG, "%s: ld%s = %lld must be a multiple of 8", who, t.name, static_cast<long long>(t.ld));
+  }
+  return MMFB_OK;
+}
+
 int ln_fwd(const mmfb_ln_args& a, cudaStream_t s) {
   int rc = check_rows(a.M, a.H, "layernorm_fwd");
   if (rc) return rc;
   if (!a.y || !a.gamma || !a.beta || !a.x) return set_error(MMFB_ERR_ARG, "layernorm_fwd: null pointer");
+  rc = check_aligned("layernorm_fwd", a.M, {{a.y, a.ldy, "y"}, {a.x, a.ldx, "x"}, {a.gamma, 0, "gamma"}, {a.beta, 0, "beta"}});
+  if (rc) return rc;
 #define LN_FWD(NV)                                                                                         \
   MMFB_LAUNCH(ln_fwd_kernel<NV>, (a.M + ROW_WARPS - 1) / ROW_WARPS, ROW_WARPS * 32, 0, s,                           \
       (const bf16*)a.y, a.ldy, (const bf16*)a.gamma, (const bf16*)a.beta, (bf16*)a.x, a.ldx, a.mean, a.rstd, \
@@ -1122,124 +738,51 @@ int ln_fwd(const mmfb_ln_args& a, cudaStream_t s) {
   return launch_ok("layernorm_fwd");
 }
 
+// Both backward kernels stride over the rows: a grid of at most two blocks per SM.
+static int ln_bwd_grid(int M) {
+  const int grid = (M + ROW_WARPS - 1) / ROW_WARPS, cap = num_sms() * 2;
+  return grid < cap ? grid : cap;
+}
+
+template <int NV, bool HAS_DX2, int ST>
+static int ln_bwd_stream(const mmfb_ln_args& a, cudaStream_t s) {
+  constexpr size_t smem = static_cast<size_t>(ROW_WARPS) * ST * (HAS_DX2 ? 3 : 2) * NV * 512 + ROW_WARPS * 256 * 4 +
+                          NV * 256 * 4 + 4096 + ROW_WARPS * ST * 8;
+  auto kern = ln_bwd_stream_kernel<NV, HAS_DX2, ST>;
+  static bool attr_set = false;  // per instantiation
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "cudaFuncSetAttribute(layernorm_bwd): %s", cudaGetErrorString(e));
+    attr_set = true;
+  }
+  MMFB_LAUNCH(kern, ln_bwd_grid(a.M), ROW_WARPS * 32, smem, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2, a.lddx2,
+              (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy, a.lddy, (bf16*)a.dz, a.lddz,
+              a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H);
+  return launch_ok("layernorm_bwd");
+}
+
 int ln_bwd(const mmfb_ln_args& a, cudaStream_t s) {
   int rc = check_rows(a.M, a.H, "layernorm_bwd");
   if (rc) return rc;
   if (!a.dx || !a.y || !a.mean || !a.rstd || !a.gamma) return set_error(MMFB_ERR_ARG, "layernorm_bwd: null pointer");
   if (a.drop_mask && !a.dz) return set_error(MMFB_ERR_ARG, "layernorm_bwd: dropout mask given without dz");
-  const int nv_ = (a.H + 255) / 256;
-  // read per call (not cached) so that one test process can run the variants back to back.
-  // default: the streaming single-pass kernel; MMFB_LN_BWD=lean / tile / pair select the others for A/B runs
-  const char* lean_env = getenv("MMFB_LN_BWD");
-  const bool lean = lean_env != nullptr && lean_env[0] == 'l';
-  const bool tile = lean_env != nullptr && lean_env[0] == 't';
-  if (tile && nv_ <= 4) {
-    const int64_t n_steps = (static_cast<int64_t>(a.M) + 3) / 4;
-#define LN_TILE(WPR, G)                                                                                                \
-  {                                                                                                                    \
-    int64_t want = (n_steps + (G) - 1) / (G);                                                                          \
-    int grid = static_cast<int>(want < num_sms() ? want : num_sms());                                                  \
-    if (grid < 1) grid = 1;                                                                                            \
-    if (a.dx2 != nullptr)                                                                                              \
-      MMFB_LAUNCH((ln_bwd_tile_kernel<WPR, G, true>), grid, (WPR) * (G) * 32, 0, s,                                               \
-          (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2, a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd,             \
-          (const bf16*)a.gamma, (bf16*)a.dy, a.lddy, (bf16*)a.dz, a.lddz, a.drop_mask, a.ldmask, a.drop_scale,         \
-          a.dgamma, a.dbeta, a.dbias, a.M, a.H);                                                                       \
-    else                                                                                                               \
-      MMFB_LAUNCH((ln_bwd_tile_kernel<WPR, G, false>), grid, (WPR) * (G) * 32, 0, s,                                              \
-          (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2, a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd,             \
-          (const bf16*)a.gamma, (bf16*)a.dy, a.lddy, (bf16*)a.dz, a.lddz, a.drop_mask, a.ldmask, a.drop_scale,         \
-          a.dgamma, a.dbeta, a.dbias, a.M, a.H);                                                                       \
+  const bool wide = a.H > 1024;
+  // dz is written only when it is a separate output; only the wide kernel reads gamma as 16-byte vectors
+  const void* dz = (a.drop_mask || a.dz != a.dy) ? a.dz : nullptr;
+  rc = check_aligned("layernorm_bwd", a.M, {{a.dx, a.lddx, "dx"}, {a.dx2, a.lddx2, "dx2"}, {a.y, a.ldy, "y"},
+                                            {a.dy, a.lddy, "dy"}, {dz, a.lddz, "dz"}, {wide ? a.gamma : nullptr, 0, "gamma"}});
+  if (rc) return rc;
+  if (wide) {
+    MMFB_LAUNCH(ln_bwd_kernel, ln_bwd_grid(a.M), ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2,
+                a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy, a.lddy, (bf16*)a.dz,
+                a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H);
+    return launch_ok("layernorm_bwd");
   }
-    if (nv_ <= 1) LN_TILE(1, 12) else if (nv_ == 2) LN_TILE(2, 6) else if (nv_ == 3) LN_TILE(3, 4) else LN_TILE(4, 3)
-#undef LN_TILE
-    return launch_ok("layernorm_bwd(tile)");
-  }
-  const bool stream = lean_env == nullptr || lean_env[0] == 's';
-  // bulk copies need 16-byte aligned rows (H % 8 == 0 is already required; leading dimensions in elements % 8 too)
-  if (stream && nv_ <= 4 && a.lddx % 8 == 0 && a.ldy % 8 == 0 && (a.dx2 == nullptr || a.lddx2 % 8 == 0)) {
-    int grid = (a.M + ROW_WARPS - 1) / ROW_WARPS;
-    const int cap = num_sms() * 2;
-    if (grid > cap) grid = cap;
-#define LN_STREAM(NV, DX2_, ST_)                                                                                      \
-  {                                                                                                                    \
-    constexpr size_t smem_ = static_cast<size_t>(ROW_WARPS) * (ST_) * ((DX2_) ? 3 : 2) * (NV) * 512 +                  \
-                             ROW_WARPS * 256 * 4 + (NV) * 256 * 4 + 4096 + ROW_WARPS * (ST_) * 8;                      \
-    static bool attr_done = false;                                                                                     \
-    if (!attr_done) {                                                                                                  \
-      cudaFuncSetAttribute(ln_bwd_stream_kernel<NV, DX2_, ST_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_); \
-      attr_done = true;                                                                                                \
-    }                                                                                                                  \
-    MMFB_LAUNCH((ln_bwd_stream_kernel<NV, DX2_, ST_>), grid, ROW_WARPS * 32, smem_, s, (const bf16*)a.dx, a.lddx,      \
-                (const bf16*)a.dx2, a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma,            \
-                (bf16*)a.dy, a.lddy, (bf16*)a.dz, a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta,      \
-                a.dbias, a.M, a.H);                                                                                    \
-  }
-    if (a.dx2 != nullptr) {
-      if (nv_ <= 1) LN_STREAM(1, true, 3) else if (nv_ == 2) LN_STREAM(2, true, 3) else if (nv_ == 3) LN_STREAM(3, true, 2) else LN_STREAM(4, true, 2)
-    } else {
-      if (nv_ <= 1) LN_STREAM(1, false, 4) else if (nv_ == 2) LN_STREAM(2, false, 4) else if (nv_ == 3) LN_STREAM(3, false, 3) else LN_STREAM(4, false, 2)
-    }
-#undef LN_STREAM
-    return launch_ok("layernorm_bwd(stream)");
-  }
-  if ((lean || stream) && nv_ <= 4) {
-    int grid = (a.M + ROW_WARPS - 1) / ROW_WARPS;
-    const int cap = num_sms() * 2;      // two resident blocks per SM, rows strided over them
-    if (grid > cap) grid = cap;
-#define LN_LEAN(NV)                                                                                                  \
-  MMFB_LAUNCH((ln_bwd_lean_kernel<NV, DX2>), grid, ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2, a.lddx2,       \
-                                                         (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, \
-                                                         (bf16*)a.dy, a.lddy, (bf16*)a.dz, a.lddz, a.drop_mask,         \
-                                                         a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H)
-#define LN_LEAN2(DX2_)                                                                                              \
-  { constexpr bool DX2 = DX2_;                                                                                       \
-    if (nv_ <= 1) LN_LEAN(1); else if (nv_ == 2) LN_LEAN(2); else if (nv_ == 3) LN_LEAN(3); else LN_LEAN(4); }
-    if (a.dx2 != nullptr) LN_LEAN2(true) else LN_LEAN2(false)
-#undef LN_LEAN2
-#undef LN_LEAN
-    return launch_ok("layernorm_bwd(lean)");
-  }
-  if (nv_ <= 4) {
-    // two kernels: a light row kernel (dy, dz) at high occupancy, then coalesced column statistics
-    const bool need_dz_buf = (a.drop_mask != nullptr) || (a.dz != nullptr && a.dz != a.dy);
-    const int rgrid = (a.M + ROW_WARPS - 1) / ROW_WARPS;
-#define LN_ROWS(NV)                                                                                              \
-  MMFB_LAUNCH(ln_bwd_rows_kernel<NV>, rgrid, ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2, a.lddx2, \
-                                                          (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, \
-                                                          (bf16*)a.dy, a.lddy, (bf16*)a.dz, a.lddz, a.drop_mask, a.ldmask, \
-                                                          a.drop_scale, a.M, a.H)
-    if (nv_ <= 1) LN_ROWS(1); else if (nv_ == 2) LN_ROWS(2); else if (nv_ == 3) LN_ROWS(3); else LN_ROWS(4);
-#undef LN_ROWS
-    rc = launch_ok("layernorm_bwd(rows)");
-    if (rc) return rc;
-    if (a.dgamma || a.dbeta || a.dbias) {
-      const void* dzp = need_dz_buf ? a.dz : a.dy;
-      const int64_t lddz = need_dz_buf ? a.lddz : a.lddy;
-      if (a.dbias && !dzp) return set_error(MMFB_ERR_ARG, "layernorm_bwd: dbias needs dy or dz to be materialised");
-      dim3 cgrid((a.H + 255) / 256, 1);
-      int rb = (a.M + 63) / 64;
-      const int cap2 = (num_sms() * 4 + cgrid.x - 1) / cgrid.x;
-      cgrid.y = rb < cap2 ? rb : cap2;
-      if (cgrid.y < 1) cgrid.y = 1;
-      MMFB_LAUNCH(ln_bwd_cols_kernel, cgrid, 256, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2, a.lddx2, (const bf16*)a.y, a.ldy,
-                                               a.mean, a.rstd, (const bf16*)dzp, lddz, a.dgamma, a.dbeta, a.dbias, a.M, a.H);
-      return launch_ok("layernorm_bwd(cols)");
-    }
-    return MMFB_OK;
-  }
-  int grid = (a.M + ROW_WARPS - 1) / ROW_WARPS;
-  const int cap = num_sms() * 2;
-  if (grid > cap) grid = cap;
-#define LN_BWD(NV)                                                                                              \
-  MMFB_LAUNCH(ln_bwd_kernel<NV>, grid, ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2, a.lddx2,       \
-                                                    (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, \
-                                                    (bf16*)a.dy, a.lddy, (bf16*)a.dz, a.lddz, a.drop_mask,         \
-                                                    a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H)
-  const int nv = (a.H + 255) / 256;
-  if (nv <= 1) LN_BWD(1); else if (nv == 2) LN_BWD(2); else if (nv == 3) LN_BWD(3); else if (nv == 4) LN_BWD(4); else LN_BWD(8);
-#undef LN_BWD
-  return launch_ok("layernorm_bwd");
+  // ln_bwd_stream<NV, HAS_DX2, ST> indexed by [dx2 given][NV - 1]; NV = 256-column slabs per row, ST = ring depth
+  static int (*const stream[2][4])(const mmfb_ln_args&, cudaStream_t) = {
+      {ln_bwd_stream<1, false, 4>, ln_bwd_stream<2, false, 4>, ln_bwd_stream<3, false, 3>, ln_bwd_stream<4, false, 2>},
+      {ln_bwd_stream<1, true, 3>, ln_bwd_stream<2, true, 3>, ln_bwd_stream<3, true, 2>, ln_bwd_stream<4, true, 2>}};
+  return stream[a.dx2 != nullptr][(a.H + 255) / 256 - 1](a, s);
 }
 
 int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s) {

@@ -10,9 +10,11 @@ def rel(a, b):
     return ((a.double() - b.double()).norm() / b.double().norm().clamp_min(1e-12)).item()
 
 
-@pytest.mark.parametrize("M,H", [(1000, 768), (333, 1024), (50, 64), (4000, 256)])
+@pytest.mark.parametrize("M,H", [(1000, 768), (333, 1024), (50, 64), (4000, 256), (7, 512), (50, 128), (5000, 256),
+                                 (37848, 768), (333, 1280), (100, 2048)])
+@pytest.mark.parametrize("with_dx2", [False, True])
 @pytest.mark.parametrize("with_drop", [False, True])
-def test_layernorm_fwd_bwd(M, H, with_drop):
+def test_layernorm_fwd_bwd(M, H, with_dx2, with_drop):
     from mmf_b200 import functional as F
     torch.manual_seed(M + H)
     y = torch.randn(M, H, device="cuda").to(torch.bfloat16)
@@ -25,7 +27,9 @@ def test_layernorm_fwd_bwd(M, H, with_drop):
     assert rel(x, ref) < 1e-2
     dx = torch.randn(M, H, device="cuda").to(torch.bfloat16)
     dx2 = torch.randn(M, H, device="cuda").to(torch.bfloat16)
-    ref.backward(dx.float() + dx2.float())
+    ref.backward(dx.float() + dx2.float() if with_dx2 else dx.float())
+    if not with_dx2:
+        dx2 = None
     dgamma = torch.zeros(H, device="cuda"); dbeta = torch.zeros(H, device="cuda"); dbias = torch.zeros(H, device="cuda")
     bits = scale = None
     if with_drop:
@@ -37,12 +41,36 @@ def test_layernorm_fwd_bwd(M, H, with_drop):
     dz_ref = yf.grad * keep.float() / 0.9 if with_drop else yf.grad
     assert rel(dz, dz_ref) < 1e-2
     assert rel(dgamma, gf.grad) < 1e-2 and rel(dbeta, bf.grad) < 1e-2
-    # bias gradient = column sum of dz: the default kernel pair sums the STORED bf16 dz, the single-pass variants
-    # (MMFB_LN_BWD=lean / tile) sum the fp32 values before rounding - both within bf16 rounding of each other
+    # bias gradient = column sum of dz: the streaming kernel (H <= 1024) sums the STORED bf16 dz when there is dropout,
+    # otherwise, and in the wide kernel, the fp32 values before rounding are summed - within bf16 rounding of each other
     assert rel(dbias, dz.float().sum(0)) < 4e-3 and rel(dbias, dz_ref.sum(0)) < 1e-2
     # accumulation semantics: a second call adds
     F.layernorm_bwd(dx, y, mean, rstd, g, dgamma, dbeta, dbias=dbias, dx2=dx2, drop_mask=bits, drop_scale=scale or 1.0)
     assert rel(dgamma, 2 * gf.grad) < 1e-2
+
+
+@pytest.mark.parametrize("H", [768, 2048])
+def test_layernorm_rejects_unaligned_rows(H):
+    """Both LayerNorm kernels read rows as 16-byte vectors: a row stride that is not a multiple of 8 elements is refused
+    with ValueError before anything is launched."""
+    from mmf_b200 import functional as F, lib
+    M = 64
+    padded = torch.randn(M, H + 4, device="cuda").to(torch.bfloat16)
+    y_bad = padded[:, :H]
+    y = y_bad.contiguous()
+    g = torch.ones(H, device="cuda", dtype=torch.bfloat16)
+    b = torch.zeros(H, device="cuda", dtype=torch.bfloat16)
+    _, mean, rstd = F.layernorm_fwd(y, g, b)
+    dx = torch.randn(M, H, device="cuda").to(torch.bfloat16)
+    dgamma, dbeta = torch.zeros(H, device="cuda"), torch.zeros(H, device="cuda")
+    n0 = lib.launch_count()
+    with pytest.raises(ValueError, match="ldy"):
+        F.layernorm_fwd(y_bad, g, b)
+    with pytest.raises(ValueError, match="ldy"):
+        F.layernorm_bwd(dx, y_bad, mean, rstd, g, dgamma, dbeta)
+    with pytest.raises(ValueError, match="lddx"):
+        F.layernorm_bwd(y_bad, y, mean, rstd, g, dgamma, dbeta)
+    assert lib.launch_count() == n0
 
 
 def test_colsum_and_cast():

@@ -1,14 +1,12 @@
 #!/usr/bin/env python
 """Kernel-level timings at the bench shapes (BASELINE.json configs[1], batch 166): every kernel of one fusion layer timed
 ALONE with CUDA events on the launching stream, L2 flushed between launches (a 160 MB buffer is zeroed), mean of N after
-warm-up.  Variants that are selected per call by an environment switch are timed side by side in one process; library
-variants (MMFB_LIB) need one process each:  MMFB_LIB=.../libmmfb200_x2.so python tools/kbench.py --only gemm
+warm-up.  Another build of the library is timed in a process of its own:  MMFB_LIB=<path> python tools/kbench.py --only ln
 
     python tools/kbench.py [--batch 166] [--iters 20] [--only attn,ln,gemm,rows] [--json out.json]
 
-The whole-step A/B (tools/ab.py) cannot resolve +-1 % effects: the part sits at its 1 kW power cap and the SM clock moves
-+-4 % between runs; these isolated timings do.  Algorithmic FLOPs / bytes per launch are printed with each kernel so the
-roofline fraction is on the same line (peaks from MEASURED_PEAKS.json).
+Algorithmic FLOPs / bytes per launch are printed with each kernel so the roofline fraction is on the same line (peaks
+from MEASURED_PEAKS.json).
 """
 import argparse
 import json
@@ -47,11 +45,7 @@ def main():
     flush = torch.empty(160 << 20, dtype=torch.uint8, device=dev)
     rows = []
 
-    def timeit(name, fn, flops=None, nbytes=None, env=None):
-        old = {}
-        for k, v in (env or {}).items():
-            old[k] = os.environ.get(k)
-            os.environ[k] = v
+    def timeit(name, fn, flops=None, nbytes=None):
         try:
             for _ in range(3):
                 fn()
@@ -65,16 +59,10 @@ def main():
                 e1.record()
                 torch.cuda.synchronize()
                 ts.append(e0.elapsed_time(e1) * 1e3)
-        except Exception as e:      # a variant that traps must not end the whole run
+        except Exception as e:      # a kernel that fails must not end the whole run
             print("%-58s FAILED: %s" % (name, str(e)[:120]))
             rows.append({"kernel": name, "failed": str(e)[:200]})
             return None
-        finally:
-            for k, v in old.items():
-                if v is None:
-                    os.environ.pop(k, None)
-                else:
-                    os.environ[k] = v
         us = statistics.mean(ts)
         extra = ""
         row = {"kernel": name, "us": us, "us_min": min(ts)}
@@ -106,12 +94,12 @@ def main():
         b_fwd = M * 3 * H * 2 + M * H * 2 + M * H * 4 + bits.numel() * 4
         b_bwd = M * 3 * H * 2 * 2 + M * H * 2 + bits.numel() * 4
         timeit("attention_fwd", lambda: F.attention_fwd(q, k, v, B, heads, S, S, mask, bits, 1 / 0.9, save_lo=True),
-               f_fwd, b_fwd, {})
+               f_fwd, b_fwd)
         ctx, lse2, c32 = F.attention_fwd(q, k, v, B, heads, S, S, mask, bits, 1 / 0.9, save_lo=True)
         dq = torch.empty_like(qkv)
         timeit("attention_bwd (+delta)",
                lambda: F.attention_bwd(dctx, q, k, v, ctx, lse2, B, heads, S, S, mask, bits, 1 / 0.9, dq=dq[:, :H],
-                                       dk=dq[:, H:2 * H], dv=dq[:, 2 * H:], ctx_lo=c32), f_bwd, b_bwd, {})
+                                       dk=dq[:, H:2 * H], dv=dq[:, 2 * H:], ctx_lo=c32), f_bwd, b_bwd)
         timeit("dropout_bits attention [B,h,S,S]", lambda: F.dropout_bits((B, heads, S), S, 0.1, 7, 0, dev), None, bits.numel() * 4)
         del qkv, dctx, dq, ctx, c32
 
@@ -123,10 +111,8 @@ def main():
         bits = F.dropout_bits((M,), H, 0.1, 1, 0, dev)
         dg, db_, dbias = (torch.zeros(H, device=dev) for _ in range(3))
         nb = M * (8.0 * H + H / 8.0 + 8.0)
-        for tag, env in (("default single pass", {}), ("MMFB_LN_BWD=pair", {"MMFB_LN_BWD": "pair"}), ("MMFB_LN_BWD=tile", {"MMFB_LN_BWD": "tile"}),
-                         ("MMFB_LN_BWD=stream", {"MMFB_LN_BWD": "stream"}), ("MMFB_LN_BWD=lean", {"MMFB_LN_BWD": "lean"})):
-            timeit("layernorm_bwd +dropout +dgamma/dbeta/dbias [%s]" % tag,
-                   lambda: F.layernorm_bwd(dx, y, mean, rstd, g, dg, db_, dbias=dbias, drop_mask=bits, drop_scale=1 / 0.9), None, nb, env)
+        timeit("layernorm_bwd +dropout +dgamma/dbeta/dbias",
+               lambda: F.layernorm_bwd(dx, y, mean, rstd, g, dg, db_, dbias=dbias, drop_mask=bits, drop_scale=1 / 0.9), None, nb)
         timeit("layernorm_fwd", lambda: F.layernorm_fwd(y, g, torch.zeros_like(g)), None, M * (4.0 * H + 8))
         big = torch.randn(M, 3 * H, device=dev).to(bf)
         acc = torch.zeros(3 * H, device=dev)
