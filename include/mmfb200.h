@@ -73,7 +73,8 @@ int mmfb_gemm(const mmfb_gemm_args* args, mmfb_stream stream);
  *   BertBiAttention.forward vilbert.py:421-461 (cross: q from one stream, k/v from the other).
  * q [B*Sq, ldq], k/v [B*Skv, ld*]: bf16, head h in columns [h*head_dim, (h+1)*head_dim); usually three
  * column slices of one fused projection buffer.  mask: additive fp32 [B, Skv] (the reference's
- * [B,1,1,Skv] tensor) or NULL.  lse2 [B, heads, Sq] fp32 receives the log2-domain row log-sum-exp
+ * [B,1,1,Skv] tensor) or NULL; values below -10000 (finfo(dtype).min, -inf) act exactly like -10000, so a fully
+ * masked row gives the softmax of its raw scores and stays finite.  lse2 [B, heads, Sq] fp32 receives the log2-domain row log-sum-exp
  * (saved for backward).  drop_mask: keep bits [B, heads, Sq, ceil(Skv/32)] (bit kv%32) or NULL.
  * Limits: head_dim 64 or 128; Skv <= 384 (d=64) / 256 (d=128) - MMF's path has S <= 324. */
 typedef struct {
@@ -173,7 +174,8 @@ int mmfb_gelu_bwd(const void* dh, const void* u, void* du, int64_t n, mmfb_strea
 /* Cross-entropy over vocabulary-sized rows, forward and backward in ONE kernel: for every row m of the bf16 logits [M, V]
  * (row stride ldl, V % 8 == 0) with label[m] != ignore_index,  loss_m = logsumexp(z_m) - z_m[label[m]]  is added to
  * *loss_sum (and stored in row_loss[m] when given) and the row is OVERWRITTEN by
- * d(logits) = (softmax(z_m) - onehot(label[m])) * grad_scale;  ignored rows are overwritten by zeros.
+ * d(logits) = (softmax(z_m) - onehot(label[m])) * grad_scale;  ignored rows are overwritten by zeros.  A label outside
+ * [0, V) that is not ignore_index is treated like ignore_index: zero gradient, row_loss 0, nothing added to *loss_sum.
  * Replaces CrossEntropyLoss(ignore_index=-1) over prediction_scores.view(-1, vocab_size) of the masked-LM heads
  * (mmf/models/visual_bert.py:215,269-277; mmf/models/transformers/heads/mlm.py:46-97) inside the chunked
  * linear + cross-entropy head: the full [tokens, 30522] logits tensor never exists in HBM. */

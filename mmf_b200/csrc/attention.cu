@@ -1,8 +1,8 @@
 // Fused multi-head (self / cross) attention for the fusion block, forward and backward (sm_90a).
 //
 // Reference semantics (mmf/modules/hf_layers.py:182-210; mmf/models/vilbert.py:81-103, 421-461):
-//     scores = Q K^T / sqrt(d) + M        M = additive mask [B, Skv] (0 / -10000), NOT -inf
-//     probs  = dropout(softmax(scores))   a fully masked row becomes uniform, never NaN
+//     scores = Q K^T / sqrt(d) + M        M = additive mask [B, Skv] (0 / -10000); lower values count as -10000
+//     probs  = dropout(softmax(scores))   a fully masked row is the softmax of its raw scores, never NaN
 //     ctx    = probs V, heads merged back to [B, Sq, h*d]
 //
 // Every kernel works on 64-row tiles of one (batch, head): four warps, each owning 16 rows of the resident tile, and a
@@ -31,6 +31,13 @@ namespace mmfb {
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr int AT_ROWS = 64;       // rows of every staged tile
 constexpr int AT_THREADS = 128;   // four warps x 16 rows
+
+// An additive mask value as staged in shared memory (log2 domain).  Values below -10000 (HF's finfo(dtype).min, -inf)
+// are clamped to -10000 first: their product with log2(e) would be -inf in fp32, and a query whose first key block is
+// fully masked would then compute -inf - (-inf) = NaN in the online softmax.  -10000 is the reference's own convention
+// and stays finite, so such a row keeps a finite log-sum-exp (softmax of its raw scores).  Masks at or above -10000 are
+// unchanged bit for bit.
+__device__ __forceinline__ float staged_mask(float m) { return fmaxf(m, -10000.0f) * LOG2E; }
 
 // byte offset of the 16-byte chunk holding column c (a multiple of 8) of row r in a staged tile: 64-column panels of
 // ROWS x 128 B, SWIZZLE_128B (chunk index XOR row % 8), as written by a TMA box {64, ROWS}
@@ -148,7 +155,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
   // additive mask in the log2 domain; padded key columns get -inf so that exp2 yields exactly 0
   for (int i = threadIdx.x; i < NKB * AT_ROWS; i += AT_THREADS)
-    sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + i] * LOG2E : 0.0f) : -INFINITY;
+    sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
   __syncthreads();
 
   const int g = lane >> 2, t4 = lane & 3;
@@ -315,7 +322,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     }
   }
   for (int i = threadIdx.x; i < NKB * AT_ROWS; i += AT_THREADS)
-    sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + i] * LOG2E : 0.0f) : -INFINITY;
+    sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
   __syncthreads();
 
   const int g = lane >> 2, t4 = lane & 3;
@@ -439,7 +446,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   }
   for (int i = threadIdx.x; i < AT_ROWS; i += AT_THREADS) {
     const int kv = k0 + i;
-    sMask[i] = (kv < p.Skv) ? (p.mask != nullptr ? p.mask[static_cast<int64_t>(b) * p.Skv + kv] * LOG2E : 0.0f) : -INFINITY;
+    sMask[i] = (kv < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + kv]) : 0.0f) : -INFINITY;
   }
   __syncthreads();
 
