@@ -99,6 +99,19 @@ typedef struct {
 int mmfb_attention_fwd(const mmfb_attn_args* args, mmfb_stream stream);
 int mmfb_attention_bwd(const mmfb_attn_args* args, mmfb_stream stream);
 
+/* Variable-length (packed) self-attention: padded tokens are removed before the call, so no work is spent on them.
+ * cu_seqlens: int32 [B+1] on the DEVICE, a non-decreasing prefix sum with cu_seqlens[0] = 0 and cu_seqlens[B] = total;
+ * sample b owns the packed rows [cu_seqlens[b], cu_seqlens[b+1]) of every row buffer (queries and keys share it).
+ * A sample of length 0 is legal: nothing is computed or written for it.  The lengths are never read on the host.
+ *   args->B = samples; args->Sq = args->Skv = max_len >= every length (sets the grid; rows past max_len are not used);
+ *   args->mask must be NULL (MMFB_ERR_ARG otherwise): packing has already removed the masked keys;
+ *   q, k, v, ctx, ctx_lo, dctx, dq, dk, dv: [total, ld] rows, same head-column layout as mmfb_attention_fwd;
+ *   lse2, delta: fp32 [heads, total];
+ *   drop_mask: keep bits int32 [heads, total, ceil(max_len/32)], bit kv%32 of word kv/32 for key kv WITHIN the sample.
+ * Limits: head_dim 64 or 128; max_len <= 384 (d=64) / 256 (d=128).  total = 0 returns MMFB_OK without a launch. */
+int mmfb_attention_varlen_fwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream);
+int mmfb_attention_varlen_bwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream);
+
 /* LayerNorm over the last dimension (eps 1e-12 on this path), one warp per row.
  * fwd: x = LN(y)*gamma + beta, optional dropout on x (embeddings), saves mean / rstd (fp32 [M]).
  * bwd: dy = dLN(dx (+dx2)); dz = dropout-backward(dy) for the dense branch that fed y = dropout(dense)+resid;

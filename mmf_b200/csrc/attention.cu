@@ -21,6 +21,9 @@
 //   dq kernel : CTA owns 64 query rows, loops over key blocks:    dQ = scale * dS K
 //   dkv kernel: CTA owns 64 key rows, loops over query blocks:    dV = P^T dO,  dK = scale * dS^T Q
 //               (computed as S^T = K Q^T and dP^T = V dO^T, so the key rows stay the rows of every register tile)
+// VARLEN instantiations (packed self-attention, include/mmfb200.h): the samples' rows are packed back to back, so a tile
+// may run into the next sample; those rows are masked (keys), not stored (queries) or given P = 0 (dk/dv), and every CTA
+// stays within its own sample's blocks.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -115,10 +118,27 @@ struct AttnFwdDev {
   int W;
   float dscale;           // 1/(1-p)
   float scale2;           // log2(e)/sqrt(d)
+  const int* cu;          // VARLEN: [B+1] first packed row of every sample (Sq = Skv = max_len)
+  int total;              // VARLEN: packed rows
 };
 
-// grid (query tiles, heads, batch); smem: Q tile, two stages of (K block, V block), the key mask (log2 domain)
-template <int D>
+// VARLEN: sample b owns the packed rows [cu[b], cu[b+1]) of every row buffer (clamped to `total` and to max_len rows);
+// returns that range as (first row, length).  Read after griddep_wait, like every other global read.
+__device__ __forceinline__ int2 varlen_rows(const int* cu, int b, int total, int max_len) {
+  const int s0 = __ldg(cu + b);
+  return make_int2(s0, min(min(__ldg(cu + b + 1), total) - s0, max_len));
+}
+
+// PACKED_ROW: tile row coordinate (dense: within batch b; packed: sample b starts at row seq0).
+// HEAD_ROW: first row of (batch-head bh, head h) in lse2 / delta / the keep bits: [B, H, Sq] dense, [H, total] packed.  A macro so
+// that the dense kernels keep the exact expressions (and code) they had before the packed mode existed.
+#define PACKED_ROW(r) (VARLEN ? seq0 + (r) : (r))
+#define HEAD_ROW(bh) (VARLEN ? static_cast<int64_t>(h) * p.total + seq0 : static_cast<int64_t>(bh) * p.Sq)
+
+// grid (query tiles, heads, batch); smem: Q tile, two stages of (K block, V block), the key mask (log2 domain).
+// VARLEN: packed self-attention (no additive mask); the tensor maps span the packed rows with a batch extent of 1, tiles
+// load at row cu[b] + block * 64, and rows past the end of the sample (the next sample's rows) are masked / not stored.
+template <int D, bool VARLEN>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, AttnFwdDev p) {
@@ -144,18 +164,33 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
   __syncthreads();
   griddep_wait();
+  // dense: the sample's rows start at row 0 of batch b; VARLEN: at packed row seq0 of the single batch
+  int seq0 = 0, len = p.Skv, nkb = NKB;
+  if constexpr (VARLEN) {
+    const int2 r = varlen_rows(p.cu, b, p.total, p.Skv);
+    seq0 = r.x;
+    len = r.y;
+    if (q0 >= len) return;                     // no query of this tile exists (empty samples: every tile)
+    nkb = (len + AT_ROWS - 1) / AT_ROWS;       // the sample's own key blocks only
+  }
+  const int tb = VARLEN ? 0 : b;
   if (threadIdx.x == 0) {
     mbar_expect_tx(&bars[0], TB);
-    load_tile<D, AT_ROWS>(sQ, &tmQ, &bars[0], h * D, q0, b);
-    for (int kb = 0; kb < 2 && kb < NKB; ++kb) {
+    load_tile<D, AT_ROWS>(sQ, &tmQ, &bars[0], h * D, PACKED_ROW(q0), tb);
+    for (int kb = 0; kb < 2 && kb < nkb; ++kb) {
       mbar_expect_tx(&bars[1 + kb], 2 * TB);
-      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, kb * AT_ROWS, b);
-      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, kb * AT_ROWS, b);
+      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, PACKED_ROW(kb * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, PACKED_ROW(kb * AT_ROWS), tb);
     }
   }
-  // additive mask in the log2 domain; padded key columns get -inf so that exp2 yields exactly 0
-  for (int i = threadIdx.x; i < NKB * AT_ROWS; i += AT_THREADS)
-    sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
+  // additive mask in the log2 domain; padded key columns (VARLEN: keys past the sample) get -inf so that exp2 yields
+  // exactly 0
+  for (int i = threadIdx.x; i < nkb * AT_ROWS; i += AT_THREADS) {
+    if constexpr (VARLEN)
+      sMask[i] = (i < len) ? 0.0f : -INFINITY;
+    else
+      sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
+  }
   __syncthreads();
 
   const int g = lane >> 2, t4 = lane & 3;
@@ -168,12 +203,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     const int q = q0 + r0 + g + hr * 8;
-    if (p.dmask != nullptr && q < p.Sq) dm[hr] = p.dmask + (static_cast<int64_t>(b * p.H + h) * p.Sq + q) * p.W;
+    if (p.dmask != nullptr && q < (VARLEN ? len : p.Sq)) dm[hr] = p.dmask + (HEAD_ROW(b * p.H + h) + q) * p.W;
   }
   mbar_wait(&bars[0], 0);
   const uint32_t uQ = smem_u32(sQ);
 
-  for (int kb = 0; kb < NKB; ++kb) {
+  for (int kb = 0; kb < nkb; ++kb) {
     const int st = kb & 1;
     mbar_wait(&bars[1 + st], (kb >> 1) & 1);
     const uint32_t uK = smem_u32(sKV + 2 * st * TB), uV = uK + TB;
@@ -235,10 +270,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     // proxy) that thread 0 issues next; a barrier alone does not order the two proxies
     fence_proxy_async();
     __syncthreads();
-    if (threadIdx.x == 0 && kb + 2 < NKB) {
+    if (threadIdx.x == 0 && kb + 2 < nkb) {
       mbar_expect_tx(&bars[1 + st], 2 * TB);
-      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, (kb + 2) * AT_ROWS, b);
-      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, (kb + 2) * AT_ROWS, b);
+      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, PACKED_ROW((kb + 2) * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, PACKED_ROW((kb + 2) * AT_ROWS), tb);
     }
   }
 
@@ -248,11 +283,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const int q = q0 + r0 + g + hr * 8;
-    if (q >= p.Sq) continue;
-    if (t4 == 0) p.lse2[static_cast<int64_t>(b * p.H + h) * p.Sq + q] = mrow[hr] + log2f(l);
+    if (q >= (VARLEN ? len : p.Sq)) continue;
+    if (t4 == 0) p.lse2[HEAD_ROW(b * p.H + h) + q] = mrow[hr] + log2f(l);
     const float inv = p.dscale / l;
-    bf16* dst = p.ctx + (static_cast<int64_t>(b) * p.Sq + q) * p.ldo + h * D;
-    bf16* dlo = p.ctx_lo != nullptr ? p.ctx_lo + (static_cast<int64_t>(b) * p.Sq + q) * (p.H * D) + h * D : nullptr;
+    const int64_t row = VARLEN ? static_cast<int64_t>(seq0) + q : static_cast<int64_t>(b) * p.Sq + q;
+    bf16* dst = p.ctx + row * p.ldo + h * D;
+    bf16* dlo = p.ctx_lo != nullptr ? p.ctx_lo + row * (p.H * D) + h * D : nullptr;
 #pragma unroll
     for (int i = 0; i < DT; ++i) {
       const int c = i * 8 + 2 * t4;
@@ -280,10 +316,12 @@ struct AttnBwdDev {
   float dscale, scale, scale2;
   bf16* out0; int64_t ld0;   // dq (dq kernel) / dk (dkv kernel)
   bf16* out1; int64_t ld1;   // dv (dkv kernel)
+  const int* cu;             // VARLEN, as in AttnFwdDev
+  int total;
 };
 
-// dQ for 64 query rows.  smem: Q, dO tiles; two stages of (K block, V block)
-template <int D, bool DROP>
+// dQ for 64 query rows.  smem: Q, dO tiles; two stages of (K block, V block).  VARLEN as in the forward.
+template <int D, bool DROP, bool VARLEN>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, AttnBwdDev p) {
@@ -311,18 +349,31 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   }
   __syncthreads();
   griddep_wait();
+  int seq0 = 0, len = p.Skv, nkb = NKB;
+  if constexpr (VARLEN) {
+    const int2 r = varlen_rows(p.cu, b, p.total, p.Skv);
+    seq0 = r.x;
+    len = r.y;
+    if (q0 >= len) return;
+    nkb = (len + AT_ROWS - 1) / AT_ROWS;
+  }
+  const int tb = VARLEN ? 0 : b;
   if (threadIdx.x == 0) {
     mbar_expect_tx(&bars[0], 2 * TB);
-    load_tile<D, AT_ROWS>(sQ, &tmQ, &bars[0], h * D, q0, b);
-    load_tile<D, AT_ROWS>(sdO, &tmdO, &bars[0], h * D, q0, b);
-    for (int kb = 0; kb < 2 && kb < NKB; ++kb) {
+    load_tile<D, AT_ROWS>(sQ, &tmQ, &bars[0], h * D, PACKED_ROW(q0), tb);
+    load_tile<D, AT_ROWS>(sdO, &tmdO, &bars[0], h * D, PACKED_ROW(q0), tb);
+    for (int kb = 0; kb < 2 && kb < nkb; ++kb) {
       mbar_expect_tx(&bars[1 + kb], 2 * TB);
-      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, kb * AT_ROWS, b);
-      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, kb * AT_ROWS, b);
+      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, PACKED_ROW(kb * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, PACKED_ROW(kb * AT_ROWS), tb);
     }
   }
-  for (int i = threadIdx.x; i < NKB * AT_ROWS; i += AT_THREADS)
-    sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
+  for (int i = threadIdx.x; i < nkb * AT_ROWS; i += AT_THREADS) {
+    if constexpr (VARLEN)
+      sMask[i] = (i < len) ? 0.0f : -INFINITY;
+    else
+      sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
+  }
   __syncthreads();
 
   const int g = lane >> 2, t4 = lane & 3;
@@ -333,10 +384,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     const int q = q0 + r0 + g + hr * 8;
-    const bool ok = q < p.Sq;
-    lse[hr] = ok ? p.lse2[bh * p.Sq + q] : INFINITY;      // rows past the sequence: P = 0
-    dlt[hr] = ok ? p.delta[bh * p.Sq + q] : 0.0f;
-    if (DROP && ok) dm[hr] = p.dmask + (bh * p.Sq + q) * p.W;
+    const bool ok = q < (VARLEN ? len : p.Sq);
+    lse[hr] = ok ? p.lse2[HEAD_ROW(bh) + q] : INFINITY;      // rows past the sequence: P = 0
+    dlt[hr] = ok ? p.delta[HEAD_ROW(bh) + q] : 0.0f;
+    if (DROP && ok) dm[hr] = p.dmask + (HEAD_ROW(bh) + q) * p.W;
   }
   float dq[DT][4];
 #pragma unroll
@@ -344,7 +395,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   mbar_wait(&bars[0], 0);
   const uint32_t uQ = smem_u32(sQ), udO = smem_u32(sdO);
 
-  for (int kb = 0; kb < NKB; ++kb) {
+  for (int kb = 0; kb < nkb; ++kb) {
     const int st = kb & 1;
     mbar_wait(&bars[1 + st], (kb >> 1) & 1);
     const uint32_t uK = smem_u32(sKV + 2 * st * TB), uV = uK + TB;
@@ -386,17 +437,18 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     mma_pb<D, 4, AT_ROWS>(dq, sf, uK, lane);
     fence_proxy_async();
     __syncthreads();
-    if (threadIdx.x == 0 && kb + 2 < NKB) {
+    if (threadIdx.x == 0 && kb + 2 < nkb) {
       mbar_expect_tx(&bars[1 + st], 2 * TB);
-      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, (kb + 2) * AT_ROWS, b);
-      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, (kb + 2) * AT_ROWS, b);
+      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, PACKED_ROW((kb + 2) * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, PACKED_ROW((kb + 2) * AT_ROWS), tb);
     }
   }
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     const int q = q0 + r0 + g + hr * 8;
-    if (q >= p.Sq) continue;
-    bf16* dst = p.out0 + (static_cast<int64_t>(b) * p.Sq + q) * p.ld0 + h * D;
+    if (q >= (VARLEN ? len : p.Sq)) continue;
+    const int64_t row = VARLEN ? static_cast<int64_t>(seq0) + q : static_cast<int64_t>(b) * p.Sq + q;
+    bf16* dst = p.out0 + row * p.ld0 + h * D;
 #pragma unroll
     for (int i = 0; i < DT; ++i)
       *reinterpret_cast<uint32_t*>(dst + i * 8 + 2 * t4) = pack_bf16x2(dq[i][hr * 2] * p.scale, dq[i][hr * 2 + 1] * p.scale);
@@ -404,8 +456,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 }
 
 // dK, dV for 64 key rows.  smem: K, V tiles; two stages of (Q block, dO block) of QB query rows.  The register tiles are
-// transposed products (rows = keys, columns = queries).
-template <int D, bool DROP, int QB>
+// transposed products (rows = keys, columns = queries).  VARLEN as in the forward; query rows past the end of the sample
+// take lse = +inf and delta = 0 (P = 0), like rows past Sq.
+template <int D, bool DROP, int QB, bool VARLEN>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO, AttnBwdDev p) {
@@ -434,19 +487,31 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   }
   __syncthreads();
   griddep_wait();
+  int seq0 = 0, len = p.Skv, nqb = NQB;
+  if constexpr (VARLEN) {
+    const int2 r = varlen_rows(p.cu, b, p.total, p.Skv);
+    seq0 = r.x;
+    len = r.y;
+    if (k0 >= len) return;                      // no key of this tile exists
+    nqb = (len + QB - 1) / QB;                  // the sample's own query blocks only
+  }
+  const int tb = VARLEN ? 0 : b;
   if (threadIdx.x == 0) {
     mbar_expect_tx(&bars[0], 2 * TB);
-    load_tile<D, AT_ROWS>(sK, &tmK, &bars[0], h * D, k0, b);
-    load_tile<D, AT_ROWS>(sV, &tmV, &bars[0], h * D, k0, b);
-    for (int qb = 0; qb < 2 && qb < NQB; ++qb) {
+    load_tile<D, AT_ROWS>(sK, &tmK, &bars[0], h * D, PACKED_ROW(k0), tb);
+    load_tile<D, AT_ROWS>(sV, &tmV, &bars[0], h * D, PACKED_ROW(k0), tb);
+    for (int qb = 0; qb < 2 && qb < nqb; ++qb) {
       mbar_expect_tx(&bars[1 + qb], 2 * QTB);
-      load_tile<D, QB>(sQd + 2 * qb * QTB, &tmQ, &bars[1 + qb], h * D, qb * QB, b);
-      load_tile<D, QB>(sQd + (2 * qb + 1) * QTB, &tmdO, &bars[1 + qb], h * D, qb * QB, b);
+      load_tile<D, QB>(sQd + 2 * qb * QTB, &tmQ, &bars[1 + qb], h * D, PACKED_ROW(qb * QB), tb);
+      load_tile<D, QB>(sQd + (2 * qb + 1) * QTB, &tmdO, &bars[1 + qb], h * D, PACKED_ROW(qb * QB), tb);
     }
   }
   for (int i = threadIdx.x; i < AT_ROWS; i += AT_THREADS) {
     const int kv = k0 + i;
-    sMask[i] = (kv < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + kv]) : 0.0f) : -INFINITY;
+    if constexpr (VARLEN)
+      sMask[i] = (kv < len) ? 0.0f : -INFINITY;
+    else
+      sMask[i] = (kv < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + kv]) : 0.0f) : -INFINITY;
   }
   __syncthreads();
 
@@ -465,7 +530,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   mbar_wait(&bars[0], 0);
   const uint32_t uK = smem_u32(sK), uV = smem_u32(sV);
 
-  for (int qb = 0; qb < NQB; ++qb) {
+  for (int qb = 0; qb < nqb; ++qb) {
     const int st = qb & 1;
     mbar_wait(&bars[1 + st], (qb >> 1) & 1);
     const uint32_t uQ = smem_u32(sQd + 2 * st * QTB), udO = uQ + QTB;
@@ -483,11 +548,11 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
         const int q = qb * QB + nt * 8 + 2 * t4 + j;
-        const bool ok = q < p.Sq;
-        const float lse = ok ? __ldg(p.lse2 + bh * p.Sq + q) : INFINITY;
-        const float dlt = ok ? __ldg(p.delta + bh * p.Sq + q) : 0.0f;
+        const bool ok = q < (VARLEN ? len : p.Sq);
+        const float lse = ok ? __ldg(p.lse2 + HEAD_ROW(bh) + q) : INFINITY;
+        const float dlt = ok ? __ldg(p.delta + HEAD_ROW(bh) + q) : 0.0f;
         uint32_t w = 0xFFFFFFFFu;
-        if (DROP && ok && k0 + r0 < p.Skv) w = __ldg(p.dmask + (bh * p.Sq + q) * p.W + kw);
+        if (DROP && ok && k0 + r0 < (VARLEN ? len : p.Skv)) w = __ldg(p.dmask + (HEAD_ROW(bh) + q) * p.W + kw);
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           const int e = hr * 2 + j;
@@ -506,18 +571,19 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     mma_pb<D, NT / 2, QB>(dk, sf, uQ, lane);
     fence_proxy_async();
     __syncthreads();
-    if (threadIdx.x == 0 && qb + 2 < NQB) {
+    if (threadIdx.x == 0 && qb + 2 < nqb) {
       mbar_expect_tx(&bars[1 + st], 2 * QTB);
-      load_tile<D, QB>(sQd + 2 * st * QTB, &tmQ, &bars[1 + st], h * D, (qb + 2) * QB, b);
-      load_tile<D, QB>(sQd + (2 * st + 1) * QTB, &tmdO, &bars[1 + st], h * D, (qb + 2) * QB, b);
+      load_tile<D, QB>(sQd + 2 * st * QTB, &tmQ, &bars[1 + st], h * D, PACKED_ROW((qb + 2) * QB), tb);
+      load_tile<D, QB>(sQd + (2 * st + 1) * QTB, &tmdO, &bars[1 + st], h * D, PACKED_ROW((qb + 2) * QB), tb);
     }
   }
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     const int kv = k0 + r0 + g + hr * 8;
-    if (kv >= p.Skv) continue;
-    bf16* dK = p.out0 + (static_cast<int64_t>(b) * p.Skv + kv) * p.ld0 + h * D;
-    bf16* dV = p.out1 + (static_cast<int64_t>(b) * p.Skv + kv) * p.ld1 + h * D;
+    if (kv >= (VARLEN ? len : p.Skv)) continue;
+    const int64_t row = VARLEN ? static_cast<int64_t>(seq0) + kv : static_cast<int64_t>(b) * p.Skv + kv;
+    bf16* dK = p.out0 + row * p.ld0 + h * D;
+    bf16* dV = p.out1 + row * p.ld1 + h * D;
 #pragma unroll
     for (int i = 0; i < DT; ++i) {
       *reinterpret_cast<uint32_t*>(dK + i * 8 + 2 * t4) = pack_bf16x2(dk[i][hr * 2] * p.scale, dk[i][hr * 2 + 1] * p.scale);
@@ -528,6 +594,13 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 
 // delta[b,h,q] = sum_d dO[b,q,h,d] * O[b,q,h,d].  One warp per token row, 16-byte vector loads; a head of D
 // elements is owned by D/8 consecutive lanes and reduced with shuffles (coalesced 512 B / 1 KB per warp access).
+// Every row is a query row of some sample, so the packed layout [H, total] is this kernel's own with B = 1, Sq = total:
+// the varlen backward launches it unchanged (it is defined once, in the dense translation unit).
+#ifdef MMFB_ATTN_VARLEN_TU
+__global__ void attn_delta_kernel(const bf16* __restrict__ dO, int64_t ld_do, const bf16* __restrict__ O,
+                                  int64_t ld_o, const bf16* __restrict__ Olo, float* __restrict__ delta, int B, int H,
+                                  int Sq, int D);
+#else
 __global__ void attn_delta_kernel(const bf16* __restrict__ dO, int64_t ld_do, const bf16* __restrict__ O,
                                   int64_t ld_o, const bf16* __restrict__ Olo, float* __restrict__ delta, int B, int H,
                                   int Sq, int D) {
@@ -576,6 +649,8 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ dO, int64_t ld_do, co
   }
 }
 
+#endif  // MMFB_ATTN_VARLEN_TU
+
 // ----------------------------------------------------------------------------------------------
 // host
 // ----------------------------------------------------------------------------------------------
@@ -596,14 +671,21 @@ static int set_smem(const void* kern, int bytes, const char* who) {
   return MMFB_OK;
 }
 
-template <int D>
-static int attn_fwd_launch(const mmfb_attn_args& a, cudaStream_t stream) {
+// A tensor map over the [rows, heads * D] head columns of one operand: dense = B batches of S rows; packed (VARLEN) =
+// one batch of `total` rows, so that a tile at cu[b] + block * 64 never depends on B
+static int head_map(CUtensorMap* m, const void* ptr, int W, int64_t ld, int rows, int batches, int box_rows) {
+  return make_tmap_3d(m, ptr, W, rows, batches, ld, ld * rows, 64, box_rows);
+}
+
+template <int D, bool VARLEN>
+static int attn_fwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream) {
   const int W = a.heads * D;
+  const int nb = VARLEN ? 1 : a.B, rq = VARLEN ? total : a.Sq, rkv = VARLEN ? total : a.Skv;
   CUtensorMap tmQ, tmK, tmV;
   int rc;
-  if ((rc = make_tmap_3d(&tmQ, a.q, W, a.Sq, a.B, a.ldq, a.ldq * a.Sq, 64, AT_ROWS))) return rc;
-  if ((rc = make_tmap_3d(&tmK, a.k, W, a.Skv, a.B, a.ldk, a.ldk * a.Skv, 64, AT_ROWS))) return rc;
-  if ((rc = make_tmap_3d(&tmV, a.v, W, a.Skv, a.B, a.ldv, a.ldv * a.Skv, 64, AT_ROWS))) return rc;
+  if ((rc = head_map(&tmQ, a.q, W, a.ldq, rq, nb, AT_ROWS))) return rc;
+  if ((rc = head_map(&tmK, a.k, W, a.ldk, rkv, nb, AT_ROWS))) return rc;
+  if ((rc = head_map(&tmV, a.v, W, a.ldv, rkv, nb, AT_ROWS))) return rc;
   const int NKB = (a.Skv + AT_ROWS - 1) / AT_ROWS;
   const int smem = 5 * (D / 64) * AT_ROWS * 128 + NKB * AT_ROWS * 4 + 64 + 1024;
   AttnFwdDev p;
@@ -614,7 +696,8 @@ static int attn_fwd_launch(const mmfb_attn_args& a, cudaStream_t stream) {
   p.ctx_lo = reinterpret_cast<bf16*>(a.ctx_lo);
   p.dmask = a.drop_mask; p.W = (a.Skv + 31) / 32; p.dscale = a.drop_mask ? a.drop_scale : 1.0f;
   p.scale2 = LOG2E / sqrtf(static_cast<float>(D));
-  auto kern = attn_fwd_kernel<D>;
+  p.cu = cu; p.total = total;
+  auto kern = attn_fwd_kernel<D, VARLEN>;
   static int smem_set = 0;
   if (smem > smem_set) {
     if ((rc = set_smem(reinterpret_cast<const void*>(kern), smem, "attn_fwd"))) return rc;
@@ -628,28 +711,22 @@ static int attn_fwd_launch(const mmfb_attn_args& a, cudaStream_t stream) {
   return MMFB_OK;
 }
 
-int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream) {
-  int rc = check_attn_common(a, "attn_fwd");
-  if (rc) return rc;
-  if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2) return set_error(MMFB_ERR_ARG, "attn_fwd: null pointer");
-  return a.head_dim == 64 ? attn_fwd_launch<64>(a, stream) : attn_fwd_launch<128>(a, stream);
-}
-
-template <int D, bool DROP>
-static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, cudaStream_t stream) {
+template <int D, bool DROP, bool VARLEN>
+static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, int total, cudaStream_t stream) {
   constexpr int QB = (D == 64) ? 64 : 32;   // query block of the dK/dV kernel: d = 128 keeps its tiles in registers
   const int W = a.heads * D;
+  const int nb = VARLEN ? 1 : a.B, rq = VARLEN ? total : a.Sq, rkv = VARLEN ? total : a.Skv;
   CUtensorMap tmQ, tmK, tmV, tmdO, tmQc, tmdOc;
   int rc;
-  if ((rc = make_tmap_3d(&tmQ, a.q, W, a.Sq, a.B, a.ldq, a.ldq * a.Sq, 64, AT_ROWS))) return rc;
-  if ((rc = make_tmap_3d(&tmdO, a.dctx, W, a.Sq, a.B, a.ld_dctx, a.ld_dctx * a.Sq, 64, AT_ROWS))) return rc;
-  if ((rc = make_tmap_3d(&tmK, a.k, W, a.Skv, a.B, a.ldk, a.ldk * a.Skv, 64, AT_ROWS))) return rc;
-  if ((rc = make_tmap_3d(&tmV, a.v, W, a.Skv, a.B, a.ldv, a.ldv * a.Skv, 64, AT_ROWS))) return rc;
+  if ((rc = head_map(&tmQ, a.q, W, a.ldq, rq, nb, AT_ROWS))) return rc;
+  if ((rc = head_map(&tmdO, a.dctx, W, a.ld_dctx, rq, nb, AT_ROWS))) return rc;
+  if ((rc = head_map(&tmK, a.k, W, a.ldk, rkv, nb, AT_ROWS))) return rc;
+  if ((rc = head_map(&tmV, a.v, W, a.ldv, rkv, nb, AT_ROWS))) return rc;
   tmQc = tmQ;
   tmdOc = tmdO;
   if (QB != AT_ROWS) {
-    if ((rc = make_tmap_3d(&tmQc, a.q, W, a.Sq, a.B, a.ldq, a.ldq * a.Sq, 64, QB))) return rc;
-    if ((rc = make_tmap_3d(&tmdOc, a.dctx, W, a.Sq, a.B, a.ld_dctx, a.ld_dctx * a.Sq, 64, QB))) return rc;
+    if ((rc = head_map(&tmQc, a.q, W, a.ldq, rq, nb, QB))) return rc;
+    if ((rc = head_map(&tmdOc, a.dctx, W, a.ld_dctx, rq, nb, QB))) return rc;
   }
   const int TB = (D / 64) * AT_ROWS * 128;
   const int NKB = (a.Skv + AT_ROWS - 1) / AT_ROWS;
@@ -658,38 +735,40 @@ static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, cud
   static int set_q = 0;
   static bool set_kv = false;
   if (smem_q > set_q) {
-    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel<D, DROP>), smem_q, "attn_bwd_dq"))) return rc;
+    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel<D, DROP, VARLEN>), smem_q, "attn_bwd_dq"))) return rc;
     set_q = smem_q;
   }
   if (!set_kv) {
-    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dkv_kernel<D, DROP, QB>), smem_kv, "attn_bwd_dkv"))) return rc;
+    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dkv_kernel<D, DROP, QB, VARLEN>), smem_kv, "attn_bwd_dkv")))
+      return rc;
     set_kv = true;
   }
   AttnBwdDev p = base;
   p.out0 = reinterpret_cast<bf16*>(a.dq); p.ld0 = a.ld_dq; p.out1 = nullptr; p.ld1 = 0;
-  MMFB_LAUNCH((attn_bwd_dq_kernel<D, DROP>), dim3((a.Sq + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS, smem_q, stream,
-              tmQ, tmdO, tmK, tmV, p);
+  MMFB_LAUNCH((attn_bwd_dq_kernel<D, DROP, VARLEN>), dim3((a.Sq + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS, smem_q,
+              stream, tmQ, tmdO, tmK, tmV, p);
   count_launch();
   p.out0 = reinterpret_cast<bf16*>(a.dk); p.ld0 = a.ld_dk;
   p.out1 = reinterpret_cast<bf16*>(a.dv); p.ld1 = a.ld_dv;
-  MMFB_LAUNCH((attn_bwd_dkv_kernel<D, DROP, QB>), dim3((a.Skv + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS, smem_kv,
-              stream, tmK, tmV, tmQc, tmdOc, p);
+  MMFB_LAUNCH((attn_bwd_dkv_kernel<D, DROP, QB, VARLEN>), dim3((a.Skv + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS,
+              smem_kv, stream, tmK, tmV, tmQc, tmdOc, p);
   count_launch();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_bwd launch: %s", cudaGetErrorString(e));
   return MMFB_OK;
 }
 
-template <int D>
-static int attn_bwd_launch(const mmfb_attn_args& a, cudaStream_t stream) {
-  // delta = rowsum(dO * O)
+template <int D, bool VARLEN>
+static int attn_bwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream) {
+  // delta = rowsum(dO * O); packed rows are one batch of `total` query rows
   {
-    const int64_t warps = static_cast<int64_t>(a.B) * a.Sq;
+    const int nb = VARLEN ? 1 : a.B, rq = VARLEN ? total : a.Sq;
+    const int64_t warps = static_cast<int64_t>(nb) * rq;
     const int threads = 256;
     const int64_t blocks = (warps * 32 + threads - 1) / threads;
     MMFB_LAUNCH(attn_delta_kernel, static_cast<unsigned>(blocks), threads, 0, stream,
         reinterpret_cast<const bf16*>(a.dctx), a.ld_dctx, reinterpret_cast<const bf16*>(a.ctx), a.ldo, reinterpret_cast<const bf16*>(a.ctx_lo), a.delta,
-        a.B, a.heads, a.Sq, D);
+        nb, a.heads, rq, D);
     count_launch();
   }
   AttnBwdDev p;
@@ -698,7 +777,21 @@ static int attn_bwd_launch(const mmfb_attn_args& a, cudaStream_t stream) {
   p.dmask = a.drop_mask; p.W = (a.Skv + 31) / 32; p.dscale = a.drop_mask ? a.drop_scale : 1.0f;
   p.scale = 1.0f / sqrtf(static_cast<float>(D));
   p.scale2 = LOG2E * p.scale;
-  return a.drop_mask != nullptr ? attn_bwd_kernels<D, true>(a, p, stream) : attn_bwd_kernels<D, false>(a, p, stream);
+  p.cu = cu; p.total = total;
+  return a.drop_mask != nullptr ? attn_bwd_kernels<D, true, VARLEN>(a, p, total, stream)
+                                : attn_bwd_kernels<D, false, VARLEN>(a, p, total, stream);
+}
+
+// The dense entry points instantiate the dense kernels only, and attention_varlen.cu (which includes this file) the
+// packed ones: instantiated in one translation unit, the two share inlined helpers that the compiler then schedules
+// differently, and the dense d = 64 forward would not keep the code it has without the packed mode.
+#ifndef MMFB_ATTN_VARLEN_TU
+int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream) {
+  int rc = check_attn_common(a, "attn_fwd");
+  if (rc) return rc;
+  if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2) return set_error(MMFB_ERR_ARG, "attn_fwd: null pointer");
+  return a.head_dim == 64 ? attn_fwd_launch<64, false>(a, nullptr, 0, stream)
+                          : attn_fwd_launch<128, false>(a, nullptr, 0, stream);
 }
 
 int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
@@ -706,7 +799,41 @@ int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
   if (rc) return rc;
   if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2 || !a.dctx || !a.delta || !a.dq || !a.dk || !a.dv)
     return set_error(MMFB_ERR_ARG, "attn_bwd: null pointer");
-  return a.head_dim == 64 ? attn_bwd_launch<64>(a, stream) : attn_bwd_launch<128>(a, stream);
+  return a.head_dim == 64 ? attn_bwd_launch<64, false>(a, nullptr, 0, stream)
+                          : attn_bwd_launch<128, false>(a, nullptr, 0, stream);
 }
+
+#else   // MMFB_ATTN_VARLEN_TU
+
+// Packed self-attention: Sq = Skv = max_len (the grid extent), no additive mask, `cu` on the device and never read here.
+static int check_varlen(const mmfb_attn_args& a, const int32_t* cu, int total, const char* who) {
+  int rc = check_attn_common(a, who);
+  if (rc) return rc;
+  if (a.Sq != a.Skv) return set_error(MMFB_ERR_ARG, "%s: self-attention only, Sq (%d) must equal Skv (%d) = max_len", who, a.Sq, a.Skv);
+  if (a.mask != nullptr) return set_error(MMFB_ERR_ARG, "%s: mask must be NULL (packing has removed the masked keys)", who);
+  if (!cu) return set_error(MMFB_ERR_ARG, "%s: null cu_seqlens", who);
+  if (total < 0) return set_error(MMFB_ERR_ARG, "%s: negative total (%d)", who, total);
+  return MMFB_OK;
+}
+
+int attn_varlen_fwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream) {
+  int rc = check_varlen(a, cu, total, "attn_varlen_fwd");
+  if (rc) return rc;
+  if (total == 0) return MMFB_OK;           // every sample is empty: nothing to compute or write
+  if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2) return set_error(MMFB_ERR_ARG, "attn_varlen_fwd: null pointer");
+  return a.head_dim == 64 ? attn_fwd_launch<64, true>(a, cu, total, stream)
+                          : attn_fwd_launch<128, true>(a, cu, total, stream);
+}
+
+int attn_varlen_bwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream) {
+  int rc = check_varlen(a, cu, total, "attn_varlen_bwd");
+  if (rc) return rc;
+  if (total == 0) return MMFB_OK;
+  if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2 || !a.dctx || !a.delta || !a.dq || !a.dk || !a.dv)
+    return set_error(MMFB_ERR_ARG, "attn_varlen_bwd: null pointer");
+  return a.head_dim == 64 ? attn_bwd_launch<64, true>(a, cu, total, stream)
+                          : attn_bwd_launch<128, true>(a, cu, total, stream);
+}
+#endif  // MMFB_ATTN_VARLEN_TU
 
 }  // namespace mmfb

@@ -136,6 +136,18 @@ int mmfb_attention_bwd(const mmfb_attn_args* args, mmfb_stream stream) {
   return attn_bwd(*args, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int mmfb_attention_varlen_fwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_attention_varlen_fwd: null args");
+  MMFB_REQUIRE_DEVICE();
+  return attn_varlen_fwd(*args, cu_seqlens, total, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int mmfb_attention_varlen_bwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_attention_varlen_bwd: null args");
+  MMFB_REQUIRE_DEVICE();
+  return attn_varlen_bwd(*args, cu_seqlens, total, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int mmfb_layernorm_fwd(const mmfb_ln_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_layernorm_fwd: null args");
   MMFB_REQUIRE_DEVICE();

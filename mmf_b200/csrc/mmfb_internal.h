@@ -52,6 +52,8 @@ cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
 int gemm(const mmfb_gemm_args& a, cudaStream_t stream);
 int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream);
 int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream);
+int attn_varlen_fwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream);
+int attn_varlen_bwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream);
 int ln_fwd(const mmfb_ln_args& a, cudaStream_t s);
 int ln_bwd(const mmfb_ln_args& a, cudaStream_t s);
 int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s);

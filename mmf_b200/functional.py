@@ -146,6 +146,89 @@ def attention_bwd(dctx, q, k, v, ctx, lse2, B, heads, Sq, Skv, mask=None, drop_m
     return dq, dk, dv
 
 
+def _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale):
+    """packed self-attention operands: q/k/v [total, h*d] rows of B samples delimited by cu_seqlens (int32 [B+1])"""
+    if not isinstance(cu_seqlens, torch.Tensor) or cu_seqlens.dtype != torch.int32:
+        raise ValueError("cu_seqlens must be an int32 tensor")
+    if cu_seqlens.dim() != 1 or cu_seqlens.numel() < 2 or not cu_seqlens.is_contiguous():
+        raise ValueError("cu_seqlens must be a contiguous int32 vector [B+1] with B >= 1, got shape %s"
+                         % (tuple(cu_seqlens.shape),))
+    if not cu_seqlens.is_cuda:
+        raise RuntimeError("cu_seqlens must be a CUDA tensor: the kernels read it on the device")
+    for t, n in ((q, "q"), (k, "k"), (v, "v")):
+        _req(t, torch.bfloat16, n)
+        if t.dim() != 2:
+            raise ValueError("attention_varlen: %s must be 2-D [total, heads*head_dim]" % n)
+    total, W = q.shape
+    if k.shape[0] != total or v.shape[0] != total:
+        raise ValueError("attention_varlen: q/k/v must all hold total=%d rows" % total)
+    if W % heads:
+        raise ValueError(
+            "The hidden size (%d) is not a multiple of the number of attention heads (%d)" % (W, heads))
+    B = cu_seqlens.numel() - 1
+    max_len = int(max_len)
+    a = AttnArgs()
+    a.q, a.ldq = q.data_ptr(), q.stride(0)
+    a.k, a.ldk = k.data_ptr(), k.stride(0)
+    a.v, a.ldv = v.data_ptr(), v.stride(0)
+    if drop_mask is not None:
+        _req(drop_mask, torch.int32, "drop_mask")
+        if tuple(drop_mask.shape) != (heads, total, (max_len + 31) // 32) or not drop_mask.is_contiguous():
+            raise ValueError("attention_varlen: drop_mask must be contiguous int32 [heads, total, ceil(max_len/32)]")
+        a.drop_mask, a.drop_scale = drop_mask.data_ptr(), float(drop_scale)
+    a.B, a.heads, a.Sq, a.Skv, a.head_dim = B, heads, max_len, max_len, W // heads
+    return a, total, W
+
+
+def attention_varlen_fwd(q, k, v, cu_seqlens, max_len, heads, drop_mask=None, drop_scale=1.0, out=None, save_lo=False):
+    """Packed self-attention: ctx, lse2 (, ctx_lo).  Sample b is rows [cu_seqlens[b], cu_seqlens[b+1]) of q/k/v
+    [total, h*d] (views allowed) and attends to its own rows only; max_len bounds every length.  lse2 is fp32
+    [heads, total].  The lengths stay on the device: nothing here synchronises."""
+    a, total, W = _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale)
+    ctx = out if out is not None else torch.empty(total, W, dtype=torch.bfloat16, device=q.device)
+    _req(ctx, torch.bfloat16, "out")
+    lse2 = torch.empty(heads, total, dtype=torch.float32, device=q.device)
+    a.ctx, a.ldo, a.lse2 = ctx.data_ptr(), ctx.stride(0), lse2.data_ptr()
+    ctx_lo = None
+    if save_lo:
+        ctx_lo = torch.empty(total, W, dtype=torch.bfloat16, device=q.device)
+        a.ctx_lo = ctx_lo.data_ptr()
+    check(LIB.mmfb_attention_varlen_fwd(ctypes.byref(a), cu_seqlens.data_ptr(), total, _stream_ptr()))
+    if save_lo:
+        return ctx, lse2, ctx_lo
+    return ctx, lse2
+
+
+def attention_varlen_bwd(dctx, q, k, v, ctx, lse2, cu_seqlens, max_len, heads, drop_mask=None, drop_scale=1.0,
+                         dq=None, dk=None, dv=None, ctx_lo=None):
+    """dq, dk, dv of attention_varlen_fwd (packed rows, probabilities recomputed from the saved lse2 [heads, total])."""
+    a, total, W = _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale)
+    _req(dctx, torch.bfloat16, "dctx")
+    _req(ctx, torch.bfloat16, "ctx")
+    if dctx.shape[0] != total or ctx.shape[0] != total:
+        raise ValueError("attention_varlen: dctx and ctx must hold total=%d rows" % total)
+    if not lse2.is_cuda or lse2.dtype != torch.float32 or tuple(lse2.shape) != (heads, total) or not lse2.is_contiguous():
+        raise ValueError("attention_varlen: lse2 must be contiguous fp32 [heads, total]")
+    dq = dq if dq is not None else torch.empty(total, W, dtype=torch.bfloat16, device=q.device)
+    dk = dk if dk is not None else torch.empty(total, W, dtype=torch.bfloat16, device=q.device)
+    dv = dv if dv is not None else torch.empty(total, W, dtype=torch.bfloat16, device=q.device)
+    for t, n in ((dq, "dq"), (dk, "dk"), (dv, "dv")):
+        _req(t, torch.bfloat16, n)
+    delta = torch.empty(heads, total, dtype=torch.float32, device=q.device)
+    a.ctx, a.ldo, a.lse2 = ctx.data_ptr(), ctx.stride(0), lse2.data_ptr()
+    a.dctx, a.ld_dctx, a.delta = dctx.data_ptr(), dctx.stride(0), delta.data_ptr()
+    if ctx_lo is not None:
+        _req(ctx_lo, torch.bfloat16, "ctx_lo")
+        if not ctx_lo.is_contiguous() or tuple(ctx_lo.shape) != (total, W):
+            raise ValueError("ctx_lo must be contiguous [total, heads*head_dim]")
+        a.ctx_lo = ctx_lo.data_ptr()
+    a.dq, a.ld_dq = dq.data_ptr(), dq.stride(0)
+    a.dk, a.ld_dk = dk.data_ptr(), dk.stride(0)
+    a.dv, a.ld_dv = dv.data_ptr(), dv.stride(0)
+    check(LIB.mmfb_attention_varlen_bwd(ctypes.byref(a), cu_seqlens.data_ptr(), total, _stream_ptr()))
+    return dq, dk, dv
+
+
 def pack_keep_bits(keep):
     """bool [..., n] -> int32 [..., ceil(n/32)] keep-bit words (bit j of word w = element 32*w + j)."""
     n = keep.shape[-1]

@@ -41,6 +41,9 @@ class GraphedStep:
     def __init__(self, model, loss_fn, example_batch, warmup=3):
         """loss_fn(batch) -> scalar loss; `example_batch`: (nested dict / list of) CUDA tensors with the shapes of every later
         batch.  The model must be in the mode (train / eval) it will be replayed in."""
+        if any(getattr(m.__dict__.get("_runner"), "skip_padding", False) for m in model.modules()):
+            raise RuntimeError("GraphedStep: the model has skip_padding encoders, which read the token count on the host and "
+                               "cannot be captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)")
         self.model, self.loss_fn = model, loss_fn
         self.static = _map(lambda t: t.detach().clone(), example_batch)
         dev = next(t for t in _flatten(self.static) if t.is_cuda).device

@@ -73,6 +73,8 @@ class EncoderRunner:
         self.pack = None
         self.weights = None
         self.grad_ready_hook = None   # callable(layer_index) - set by mmf_b200.ddp for bucket all-reduce overlap
+        # skip padded tokens: pack the valid rows once per encoder call and run variable-length attention (run_bert_encoder)
+        self.skip_padding = False
 
     def _probs(self, m):
         def p_of(mod):
@@ -125,6 +127,47 @@ class EncoderRunner:
         return d
 
 
+class _Packing:
+    """Valid rows of a padded [B, S] batch: `rows` (int64 [total]) are their flat indices in sample order, `varlen` the
+    descriptor the engine's attention reads."""
+
+    def __init__(self, rows, varlen):
+        self.rows, self.varlen = rows, varlen
+
+    def pack(self, t):
+        """[B*S, H] -> [total, H]: the valid rows, in their original order within each sample"""
+        return t.index_select(0, self.rows)
+
+    def unpack(self, t, BS):
+        """[total, H] -> [B*S, H] with exact zero rows at padded positions"""
+        return t.new_zeros(BS, t.shape[1]).index_copy_(0, self.rows, t)
+
+
+def _plan_packing(mask, B, S):
+    """The packing of an additive [B, S] fp32 mask (0 = token, <= -10000 = padding), or None when no row is padded.
+    One device-to-host copy fetches the counts; the row indices are built on the device without another one."""
+    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("skip_padding cannot run under CUDA-graph capture: packing needs the valid-token count on the host "
+                           "(turn it off with mmf_b200.patch.set_skip_padding(model, False) before capturing)")
+    valid = mask == 0
+    lens = valid.sum(1, dtype=torch.int32)
+    soft = ((mask != 0) & (mask > -10000.0)).sum()
+    n_soft, total, max_len = (int(v) for v in torch.stack([soft.to(torch.int64), lens.sum(dtype=torch.int64),
+                                                           lens.max().to(torch.int64)]).tolist())
+    if n_soft:
+        raise ValueError("skip_padding needs a key-padding mask of 0 (token) and <= -10000 (padding); %d value(s) are a "
+                         "soft bias, which cannot be packed away" % n_soft)
+    if total == B * S:
+        return None
+    cu = torch.zeros(B + 1, dtype=torch.int32, device=mask.device)
+    cu[1:] = torch.cumsum(lens, 0, dtype=torch.int32)
+    flat = valid.reshape(-1)
+    dest = torch.where(flat, torch.cumsum(flat, 0) - 1, torch.full_like(flat, total, dtype=torch.int64))
+    rows = torch.empty(total + 1, dtype=torch.int64, device=mask.device)
+    rows.scatter_(0, dest, torch.arange(B * S, device=mask.device))     # padded rows all land in the spare last slot
+    return _Packing(rows[:total], E.Varlen(cu, B, total, max_len))
+
+
 class _BertEncoderFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, runner, add_mask, training, want_hiddens, x, *params):
@@ -132,7 +175,15 @@ class _BertEncoderFn(torch.autograd.Function):
         need_grad = any(ctx.needs_input_grad)   # (grad mode itself is always off inside Function.forward)
         runner.pack.refresh()
         xb = x.detach().to(torch.bfloat16).contiguous()
-        out, saved, hiddens = runner.forward(xb, add_mask, training, need_grad)
+        packing = add_mask if isinstance(add_mask, _Packing) else None
+        if packing is None:
+            out, saved, hiddens = runner.forward(xb, add_mask, training, need_grad)
+        else:                                   # the layers run on the [total, H] valid rows only
+            vl = packing.varlen
+            xp = packing.pack(xb.view(B * S, H)).view(1, vl.total, H)
+            out, saved, hiddens = runner.forward(xp, vl, training, need_grad)
+            out = packing.unpack(out, B * S)
+            hiddens = [packing.unpack(h, B * S) for h in hiddens] if want_hiddens else hiddens
         ctx.runner, ctx.saved, ctx.add_mask, ctx.dims, ctx.in_dtype = runner, saved, add_mask, (B, S, H), x.dtype
         outs = [out.view(B, S, H).to(x.dtype)]
         if want_hiddens:
@@ -148,7 +199,12 @@ class _BertEncoderFn(torch.autograd.Function):
             raise RuntimeError("B200 encoder: backward called twice or activations were not saved")
         aliased = runner.pack.prepare_grads()
         d = dout.to(torch.bfloat16).contiguous().view(B * S, H)
-        dx = runner.backward(d, ctx.saved, ctx.add_mask, B, S)
+        if isinstance(ctx.add_mask, _Packing):
+            packing = ctx.add_mask
+            dx = runner.backward(packing.pack(d), ctx.saved, packing.varlen, 1, packing.varlen.total)
+            dx = packing.unpack(dx, B * S)
+        else:
+            dx = runner.backward(d, ctx.saved, ctx.add_mask, B, S)
         ctx.saved = None
         return (None, None, None, None, dx.view(B, S, H).to(ctx.in_dtype)) + tuple(runner.pack.autograd_grads(aliased))
 
@@ -163,6 +219,14 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
     if H != runner.weights[0].hidden:
         raise ValueError("hidden size %d does not match the encoder's %d" % (H, runner.weights[0].hidden))
     mask = E.additive_mask_2d(attention_mask, B, S)
+    if runner.skip_padding and mask is not None:
+        packing = _plan_packing(mask, B, S)
+        if packing is not None and packing.varlen.total == 0:
+            # every token is padding: nothing to compute, every output row (and every input-gradient row) is zero
+            z = hidden_states * 0
+            return (z,) + ((z.detach(),) * len(runner.layers) if output_hidden_states else ())
+        if packing is not None:
+            mask = packing
     outs = _BertEncoderFn.apply(runner, mask, training, output_hidden_states, hidden_states, *runner.pack.params)
     return outs
 
@@ -244,6 +308,7 @@ class B200BertEncoder(nn.Module):
             for _ in range(config.num_hidden_layers)])
         _init_bert_weights(self, float(getattr(config, "initializer_range", 0.02)))
         self._runner = EncoderRunner(self.layer)
+        self._runner.skip_padding = bool(getattr(config, "skip_padding", False))
 
     def forward(self, hidden_states, attention_mask=None, encoder_hidden_states=None, encoder_attention_mask=None,
                 output_attentions=False, output_hidden_states=False, return_dict=False, head_mask=None):

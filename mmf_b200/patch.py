@@ -4,6 +4,9 @@
 HuggingFace `BertEncoder` (and every subclass that overrides `forward`, e.g. MMF's `BertEncoderJit`) to the B200 engine
 with the contract of `BertEncoderJit.forward` (hf_layers.py:316-355).  Parameters keep their names; their storage is
 re-homed into the engine's flat pack on the first CUDA forward.
+
+`set_skip_padding()` switches the single-stream encoders of a model to packed execution: padded tokens are removed once
+per encoder call and attention runs over each sample's own tokens (variable-length kernels), so padding costs nothing.
 """
 import types
 
@@ -63,3 +66,29 @@ def undo_replace_with_b200():
     for cls, fwd in list(_saved.items()):
         cls.forward = fwd
         del _saved[cls]
+
+
+def _routed(m):
+    """True if `m`'s forward is the engine's (replace_with_b200 on its class, or attach_encoder on the instance)"""
+    f = m.__dict__.get("forward", None) or getattr(type(m), "forward", None)
+    return getattr(f, "__func__", f) is _b200_encoder_forward
+
+
+def set_skip_padding(module, enabled=True):
+    """Sets `skip_padding` on every single-stream encoder runner under `module` (B200BertEncoder - and so VisualBERT, MMBT,
+    UNITER, VinVL and the TransformerEncoder plugin -, VisualBERT's bypass `additional_layer`, encoders routed by
+    attach_encoder / replace_with_b200) and returns how many it set.  ViLBERT, LXMERT and ViT runners are left alone.
+
+    With the flag on, an encoder call with a key-padding mask runs on the valid rows only: its outputs (and the input
+    gradient) are exactly zero at padded positions instead of the values the dense path computes there.  For any loss that
+    does not read padded positions it computes the same function and gradients as the dense path, up to rounding and the
+    dropout masks drawn.  It reads the token count on the host, so it cannot be captured in a CUDA graph."""
+    n = 0
+    for m in module.modules():
+        r = m.__dict__.get("_runner")
+        if r is None and hasattr(m, "layer") and _routed(m):
+            r = _runner_of(m)
+        if type(r) is EncoderRunner:
+            r.skip_padding = bool(enabled)
+            n += 1
+    return n
