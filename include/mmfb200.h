@@ -112,6 +112,31 @@ int mmfb_attention_bwd(const mmfb_attn_args* args, mmfb_stream stream);
 int mmfb_attention_varlen_fwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream);
 int mmfb_attention_varlen_bwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream);
 
+/* Variable-length (packed) cross-attention: the queries come from one packed stream and the keys / values from another
+ * (ViLBERT co-attention, LXMERT cross-modality layers).  cu_q, cu_kv: int32 [B+1] on the DEVICE, each a non-decreasing
+ * prefix sum from 0 to total_q / total_kv; sample b's queries are rows [cu_q[b], cu_q[b+1]) of q, ctx, ctx_lo, dctx, dq
+ * and its keys rows [cu_kv[b], cu_kv[b+1]) of k, v, dk, dv.  The lengths are never read on the host.
+ *   args->B = samples; args->Sq = max_q >= every query length (sets the grid), args->Skv = max_kv >= every key length;
+ *   args->mask must be NULL (MMFB_ERR_ARG otherwise): packing has already removed the masked keys;
+ *   q, ctx, ctx_lo, dctx, dq: [total_q, ld] rows; k, v, dk, dv: [total_kv, ld] rows; same head-column layout as
+ *   mmfb_attention_fwd;
+ *   lse2, delta: fp32 [heads, total_q];
+ *   drop_mask: keep bits int32 [heads, total_q, ceil(max_kv/32)], bit kv%32 of word kv/32 for key kv WITHIN the sample.
+ * Empty sides are defined and never produce NaN:
+ *   a sample with queries but no keys writes ctx = ctx_lo = 0 and dq = 0 on its query rows, and lse2 = -inf (the log of an
+ *   empty sum; the backward does not read it);
+ *   a sample with keys but no queries writes dk = dv = 0 on its key rows (so the backward runs even when total_q = 0).
+ * Every query row in [0, total_q) gets ctx / lse2 / dq, every key row in [0, total_kv) gets dk / dv, as long as the
+ * lengths respect max_q / max_kv; lengths are clamped to them and to the totals, so a bad cu never reaches outside the
+ * buffers.  Sq / Skv / totals of 0 are legal; the forward returns MMFB_OK without a launch when total_q = 0, the backward
+ * when both totals are 0.  Packed self-attention is this call with cu_kv = cu_q and computes bit for bit what
+ * mmfb_attention_varlen_fwd / _bwd do.
+ * Limits: head_dim 64 or 128; max_kv <= 384 (d=64) / 256 (d=128); max_q only by the grid. */
+int mmfb_attention_varlen_cross_fwd(const mmfb_attn_args* args, const int32_t* cu_q, int total_q, const int32_t* cu_kv,
+                                    int total_kv, mmfb_stream stream);
+int mmfb_attention_varlen_cross_bwd(const mmfb_attn_args* args, const int32_t* cu_q, int total_q, const int32_t* cu_kv,
+                                    int total_kv, mmfb_stream stream);
+
 /* LayerNorm over the last dimension (eps 1e-12 on this path), one warp per row.
  * fwd: x = LN(y)*gamma + beta, optional dropout on x (embeddings), saves mean / rstd (fp32 [M]).
  * bwd: dy = dLN(dx (+dx2)); dz = dropout-backward(dy) for the dense branch that fed y = dropout(dense)+resid;

@@ -21,9 +21,10 @@
 //   dq kernel : CTA owns 64 query rows, loops over key blocks:    dQ = scale * dS K
 //   dkv kernel: CTA owns 64 key rows, loops over query blocks:    dV = P^T dO,  dK = scale * dS^T Q
 //               (computed as S^T = K Q^T and dP^T = V dO^T, so the key rows stay the rows of every register tile)
-// VARLEN instantiations (packed self-attention, include/mmfb200.h): the samples' rows are packed back to back, so a tile
-// may run into the next sample; those rows are masked (keys), not stored (queries) or given P = 0 (dk/dv), and every CTA
-// stays within its own sample's blocks.
+// VARLEN instantiations (packed self- and cross-attention, include/mmfb200.h): the samples' rows are packed back to back,
+// so a tile may run into the next sample; those rows are masked (keys), not stored (queries) or given P = 0 (dk/dv), and
+// every CTA stays within its own sample's blocks.  Queries and keys each have their own packing (cu / total for the query
+// side, cu_kv / total_kv for the key side); packed self-attention passes the same one twice.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -118,26 +119,32 @@ struct AttnFwdDev {
   int W;
   float dscale;           // 1/(1-p)
   float scale2;           // log2(e)/sqrt(d)
-  const int* cu;          // VARLEN: [B+1] first packed row of every sample (Sq = Skv = max_len)
-  int total;              // VARLEN: packed rows
+  const int* cu;          // VARLEN: [B+1] first packed query row of every sample (Sq = max_q)
+  int total;              // VARLEN: packed query rows
+  const int* cu_kv;       // VARLEN: [B+1] first packed key row of every sample (Skv = max_kv; self-attention: cu)
+  int total_kv;           // VARLEN: packed key rows
 };
 
-// VARLEN: sample b owns the packed rows [cu[b], cu[b+1]) of every row buffer (clamped to `total` and to max_len rows);
-// returns that range as (first row, length).  Read after griddep_wait, like every other global read.
+// VARLEN: sample b owns the packed rows [cu[b], cu[b+1]) of one side's row buffers (clamped to [0, total] and to max_len
+// rows); returns that range as (first row, length), the length never negative.  Read after griddep_wait, like every other
+// global read.
 __device__ __forceinline__ int2 varlen_rows(const int* cu, int b, int total, int max_len) {
-  const int s0 = __ldg(cu + b);
-  return make_int2(s0, min(min(__ldg(cu + b + 1), total) - s0, max_len));
+  const int s0 = min(max(__ldg(cu + b), 0), total);
+  return make_int2(s0, max(min(min(__ldg(cu + b + 1), total) - s0, max_len), 0));
 }
 
-// PACKED_ROW: tile row coordinate (dense: within batch b; packed: sample b starts at row seq0).
-// HEAD_ROW: first row of (batch-head bh, head h) in lse2 / delta / the keep bits: [B, H, Sq] dense, [H, total] packed.  A macro so
-// that the dense kernels keep the exact expressions (and code) they had before the packed mode existed.
+// PACKED_ROW / PACKED_KV_ROW: tile row coordinate of a query / key tile (dense: within batch b; packed: sample b starts at
+// query row seq0 and key row kv0).
+// HEAD_ROW: first row of (batch-head bh, head h) in lse2 / delta / the keep bits: [B, H, Sq] dense, [H, total] packed (query
+// rows).  Macros so that the dense kernels keep the exact expressions (and code) they had before the packed mode existed.
 #define PACKED_ROW(r) (VARLEN ? seq0 + (r) : (r))
+#define PACKED_KV_ROW(r) (VARLEN ? kv0 + (r) : (r))
 #define HEAD_ROW(bh) (VARLEN ? static_cast<int64_t>(h) * p.total + seq0 : static_cast<int64_t>(bh) * p.Sq)
 
 // grid (query tiles, heads, batch); smem: Q tile, two stages of (K block, V block), the key mask (log2 domain).
-// VARLEN: packed self-attention (no additive mask); the tensor maps span the packed rows with a batch extent of 1, tiles
-// load at row cu[b] + block * 64, and rows past the end of the sample (the next sample's rows) are masked / not stored.
+// VARLEN: packed attention (no additive mask); the tensor maps span each side's packed rows with a batch extent of 1, tiles
+// load at row cu[b] + block * 64 (queries) / cu_kv[b] + block * 64 (keys), and rows past the end of the sample (the next
+// sample's rows) are masked / not stored.  A sample without keys writes ctx = ctx_lo = 0 and lse2 = -inf (empty sum).
 template <int D, bool VARLEN>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -164,14 +171,18 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
   __syncthreads();
   griddep_wait();
-  // dense: the sample's rows start at row 0 of batch b; VARLEN: at packed row seq0 of the single batch
+  // dense: the sample's rows start at row 0 of batch b; VARLEN: at packed query row seq0 / key row kv0 of the single batch
   int seq0 = 0, len = p.Skv, nkb = NKB;
+  int kv0 = 0, kvlen = p.Skv;
   if constexpr (VARLEN) {
-    const int2 r = varlen_rows(p.cu, b, p.total, p.Skv);
+    const int2 r = varlen_rows(p.cu, b, p.total, p.Sq);
     seq0 = r.x;
     len = r.y;
     if (q0 >= len) return;                     // no query of this tile exists (empty samples: every tile)
-    nkb = (len + AT_ROWS - 1) / AT_ROWS;       // the sample's own key blocks only
+    const int2 rk = varlen_rows(p.cu_kv, b, p.total_kv, p.Skv);
+    kv0 = rk.x;
+    kvlen = rk.y;
+    nkb = (kvlen + AT_ROWS - 1) / AT_ROWS;     // the sample's own key blocks only (none without keys)
   }
   const int tb = VARLEN ? 0 : b;
   if (threadIdx.x == 0) {
@@ -179,15 +190,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     load_tile<D, AT_ROWS>(sQ, &tmQ, &bars[0], h * D, PACKED_ROW(q0), tb);
     for (int kb = 0; kb < 2 && kb < nkb; ++kb) {
       mbar_expect_tx(&bars[1 + kb], 2 * TB);
-      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, PACKED_ROW(kb * AT_ROWS), tb);
-      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, PACKED_ROW(kb * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, PACKED_KV_ROW(kb * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, PACKED_KV_ROW(kb * AT_ROWS), tb);
     }
   }
   // additive mask in the log2 domain; padded key columns (VARLEN: keys past the sample) get -inf so that exp2 yields
   // exactly 0
   for (int i = threadIdx.x; i < nkb * AT_ROWS; i += AT_THREADS) {
     if constexpr (VARLEN)
-      sMask[i] = (i < len) ? 0.0f : -INFINITY;
+      sMask[i] = (i < kvlen) ? 0.0f : -INFINITY;
     else
       sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
   }
@@ -272,8 +283,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     __syncthreads();
     if (threadIdx.x == 0 && kb + 2 < nkb) {
       mbar_expect_tx(&bars[1 + st], 2 * TB);
-      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, PACKED_ROW((kb + 2) * AT_ROWS), tb);
-      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, PACKED_ROW((kb + 2) * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, PACKED_KV_ROW((kb + 2) * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, PACKED_KV_ROW((kb + 2) * AT_ROWS), tb);
     }
   }
 
@@ -284,8 +295,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const int q = q0 + r0 + g + hr * 8;
     if (q >= (VARLEN ? len : p.Sq)) continue;
-    if (t4 == 0) p.lse2[HEAD_ROW(b * p.H + h) + q] = mrow[hr] + log2f(l);
-    const float inv = p.dscale / l;
+    if (t4 == 0) p.lse2[HEAD_ROW(b * p.H + h) + q] = mrow[hr] + log2f(l);   // VARLEN without keys: -inf + log2(0)
+    const float inv = (VARLEN && kvlen == 0) ? 0.0f : p.dscale / l;         // no keys: o = 0 and l = 0, the row is 0
     const int64_t row = VARLEN ? static_cast<int64_t>(seq0) + q : static_cast<int64_t>(b) * p.Sq + q;
     bf16* dst = p.ctx + row * p.ldo + h * D;
     bf16* dlo = p.ctx_lo != nullptr ? p.ctx_lo + row * (p.H * D) + h * D : nullptr;
@@ -318,9 +329,12 @@ struct AttnBwdDev {
   bf16* out1; int64_t ld1;   // dv (dkv kernel)
   const int* cu;             // VARLEN, as in AttnFwdDev
   int total;
+  const int* cu_kv;
+  int total_kv;
 };
 
-// dQ for 64 query rows.  smem: Q, dO tiles; two stages of (K block, V block).  VARLEN as in the forward.
+// dQ for 64 query rows.  smem: Q, dO tiles; two stages of (K block, V block).  VARLEN as in the forward (a sample without
+// keys writes dq = 0).
 template <int D, bool DROP, bool VARLEN>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
@@ -350,12 +364,16 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   __syncthreads();
   griddep_wait();
   int seq0 = 0, len = p.Skv, nkb = NKB;
+  int kv0 = 0, kvlen = p.Skv;
   if constexpr (VARLEN) {
-    const int2 r = varlen_rows(p.cu, b, p.total, p.Skv);
+    const int2 r = varlen_rows(p.cu, b, p.total, p.Sq);
     seq0 = r.x;
     len = r.y;
     if (q0 >= len) return;
-    nkb = (len + AT_ROWS - 1) / AT_ROWS;
+    const int2 rk = varlen_rows(p.cu_kv, b, p.total_kv, p.Skv);
+    kv0 = rk.x;
+    kvlen = rk.y;
+    nkb = (kvlen + AT_ROWS - 1) / AT_ROWS;
   }
   const int tb = VARLEN ? 0 : b;
   if (threadIdx.x == 0) {
@@ -364,13 +382,13 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     load_tile<D, AT_ROWS>(sdO, &tmdO, &bars[0], h * D, PACKED_ROW(q0), tb);
     for (int kb = 0; kb < 2 && kb < nkb; ++kb) {
       mbar_expect_tx(&bars[1 + kb], 2 * TB);
-      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, PACKED_ROW(kb * AT_ROWS), tb);
-      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, PACKED_ROW(kb * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + 2 * kb * TB, &tmK, &bars[1 + kb], h * D, PACKED_KV_ROW(kb * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + (2 * kb + 1) * TB, &tmV, &bars[1 + kb], h * D, PACKED_KV_ROW(kb * AT_ROWS), tb);
     }
   }
   for (int i = threadIdx.x; i < nkb * AT_ROWS; i += AT_THREADS) {
     if constexpr (VARLEN)
-      sMask[i] = (i < len) ? 0.0f : -INFINITY;
+      sMask[i] = (i < kvlen) ? 0.0f : -INFINITY;
     else
       sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
   }
@@ -439,8 +457,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     __syncthreads();
     if (threadIdx.x == 0 && kb + 2 < nkb) {
       mbar_expect_tx(&bars[1 + st], 2 * TB);
-      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, PACKED_ROW((kb + 2) * AT_ROWS), tb);
-      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, PACKED_ROW((kb + 2) * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + 2 * st * TB, &tmK, &bars[1 + st], h * D, PACKED_KV_ROW((kb + 2) * AT_ROWS), tb);
+      load_tile<D, AT_ROWS>(sKV + (2 * st + 1) * TB, &tmV, &bars[1 + st], h * D, PACKED_KV_ROW((kb + 2) * AT_ROWS), tb);
     }
   }
 #pragma unroll
@@ -457,7 +475,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
 // dK, dV for 64 key rows.  smem: K, V tiles; two stages of (Q block, dO block) of QB query rows.  The register tiles are
 // transposed products (rows = keys, columns = queries).  VARLEN as in the forward; query rows past the end of the sample
-// take lse = +inf and delta = 0 (P = 0), like rows past Sq.
+// take lse = +inf and delta = 0 (P = 0), like rows past Sq, and a sample without queries writes dk = dv = 0.
 template <int D, bool DROP, int QB, bool VARLEN>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
@@ -488,18 +506,22 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   __syncthreads();
   griddep_wait();
   int seq0 = 0, len = p.Skv, nqb = NQB;
+  int kv0 = 0, kvlen = p.Skv;
   if constexpr (VARLEN) {
-    const int2 r = varlen_rows(p.cu, b, p.total, p.Skv);
+    const int2 rk = varlen_rows(p.cu_kv, b, p.total_kv, p.Skv);
+    kv0 = rk.x;
+    kvlen = rk.y;
+    if (k0 >= kvlen) return;                    // no key of this tile exists
+    const int2 r = varlen_rows(p.cu, b, p.total, p.Sq);
     seq0 = r.x;
     len = r.y;
-    if (k0 >= len) return;                      // no key of this tile exists
-    nqb = (len + QB - 1) / QB;                  // the sample's own query blocks only
+    nqb = (len + QB - 1) / QB;                  // the sample's own query blocks only (none without queries)
   }
   const int tb = VARLEN ? 0 : b;
   if (threadIdx.x == 0) {
     mbar_expect_tx(&bars[0], 2 * TB);
-    load_tile<D, AT_ROWS>(sK, &tmK, &bars[0], h * D, PACKED_ROW(k0), tb);
-    load_tile<D, AT_ROWS>(sV, &tmV, &bars[0], h * D, PACKED_ROW(k0), tb);
+    load_tile<D, AT_ROWS>(sK, &tmK, &bars[0], h * D, PACKED_KV_ROW(k0), tb);
+    load_tile<D, AT_ROWS>(sV, &tmV, &bars[0], h * D, PACKED_KV_ROW(k0), tb);
     for (int qb = 0; qb < 2 && qb < nqb; ++qb) {
       mbar_expect_tx(&bars[1 + qb], 2 * QTB);
       load_tile<D, QB>(sQd + 2 * qb * QTB, &tmQ, &bars[1 + qb], h * D, PACKED_ROW(qb * QB), tb);
@@ -509,7 +531,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   for (int i = threadIdx.x; i < AT_ROWS; i += AT_THREADS) {
     const int kv = k0 + i;
     if constexpr (VARLEN)
-      sMask[i] = (kv < len) ? 0.0f : -INFINITY;
+      sMask[i] = (kv < kvlen) ? 0.0f : -INFINITY;
     else
       sMask[i] = (kv < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + kv]) : 0.0f) : -INFINITY;
   }
@@ -552,7 +574,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
         const float lse = ok ? __ldg(p.lse2 + HEAD_ROW(bh) + q) : INFINITY;
         const float dlt = ok ? __ldg(p.delta + HEAD_ROW(bh) + q) : 0.0f;
         uint32_t w = 0xFFFFFFFFu;
-        if (DROP && ok && k0 + r0 < (VARLEN ? len : p.Skv)) w = __ldg(p.dmask + (HEAD_ROW(bh) + q) * p.W + kw);
+        if (DROP && ok && k0 + r0 < (VARLEN ? kvlen : p.Skv)) w = __ldg(p.dmask + (HEAD_ROW(bh) + q) * p.W + kw);
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           const int e = hr * 2 + j;
@@ -580,8 +602,8 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     const int kv = k0 + r0 + g + hr * 8;
-    if (kv >= (VARLEN ? len : p.Skv)) continue;
-    const int64_t row = VARLEN ? static_cast<int64_t>(seq0) + kv : static_cast<int64_t>(b) * p.Skv + kv;
+    if (kv >= (VARLEN ? kvlen : p.Skv)) continue;
+    const int64_t row = VARLEN ? static_cast<int64_t>(kv0) + kv : static_cast<int64_t>(b) * p.Skv + kv;
     bf16* dK = p.out0 + row * p.ld0 + h * D;
     bf16* dV = p.out1 + row * p.ld1 + h * D;
 #pragma unroll
@@ -672,20 +694,27 @@ static int set_smem(const void* kern, int bytes, const char* who) {
 }
 
 // A tensor map over the [rows, heads * D] head columns of one operand: dense = B batches of S rows; packed (VARLEN) =
-// one batch of `total` rows, so that a tile at cu[b] + block * 64 never depends on B
+// one batch of `total` rows of its side, so that a tile at cu[b] + block * 64 never depends on B.  A packed side with no
+// rows has no valid map; the caller then passes the other side's map, which no CTA loads through (every sample's loop over
+// the empty side has no blocks).
 static int head_map(CUtensorMap* m, const void* ptr, int W, int64_t ld, int rows, int batches, int box_rows) {
   return make_tmap_3d(m, ptr, W, rows, batches, ld, ld * rows, 64, box_rows);
 }
 
 template <int D, bool VARLEN>
-static int attn_fwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream) {
+static int attn_fwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total, const int32_t* cu_kv, int total_kv,
+                           cudaStream_t stream) {
   const int W = a.heads * D;
-  const int nb = VARLEN ? 1 : a.B, rq = VARLEN ? total : a.Sq, rkv = VARLEN ? total : a.Skv;
+  const int nb = VARLEN ? 1 : a.B, rq = VARLEN ? total : a.Sq, rkv = VARLEN ? total_kv : a.Skv;
   CUtensorMap tmQ, tmK, tmV;
   int rc;
   if ((rc = head_map(&tmQ, a.q, W, a.ldq, rq, nb, AT_ROWS))) return rc;
-  if ((rc = head_map(&tmK, a.k, W, a.ldk, rkv, nb, AT_ROWS))) return rc;
-  if ((rc = head_map(&tmV, a.v, W, a.ldv, rkv, nb, AT_ROWS))) return rc;
+  if (rkv > 0) {
+    if ((rc = head_map(&tmK, a.k, W, a.ldk, rkv, nb, AT_ROWS))) return rc;
+    if ((rc = head_map(&tmV, a.v, W, a.ldv, rkv, nb, AT_ROWS))) return rc;
+  } else {
+    tmK = tmV = tmQ;                         // no keys at all: every sample writes zeros without loading a key block
+  }
   const int NKB = (a.Skv + AT_ROWS - 1) / AT_ROWS;
   const int smem = 5 * (D / 64) * AT_ROWS * 128 + NKB * AT_ROWS * 4 + 64 + 1024;
   AttnFwdDev p;
@@ -697,6 +726,7 @@ static int attn_fwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total
   p.dmask = a.drop_mask; p.W = (a.Skv + 31) / 32; p.dscale = a.drop_mask ? a.drop_scale : 1.0f;
   p.scale2 = LOG2E / sqrtf(static_cast<float>(D));
   p.cu = cu; p.total = total;
+  p.cu_kv = cu_kv; p.total_kv = total_kv;
   auto kern = attn_fwd_kernel<D, VARLEN>;
   static int smem_set = 0;
   if (smem > smem_set) {
@@ -712,19 +742,27 @@ static int attn_fwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total
 }
 
 template <int D, bool DROP, bool VARLEN>
-static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, int total, cudaStream_t stream) {
+static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, int total, int total_kv, cudaStream_t stream) {
   constexpr int QB = (D == 64) ? 64 : 32;   // query block of the dK/dV kernel: d = 128 keeps its tiles in registers
   const int W = a.heads * D;
-  const int nb = VARLEN ? 1 : a.B, rq = VARLEN ? total : a.Sq, rkv = VARLEN ? total : a.Skv;
+  const int nb = VARLEN ? 1 : a.B, rq = VARLEN ? total : a.Sq, rkv = VARLEN ? total_kv : a.Skv;
   CUtensorMap tmQ, tmK, tmV, tmdO, tmQc, tmdOc;
   int rc;
-  if ((rc = head_map(&tmQ, a.q, W, a.ldq, rq, nb, AT_ROWS))) return rc;
-  if ((rc = head_map(&tmdO, a.dctx, W, a.ld_dctx, rq, nb, AT_ROWS))) return rc;
-  if ((rc = head_map(&tmK, a.k, W, a.ldk, rkv, nb, AT_ROWS))) return rc;
-  if ((rc = head_map(&tmV, a.v, W, a.ldv, rkv, nb, AT_ROWS))) return rc;
+  // a packed side without rows borrows the other side's maps (never loaded through, see head_map); rq + rkv > 0
+  if (rq > 0) {
+    if ((rc = head_map(&tmQ, a.q, W, a.ldq, rq, nb, AT_ROWS))) return rc;
+    if ((rc = head_map(&tmdO, a.dctx, W, a.ld_dctx, rq, nb, AT_ROWS))) return rc;
+  }
+  if (rkv > 0) {
+    if ((rc = head_map(&tmK, a.k, W, a.ldk, rkv, nb, AT_ROWS))) return rc;
+    if ((rc = head_map(&tmV, a.v, W, a.ldv, rkv, nb, AT_ROWS))) return rc;
+  } else {
+    tmK = tmV = tmQ;
+  }
+  if (rq <= 0) tmQ = tmdO = tmK;
   tmQc = tmQ;
   tmdOc = tmdO;
-  if (QB != AT_ROWS) {
+  if (QB != AT_ROWS && rq > 0) {
     if ((rc = head_map(&tmQc, a.q, W, a.ldq, rq, nb, QB))) return rc;
     if ((rc = head_map(&tmdOc, a.dctx, W, a.ld_dctx, rq, nb, QB))) return rc;
   }
@@ -744,24 +782,31 @@ static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, int
     set_kv = true;
   }
   AttnBwdDev p = base;
-  p.out0 = reinterpret_cast<bf16*>(a.dq); p.ld0 = a.ld_dq; p.out1 = nullptr; p.ld1 = 0;
-  MMFB_LAUNCH((attn_bwd_dq_kernel<D, DROP, VARLEN>), dim3((a.Sq + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS, smem_q,
-              stream, tmQ, tmdO, tmK, tmV, p);
-  count_launch();
-  p.out0 = reinterpret_cast<bf16*>(a.dk); p.ld0 = a.ld_dk;
-  p.out1 = reinterpret_cast<bf16*>(a.dv); p.ld1 = a.ld_dv;
-  MMFB_LAUNCH((attn_bwd_dkv_kernel<D, DROP, QB, VARLEN>), dim3((a.Skv + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS,
-              smem_kv, stream, tmK, tmV, tmQc, tmdOc, p);
-  count_launch();
+  // dense: both always launch.  Packed: no query rows -> no dq kernel (the dk/dv kernel still writes every key row, as 0),
+  // no key rows -> no dk/dv kernel (the dq kernel writes every query row, as 0)
+  if (rq > 0 && a.Sq > 0) {
+    p.out0 = reinterpret_cast<bf16*>(a.dq); p.ld0 = a.ld_dq; p.out1 = nullptr; p.ld1 = 0;
+    MMFB_LAUNCH((attn_bwd_dq_kernel<D, DROP, VARLEN>), dim3((a.Sq + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS, smem_q,
+                stream, tmQ, tmdO, tmK, tmV, p);
+    count_launch();
+  }
+  if (rkv > 0 && a.Skv > 0) {
+    p.out0 = reinterpret_cast<bf16*>(a.dk); p.ld0 = a.ld_dk;
+    p.out1 = reinterpret_cast<bf16*>(a.dv); p.ld1 = a.ld_dv;
+    MMFB_LAUNCH((attn_bwd_dkv_kernel<D, DROP, QB, VARLEN>), dim3((a.Skv + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS,
+                smem_kv, stream, tmK, tmV, tmQc, tmdOc, p);
+    count_launch();
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "attn_bwd launch: %s", cudaGetErrorString(e));
   return MMFB_OK;
 }
 
 template <int D, bool VARLEN>
-static int attn_bwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream) {
+static int attn_bwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total, const int32_t* cu_kv, int total_kv,
+                           cudaStream_t stream) {
   // delta = rowsum(dO * O); packed rows are one batch of `total` query rows
-  {
+  if (!VARLEN || total > 0) {
     const int nb = VARLEN ? 1 : a.B, rq = VARLEN ? total : a.Sq;
     const int64_t warps = static_cast<int64_t>(nb) * rq;
     const int threads = 256;
@@ -778,8 +823,9 @@ static int attn_bwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total
   p.scale = 1.0f / sqrtf(static_cast<float>(D));
   p.scale2 = LOG2E * p.scale;
   p.cu = cu; p.total = total;
-  return a.drop_mask != nullptr ? attn_bwd_kernels<D, true, VARLEN>(a, p, total, stream)
-                                : attn_bwd_kernels<D, false, VARLEN>(a, p, total, stream);
+  p.cu_kv = cu_kv; p.total_kv = total_kv;
+  return a.drop_mask != nullptr ? attn_bwd_kernels<D, true, VARLEN>(a, p, total, total_kv, stream)
+                                : attn_bwd_kernels<D, false, VARLEN>(a, p, total, total_kv, stream);
 }
 
 // The dense entry points instantiate the dense kernels only, and attention_varlen.cu (which includes this file) the
@@ -790,8 +836,8 @@ int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream) {
   int rc = check_attn_common(a, "attn_fwd");
   if (rc) return rc;
   if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2) return set_error(MMFB_ERR_ARG, "attn_fwd: null pointer");
-  return a.head_dim == 64 ? attn_fwd_launch<64, false>(a, nullptr, 0, stream)
-                          : attn_fwd_launch<128, false>(a, nullptr, 0, stream);
+  return a.head_dim == 64 ? attn_fwd_launch<64, false>(a, nullptr, 0, nullptr, 0, stream)
+                          : attn_fwd_launch<128, false>(a, nullptr, 0, nullptr, 0, stream);
 }
 
 int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
@@ -799,8 +845,8 @@ int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
   if (rc) return rc;
   if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2 || !a.dctx || !a.delta || !a.dq || !a.dk || !a.dv)
     return set_error(MMFB_ERR_ARG, "attn_bwd: null pointer");
-  return a.head_dim == 64 ? attn_bwd_launch<64, false>(a, nullptr, 0, stream)
-                          : attn_bwd_launch<128, false>(a, nullptr, 0, stream);
+  return a.head_dim == 64 ? attn_bwd_launch<64, false>(a, nullptr, 0, nullptr, 0, stream)
+                          : attn_bwd_launch<128, false>(a, nullptr, 0, nullptr, 0, stream);
 }
 
 #else   // MMFB_ATTN_VARLEN_TU
@@ -821,8 +867,8 @@ int attn_varlen_fwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaS
   if (rc) return rc;
   if (total == 0) return MMFB_OK;           // every sample is empty: nothing to compute or write
   if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2) return set_error(MMFB_ERR_ARG, "attn_varlen_fwd: null pointer");
-  return a.head_dim == 64 ? attn_fwd_launch<64, true>(a, cu, total, stream)
-                          : attn_fwd_launch<128, true>(a, cu, total, stream);
+  return a.head_dim == 64 ? attn_fwd_launch<64, true>(a, cu, total, cu, total, stream)
+                          : attn_fwd_launch<128, true>(a, cu, total, cu, total, stream);
 }
 
 int attn_varlen_bwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream) {
@@ -831,8 +877,49 @@ int attn_varlen_bwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaS
   if (total == 0) return MMFB_OK;
   if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2 || !a.dctx || !a.delta || !a.dq || !a.dk || !a.dv)
     return set_error(MMFB_ERR_ARG, "attn_varlen_bwd: null pointer");
-  return a.head_dim == 64 ? attn_bwd_launch<64, true>(a, cu, total, stream)
-                          : attn_bwd_launch<128, true>(a, cu, total, stream);
+  return a.head_dim == 64 ? attn_bwd_launch<64, true>(a, cu, total, cu, total, stream)
+                          : attn_bwd_launch<128, true>(a, cu, total, cu, total, stream);
+}
+
+// Packed cross-attention: queries from one packing (cu_q / total_q, Sq = max_q), keys and values from another (cu_kv /
+// total_kv, Skv = max_kv).  Either side of a sample may be empty, and so may a whole side; Sq / Skv = 0 are legal then.
+static int check_varlen_cross(const mmfb_attn_args& a, const int32_t* cu_q, int total_q, const int32_t* cu_kv, int total_kv,
+                              const char* who) {
+  if (a.B <= 0 || a.heads <= 0 || a.Sq < 0 || a.Skv < 0)
+    return set_error(MMFB_ERR_ARG, "%s: B and heads must be positive, Sq and Skv not negative", who);
+  if (a.head_dim != 64 && a.head_dim != 128)
+    return set_error(MMFB_ERR_ARG, "%s: head_dim must be 64 or 128 (got %d)", who, a.head_dim);
+  const int max_kv = a.head_dim == 64 ? 384 : 256;
+  if (a.Skv > max_kv)
+    return set_error(MMFB_ERR_ARG, "%s: Skv=%d exceeds the single-pass limit %d for head_dim %d", who, a.Skv, max_kv,
+                     a.head_dim);
+  if (a.mask != nullptr) return set_error(MMFB_ERR_ARG, "%s: mask must be NULL (packing has removed the masked keys)", who);
+  if (!cu_q || !cu_kv) return set_error(MMFB_ERR_ARG, "%s: null cu_q / cu_kv", who);
+  if (total_q < 0 || total_kv < 0) return set_error(MMFB_ERR_ARG, "%s: negative total (%d, %d)", who, total_q, total_kv);
+  return MMFB_OK;
+}
+
+int attn_varlen_cross_fwd(const mmfb_attn_args& a, const int32_t* cu_q, int total_q, const int32_t* cu_kv, int total_kv,
+                          cudaStream_t stream) {
+  int rc = check_varlen_cross(a, cu_q, total_q, cu_kv, total_kv, "attn_varlen_cross_fwd");
+  if (rc) return rc;
+  if (total_q == 0 || a.Sq == 0) return MMFB_OK;   // no query row: nothing to write
+  if (!a.q || !a.ctx || !a.lse2 || (total_kv > 0 && (!a.k || !a.v)))
+    return set_error(MMFB_ERR_ARG, "attn_varlen_cross_fwd: null pointer");
+  return a.head_dim == 64 ? attn_fwd_launch<64, true>(a, cu_q, total_q, cu_kv, total_kv, stream)
+                          : attn_fwd_launch<128, true>(a, cu_q, total_q, cu_kv, total_kv, stream);
+}
+
+int attn_varlen_cross_bwd(const mmfb_attn_args& a, const int32_t* cu_q, int total_q, const int32_t* cu_kv, int total_kv,
+                          cudaStream_t stream) {
+  int rc = check_varlen_cross(a, cu_q, total_q, cu_kv, total_kv, "attn_varlen_cross_bwd");
+  if (rc) return rc;
+  if (total_q == 0 && total_kv == 0) return MMFB_OK;
+  if ((total_q > 0 && (!a.q || !a.ctx || !a.lse2 || !a.dctx || !a.delta || !a.dq)) ||
+      (total_kv > 0 && (!a.k || !a.v || !a.dk || !a.dv)))
+    return set_error(MMFB_ERR_ARG, "attn_varlen_cross_bwd: null pointer");
+  return a.head_dim == 64 ? attn_bwd_launch<64, true>(a, cu_q, total_q, cu_kv, total_kv, stream)
+                          : attn_bwd_launch<128, true>(a, cu_q, total_q, cu_kv, total_kv, stream);
 }
 #endif  // MMFB_ATTN_VARLEN_TU
 

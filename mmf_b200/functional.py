@@ -229,6 +229,107 @@ def attention_varlen_bwd(dctx, q, k, v, ctx, lse2, cu_seqlens, max_len, heads, d
     return dq, dk, dv
 
 
+def _cu_check(cu, name):
+    if not isinstance(cu, torch.Tensor) or cu.dtype != torch.int32:
+        raise ValueError("%s must be an int32 tensor" % name)
+    if cu.dim() != 1 or cu.numel() < 2 or not cu.is_contiguous():
+        raise ValueError("%s must be a contiguous int32 vector [B+1] with B >= 1, got shape %s" % (name, tuple(cu.shape)))
+    if not cu.is_cuda:
+        raise RuntimeError("%s must be a CUDA tensor: the kernels read it on the device" % name)
+
+
+def _varlen_cross_args(q, k, v, cu_q, cu_kv, max_q, max_kv, heads, drop_mask, drop_scale):
+    """packed cross-attention operands: q [total_q, h*d] rows delimited by cu_q, k/v [total_kv, h*d] rows delimited by cu_kv
+    (int32 [B+1] each, same B)"""
+    _cu_check(cu_q, "cu_q")
+    _cu_check(cu_kv, "cu_kv")
+    if cu_q.numel() != cu_kv.numel():
+        raise ValueError("cu_q and cu_kv must describe the same number of samples (%d vs %d)"
+                         % (cu_q.numel() - 1, cu_kv.numel() - 1))
+    for t, n in ((q, "q"), (k, "k"), (v, "v")):
+        _req(t, torch.bfloat16, n)
+        if t.dim() != 2:
+            raise ValueError("attention_varlen_cross: %s must be 2-D [rows, heads*head_dim]" % n)
+    total_q, W = q.shape
+    total_kv = k.shape[0]
+    if v.shape[0] != total_kv:
+        raise ValueError("attention_varlen_cross: k and v must hold the same number of rows (%d vs %d)" % (total_kv, v.shape[0]))
+    if k.shape[1] != W or v.shape[1] != W:
+        raise ValueError("attention_varlen_cross: q, k and v must have the same width")
+    if W % heads:
+        raise ValueError(
+            "The hidden size (%d) is not a multiple of the number of attention heads (%d)" % (W, heads))
+    max_q, max_kv = int(max_q), int(max_kv)
+    a = AttnArgs()
+    a.q, a.ldq = q.data_ptr(), q.stride(0)
+    a.k, a.ldk = k.data_ptr(), k.stride(0)
+    a.v, a.ldv = v.data_ptr(), v.stride(0)
+    if drop_mask is not None:
+        _req(drop_mask, torch.int32, "drop_mask")
+        if tuple(drop_mask.shape) != (heads, total_q, (max_kv + 31) // 32) or not drop_mask.is_contiguous():
+            raise ValueError("attention_varlen_cross: drop_mask must be contiguous int32 [heads, total_q, ceil(max_kv/32)]")
+        a.drop_mask, a.drop_scale = drop_mask.data_ptr(), float(drop_scale)
+    a.B, a.heads, a.Sq, a.Skv, a.head_dim = cu_q.numel() - 1, heads, max_q, max_kv, W // heads
+    return a, total_q, total_kv, W
+
+
+def attention_varlen_cross_fwd(q, k, v, cu_q, cu_kv, max_q, max_kv, heads, drop_mask=None, drop_scale=1.0, out=None,
+                               save_lo=False):
+    """Packed cross-attention: ctx, lse2 (, ctx_lo).  Sample b's queries are rows [cu_q[b], cu_q[b+1]) of q [total_q, h*d]
+    and attend to its keys, rows [cu_kv[b], cu_kv[b+1]) of k / v [total_kv, h*d] (views allowed); max_q / max_kv bound the
+    lengths.  lse2 is fp32 [heads, total_q].  A sample without keys gets ctx = ctx_lo = 0.  Nothing here synchronises."""
+    a, total_q, total_kv, W = _varlen_cross_args(q, k, v, cu_q, cu_kv, max_q, max_kv, heads, drop_mask, drop_scale)
+    ctx = out if out is not None else torch.empty(total_q, W, dtype=torch.bfloat16, device=q.device)
+    _req(ctx, torch.bfloat16, "out")
+    if ctx.shape[0] != total_q:
+        raise ValueError("attention_varlen_cross: out must hold total_q=%d rows" % total_q)
+    lse2 = torch.empty(heads, total_q, dtype=torch.float32, device=q.device)
+    a.ctx, a.ldo, a.lse2 = ctx.data_ptr(), ctx.stride(0), lse2.data_ptr()
+    ctx_lo = None
+    if save_lo:
+        ctx_lo = torch.empty(total_q, W, dtype=torch.bfloat16, device=q.device)
+        a.ctx_lo = ctx_lo.data_ptr()
+    check(LIB.mmfb_attention_varlen_cross_fwd(ctypes.byref(a), cu_q.data_ptr(), total_q, cu_kv.data_ptr(), total_kv,
+                                              _stream_ptr()))
+    if save_lo:
+        return ctx, lse2, ctx_lo
+    return ctx, lse2
+
+
+def attention_varlen_cross_bwd(dctx, q, k, v, ctx, lse2, cu_q, cu_kv, max_q, max_kv, heads, drop_mask=None, drop_scale=1.0,
+                               dq=None, dk=None, dv=None, ctx_lo=None):
+    """dq [total_q, h*d], dk, dv [total_kv, h*d] of attention_varlen_cross_fwd (probabilities recomputed from the saved lse2
+    [heads, total_q]).  Key rows of a sample without queries get dk = dv = 0."""
+    a, total_q, total_kv, W = _varlen_cross_args(q, k, v, cu_q, cu_kv, max_q, max_kv, heads, drop_mask, drop_scale)
+    _req(dctx, torch.bfloat16, "dctx")
+    _req(ctx, torch.bfloat16, "ctx")
+    if dctx.shape[0] != total_q or ctx.shape[0] != total_q:
+        raise ValueError("attention_varlen_cross: dctx and ctx must hold total_q=%d rows" % total_q)
+    if not lse2.is_cuda or lse2.dtype != torch.float32 or tuple(lse2.shape) != (heads, total_q) or not lse2.is_contiguous():
+        raise ValueError("attention_varlen_cross: lse2 must be contiguous fp32 [heads, total_q]")
+    dq = dq if dq is not None else torch.empty(total_q, W, dtype=torch.bfloat16, device=q.device)
+    dk = dk if dk is not None else torch.empty(total_kv, W, dtype=torch.bfloat16, device=q.device)
+    dv = dv if dv is not None else torch.empty(total_kv, W, dtype=torch.bfloat16, device=q.device)
+    for t, n, rows in ((dq, "dq", total_q), (dk, "dk", total_kv), (dv, "dv", total_kv)):
+        _req(t, torch.bfloat16, n)
+        if t.shape[0] != rows:
+            raise ValueError("attention_varlen_cross: %s must hold %d rows" % (n, rows))
+    delta = torch.empty(heads, total_q, dtype=torch.float32, device=q.device)
+    a.ctx, a.ldo, a.lse2 = ctx.data_ptr(), ctx.stride(0), lse2.data_ptr()
+    a.dctx, a.ld_dctx, a.delta = dctx.data_ptr(), dctx.stride(0), delta.data_ptr()
+    if ctx_lo is not None:
+        _req(ctx_lo, torch.bfloat16, "ctx_lo")
+        if not ctx_lo.is_contiguous() or tuple(ctx_lo.shape) != (total_q, W):
+            raise ValueError("ctx_lo must be contiguous [total_q, heads*head_dim]")
+        a.ctx_lo = ctx_lo.data_ptr()
+    a.dq, a.ld_dq = dq.data_ptr(), dq.stride(0)
+    a.dk, a.ld_dk = dk.data_ptr(), dk.stride(0)
+    a.dv, a.ld_dv = dv.data_ptr(), dv.stride(0)
+    check(LIB.mmfb_attention_varlen_cross_bwd(ctypes.byref(a), cu_q.data_ptr(), total_q, cu_kv.data_ptr(), total_kv,
+                                              _stream_ptr()))
+    return dq, dk, dv
+
+
 def pack_keep_bits(keep):
     """bool [..., n] -> int32 [..., ceil(n/32)] keep-bit words (bit j of word w = element 32*w + j)."""
     n = keep.shape[-1]

@@ -44,6 +44,10 @@ class GraphedStep:
         if any(getattr(m.__dict__.get("_runner"), "skip_padding", False) for m in model.modules()):
             raise RuntimeError("GraphedStep: the model has skip_padding encoders, which read the token count on the host and "
                                "cannot be captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)")
+        if any(getattr(m.__dict__.get("_runner"), "pack_streams", False) for m in model.modules()):
+            raise RuntimeError("GraphedStep: the model has two-stream encoders with pack_streams set, which read the token "
+                               "counts on the host and cannot be captured; turn them off with "
+                               "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)")
         self.model, self.loss_fn = model, loss_fn
         self.static = _map(lambda t: t.detach().clone(), example_batch)
         dev = next(t for t in _flatten(self.static) if t.is_cuda).device

@@ -135,6 +135,9 @@ def _load():
     lib.mmfb_cast_f32_bf16.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
     for name in ("mmfb_attention_varlen_fwd", "mmfb_attention_varlen_bwd"):
         getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
+    for name in ("mmfb_attention_varlen_cross_fwd", "mmfb_attention_varlen_cross_bwd"):
+        getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
+                                       ctypes.c_void_p]
     return lib
 
 

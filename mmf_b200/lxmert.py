@@ -16,7 +16,8 @@ from torch import nn
 from . import engine as E
 from . import ops
 from .modules import (B200BertAttention, B200BertIntermediate, B200BertLayer, B200BertSelfAttention,
-                      B200BertSelfOutput, _Holder, _fresh_dropout_state, _init_bert_weights, _require_cuda)
+                      B200BertSelfOutput, _Holder, _Packing, _fresh_dropout_state, _init_bert_weights, _require_cuda,
+                      plan_two_stream)
 
 
 class B200VisualFeatEncoder(nn.Module):
@@ -78,6 +79,8 @@ class LxmertRunner:
         self.pack = None
         self.w = None
         self.grad_ready_hook = None
+        # skip padded tokens in both streams (modules.plan_two_stream): every layer runs on each stream's valid rows only
+        self.pack_streams = False
 
     def _mod(self, kind, i):
         return {"l": self.layer, "r": self.r_layers, "x": self.x_layers}[kind][i]
@@ -146,7 +149,11 @@ class _LxmertEncoderFn(torch.autograd.Function):
         runner.pack.refresh()
         l = lang.detach().to(torch.bfloat16).contiguous().view(B * T, H)
         v = visn.detach().to(torch.bfloat16).contiguous().view(B * R, H)
-        l, v, saved = runner.forward(l, v, lmask, vmask, B, T, R, training, need_grad)
+        if isinstance(lmask, _Packing):
+            l, v, saved = runner.forward(lmask.pack(l), vmask.pack(v), lmask.varlen, vmask.varlen, B, T, R, training, need_grad)
+            l, v = lmask.unpack(l, B * T), vmask.unpack(v, B * R)
+        else:
+            l, v, saved = runner.forward(l, v, lmask, vmask, B, T, R, training, need_grad)
         ctx.runner, ctx.saved, ctx.masks, ctx.dims, ctx.dtypes = runner, saved, (lmask, vmask), (B, T, R, H), (lang.dtype, visn.dtype)
         return l.view(B, T, H).to(lang.dtype), v.view(B, R, H).to(visn.dtype)
 
@@ -160,7 +167,12 @@ class _LxmertEncoderFn(torch.autograd.Function):
         dev = runner.pack.device
         dl = (dlang if dlang is not None else torch.zeros(B, T, H, device=dev)).to(torch.bfloat16).contiguous().view(B * T, H)
         dv = (dvisn if dvisn is not None else torch.zeros(B, R, H, device=dev)).to(torch.bfloat16).contiguous().view(B * R, H)
-        dl, dv = runner.backward(dl, dv, ctx.saved, ctx.masks[0], ctx.masks[1], B, T, R)
+        lm, vm = ctx.masks
+        if isinstance(lm, _Packing):
+            dl, dv = runner.backward(lm.pack(dl), vm.pack(dv), ctx.saved, lm.varlen, vm.varlen, B, T, R)
+            dl, dv = lm.unpack(dl, B * T), vm.unpack(dv, B * R)
+        else:
+            dl, dv = runner.backward(dl, dv, ctx.saved, lm, vm, B, T, R)
         ctx.saved = None
         return (None, None, None, None, dl.view(B, T, H).to(ctx.dtypes[0]), dv.view(B, R, H).to(ctx.dtypes[1])) + tuple(
             runner.pack.autograd_grads(aliased))
@@ -182,6 +194,7 @@ class B200LXMERTEncoder(nn.Module):
         self.r_layers = nn.ModuleList([mk() for _ in range(self.num_r_layers)])
         _init_bert_weights(self, float(getattr(config, "initializer_range", 0.02)))
         self._runner = LxmertRunner(self.layer, self.r_layers, self.x_layers)
+        self._runner.pack_streams = bool(getattr(config, "skip_padding", False))
 
     def forward(self, lang_feats, lang_attention_mask, visn_feats, visn_attention_mask=None):
         _require_cuda(lang_feats, "lang_feats")
@@ -191,5 +204,11 @@ class B200LXMERTEncoder(nn.Module):
         self._runner.ensure(lang_feats.device)
         lmask = E.additive_mask_2d(lang_attention_mask, B, T)
         vmask = E.additive_mask_2d(visn_attention_mask, B, R)
-        return _LxmertEncoderFn.apply(self._runner, lmask, vmask, self.training, lang_feats, visn.to(lang_feats.dtype),
-                                      *self._runner.pack.params)
+        visn = visn.to(lang_feats.dtype)
+        if self._runner.pack_streams:
+            plan = plan_two_stream(lmask, vmask, B, T, R, lang_feats.device)
+            if plan == "empty":       # every token of both streams is padding: outputs and input gradients are zeros
+                return lang_feats * 0, visn * 0
+            if plan is not None:
+                lmask, vmask = plan
+        return _LxmertEncoderFn.apply(self._runner, lmask, vmask, self.training, lang_feats, visn, *self._runner.pack.params)

@@ -129,34 +129,52 @@ class EncoderRunner:
 
 class _Packing:
     """Valid rows of a padded [B, S] batch: `rows` (int64 [total]) are their flat indices in sample order, `varlen` the
-    descriptor the engine's attention reads."""
+    descriptor the engine's attention reads.  rows = None is the trivial packing of an unpadded stream (every row, in
+    place), which packs and unpacks without a copy."""
 
     def __init__(self, rows, varlen):
         self.rows, self.varlen = rows, varlen
 
     def pack(self, t):
         """[B*S, H] -> [total, H]: the valid rows, in their original order within each sample"""
-        return t.index_select(0, self.rows)
+        return t if self.rows is None else t.index_select(0, self.rows)
 
     def unpack(self, t, BS):
         """[total, H] -> [B*S, H] with exact zero rows at padded positions"""
-        return t.new_zeros(BS, t.shape[1]).index_copy_(0, self.rows, t)
+        return t if self.rows is None else t.new_zeros(BS, t.shape[1]).index_copy_(0, self.rows, t)
 
 
-def _plan_packing(mask, B, S):
-    """The packing of an additive [B, S] fp32 mask (0 = token, <= -10000 = padding), or None when no row is padded.
-    One device-to-host copy fetches the counts; the row indices are built on the device without another one."""
+def _no_capture(what):
     if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
-        raise RuntimeError("skip_padding cannot run under CUDA-graph capture: packing needs the valid-token count on the host "
-                           "(turn it off with mmf_b200.patch.set_skip_padding(model, False) before capturing)")
+        raise RuntimeError("%s cannot run under CUDA-graph capture: packing needs the valid-token count on the host "
+                           "(turn it off with mmf_b200.patch.set_skip_padding(model, False) before capturing)" % what)
+
+
+def _mask_counts(mask):
+    """device side of a packing plan: (valid [B, S], lens int32 [B], int64 [3] = soft values, total, max_len)"""
     valid = mask == 0
     lens = valid.sum(1, dtype=torch.int32)
     soft = ((mask != 0) & (mask > -10000.0)).sum()
-    n_soft, total, max_len = (int(v) for v in torch.stack([soft.to(torch.int64), lens.sum(dtype=torch.int64),
-                                                           lens.max().to(torch.int64)]).tolist())
+    return valid, lens, torch.stack([soft.to(torch.int64), lens.sum(dtype=torch.int64), lens.max().to(torch.int64)])
+
+
+def _check_soft(n_soft, what="skip_padding"):
     if n_soft:
-        raise ValueError("skip_padding needs a key-padding mask of 0 (token) and <= -10000 (padding); %d value(s) are a "
-                         "soft bias, which cannot be packed away" % n_soft)
+        raise ValueError("%s needs a key-padding mask of 0 (token) and <= -10000 (padding); %d value(s) are a "
+                         "soft bias, which cannot be packed away" % (what, n_soft))
+
+
+def _plan_packing(mask, B, S, counts=None):
+    """The packing of an additive [B, S] fp32 mask (0 = token, <= -10000 = padding), or None when no row is padded.
+    One device-to-host copy fetches the counts; the row indices are built on the device without another one.  `counts` =
+    (valid, lens, (n_soft, total, max_len) on the host) when the caller has already fetched them (two-stream plans fetch
+    both streams' counts in one copy)."""
+    if counts is None:
+        _no_capture("skip_padding")
+        valid, lens, st = _mask_counts(mask)
+        counts = (valid, lens, tuple(int(v) for v in st.tolist()))
+    valid, lens, (n_soft, total, max_len) = counts
+    _check_soft(n_soft)
     if total == B * S:
         return None
     cu = torch.zeros(B + 1, dtype=torch.int32, device=mask.device)
@@ -166,6 +184,52 @@ def _plan_packing(mask, B, S):
     rows = torch.empty(total + 1, dtype=torch.int64, device=mask.device)
     rows.scatter_(0, dest, torch.arange(B * S, device=mask.device))     # padded rows all land in the spare last slot
     return _Packing(rows[:total], E.Varlen(cu, B, total, max_len))
+
+
+def _trivial_packing(B, S, device):
+    """every row of an unpadded [B, S] stream, as a packing: cu = arange(B+1) * S"""
+    cu = (torch.arange(B + 1, dtype=torch.int32, device=device) * S).contiguous()
+    return _Packing(None, E.Varlen(cu, B, B * S, S))
+
+
+def plan_two_stream(mask_a, mask_b, B, Sa, Sb, device):
+    """Packing of a two-stream encoder call (ViLBERT, LXMERT) from the additive key-padding masks of its streams ([B, Sa],
+    [B, Sb] fp32, or None = no padding).  Returns
+      None            - nothing is padded, or some sample has tokens in one stream and none in the other: the dense path
+                        runs.  (There those queries attend over the other stream's padded rows and the valid outputs depend
+                        on them, so packing would change the function, not just skip work);
+      "empty"         - every row of both streams is padding: the outputs and input gradients are zeros;
+      (pack_a, pack_b) - a packing per stream; an unpadded stream gets the trivial one.
+    Both streams' counts reach the host in one device-to-host copy.  A soft mask raises ValueError; stream capture raises
+    RuntimeError."""
+    if mask_a is None and mask_b is None:
+        return None
+    _no_capture("pack_streams")
+    counts, stats = [], []
+    for m, S in ((mask_a, Sa), (mask_b, Sb)):
+        if m is None:
+            counts.append((None, torch.full((B,), S, dtype=torch.int32, device=device)))
+            stats.append(torch.tensor([0, B * S, S], dtype=torch.int64, device=device))
+        else:
+            valid, lens, st = _mask_counts(m)
+            counts.append((valid, lens))
+            stats.append(st)
+    one_sided = ((counts[0][1] > 0) != (counts[1][1] > 0)).sum().to(torch.int64).reshape(1)
+    host = torch.cat(stats + [one_sided]).tolist()            # the one device-to-host copy
+    st_a, st_b, n_one_sided = tuple(host[0:3]), tuple(host[3:6]), host[6]
+    _check_soft(st_a[0], "pack_streams")
+    _check_soft(st_b[0], "pack_streams")
+    if st_a[1] == B * Sa and st_b[1] == B * Sb:
+        return None
+    if st_a[1] == 0 and st_b[1] == 0:
+        return "empty"
+    if n_one_sided:
+        return None
+    plans = []
+    for m, S, (valid, lens), st in ((mask_a, Sa, counts[0], st_a), (mask_b, Sb, counts[1], st_b)):
+        plan = None if m is None else _plan_packing(m, B, S, counts=(valid, lens, st))
+        plans.append(plan if plan is not None else _trivial_packing(B, S, device))
+    return tuple(plans)
 
 
 class _BertEncoderFn(torch.autograd.Function):
@@ -391,6 +455,9 @@ class VilbertRunner:
         self.steps = vilbert_schedule(list(v_ids), list(t_ids), len(self.layer), len(self.v_layer))
         self.pack = None
         self.grad_ready_hook = None
+        # skip padded tokens in both streams: pack each stream's valid rows once per encoder call and run variable-length
+        # self- and cross-attention (plan_two_stream)
+        self.pack_streams = False
 
     def ensure(self, device):
         if self.pack is not None and self.pack.intact() and self.pack.device == device:
@@ -466,7 +533,13 @@ class _VilbertEncoderFn(torch.autograd.Function):
         t = txt.detach().to(torch.bfloat16).contiguous().view(B * T, Ht)
         v = img.detach().to(torch.bfloat16).contiguous().view(B * R, Hv)
         blocks = [] if want_blocks else None
-        t, v, saved = runner.forward(t, v, tmask, imask, B, T, R, training, need_grad, blocks)
+        if isinstance(tmask, _Packing):             # both streams run on their valid rows only
+            t, v, saved = runner.forward(tmask.pack(t), imask.pack(v), tmask.varlen, imask.varlen, B, T, R, training,
+                                         need_grad, blocks)
+            t, v = tmask.unpack(t, B * T), imask.unpack(v, B * R)
+            blocks = [(tmask.unpack(bt, B * T), imask.unpack(bv, B * R)) for bt, bv in blocks] if want_blocks else blocks
+        else:
+            t, v, saved = runner.forward(t, v, tmask, imask, B, T, R, training, need_grad, blocks)
         ctx.runner, ctx.saved, ctx.masks, ctx.dims, ctx.dtypes = runner, saved, (tmask, imask), (B, T, R, Ht, Hv), (txt.dtype, img.dtype)
         outs = [t.view(B, T, Ht).to(txt.dtype), v.view(B, R, Hv).to(img.dtype)]
         if want_blocks:
@@ -484,7 +557,12 @@ class _VilbertEncoderFn(torch.autograd.Function):
         aliased = runner.pack.prepare_grads()
         dt = (dtxt if dtxt is not None else torch.zeros(B, T, Ht, device=runner.pack.device)).to(torch.bfloat16).contiguous().view(B * T, Ht)
         dv = (dimg if dimg is not None else torch.zeros(B, R, Hv, device=runner.pack.device)).to(torch.bfloat16).contiguous().view(B * R, Hv)
-        dt, dv = runner.backward(dt, dv, ctx.saved, ctx.masks[0], ctx.masks[1], B, T, R)
+        tm, im = ctx.masks
+        if isinstance(tm, _Packing):
+            dt, dv = runner.backward(tm.pack(dt), im.pack(dv), ctx.saved, tm.varlen, im.varlen, B, T, R)
+            dt, dv = tm.unpack(dt, B * T), im.unpack(dv, B * R)
+        else:
+            dt, dv = runner.backward(dt, dv, ctx.saved, tm, im, B, T, R)
         ctx.saved = None
         return (None, None, None, None, None, dt.view(B, T, Ht).to(ctx.dtypes[0]), dv.view(B, R, Hv).to(ctx.dtypes[1])) + tuple(
             runner.pack.autograd_grads(aliased))
@@ -518,6 +596,7 @@ class B200ViLBertEncoder(nn.Module):
         self.c_layer = nn.ModuleList([B200ConnectionLayer(config) for _ in range(len(self.v_biattention_id))])
         _init_bert_weights(self, float(getattr(config, "initializer_range", 0.02)))
         self._runner = VilbertRunner(self.layer, self.v_layer, self.c_layer, self.v_biattention_id, self.t_biattention_id)
+        self._runner.pack_streams = bool(getattr(config, "skip_padding", False))
 
     def forward(self, txt_embedding, image_embedding, txt_attention_mask, txt_attention_mask2, image_attention_mask,
                 co_attention_mask=None, output_all_encoded_layers=True, output_all_attention_masks=False):
@@ -535,6 +614,17 @@ class B200ViLBertEncoder(nn.Module):
         self._runner.ensure(txt_embedding.device)
         tmask = E.additive_mask_2d(txt_attention_mask, B, T)
         imask = E.additive_mask_2d(image_attention_mask, B, R)
+        if self._runner.pack_streams:
+            plan = plan_two_stream(tmask, imask, B, T, R, txt_embedding.device)
+            if plan == "empty":
+                # every token of both streams is padding: every output (and input-gradient) row is zero
+                zt, zi = txt_embedding * 0, image_embedding * 0
+                if output_all_encoded_layers:
+                    n = len(self.c_layer)
+                    return [zt.detach()] * n, [zi.detach()] * n, ([], [], [])
+                return [zt], [zi], ([], [], [])
+            if plan is not None:
+                tmask, imask = plan
         outs = _VilbertEncoderFn.apply(self._runner, tmask, imask, self.training, bool(output_all_encoded_layers),
                                        txt_embedding, image_embedding, *self._runner.pack.params)
         if output_all_encoded_layers:

@@ -7,10 +7,12 @@ re-homed into the engine's flat pack on the first CUDA forward.
 
 `set_skip_padding()` switches the single-stream encoders of a model to packed execution: padded tokens are removed once
 per encoder call and attention runs over each sample's own tokens (variable-length kernels), so padding costs nothing.
+With `two_stream=True` it also packs both streams of the ViLBERT and LXMERT encoders (variable-length cross-attention).
 """
 import types
 
-from .modules import EncoderRunner, run_bert_encoder
+from .lxmert import LxmertRunner
+from .modules import EncoderRunner, VilbertRunner, run_bert_encoder
 
 _saved = {}
 
@@ -74,15 +76,20 @@ def _routed(m):
     return getattr(f, "__func__", f) is _b200_encoder_forward
 
 
-def set_skip_padding(module, enabled=True):
+def set_skip_padding(module, enabled=True, two_stream=False):
     """Sets `skip_padding` on every single-stream encoder runner under `module` (B200BertEncoder - and so VisualBERT, MMBT,
     UNITER, VinVL and the TransformerEncoder plugin -, VisualBERT's bypass `additional_layer`, encoders routed by
-    attach_encoder / replace_with_b200) and returns how many it set.  ViLBERT, LXMERT and ViT runners are left alone.
+    attach_encoder / replace_with_b200) and returns how many it set.  ViLBERT, LXMERT and ViT runners are left alone unless
+    `two_stream` is True: then `pack_streams` is set on every ViLBERT and LXMERT runner too, and they count as well.  ViT
+    runners are always left alone.
 
     With the flag on, an encoder call with a key-padding mask runs on the valid rows only: its outputs (and the input
     gradient) are exactly zero at padded positions instead of the values the dense path computes there.  For any loss that
     does not read padded positions it computes the same function and gradients as the dense path, up to rounding and the
-    dropout masks drawn.  It reads the token count on the host, so it cannot be captured in a CUDA graph."""
+    dropout masks drawn.  It reads the token count on the host, so it cannot be captured in a CUDA graph.
+
+    A two-stream call falls back to the dense path when some sample has tokens in one stream and none in the other: there
+    the dense outputs of those tokens depend on the other stream's padded rows."""
     n = 0
     for m in module.modules():
         r = m.__dict__.get("_runner")
@@ -90,5 +97,8 @@ def set_skip_padding(module, enabled=True):
             r = _runner_of(m)
         if type(r) is EncoderRunner:
             r.skip_padding = bool(enabled)
+            n += 1
+        elif two_stream and isinstance(r, (VilbertRunner, LxmertRunner)):
+            r.pack_streams = bool(enabled)
             n += 1
     return n
