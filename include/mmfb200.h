@@ -137,6 +137,22 @@ int mmfb_attention_varlen_cross_fwd(const mmfb_attn_args* args, const int32_t* c
 int mmfb_attention_varlen_cross_bwd(const mmfb_attn_args* args, const int32_t* cu_q, int total_q, const int32_t* cu_kv,
                                     int total_kv, mmfb_stream stream);
 
+/* Attention probabilities of one DENSE mmfb_attention_fwd call, for inspection (the reference's output_attentions /
+ * ViLBERT visualization outputs, hf_layers.py:196-210, vilbert.py:94-112, 419-475):
+ *   probs[b, h, q, k] = exp2(S[b,h,q,k] * log2(e)/sqrt(d) + M'[b,k] - lse2[b,h,q])      (* keep(b,h,q,k) * drop_scale)
+ * S = Q K^T of the call's q / k head slices, M' = log2(e) * max(mask[b,k], -10000) (the clamp of the forward and backward),
+ * lse2 the row statistics that forward wrote.  Pass the inputs of that forward: q, ldq, k, ldk, mask, lse2, drop_mask,
+ * drop_scale, B, heads, Sq, Skv, head_dim; v, ctx and the backward fields are not read.
+ *   probs: DEVICE buffer, contiguous [B, heads, Sq, Skv], fp32 (probs_dtype = MMFB_PROBS_F32) or bf16 (MMFB_PROBS_BF16),
+ *   aligned to its element size.  Every element is written and nothing outside it.
+ *   Without drop_mask a row sums to 1 (up to rounding).  With drop_mask (the keep bits the forward used) it is the
+ *   post-dropout probability the reference returns in train mode: dropped entries are exactly 0 and kept ones are
+ *   scaled by drop_scale = 1/(1-p).
+ * Returns MMFB_ERR_ARG for a bad dtype, a null pointer or a shape mmfb_attention_fwd rejects.  One kernel launch; limits as
+ * mmfb_attention_fwd.  There is no packed (varlen) variant. */
+enum { MMFB_PROBS_F32 = 0, MMFB_PROBS_BF16 = 1 };
+int mmfb_attention_probs(const mmfb_attn_args* args, void* probs, int probs_dtype, mmfb_stream stream);
+
 /* LayerNorm over the last dimension (eps 1e-12 on this path), one warp per row.
  * fwd: x = LN(y)*gamma + beta, optional dropout on x (embeddings), saves mean / rstd (fp32 [M]).
  * bwd: dy = dLN(dx (+dx2)); dz = dropout-backward(dy) for the dense branch that fed y = dropout(dense)+resid;

@@ -618,7 +618,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 // elements is owned by D/8 consecutive lanes and reduced with shuffles (coalesced 512 B / 1 KB per warp access).
 // Every row is a query row of some sample, so the packed layout [H, total] is this kernel's own with B = 1, Sq = total:
 // the varlen backward launches it unchanged (it is defined once, in the dense translation unit).
-#ifdef MMFB_ATTN_VARLEN_TU
+#if defined(MMFB_ATTN_VARLEN_TU) || defined(MMFB_ATTN_PROBS_TU)
 __global__ void attn_delta_kernel(const bf16* __restrict__ dO, int64_t ld_do, const bf16* __restrict__ O,
                                   int64_t ld_o, const bf16* __restrict__ Olo, float* __restrict__ delta, int B, int H,
                                   int Sq, int D);
@@ -671,7 +671,7 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ dO, int64_t ld_do, co
   }
 }
 
-#endif  // MMFB_ATTN_VARLEN_TU
+#endif  // MMFB_ATTN_VARLEN_TU || MMFB_ATTN_PROBS_TU
 
 // ----------------------------------------------------------------------------------------------
 // host
@@ -830,8 +830,9 @@ static int attn_bwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total
 
 // The dense entry points instantiate the dense kernels only, and attention_varlen.cu (which includes this file) the
 // packed ones: instantiated in one translation unit, the two share inlined helpers that the compiler then schedules
-// differently, and the dense d = 64 forward would not keep the code it has without the packed mode.
-#ifndef MMFB_ATTN_VARLEN_TU
+// differently, and the dense d = 64 forward would not keep the code it has without the packed mode.  attention_probs.cu
+// includes this file for its helpers only and instantiates neither.
+#if !defined(MMFB_ATTN_VARLEN_TU) && !defined(MMFB_ATTN_PROBS_TU)
 int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream) {
   int rc = check_attn_common(a, "attn_fwd");
   if (rc) return rc;
@@ -849,7 +850,7 @@ int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
                           : attn_bwd_launch<128, false>(a, nullptr, 0, nullptr, 0, stream);
 }
 
-#else   // MMFB_ATTN_VARLEN_TU
+#elif defined(MMFB_ATTN_VARLEN_TU)
 
 // Packed self-attention: Sq = Skv = max_len (the grid extent), no additive mask, `cu` on the device and never read here.
 static int check_varlen(const mmfb_attn_args& a, const int32_t* cu, int total, const char* who) {

@@ -162,6 +162,12 @@ int mmfb_attention_varlen_cross_bwd(const mmfb_attn_args* args, const int32_t* c
   return attn_varlen_cross_bwd(*args, cu_q, total_q, cu_kv, total_kv, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int mmfb_attention_probs(const mmfb_attn_args* args, void* probs, int probs_dtype, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_attention_probs: null args");
+  MMFB_REQUIRE_DEVICE();
+  return attn_probs(*args, probs, probs_dtype, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int mmfb_layernorm_fwd(const mmfb_ln_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_layernorm_fwd: null args");
   MMFB_REQUIRE_DEVICE();

@@ -146,6 +146,48 @@ def attention_bwd(dctx, q, k, v, ctx, lse2, B, heads, Sq, Skv, mask=None, drop_m
     return dq, dk, dv
 
 
+_PROBS_DTYPES = {torch.float32: lib.MMFB_PROBS_F32, torch.bfloat16: lib.MMFB_PROBS_BF16}
+
+
+def attention_probs(q, k, lse2, B, heads, Sq, Skv, mask=None, drop_mask=None, drop_scale=1.0, dtype=torch.float32,
+                    out=None):
+    """The attention probabilities [B, heads, Sq, Skv] of one attention_fwd call, from that call's q, k, mask, keep bits
+    and the lse2 it returned: softmax(QK^T/sqrt(d) + mask) with the mask clamped at -10000 as in the forward; with keep
+    bits, the post-dropout probabilities (dropped entries 0, kept ones scaled by drop_scale).  dtype: torch.float32 or
+    torch.bfloat16.  `out`, when given, must be a contiguous tensor of that shape and dtype."""
+    # layouts first (ValueError), then the device (_attn_args: RuntimeError for a CPU tensor)
+    if dtype not in _PROBS_DTYPES:
+        raise ValueError("attention_probs: dtype must be torch.float32 or torch.bfloat16, got %s" % (dtype,))
+    for t, n in ((q, "q"), (k, "k")):
+        if t.dtype != torch.bfloat16 or t.dim() != 2 or t.stride(-1) != 1:
+            raise ValueError("attention_probs: %s must be a 2-D bf16 head-column slice, contiguous in its last dimension" % n)
+    if k.shape[1] != q.shape[1] or q.shape[1] % heads:
+        raise ValueError("attention_probs: q and k must have the same width, a multiple of heads=%d" % heads)
+    if q.shape[0] != B * Sq or k.shape[0] != B * Skv:
+        raise ValueError("attention_probs: q/k row counts do not match B*Sq / B*Skv")
+    if mask is not None and (mask.dtype != torch.float32 or tuple(mask.shape) != (B, Skv) or not mask.is_contiguous()):
+        raise ValueError("attention_probs: additive mask must be contiguous fp32 [B, Skv]")
+    if drop_mask is not None and (drop_mask.dtype != torch.int32 or not drop_mask.is_contiguous()
+                                  or tuple(drop_mask.shape) != (B, heads, Sq, (Skv + 31) // 32)):
+        raise ValueError("attention_probs: drop_mask must be contiguous int32 [B, heads, Sq, ceil(Skv/32)]")
+    if (not isinstance(lse2, torch.Tensor) or lse2.dtype != torch.float32 or tuple(lse2.shape) != (B, heads, Sq)
+            or not lse2.is_contiguous()):
+        raise ValueError("attention_probs: lse2 must be contiguous fp32 [B, heads, Sq]")
+    if out is not None and (out.dtype != dtype or tuple(out.shape) != (B, heads, Sq, Skv) or not out.is_contiguous()
+                            or out.device != q.device):
+        raise ValueError("attention_probs: out must be a contiguous %s tensor [B, heads, Sq, Skv] = %s on %s"
+                         % (dtype, (B, heads, Sq, Skv), q.device))
+    a = _attn_args(q, k, k, B, heads, Sq, Skv, mask, drop_mask, drop_scale)
+    a.v, a.ldv = 0, 0
+    if not lse2.is_cuda:
+        raise RuntimeError("lse2 must be a CUDA tensor: the B200 path has no CPU fallback")
+    if out is None:
+        out = torch.empty(B, heads, Sq, Skv, dtype=dtype, device=q.device)
+    a.lse2 = lse2.data_ptr()
+    check(LIB.mmfb_attention_probs(ctypes.byref(a), out.data_ptr(), _PROBS_DTYPES[dtype], _stream_ptr()))
+    return out
+
+
 def _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale):
     """packed self-attention operands: q/k/v [total, h*d] rows of B samples delimited by cu_seqlens (int32 [B+1])"""
     if not isinstance(cu_seqlens, torch.Tensor) or cu_seqlens.dtype != torch.int32:

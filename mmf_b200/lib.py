@@ -138,8 +138,11 @@ def _load():
     for name in ("mmfb_attention_varlen_cross_fwd", "mmfb_attention_varlen_cross_bwd"):
         getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                        ctypes.c_void_p]
+    lib.mmfb_attention_probs.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
     return lib
 
+
+MMFB_PROBS_F32, MMFB_PROBS_BF16 = 0, 1
 
 LIB = _load()
 LIB_PATH = _LIB_PATH

@@ -364,8 +364,9 @@ class B200VisualBERTForClassification(nn.Module):
         super().__init__()
         from .visual_bert import B200VisualBERTBase
         self.config = config
-        if config.get("output_attentions", False):
-            raise NotImplementedError("attention probabilities are never materialised on the B200 path")
+        # The reference's trunk calls its encoder without output_attentions (visual_bert.py:144-157), so the
+        # attention_weights it reports are always the empty tuple; so are they here.
+        self.output_attentions = bool(config.get("output_attentions", False))
         self.output_hidden_states = bool(config.get("output_hidden_states", False))
         self.pooler_strategy = config.get("pooler_strategy", "default")
         self.bert_config = bert_config_of(config)
@@ -389,6 +390,8 @@ class B200VisualBERTForClassification(nn.Module):
             b = pooled_output.size(0)
             pooled_output = torch.cat([pooled_output[: b // 2], pooled_output[b // 2:]], dim=1)
         out = {}
+        if self.output_attentions:
+            out["attention_weights"] = ()
         if self.output_hidden_states:
             out["sequence_output"], out["pooled_output"] = sequence_output, pooled_output
         if self.pooler_strategy == "vqa":                              # second-last attended token (integer gather)

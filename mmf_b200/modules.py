@@ -100,18 +100,20 @@ class EncoderRunner:
             o1 = self.pack.offsets[(i + 1) * per] if (i + 1) * per < len(self.pack.offsets) else self.pack.total
             self.layer_param_ranges.append((o0, o1))
 
-    def forward(self, x, add_mask, training, need_grad, first_layer=0, last_layer=None):
+    def forward(self, x, add_mask, training, need_grad, first_layer=0, last_layer=None, probs=None):
+        """probs: an engine.ProbsSink that receives every layer's attention probabilities, or None"""
         B, S, H = x.shape
         h = x.reshape(B * S, H)
         saved = []
         ds = _fresh_dropout_state(prefetchable=True) if training else None
         last_layer = len(self.layers) if last_layer is None else last_layer
         hiddens = []
+        extra = {} if probs is None else {"probs": probs}
         for i in range(first_layer, last_layer):
             m = self.layers[i]
             pa, ph = self._probs(m) if training else (0.0, 0.0)
             hiddens.append(h)
-            h, s = self._fwd(h, add_mask, self.weights[i], B, S, pa, ph, ds)
+            h, s = self._fwd(h, add_mask, self.weights[i], B, S, pa, ph, ds, **extra)
             saved.append(s if need_grad else None)
         return h, saved, hiddens
 
@@ -232,16 +234,24 @@ def plan_two_stream(mask_a, mask_b, B, Sa, Sb, device):
     return tuple(plans)
 
 
+def _probs_sink(*dtypes):
+    """A ProbsSink whose kernel output dtype is the callers' hidden-state dtype when that is fp32 or bf16 (and the same for
+    every stream); fp32 otherwise, cast on the host afterwards."""
+    dt = dtypes[0] if len(set(dtypes)) == 1 and dtypes[0] in (torch.float32, torch.bfloat16) else torch.float32
+    return E.ProbsSink(dt)
+
+
 class _BertEncoderFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, runner, add_mask, training, want_hiddens, x, *params):
+    def forward(ctx, runner, add_mask, training, want_hiddens, want_attn, x, *params):
         B, S, H = x.shape
         need_grad = any(ctx.needs_input_grad)   # (grad mode itself is always off inside Function.forward)
         runner.pack.refresh()
         xb = x.detach().to(torch.bfloat16).contiguous()
         packing = add_mask if isinstance(add_mask, _Packing) else None
+        probs = _probs_sink(x.dtype) if want_attn else None
         if packing is None:
-            out, saved, hiddens = runner.forward(xb, add_mask, training, need_grad)
+            out, saved, hiddens = runner.forward(xb, add_mask, training, need_grad, probs=probs)
         else:                                   # the layers run on the [total, H] valid rows only
             vl = packing.varlen
             xp = packing.pack(xb.view(B * S, H)).view(1, vl.total, H)
@@ -252,6 +262,9 @@ class _BertEncoderFn(torch.autograd.Function):
         outs = [out.view(B, S, H).to(x.dtype)]
         if want_hiddens:
             outs += [h.view(B, S, H).to(x.dtype) for h in hiddens]
+        if want_attn:
+            outs += [p.to(x.dtype) for p in probs]
+        if len(outs) > 1:
             ctx.mark_non_differentiable(*outs[1:])
         return tuple(outs)
 
@@ -270,11 +283,16 @@ class _BertEncoderFn(torch.autograd.Function):
         else:
             dx = runner.backward(d, ctx.saved, ctx.add_mask, B, S)
         ctx.saved = None
-        return (None, None, None, None, dx.view(B, S, H).to(ctx.in_dtype)) + tuple(runner.pack.autograd_grads(aliased))
+        return (None, None, None, None, None, dx.view(B, S, H).to(ctx.in_dtype)) + tuple(runner.pack.autograd_grads(aliased))
 
 
-def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hidden_states=False):
-    """hidden_states [B,S,H] (fp32 or bf16), attention_mask additive [B,1,1,S] / [B,S] / None."""
+def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hidden_states=False, output_attentions=False):
+    """hidden_states [B,S,H] (fp32 or bf16), attention_mask additive [B,1,1,S] / [B,S] / None.
+    Returns (last,), then the L layer inputs if output_hidden_states, then the L layers' attention probabilities
+    [B, heads, S, S] (hidden-state dtype, post-dropout in training) if output_attentions.  The hidden states and
+    probabilities are outputs for inspection: they carry no gradient, so a loss that reads them back-propagates nothing
+    through them.  A call that asks for probabilities runs the dense path even with skip_padding set, so they have the
+    reference's [B, heads, S, S] shape, padded rows and keys included."""
     _require_cuda(hidden_states, "hidden_states")
     if hidden_states.dim() != 3:
         raise ValueError("hidden_states must be [batch, seq, hidden], got %s" % (tuple(hidden_states.shape),))
@@ -283,7 +301,7 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
     if H != runner.weights[0].hidden:
         raise ValueError("hidden size %d does not match the encoder's %d" % (H, runner.weights[0].hidden))
     mask = E.additive_mask_2d(attention_mask, B, S)
-    if runner.skip_padding and mask is not None:
+    if runner.skip_padding and mask is not None and not output_attentions:
         packing = _plan_packing(mask, B, S)
         if packing is not None and packing.varlen.total == 0:
             # every token is padding: nothing to compute, every output row (and every input-gradient row) is zero
@@ -291,8 +309,17 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
             return (z,) + ((z.detach(),) * len(runner.layers) if output_hidden_states else ())
         if packing is not None:
             mask = packing
-    outs = _BertEncoderFn.apply(runner, mask, training, output_hidden_states, hidden_states, *runner.pack.params)
+    outs = _BertEncoderFn.apply(runner, mask, training, output_hidden_states, bool(output_attentions), hidden_states,
+                                *runner.pack.params)
     return outs
+
+
+def split_encoder_outputs(outs, n_layers, output_hidden_states, output_attentions):
+    """(last, hidden states or None, attentions or None) of run_bert_encoder's outputs; the hidden states in the reference's
+    layout: the L layer inputs, then the last output"""
+    hidden = tuple(outs[1:1 + n_layers]) + (outs[0],) if output_hidden_states else None
+    attn = tuple(outs[len(outs) - n_layers:]) if output_attentions else None
+    return outs[0], hidden, attn
 
 
 class _Holder(nn.Module):
@@ -376,18 +403,23 @@ class B200BertEncoder(nn.Module):
 
     def forward(self, hidden_states, attention_mask=None, encoder_hidden_states=None, encoder_attention_mask=None,
                 output_attentions=False, output_hidden_states=False, return_dict=False, head_mask=None):
-        """Same contract as BertEncoderJit.forward (hf_layers.py:316-355): returns (last_hidden,
-        [all_hidden_states], ...).  Attention probabilities never exist in HBM on this path."""
-        if output_attentions:
-            raise NotImplementedError("output_attentions: the fused kernel never materialises attention probabilities")
+        """Same contract as BertEncoderJit.forward (hf_layers.py:316-355): returns (last_hidden,), then
+        (all_hidden_states) if output_hidden_states, then (attn_0, ..., attn_{L-1}) if output_attentions.  The
+        probabilities are written by one extra kernel per layer only when asked for; like the hidden states they are
+        outputs for inspection and carry no gradient."""
         if head_mask is not None and not (isinstance(head_mask, (list, tuple)) and all(h is None for h in head_mask)):
             raise NotImplementedError("head_mask is not supported on the B200 path")
         # `encoder_hidden_states` is ignored exactly as BertLayerJit ignores it (hf_layers.py:281-283; MMFT passes
         # `[None]*L` there, huggingface.py:229-235)
-        outs = run_bert_encoder(self._runner, hidden_states, attention_mask, self.training, output_hidden_states)
-        if output_hidden_states:
-            return (outs[0], tuple(outs[1:]) + (outs[0],))
-        return (outs[0],)
+        outs = run_bert_encoder(self._runner, hidden_states, attention_mask, self.training, output_hidden_states,
+                                output_attentions)
+        return encoder_result(outs, len(self.layer), output_hidden_states, output_attentions)
+
+
+def encoder_result(outs, n_layers, output_hidden_states, output_attentions):
+    """BertEncoderJit.forward's return structure (hf_layers.py:349-355) from run_bert_encoder's outputs"""
+    last, hidden, attn = split_encoder_outputs(outs, n_layers, output_hidden_states, output_attentions)
+    return (last,) + ((hidden,) if output_hidden_states else ()) + ((attn,) if output_attentions else ())
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -480,19 +512,22 @@ class VilbertRunner:
         d = getattr(mod, "dropout", None)
         return float(getattr(d, "p", 0.0)) if d is not None else 0.0
 
-    def forward(self, txt, img, tmask, imask, B, T, R, training, need_grad, block_states=None):
+    def forward(self, txt, img, tmask, imask, B, T, R, training, need_grad, block_states=None, probs=None):
+        """probs: an engine.ProbsSink that receives the attention probabilities in schedule order - one per text or image
+        layer, two (attn1, attn2) per co-attention block - or None"""
         ds = _fresh_dropout_state() if training else None
         saved = []
+        extra = {} if probs is None else {"probs": probs}
         for kind, i in self.steps:
             w = self.w[(kind, i)]
             if kind == "t":
                 m = self.layer[i]
                 pa, ph = (self._p(m.attention.self), self._p(m.attention.output)) if training else (0.0, 0.0)
-                txt, s = E.bert_layer_fwd(txt, tmask, w, B, T, pa, ph, ds)
+                txt, s = E.bert_layer_fwd(txt, tmask, w, B, T, pa, ph, ds, **extra)
             elif kind == "v":
                 m = self.v_layer[i]
                 pa, ph = (self._p(m.attention.self), self._p(m.attention.output)) if training else (0.0, 0.0)
-                img, s = E.bert_layer_fwd(img, imask, w, B, R, pa, ph, ds)
+                img, s = E.bert_layer_fwd(img, imask, w, B, R, pa, ph, ds, **extra)
             else:
                 m = self.c_layer[i]
                 if training:
@@ -500,7 +535,7 @@ class VilbertRunner:
                     pvh, pth = float(m.biOutput.dropout1.p), float(m.biOutput.dropout2.p)
                 else:
                     pva = pta = pvh = pth = 0.0
-                img, txt, s = E.connection_fwd(img, txt, imask, tmask, w, B, R, T, pva, pta, pvh, pth, ds)
+                img, txt, s = E.connection_fwd(img, txt, imask, tmask, w, B, R, T, pva, pta, pvh, pth, ds, **extra)
                 if block_states is not None:
                     block_states.append((txt, img))      # the states the reference appends per co-attention block
             saved.append(s if need_grad else None)
@@ -525,7 +560,7 @@ class VilbertRunner:
 
 class _VilbertEncoderFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, runner, tmask, imask, training, want_blocks, txt, img, *params):
+    def forward(ctx, runner, tmask, imask, training, want_blocks, want_attn, txt, img, *params):
         B, T, Ht = txt.shape
         _, R, Hv = img.shape
         need_grad = any(ctx.needs_input_grad)
@@ -533,18 +568,26 @@ class _VilbertEncoderFn(torch.autograd.Function):
         t = txt.detach().to(torch.bfloat16).contiguous().view(B * T, Ht)
         v = img.detach().to(torch.bfloat16).contiguous().view(B * R, Hv)
         blocks = [] if want_blocks else None
+        probs = _probs_sink(txt.dtype, img.dtype) if want_attn else None
         if isinstance(tmask, _Packing):             # both streams run on their valid rows only
             t, v, saved = runner.forward(tmask.pack(t), imask.pack(v), tmask.varlen, imask.varlen, B, T, R, training,
                                          need_grad, blocks)
             t, v = tmask.unpack(t, B * T), imask.unpack(v, B * R)
             blocks = [(tmask.unpack(bt, B * T), imask.unpack(bv, B * R)) for bt, bv in blocks] if want_blocks else blocks
         else:
-            t, v, saved = runner.forward(t, v, tmask, imask, B, T, R, training, need_grad, blocks)
+            t, v, saved = runner.forward(t, v, tmask, imask, B, T, R, training, need_grad, blocks, probs=probs)
         ctx.runner, ctx.saved, ctx.masks, ctx.dims, ctx.dtypes = runner, saved, (tmask, imask), (B, T, R, Ht, Hv), (txt.dtype, img.dtype)
         outs = [t.view(B, T, Ht).to(txt.dtype), v.view(B, R, Hv).to(img.dtype)]
         if want_blocks:
             for bt, bv in blocks:
                 outs += [bt.view(B, T, Ht).to(txt.dtype), bv.view(B, R, Hv).to(img.dtype)]
+        if want_attn:
+            # schedule order; text-query probabilities in the text dtype, image-query ones in the image dtype
+            it = iter(probs)
+            for kind, _ in runner.steps:
+                for q_stream in {"t": "t", "v": "v", "c": "tv"}[kind]:
+                    outs.append(next(it).to(txt.dtype if q_stream == "t" else img.dtype))
+        if len(outs) > 2:
             ctx.mark_non_differentiable(*outs[2:])
         return tuple(outs)
 
@@ -564,8 +607,8 @@ class _VilbertEncoderFn(torch.autograd.Function):
         else:
             dt, dv = runner.backward(dt, dv, ctx.saved, tm, im, B, T, R)
         ctx.saved = None
-        return (None, None, None, None, None, dt.view(B, T, Ht).to(ctx.dtypes[0]), dv.view(B, R, Hv).to(ctx.dtypes[1])) + tuple(
-            runner.pack.autograd_grads(aliased))
+        return (None, None, None, None, None, None, dt.view(B, T, Ht).to(ctx.dtypes[0]),
+                dv.view(B, R, Hv).to(ctx.dtypes[1])) + tuple(runner.pack.autograd_grads(aliased))
 
 
 class B200ViLBertEncoder(nn.Module):
@@ -605,15 +648,38 @@ class B200ViLBertEncoder(nn.Module):
         (vilbert.py:424-425,448-449), not applied.  output_all_encoded_layers=True reproduces the reference's lists: ONE
         entry per co-attention block - the states right after that block - and NOT the final states (vilbert.py:761-763,
         787-790).  Those per-block tensors are outputs for inspection: they carry no gradient here (the reference would
-        back-propagate through them); the differentiable result is the default output_all_encoded_layers=False path."""
-        if output_all_attention_masks:
-            raise NotImplementedError("attention probabilities are never materialised on the B200 path")
+        back-propagate through them); the differentiable result is the default output_all_encoded_layers=False path.
+
+        output_all_attention_masks=True with `config.visualization` set returns the reference's third element
+        (vilbert.py:611-795): the text layers' probabilities [B, h, T, T] and the image layers' [B, h, R, R] in schedule
+        order, and per co-attention block the pair (attn1, attn2) = (text queries over image keys [B, h, T, R], image
+        queries over text keys [B, h, R, T]); post-dropout in training, in the stream's dtype.  One extra kernel per
+        attention call writes them, and like the per-block states they carry no gradient.  A call that asks for them runs
+        the dense path even with skip_padding set.  Without `visualization` the lists are empty, as in the reference, and
+        nothing extra runs."""
         _require_cuda(txt_embedding, "txt_embedding")
         B, T, _ = txt_embedding.shape
         R = image_embedding.shape[1]
         self._runner.ensure(txt_embedding.device)
         tmask = E.additive_mask_2d(txt_attention_mask, B, T)
         imask = E.additive_mask_2d(image_attention_mask, B, R)
+        want_attn = bool(output_all_attention_masks) and bool(getattr(self.config, "visualization", False))
+        if want_attn:
+            outs = _VilbertEncoderFn.apply(self._runner, tmask, imask, self.training, bool(output_all_encoded_layers), True,
+                                           txt_embedding, image_embedding, *self._runner.pack.params)
+            nb = 2 * len(self.c_layer) if output_all_encoded_layers else 0
+            blocks, attn = outs[2:2 + nb], iter(outs[2 + nb:])
+            att_t, att_v, att_c = [], [], []
+            for kind, _ in self._runner.steps:
+                if kind == "t":
+                    att_t.append(next(attn))
+                elif kind == "v":
+                    att_v.append(next(attn))
+                else:
+                    att_c.append((next(attn), next(attn)))
+            if output_all_encoded_layers:
+                return list(blocks[0::2]), list(blocks[1::2]), (att_t, att_v, att_c)
+            return [outs[0]], [outs[1]], (att_t, att_v, att_c)
         if self._runner.pack_streams:
             plan = plan_two_stream(tmask, imask, B, T, R, txt_embedding.device)
             if plan == "empty":
@@ -625,7 +691,7 @@ class B200ViLBertEncoder(nn.Module):
                 return [zt], [zi], ([], [], [])
             if plan is not None:
                 tmask, imask = plan
-        outs = _VilbertEncoderFn.apply(self._runner, tmask, imask, self.training, bool(output_all_encoded_layers),
+        outs = _VilbertEncoderFn.apply(self._runner, tmask, imask, self.training, bool(output_all_encoded_layers), False,
                                        txt_embedding, image_embedding, *self._runner.pack.params)
         if output_all_encoded_layers:
             return list(outs[2::2]), list(outs[3::2]), ([], [], [])

@@ -12,7 +12,7 @@ With `two_stream=True` it also packs both streams of the ViLBERT and LXMERT enco
 import types
 
 from .lxmert import LxmertRunner
-from .modules import EncoderRunner, VilbertRunner, run_bert_encoder
+from .modules import EncoderRunner, VilbertRunner, encoder_result, run_bert_encoder
 
 _saved = {}
 
@@ -20,15 +20,11 @@ _saved = {}
 def _b200_encoder_forward(self, hidden_states, attention_mask=None, encoder_hidden_states=None,
                           encoder_attention_mask=None, output_attentions=False, output_hidden_states=False,
                           return_dict=False, head_mask=None, **unused):
-    if output_attentions:
-        raise NotImplementedError("output_attentions: the fused kernel never materialises attention probabilities")
     if head_mask is not None and not (isinstance(head_mask, (list, tuple)) and all(h is None for h in head_mask)):
         raise NotImplementedError("head_mask is not supported on the B200 path")
     runner = _runner_of(self)
-    outs = run_bert_encoder(runner, hidden_states, attention_mask, self.training, output_hidden_states)
-    if output_hidden_states:
-        return (outs[0], tuple(outs[1:]) + (outs[0],))
-    return (outs[0],)
+    outs = run_bert_encoder(runner, hidden_states, attention_mask, self.training, output_hidden_states, output_attentions)
+    return encoder_result(outs, len(runner.layers), output_hidden_states, output_attentions)
 
 
 def _runner_of(encoder):
@@ -89,7 +85,11 @@ def set_skip_padding(module, enabled=True, two_stream=False):
     dropout masks drawn.  It reads the token count on the host, so it cannot be captured in a CUDA graph.
 
     A two-stream call falls back to the dense path when some sample has tokens in one stream and none in the other: there
-    the dense outputs of those tokens depend on the other stream's padded rows."""
+    the dense outputs of those tokens depend on the other stream's padded rows.
+
+    A call that asks for attention probabilities (output_attentions, or ViLBERT's output_all_attention_masks with
+    `visualization`) also runs the dense path, whatever the flag: the probabilities then have the reference's
+    [B, heads, S, S] shape, padded rows and keys included."""
     n = 0
     for m in module.modules():
         r = m.__dict__.get("_runner")

@@ -120,8 +120,9 @@ class B200VisualBERTForPretraining(nn.Module):
         from .heads import B200BertPreTrainingHeads
         self.config = config
         self.output_hidden_states = bool(getattr(config, "output_hidden_states", False))
-        if getattr(config, "output_attentions", False):
-            raise NotImplementedError("attention probabilities are never materialised on the B200 path")
+        # The reference's trunk calls its encoder without output_attentions (visual_bert.py:144-157), so the
+        # attention_weights it reports are always the empty tuple; so are they here.
+        self.output_attentions = bool(getattr(config, "output_attentions", False))
         self.bert = B200VisualBERTBase(config)
         self.vocab_size = config.vocab_size
         self.cls = B200BertPreTrainingHeads(config, self.bert.embeddings.word_embeddings.weight)
@@ -133,6 +134,8 @@ class B200VisualBERTForPretraining(nn.Module):
         sequence_output, pooled_output, _ = self.bert(input_ids, attention_mask, token_type_ids, visual_embeddings,
                                                       visual_embeddings_type, image_text_alignment)
         out = {}
+        if self.output_attentions:
+            out["attention_weights"] = ()
         if self.output_hidden_states:
             out["sequence_output"], out["pooled_output"] = sequence_output, pooled_output
         if masked_lm_labels is not None:

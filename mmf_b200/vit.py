@@ -16,7 +16,7 @@ from torch import nn
 from . import engine as E
 from . import ops
 from .modules import (B200BertIntermediate, B200BertSelfAttention, EncoderRunner, _Holder, _init_bert_weights, _require_cuda,
-                      run_bert_encoder)
+                      run_bert_encoder, split_encoder_outputs)
 
 
 class _ViTSelfOutput(_Holder):
@@ -80,17 +80,17 @@ class B200ViTEncoder(nn.Module):
     def forward(self, hidden_states, attention_mask=None, head_mask=None, output_attentions=False,
                 output_hidden_states=False, return_dict=True):
         """ViTEncoder.forward (vit.py:118-175).  return_dict=True gives an object with `last_hidden_state` / `hidden_states`
-        / `attentions` attributes (HF BaseModelOutput's fields)."""
-        if output_attentions:
-            raise NotImplementedError("output_attentions: the fused kernel never materialises attention probabilities")
+        / `attentions` attributes (HF BaseModelOutput's fields).  output_attentions: `attentions` is the tuple of the
+        layers' probabilities [B, heads, S, S] (one extra kernel per layer; no gradient flows through them)."""
         if head_mask is not None and not (isinstance(head_mask, (list, tuple)) and all(h is None for h in head_mask)):
             raise NotImplementedError("head_mask is not supported on the B200 path")
-        outs = run_bert_encoder(self._runner, hidden_states, attention_mask, self.training, output_hidden_states)
-        hidden = tuple(outs[1:]) + (outs[0],) if output_hidden_states else None
+        outs = run_bert_encoder(self._runner, hidden_states, attention_mask, self.training, output_hidden_states,
+                                output_attentions)
+        last, hidden, attn = split_encoder_outputs(outs, len(self.layer), output_hidden_states, output_attentions)
         if not return_dict:
-            return tuple(v for v in (outs[0], hidden) if v is not None)
+            return tuple(v for v in (last, hidden, attn) if v is not None)
         import types
-        return types.SimpleNamespace(last_hidden_state=outs[0], hidden_states=hidden, attentions=None)
+        return types.SimpleNamespace(last_hidden_state=last, hidden_states=hidden, attentions=attn)
 
 
 class _PatchEmbeddings(nn.Module):
