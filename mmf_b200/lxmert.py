@@ -3,12 +3,14 @@
   B200VisualFeatEncoder  <->  VisualFeatEncoder   mmf/models/lxmert.py:196-223
   B200LXMERTXLayer       <->  LXMERTXLayer        mmf/models/lxmert.py:226-283   (parameter holder)
   B200LXMERTEncoder      <->  LXMERTEncoder       mmf/models/lxmert.py:286-336
+  B200LXMERTBase         <->  LXMERTBase          mmf/models/lxmert.py:339-414   (embeddings + encoder + pooler)
 
 Same sub-module / parameter names (`visn_fc.{visn_fc,visn_layer_norm,box_fc,box_layer_norm}`, `layer.{i}`,
 `r_layers.{i}`, `x_layers.{i}.{visual_attention.att,visual_attention.output,lang_self_att,visn_self_att,lang_inter,
 lang_output,visn_inter,visn_output}`) and the forward signature `(lang_feats, lang_attention_mask, (feats, boxes),
 visn_attention_mask) -> (lang_feats, visn_feats)`.  No new device code: language / relational layers are BERT layers,
 the cross-modality layer is engine.xlayer_fwd/bwd (one shared cross-attention block used in both directions).
+The registered model and its heads are in mmf_b200.models (`lxmert`).
 """
 import torch
 from torch import nn
@@ -18,6 +20,8 @@ from . import ops
 from .modules import (B200BertAttention, B200BertIntermediate, B200BertLayer, B200BertSelfAttention,
                       B200BertSelfOutput, _Holder, _Packing, _fresh_dropout_state, _init_bert_weights, _require_cuda,
                       plan_two_stream)
+from .vilbert import B200BertTextEmbeddings
+from .visual_bert import BertPooler
 
 
 class B200VisualFeatEncoder(nn.Module):
@@ -212,3 +216,42 @@ class B200LXMERTEncoder(nn.Module):
             if plan is not None:
                 lmask, vmask = plan
         return _LxmertEncoderFn.apply(self._runner, lmask, vmask, self.training, lang_feats, visn, *self._runner.pack.params)
+
+
+class B200LXMERTBase(nn.Module):
+    """LXMERTBase (lxmert.py:339-414): HF BertEmbeddings (`embeddings`), the two-stream encoder (`encoder`) and the tanh
+    pooler on the first language token (`pooler.dense`), so LXMERT checkpoints load key for key.
+
+    forward(input_ids, token_type_ids, attention_mask, visual_feats, visual_loc, visual_attention_mask,
+    output_all_attention_masks, output_all_encoded_layers) -> ((lang_feats, visn_feats), pooled_output).  Both masks
+    become (1 - m) * -10000 in the parameter dtype; visual_attention_mask=None stays None (no key of the visual stream is
+    masked).  The encoder's skip-padding (`config.skip_padding`, patch.set_skip_padding(two_stream=True)) applies here."""
+
+    def __init__(self, config):
+        super().__init__()
+        self.config = config
+        self.embeddings = B200BertTextEmbeddings(config)
+        self.encoder = B200LXMERTEncoder(config)
+        self.pooler = BertPooler(config.hidden_size)
+        for m in (self.embeddings, self.pooler):
+            _init_bert_weights(m, float(getattr(config, "initializer_range", 0.02)))
+
+    def forward(self, input_ids, token_type_ids=None, attention_mask=None, visual_feats=None, visual_loc=None,
+                visual_attention_mask=None, output_all_attention_masks=False, output_all_encoded_layers=False):
+        if output_all_encoded_layers:
+            raise NotImplementedError("LXMERT output_all_encoded_layers: the reference raises too (lxmert.py:360-361)")
+        if output_all_attention_masks:
+            raise NotImplementedError("LXMERT output_all_attention_masks: the reference raises too (lxmert.py:362-363)")
+        if attention_mask is None:
+            attention_mask = torch.ones_like(input_ids)
+        if token_type_ids is None:
+            token_type_ids = torch.zeros_like(input_ids)
+        dt = next(self.parameters()).dtype
+        ext = (1.0 - attention_mask.unsqueeze(1).unsqueeze(2).to(dt)) * -10000.0
+        ext_v = None
+        if visual_attention_mask is not None:
+            ext_v = (1.0 - visual_attention_mask.unsqueeze(1).unsqueeze(2).to(dt)) * -10000.0
+        emb = self.embeddings(input_ids, token_type_ids)
+        lang, visn = self.encoder(emb, ext, (visual_feats, visual_loc), ext_v)
+        lang, visn = lang.to(dt), visn.to(dt)
+        return (lang, visn), self.pooler(lang)

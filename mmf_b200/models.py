@@ -3,11 +3,12 @@
   registry.register_model("visual_bert")  VisualBERT   <->  mmf/models/visual_bert.py:407-601
   registry.register_model("vilbert")      ViLBERT      <->  mmf/models/vilbert.py:1336-1472
   registry.register_model("mmbt")         MMBT         <->  mmf/models/mmbt.py:565-643
+  registry.register_model("lxmert")       LXMERT       <->  mmf/models/lxmert.py:647-790
 
 Each is a `BaseModel` (mmf/models/base_model.py:67-337 contract: ctor(config) -> build() -> forward(SampleList) -> dict
 with "scores" and/or "losses"; `config_path()` names the model's default YAML; `__call__` fills "losses" from the
 configured loss list when the forward did not), built from the SAME configuration keys as the reference's YAML
-(mmf/configs/models/{visual_bert,vilbert,mmbt}/*.yaml).  `load_model_config()` reads such a YAML with PyYAML
+(mmf/configs/models/{visual_bert,vilbert,mmbt,lxmert}/*.yaml).  `load_model_config()` reads such a YAML with PyYAML
 (`includes:` honoured) when an MMF checkout is at hand; the defaults themselves are restated in `MODEL_DEFAULTS` so that
 nothing is read from the reference tree at run time (tests/test_models_cpu.py pins the restatement to the YAML files).
 
@@ -114,6 +115,20 @@ MODEL_DEFAULTS = {
         text_encoder=dict(type="transformer", params=dict(
             num_segments=2, bert_model_name="bert-base-uncased", hidden_size=768, num_hidden_layers=12,
             num_attention_heads=12, output_attentions=False, output_hidden_states=False))),
+    # mmf/configs/models/lxmert/defaults.yaml:1-74
+    "lxmert": dict(
+        bert_model_name="bert-base-uncased", training_head_type="pretraining", random_initialize=False, num_labels=3129,
+        gqa_labels=1534, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072, hidden_size=768,
+        hidden_act="gelu", hidden_dropout_prob=0.1, attention_probs_dropout_prob=0.1, max_position_embeddings=512,
+        type_vocab_size=2, initializer_range=0.02, pad_token_id=0, layer_norm_eps=1e-12, mode="lxr", l_layers=9,
+        x_layers=5, r_layers=5, visual_feat_dim=2048, visual_pos_dim=4, task_matched=True, task_mask_lm=True,
+        task_obj_predict=True, task_qa=True, visual_losses=["obj", "feat"],
+        visual_loss_config=dict(obj=[3129, "ce", [-1], 6.67], attr=[400, "ce", [-1], 6.67],
+                                feat=[2048, "l2", [-1, 2048], 6.67]),
+        special_visual_initialize=True, hard_cap_seq_len=36, cut_first="text", embedding_strategy="plain",
+        bypass_transformer=False, output_attentions=False, output_hidden_states=False, text_only=False,
+        freeze_base=False, finetune_lr_multiplier=1, vocab_size=30522, fast_mode=False, dynamic_attention=False,
+        in_batch_pairs=False, visualization=False, model="bert"),
 }
 
 
@@ -762,3 +777,253 @@ class MMBT(BaseModel):
 
     def forward(self, sample_list):
         return self.model(sample_list)
+
+
+# ------------------------------------------------------------------------------------------------------
+# LXMERT
+# ------------------------------------------------------------------------------------------------------
+class B200LogitHead(nn.Sequential):
+    """nn.Sequential(Linear(in, 2H), GeLU(), LayerNorm(2H, eps=1e-12), Linear(2H, out)) of BertVisualAnswerHead
+    (lxmert.py:143-156), keys `0.*`, `2.*`, `3.*`: the first GEMM with the bias + GELU epilogue, the row LayerNorm, the
+    output GEMM."""
+
+    def __init__(self, in_dim, hid_dim, out_dim):
+        super().__init__(nn.Linear(in_dim, hid_dim), nn.GELU(), nn.LayerNorm(hid_dim, eps=1e-12),
+                         B200Linear(hid_dim, out_dim))
+
+    def forward(self, x):
+        shape = x.shape
+        h = ops.linear_gelu(x.reshape(-1, shape[-1]), self[0].weight, self[0].bias)
+        h = ops.layer_norm(h, self[2].weight, self[2].bias, self[2].eps)
+        y = self[3](h)
+        return y.view(*shape[:-1], y.shape[-1])
+
+
+class B200BertVisualAnswerHead(nn.Module):
+    """BertVisualAnswerHead (lxmert.py:129-162): `logit_fc`, plus `logit_gqa` when num_labels is the [num_labels,
+    gqa_labels] pair; forward(h, name) takes `logit_gqa` when the dataset name contains "gqa"."""
+
+    def __init__(self, config, num_labels):
+        super().__init__()
+        hid = config.hidden_size
+        if config.training_head_type == "nlvr2":
+            in_dim, out_dim = hid * 2, 2
+        else:
+            in_dim, out_dim = hid, config.num_labels
+        if isinstance(num_labels, (list, tuple)):
+            self.logit_gqa = B200LogitHead(in_dim, hid * 2, num_labels[1])
+            out_dim = num_labels[0]
+        self.logit_fc = B200LogitHead(in_dim, hid * 2, out_dim)
+
+    def forward(self, hidden_states, name=None):
+        if name is None or "gqa" not in name:
+            return self.logit_fc(hidden_states)
+        return self.logit_gqa(hidden_states)
+
+
+class B200BertVisualObjHead(nn.Module):
+    """BertVisualObjHead (lxmert.py:165-186): one transform, then `decoder_dict.<key>` per entry of visual_losses"""
+
+    def __init__(self, config, visual_losses, visual_loss_config):
+        super().__init__()
+        self.transform = B200BertPredictionHeadTransform(config)
+        self.visual_losses = list(visual_losses)
+        self.decoder_dict = nn.ModuleDict({key: B200Linear(config.hidden_size, visual_loss_config[key][0])
+                                           for key in self.visual_losses})
+
+    def forward(self, hidden_states):
+        h = self.transform(hidden_states)
+        return {key: self.decoder_dict[key](h) for key in self.visual_losses}
+
+
+_LXMERT_LOSSES = {
+    "l2": lambda x, y: nn.functional.smooth_l1_loss(x, y, reduction="none"),
+    "ce": lambda x, y: nn.functional.cross_entropy(x, y, ignore_index=-1, reduction="none"),
+}
+
+
+class B200LXMERTForPretraining(nn.Module):
+    """LXMERTForPretraining (lxmert.py:417-572): trunk, `cls` (BertPreTrainingHeads with the decoder tied to the word
+    embeddings), `obj_predict_head`, `answer_head`.  The losses are the reference's, in fp32 from the bf16 head outputs.
+    The masked-LM loss runs on the fused vocabulary GEMM + cross-entropy (heads.masked_lm_loss(positions="fused")): the
+    same loss without the [B, T, V] logits; a batch without a labelled position gives the zero loss documented there."""
+
+    def __init__(self, config):
+        super().__init__()
+        from .lxmert import B200LXMERTBase
+        self.config = config
+        bc = bert_config_of(config)
+        self.bert = B200LXMERTBase(bc)
+        self.num_labels, self.gqa_labels = config.num_labels, config.gqa_labels
+        self.task_mask_lm, self.task_obj_predict = config.task_mask_lm, config.task_obj_predict
+        self.task_matched, self.task_qa = config.task_matched, config.task_qa
+        self.visual_losses, self.visual_loss_config = list(config.visual_losses), config.visual_loss_config
+        self.cls = B200BertPreTrainingHeads(bc, self.bert.embeddings.word_embeddings.weight)
+        # the reference's own LM head has a bias-free decoder and one `predictions.bias` (lxmert.py:108-126): no
+        # `decoder.bias` alias, so the state_dict keys are LXMERT's
+        self.cls.predictions.decoder.register_parameter("bias", None)
+        if self.task_obj_predict:
+            self.obj_predict_head = B200BertVisualObjHead(bc, self.visual_losses, self.visual_loss_config)
+        if self.task_qa:
+            self.answer_head = B200BertVisualAnswerHead(bc, [self.num_labels, self.gqa_labels])
+        for m in (getattr(self, "obj_predict_head", None), getattr(self, "answer_head", None)):
+            if m is not None:
+                _init_bert_weights(m, float(bc.initializer_range))
+
+    def forward(self, input_ids, token_type_ids=None, attention_mask=None, visual_feats=None, visual_pos=None,
+                visual_attention_mask=None, masked_lm_labels=None, masked_image_labels=None, obj_labels=None,
+                matched_label=None, ans=None, num_features=None, name=None, output_all_attention_masks=False,
+                output_all_encoded_layers=False):
+        (lang_output, visn_output), pooled_output = self.bert(
+            input_ids, token_type_ids, attention_mask, visual_feats, visual_pos, visual_attention_mask,
+            output_all_attention_masks, output_all_encoded_layers)
+        output = {}
+        if ans is not None and self.task_qa:
+            answer_score = self.answer_head(pooled_output, name)
+            n = self.config.num_labels if name is None or "gqa" not in name else self.config.gqa_labels
+            output["answer_loss"] = nn.functional.cross_entropy(answer_score.reshape(-1, n).float(), ans.argmax(-1),
+                                                                ignore_index=-1)
+        if masked_lm_labels is not None and self.task_mask_lm:
+            output["masked_lm_loss"] = masked_lm_loss(self.cls, lang_output, masked_lm_labels, positions="fused")[0]
+        if matched_label is not None and self.task_matched:
+            score = self.cls.seq_relationship(pooled_output)
+            output["matched_loss"] = nn.functional.cross_entropy(score.reshape(-1, 2).float(), matched_label.long(),
+                                                                 ignore_index=-1)
+        if obj_labels is not None and self.task_obj_predict:
+            total = 0.0
+            scores = self.obj_predict_head(visn_output)
+            for key in self.visual_losses:
+                output_dim, loss_name, _, weight = self.visual_loss_config[key]
+                if key == "attr":                                       # the reference skips it (lxmert.py:549-550)
+                    continue
+                if key == "obj":
+                    top = obj_labels.max(-1)
+                    mask_conf = top.values
+                    loss = _LXMERT_LOSSES[loss_name](scores[key].reshape(-1, output_dim).float(), top.indices.reshape(-1))
+                elif key == "feat":
+                    mask_conf = (masked_image_labels == 1).float()
+                    loss = _LXMERT_LOSSES[loss_name](scores[key].reshape(-1, output_dim).float(),
+                                                     visual_feats.reshape(-1, output_dim).float())
+                else:
+                    raise NotImplementedError("LXMERT visual loss %r: the reference defines obj, attr and feat" % key)
+                if loss.dim() > 1:                                      # regression losses
+                    loss = loss.mean(1)
+                total = total + (loss * mask_conf.reshape(-1)).mean() * weight
+            output["visn_loss"] = total
+        return output
+
+
+class B200LXMERTForClassification(nn.Module):
+    """LXMERTForClassification (lxmert.py:575-644): trunk + `classifier` (BertVisualAnswerHead over the pooled output;
+    nlvr2 views it as [-1, 2H])"""
+
+    def __init__(self, config):
+        super().__init__()
+        from .lxmert import B200LXMERTBase
+        self.config = config
+        self.num_labels, self.gqa_labels = config.num_labels, config.gqa_labels
+        self.mode = config.mode
+        bc = bert_config_of(config)
+        self.bert = B200LXMERTBase(bc)
+        self.classifier = B200BertVisualAnswerHead(bc, [self.num_labels, self.gqa_labels])
+        _init_bert_weights(self.classifier, float(bc.initializer_range))
+
+    def forward(self, input_ids, token_type_ids=None, attention_mask=None, visual_feats=None, visual_pos=None,
+                visual_attention_mask=None, masked_lm_labels=None, obj_labels=None, matched_label=None, ans=None,
+                max_features=None, output_all_attention_masks=False, output_all_encoded_layers=False):
+        (_, _), pooled_output = self.bert(input_ids, token_type_ids, attention_mask, visual_feats, visual_pos,
+                                          visual_attention_mask, output_all_encoded_layers, output_all_attention_masks)
+        if self.config.training_head_type == "nlvr2":
+            pooled_output = pooled_output.view(-1, pooled_output.size(1) * 2)
+        logits = self.classifier(pooled_output)
+        return {"scores": logits.contiguous().view(-1, self.config.num_labels).to(pooled_output.dtype)}
+
+
+# options of the reference's YAML that its LXMERT does not implement ("need to implement", defaults.yaml:63-73) or that
+# only other models read: a value other than the default raises instead of being ignored
+_LXMERT_UNSUPPORTED = ("dynamic_attention", "in_batch_pairs", "fast_mode", "output_attentions", "output_hidden_states",
+                       "visualization")
+
+
+@registry.register_model("lxmert")
+class LXMERT(BaseModel):
+    """The registered `lxmert` model (lxmert.py:647-786).
+
+    The SampleList plumbing is the reference's, including its argument swap (lxmert.py:705-708): `input_mask` goes in as
+    `token_type_ids` and `segment_ids` as `attention_mask`.  That is what MMF computes for this model, so it is what is
+    computed here.  The text mask is then (1 - segment_ids) * -10000: with segment ids of 0 every text key gets -10000,
+    and such a row is the softmax of the raw scores (DESIGN.md 4.2), as in the fp32 reference.
+
+    Because of the swap the text "padding" is every token with segment id 0, [CLS] and the masked-LM positions included.
+    Packing it away would zero those rows and change the losses, so forward() raises ValueError when the encoder's
+    two-stream skip-padding (`pack_streams`) is set.  B200LXMERTBase called with real masks keeps the packed path."""
+
+    @classmethod
+    def config_path(cls):
+        return "configs/models/lxmert/pretrain.yaml"
+
+    def build(self):
+        for key in _LXMERT_UNSUPPORTED:
+            if self.config.get(key, False):
+                raise NotImplementedError("LXMERT `%s: true` is not implemented (the reference's YAML marks it as not "
+                                          "implemented or its LXMERT never reads it)" % key)
+        if self.config.training_head_type == "pretraining":
+            self.model = B200LXMERTForPretraining(self.config)
+        else:
+            self.model = B200LXMERTForClassification(self.config)
+        if self.config.get("freeze_base", False):
+            for p in self.model.bert.parameters():
+                p.requires_grad = False
+
+    def get_image_and_text_features(self, sl, device):               # lxmert.py:666-719
+        feats = _sl_get(sl, "image_feature_0", None)
+        R = feats.shape[1]
+        info = _sl_get(sl, "image_info_0", {})
+        bbox = _sl_get(info, "bbox", None)
+        if bbox is not None:
+            bbox = bbox[:, :R, :4]
+        labels = _sl_get(sl, "image_labels", None)
+        if labels is not None:
+            labels = labels[:, :R, None].unsqueeze(-1).to(device)
+        cls_prob = _sl_get(info, "cls_prob", None)
+        if cls_prob is not None:
+            cls_prob = torch.as_tensor(cls_prob)[:, :R, None].to(device)
+        answers = _sl_get(sl, "targets", None)
+        if answers is None:
+            answers = _sl_get(sl, "answers", None)
+        if answers is not None:
+            answers = torch.as_tensor(answers).to(device)
+        is_correct = _sl_get(sl, "is_correct", None)
+        if is_correct is not None:
+            is_correct = torch.as_tensor(is_correct).to(device)
+        return {"input_ids": sl["input_ids"], "token_type_ids": sl["input_mask"], "attention_mask": sl["segment_ids"],
+                "masked_lm_labels": _sl_get(sl, "lm_label_ids", None), "visual_feats": feats, "pos": bbox,
+                "masked_image_labels": labels, "obj_labels": cls_prob, "matched_label": is_correct, "ans": answers,
+                "image_dim": _sl_get(info, "max_features", None), "dataset_name": str(sl["dataset_name"])}
+
+    def forward(self, sample_list):
+        if self.model.bert.encoder._runner.pack_streams:
+            raise ValueError("the registered LXMERT model passes segment_ids as the text attention mask (the reference's "
+                             "argument swap, lxmert.py:707-708): its text padding is every segment-0 token, [CLS] and the "
+                             "masked-LM positions included, so two-stream skip-padding would change the losses; turn it off "
+                             "for this model (patch.set_skip_padding(model, False, two_stream=True))")
+        p = self.get_image_and_text_features(sample_list, sample_list["input_ids"].device)
+        if p["visual_feats"] is not None and p["image_dim"] is not None:
+            p["image_attention_mask"] = image_mask_from_dim(p["visual_feats"], p["image_dim"].to(p["visual_feats"].device))
+        else:
+            p["image_attention_mask"] = None
+        if self.config.training_head_type == "pretraining":
+            out = self.model(input_ids=p["input_ids"], token_type_ids=p["token_type_ids"],
+                             attention_mask=p["attention_mask"], visual_feats=p["visual_feats"], visual_pos=p["pos"],
+                             visual_attention_mask=p["image_attention_mask"], masked_lm_labels=p["masked_lm_labels"],
+                             masked_image_labels=p["masked_image_labels"], obj_labels=p["obj_labels"],
+                             matched_label=p["matched_label"], ans=p["ans"], name=p["dataset_name"])
+            key = "%s/%s" % (sample_list["dataset_name"], sample_list["dataset_type"])
+            out["losses"] = {}
+            for name in ("masked_lm_loss", "matched_loss", "visn_loss", "answer_loss"):
+                if name in out:
+                    out["losses"][key + "/" + name] = out.pop(name)
+            return out
+        return self.model(input_ids=p["input_ids"], token_type_ids=p["token_type_ids"],
+                          attention_mask=p["attention_mask"], visual_feats=p["visual_feats"], visual_pos=p["pos"],
+                          visual_attention_mask=p["image_attention_mask"])

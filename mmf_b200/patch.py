@@ -87,6 +87,10 @@ def set_skip_padding(module, enabled=True, two_stream=False):
     A two-stream call falls back to the dense path when some sample has tokens in one stream and none in the other: there
     the dense outputs of those tokens depend on the other stream's padded rows.
 
+    The registered `lxmert` model refuses packed streams (ValueError): like the reference, it passes segment ids as the text
+    attention mask, so its text "padding" includes [CLS] and the masked-LM positions.  B200LXMERTBase and
+    B200LXMERTEncoder called with real masks keep the packed path.
+
     A call that asks for attention probabilities (output_attentions, or ViLBERT's output_all_attention_masks with
     `visualization`) also runs the dense path, whatever the flag: the probabilities then have the reference's
     [B, heads, S, S] shape, padded rows and keys included."""
