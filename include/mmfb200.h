@@ -179,7 +179,10 @@ typedef struct {
 int mmfb_layernorm_fwd(const mmfb_ln_args* args, mmfb_stream stream);
 int mmfb_layernorm_bwd(const mmfb_ln_args* args, mmfb_stream stream);
 
-/* out[n] += sum_m X[m,n]   (bias gradients), X bf16 [M,N], out fp32 [N] */
+/* out[n] += sum_m X[m,n]   (bias gradients), X bf16 [M,N], out fp32 [N].
+ * Like the LayerNorm calls, the column sums, embed_compose / embed_scatter / embed_scatter_sorted and dropout_apply read
+ * and write bf16 rows as 16-byte vectors: every row tensor they use starts 16-byte aligned and, when M > 1, has a leading
+ * dimension that is a multiple of 8 (the gathered src / dsrc rows whatever M is); MMFB_ERR_ARG otherwise. */
 int mmfb_colsum(const void* X, int64_t ldx, float* out, int M, int N, mmfb_stream stream);
 
 /* Philox keep-bits for nn.Dropout(p): word w bit j <-> element 32*w+j, P(bit=1) = 1-p (16-bit resolution) */

@@ -704,9 +704,11 @@ static int launch_ok(const char* who) {
   return MMFB_OK;
 }
 
-// The LayerNorm kernels move rows as 16-byte vectors (the streaming backward with cp.async.bulk), so every row a kernel
-// reads or writes must start on a 16-byte boundary: the base pointer aligned and, when there is more than one row, the
-// leading dimension a multiple of 8 elements.  Null tensors are not used by the call and are skipped.
+// The row kernels (LayerNorm, column sums, embedding compose / scatter, dropout apply) move rows as 16-byte vectors (the
+// streaming LayerNorm backward with cp.async.bulk), so every row a kernel reads or writes must start on a 16-byte
+// boundary: the base pointer aligned and, when there is more than one row, the leading dimension a multiple of 8
+// elements.  Null tensors are not used by the call and are skipped.  A misaligned view is refused with MMFB_ERR_ARG
+// before anything is launched, instead of faulting in the kernel.
 struct RowTensor {
   const void* p;
   int64_t ld;        // 0 for the [H] vectors
@@ -787,6 +789,8 @@ int ln_bwd(const mmfb_ln_args& a, cudaStream_t s) {
 
 int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s) {
   if (M <= 0 || N <= 0 || N % 8) return set_error(MMFB_ERR_ARG, "colsum: bad shape %dx%d", M, N);
+  const int rc = check_aligned("colsum", M, {{X, ldx, "x"}});
+  if (rc) return rc;
   dim3 grid((N + 255) / 256, 1);
   int rows_blocks = (M + 63) / 64;
   const int cap = (num_sms() * 4 + grid.x - 1) / grid.x;
@@ -810,6 +814,15 @@ int compose(const mmfb_compose_args& a, cudaStream_t s) {
   int rc = check_rows(a.M, a.H, "embed_compose");
   if (rc) return rc;
   if (!a.y) return set_error(MMFB_ERR_ARG, "embed_compose: null output");
+  // a term is read only when both its tensor and its index vector are given; the gathered source rows can be any rows
+  // of their buffer, so their leading dimension is checked whatever M is (the row count 2 below)
+  auto used_src = [&](int k) { return a.src_row[k] != nullptr ? a.src[k] : nullptr; };
+  auto used_tab = [&](int k) { return a.tab_idx[k] != nullptr ? a.tab[k] : nullptr; };
+  rc = check_aligned("embed_compose", 2, {{used_src(0), a.ldsrc[0], "src0"}, {used_src(1), a.ldsrc[1], "src1"},
+                                          {used_tab(0), a.H, "tab0"}, {used_tab(1), a.H, "tab1"}, {used_tab(2), a.H, "tab2"}});
+  if (rc) return rc;
+  rc = check_aligned("embed_compose", a.M, {{a.y, a.ldy, "y"}});
+  if (rc) return rc;
   ComposeDev c;
   for (int k = 0; k < 2; ++k) { c.src[k] = (const bf16*)a.src[k]; c.ldsrc[k] = a.ldsrc[k]; c.srow[k] = a.src_row[k]; }
   for (int k = 0; k < 3; ++k) { c.tab[k] = (const bf16*)a.tab[k]; c.tidx[k] = a.tab_idx[k]; }
@@ -821,6 +834,13 @@ int scatter(const mmfb_scatter_args& a, cudaStream_t s) {
   int rc = check_rows(a.M, a.H, "embed_scatter");
   if (rc) return rc;
   if (!a.dy) return set_error(MMFB_ERR_ARG, "embed_scatter: null input");
+  // the fp32 table gradients take scalar atomics and need no 16-byte rows; the dense-source gradients are stored to
+  // gathered rows (any row of their buffer: leading dimension checked whatever M is)
+  rc = check_aligned("embed_scatter", a.M, {{a.dy, a.lddy, "dy"}});
+  if (rc) return rc;
+  rc = check_aligned("embed_scatter", 2, {{a.src_row[0] != nullptr ? a.dsrc[0] : nullptr, a.ldsrc[0], "dsrc0"},
+                                          {a.src_row[1] != nullptr ? a.dsrc[1] : nullptr, a.ldsrc[1], "dsrc1"}});
+  if (rc) return rc;
   ScatterDev c;
   for (int k = 0; k < 2; ++k) { c.dsrc[k] = (bf16*)a.dsrc[k]; c.ldsrc[k] = a.ldsrc[k]; c.srow[k] = a.src_row[k]; }
   for (int k = 0; k < 3; ++k) { c.dtab[k] = a.dtab[k]; c.tidx[k] = a.tab_idx[k]; }
@@ -833,6 +853,8 @@ int scatter_sorted(const void* dy, int64_t lddy, const int32_t* order, const int
   int rc = check_rows(M, H, "embed_scatter_sorted");
   if (rc) return rc;
   if (H > 1024) return set_error(MMFB_ERR_ARG, "embed_scatter_sorted: hidden size %d > 1024", H);
+  rc = check_aligned("embed_scatter_sorted", M, {{dy, lddy, "dy"}});
+  if (rc) return rc;
   const int warps = (M + 31) / 32;
   const int grid = (warps + ROW_WARPS - 1) / ROW_WARPS;
   const int nv = (H + 255) / 256;
@@ -863,6 +885,9 @@ int add_bf16(const void* a, const void* b, void* out, int64_t n, cudaStream_t s)
 int dropout_apply(const void* x, int64_t ldx, const uint32_t* bits, int64_t ldm, float scale, void* out, int64_t ldo, int M,
                   int H, cudaStream_t s) {
   int rc = check_rows(M, H, "dropout_apply");
+  if (rc) return rc;
+  // the keep-bit words are read one 4-byte word at a time: no row constraint on them
+  rc = check_aligned("dropout_apply", M, {{x, ldx, "x"}, {out, ldo, "out"}});
   if (rc) return rc;
   const int64_t threads = static_cast<int64_t>(M) * 32;
   MMFB_LAUNCH(dropout_apply_kernel, static_cast<unsigned>((threads + 255) / 256), 256, 0, s, (const bf16*)x, ldx, bits, ldm, scale,

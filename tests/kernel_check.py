@@ -18,9 +18,14 @@ can exceed these terms without any kernel bug; use sign-random inputs with this 
 
 On failure the message names the worst element in the kernel's own coordinates (`*_layout` below), so a broken tile,
 row, head or slab is visible at once.
+
+Kernels that only sum are also run on small-integer inputs and must then equal the fp64 result exactly (`exact_ints`,
+`assert_equal`); the element-wise kernels are compared bit for bit (`assert_bits_equal`); the dropout keep-bits are
+compared with a numpy model of the Philox stream (`dropout_uniforms`, `assert_keep_bits`).
 """
 import math
 
+import numpy as np
 import torch
 
 SAFETY = 4.0
@@ -91,16 +96,112 @@ def attn_layout(B, heads, S, d, rows="query"):
 
 
 def row_layout():
-    """[M, H] or [M] or [H]: (row, 256-column slab, column) of the one-warp-per-row kernels."""
+    """[M, H] or [M] or [H]: (row, 256-column slab, lane, column) of the one-warp-per-row kernels."""
     def f(idx):
         if len(idx) == 2:
-            return "row %d, slab %d (column %d)" % (idx[0], idx[1] // 256, idx[1])
+            return "row %d, slab %d, lane %d (column %d)" % (idx[0], idx[1] // 256, (idx[1] % 256) // 8, idx[1])
         return "index %d (row, or slab %d of the column vector)" % (idx[0], idx[0] // 256)
     return f
 
 
 def flat_layout():
     return lambda idx: "element %s" % (idx,)
+
+
+def flat8_layout(n):
+    """flat [n] buffers of the element-wise kernels (relu_bwd, add_bf16, gelu_bwd, cast_f32_bf16): each thread of a
+    256-thread block owns one 8-element vector; the last n % 8 elements are the scalar tail loop of one thread."""
+    def f(idx):
+        i = idx[0]
+        t = i // 8
+        if i >= n - n % 8:
+            return "tail element %d of %d (scalar loop of thread %d, block %d; element %d)" % (i % 8, n % 8, t % 256, t // 256, i)
+        return "8-element vector %d (block %d, thread %d), element %d of the vector (element %d)" % (t, t // 256, t % 256, i % 8, i)
+    return f
+
+
+def colsum_layout():
+    """[N] column sums: (256-column block = blockIdx.x, lane of the 8-column vector, column)."""
+    return lambda idx: "column block %d, lane %d (column %d)" % (idx[0] // 256, (idx[0] % 256) // 8, idx[0])
+
+
+def scatter_sorted_layout(sorted_idx):
+    """[V, H] table gradient of the sorted scatter: the table row, its slab and lane, and the sorted positions of the
+    row's run with the warps (32 positions each) and blocks (256 positions) it spans; a run is flushed at every warp
+    end, so a run that spans several warps is where a lost or doubled row shows."""
+    s = sorted_idx.detach().cpu().to(torch.int64)
+
+    def f(idx):
+        v, c = idx
+        pos = torch.nonzero(s == v).flatten()
+        head = "table row %d, slab %d, lane %d (column %d)" % (v, c // 256, (c % 256) // 8, c)
+        if pos.numel() == 0:
+            return head + ": no sorted position has this index"
+        p0, p1 = int(pos[0]), int(pos[-1])
+        return head + ": run of %d at sorted positions %d..%d, warps %d..%d, blocks %d..%d" % (
+            p1 - p0 + 1, p0, p1, p0 // 32, p1 // 32, p0 // 256, p1 // 256)
+    return f
+
+
+def adamw_layout(group_of_block):
+    """flat [n] AdamW buffers: (8-element block, its hyper-parameter group, CUDA block and thread)."""
+    gid = None if group_of_block is None else group_of_block.detach().cpu().to(torch.int64)
+
+    def f(idx):
+        b = idx[0] // 8
+        g = 0 if gid is None else int(gid[b])
+        return "8-element block %d (CUDA block %d, thread %d), group %d, element %d" % (b, b // 256, b % 256, g, idx[0])
+    return f
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# exact comparisons: exact-sum inputs and the bit-exact element-wise kernels
+# ------------------------------------------------------------------------------------------------------------------
+# A worst-case bound on a long fp32 sum is about U_F32 x depth x sum |x|; on random-sign data that exceeds one row's
+# contribution, so a sum that dropped or repeated a row would pass it.  The summing kernels (column sums, the scatter
+# atomics, the sorted scatter, compose) therefore also run on small integers: every partial sum is then an integer far
+# below 2^24 (exact in fp32; compose's |y| <= 5 x 16 = 80 is also exact in bf16), so whatever the summation or atomic
+# order, the output must EQUAL the fp64 sum.
+def exact_ints(*shape, gen, device="cpu", lo=-16, hi=16):
+    """bf16 integers in [lo, hi]"""
+    return torch.randint(lo, hi + 1, shape, generator=gen, device=device).to(torch.bfloat16)
+
+
+def assert_equal(out, ref, layout, what="output"):
+    """Exact-input check: torch.equal of the output (widened to fp64, which is exact) and the fp64 reference.  On failure
+    the message names the element with the largest |err| in kernel coordinates and how many elements differ."""
+    out64 = out.detach().to(torch.float64)
+    ref = ref.detach().to(device=out64.device, dtype=torch.float64)
+    assert out64.shape == ref.shape, (what, tuple(out64.shape), tuple(ref.shape))
+    if torch.equal(out64, ref):
+        return
+    err = torch.nan_to_num((out64 - ref).abs(), nan=math.inf, posinf=math.inf)
+    flat = int(torch.argmax(torch.nan_to_num(err, posinf=1e308)).item())
+    idx = tuple(int(i) for i in torch.unravel_index(torch.tensor(flat), err.shape))
+    n_bad = int((out64 != ref).sum().item())
+    raise AssertionError("%s: %d element(s) differ from the exact result; largest |err| at %s: got %r, exact %r"
+                         % (what, n_bad, layout(idx), out64[idx].item(), ref[idx].item()))
+
+
+_INT_VIEW = {torch.bfloat16: torch.int16, torch.float16: torch.int16, torch.float32: torch.int32}
+
+
+def assert_bits_equal(out, ref, layout, what="output"):
+    """Bit-exact check of an element-wise kernel: NaN exactly where the reference is NaN (any payload), and the same bit
+    pattern everywhere else (the sign of zero, denormals and infinities included)."""
+    out, ref = out.detach(), ref.detach().to(out.device)
+    assert out.dtype == ref.dtype and out.shape == ref.shape, (what, out.dtype, ref.dtype, tuple(out.shape), tuple(ref.shape))
+    iv = _INT_VIEW[out.dtype]
+    on, rn = torch.isnan(out), torch.isnan(ref)
+    bad = (on != rn) | (~rn & (out.view(iv) != ref.view(iv)))
+    if not bool(bad.any()):
+        return
+    flat = int(torch.nonzero(bad.flatten())[0].item())
+    idx = tuple(int(i) for i in torch.unravel_index(torch.tensor(flat), out.shape))
+    mask = (1 << (8 * out.element_size())) - 1
+    raise AssertionError("%s: %d element(s) not bit-exact; first at %s: got %r (0x%x), expected %r (0x%x)" % (
+        what, int(bad.sum().item()), layout(idx), out[idx].item(), out.view(iv)[idx].item() & mask, ref[idx].item(),
+        ref.view(iv)[idx].item() & mask))
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -267,3 +368,202 @@ def layernorm_bwd_ref(fw, dx, g, dx2=None, keep=None, dscale=1.0, n_sum_terms=1)
     res["dbeta"] = d.sum(0)
     res["b_dbeta"] = U_F32 * n_sum_terms * d.abs().sum(0)
     return res
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# column sums, embedding compose and scatter
+# ------------------------------------------------------------------------------------------------------------------
+def colsum_grid_y(M, N, sms):
+    """row blocks of the column-sum launch: one per 64 rows, capped so that the grid holds about 4 blocks per SM"""
+    gx = (N + 255) // 256
+    cap = (4 * sms + gx - 1) // gx
+    return max(1, min((M + 63) // 64, cap))
+
+
+def colsum_ref(x, out0, sms):
+    """out0 + sum_m x[m] in fp64 and its bound.  The fp32 chain of one column is the rows one warp adds
+    (ceil(M / (8 grid.y))), the 8-warp block sum and one atomic per row block (grid.y), each add rounding at most
+    U_F32 of the sum of the |terms|."""
+    M, N = x.shape
+    gy = colsum_grid_y(M, N, sms)
+    depth = -(-M // (8 * gy)) + 8 + gy
+    x64, o64 = x.to(torch.float64), out0.to(torch.float64)
+    return o64 + x64.sum(0), U_F32 * depth * (o64.abs() + x64.abs().sum(0))
+
+
+def _gather_terms(M, H, terms, device):
+    """sum and sum of |.| of the rows t[i[r]] (i < 0: no term) of (buffer, index) pairs, in fp64"""
+    y = torch.zeros(M, H, dtype=torch.float64, device=device)
+    a = torch.zeros_like(y)
+    for t, i in terms:
+        i = i.to(device=device, dtype=torch.int64)
+        rows = t.to(torch.float64)[i.clamp_min(0)] * (i >= 0).to(torch.float64)[:, None]
+        y += rows
+        a += rows.abs()
+    return y, a
+
+
+def compose_ref(M, H, srcs, tabs, device):
+    """y[r] = sum_k src_k[row_k[r]] + sum_k tab_k[idx_k[r]] in fp64 and its bound: up to 5 terms added in fp32 (at most
+    4 roundings of U_F32 sum |terms|), then the bf16 output rounding"""
+    y, a = _gather_terms(M, H, list(srcs) + list(tabs), device)
+    return y, U_BF16 * y.abs() + 4 * U_F32 * a
+
+
+def scatter_table_ref(dtab0, dy, idx):
+    """dtab0[v] + sum_{r: idx[r] = v} dy[r] in fp64 and its bound.  Both scatters add n_v terms into row v in fp32 in an
+    order that is not fixed (atomics; the sorted scatter first sums each run in registers, with one atomic per run):
+    n_v roundings of at most U_F32 (|dtab0[v]| + sum |dy[r]|)."""
+    V = dtab0.shape[0]
+    i = idx.to(device=dy.device, dtype=torch.int64)
+    ok = i >= 0
+    d64 = dy.to(torch.float64)[ok]
+    ref, a = dtab0.to(torch.float64).clone(), dtab0.to(torch.float64).abs()
+    ref.index_add_(0, i[ok], d64)
+    a.index_add_(0, i[ok], d64.abs())
+    n = torch.bincount(i[ok], minlength=V).to(torch.float64)
+    return ref, U_F32 * n[:, None] * a
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# dropout keep-bits: a numpy model of the Philox stream, stated per element
+# ------------------------------------------------------------------------------------------------------------------
+_M32 = 0xFFFFFFFF
+
+
+def philox4x32_7(seed, ctr):
+    """Philox4x32 with 7 rounds as common.cuh defines it: key = (seed low, seed high), counter = (ctr low, ctr high,
+    0x243F6A88, 0x85A308D3).  ctr: uint64 array.  Returns the four uint32 outputs (uint64 arrays holding 32-bit values)."""
+    ctr = np.asarray(ctr, dtype=np.uint64)
+    m32, s32 = np.uint64(_M32), np.uint64(32)
+    c0, c1 = ctr & m32, ctr >> s32
+    c2, c3 = np.full_like(ctr, 0x243F6A88), np.full_like(ctr, 0x85A308D3)
+    k0, k1 = seed & _M32, (seed >> 32) & _M32
+    for _ in range(7):
+        p0, p1 = c0 * np.uint64(0xD2511F53), c2 * np.uint64(0xCD9E8D57)      # < 2^64: exact
+        c0, c1, c2, c3 = (p1 >> s32) ^ c1 ^ np.uint64(k0), p1 & m32, (p0 >> s32) ^ c3 ^ np.uint64(k1), p0 & m32
+        k0, k1 = (k0 + 0x9E3779B9) & _M32, (k1 + 0xBB67AE85) & _M32
+    return c0, c1, c2, c3
+
+
+def dropout_thresh16(p):
+    """the kernel's 16-bit threshold, evaluated in fp32 like the host code: min(65535, floor(p 65536 + 0.5))"""
+    t = np.float32(p) * np.float32(65536.0) + np.float32(0.5)
+    return min(65535, int(np.floor(t)))
+
+
+def dropout_planes(nwords, seed, offset, epoch=0):
+    """[16, nwords] uint32: row b holds bit b of the 32 uniforms of each word (bit e of the row = uniform e).  Word w
+    draws the Philox counters offset + (epoch << 40) + 4 w + i, i = 0..3 (mod 2^64), and output k of draw i is the
+    plane of bit 15 - (4 i + k)."""
+    base = np.uint64((offset + (epoch << 40)) % 2 ** 64)
+    w4 = np.arange(nwords, dtype=np.uint64) * np.uint64(4)
+    planes = np.empty((16, nwords), dtype=np.uint32)
+    for i in range(4):
+        out = philox4x32_7(seed, base + w4 + np.uint64(i))
+        for k in range(4):
+            planes[15 - (4 * i + k)] = out[k].astype(np.uint32)
+    return planes
+
+
+def uniforms_from_planes(planes):
+    """[16, W] bit-planes -> [W, 32] uint32 sixteen-bit uniforms r_e (bit b of r_e = bit e of plane b)"""
+    e = np.arange(32, dtype=np.uint32)
+    r = np.zeros((planes.shape[1], 32), dtype=np.uint32)
+    for b in range(16):
+        r |= ((planes[b][:, None] >> e) & np.uint32(1)) << np.uint32(b)
+    return r
+
+
+def dropout_uniforms(nwords, seed, offset, epoch=0):
+    """[nwords, 32] uniforms of the keep-bit words; element 32 w + e is kept where uniforms[w, e] >= thresh16"""
+    return uniforms_from_planes(dropout_planes(nwords, seed, offset, epoch))
+
+
+def assert_keep_bits(words, uniforms, p, what="keep bits"):
+    """words (int32, any shape, flat = word index) against the model: bit e of word w = (uniforms[w, e] >= thresh16)"""
+    t = dropout_thresh16(p)
+    got = np.ascontiguousarray(words.detach().cpu().numpy()).view(np.uint32).reshape(-1)
+    assert got.shape[0] == uniforms.shape[0], (what, got.shape, uniforms.shape)
+    gk = ((got[:, None] >> np.arange(32, dtype=np.uint32)) & np.uint32(1)).astype(bool)
+    bad = gk != (uniforms >= t)
+    if bad.any():
+        w, e = (int(v) for v in np.argwhere(bad)[0])
+        raise AssertionError("%s: %d keep bit(s) in %d word(s) differ from the model; first: word %d, bit %d at p = %r "
+                             "(thresh16 %d): kernel %d, uniform %d" % (what, int(bad.sum()), int(bad.any(1).sum()), w, e,
+                                                                       p, t, int(gk[w, e]), int(uniforms[w, e])))
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# AdamW (include/mmfb200.h: mmfb_adamw), one step in fp64 with the error bound carried across steps
+# ------------------------------------------------------------------------------------------------------------------
+def _f32(x):
+    return float(np.float32(x))
+
+
+def adamw_step_ref(st, g, groups, gid, *, beta1, beta2, eps, mode, grad_scale):
+    """Advances st = {p, m, v, e_p, e_m, e_v} (fp64 [n]; e_* the error bounds of the kernel's fp32 state) by one step
+    with gradient g (fp32 [n]), the operation order of the kernel, and hyper-parameters rounded to fp32 as the C ABI
+    passes them.  Each fp32 operation adds U_F32 of its result (first order); errors already in p, m and v propagate
+    through the update."""
+    U = U_F32
+    dev = st["p"].device
+    grp = (torch.zeros(st["p"].numel() // 8, dtype=torch.int64, device=dev) if gid is None
+           else gid.to(device=dev, dtype=torch.int64)).repeat_interleave(8)
+
+    def per(key):           # the hyper-parameter of each element's group
+        return torch.tensor([_f32(gr[key]) for gr in groups], dtype=torch.float64, device=dev)[grp]
+    lr, wd, step, bc2s = per("lr"), per("weight_decay"), per("step_size"), per("bc2_sqrt")
+    b1, b2, eps, gs = _f32(beta1), _f32(beta2), _f32(eps), _f32(grad_scale)
+    c1, c2 = float(np.float32(1) - np.float32(b1)), float(np.float32(1) - np.float32(b2))
+    p, m, v, e_p, e_m, e_v = (st[k] for k in ("p", "m", "v", "e_p", "e_m", "e_v"))
+    gr = g.to(torch.float64) * gs
+    e_gr = U * gr.abs()
+    lw = lr * wd
+    if mode == 1:
+        p1 = p * (1 - lw)                                               # lr*wd, 1 - lr*wd and the product: 3 roundings
+        e_p = e_p * (1 - lw) + p.abs() * U * (lw + (1 - lw)) + U * p1.abs()
+        p = p1
+        d = gr - m                                                      # m.lerp_(g, 1 - b1) = fma(g - m, 1 - b1, m)
+        m_new = m + c1 * d
+        e_m = (1 - c1) * e_m + c1 * (e_gr + U * d.abs()) + U * m_new.abs()
+    else:
+        m_new = b1 * m + c1 * gr                                        # fma(g, 1 - b1, m * b1)
+        e_m = b1 * e_m + c1 * e_gr + U * b1 * m.abs() + U * m_new.abs()
+    v_new = b2 * v + c2 * gr * gr                                       # fma(g * g, 1 - b2, v * b2)
+    e_v = b2 * e_v + c2 * (2 * gr.abs() * e_gr + U * gr * gr) + U * b2 * v + U * v_new
+    s = v_new.sqrt()
+    e_s = e_v / (2 * s) + U * s
+    if mode == 1:
+        s, e_s = s / bc2s, e_s / bc2s + U * s / bc2s
+    den = s + eps
+    e_den = e_s + U * den
+    q = m_new / den
+    e_q = e_m / den + q.abs() * e_den / den + U * q.abs()
+    p1 = p - step * q                                                   # fma(-step, m / denom, p)
+    e_p = e_p + step * e_q + U * p1.abs()
+    if mode == 0:
+        dec = wd > 0                                                    # fma(p, -lr * wd, p)
+        p2 = torch.where(dec, p1 * (1 - lw), p1)
+        e_p = torch.where(dec, e_p * (1 + lw) + U * lw * p1.abs() + U * p2.abs(), e_p)
+        p1 = p2
+    st.update(p=p1, m=m_new, v=v_new, e_p=e_p, e_m=e_m, e_v=e_v)
+    return st
+
+
+def adamw_state(p, m, v):
+    """fp64 copy of the fp32 optimizer state with zero error bounds, for adamw_step_ref"""
+    st = {k: t.detach().to(torch.float64).clone() for k, t in (("p", p), ("m", m), ("v", v))}
+    st.update({"e_" + k: torch.zeros_like(st[k]) for k in ("p", "m", "v")})
+    return st
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# element-wise GELU backward
+# ------------------------------------------------------------------------------------------------------------------
+def gelu_bwd_ref(dh, u):
+    """du = dh GELU'(u) in fp64 and its bound: GELU' in fp32 with the erf / ex2 approximations (|err| <= 2^-21 (1 + |u|),
+    as in the GEMM's gelu_bwd epilogue), the fp32 product and the bf16 output rounding"""
+    dh64, u64 = dh.to(torch.float64), u.to(torch.float64)
+    ref = dh64 * gelu_grad64(u64)
+    return ref, U_BF16 * ref.abs() + U_F32 * ref.abs() + dh64.abs() * 2.0 ** -21 * (1 + u64.abs())
