@@ -126,23 +126,7 @@ class B200DataParallel(nn.Module):
         """offset (elements) in the flat buffer where the parameters of execution step `step_index` start; the
         packs are laid out in execution order, so everything at or above it is complete once that step's backward
         has been enqueued."""
-        ranges = getattr(runner, "step_offsets", None)
-        if ranges is None:
-            per_step = []
-            if hasattr(runner, "steps"):      # ViLBERT: variable number of params per step
-                from .engine import BertLayerW, ConnectionW
-                idx = 0
-                for kind, i in runner.steps:
-                    per_step.append(runner.pack.offsets[idx])
-                    mods = {"t": runner.layer, "v": runner.v_layer, "c": runner.c_layer}[kind]
-                    idx += len((ConnectionW if kind == "c" else BertLayerW).params(mods[i]))
-            elif hasattr(runner, "layer_param_ranges"):
-                per_step = [r[0] for r in runner.layer_param_ranges]
-            else:                             # single-step runners (embedding front-end): one bucket
-                per_step = [0]
-            runner.step_offsets = per_step
-            ranges = per_step
-        return ranges[step_index]
+        return runner.step_offsets[step_index]
 
     def _avg(self, flat):
         """mean over ranks: NCCL reduces with AVG in one pass; gloo (CPU tests) has no AVG"""

@@ -24,6 +24,7 @@ class _EmbedRunner:
         self.tables, self.others = list(tables), list(others)
         self.pack = None
         self.grad_ready_hook = None
+        self.step_offsets = [0]   # one step: one gradient bucket
         self.eps = F.LN_EPS       # set by the owning module from its LayerNorm holder
 
     def ensure(self, device):

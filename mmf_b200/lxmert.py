@@ -9,7 +9,8 @@ Same sub-module / parameter names (`visn_fc.{visn_fc,visn_layer_norm,box_fc,box_
 `r_layers.{i}`, `x_layers.{i}.{visual_attention.att,visual_attention.output,lang_self_att,visn_self_att,lang_inter,
 lang_output,visn_inter,visn_output}`) and the forward signature `(lang_feats, lang_attention_mask, (feats, boxes),
 visn_attention_mask) -> (lang_feats, visn_feats)`.  No new device code: language / relational layers are BERT layers,
-the cross-modality layer is engine.xlayer_fwd/bwd (one shared cross-attention block used in both directions).
+the cross-modality layer is engine.xlayer_fwd/bwd (one shared cross-attention block used in both directions), and
+modules.TwoStreamRunner runs them as it runs ViLBERT's layers.
 The registered model and its heads are in mmf_b200.models (`lxmert`).
 """
 import torch
@@ -18,8 +19,7 @@ from torch import nn
 from . import engine as E
 from . import ops
 from .modules import (B200BertAttention, B200BertIntermediate, B200BertLayer, B200BertSelfAttention,
-                      B200BertSelfOutput, _Holder, _Packing, _fresh_dropout_state, _init_bert_weights, _require_cuda,
-                      plan_two_stream)
+                      B200BertSelfOutput, TwoStreamRunner, _Holder, _init_bert_weights, _require_cuda, run_two_stream_encoder)
 from .vilbert import B200BertTextEmbeddings
 from .visual_bert import BertPooler
 
@@ -73,115 +73,6 @@ class B200LXMERTXLayer(_Holder):
         self.visn_output = B200BertSelfOutput(it, h, ph, 1e-12)
 
 
-class LxmertRunner:
-    """execution order: language layers, relational (vision) layers, cross-modality layers (lxmert.py:318-334)"""
-
-    def __init__(self, layer, r_layers, x_layers):
-        self.layer, self.r_layers, self.x_layers = list(layer), list(r_layers), list(x_layers)
-        self.steps = [("l", i) for i in range(len(self.layer))] + [("r", i) for i in range(len(self.r_layers))] + \
-                     [("x", i) for i in range(len(self.x_layers))]
-        self.pack = None
-        self.w = None
-        self.grad_ready_hook = None
-        # skip padded tokens in both streams (modules.plan_two_stream): every layer runs on each stream's valid rows only
-        self.pack_streams = False
-
-    def _mod(self, kind, i):
-        return {"l": self.layer, "r": self.r_layers, "x": self.x_layers}[kind][i]
-
-    def ensure(self, device):
-        if self.pack is not None and self.pack.intact() and self.pack.device == device:
-            return
-        params = []
-        for kind, i in self.steps:
-            params += (E.XLayerW if kind == "x" else E.BertLayerW).params(self._mod(kind, i))
-        for p in params:
-            _require_cuda(p, "encoder parameter")
-        self.pack = E.ParamPack(params, device)
-        self.w = {(k, i): (E.XLayerW if k == "x" else E.BertLayerW)(self.pack, self._mod(k, i)) for k, i in self.steps}
-        # offsets where the parameters of each execution step start (data-parallel bucket boundaries)
-        self.step_offsets, idx = [], 0
-        for kind, i in self.steps:
-            self.step_offsets.append(self.pack.offsets[idx])
-            idx += len((E.XLayerW if kind == "x" else E.BertLayerW).params(self._mod(kind, i)))
-
-    @staticmethod
-    def _p(mod):
-        d = getattr(mod, "dropout", None)
-        return float(getattr(d, "p", 0.0)) if d is not None else 0.0
-
-    def forward(self, lang, visn, lmask, vmask, B, T, R, training, need_grad):
-        ds = _fresh_dropout_state() if training else None
-        saved = []
-        for kind, i in self.steps:
-            m, w = self._mod(kind, i), self.w[(kind, i)]
-            if kind == "x":
-                pa, ph = (self._p(m.visual_attention.att), self._p(m.visual_attention.output)) if training else (0.0, 0.0)
-                lang, visn, s = E.xlayer_fwd(lang, visn, lmask, vmask, w, B, T, R, pa, ph, ds)
-            else:
-                pa, ph = (self._p(m.attention.self), self._p(m.attention.output)) if training else (0.0, 0.0)
-                if kind == "l":
-                    lang, s = E.bert_layer_fwd(lang, lmask, w, B, T, pa, ph, ds)
-                else:
-                    visn, s = E.bert_layer_fwd(visn, vmask, w, B, R, pa, ph, ds)
-            saved.append(s if need_grad else None)
-        return lang, visn, saved
-
-    def backward(self, dl, dv, saved, lmask, vmask, B, T, R):
-        for j in range(len(self.steps) - 1, -1, -1):
-            kind, i = self.steps[j]
-            w = self.w[(kind, i)]
-            if kind == "x":
-                dl, dv = E.xlayer_bwd(dl, dv, saved[j], lmask, vmask, w, B, T, R)
-            elif kind == "l":
-                dl = E.bert_layer_bwd(dl, saved[j], lmask, w, B, T)
-            else:
-                dv = E.bert_layer_bwd(dv, saved[j], vmask, w, B, R)
-            saved[j] = None
-            if self.grad_ready_hook is not None:
-                E.join_side()
-                self.grad_ready_hook(j)
-        return dl, dv
-
-
-class _LxmertEncoderFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, runner, lmask, vmask, training, lang, visn, *params):
-        B, T, H = lang.shape
-        R = visn.shape[1]
-        need_grad = any(ctx.needs_input_grad)
-        runner.pack.refresh()
-        l = lang.detach().to(torch.bfloat16).contiguous().view(B * T, H)
-        v = visn.detach().to(torch.bfloat16).contiguous().view(B * R, H)
-        if isinstance(lmask, _Packing):
-            l, v, saved = runner.forward(lmask.pack(l), vmask.pack(v), lmask.varlen, vmask.varlen, B, T, R, training, need_grad)
-            l, v = lmask.unpack(l, B * T), vmask.unpack(v, B * R)
-        else:
-            l, v, saved = runner.forward(l, v, lmask, vmask, B, T, R, training, need_grad)
-        ctx.runner, ctx.saved, ctx.masks, ctx.dims, ctx.dtypes = runner, saved, (lmask, vmask), (B, T, R, H), (lang.dtype, visn.dtype)
-        return l.view(B, T, H).to(lang.dtype), v.view(B, R, H).to(visn.dtype)
-
-    @staticmethod
-    def backward(ctx, dlang, dvisn):
-        runner = ctx.runner
-        B, T, R, H = ctx.dims
-        if ctx.saved is None:
-            raise RuntimeError("B200 LXMERT encoder: backward called twice")
-        aliased = runner.pack.prepare_grads()
-        dev = runner.pack.device
-        dl = (dlang if dlang is not None else torch.zeros(B, T, H, device=dev)).to(torch.bfloat16).contiguous().view(B * T, H)
-        dv = (dvisn if dvisn is not None else torch.zeros(B, R, H, device=dev)).to(torch.bfloat16).contiguous().view(B * R, H)
-        lm, vm = ctx.masks
-        if isinstance(lm, _Packing):
-            dl, dv = runner.backward(lm.pack(dl), vm.pack(dv), ctx.saved, lm.varlen, vm.varlen, B, T, R)
-            dl, dv = lm.unpack(dl, B * T), vm.unpack(dv, B * R)
-        else:
-            dl, dv = runner.backward(dl, dv, ctx.saved, lm, vm, B, T, R)
-        ctx.saved = None
-        return (None, None, None, None, dl.view(B, T, H).to(ctx.dtypes[0]), dv.view(B, R, H).to(ctx.dtypes[1])) + tuple(
-            runner.pack.autograd_grads(aliased))
-
-
 class B200LXMERTEncoder(nn.Module):
     """config: BertConfig-like + visual_feat_dim, visual_pos_dim, l_layers, x_layers, r_layers
     (mmf/configs/models/lxmert/defaults.yaml)."""
@@ -197,25 +88,20 @@ class B200LXMERTEncoder(nn.Module):
         self.x_layers = nn.ModuleList([B200LXMERTXLayer(config) for _ in range(self.num_x_layers)])
         self.r_layers = nn.ModuleList([mk() for _ in range(self.num_r_layers)])
         _init_bert_weights(self, float(getattr(config, "initializer_range", 0.02)))
-        self._runner = LxmertRunner(self.layer, self.r_layers, self.x_layers)
+        # execution order: language layers, relational (vision) layers, cross-modality layers (lxmert.py:318-334)
+        self._runner = TwoStreamRunner([(m, E.BertLayerW, (0,)) for m in self.layer] +
+                                       [(m, E.BertLayerW, (1,)) for m in self.r_layers] +
+                                       [(m, E.XLayerW, (0, 1)) for m in self.x_layers])
         self._runner.pack_streams = bool(getattr(config, "skip_padding", False))
 
     def forward(self, lang_feats, lang_attention_mask, visn_feats, visn_attention_mask=None):
         _require_cuda(lang_feats, "lang_feats")
         visn = self.visn_fc(visn_feats)
-        B, T, _ = lang_feats.shape
-        R = visn.shape[1]
-        self._runner.ensure(lang_feats.device)
-        lmask = E.additive_mask_2d(lang_attention_mask, B, T)
-        vmask = E.additive_mask_2d(visn_attention_mask, B, R)
         visn = visn.to(lang_feats.dtype)
-        if self._runner.pack_streams:
-            plan = plan_two_stream(lmask, vmask, B, T, R, lang_feats.device)
-            if plan == "empty":       # every token of both streams is padding: outputs and input gradients are zeros
-                return lang_feats * 0, visn * 0
-            if plan is not None:
-                lmask, vmask = plan
-        return _LxmertEncoderFn.apply(self._runner, lmask, vmask, self.training, lang_feats, visn, *self._runner.pack.params)
+        outs = run_two_stream_encoder(self._runner, lang_feats, visn, lang_attention_mask, visn_attention_mask, self.training)
+        if outs is None:              # every token of both streams is padding: outputs and input gradients are zeros
+            return lang_feats * 0, visn * 0
+        return outs
 
 
 class B200LXMERTBase(nn.Module):

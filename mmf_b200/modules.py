@@ -4,6 +4,8 @@ return structure as the reference's encoders, computing on the B200 engine.
   B200BertEncoder     <->  BertEncoderJit           mmf/modules/hf_layers.py:295-355
   B200ViLBertEncoder  <->  vilbert.BertEncoder      mmf/models/vilbert.py:559-796
 
+EncoderRunner runs a single-stream layer stack, TwoStreamRunner the ViLBERT and LXMERT (mmf_b200.lxmert) ones.
+
 Parameter names are the reference's (`layer.{i}.attention.self.query.weight`, `c_layer.{i}.biattention.query1.bias`,
 `c_layer.{i}.biOutput.q_dense1.weight` ... SURVEY.md 5 "Checkpoint / resume"), so zoo checkpoints and
 `pretrained_state_mapping` keep loading.  The nn.Linear / nn.LayerNorm children below are parameter HOLDERS:
@@ -50,7 +52,7 @@ def _check_erf_gelu(layer):
 _SEED_COUNTER = [0]
 
 
-def _fresh_dropout_state(prefetchable=False):
+def _fresh_dropout_state():
     """One Philox stream per forward, derived from torch's seed so `torch.manual_seed` makes runs repeatable.
     (The bits are drawn on the compute stream: the GEMMs a side-stream generator would overlap occupy every SM.)"""
     _SEED_COUNTER[0] += 1
@@ -61,70 +63,71 @@ def _fresh_dropout_state(prefetchable=False):
 # ------------------------------------------------------------------------------------------------------
 # single-stream BERT encoder
 # ------------------------------------------------------------------------------------------------------
-class EncoderRunner:
-    """Engine state of one BERT-style layer stack (built lazily on the first CUDA forward)."""
+class _LayerStack:
+    """Engine state of layers run in a fixed order, layer i with handles class Ws[i] (built lazily on the first CUDA
+    forward): ONE ParamPack over the layers' parameters in execution order, so that data-parallel gradient buckets complete
+    in reverse order, and each layer's handles."""
 
-    W = E.BertLayerW                       # parameter handles of one layer
-    _fwd = staticmethod(E.bert_layer_fwd)  # (x, add_mask, w, B, S, p_attn, p_hidden, ds) -> (out, saved)
-    _bwd = staticmethod(E.bert_layer_bwd)  # (dout, saved, add_mask, w, B, S) -> dx
-
-    def __init__(self, layers):
-        self.layers = list(layers)
+    def __init__(self, layers, Ws):
+        self._stack = list(zip(layers, Ws))
+        self._starts = None
         self.pack = None
         self.weights = None
-        self.grad_ready_hook = None   # callable(layer_index) - set by mmf_b200.ddp for bucket all-reduce overlap
-        # skip padded tokens: pack the valid rows once per encoder call and run variable-length attention (run_bert_encoder)
-        self.skip_padding = False
-
-    def _probs(self, m):
-        def p_of(mod):
-            d = getattr(mod, "dropout", None)
-            return float(getattr(d, "p", 0.0)) if d is not None else 0.0
-        return p_of(m.attention.self), p_of(m.attention.output)
+        self.grad_ready_hook = None   # callable(step_index) - set by mmf_b200.ddp for bucket all-reduce overlap
 
     def ensure(self, device):
         if self.pack is not None and self.pack.intact() and self.pack.device == device:
             return
-        params = []
-        for m in self.layers:
+        for m, _ in self._stack:
             _check_erf_gelu(m)
-            params += self.W.params(m)
+        params = [p for m, W in self._stack for p in W.params(m)]
         for p in params:
             _require_cuda(p, "encoder parameter")
         self.pack = E.ParamPack(params, device)
-        self.weights = [self.W(self.pack, m) for m in self.layers]
-        self.layer_param_ranges = []
-        per = len(self.W.params(self.layers[0])) if self.layers else 0
-        for i in range(len(self.layers)):
-            o0 = self.pack.offsets[i * per]
-            o1 = self.pack.offsets[(i + 1) * per] if (i + 1) * per < len(self.pack.offsets) else self.pack.total
-            self.layer_param_ranges.append((o0, o1))
+        self.weights = [W(self.pack, m) for m, W in self._stack]
 
-    def forward(self, x, add_mask, training, need_grad, first_layer=0, last_layer=None, probs=None):
+    @property
+    def step_offsets(self):
+        """offset in the pack's flat buffers where each layer's parameters start (the data-parallel bucket boundaries)"""
+        if self._starts is None:
+            self._starts = [0]
+            for m, W in self._stack[:-1]:
+                self._starts.append(self._starts[-1] + len(W.params(m)))
+        return [self.pack.offsets[i] for i in self._starts]
+
+
+class EncoderRunner(_LayerStack):
+    """Engine state of one BERT-style layer stack."""
+
+    W = E.BertLayerW                       # parameter handles and block functions of one layer
+
+    def __init__(self, layers):
+        self.layers = list(layers)
+        super().__init__(self.layers, [self.W] * len(self.layers))
+        # skip padded tokens: pack the valid rows once per encoder call and run variable-length attention (run_bert_encoder)
+        self.skip_padding = False
+
+    def forward(self, x, add_mask, training, need_grad, probs=None):
         """probs: an engine.ProbsSink that receives every layer's attention probabilities, or None"""
         B, S, H = x.shape
         h = x.reshape(B * S, H)
         saved = []
-        ds = _fresh_dropout_state(prefetchable=True) if training else None
-        last_layer = len(self.layers) if last_layer is None else last_layer
+        ds = _fresh_dropout_state() if training else None
         hiddens = []
         extra = {} if probs is None else {"probs": probs}
-        for i in range(first_layer, last_layer):
-            m = self.layers[i]
-            pa, ph = self._probs(m) if training else (0.0, 0.0)
+        for m, w in zip(self.layers, self.weights):
+            pa, ph = self.W.dropout_p(m) if training else (0.0, 0.0)
             hiddens.append(h)
-            h, s = self._fwd(h, add_mask, self.weights[i], B, S, pa, ph, ds, **extra)
+            h, s = self.W.fwd(h, add_mask, w, B, S, pa, ph, ds, **extra)
             saved.append(s if need_grad else None)
         return h, saved, hiddens
 
-    def backward(self, dout, saved, add_mask, B, S, first_layer=0):
+    def backward(self, dout, saved, add_mask, B, S):
         d = dout
-        for j in range(len(saved) - 1, -1, -1):
-            i = first_layer + j
-            d = self._bwd(d, saved[j], add_mask, self.weights[i], B, S)
-            saved[j] = None
+        for i in range(len(saved) - 1, -1, -1):
+            d = self.W.bwd(d, saved[i], add_mask, self.weights[i], B, S)
+            saved[i] = None
             if self.grad_ready_hook is not None:
-                E.join_side(d.device)
                 self.grad_ready_hook(i)
         return d
 
@@ -314,6 +317,118 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
     return outs
 
 
+class TwoStreamRunner(_LayerStack):
+    """Engine state of a two-stream layer stack (ViLBERT, LXMERT).  `steps` lists
+    the layers in execution order as (module, W, streams): W is the layer's handles class (which also holds its block
+    functions) and `streams` the stream indices the block function takes, in its argument order - (0,) or (1,) for a
+    single-stream layer, both for a layer that joins them (ViLBERT's co-attention takes (image, text) = (1, 0), LXMERT's
+    cross-modality layer (language, vision) = (0, 1)).  Stream 0 is text / language, stream 1 image / vision."""
+
+    def __init__(self, steps):
+        self.steps = list(steps)
+        super().__init__([m for m, _, _ in self.steps], [W for _, W, _ in self.steps])
+        # skip padded tokens in both streams: pack each stream's valid rows once per encoder call and run variable-length
+        # self- and cross-attention (plan_two_stream)
+        self.pack_streams = False
+
+    def forward(self, xs, masks, lens, B, training, need_grad, block_states=None, probs=None):
+        """xs: the two streams' [rows, H] activations, replaced by the outputs; masks: their additive masks, None or Varlen
+        descriptors; lens: their sequence lengths.  Returns what the backward needs.  block_states: a list that receives
+        (stream 0, stream 1) after every step that joins the streams, or None.  probs: an engine.ProbsSink that receives
+        the attention probabilities in step order, or None."""
+        ds = _fresh_dropout_state() if training else None
+        extra = {} if probs is None else {"probs": probs}
+        saved = []
+        for (m, W, streams), w in zip(self.steps, self.weights):
+            ps = [p if training else 0.0 for p in W.dropout_p(m)]
+            *outs, s = W.fwd(*[xs[k] for k in streams], *[masks[k] for k in streams], w, B, *[lens[k] for k in streams],
+                             *ps, ds, **extra)
+            for k, o in zip(streams, outs):
+                xs[k] = o
+            if block_states is not None and len(streams) == 2:
+                block_states.append(tuple(xs))
+            saved.append(s if need_grad else None)
+        return saved
+
+    def backward(self, grads, saved, masks, lens, B):
+        """grads: the two streams' output gradients, replaced by the input gradients"""
+        for j in range(len(self.steps) - 1, -1, -1):
+            _, W, streams = self.steps[j]
+            d = W.bwd(*[grads[k] for k in streams], saved[j], *[masks[k] for k in streams], self.weights[j], B,
+                      *[lens[k] for k in streams])
+            for k, g in zip(streams, d if len(streams) == 2 else (d,)):
+                grads[k] = g
+            saved[j] = None
+            if self.grad_ready_hook is not None:
+                self.grad_ready_hook(j)
+
+
+class _TwoStreamEncoderFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, runner, masks, training, want_blocks, want_attn, x0, x1, *params):
+        B = x0.shape[0]
+        lens, Hs, dts = (x0.shape[1], x1.shape[1]), (x0.shape[2], x1.shape[2]), (x0.dtype, x1.dtype)
+        need_grad = any(ctx.needs_input_grad)
+        runner.pack.refresh()
+        xs = [x.detach().to(torch.bfloat16).contiguous().view(B * S, H) for x, S, H in zip((x0, x1), lens, Hs)]
+        packings = masks if isinstance(masks[0], _Packing) else None
+        if packings is not None:                  # both streams run on their valid rows only
+            xs, masks = [pk.pack(x) for pk, x in zip(packings, xs)], [pk.varlen for pk in packings]
+        blocks = [] if want_blocks else None
+        probs = _probs_sink(*dts) if want_attn else None
+        saved = runner.forward(xs, list(masks), lens, B, training, need_grad, blocks, probs)
+        ctx.runner, ctx.saved, ctx.masks, ctx.packings, ctx.dims = runner, saved, masks, packings, (B, lens, Hs, dts)
+        states = [xs] + (blocks or [])
+        outs = [_unpacked(packings, k, t, B, lens).view(B, lens[k], Hs[k]).to(dts[k]) for st in states
+                for k, t in enumerate(st)]
+        if want_attn:
+            # step order, one per query stream (stream 0's first); each in its query stream's dtype
+            it = iter(probs)
+            outs += [next(it).to(dts[k]) for _, _, streams in runner.steps for k in sorted(streams)]
+        if len(outs) > 2:
+            ctx.mark_non_differentiable(*outs[2:])
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, d0, d1, *unused):
+        runner = ctx.runner
+        B, lens, Hs, dts = ctx.dims
+        if ctx.saved is None:
+            raise RuntimeError("B200 two-stream encoder: backward called twice")
+        aliased = runner.pack.prepare_grads()
+        grads = [(d if d is not None else torch.zeros(B, S, H, device=runner.pack.device)).to(torch.bfloat16).contiguous()
+                 .view(B * S, H) for d, S, H in zip((d0, d1), lens, Hs)]
+        if ctx.packings is not None:
+            grads = [pk.pack(d) for pk, d in zip(ctx.packings, grads)]
+        runner.backward(grads, ctx.saved, ctx.masks, lens, B)
+        ctx.saved = None
+        dx = [_unpacked(ctx.packings, k, d, B, lens).view(B, lens[k], Hs[k]).to(dts[k]) for k, d in enumerate(grads)]
+        return (None, None, None, None, None) + tuple(dx) + tuple(runner.pack.autograd_grads(aliased))
+
+
+def _unpacked(packings, k, t, B, lens):
+    return t if packings is None else packings[k].unpack(t, B * lens[k])
+
+
+def run_two_stream_encoder(runner, x0, x1, mask0, mask1, training, want_blocks=False, want_attn=False):
+    """x0 / x1: the streams' [B, S, H] states (fp32 or bf16), mask0 / mask1 their additive [B,1,1,S] / [B,S] / None masks.
+    Returns the two outputs, then (stream 0, stream 1) after every step that joins the streams if want_blocks, then the
+    attention probabilities in step order if want_attn; the block states and probabilities carry no gradient.  With
+    `runner.pack_streams` set the layers run on the valid rows (a call that asks for probabilities runs the dense path);
+    returns None when every token of both streams is padding, where every output and input-gradient row is zero."""
+    B, S0, _ = x0.shape
+    S1 = x1.shape[1]
+    runner.ensure(x0.device)
+    masks = (E.additive_mask_2d(mask0, B, S0), E.additive_mask_2d(mask1, B, S1))
+    if runner.pack_streams and not want_attn:
+        plan = plan_two_stream(*masks, B, S0, S1, x0.device)
+        if plan == "empty":
+            return None
+        if plan is not None:
+            masks = plan
+    return _TwoStreamEncoderFn.apply(runner, masks, training, want_blocks, want_attn, x0, x1, *runner.pack.params)
+
+
 def split_encoder_outputs(outs, n_layers, output_hidden_states, output_attentions):
     """(last, hidden states or None, attentions or None) of run_bert_encoder's outputs; the hidden states in the reference's
     layout: the L layer inputs, then the last output"""
@@ -481,136 +596,6 @@ def vilbert_schedule(v_ids, t_ids, n_t, n_v):
     return steps
 
 
-class VilbertRunner:
-    def __init__(self, layer, v_layer, c_layer, v_ids, t_ids):
-        self.layer, self.v_layer, self.c_layer = list(layer), list(v_layer), list(c_layer)
-        self.steps = vilbert_schedule(list(v_ids), list(t_ids), len(self.layer), len(self.v_layer))
-        self.pack = None
-        self.grad_ready_hook = None
-        # skip padded tokens in both streams: pack each stream's valid rows once per encoder call and run variable-length
-        # self- and cross-attention (plan_two_stream)
-        self.pack_streams = False
-
-    def ensure(self, device):
-        if self.pack is not None and self.pack.intact() and self.pack.device == device:
-            return
-        params = []
-        # parameter order = execution order, so that gradient buckets complete in reverse order
-        for kind, i in self.steps:
-            m = {"t": self.layer, "v": self.v_layer, "c": self.c_layer}[kind][i]
-            params += (E.ConnectionW if kind == "c" else E.BertLayerW).params(m)
-        for p in params:
-            _require_cuda(p, "encoder parameter")
-        self.pack = E.ParamPack(params, device)
-        self.w = {}
-        for kind, i in self.steps:
-            m = {"t": self.layer, "v": self.v_layer, "c": self.c_layer}[kind][i]
-            self.w[(kind, i)] = (E.ConnectionW if kind == "c" else E.BertLayerW)(self.pack, m)
-
-    @staticmethod
-    def _p(mod):
-        d = getattr(mod, "dropout", None)
-        return float(getattr(d, "p", 0.0)) if d is not None else 0.0
-
-    def forward(self, txt, img, tmask, imask, B, T, R, training, need_grad, block_states=None, probs=None):
-        """probs: an engine.ProbsSink that receives the attention probabilities in schedule order - one per text or image
-        layer, two (attn1, attn2) per co-attention block - or None"""
-        ds = _fresh_dropout_state() if training else None
-        saved = []
-        extra = {} if probs is None else {"probs": probs}
-        for kind, i in self.steps:
-            w = self.w[(kind, i)]
-            if kind == "t":
-                m = self.layer[i]
-                pa, ph = (self._p(m.attention.self), self._p(m.attention.output)) if training else (0.0, 0.0)
-                txt, s = E.bert_layer_fwd(txt, tmask, w, B, T, pa, ph, ds, **extra)
-            elif kind == "v":
-                m = self.v_layer[i]
-                pa, ph = (self._p(m.attention.self), self._p(m.attention.output)) if training else (0.0, 0.0)
-                img, s = E.bert_layer_fwd(img, imask, w, B, R, pa, ph, ds, **extra)
-            else:
-                m = self.c_layer[i]
-                if training:
-                    pva, pta = float(m.biattention.dropout1.p), float(m.biattention.dropout2.p)
-                    pvh, pth = float(m.biOutput.dropout1.p), float(m.biOutput.dropout2.p)
-                else:
-                    pva = pta = pvh = pth = 0.0
-                img, txt, s = E.connection_fwd(img, txt, imask, tmask, w, B, R, T, pva, pta, pvh, pth, ds, **extra)
-                if block_states is not None:
-                    block_states.append((txt, img))      # the states the reference appends per co-attention block
-            saved.append(s if need_grad else None)
-        return txt, img, saved
-
-    def backward(self, dtxt, dimg, saved, tmask, imask, B, T, R):
-        for j in range(len(self.steps) - 1, -1, -1):
-            kind, i = self.steps[j]
-            w = self.w[(kind, i)]
-            if kind == "t":
-                dtxt = E.bert_layer_bwd(dtxt, saved[j], tmask, w, B, T)
-            elif kind == "v":
-                dimg = E.bert_layer_bwd(dimg, saved[j], imask, w, B, R)
-            else:
-                dimg, dtxt = E.connection_bwd(dimg, dtxt, saved[j], imask, tmask, w, B, R, T)
-            saved[j] = None
-            if self.grad_ready_hook is not None:
-                E.join_side()
-                self.grad_ready_hook(j)
-        return dtxt, dimg
-
-
-class _VilbertEncoderFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, runner, tmask, imask, training, want_blocks, want_attn, txt, img, *params):
-        B, T, Ht = txt.shape
-        _, R, Hv = img.shape
-        need_grad = any(ctx.needs_input_grad)
-        runner.pack.refresh()
-        t = txt.detach().to(torch.bfloat16).contiguous().view(B * T, Ht)
-        v = img.detach().to(torch.bfloat16).contiguous().view(B * R, Hv)
-        blocks = [] if want_blocks else None
-        probs = _probs_sink(txt.dtype, img.dtype) if want_attn else None
-        if isinstance(tmask, _Packing):             # both streams run on their valid rows only
-            t, v, saved = runner.forward(tmask.pack(t), imask.pack(v), tmask.varlen, imask.varlen, B, T, R, training,
-                                         need_grad, blocks)
-            t, v = tmask.unpack(t, B * T), imask.unpack(v, B * R)
-            blocks = [(tmask.unpack(bt, B * T), imask.unpack(bv, B * R)) for bt, bv in blocks] if want_blocks else blocks
-        else:
-            t, v, saved = runner.forward(t, v, tmask, imask, B, T, R, training, need_grad, blocks, probs=probs)
-        ctx.runner, ctx.saved, ctx.masks, ctx.dims, ctx.dtypes = runner, saved, (tmask, imask), (B, T, R, Ht, Hv), (txt.dtype, img.dtype)
-        outs = [t.view(B, T, Ht).to(txt.dtype), v.view(B, R, Hv).to(img.dtype)]
-        if want_blocks:
-            for bt, bv in blocks:
-                outs += [bt.view(B, T, Ht).to(txt.dtype), bv.view(B, R, Hv).to(img.dtype)]
-        if want_attn:
-            # schedule order; text-query probabilities in the text dtype, image-query ones in the image dtype
-            it = iter(probs)
-            for kind, _ in runner.steps:
-                for q_stream in {"t": "t", "v": "v", "c": "tv"}[kind]:
-                    outs.append(next(it).to(txt.dtype if q_stream == "t" else img.dtype))
-        if len(outs) > 2:
-            ctx.mark_non_differentiable(*outs[2:])
-        return tuple(outs)
-
-    @staticmethod
-    def backward(ctx, dtxt, dimg, *unused):
-        runner = ctx.runner
-        B, T, R, Ht, Hv = ctx.dims
-        if ctx.saved is None:
-            raise RuntimeError("B200 ViLBERT encoder: backward called twice")
-        aliased = runner.pack.prepare_grads()
-        dt = (dtxt if dtxt is not None else torch.zeros(B, T, Ht, device=runner.pack.device)).to(torch.bfloat16).contiguous().view(B * T, Ht)
-        dv = (dimg if dimg is not None else torch.zeros(B, R, Hv, device=runner.pack.device)).to(torch.bfloat16).contiguous().view(B * R, Hv)
-        tm, im = ctx.masks
-        if isinstance(tm, _Packing):
-            dt, dv = runner.backward(tm.pack(dt), im.pack(dv), ctx.saved, tm.varlen, im.varlen, B, T, R)
-            dt, dv = tm.unpack(dt, B * T), im.unpack(dv, B * R)
-        else:
-            dt, dv = runner.backward(dt, dv, ctx.saved, tm, im, B, T, R)
-        ctx.saved = None
-        return (None, None, None, None, None, None, dt.view(B, T, Ht).to(ctx.dtypes[0]),
-                dv.view(B, R, Hv).to(ctx.dtypes[1])) + tuple(runner.pack.autograd_grads(aliased))
-
-
 class B200ViLBertEncoder(nn.Module):
     """vilbert.BertEncoder (vilbert.py:559-796) on the B200 engine.  `config` carries the reference's ViLBERT keys
     (mmf/configs/models/vilbert/defaults.yaml).  dynamic_attention, in_batch_pairs, fast_mode and fixed_*_layer > 0
@@ -638,7 +623,10 @@ class B200ViLBertEncoder(nn.Module):
             for _ in range(config.v_num_hidden_layers)])
         self.c_layer = nn.ModuleList([B200ConnectionLayer(config) for _ in range(len(self.v_biattention_id))])
         _init_bert_weights(self, float(getattr(config, "initializer_range", 0.02)))
-        self._runner = VilbertRunner(self.layer, self.v_layer, self.c_layer, self.v_biattention_id, self.t_biattention_id)
+        kinds = {"t": (self.layer, E.BertLayerW, (0,)), "v": (self.v_layer, E.BertLayerW, (1,)),
+                 "c": (self.c_layer, E.ConnectionW, (1, 0))}
+        self._runner = TwoStreamRunner([(kinds[k][0][i],) + kinds[k][1:] for k, i in vilbert_schedule(
+            self.v_biattention_id, self.t_biattention_id, len(self.layer), len(self.v_layer))])
         self._runner.pack_streams = bool(getattr(config, "skip_padding", False))
 
     def forward(self, txt_embedding, image_embedding, txt_attention_mask, txt_attention_mask2, image_attention_mask,
@@ -658,41 +646,24 @@ class B200ViLBertEncoder(nn.Module):
         the dense path even with skip_padding set.  Without `visualization` the lists are empty, as in the reference, and
         nothing extra runs."""
         _require_cuda(txt_embedding, "txt_embedding")
-        B, T, _ = txt_embedding.shape
-        R = image_embedding.shape[1]
-        self._runner.ensure(txt_embedding.device)
-        tmask = E.additive_mask_2d(txt_attention_mask, B, T)
-        imask = E.additive_mask_2d(image_attention_mask, B, R)
         want_attn = bool(output_all_attention_masks) and bool(getattr(self.config, "visualization", False))
-        if want_attn:
-            outs = _VilbertEncoderFn.apply(self._runner, tmask, imask, self.training, bool(output_all_encoded_layers), True,
-                                           txt_embedding, image_embedding, *self._runner.pack.params)
-            nb = 2 * len(self.c_layer) if output_all_encoded_layers else 0
-            blocks, attn = outs[2:2 + nb], iter(outs[2 + nb:])
-            att_t, att_v, att_c = [], [], []
-            for kind, _ in self._runner.steps:
-                if kind == "t":
-                    att_t.append(next(attn))
-                elif kind == "v":
-                    att_v.append(next(attn))
-                else:
-                    att_c.append((next(attn), next(attn)))
+        outs = run_two_stream_encoder(self._runner, txt_embedding, image_embedding, txt_attention_mask, image_attention_mask,
+                                      self.training, bool(output_all_encoded_layers), want_attn)
+        if outs is None:
+            # every token of both streams is padding: every output (and input-gradient) row is zero
+            zt, zi = txt_embedding * 0, image_embedding * 0
             if output_all_encoded_layers:
-                return list(blocks[0::2]), list(blocks[1::2]), (att_t, att_v, att_c)
-            return [outs[0]], [outs[1]], (att_t, att_v, att_c)
-        if self._runner.pack_streams:
-            plan = plan_two_stream(tmask, imask, B, T, R, txt_embedding.device)
-            if plan == "empty":
-                # every token of both streams is padding: every output (and input-gradient) row is zero
-                zt, zi = txt_embedding * 0, image_embedding * 0
-                if output_all_encoded_layers:
-                    n = len(self.c_layer)
-                    return [zt.detach()] * n, [zi.detach()] * n, ([], [], [])
-                return [zt], [zi], ([], [], [])
-            if plan is not None:
-                tmask, imask = plan
-        outs = _VilbertEncoderFn.apply(self._runner, tmask, imask, self.training, bool(output_all_encoded_layers), False,
-                                       txt_embedding, image_embedding, *self._runner.pack.params)
+                n = len(self.c_layer)
+                return [zt.detach()] * n, [zi.detach()] * n, ([], [], [])
+            return [zt], [zi], ([], [], [])
+        nb = 2 * len(self.c_layer) if output_all_encoded_layers else 0
+        blocks, attn = outs[2:2 + nb], iter(outs[2 + nb:])
+        att_t, att_v, att_c = [], [], []
+        for _, _, streams in self._runner.steps if want_attn else ():
+            if len(streams) == 2:
+                att_c.append((next(attn), next(attn)))
+            else:
+                (att_v if streams == (1,) else att_t).append(next(attn))
         if output_all_encoded_layers:
-            return list(outs[2::2]), list(outs[3::2]), ([], [], [])
-        return [outs[0]], [outs[1]], ([], [], [])
+            return list(blocks[0::2]), list(blocks[1::2]), (att_t, att_v, att_c)
+        return [outs[0]], [outs[1]], (att_t, att_v, att_c)

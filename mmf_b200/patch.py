@@ -11,8 +11,7 @@ With `two_stream=True` it also packs both streams of the ViLBERT and LXMERT enco
 """
 import types
 
-from .lxmert import LxmertRunner
-from .modules import EncoderRunner, VilbertRunner, encoder_result, run_bert_encoder
+from .modules import EncoderRunner, TwoStreamRunner, encoder_result, run_bert_encoder
 
 _saved = {}
 
@@ -102,7 +101,7 @@ def set_skip_padding(module, enabled=True, two_stream=False):
         if type(r) is EncoderRunner:
             r.skip_padding = bool(enabled)
             n += 1
-        elif two_stream and isinstance(r, (VilbertRunner, LxmertRunner)):
+        elif two_stream and isinstance(r, TwoStreamRunner):
             r.pack_streams = bool(enabled)
             n += 1
     return n

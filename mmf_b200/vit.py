@@ -51,12 +51,8 @@ class B200ViTLayer(_Holder):
 
 
 class ViTRunner(EncoderRunner):
+    """its own type: mmf_b200.patch.set_skip_padding never packs a ViT stack"""
     W = E.ViTLayerW
-    _fwd = staticmethod(E.vit_layer_fwd)
-    _bwd = staticmethod(E.vit_layer_bwd)
-
-    def _probs(self, m):
-        return float(m.attention.attention.dropout.p), float(m.attention.output.dropout.p)
 
 
 class B200ViTEncoder(nn.Module):
