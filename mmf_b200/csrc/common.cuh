@@ -108,6 +108,26 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uin
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// TMA stores: shared -> global, tracked per thread in bulk async-groups.  The smem source must be made visible to the
+// async proxy first (fence_proxy_async by every writing thread, then a barrier); elements outside the tensor map are
+// not written.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed store groups may still be reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// every store group of this thread has completed its global writes
+__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// named barrier over `count` threads (a multiple of 32); id 0 is __syncthreads'
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
 // --------------------------------------------------------------------------------------
 // wgmma (warpgroup MMA, sm_90a): D[64 x N] (+)= A[64 x 16] * B[16 x N]^T, bf16 operands from shared memory,

@@ -2,13 +2,16 @@
 //
 //   C[M,N] = epilogue( A[M,K] * B[N,K]^T )       bf16 operands, fp32 accumulation in registers
 //
-// One CTA per (128 x BN output tile, K split), 384 threads = three warpgroups:
+// Persistent: min(work units, SMs) CTAs, a work unit being one (128 x BN output tile, K split) pair; CTA b runs units
+// b, b + gridDim.x, ...  384 threads = three warpgroups:
 //   warpgroup 0    : TMA producer (one thread) - fills a STAGES-deep smem ring of 128x64 A tiles and BNx64 B tiles
-//                    (SWIZZLE_128B), signalling `full[s]` with complete_tx bytes
+//                    (SWIZZLE_128B), signalling `full[s]` with complete_tx bytes; it runs ahead into the next unit
+//                    while the consumers run the current unit's epilogue
 //   warpgroups 1,2 : consumers - each owns 64 rows of the tile and issues wgmma m64nBNk16 straight from the smem
 //                    ring (one k-block in flight while the previous one retires and its slot is released through
-//                    `empty[s]`), then runs the fused elementwise epilogue from its accumulator registers and writes
-//                    bf16 pairs (or fp32 vector reductions for the split-K weight-gradient GEMM) to global memory.
+//                    `empty[s]`), then runs the fused elementwise epilogue from its accumulator registers into smem
+//                    staging boxes that one thread writes out with TMA bulk tensor stores (or fp32 vector reductions
+//                    for the split-K weight-gradient GEMM).
 //
 // Operand layouts: each of A and B may be K-major (row-major [rows, K]) or MN-major (row-major
 // [K, rows]); the latter is what the backward pass needs (dgrad reads W[out,in] as B[N=in,K=out],
@@ -20,6 +23,7 @@
 // mmf/models/vilbert.py:77-79,127,144-145,396-412,504-509 and their autograd backward
 // (mmf/trainers/core/training_loop.py:211-213).
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "mmfb_internal.h"
@@ -52,7 +56,15 @@ struct Cfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
+  // epilogue staging, separate from the ring: per consumer warpgroup STG_BOXES buffers of one 64 x 64 bf16 TMA store
+  // box (8 KB, SWIZZLE_128B), used round-robin
+  static constexpr int BOX_BYTES = 64 * 64 * 2;
+  static constexpr int STG_BOXES = 2;
+  static constexpr int STG_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFFSET = STG_OFFSET + 2 * STG_BOXES * BOX_BYTES;
+  static constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;
+  static_assert(STG_BOXES >= 2, "the store of one box must be able to overlap the writes of the next");
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget of one CTA per SM");
 };
 
 template <int BN, int TA, int TB>
@@ -61,14 +73,31 @@ __device__ __forceinline__ void wgmma_tile(float (&acc)[BN / 2], uint64_t da, ui
   else wgmma_n128<TA, TB>(acc, da, db, accumulate);
 }
 
+// Work unit u = (tile, split), in (m, n, split) order: the CTAs running at one time share A row-blocks in L2.
+struct Unit {
+  int m0, n0, kb0, kb1;
+};
+template <int BN>
+__device__ __forceinline__ Unit decode_unit(int u, const GemmDev& p, int tiles_n, int kb_total, int kb_per_split) {
+  const int split = u % p.splits;
+  const int t = u / p.splits;
+  Unit w;
+  w.m0 = (t / tiles_n) * BM;
+  w.n0 = (t % tiles_n) * BN;
+  w.kb0 = split * kb_per_split;
+  w.kb1 = min(kb_total, w.kb0 + kb_per_split);
+  return w;
+}
+
 template <int BN, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmDev p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2, GemmDev p) {
   using C = Cfg<BN>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * C::STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);
   uint64_t* full = bars;                  // [STAGES]
   uint64_t* empty = bars + STAGES;        // [STAGES]
 
@@ -77,15 +106,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int tiles_n = (p.N + BN - 1) / BN;
   const int kb_total = (p.K + BK - 1) / BK;
   const int kb_per_split = (kb_total + p.splits - 1) / p.splits;
-  const int split = blockIdx.x % p.splits;
-  const int t = blockIdx.x / p.splits;
-  const int m0 = (t / tiles_n) * BM, n0 = (t % tiles_n) * BN;
-  const int kb0 = split * kb_per_split;
-  const int kb1 = min(kb_total, kb0 + kb_per_split);
+  const int units = ((p.M + BM - 1) / BM) * tiles_n * p.splits;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (EPI != EPI_ATOMIC_F32) tma_prefetch_desc(&tmC);
+    if (EPI == EPI_BIAS_GELU) tma_prefetch_desc(&tmC2);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 256);          // every consumer thread releases the slot after its wgmma retired
@@ -95,29 +122,35 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   __syncthreads();
   griddep_wait();        // operands / aux / bias of this GEMM may come from the kernel that is still finishing
 
+  // The ring position (slot s, phase ph) runs on over all k-blocks of all units of this CTA, in the same order in the
+  // producer and in both consumers, and is never reset between units: the producer fills the next unit's first slots
+  // while the consumers run the current unit's epilogue.
   if (wg == 0) {
     // ------------------------------ TMA producer ------------------------------
     if (threadIdx.x == 0) {
       int s = 0;
       uint32_t ph = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* sa = smem + s * C::STAGE_BYTES;
-        uint8_t* sb = sa + C::A_BYTES;
-        mbar_expect_tx(&full[s], C::STAGE_BYTES);
-        if (!A_MN) {
-          tma_load_2d(sa, &tmA, &full[s], kb * BK, m0);
-        } else {
+      for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        const Unit w = decode_unit<BN>(u, p, tiles_n, kb_total, kb_per_split);
+        for (int kb = w.kb0; kb < w.kb1; ++kb) {
+          mbar_wait(&empty[s], ph ^ 1);
+          uint8_t* sa = smem + s * C::STAGE_BYTES;
+          uint8_t* sb = sa + C::A_BYTES;
+          mbar_expect_tx(&full[s], C::STAGE_BYTES);
+          if (!A_MN) {
+            tma_load_2d(sa, &tmA, &full[s], kb * BK, w.m0);
+          } else {
 #pragma unroll
-          for (int pnl = 0; pnl < BM / 64; ++pnl) tma_load_2d(sa + pnl * 8192, &tmA, &full[s], m0 + pnl * 64, kb * BK);
-        }
-        if (!B_MN) {
-          tma_load_2d(sb, &tmB, &full[s], kb * BK, n0);
-        } else {
+            for (int pnl = 0; pnl < BM / 64; ++pnl) tma_load_2d(sa + pnl * 8192, &tmA, &full[s], w.m0 + pnl * 64, kb * BK);
+          }
+          if (!B_MN) {
+            tma_load_2d(sb, &tmB, &full[s], kb * BK, w.n0);
+          } else {
 #pragma unroll
-          for (int pnl = 0; pnl < BN / 64; ++pnl) tma_load_2d(sb + pnl * 8192, &tmB, &full[s], n0 + pnl * 64, kb * BK);
+            for (int pnl = 0; pnl < BN / 64; ++pnl) tma_load_2d(sb + pnl * 8192, &tmB, &full[s], w.n0 + pnl * 64, kb * BK);
+          }
+          if (++s == STAGES) { s = 0; ph ^= 1; }
         }
-        if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
     return;
@@ -125,82 +158,147 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
   // ------------------------------ consumers ------------------------------
   const int half = wg - 1;                       // rows [64 half, 64 half + 64) of the tile
-  float acc[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
-  {
-    int s = 0, prev = -1;
-    uint32_t ph = 0;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      mbar_wait(&full[s], ph);
-      const uint32_t sa = smem_u32(smem + s * C::STAGE_BYTES) + half * 8192;   // K-major: 64 rows x 128 B; MN-major: panel
-      const uint32_t sb = smem_u32(smem + s * C::STAGE_BYTES) + C::A_BYTES;
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < BK / 16; ++kk) {
-        const uint64_t da = A_MN ? gmma_desc_sw128(sa + kk * 2048, 8192, 1024) : gmma_desc_sw128(sa + kk * 32, 16, 1024);
-        const uint64_t db = B_MN ? gmma_desc_sw128(sb + kk * 2048, 8192, 1024) : gmma_desc_sw128(sb + kk * 32, 16, 1024);
-        wgmma_tile<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (kb > kb0 || kk > 0) ? 1u : 0u);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                   // the previous k-block's wgmmas have retired: its slot may be refilled
-      if (prev >= 0) mbar_arrive(&empty[prev]);
-      prev = s;
-      if (++s == STAGES) { s = 0; ph ^= 1; }
-    }
-    wgmma_wait<0>();
-  }
-
-  // ------------------------------ epilogue (registers -> global) ------------------------------
   const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const bool issuer = (threadIdx.x & 127) == 0;  // issues this warpgroup's TMA stores
+  uint8_t* stg = smem + C::STG_OFFSET + half * C::STG_BOXES * C::BOX_BYTES;
+  int s = 0;
+  uint32_t ph = 0;
+  uint32_t box = 0;                              // staging boxes this warpgroup has stored so far (all units)
+  for (int u = blockIdx.x; u < units; u += gridDim.x) {
+    const Unit w = decode_unit<BN>(u, p, tiles_n, kb_total, kb_per_split);
+    float acc[BN / 2];
 #pragma unroll
-  for (int rh = 0; rh < 2; ++rh) {
-    const int m = m0 + half * 64 + warp * 16 + (lane >> 2) + rh * 8;
-    if (m >= p.M) continue;
-    const uint32_t* mrow = (EPI == EPI_BIAS_DROP_RESID && p.dmask != nullptr) ? p.dmask + static_cast<int64_t>(m) * p.ldmask
-                                                                               : nullptr;
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+    {
+      int prev = -1;
+      for (int kb = w.kb0; kb < w.kb1; ++kb) {
+        mbar_wait(&full[s], ph);
+        const uint32_t sa = smem_u32(smem + s * C::STAGE_BYTES) + half * 8192;   // K-major: 64 rows x 128 B; MN-major: panel
+        const uint32_t sb = smem_u32(smem + s * C::STAGE_BYTES) + C::A_BYTES;
+        wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int n = n0 + j * 8 + (lane & 3) * 2;
-      if (n >= p.N) continue;                    // N % 8 == 0: n < N implies n + 1 < N
-      float v0 = acc[j * 4 + rh * 2], v1 = acc[j * 4 + rh * 2 + 1];
-      if (EPI == EPI_ATOMIC_F32) {
-        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p.c32 + static_cast<int64_t>(m) * p.ldc + n), "f"(v0),
-                     "f"(v1)
-                     : "memory");
-        continue;
+        for (int kk = 0; kk < BK / 16; ++kk) {
+          const uint64_t da = A_MN ? gmma_desc_sw128(sa + kk * 2048, 8192, 1024) : gmma_desc_sw128(sa + kk * 32, 16, 1024);
+          const uint64_t db = B_MN ? gmma_desc_sw128(sb + kk * 2048, 8192, 1024) : gmma_desc_sw128(sb + kk * 32, 16, 1024);
+          wgmma_tile<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (kb > w.kb0 || kk > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                   // the previous k-block's wgmmas have retired: its slot may be refilled
+        if (prev >= 0) mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
       }
-      if (EPI == EPI_BIAS || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_DROP_RESID || EPI == EPI_BIAS_RELU) {
-        if (p.bias != nullptr) {
-          const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
-          v0 += b.x;
-          v1 += b.y;
+      wgmma_wait<0>();
+      mbar_arrive(&empty[prev]);           // every unit owns at least one k-block
+    }
+
+    if (EPI == EPI_ATOMIC_F32) {
+      // ---------------------------- split-K epilogue: fp32 vector reductions ----------------------------
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        const int m = w.m0 + half * 64 + warp * 16 + (lane >> 2) + rh * 8;
+        if (m >= p.M) continue;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int n = w.n0 + j * 8 + (lane & 3) * 2;
+          if (n >= p.N) continue;                // N % 8 == 0: n < N implies n + 1 < N
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p.c32 + static_cast<int64_t>(m) * p.ldc + n),
+                       "f"(acc[j * 4 + rh * 2]), "f"(acc[j * 4 + rh * 2 + 1])
+                       : "memory");
         }
       }
-      if (EPI == EPI_BIAS_RELU) {
-        v0 = fmaxf(v0, 0.0f);
-        v1 = fmaxf(v1, 0.0f);
+      continue;
+    }
+
+    // ------------------ epilogue: registers -> smem staging -> TMA bulk tensor stores ------------------
+    // One 64-column chunk of this warpgroup's 64 rows at a time (one box per output).  Rows past M and columns past N
+    // are computed without reading aux / mask / bias and clipped by the store's tensor map.
+    // Box i goes to buffer i % STG_BOXES, which box i - STG_BOXES used last: before the barrier of box i - 1 the issuer
+    // waited until that store had read its source out.  C's box of a chunk is written as it is computed; C2's values
+    // (EPI_BIAS_GELU) wait in registers until C's box has been handed to the TMA unit.
+    const auto store_box = [&](const CUtensorMap* tm, uint8_t* bx, int c0, int c1) {
+      fence_proxy_async();
+      if (issuer) tma_store_wait_read<C::STG_BOXES - 2>();   // frees the buffer of the box after this one
+      named_bar_sync(1 + half, 128);
+      if (issuer) {
+        tma_store_2d(tm, bx, c0, c1);
+        tma_store_commit();
       }
-      if (EPI == EPI_BIAS_DROP_RESID && mrow != nullptr) {
-        const uint32_t bits = __ldg(mrow + (n >> 5)) >> (n & 31);
-        v0 = (bits & 1u) ? v0 * p.dscale : 0.0f;
-        v1 = (bits & 2u) ? v1 * p.dscale : 0.0f;
-      }
-      if ((EPI == EPI_BIAS_DROP_RESID || EPI == EPI_GELU_BWD || EPI == EPI_ADD_AUX) && p.aux != nullptr) {
-        const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.aux + static_cast<int64_t>(m) * p.ldaux + n)));
-        if (EPI == EPI_GELU_BWD) {
-          v0 *= gelu_erf_grad(x.x);
-          v1 *= gelu_erf_grad(x.y);
-        } else {
-          v0 += x.x;
-          v1 += x.y;
+      ++box;
+    };
+    // SWIZZLE_128B: 16-byte chunk jj of row r sits at chunk jj ^ (r % 8); the 32 lanes of a warp hit 32 banks
+    const uint32_t st_row0 = (warp * 16 + (lane >> 2)) * 128 + (lane & 3) * 4;
+    // Epilogues that read aux / mask store with a plain C++ store, which the compiler may move below the loads of later
+    // pairs so that their latencies overlap.  EPI_BIAS_GELU reads no per-element operand; there the ordered asm store
+    // keeps the compiler from holding many u and gelu(u) values at once (it would spill).
+    const auto st_pair = [&](uint8_t* bx, int rh, int jj, uint32_t v) {
+      uint8_t* dst = bx + st_row0 + rh * 8 * 128 + ((jj ^ (lane >> 2)) << 4);
+      if (EPI == EPI_BIAS_GELU) asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(dst)), "r"(v) : "memory");
+      else *reinterpret_cast<uint32_t*>(dst) = v;
+    };
+#pragma unroll
+    for (int cb = 0; cb < BN / 64; ++cb) {
+      if (w.n0 + cb * 64 >= p.N || w.m0 + half * 64 >= p.M) continue;   // the whole box is clipped (warpgroup-uniform)
+      uint8_t* bx = stg + (box % C::STG_BOXES) * C::BOX_BYTES;
+      uint32_t h[2][8];                          // gelu(u) of EPI_BIAS_GELU
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        const int m = w.m0 + half * 64 + warp * 16 + (lane >> 2) + rh * 8;
+        const bool row_in = m < p.M;
+        const uint32_t* mrow = (EPI == EPI_BIAS_DROP_RESID && p.dmask != nullptr && row_in)
+                                   ? p.dmask + static_cast<int64_t>(m) * p.ldmask
+                                   : nullptr;
+        const bf16* arow = (EPI == EPI_BIAS_DROP_RESID || EPI == EPI_GELU_BWD || EPI == EPI_ADD_AUX) && p.aux != nullptr &&
+                                   row_in
+                               ? p.aux + static_cast<int64_t>(m) * p.ldaux
+                               : nullptr;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int j = cb * 8 + jj;
+          const int n = w.n0 + j * 8 + (lane & 3) * 2;
+          float v0 = acc[j * 4 + rh * 2], v1 = acc[j * 4 + rh * 2 + 1];
+          if (EPI == EPI_BIAS || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_DROP_RESID || EPI == EPI_BIAS_RELU) {
+            if (p.bias != nullptr && n < p.N) {
+              const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
+              v0 += b.x;
+              v1 += b.y;
+            }
+          }
+          if (EPI == EPI_BIAS_RELU) {
+            v0 = fmaxf(v0, 0.0f);
+            v1 = fmaxf(v1, 0.0f);
+          }
+          if (EPI == EPI_BIAS_DROP_RESID && mrow != nullptr && n < p.N) {
+            const uint32_t bits = __ldg(mrow + (n >> 5)) >> (n & 31);
+            v0 = (bits & 1u) ? v0 * p.dscale : 0.0f;
+            v1 = (bits & 2u) ? v1 * p.dscale : 0.0f;
+          }
+          if ((EPI == EPI_BIAS_DROP_RESID || EPI == EPI_GELU_BWD || EPI == EPI_ADD_AUX) && arow != nullptr && n < p.N) {
+            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(arow + n)));
+            if (EPI == EPI_GELU_BWD) {
+              v0 *= gelu_erf_grad(x.x);
+              v1 *= gelu_erf_grad(x.y);
+            } else {
+              v0 += x.x;
+              v1 += x.y;
+            }
+          }
+          st_pair(bx, rh, jj, pack_bf16x2(v0, v1));
+          if (EPI == EPI_BIAS_GELU) h[rh][jj] = pack_bf16x2(gelu_erf(v0), gelu_erf(v1));
         }
       }
-      const int64_t off = static_cast<int64_t>(m) * p.ldc + n;
-      *reinterpret_cast<uint32_t*>(p.c + off) = pack_bf16x2(v0, v1);
-      if (EPI == EPI_BIAS_GELU) *reinterpret_cast<uint32_t*>(p.c2 + off) = pack_bf16x2(gelu_erf(v0), gelu_erf(v1));
+      store_box(&tmC, bx, w.n0 + cb * 64, w.m0 + half * 64);
+      if (EPI == EPI_BIAS_GELU) {
+        bx = stg + (box % C::STG_BOXES) * C::BOX_BYTES;
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh)
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) st_pair(bx, rh, jj, h[rh][jj]);
+        store_box(&tmC2, bx, w.n0 + cb * 64, w.m0 + half * 64);
+      }
     }
   }
+  if (EPI != EPI_ATOMIC_F32 && issuer) tma_store_wait_all();   // the staging smem must outlive the reads of the stores
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -224,6 +322,13 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
         reinterpret_cast<uintptr_t>(a.aux)) & 3) ||
       (a.aux != nullptr && (a.ldaux % 2)))
     return set_error(MMFB_ERR_ARG, "gemm: C / C2 / bias / aux must be 4-byte aligned");
+  // bf16 outputs are written by TMA stores of 64 x 64 boxes: tensor [M, N] with row pitch ldc (C and C2 need 16-byte
+  // alignment, which make_tmap_2d checks); columns past N and rows past M are not written
+  CUtensorMap tmC, tmC2;
+  memset(&tmC, 0, sizeof(tmC));
+  memset(&tmC2, 0, sizeof(tmC2));
+  if (EPI != EPI_ATOMIC_F32 && (rc = make_tmap_2d(&tmC, a.C, a.N, a.M, a.ldc, 64, 64))) return rc;
+  if (EPI == EPI_BIAS_GELU && (rc = make_tmap_2d(&tmC2, a.C2, a.N, a.M, a.ldc, 64, 64))) return rc;
   GemmDev p;
   p.M = a.M; p.N = a.N; p.K = a.K;
   p.splits = (EPI == EPI_ATOMIC_F32 && a.splits > 0) ? a.splits : 1;
@@ -249,8 +354,9 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
     if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "cudaFuncSetAttribute(gemm): %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  const int tiles = ((a.M + BM - 1) / BM) * ((a.N + BN - 1) / BN) * p.splits;
-  MMFB_LAUNCH(kern, tiles, NUM_THREADS, C::SMEM_BYTES, stream, tmA, tmB, p);
+  // persistent: at most one CTA per SM, each striding over the (tile, split) work units
+  const int units = ((a.M + BM - 1) / BM) * ((a.N + BN - 1) / BN) * p.splits;
+  MMFB_LAUNCH(kern, units < num_sms() ? units : num_sms(), NUM_THREADS, C::SMEM_BYTES, stream, tmA, tmB, tmC, tmC2, p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "gemm launch: %s", cudaGetErrorString(e));
   count_launch();
