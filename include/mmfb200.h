@@ -57,7 +57,8 @@ typedef struct {
   void* C; int64_t ldc;          /* bf16 [M,N]; fp32 [M,N] for MMFB_EPI_ATOMIC_F32 */
   void* C2;                      /* second bf16 output (MMFB_EPI_BIAS_GELU), same ldc */
   const void* bias;              /* bf16 [N] or NULL */
-  const void* aux; int64_t ldaux;/* bf16 [M,N] residual / pre-activation or NULL */
+  const void* aux; int64_t ldaux;/* bf16 [M,N] residual / pre-activation or NULL; the epilogues that read it (2, 3, 4)
+                                  * load it by TMA: 16-byte aligned, ldaux % 8 == 0, else MMFB_ERR_ARG */
   const uint32_t* drop_mask; int64_t ldmask; float drop_scale; /* keep-bits [M, ldmask] words or NULL */
   int M, N, K;
   int epi;

@@ -11,7 +11,8 @@
 //                    ring (one k-block in flight while the previous one retires and its slot is released through
 //                    `empty[s]`), then runs the fused elementwise epilogue from its accumulator registers into smem
 //                    staging boxes that one thread writes out with TMA bulk tensor stores (or fp32 vector reductions
-//                    for the split-K weight-gradient GEMM).
+//                    for the split-K weight-gradient GEMM).  That thread also fills the boxes with the epilogue's aux
+//                    operand by TMA loads, issued while the unit's wgmmas run.
 //
 // Operand layouts: each of A and B may be K-major (row-major [rows, K]) or MN-major (row-major
 // [K, rows]); the latter is what the backward pass needs (dgrad reads W[out,in] as B[N=in,K=out],
@@ -42,12 +43,16 @@ struct GemmDev {
   float* c32;            // EPI_ATOMIC_F32 destination
   int64_t ldc;
   const bf16* bias;      // [N] or null
-  const bf16* aux;       // residual / pre-activation, [M, ldaux]
-  int64_t ldaux;
+  const bf16* aux;       // residual / pre-activation, [M, ldaux], or null; read through the aux tensor map
   const uint32_t* dmask; // dropout keep-bits, [M, ldmask] words (bit n%32 of word n/32), or null
   int64_t ldmask;
   float dscale;          // 1/(1-p)
 };
+
+// epilogues that read a per-element bf16 operand (aux): it is loaded by TMA into the output staging boxes
+__host__ __device__ constexpr bool epi_reads_aux(int epi) {
+  return epi == EPI_BIAS_DROP_RESID || epi == EPI_GELU_BWD || epi == EPI_ADD_AUX;
+}
 
 template <int BN>
 struct Cfg {
@@ -57,13 +62,15 @@ struct Cfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   // epilogue staging, separate from the ring: per consumer warpgroup STG_BOXES buffers of one 64 x 64 bf16 TMA store
-  // box (8 KB, SWIZZLE_128B), used round-robin
+  // box (8 KB, SWIZZLE_128B), used round-robin.  Two boxes (not four on a 3-stage ring) measured faster for the aux
+  // epilogues too, where they hold the aux boxes of the first two chunks, loaded during the K loop.
   static constexpr int BOX_BYTES = 64 * 64 * 2;
   static constexpr int STG_BOXES = 2;
   static constexpr int STG_OFFSET = STAGES * STAGE_BYTES;
   static constexpr int BAR_OFFSET = STG_OFFSET + 2 * STG_BOXES * BOX_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 256 + 1024;
   static_assert(STG_BOXES >= 2, "the store of one box must be able to overlap the writes of the next");
+  static_assert((2 * STAGES + 2 * STG_BOXES) * 8 <= 256, "ring and aux mbarriers fit the barrier area");
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget of one CTA per SM");
 };
 
@@ -92,7 +99,8 @@ __device__ __forceinline__ Unit decode_unit(int u, const GemmDev& p, int tiles_n
 template <int BN, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2, GemmDev p) {
+            const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
+            const __grid_constant__ CUtensorMap tmX, GemmDev p) {
   using C = Cfg<BN>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -100,6 +108,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::BAR_OFFSET);
   uint64_t* full = bars;                  // [STAGES]
   uint64_t* empty = bars + STAGES;        // [STAGES]
+  uint64_t* auxb = bars + 2 * STAGES;     // [2][STG_BOXES]: aux box loaded into staging buffer b of a warpgroup
+  const bool has_aux = epi_reads_aux(EPI) && p.aux != nullptr;
 
   griddep_launch();
   const int wg = threadIdx.x >> 7;
@@ -113,10 +123,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     tma_prefetch_desc(&tmB);
     if (EPI != EPI_ATOMIC_F32) tma_prefetch_desc(&tmC);
     if (EPI == EPI_BIAS_GELU) tma_prefetch_desc(&tmC2);
+    if (has_aux) tma_prefetch_desc(&tmX);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 256);          // every consumer thread releases the slot after its wgmma retired
     }
+    if (epi_reads_aux(EPI))
+      for (int b = 0; b < 2 * C::STG_BOXES; ++b) mbar_init(&auxb[b], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -166,6 +179,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   uint32_t box = 0;                              // staging boxes this warpgroup has stored so far (all units)
   for (int u = blockIdx.x; u < units; u += gridDim.x) {
     const Unit w = decode_unit<BN>(u, p, tiles_n, kb_total, kb_per_split);
+    // 64-column chunks of this warpgroup's rows that are not wholly clipped: a prefix of the unit's chunks
+    const int nch = w.m0 + half * 64 < p.M ? min(BN / 64, (p.N - w.n0 + 63) / 64) : 0;
+    // TMA load of chunk cb's aux box into the staging buffer of box `bi`, where the chunk's results will be written:
+    // each thread finds its aux pair at the swizzled address it stores the result to.  Rows past M and columns past N
+    // are zero-filled and their results clipped by the store.
+    const auto load_aux = [&](int cb, uint32_t bi) {
+      const uint32_t b = half * C::STG_BOXES + bi % C::STG_BOXES;
+      mbar_expect_tx(&auxb[b], C::BOX_BYTES);
+      tma_load_2d(stg + (bi % C::STG_BOXES) * C::BOX_BYTES, &tmX, &auxb[b], w.n0 + cb * 64, w.m0 + half * 64);
+    };
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
@@ -183,6 +206,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           wgmma_tile<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, (kb > w.kb0 || kk > 0) ? 1u : 0u);
         }
         wgmma_commit();
+        if (has_aux && issuer && kb == w.kb0) {
+          // while the first k-block's wgmmas run: once the previous unit's stores have read their boxes out, prefetch
+          // the aux boxes of this unit's first STG_BOXES chunks, hidden behind the rest of the K loop
+          tma_store_wait_read<0>();
+          for (int cb = 0; cb < min(nch, C::STG_BOXES); ++cb) load_aux(cb, box + cb);
+        }
         wgmma_wait<1>();                   // the previous k-block's wgmmas have retired: its slot may be refilled
         if (prev >= 0) mbar_arrive(&empty[prev]);
         prev = s;
@@ -212,7 +241,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
     // ------------------ epilogue: registers -> smem staging -> TMA bulk tensor stores ------------------
     // One 64-column chunk of this warpgroup's 64 rows at a time (one box per output).  Rows past M and columns past N
-    // are computed without reading aux / mask / bias and clipped by the store's tensor map.
+    // are computed without reading mask / bias (aux reads there find TMA's zero fill) and clipped by the store's tensor
+    // map.  With aux, each box's buffer already holds the chunk's aux box, which the results overwrite in place.
     // Box i goes to buffer i % STG_BOXES, which box i - STG_BOXES used last: before the barrier of box i - 1 the issuer
     // waited until that store had read its source out.  C's box of a chunk is written as it is computed; C2's values
     // (EPI_BIAS_GELU) wait in registers until C's box has been handed to the TMA unit.
@@ -231,15 +261,28 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     // Epilogues that read aux / mask store with a plain C++ store, which the compiler may move below the loads of later
     // pairs so that their latencies overlap.  EPI_BIAS_GELU reads no per-element operand; there the ordered asm store
     // keeps the compiler from holding many u and gelu(u) values at once (it would spill).
+    const auto pair_at = [&](uint8_t* bx, int rh, int jj) {
+      return reinterpret_cast<uint32_t*>(bx + st_row0 + rh * 8 * 128 + ((jj ^ (lane >> 2)) << 4));
+    };
     const auto st_pair = [&](uint8_t* bx, int rh, int jj, uint32_t v) {
-      uint8_t* dst = bx + st_row0 + rh * 8 * 128 + ((jj ^ (lane >> 2)) << 4);
+      uint32_t* dst = pair_at(bx, rh, jj);
       if (EPI == EPI_BIAS_GELU) asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(dst)), "r"(v) : "memory");
-      else *reinterpret_cast<uint32_t*>(dst) = v;
+      else *dst = v;
     };
 #pragma unroll
     for (int cb = 0; cb < BN / 64; ++cb) {
-      if (w.n0 + cb * 64 >= p.N || w.m0 + half * 64 >= p.M) continue;   // the whole box is clipped (warpgroup-uniform)
+      if (cb >= nch) continue;                   // the whole box is clipped (warpgroup-uniform)
       uint8_t* bx = stg + (box % C::STG_BOXES) * C::BOX_BYTES;
+      if constexpr (C::STG_BOXES < BN / 64) {
+        // chunks past the prefetched ones: chunk cb + STG_BOXES - 1 takes the buffer of chunk cb - 1, whose store the
+        // issuer waits to have read out; its aux load then runs while this chunk is computed
+        if (has_aux && issuer && cb >= 1 && cb + C::STG_BOXES - 1 < nch) {
+          tma_store_wait_read<0>();
+          load_aux(cb + C::STG_BOXES - 1, box + C::STG_BOXES - 1);
+        }
+      }
+      // every box of a kernel with aux has had exactly one aux load: box / STG_BOXES loads used this buffer before
+      if (has_aux) mbar_wait(&auxb[half * C::STG_BOXES + box % C::STG_BOXES], (box / C::STG_BOXES) & 1);
       uint32_t h[2][8];                          // gelu(u) of EPI_BIAS_GELU
 #pragma unroll
       for (int rh = 0; rh < 2; ++rh) {
@@ -248,10 +291,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const uint32_t* mrow = (EPI == EPI_BIAS_DROP_RESID && p.dmask != nullptr && row_in)
                                    ? p.dmask + static_cast<int64_t>(m) * p.ldmask
                                    : nullptr;
-        const bf16* arow = (EPI == EPI_BIAS_DROP_RESID || EPI == EPI_GELU_BWD || EPI == EPI_ADD_AUX) && p.aux != nullptr &&
-                                   row_in
-                               ? p.aux + static_cast<int64_t>(m) * p.ldaux
-                               : nullptr;
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int j = cb * 8 + jj;
@@ -273,8 +312,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             v0 = (bits & 1u) ? v0 * p.dscale : 0.0f;
             v1 = (bits & 2u) ? v1 * p.dscale : 0.0f;
           }
-          if ((EPI == EPI_BIAS_DROP_RESID || EPI == EPI_GELU_BWD || EPI == EPI_ADD_AUX) && arow != nullptr && n < p.N) {
-            const float2 x = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(arow + n)));
+          if (has_aux) {
+            const float2 x = unpack_bf16x2(*pair_at(bx, rh, jj));
             if (EPI == EPI_GELU_BWD) {
               v0 *= gelu_erf_grad(x.x);
               v1 *= gelu_erf_grad(x.y);
@@ -307,6 +346,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 template <int BN, bool A_MN, bool B_MN, int EPI>
 static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
   using C = Cfg<BN>;
+  constexpr bool AUX = epi_reads_aux(EPI);
   CUtensorMap tmA, tmB;
   // operand maps: K-major -> tensor [rows, K] (inner = K), box {64, rows_per_tile}
   //               MN-major -> tensor [K, rows] (inner = rows), box {64, 64}
@@ -322,13 +362,19 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
         reinterpret_cast<uintptr_t>(a.aux)) & 3) ||
       (a.aux != nullptr && (a.ldaux % 2)))
     return set_error(MMFB_ERR_ARG, "gemm: C / C2 / bias / aux must be 4-byte aligned");
+  // the epilogues that read aux load it by TMA in 64 x 64 boxes, like C's stores
+  if (AUX && a.aux != nullptr && ((reinterpret_cast<uintptr_t>(a.aux) & 15) || (a.ldaux % 8)))
+    return set_error(MMFB_ERR_ARG, "gemm: aux must be 16-byte aligned with ldaux a multiple of 8 (aux=%p ldaux=%lld)",
+                     a.aux, (long long)a.ldaux);
   // bf16 outputs are written by TMA stores of 64 x 64 boxes: tensor [M, N] with row pitch ldc (C and C2 need 16-byte
   // alignment, which make_tmap_2d checks); columns past N and rows past M are not written
-  CUtensorMap tmC, tmC2;
+  CUtensorMap tmC, tmC2, tmX;
   memset(&tmC, 0, sizeof(tmC));
   memset(&tmC2, 0, sizeof(tmC2));
+  memset(&tmX, 0, sizeof(tmX));
   if (EPI != EPI_ATOMIC_F32 && (rc = make_tmap_2d(&tmC, a.C, a.N, a.M, a.ldc, 64, 64))) return rc;
   if (EPI == EPI_BIAS_GELU && (rc = make_tmap_2d(&tmC2, a.C2, a.N, a.M, a.ldc, 64, 64))) return rc;
+  if (AUX && a.aux != nullptr && (rc = make_tmap_2d(&tmX, a.aux, a.N, a.M, a.ldaux, 64, 64))) return rc;
   GemmDev p;
   p.M = a.M; p.N = a.N; p.K = a.K;
   p.splits = (EPI == EPI_ATOMIC_F32 && a.splits > 0) ? a.splits : 1;
@@ -342,7 +388,6 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
   p.ldc = a.ldc;
   p.bias = reinterpret_cast<const bf16*>(a.bias);
   p.aux = reinterpret_cast<const bf16*>(a.aux);
-  p.ldaux = a.ldaux;
   p.dmask = a.drop_mask;
   p.ldmask = a.ldmask;
   p.dscale = a.drop_scale;
@@ -356,7 +401,8 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
   }
   // persistent: at most one CTA per SM, each striding over the (tile, split) work units
   const int units = ((a.M + BM - 1) / BM) * ((a.N + BN - 1) / BN) * p.splits;
-  MMFB_LAUNCH(kern, units < num_sms() ? units : num_sms(), NUM_THREADS, C::SMEM_BYTES, stream, tmA, tmB, tmC, tmC2, p);
+  MMFB_LAUNCH(kern, units < num_sms() ? units : num_sms(), NUM_THREADS, C::SMEM_BYTES, stream, tmA, tmB, tmC, tmC2, tmX,
+              p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "gemm launch: %s", cudaGetErrorString(e));
   count_launch();
