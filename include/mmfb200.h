@@ -282,6 +282,44 @@ typedef struct {
 } mmfb_adamw_args;
 int mmfb_adamw(const mmfb_adamw_args* args, mmfb_stream stream);
 
+/* Optimal-transport distance of word-region alignment (UNITER's WRA loss): cosine cost, the IPOT transport plan and
+ * trace(C T) in ONE kernel, one CTA per sample; the gradient through the cosine cost in a second one.  Replaces
+ * optimal_transport_dist (mmf/modules/ot.py:80-102: cost_matrix_cosine :15-25, ipot :37-77, trace :28-34) as called by
+ * the WRA head (mmf/models/transformers/heads/wra.py:64-76) and follows it operation for operation in fp32:
+ *   C[m,n] = 1 - x^[m] . y^[n],  x^ = x / max(|x|, 1e-5);  0 where m >= x_len or n >= y_len
+ *   sigma = 1 / x_len (0 on padding), T = 1, A = exp(-C^T / beta) (both 0 on padded pairs)
+ *   iterations x { Q = A * T;  k x { delta = 1 / (y_len * Q sigma + 1e4 * y_pad);  sigma = 1 / (x_len * delta Q + 1e4 * x_pad) };
+ *                  T = delta * Q * sigma };   T = 0 on padded pairs;   dist = sum_{m,n} C[m,n] T[n,m]
+ * (k > 1 raises a shape error in the reference unless M = 1; the inner pass above is its evident intent.)
+ * x: bf16 text rows, sample b row m at x + b * bsx + m * ldx (elements); y: bf16 region rows likewise - both may be views
+ * into one [B, M + N, H] encoder output.  x_len / y_len: int32 [B] in HOST memory (they are validated and travel to the
+ * kernel as launch parameters): the valid rows of a sample are its first x_len / y_len rows; rows past them are not read.
+ * fwd writes dist fp32 [B], plan fp32 [B, N, M] (exact zeros on padded pairs), optionally cost fp32 [B, M, N], and
+ * saved fp32 [B, 2 * (M + N)] for the backward (the clamped row norms and each row's x^ . dx^ term).
+ * bwd: the reference detaches the plan (ot.py:98-101), so d dist / d C = T^T.  Given g = d loss / d dist fp32 [B] and
+ * plan / saved of the forward it writes dx, dy (bf16, addressed like x and y; all M / N rows, exact zeros at padded rows):
+ *   dx[m] = (d - x^[m] (x^[m] . d)) / |x_m|,  d = -g * sum_n T[n,m] y^[n]   (no projection term where |x_m| was clamped).
+ * Limits (MMFB_ERR_ARG otherwise): 1 <= M, N <= 128; H a multiple of 64 up to 1024; 1 <= x_len <= M, 1 <= y_len <= N;
+ * beta > 0, iterations >= 1, k >= 1; x, y, dx, dy 16-byte aligned with row and sample pitches that are multiples of 8.
+ * One launch per 256 samples. */
+typedef struct {
+  const void* x; int64_t ldx; int64_t bsx;
+  const void* y; int64_t ldy; int64_t bsy;
+  const int32_t* x_len; const int32_t* y_len;   /* HOST int32 [B] */
+  float* dist;                                  /* fp32 [B] (fwd) */
+  float* plan;                                  /* fp32 [B, N, M]: written by fwd, read by bwd */
+  float* cost;                                  /* fp32 [B, M, N] or NULL (fwd) */
+  float* saved;                                 /* fp32 [B, 2 * (M + N)]: written by fwd, read by bwd */
+  /* backward only */
+  const float* g;                               /* fp32 [B] */
+  void* dx; int64_t lddx; int64_t bsdx;
+  void* dy; int64_t lddy; int64_t bsdy;
+  int B, M, N, H;
+  float beta; int iterations; int k;            /* fwd; the reference's defaults are 0.5, 50, 1 */
+} mmfb_ot_args;
+int mmfb_ot_fwd(const mmfb_ot_args* args, mmfb_stream stream);
+int mmfb_ot_bwd(const mmfb_ot_args* args, mmfb_stream stream);
+
 /* library / diagnostics */
 const char* mmfb_last_error(void);
 int mmfb_version(void);

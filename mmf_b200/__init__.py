@@ -35,6 +35,7 @@ _LAZY = {
     "ViLBERT": ("models", "ViLBERT"),
     "MMBT": ("models", "MMBT"),
     "MMFTransformer": ("mmft", "MMFTransformer"),
+    "UNITER": ("uniter_model", "UNITER"),
     "build_model": ("models", "build_model"),
     "load_model_config": ("models", "load_model_config"),
     "GraphedStep": ("graphs", "GraphedStep"),

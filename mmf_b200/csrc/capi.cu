@@ -247,5 +247,15 @@ int mmfb_cast_f32_bf16(const float* in, void* out, int64_t n, mmfb_stream stream
   MMFB_REQUIRE_DEVICE();
   return cast_params(in, out, n, reinterpret_cast<cudaStream_t>(stream));
 }
+int mmfb_ot_fwd(const mmfb_ot_args* args, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_ot_fwd: null args");
+  MMFB_REQUIRE_DEVICE();
+  return ot_fwd(*args, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_ot_bwd(const mmfb_ot_args* args, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_ot_bwd: null args");
+  MMFB_REQUIRE_DEVICE();
+  return ot_bwd(*args, reinterpret_cast<cudaStream_t>(stream));
+}
 
 }  // extern "C"

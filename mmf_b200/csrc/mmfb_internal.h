@@ -76,5 +76,7 @@ int dropout_apply(const void* x, int64_t ldx, const uint32_t* bits, int64_t ldm,
 int gelu_bwd(const void* dh, const void* u, void* du, int64_t n, cudaStream_t s);
 int scatter_sorted(const void* dy, int64_t lddy, const int32_t* order, const int32_t* sorted_idx, float* dtab, int M,
                    int H, cudaStream_t s);
+int ot_fwd(const mmfb_ot_args& a, cudaStream_t s);
+int ot_bwd(const mmfb_ot_args& a, cudaStream_t s);
 
 }  // namespace mmfb

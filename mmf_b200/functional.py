@@ -9,7 +9,7 @@ import ctypes
 import torch
 
 from . import lib
-from .lib import LIB, AdamWArgs, AttnArgs, ComposeArgs, GemmArgs, LnArgs, ScatterArgs, _ptr, _stream_ptr, check
+from .lib import LIB, AdamWArgs, AttnArgs, ComposeArgs, GemmArgs, LnArgs, OtArgs, ScatterArgs, _ptr, _stream_ptr, check
 
 
 def _req(t, dtype, name):
@@ -628,3 +628,56 @@ def unpack_keep_bits(words, n):
     w = words.to(torch.int64) & 0xFFFFFFFF
     bits = (w.unsqueeze(-1) >> torch.arange(32, device=words.device, dtype=torch.int64)) & 1
     return bits.reshape(*words.shape[:-1], -1)[..., :n].bool()
+
+
+def _ot_args(x, y, x_len, y_len):
+    """x [B, M, H], y [B, N, H]: bf16 views with a contiguous last dimension (e.g. two row ranges of one encoder output);
+    x_len / y_len: one int per sample, on the host (the library validates them and passes them as launch parameters)"""
+    _req(x, torch.bfloat16, "x"); _req(y, torch.bfloat16, "y")
+    if x.dim() != 3 or y.dim() != 3 or x.shape[0] != y.shape[0] or x.shape[2] != y.shape[2]:
+        raise ValueError("optimal transport: x [B, M, H] and y [B, N, H] required, got %s and %s" % (tuple(x.shape), tuple(y.shape)))
+    B = x.shape[0]
+    lens = []
+    for t, name in ((x_len, "x_len"), (y_len, "y_len")):
+        t = torch.as_tensor(t).reshape(-1).to(device="cpu", dtype=torch.int32).contiguous()
+        if t.numel() != B:
+            raise ValueError("optimal transport: %s must hold one length per sample (%d), got %d" % (name, B, t.numel()))
+        lens.append(t)
+    a = OtArgs()
+    a.x, a.ldx, a.bsx = x.data_ptr(), x.stride(1), x.stride(0)
+    a.y, a.ldy, a.bsy = y.data_ptr(), y.stride(1), y.stride(0)
+    a.x_len, a.y_len = lens[0].data_ptr(), lens[1].data_ptr()
+    a.B, a.M, a.N, a.H = B, x.shape[1], y.shape[1], x.shape[2]
+    return a, lens
+
+
+def ot_fwd(x, y, x_len, y_len, beta=0.5, iterations=50, k=1, want_cost=False):
+    """dist [B], plan T [B, N, M], saved [B, 2 (M + N)] (, cost [B, M, N]) of mmfb_ot_fwd: cosine cost + IPOT + trace(C T),
+    one CTA per sample (mmf/modules/ot.py:80-102)."""
+    a, lens = _ot_args(x, y, x_len, y_len)
+    B, M, N = a.B, a.M, a.N
+    dist = torch.empty(B, dtype=torch.float32, device=x.device)
+    plan = torch.empty(B, N, M, dtype=torch.float32, device=x.device)
+    saved = torch.empty(B, 2 * (M + N), dtype=torch.float32, device=x.device)
+    cost = torch.empty(B, M, N, dtype=torch.float32, device=x.device) if want_cost else None
+    a.dist, a.plan, a.saved, a.cost = dist.data_ptr(), plan.data_ptr(), saved.data_ptr(), _ptr(cost)
+    a.beta, a.iterations, a.k = float(beta), int(iterations), int(k)
+    check(LIB.mmfb_ot_fwd(ctypes.byref(a), _stream_ptr()))
+    return (dist, plan, saved, cost) if want_cost else (dist, plan, saved)
+
+
+def ot_bwd(g, plan, saved, x, y, x_len, y_len, dx, dy):
+    """dx, dy (bf16 views addressed like x, y; every row is written, padded rows with zeros) from g = d loss / d dist [B]"""
+    a, lens = _ot_args(x, y, x_len, y_len)
+    _req(g, torch.float32, "g"); _req(plan, torch.float32, "plan"); _req(saved, torch.float32, "saved")
+    _req(dx, torch.bfloat16, "dx"); _req(dy, torch.bfloat16, "dy")
+    if dx.shape != x.shape or dy.shape != y.shape:
+        raise ValueError("optimal transport: dx / dy must have the shapes of x / y")
+    if not (g.is_contiguous() and plan.is_contiguous() and saved.is_contiguous()) or g.numel() != a.B or \
+            tuple(plan.shape) != (a.B, a.N, a.M) or tuple(saved.shape) != (a.B, 2 * (a.M + a.N)):
+        raise ValueError("optimal transport: g [B], plan [B, N, M] and saved [B, 2 (M + N)] must be the forward's, contiguous")
+    a.g, a.plan, a.saved = g.data_ptr(), plan.data_ptr(), saved.data_ptr()
+    a.dx, a.lddx, a.bsdx = dx.data_ptr(), dx.stride(1), dx.stride(0)
+    a.dy, a.lddy, a.bsdy = dy.data_ptr(), dy.stride(1), dy.stride(0)
+    check(LIB.mmfb_ot_bwd(ctypes.byref(a), _stream_ptr()))
+    return dx, dy

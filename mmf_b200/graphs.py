@@ -48,6 +48,10 @@ class GraphedStep:
             raise RuntimeError("GraphedStep: the model has two-stream encoders with pack_streams set, which read the token "
                                "counts on the host and cannot be captured; turn them off with "
                                "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)")
+        for m in model.modules():
+            if getattr(m, "graph_capturable", True) is False:
+                raise RuntimeError("GraphedStep: %s draws its task and region masks on the host in every forward and gathers "
+                                   "a data-dependent number of rows, so its step cannot be captured" % type(m).__name__)
         self.model, self.loss_fn = model, loss_fn
         self.static = _map(lambda t: t.detach().clone(), example_batch)
         dev = next(t for t in _flatten(self.static) if t.is_cuda).device

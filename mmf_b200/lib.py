@@ -105,6 +105,20 @@ class ScatterArgs(ctypes.Structure):
     ]
 
 
+class OtArgs(ctypes.Structure):
+    _fields_ = [
+        ("x", ctypes.c_void_p), ("ldx", ctypes.c_int64), ("bsx", ctypes.c_int64),
+        ("y", ctypes.c_void_p), ("ldy", ctypes.c_int64), ("bsy", ctypes.c_int64),
+        ("x_len", ctypes.c_void_p), ("y_len", ctypes.c_void_p),
+        ("dist", ctypes.c_void_p), ("plan", ctypes.c_void_p), ("cost", ctypes.c_void_p), ("saved", ctypes.c_void_p),
+        ("g", ctypes.c_void_p),
+        ("dx", ctypes.c_void_p), ("lddx", ctypes.c_int64), ("bsdx", ctypes.c_int64),
+        ("dy", ctypes.c_void_p), ("lddy", ctypes.c_int64), ("bsdy", ctypes.c_int64),
+        ("B", ctypes.c_int), ("M", ctypes.c_int), ("N", ctypes.c_int), ("H", ctypes.c_int),
+        ("beta", ctypes.c_float), ("iterations", ctypes.c_int), ("k", ctypes.c_int),
+    ]
+
+
 def _load():
     if not os.path.exists(_LIB_PATH):
         try:
@@ -139,6 +153,8 @@ def _load():
         getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                        ctypes.c_void_p]
     lib.mmfb_attention_probs.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
+    for name in ("mmfb_ot_fwd", "mmfb_ot_bwd"):
+        getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p]
     return lib
 
 

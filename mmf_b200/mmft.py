@@ -9,6 +9,9 @@
       "mlp"  MLPHead  <-> mmf/models/transformers/heads/mlp.py:19-96    pooler -> [dropout, transform] x n -> Linear
       "mlm"  MLMHead  <-> heads/mlm.py:20-97     labelled positions gathered FIRST, transform -> vocabulary decoder -> CE
       "itm"  ITMHead  <-> heads/itm.py:19-74     pooler -> Linear(H, 2) -> CE
+      "mrc"  MRCHead  <-> heads/mrc.py:15-90     masked regions -> Linear -> GELU -> LayerNorm -> Linear(1601) -> KL / CE
+      "mrfr" MRFRHead <-> heads/mrfr.py:15-93    masked regions -> Linear -> GELU -> LayerNorm -> tied projection -> MSE
+      "wra"  WRAHead  <-> heads/wra.py:13-83     optimal-transport distance of text rows x region rows (one kernel)
 
 The backend is the registered "b200" transformer backend (mmf_b200.mmft_backend); a config that says `backend.type:
 huggingface` (the reference default, configs/models/mmf_transformer/defaults.yaml:4-7) is served by it as well - that is
@@ -156,6 +159,118 @@ class ITMHead(nn.Module):
         score = self.cls.seq_relationship(self.pooler(sequence_output))
         loss = nn.functional.cross_entropy(score.reshape(-1, 2).float(), labels.reshape(-1), ignore_index=c.ignore_index)
         return {"losses": {c.loss_name: loss}}
+
+
+def compute_masked_hidden(hidden, mask):
+    """heads/utils.py:169-179: the rows of hidden [B, S, H] where the bool mask [B, S] is True, as [n, H]"""
+    mask = mask.unsqueeze(-1).expand_as(hidden)
+    return hidden[mask].contiguous().view(-1, hidden.size(-1))
+
+
+def _required(processed_sample_list, key, head):
+    assert key in processed_sample_list and processed_sample_list[key] is not None, (
+        "%s pretraining requires %s to be in sample list with value not None." % (head, key))
+    return processed_sample_list[key]
+
+
+def _linear_gelu_ln(seq, x):
+    """nn.Sequential(Linear, GELU, LayerNorm) of the region heads: GEMM with the GELU epilogue, then the row LayerNorm"""
+    h = ops.linear_gelu(x, seq[0].weight, seq[0].bias)
+    return ops.layer_norm(h, seq[2].weight, seq[2].bias, seq[2].eps)
+
+
+@register_transformer_head("mrc")
+class MRCHead(nn.Module):
+    """Masked region classification (heads/mrc.py:15-90); parameters `region_classifier.{0,2,3}.*`"""
+
+    def __init__(self, hidden_size=768, loss_name="mrc_loss", ignore_index=-1, mrc_label_key="region_class",
+                 mrc_mask_key="image_region_mask", label_dim=1601, eps=1e-12, use_kl=True, *args, **kwargs):
+        super().__init__()
+        self.loss_name, self.ignore_index, self.use_kl = loss_name, ignore_index, use_kl
+        self.mrc_label_key, self.mrc_mask_key = mrc_label_key, mrc_mask_key
+        self.region_classifier = nn.Sequential(nn.Linear(hidden_size, hidden_size), nn.GELU(),
+                                               nn.LayerNorm(hidden_size, eps=eps), nn.Linear(hidden_size, label_dim))
+
+    def forward(self, sequence_output, encoded_layers=None, processed_sample_list=None):
+        region_labels = _required(processed_sample_list, self.mrc_label_key, "MRC")
+        masks = _required(processed_sample_list, self.mrc_mask_key, "MRC")
+        h = _linear_gelu_ln(self.region_classifier, compute_masked_hidden(sequence_output, masks))
+        last = self.region_classifier[3]
+        logits = ops.linear_any(h, last.weight, last.bias).float()       # label_dim = 1601 is not a multiple of 8
+        if self.use_kl:
+            loss = nn.functional.kl_div(nn.functional.log_softmax(logits, dim=-1), region_labels.float(),
+                                        reduction="batchmean")
+        else:
+            targets = torch.max(region_labels[:, 1:], dim=-1)[1] + 1      # background class should not be the target
+            loss = nn.functional.cross_entropy(logits, targets, ignore_index=self.ignore_index, reduction="mean")
+        return {"losses": {self.loss_name: loss}}
+
+
+@register_transformer_head("mrfr")
+class MRFRHead(nn.Module):
+    """Masked region feature regression (heads/mrfr.py:15-93).  `linear_proj_weight` IS the image embedding's projection
+    weight [hidden, img_dim] (one Parameter under two names, as in the reference); the projection back to the feature
+    space reads it transposed, in place (ops.linear_t), and autograd adds both uses' gradients."""
+
+    def __init__(self, img_embedding_weight, hidden_size=768, loss_name="mrfr_loss", mrfr_target_key="mrfr_region_target",
+                 mrfr_mask_key="mrfr_region_mask", img_dim=2048, eps=1e-12, *args, **kwargs):
+        super().__init__()
+        self.loss_name, self.mrfr_target_key, self.mrfr_mask_key = loss_name, mrfr_target_key, mrfr_mask_key
+        assert img_embedding_weight is not None and tuple(img_embedding_weight.shape) == (hidden_size, img_dim), (
+            "MRFR head requires 'img_embedding_weight' with shape (%d, %d)." % (hidden_size, img_dim))
+        self.linear_proj_weight = img_embedding_weight
+        self.linear_proj_bias = nn.Parameter(torch.zeros(img_dim))
+        self.feat_regress = nn.Sequential(nn.Linear(hidden_size, hidden_size), nn.GELU(), nn.LayerNorm(hidden_size, eps=eps))
+
+    def forward(self, sequence_output, encoded_layers=None, processed_sample_list=None):
+        feat_targets = _required(processed_sample_list, self.mrfr_target_key, "MRFR")
+        masks = _required(processed_sample_list, self.mrfr_mask_key, "MRFR")
+        h = _linear_gelu_ln(self.feat_regress, compute_masked_hidden(sequence_output, masks))
+        prediction = ops.linear_t(h, self.linear_proj_weight, self.linear_proj_bias)
+        loss = nn.functional.mse_loss(prediction.float(), feat_targets.float(), reduction="mean")
+        return {"losses": {self.loss_name: loss}}
+
+
+@register_transformer_head("wra")
+class WRAHead(nn.Module):
+    """Word-region alignment (heads/wra.py:13-83): the optimal-transport distance between each sample's text rows and
+    region rows - cost, IPOT plan and distance in one kernel (ops.optimal_transport_dist) - positives minus negatives.
+
+    The kernel takes lengths, not masks: `txt_pad` / `img_pad` must mark a suffix of each row as padding, which is what
+    UNITER's `_preprocess_wra` builds (uniter.py:560-583).  `wra_info` may carry the lengths as host lists (`txt_lens`,
+    `img_lens`); otherwise they are read back from the pads, and a pad that is not a suffix raises ValueError."""
+
+    def __init__(self, loss_name="wra_loss", ot_inputs_key="wra_info", wra_label_key="is_correct", *args, **kwargs):
+        super().__init__()
+        self.loss_name, self.ot_inputs_key, self.wra_label_key = loss_name, ot_inputs_key, wra_label_key
+
+    @staticmethod
+    def _lengths(pad, lens, width, what):
+        if lens is not None:
+            return [int(v) for v in lens]
+        pad = pad.bool().cpu()
+        n = (~pad).sum(1)
+        if pad.size(1) != width or not torch.equal(pad, torch.arange(width).unsqueeze(0) >= n.unsqueeze(1)):
+            raise ValueError("WRA: %s must be [B, %d] and mark a suffix of each row as padding" % (what, width))
+        return n.tolist()
+
+    def forward(self, sequence_output, encoded_layers=None, processed_sample_list=None):
+        ot_inputs = _required(processed_sample_list, self.ot_inputs_key, "WRA")
+        assert ot_inputs.get("txt_pad") is not None and ot_inputs.get("img_pad") is not None, (
+            "WRA pretraining requires 'txt_pad', and 'img_pad' to be in 'processed_sample_list[%s]' with values not None."
+            % self.ot_inputs_key)
+        assert processed_sample_list.get(self.wra_label_key) is not None, (
+            "WRA pretraining requires %s to be in sample list with value not None." % self.wra_label_key)
+        tl = processed_sample_list["input_ids"].size(1)
+        il = processed_sample_list["image_feat"].size(1)
+        x_len = self._lengths(ot_inputs["txt_pad"], ot_inputs.get("txt_lens"), tl, "txt_pad")
+        y_len = self._lengths(ot_inputs["img_pad"], ot_inputs.get("img_lens"), il, "img_pad")
+        itm_labels = processed_sample_list[self.wra_label_key]
+        ot_dist = ops.optimal_transport_dist(sequence_output, tl, il, x_len, y_len).to(sequence_output.dtype)
+        ot_pos = ot_dist.masked_select(itm_labels == 1)
+        ot_neg = ot_dist.masked_select(itm_labels == 0)
+        loss = (ot_pos.sum() - ot_neg.sum()) / (ot_pos.size(0) + ot_neg.size(0))
+        return {"losses": {self.loss_name: loss}}
 
 
 # ------------------------------------------------------------------------------------------------------

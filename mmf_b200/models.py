@@ -4,6 +4,7 @@
   registry.register_model("vilbert")      ViLBERT      <->  mmf/models/vilbert.py:1336-1472
   registry.register_model("mmbt")         MMBT         <->  mmf/models/mmbt.py:565-643
   registry.register_model("lxmert")       LXMERT       <->  mmf/models/lxmert.py:647-790
+  registry.register_model("uniter")       UNITER       <->  mmf/models/uniter.py:615-774   (mmf_b200/uniter_model.py)
 
 Each is a `BaseModel` (mmf/models/base_model.py:67-337 contract: ctor(config) -> build() -> forward(SampleList) -> dict
 with "scores" and/or "losses"; `config_path()` names the model's default YAML; `__call__` fills "losses" from the
@@ -1027,3 +1028,6 @@ class LXMERT(BaseModel):
         return self.model(input_ids=p["input_ids"], token_type_ids=p["token_type_ids"],
                           attention_mask=p["attention_mask"], visual_feats=p["visual_feats"], visual_pos=p["pos"],
                           visual_attention_mask=p["image_attention_mask"])
+
+
+from . import uniter_model  # noqa: E402,F401  (registers "uniter"; it needs the names defined above)

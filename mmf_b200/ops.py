@@ -285,3 +285,75 @@ class _LinearCrossEntropy(torch.autograd.Function):
 def linear_cross_entropy(h2d, weight, bias, labels, ignore_index=-1, chunk_rows=2048):
     """mean_i CE((h W^T + b)_i, labels_i) over the rows with labels_i != ignore_index (0 when there is none), fp32 scalar."""
     return _LinearCrossEntropy.apply(h2d, weight, bias, labels, int(ignore_index), int(chunk_rows))
+
+
+class _LinearT(torch.autograd.Function):
+    """y = x W + b with W stored [K, N]: the GEMM reads the weight MN-major (the layout the dgrad calls use), so a weight
+    that is another layer's nn.Linear weight - MRFR's projection back to the feature space, tied to UNITER's img_linear
+    (heads/mrfr.py:48-49, 86-88) - is consumed as it lies and autograd sums both uses' gradients into the one parameter."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        xb, wb, bb = _bf16(x), _bf16(weight), _bf16(bias)
+        y = F.gemm(xb, wb, b_mn=True, epi=lib.EPI_BIAS, bias=bb)
+        ctx.save_for_backward(xb, wb)
+        ctx.dtypes = (x.dtype, weight.dtype, bias.dtype)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xb, wb = ctx.saved_tensors
+        dyb = dy.to(torch.bfloat16).contiguous()
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dx = F.gemm(dyb, wb, epi=lib.EPI_BIAS).to(ctx.dtypes[0])              # dy [M, N] @ W[K, N]^T
+        if ctx.needs_input_grad[1]:
+            dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)       # x^T dy: [K, N]
+            F.gemm(xb, dyb, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
+                   splits=best_splits(wb.shape[0], wb.shape[1], xb.shape[0]))
+            dw = dw.to(ctx.dtypes[1])
+        if ctx.needs_input_grad[2]:
+            db = torch.zeros(wb.shape[1], dtype=torch.float32, device=wb.device)
+            F.colsum(dyb, db)
+            db = db.to(ctx.dtypes[2])
+        return dx, dw, db
+
+
+def linear_t(x2d, weight_kn, bias):
+    """F.linear(x, weight_kn.t(), bias): x2d [M, K], weight_kn [K, N] -> bf16 [M, N]; K and N multiples of 8."""
+    return _LinearT.apply(x2d, weight_kn, bias)
+
+
+class _OptimalTransport(torch.autograd.Function):
+    """dist [B] of mmfb_ot_fwd over two row ranges of one sequence buffer; the backward (mmfb_ot_bwd) writes both ranges of
+    the sequence gradient in place.  The plan is a constant of the backward, as in the reference (ot.py:98-101)."""
+
+    @staticmethod
+    def forward(ctx, seq, T_len, R_len, x_len, y_len, beta, iteration, k):
+        sb = seq.detach()
+        if sb.dtype != torch.bfloat16 or sb.stride(-1) != 1 or sb.stride(0) % 8 or sb.stride(1) % 8:
+            sb = sb.to(torch.bfloat16).contiguous()
+        x, y = sb[:, :T_len], sb[:, T_len:T_len + R_len]
+        dist, plan, saved = F.ot_fwd(x, y, x_len, y_len, beta, iteration, k)
+        ctx.save_for_backward(sb, plan, saved)
+        ctx.meta = (T_len, R_len, x_len, y_len, seq.dtype)
+        return dist
+
+    @staticmethod
+    def backward(ctx, g):
+        sb, plan, saved = ctx.saved_tensors
+        T_len, R_len, x_len, y_len, dtype = ctx.meta
+        full = T_len + R_len == sb.shape[1]
+        dseq = (torch.empty if full else torch.zeros)(sb.shape, dtype=torch.bfloat16, device=sb.device)
+        F.ot_bwd(g.float().contiguous(), plan, saved, sb[:, :T_len], sb[:, T_len:T_len + R_len], x_len, y_len,
+                 dseq[:, :T_len], dseq[:, T_len:T_len + R_len])
+        return (dseq.to(dtype),) + (None,) * 7
+
+
+def optimal_transport_dist(seq, T_len, R_len, x_len, y_len, beta=0.5, iteration=50, k=1):
+    """optimal_transport_dist(seq[:, :T_len].float(), seq[:, T_len:T_len + R_len].float(), txt_pad, img_pad) of
+    mmf/modules/ot.py:80-102 for prefix pads: sample b's valid text rows are its first x_len[b], its valid regions the first
+    y_len[b] (host integers).  seq [B, S >= T_len + R_len, H]; returns fp32 [B].  T_len, R_len <= 128, H % 64 == 0."""
+    x_len = torch.as_tensor(x_len).reshape(-1).to(device="cpu", dtype=torch.int32)
+    y_len = torch.as_tensor(y_len).reshape(-1).to(device="cpu", dtype=torch.int32)
+    return _OptimalTransport.apply(seq, int(T_len), int(R_len), x_len, y_len, float(beta), int(iteration), int(k))

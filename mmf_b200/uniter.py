@@ -58,10 +58,11 @@ class B200UNITERModelBase(nn.Module):
     max_position_embeddings, type_vocab_size, dropouts ...).  Random-init here (the reference pulls bert-base-uncased
     from the hub); weights arrive through load_state_dict."""
 
-    def __init__(self, config, img_dim=2048, hidden_dropout_prob=0.0):
+    def __init__(self, config, img_dim=2048, hidden_dropout_prob=0.0, text_config=None):
         super().__init__()
         self.config = config
-        self.text_embeddings = B200BertTextEmbeddings(config)
+        # the reference builds the text embeddings from a BertConfig of their own (uniter.py:119-125)
+        self.text_embeddings = B200BertTextEmbeddings(config if text_config is None else text_config)
         self.img_embeddings = B200UNITERImageEmbeddings(img_dim=img_dim, hidden_size=config.hidden_size,
                                                         hidden_dropout_prob=hidden_dropout_prob)
         self.encoder = B200BertEncoder(config)
