@@ -5,14 +5,16 @@
 //     probs  = dropout(softmax(scores))   a fully masked row is the softmax of its raw scores, never NaN
 //     ctx    = probs V, heads merged back to [B, Sq, h*d]
 //
-// Every kernel works on 64-row tiles of one (batch, head): four warps, each owning 16 rows of the resident tile, and a
-// loop over 64-row blocks of the other sequence.  TMA stages the head slices straight out of the fused [tokens, 3*H]
-// projection buffers (3-D tensor maps: sequence tails are zero-filled, never read from the next sample) into
-// 128-byte-swizzled shared memory; the looped blocks go through a two-stage ring signalled by mbarriers, so the load of
-// block i+2 overlaps the math of block i+1.  The products run on the tensor cores with mma.sync m16n8k16 (bf16 in,
-// fp32 accumulate): operand fragments come from shared memory through ldmatrix (.trans for the operands that are
-// consumed along their rows), and a probability / gradient tile computed in registers is reused directly as the A
-// operand of the next product - the accumulator layout of two adjacent n8 tiles is the A layout of one k16 step.
+// Every kernel works on 64-row tiles of one (batch, head): one warpgroup of four warps, each owning 16 rows of the
+// resident tile, and a loop over 64-row blocks of the other sequence.  TMA stages the head slices straight out of the
+// fused [tokens, 3*H] projection buffers (3-D tensor maps: sequence tails are zero-filled, never read from the next
+// sample) into 128-byte-swizzled shared memory; the looped blocks go through a two-stage ring signalled by mbarriers, so
+// the load of block i+2 overlaps the math of block i+1.  The products run on the tensor cores with wgmma m64nNk16 (bf16
+// in, fp32 accumulate).  A product of two staged tiles reads both through shared-memory descriptors of the swizzled
+// layout TMA wrote (no ldmatrix, no operand fragments in registers); a probability / gradient tile computed in registers
+// is the A operand of the next product as it stands - the accumulator layout of two adjacent n8 tiles is the A layout
+// of one k16 step - with the staged tile as the MN-major B operand.  Every wgmma group is waited for before its
+// accumulators are read, and the last one of a block before the stage is refilled.
 //
 // Forward: online softmax over the key blocks in the log2 domain (the 1/sqrt(d) scale folded into log2(e)); the row
 // log-sum-exp is saved for the backward.
@@ -43,52 +45,33 @@ constexpr int AT_THREADS = 128;   // four warps x 16 rows
 // unchanged bit for bit.
 __device__ __forceinline__ float staged_mask(float m) { return fmaxf(m, -10000.0f) * LOG2E; }
 
-// byte offset of the 16-byte chunk holding column c (a multiple of 8) of row r in a staged tile: 64-column panels of
-// ROWS x 128 B, SWIZZLE_128B (chunk index XOR row % 8), as written by a TMA box {64, ROWS}
-template <int ROWS>
-__device__ __forceinline__ uint32_t tile_off(int r, int c) {
-  return (c >> 6) * (ROWS * 128) + r * 128 + ((((c >> 3) & 7) ^ (r & 7)) << 4);
-}
-
-// TMA of one [ROWS x D] head slice (D/64 boxes) into `dst`, credited to `bar`
+// TMA of one [ROWS x D] head slice into `dst`, credited to `bar`: D/64 boxes {64, ROWS}, each a 64-column panel of
+// ROWS x 128 B lines, SWIZZLE_128B (16-byte chunk index XOR row % 8) - the layout the wgmma descriptors name
 template <int D, int ROWS>
 __device__ __forceinline__ void load_tile(uint8_t* dst, const CUtensorMap* m, uint64_t* bar, int col0, int row0, int b) {
 #pragma unroll
   for (int c = 0; c < D / 64; ++c) tma_load_3d(dst + c * ROWS * 128, m, bar, col0 + c * 64, row0, b);
 }
 
-// acc[16 x 8 NT] (+)= A[16 rows from r0 of tile a, D] * B[8 NT rows of tile b, D]^T   (both tiles K-major along D)
+// Issues acc[64 x 8 NT] = A[64 rows of tile a, D] * B[8 NT rows of tile b, D]^T, one wgmma per k16 step (both tiles K-major
+// along D: a step is 32 B further along the 128-byte lines, the second 64-column panel follows the first).  The first
+// step overwrites acc.  The caller fences before and commits / waits after.
 template <int D, int NT, int AROWS, int BROWS>
-__device__ __forceinline__ void mma_abt(float (&acc)[NT][4], uint32_t a, int r0, uint32_t b, int lane) {
-  const int mi = lane >> 3, lr = lane & 7;
+__device__ __forceinline__ void wg_abt(float (&acc)[NT][4], uint32_t a, uint32_t b) {
 #pragma unroll
   for (int ks = 0; ks < D / 16; ++ks) {
-    uint32_t af[4];
-    ldsm_x4(af, a + tile_off<AROWS>(r0 + (mi & 1) * 8 + lr, ks * 16 + (mi >> 1) * 8));
-#pragma unroll
-    for (int np = 0; np < NT / 2; ++np) {
-      uint32_t bf[4];
-      ldsm_x4(bf, b + tile_off<BROWS>(np * 16 + (mi >> 1) * 8 + lr, ks * 16 + (mi & 1) * 8));
-      mma_bf16_16816(acc[2 * np], af, bf[0], bf[1]);
-      mma_bf16_16816(acc[2 * np + 1], af, bf[2], bf[3]);
-    }
+    const uint64_t da = gmma_desc_sw128(a + (ks >> 2) * (AROWS * 128) + (ks & 3) * 32, 16, 1024);
+    const uint64_t db = gmma_desc_sw128(b + (ks >> 2) * (BROWS * 128) + (ks & 3) * 32, 16, 1024);
+    wgmma_ss(acc, da, db, ks > 0 ? 1u : 0u);
   }
 }
 
-// acc[16 x D] += P[16 x 16 KS] * B[16 KS rows of tile b, D]   (P: bf16 A fragments in registers, B consumed along rows)
+// Issues acc[64 x D] += P[64 x 16 KS] * B[16 KS rows of tile b, D]   (P: bf16 A fragments in registers; B is read MN-major:
+// its rows are the k dimension, a k16 step is 16 lines = 2048 B, LBO the stride of its 64-column panels)
 template <int D, int KS, int BROWS>
-__device__ __forceinline__ void mma_pb(float (&acc)[D / 8][4], const uint32_t (&pf)[KS][4], uint32_t b, int lane) {
-  const int mi = lane >> 3, lr = lane & 7;
+__device__ __forceinline__ void wg_pb(float (&acc)[D / 8][4], const uint32_t (&pf)[KS][4], uint32_t b) {
 #pragma unroll
-  for (int ks = 0; ks < KS; ++ks) {
-#pragma unroll
-    for (int dp = 0; dp < D / 16; ++dp) {
-      uint32_t bf[4];
-      ldsm_x4_t(bf, b + tile_off<BROWS>(ks * 16 + (mi & 1) * 8 + lr, dp * 16 + (mi >> 1) * 8));
-      mma_bf16_16816(acc[2 * dp], pf[ks], bf[0], bf[1]);
-      mma_bf16_16816(acc[2 * dp + 1], pf[ks], bf[2], bf[3]);
-    }
-  }
+  for (int ks = 0; ks < KS; ++ks) wgmma_rs(acc, pf[ks], gmma_desc_sw128(b + ks * 2048, BROWS * 128, 1024), 1u);
 }
 
 // accumulator tile [16 x 8 NT] (fp32) -> bf16 A fragments of NT/2 k16 steps
@@ -224,9 +207,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     mbar_wait(&bars[1 + st], (kb >> 1) & 1);
     const uint32_t uK = smem_u32(sKV + 2 * st * TB), uV = uK + TB;
     float s[8][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.0f;
-    mma_abt<D, 8, AT_ROWS, AT_ROWS>(s, uQ, r0, uK, lane);
+    wgmma_fence();
+    wg_abt<D, 8, AT_ROWS, AT_ROWS>(s, uQ, uK);
+    wgmma_commit();
+    wgmma_wait<0>();
     // scale + mask, block row max (the four threads of a quad share a row)
     float bmax[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -276,10 +260,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     }
     uint32_t pf[4][4];
     acc_to_a<8>(s, pf);
-    mma_pb<D, 4, AT_ROWS>(o, pf, uV, lane);
-    // every warp is done with this stage: its ldmatrix reads (generic proxy) are ordered before the TMA refill (async
-    // proxy) that thread 0 issues next; a barrier alone does not order the two proxies
-    fence_proxy_async();
+    wgmma_fence();
+    wg_pb<D, 4, AT_ROWS>(o, pf, uV);
+    wgmma_commit();
+    wgmma_wait<0>();
+    // every warp's wgmmas on this stage have retired: thread 0 may refill it (wgmma and TMA are both async-proxy accesses,
+    // so the barrier orders them)
     __syncthreads();
     if (threadIdx.x == 0 && kb + 2 < nkb) {
       mbar_expect_tx(&bars[1 + st], 2 * TB);
@@ -418,13 +404,11 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     mbar_wait(&bars[1 + st], (kb >> 1) & 1);
     const uint32_t uK = smem_u32(sKV + 2 * st * TB), uV = uK + TB;
     float s[8][4], dp[8][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.0f;
-      dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.0f;
-    }
-    mma_abt<D, 8, AT_ROWS, AT_ROWS>(s, uQ, r0, uK, lane);
-    mma_abt<D, 8, AT_ROWS, AT_ROWS>(dp, udO, r0, uV, lane);
+    wgmma_fence();
+    wg_abt<D, 8, AT_ROWS, AT_ROWS>(s, uQ, uK);
+    wg_abt<D, 8, AT_ROWS, AT_ROWS>(dp, udO, uV);
+    wgmma_commit();
+    wgmma_wait<0>();
     uint32_t bits[2][2] = {{0xFFFFFFFFu, 0xFFFFFFFFu}, {0xFFFFFFFFu, 0xFFFFFFFFu}};
     if (DROP) {
 #pragma unroll
@@ -452,8 +436,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     }
     uint32_t sf[4][4];
     acc_to_a<8>(s, sf);
-    mma_pb<D, 4, AT_ROWS>(dq, sf, uK, lane);
-    fence_proxy_async();
+    wgmma_fence();
+    wg_pb<D, 4, AT_ROWS>(dq, sf, uK);
+    wgmma_commit();
+    wgmma_wait<0>();
     __syncthreads();
     if (threadIdx.x == 0 && kb + 2 < nkb) {
       mbar_expect_tx(&bars[1 + st], 2 * TB);
@@ -557,13 +543,11 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     mbar_wait(&bars[1 + st], (qb >> 1) & 1);
     const uint32_t uQ = smem_u32(sQd + 2 * st * QTB), udO = uQ + QTB;
     float s[NT][4], dp[NT][4];
-#pragma unroll
-    for (int i = 0; i < NT; ++i) {
-      s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.0f;
-      dp[i][0] = dp[i][1] = dp[i][2] = dp[i][3] = 0.0f;
-    }
-    mma_abt<D, NT, AT_ROWS, QB>(s, uK, r0, uQ, lane);      // S^T  [keys x queries]
-    mma_abt<D, NT, AT_ROWS, QB>(dp, uV, r0, udO, lane);    // dP^T
+    wgmma_fence();
+    wg_abt<D, NT, AT_ROWS, QB>(s, uK, uQ);                  // S^T  [keys x queries]
+    wg_abt<D, NT, AT_ROWS, QB>(dp, uV, udO);                // dP^T
+    wgmma_commit();
+    wgmma_wait<0>();
     float pd[NT][4];                                        // dropped probabilities P^T * keep * dscale
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
@@ -589,9 +573,11 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     uint32_t pf[NT / 2][4], sf[NT / 2][4];
     acc_to_a<NT>(pd, pf);
     acc_to_a<NT>(s, sf);
-    mma_pb<D, NT / 2, QB>(dv, pf, udO, lane);
-    mma_pb<D, NT / 2, QB>(dk, sf, uQ, lane);
-    fence_proxy_async();
+    wgmma_fence();
+    wg_pb<D, NT / 2, QB>(dv, pf, udO);
+    wg_pb<D, NT / 2, QB>(dk, sf, uQ);
+    wgmma_commit();
+    wgmma_wait<0>();
     __syncthreads();
     if (threadIdx.x == 0 && qb + 2 < nqb) {
       mbar_expect_tx(&bars[1 + st], 2 * QTB);

@@ -4,7 +4,8 @@
 // with S = Q K^T of the call's q / k head slices and lse2 the row statistics its forward saved.  This is the dq kernel's
 // probability recompute (attention.cu) with the store of P in place of the gradient products: the same tiles, the same
 // staged mask (clamped at -10000, keys past Skv at -inf), the same keep bits, so P is the post-dropout probability the
-// reference returns.  It reads Q and K only, and its cost is the HBM write of P.
+// reference returns.  It reads Q and K only, and its cost is the HBM write of P, so its one product stays on mma.sync
+// m16n8k16 with ldmatrix fragments (each warp its own 16 rows).
 //
 // Its own translation unit (it includes attention.cu for the shared helpers and instantiates none of its kernels), so that
 // the existing attention kernels keep their code.
@@ -14,6 +15,31 @@
 namespace mmfb {
 
 constexpr int AP_PITCH = AT_ROWS + 4;   // fp32 pitch of a staged row: 272 B, 16-byte aligned, rows start 4 banks apart
+
+// byte offset of the 16-byte chunk holding column c (a multiple of 8) of row r in a staged tile: 64-column panels of
+// ROWS x 128 B, SWIZZLE_128B (chunk index XOR row % 8), as written by a TMA box {64, ROWS}
+template <int ROWS>
+__device__ __forceinline__ uint32_t tile_off(int r, int c) {
+  return (c >> 6) * (ROWS * 128) + r * 128 + ((((c >> 3) & 7) ^ (r & 7)) << 4);
+}
+
+// acc[16 x 8 NT] (+)= A[16 rows from r0 of tile a, D] * B[8 NT rows of tile b, D]^T   (both tiles K-major along D)
+template <int D, int NT, int AROWS, int BROWS>
+__device__ __forceinline__ void mma_abt(float (&acc)[NT][4], uint32_t a, int r0, uint32_t b, int lane) {
+  const int mi = lane >> 3, lr = lane & 7;
+#pragma unroll
+  for (int ks = 0; ks < D / 16; ++ks) {
+    uint32_t af[4];
+    ldsm_x4(af, a + tile_off<AROWS>(r0 + (mi & 1) * 8 + lr, ks * 16 + (mi >> 1) * 8));
+#pragma unroll
+    for (int np = 0; np < NT / 2; ++np) {
+      uint32_t bf[4];
+      ldsm_x4(bf, b + tile_off<BROWS>(np * 16 + (mi >> 1) * 8 + lr, ks * 16 + (mi & 1) * 8));
+      mma_bf16_16816(acc[2 * np], af, bf[0], bf[1]);
+      mma_bf16_16816(acc[2 * np + 1], af, bf[2], bf[3]);
+    }
+  }
+}
 
 struct AttnProbsDev {
   int B, H, Sq, Skv;

@@ -187,8 +187,53 @@ __device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t da, uint64_
 }
 #undef MMFB_F8
 
+// The attention kernels' shapes.  Their accumulators are d[N/8][4], one row of four per n8 tile: flattened, that is the
+// d[N/2] layout above, and per warp it is the mma.sync m16n8k16 accumulator (rows t/4 and t/4 + 8, columns 2 (t%4) and
+// 2 (t%4) + 1 of every n8 tile).
+// wgmma_ss: both operands K-major in shared memory.
+// wgmma_rs: A from registers - a[4] of thread t of warp w is rows 16 w + t/4 (+ 8 for a[1], a[3]), k columns 2 (t%4),
+//   2 (t%4) + 1 (+ 8 for a[2], a[3]), the m16n8k16 A fragment - and B MN-major in shared memory (transpose bit set).
+#define MMFB_F4(i) "+f"(d[i][0]), "+f"(d[i][1]), "+f"(d[i][2]), "+f"(d[i][3])
+#define MMFB_F16(i) MMFB_F4(i), MMFB_F4(i + 1), MMFB_F4(i + 2), MMFB_F4(i + 3)
+#define MMFB_R10(n) "%" #n "0, %" #n "1, %" #n "2, %" #n "3, %" #n "4, %" #n "5, %" #n "6, %" #n "7, %" #n "8, %" #n "9, "
+__device__ __forceinline__ void wgmma_ss(float (&d)[4][4], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
+      : MMFB_F16(0)
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_ss(float (&d)[8][4], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, " MMFB_R10(1) MMFB_R10(2)
+      "%30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : MMFB_F16(0), MMFB_F16(4)
+      : "l"(da), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_rs(float (&d)[8][4], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, " MMFB_R10(1) MMFB_R10(2)
+      "%30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
+      : MMFB_F16(0), MMFB_F16(4)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+}
+__device__ __forceinline__ void wgmma_rs(float (&d)[16][4], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, " MMFB_R10(1) MMFB_R10(2)
+      MMFB_R10(3) MMFB_R10(4) MMFB_R10(5) "%60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 1;\n\t}\n"
+      : MMFB_F16(0), MMFB_F16(4), MMFB_F16(8), MMFB_F16(12)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
+}
+#undef MMFB_F4
+#undef MMFB_F16
+#undef MMFB_R10
+
 // --------------------------------------------------------------------------------------
-// mma.sync (m16n8k16, bf16 -> fp32) and ldmatrix, for the attention kernels whose operands are register tiles
+// mma.sync (m16n8k16, bf16 -> fp32) and ldmatrix, for the kernels whose operands are small register tiles (the
+// attention-probabilities kernel, optimal transport)
 // --------------------------------------------------------------------------------------
 __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
@@ -199,11 +244,6 @@ __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a
 }
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t saddr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(saddr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t (&r)[4], uint32_t saddr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
                : "r"(saddr));
 }
