@@ -36,6 +36,7 @@ _LAZY = {
     "MMBT": ("models", "MMBT"),
     "MMFTransformer": ("mmft", "MMFTransformer"),
     "UNITER": ("uniter_model", "UNITER"),
+    "VinVL": ("vinvl_model", "VinVL"),
     "build_model": ("models", "build_model"),
     "load_model_config": ("models", "load_model_config"),
     "GraphedStep": ("graphs", "GraphedStep"),

@@ -50,8 +50,8 @@ class GraphedStep:
                                "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)")
         for m in model.modules():
             if getattr(m, "graph_capturable", True) is False:
-                raise RuntimeError("GraphedStep: %s draws its task and region masks on the host in every forward and gathers "
-                                   "a data-dependent number of rows, so its step cannot be captured" % type(m).__name__)
+                reason = getattr(m, "graph_refusal", "does work on the host in every forward")
+                raise RuntimeError("GraphedStep: %s %s, so its step cannot be captured" % (type(m).__name__, reason))
         self.model, self.loss_fn = model, loss_fn
         self.static = _map(lambda t: t.detach().clone(), example_batch)
         dev = next(t for t in _flatten(self.static) if t.is_cuda).device

@@ -12,6 +12,7 @@
       "mrc"  MRCHead  <-> heads/mrc.py:15-90     masked regions -> Linear -> GELU -> LayerNorm -> Linear(1601) -> KL / CE
       "mrfr" MRFRHead <-> heads/mrfr.py:15-93    masked regions -> Linear -> GELU -> LayerNorm -> tied projection -> MSE
       "wra"  WRAHead  <-> heads/wra.py:13-83     optimal-transport distance of text rows x region rows (one kernel)
+      "contrastive_three_way"  ThreeWayContrastiveHead  <-> heads/contrastive.py:14-79   MLPHead(num_labels=3) -> CE
 
 The backend is the registered "b200" transformer backend (mmf_b200.mmft_backend); a config that says `backend.type:
 huggingface` (the reference default, configs/models/mmf_transformer/defaults.yaml:4-7) is served by it as well - that is
@@ -158,6 +159,45 @@ class ITMHead(nn.Module):
             labels = processed_sample_list["itm_labels"][c.itm_label_key]
         score = self.cls.seq_relationship(self.pooler(sequence_output))
         loss = nn.functional.cross_entropy(score.reshape(-1, 2).float(), labels.reshape(-1), ignore_index=c.ignore_index)
+        return {"losses": {c.loss_name: loss}}
+
+
+CONTRASTIVE_LABEL_KEY = "three_way_constrastive_labels"          # the reference's spelling (contrastive.py:11)
+
+
+@register_transformer_head("contrastive_three_way")
+class ThreeWayContrastiveHead(nn.Module):
+    """VinVL's three-way contrastive head (heads/contrastive.py:14-79): an MLPHead built from the head's own merged config
+    (pooler -> Linear(H, 3) with the defaults), cross-entropy over 0 = match, 1 = corrupt caption, 2 = corrupt image.
+    Parameters `contrast_head.pooler.dense.*`, `contrast_head.classifier.0.*`.
+
+    The reference's forward takes (sequence_output, processed_sample_list), which MMFT's three-argument head call
+    (sequence_output, encoded_layers, processed_sample_list) does not fit; here the sample list is the last positional
+    argument (or the keyword), so both call forms work."""
+    DEFAULTS = dict(type="three_way_contrastive", freeze=False, lr_multiplier=1.0, hidden_size=768,
+                    loss_name="three_way_contrastive_loss", ignore_index=-1, constrastive_label_key="contrastive_labels",
+                    num_layers=0, num_labels=3, hidden_dropout_prob=0.1, layer_norm_eps=1e-6, hidden_act="gelu",
+                    pooler_name="bert_pooler", in_dim=None)          # contrastive.py:26-39
+
+    def __init__(self, config):
+        super().__init__()
+        self.config = c = ConfigNode(dict(self.DEFAULTS, **dict(config)))
+        self.contrast_head = MLPHead(c)
+
+    def forward(self, sequence_output, *args, processed_sample_list=None):
+        if processed_sample_list is None and args:
+            processed_sample_list = args[-1]
+        c = self.config
+        if c.constrastive_label_key in processed_sample_list:
+            labels = processed_sample_list[c.constrastive_label_key]
+        else:
+            assert (CONTRASTIVE_LABEL_KEY in processed_sample_list
+                    and processed_sample_list[CONTRASTIVE_LABEL_KEY] is not None), (
+                "Constrastive three way pretraining requires %s to be in sample list with value not None."
+                % CONTRASTIVE_LABEL_KEY)
+            labels = processed_sample_list[CONTRASTIVE_LABEL_KEY][c.constrastive_label_key]
+        scores = self.contrast_head(sequence_output)["scores"]
+        loss = nn.functional.cross_entropy(scores.reshape(-1, 3).float(), labels.reshape(-1), ignore_index=c.ignore_index)
         return {"losses": {c.loss_name: loss}}
 
 

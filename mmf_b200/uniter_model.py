@@ -270,6 +270,8 @@ class UNITER(BaseModel):
     """Modification for Joint Vision-Language Encoding (uniter.py:615-774)"""
 
     graph_capturable = False        # host-side task / mask draws and masked gathers: see mmf_b200.graphs.GraphedStep
+    graph_refusal = ("draws its task and region masks on the host in every forward and gathers a data-dependent number of "
+                     "rows")
 
     def __init__(self, config):
         super().__init__(config)
