@@ -77,7 +77,13 @@ int mmfb_gemm(const mmfb_gemm_args* args, mmfb_stream stream);
  * [B,1,1,Skv] tensor) or NULL; values below -10000 (finfo(dtype).min, -inf) act exactly like -10000, so a fully
  * masked row gives the softmax of its raw scores and stays finite.  lse2 [B, heads, Sq] fp32 receives the log2-domain row log-sum-exp
  * (saved for backward).  drop_mask: keep bits [B, heads, Sq, ceil(Skv/32)] (bit kv%32) or NULL.
- * Limits: head_dim 64 or 128; Skv <= 384 (d=64) / 256 (d=128) - MMF's path has S <= 324. */
+ * Limits: head_dim 64 or 128; Skv <= 384 (d=64) / 256 (d=128) - MMF's path has S <= 324.
+ * causal_len (self-attention only): T > 0 makes the last T keys a causal tail - the prefix-LM mask of M4C's multimodal
+ * transformer (mmf/models/m4c.py:418-437).  With P = Skv - T, key k < P takes mask[b, k] as above (clamp included), and
+ * key k >= P takes 0 when k <= q and -10000 otherwise, in place of mask[b, k], which is not read for those keys.  So the
+ * first P queries never see the tail, and query P + t sees tail keys P .. P + t.  0 (what a zero-initialised struct
+ * holds) means no tail.  Requires Sq == Skv and T <= Skv; a negative T is MMFB_ERR_ARG, and so is any T != 0 in the
+ * packed (varlen) entry points and mmfb_attention_probs.  Every refusal happens before a launch. */
 typedef struct {
   const void* q; int64_t ldq;
   const void* k; int64_t ldk;
@@ -95,6 +101,7 @@ typedef struct {
   void* dk; int64_t ld_dk;
   void* dv; int64_t ld_dv;
   int B, heads, Sq, Skv, head_dim;
+  int causal_len;                    /* keys in the causal tail, 0 = none (see above) */
 } mmfb_attn_args;
 
 int mmfb_attention_fwd(const mmfb_attn_args* args, mmfb_stream stream);

@@ -37,6 +37,8 @@ _LAZY = {
     "MMFTransformer": ("mmft", "MMFTransformer"),
     "UNITER": ("uniter_model", "UNITER"),
     "VinVL": ("vinvl_model", "VinVL"),
+    "M4C": ("m4c_model", "M4C"),
+    "M4CCaptioner": ("m4c_model", "M4CCaptioner"),
     "build_model": ("models", "build_model"),
     "load_model_config": ("models", "load_model_config"),
     "GraphedStep": ("graphs", "GraphedStep"),

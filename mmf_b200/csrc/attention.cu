@@ -27,6 +27,11 @@
 // so a tile may run into the next sample; those rows are masked (keys), not stored (queries) or given P = 0 (dk/dv), and
 // every CTA stays within its own sample's blocks.  Queries and keys each have their own packing (cu / total for the query
 // side, cu_kv / total_kv for the key side); packed self-attention passes the same one twice.
+// CAUSAL instantiations (dense self-attention with causal_len = T > 0, M4C's prefix-LM mask, m4c.py:418-437): keys from
+// P = Skv - T on are a causal tail.  Where a score takes its mask value, a tail key k takes 0 if k <= q and -10000
+// otherwise (the staged mask holds 0 there, mask[b, k] is not read); keys below P keep the additive mask.  No key block is
+// skipped: M4C's tails (12 / 30 keys) sit inside one 64-key block, and every value stays finite, so a query whose other
+// keys are all padding still gets the softmax of its raw scores, as in the reference.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -44,6 +49,12 @@ constexpr int AT_THREADS = 128;   // four warps x 16 rows
 // and stays finite, so such a row keeps a finite log-sum-exp (softmax of its raw scores).  Masks at or above -10000 are
 // unchanged bit for bit.
 __device__ __forceinline__ float staged_mask(float m) { return fmaxf(m, -10000.0f) * LOG2E; }
+
+// CAUSAL: the mask value (log2 domain) of query q and key kv; `staged` is the staged value of kv (0 for tail keys).  Tail
+// keys past the query take -10000, the value staged_mask gives a padded key.
+__device__ __forceinline__ float causal_mask(float staged, int q, int kv, int P, int Skv) {
+  return (kv >= P && kv < Skv && kv > q) ? -10000.0f * LOG2E : staged;
+}
 
 // TMA of one [ROWS x D] head slice into `dst`, credited to `bar`: D/64 boxes {64, ROWS}, each a 64-column panel of
 // ROWS x 128 B lines, SWIZZLE_128B (16-byte chunk index XOR row % 8) - the layout the wgmma descriptors name
@@ -106,6 +117,7 @@ struct AttnFwdDev {
   int total;              // VARLEN: packed query rows
   const int* cu_kv;       // VARLEN: [B+1] first packed key row of every sample (Skv = max_kv; self-attention: cu)
   int total_kv;           // VARLEN: packed key rows
+  int P;                  // CAUSAL: first key of the causal tail (Skv - causal_len)
 };
 
 // VARLEN: sample b owns the packed rows [cu[b], cu[b+1]) of one side's row buffers (clamped to [0, total] and to max_len
@@ -128,7 +140,7 @@ __device__ __forceinline__ int2 varlen_rows(const int* cu, int b, int total, int
 // VARLEN: packed attention (no additive mask); the tensor maps span each side's packed rows with a batch extent of 1, tiles
 // load at row cu[b] + block * 64 (queries) / cu_kv[b] + block * 64 (keys), and rows past the end of the sample (the next
 // sample's rows) are masked / not stored.  A sample without keys writes ctx = ctx_lo = 0 and lse2 = -inf (empty sum).
-template <int D, bool VARLEN>
+template <int D, bool VARLEN, bool CAUSAL>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, AttnFwdDev p) {
@@ -182,6 +194,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   for (int i = threadIdx.x; i < nkb * AT_ROWS; i += AT_THREADS) {
     if constexpr (VARLEN)
       sMask[i] = (i < kvlen) ? 0.0f : -INFINITY;
+    else if constexpr (CAUSAL)
+      sMask[i] = (i < p.Skv) ? (p.mask != nullptr && i < p.P ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f)
+                             : -INFINITY;
     else
       sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
   }
@@ -218,7 +233,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       const float2 mk = *reinterpret_cast<const float2*>(sMask + kb * AT_ROWS + nt * 8 + 2 * t4);
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        s[nt][e] = fmaf(s[nt][e], p.scale2, (e & 1) ? mk.y : mk.x);
+        float m = (e & 1) ? mk.y : mk.x;
+        if constexpr (CAUSAL) m = causal_mask(m, q0 + r0 + g + (e >> 1) * 8, kb * AT_ROWS + nt * 8 + 2 * t4 + (e & 1), p.P, p.Skv);
+        s[nt][e] = fmaf(s[nt][e], p.scale2, m);
         bmax[e >> 1] = fmaxf(bmax[e >> 1], s[nt][e]);
       }
     }
@@ -317,11 +334,12 @@ struct AttnBwdDev {
   int total;
   const int* cu_kv;
   int total_kv;
+  int P;                     // CAUSAL, as in AttnFwdDev
 };
 
-// dQ for 64 query rows.  smem: Q, dO tiles; two stages of (K block, V block).  VARLEN as in the forward (a sample without
-// keys writes dq = 0).
-template <int D, bool DROP, bool VARLEN>
+// dQ for 64 query rows.  smem: Q, dO tiles; two stages of (K block, V block).  VARLEN and CAUSAL as in the forward (a
+// sample without keys writes dq = 0).
+template <int D, bool DROP, bool VARLEN, bool CAUSAL>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
                    const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, AttnBwdDev p) {
@@ -375,6 +393,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   for (int i = threadIdx.x; i < nkb * AT_ROWS; i += AT_THREADS) {
     if constexpr (VARLEN)
       sMask[i] = (i < kvlen) ? 0.0f : -INFINITY;
+    else if constexpr (CAUSAL)
+      sMask[i] = (i < p.Skv) ? (p.mask != nullptr && i < p.P ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f)
+                             : -INFINITY;
     else
       sMask[i] = (i < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + i]) : 0.0f) : -INFINITY;
   }
@@ -425,7 +446,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         const int hr = e >> 1;
-        const float pe = ex2_approx(fmaf(s[nt][e], p.scale2, (e & 1) ? mk.y : mk.x) - lse[hr]);
+        float m = (e & 1) ? mk.y : mk.x;
+        if constexpr (CAUSAL) m = causal_mask(m, q0 + r0 + g + hr * 8, kb * AT_ROWS + nt * 8 + 2 * t4 + (e & 1), p.P, p.Skv);
+        const float pe = ex2_approx(fmaf(s[nt][e], p.scale2, m) - lse[hr]);
         float dpe = dp[nt][e];
         if (DROP) {
           const int col = nt * 8 + 2 * t4 + (e & 1);
@@ -461,8 +484,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 
 // dK, dV for 64 key rows.  smem: K, V tiles; two stages of (Q block, dO block) of QB query rows.  The register tiles are
 // transposed products (rows = keys, columns = queries).  VARLEN as in the forward; query rows past the end of the sample
-// take lse = +inf and delta = 0 (P = 0), like rows past Sq, and a sample without queries writes dk = dv = 0.
-template <int D, bool DROP, int QB, bool VARLEN>
+// take lse = +inf and delta = 0 (P = 0), like rows past Sq, and a sample without queries writes dk = dv = 0.  CAUSAL as in
+// the forward, with the key of a row and the query of a column.
+template <int D, bool DROP, int QB, bool VARLEN, bool CAUSAL>
 __global__ void __launch_bounds__(AT_THREADS)
 attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                     const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO, AttnBwdDev p) {
@@ -518,6 +542,9 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     const int kv = k0 + i;
     if constexpr (VARLEN)
       sMask[i] = (kv < kvlen) ? 0.0f : -INFINITY;
+    else if constexpr (CAUSAL)
+      sMask[i] = (kv < p.Skv) ? (p.mask != nullptr && kv < p.P ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + kv]) : 0.0f)
+                              : -INFINITY;
     else
       sMask[i] = (kv < p.Skv) ? (p.mask != nullptr ? staged_mask(p.mask[static_cast<int64_t>(b) * p.Skv + kv]) : 0.0f) : -INFINITY;
   }
@@ -562,7 +589,9 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           const int e = hr * 2 + j;
-          const float pe = ex2_approx(fmaf(s[nt][e], p.scale2, mk[hr]) - lse);
+          float m = mk[hr];
+          if constexpr (CAUSAL) m = causal_mask(m, q, k0 + r0 + g + hr * 8, p.P, p.Skv);
+          const float pe = ex2_approx(fmaf(s[nt][e], p.scale2, m) - lse);
           const bool keep = !DROP || ((w >> (ksh0 + hr * 8)) & 1u);
           const float dpe = keep ? dp[nt][e] * p.dscale : 0.0f;
           pd[nt][e] = keep ? pe * p.dscale : 0.0f;
@@ -604,7 +633,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 // elements is owned by D/8 consecutive lanes and reduced with shuffles (coalesced 512 B / 1 KB per warp access).
 // Every row is a query row of some sample, so the packed layout [H, total] is this kernel's own with B = 1, Sq = total:
 // the varlen backward launches it unchanged (it is defined once, in the dense translation unit).
-#if defined(MMFB_ATTN_VARLEN_TU) || defined(MMFB_ATTN_PROBS_TU)
+#if defined(MMFB_ATTN_VARLEN_TU) || defined(MMFB_ATTN_PROBS_TU) || defined(MMFB_ATTN_CAUSAL_TU)
 __global__ void attn_delta_kernel(const bf16* __restrict__ dO, int64_t ld_do, const bf16* __restrict__ O,
                                   int64_t ld_o, const bf16* __restrict__ Olo, float* __restrict__ delta, int B, int H,
                                   int Sq, int D);
@@ -657,7 +686,7 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ dO, int64_t ld_do, co
   }
 }
 
-#endif  // MMFB_ATTN_VARLEN_TU || MMFB_ATTN_PROBS_TU
+#endif  // MMFB_ATTN_VARLEN_TU || MMFB_ATTN_PROBS_TU || MMFB_ATTN_CAUSAL_TU
 
 // ----------------------------------------------------------------------------------------------
 // host
@@ -670,6 +699,16 @@ static int check_attn_common(const mmfb_attn_args& a, const char* who) {
   if (a.Skv > max_kv)
     return set_error(MMFB_ERR_ARG, "%s: Skv=%d exceeds the single-pass limit %d for head_dim %d", who, a.Skv, max_kv,
                      a.head_dim);
+  if (a.causal_len < 0) return set_error(MMFB_ERR_ARG, "%s: negative causal_len (%d)", who, a.causal_len);
+  if (a.causal_len > 0 && (a.Sq != a.Skv || a.causal_len > a.Skv))
+    return set_error(MMFB_ERR_ARG, "%s: a causal tail needs self-attention (Sq=%d, Skv=%d) and causal_len (%d) <= Skv", who,
+                     a.Sq, a.Skv, a.causal_len);
+  return MMFB_OK;
+}
+
+// the packed entry points and the probabilities kernel have no causal tail
+static inline int check_no_causal(const mmfb_attn_args& a, const char* who) {
+  if (a.causal_len != 0) return set_error(MMFB_ERR_ARG, "%s: causal_len must be 0 (got %d)", who, a.causal_len);
   return MMFB_OK;
 }
 
@@ -687,7 +726,7 @@ static int head_map(CUtensorMap* m, const void* ptr, int W, int64_t ld, int rows
   return make_tmap_3d(m, ptr, W, rows, batches, ld, ld * rows, 64, box_rows);
 }
 
-template <int D, bool VARLEN>
+template <int D, bool VARLEN, bool CAUSAL = false>
 static int attn_fwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total, const int32_t* cu_kv, int total_kv,
                            cudaStream_t stream) {
   const int W = a.heads * D;
@@ -713,7 +752,8 @@ static int attn_fwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total
   p.scale2 = LOG2E / sqrtf(static_cast<float>(D));
   p.cu = cu; p.total = total;
   p.cu_kv = cu_kv; p.total_kv = total_kv;
-  auto kern = attn_fwd_kernel<D, VARLEN>;
+  p.P = a.Skv - a.causal_len;
+  auto kern = attn_fwd_kernel<D, VARLEN, CAUSAL>;
   static int smem_set = 0;
   if (smem > smem_set) {
     if ((rc = set_smem(reinterpret_cast<const void*>(kern), smem, "attn_fwd"))) return rc;
@@ -727,7 +767,7 @@ static int attn_fwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total
   return MMFB_OK;
 }
 
-template <int D, bool DROP, bool VARLEN>
+template <int D, bool DROP, bool VARLEN, bool CAUSAL>
 static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, int total, int total_kv, cudaStream_t stream) {
   constexpr int QB = (D == 64) ? 64 : 32;   // query block of the dK/dV kernel: d = 128 keeps its tiles in registers
   const int W = a.heads * D;
@@ -759,11 +799,11 @@ static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, int
   static int set_q = 0;
   static bool set_kv = false;
   if (smem_q > set_q) {
-    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel<D, DROP, VARLEN>), smem_q, "attn_bwd_dq"))) return rc;
+    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dq_kernel<D, DROP, VARLEN, CAUSAL>), smem_q, "attn_bwd_dq"))) return rc;
     set_q = smem_q;
   }
   if (!set_kv) {
-    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dkv_kernel<D, DROP, QB, VARLEN>), smem_kv, "attn_bwd_dkv")))
+    if ((rc = set_smem(reinterpret_cast<const void*>(attn_bwd_dkv_kernel<D, DROP, QB, VARLEN, CAUSAL>), smem_kv, "attn_bwd_dkv")))
       return rc;
     set_kv = true;
   }
@@ -772,14 +812,14 @@ static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, int
   // no key rows -> no dk/dv kernel (the dq kernel writes every query row, as 0)
   if (rq > 0 && a.Sq > 0) {
     p.out0 = reinterpret_cast<bf16*>(a.dq); p.ld0 = a.ld_dq; p.out1 = nullptr; p.ld1 = 0;
-    MMFB_LAUNCH((attn_bwd_dq_kernel<D, DROP, VARLEN>), dim3((a.Sq + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS, smem_q,
+    MMFB_LAUNCH((attn_bwd_dq_kernel<D, DROP, VARLEN, CAUSAL>), dim3((a.Sq + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS, smem_q,
                 stream, tmQ, tmdO, tmK, tmV, p);
     count_launch();
   }
   if (rkv > 0 && a.Skv > 0) {
     p.out0 = reinterpret_cast<bf16*>(a.dk); p.ld0 = a.ld_dk;
     p.out1 = reinterpret_cast<bf16*>(a.dv); p.ld1 = a.ld_dv;
-    MMFB_LAUNCH((attn_bwd_dkv_kernel<D, DROP, QB, VARLEN>), dim3((a.Skv + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS,
+    MMFB_LAUNCH((attn_bwd_dkv_kernel<D, DROP, QB, VARLEN, CAUSAL>), dim3((a.Skv + AT_ROWS - 1) / AT_ROWS, a.heads, a.B), AT_THREADS,
                 smem_kv, stream, tmK, tmV, tmQc, tmdOc, p);
     count_launch();
   }
@@ -788,7 +828,7 @@ static int attn_bwd_kernels(const mmfb_attn_args& a, const AttnBwdDev& base, int
   return MMFB_OK;
 }
 
-template <int D, bool VARLEN>
+template <int D, bool VARLEN, bool CAUSAL = false>
 static int attn_bwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total, const int32_t* cu_kv, int total_kv,
                            cudaStream_t stream) {
   // delta = rowsum(dO * O); packed rows are one batch of `total` query rows
@@ -810,19 +850,21 @@ static int attn_bwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total
   p.scale2 = LOG2E * p.scale;
   p.cu = cu; p.total = total;
   p.cu_kv = cu_kv; p.total_kv = total_kv;
-  return a.drop_mask != nullptr ? attn_bwd_kernels<D, true, VARLEN>(a, p, total, total_kv, stream)
-                                : attn_bwd_kernels<D, false, VARLEN>(a, p, total, total_kv, stream);
+  p.P = a.Skv - a.causal_len;
+  return a.drop_mask != nullptr ? attn_bwd_kernels<D, true, VARLEN, CAUSAL>(a, p, total, total_kv, stream)
+                                : attn_bwd_kernels<D, false, VARLEN, CAUSAL>(a, p, total, total_kv, stream);
 }
 
-// The dense entry points instantiate the dense kernels only, and attention_varlen.cu (which includes this file) the
-// packed ones: instantiated in one translation unit, the two share inlined helpers that the compiler then schedules
-// differently, and the dense d = 64 forward would not keep the code it has without the packed mode.  attention_probs.cu
-// includes this file for its helpers only and instantiates neither.
-#if !defined(MMFB_ATTN_VARLEN_TU) && !defined(MMFB_ATTN_PROBS_TU)
+// The dense entry points instantiate the dense kernels only, attention_varlen.cu (which includes this file) the packed
+// ones and attention_causal.cu the dense ones with a causal tail: instantiated in one translation unit, they share inlined
+// helpers that the compiler then schedules differently, and the dense d = 64 forward would not keep the code it has
+// without the other modes.  attention_probs.cu includes this file for its helpers only and instantiates none.
+#if !defined(MMFB_ATTN_VARLEN_TU) && !defined(MMFB_ATTN_PROBS_TU) && !defined(MMFB_ATTN_CAUSAL_TU)
 int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream) {
   int rc = check_attn_common(a, "attn_fwd");
   if (rc) return rc;
   if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2) return set_error(MMFB_ERR_ARG, "attn_fwd: null pointer");
+  if (a.causal_len != 0) return attn_causal_fwd(a, stream);
   return a.head_dim == 64 ? attn_fwd_launch<64, false>(a, nullptr, 0, nullptr, 0, stream)
                           : attn_fwd_launch<128, false>(a, nullptr, 0, nullptr, 0, stream);
 }
@@ -832,6 +874,7 @@ int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
   if (rc) return rc;
   if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2 || !a.dctx || !a.delta || !a.dq || !a.dk || !a.dv)
     return set_error(MMFB_ERR_ARG, "attn_bwd: null pointer");
+  if (a.causal_len != 0) return attn_causal_bwd(a, stream);
   return a.head_dim == 64 ? attn_bwd_launch<64, false>(a, nullptr, 0, nullptr, 0, stream)
                           : attn_bwd_launch<128, false>(a, nullptr, 0, nullptr, 0, stream);
 }
@@ -842,6 +885,7 @@ int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
 static int check_varlen(const mmfb_attn_args& a, const int32_t* cu, int total, const char* who) {
   int rc = check_attn_common(a, who);
   if (rc) return rc;
+  if ((rc = check_no_causal(a, who))) return rc;
   if (a.Sq != a.Skv) return set_error(MMFB_ERR_ARG, "%s: self-attention only, Sq (%d) must equal Skv (%d) = max_len", who, a.Sq, a.Skv);
   if (a.mask != nullptr) return set_error(MMFB_ERR_ARG, "%s: mask must be NULL (packing has removed the masked keys)", who);
   if (!cu) return set_error(MMFB_ERR_ARG, "%s: null cu_seqlens", who);
@@ -881,6 +925,8 @@ static int check_varlen_cross(const mmfb_attn_args& a, const int32_t* cu_q, int 
     return set_error(MMFB_ERR_ARG, "%s: Skv=%d exceeds the single-pass limit %d for head_dim %d", who, a.Skv, max_kv,
                      a.head_dim);
   if (a.mask != nullptr) return set_error(MMFB_ERR_ARG, "%s: mask must be NULL (packing has removed the masked keys)", who);
+  int rc = check_no_causal(a, who);
+  if (rc) return rc;
   if (!cu_q || !cu_kv) return set_error(MMFB_ERR_ARG, "%s: null cu_q / cu_kv", who);
   if (total_q < 0 || total_kv < 0) return set_error(MMFB_ERR_ARG, "%s: negative total (%d, %d)", who, total_q, total_kv);
   return MMFB_OK;
@@ -908,6 +954,18 @@ int attn_varlen_cross_bwd(const mmfb_attn_args& a, const int32_t* cu_q, int tota
   return a.head_dim == 64 ? attn_bwd_launch<64, true>(a, cu_q, total_q, cu_kv, total_kv, stream)
                           : attn_bwd_launch<128, true>(a, cu_q, total_q, cu_kv, total_kv, stream);
 }
-#endif  // MMFB_ATTN_VARLEN_TU
+#elif defined(MMFB_ATTN_CAUSAL_TU)
+
+// Dense self-attention with a causal tail; attn_fwd / attn_bwd have checked the arguments (causal_len != 0 here).
+int attn_causal_fwd(const mmfb_attn_args& a, cudaStream_t stream) {
+  return a.head_dim == 64 ? attn_fwd_launch<64, false, true>(a, nullptr, 0, nullptr, 0, stream)
+                          : attn_fwd_launch<128, false, true>(a, nullptr, 0, nullptr, 0, stream);
+}
+
+int attn_causal_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
+  return a.head_dim == 64 ? attn_bwd_launch<64, false, true>(a, nullptr, 0, nullptr, 0, stream)
+                          : attn_bwd_launch<128, false, true>(a, nullptr, 0, nullptr, 0, stream);
+}
+#endif  // MMFB_ATTN_VARLEN_TU / MMFB_ATTN_CAUSAL_TU
 
 }  // namespace mmfb

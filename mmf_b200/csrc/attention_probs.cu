@@ -222,6 +222,7 @@ static int attn_probs_launch(const mmfb_attn_args& a, void* probs, cudaStream_t 
 int attn_probs(const mmfb_attn_args& a, void* probs, int probs_dtype, cudaStream_t stream) {
   int rc = check_attn_common(a, "attn_probs");
   if (rc) return rc;
+  if ((rc = check_no_causal(a, "attn_probs"))) return rc;
   if (probs_dtype != MMFB_PROBS_F32 && probs_dtype != MMFB_PROBS_BF16)
     return set_error(MMFB_ERR_ARG, "attn_probs: probs_dtype must be MMFB_PROBS_F32 or MMFB_PROBS_BF16 (got %d)", probs_dtype);
   if (!a.q || !a.k || !a.lse2 || !probs) return set_error(MMFB_ERR_ARG, "attn_probs: null pointer");

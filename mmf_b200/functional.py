@@ -75,7 +75,7 @@ def gemm(a, b, *, a_mn=False, b_mn=False, epi=lib.EPI_BIAS, bias=None, aux=None,
     return out
 
 
-def _attn_args(q, k, v, B, heads, Sq, Skv, mask, drop_mask, drop_scale):
+def _attn_args(q, k, v, B, heads, Sq, Skv, mask, drop_mask, drop_scale, causal_len=0):
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _req(t, torch.bfloat16, n)
     W = q.shape[-1]
@@ -99,14 +99,18 @@ def _attn_args(q, k, v, B, heads, Sq, Skv, mask, drop_mask, drop_scale):
             raise ValueError("attention: drop_mask must be contiguous int32 [B, heads, Sq, ceil(Skv/32)]")
         a.drop_mask, a.drop_scale = drop_mask.data_ptr(), float(drop_scale)
     a.B, a.heads, a.Sq, a.Skv, a.head_dim = B, heads, Sq, Skv, W // heads
+    a.causal_len = int(causal_len)
     return a
 
 
-def attention_fwd(q, k, v, B, heads, Sq, Skv, mask=None, drop_mask=None, drop_scale=1.0, out=None, save_lo=False):
+def attention_fwd(q, k, v, B, heads, Sq, Skv, mask=None, drop_mask=None, drop_scale=1.0, out=None, save_lo=False,
+                  causal_len=0):
     """ctx, lse2 (, ctx_lo) = fused softmax(QK^T/sqrt(d) + mask) V.  q [B*Sq, h*d], k/v [B*Skv, h*d] (views allowed).
     save_lo: also return ctx_lo = bf16(O - float(ctx)), the part of the fp32 output the bf16 ctx drops; the backward's
-    delta = rowsum(dO * (ctx + ctx_lo)) then carries no common rounding bias per row."""
-    a = _attn_args(q, k, v, B, heads, Sq, Skv, mask, drop_mask, drop_scale)
+    delta = rowsum(dO * (ctx + ctx_lo)) then carries no common rounding bias per row.
+    causal_len = T > 0 (self-attention, Sq == Skv): the last T keys are a causal tail - key k >= Skv - T takes 0 where
+    k <= q and -10000 otherwise, in place of mask[:, k] (M4C's prefix-LM mask); 0 = none."""
+    a = _attn_args(q, k, v, B, heads, Sq, Skv, mask, drop_mask, drop_scale, causal_len)
     W = q.shape[-1]
     ctx = out if out is not None else torch.empty(B * Sq, W, dtype=torch.bfloat16, device=q.device)
     lse2 = torch.empty(B, heads, Sq, dtype=torch.float32, device=q.device)
@@ -122,9 +126,10 @@ def attention_fwd(q, k, v, B, heads, Sq, Skv, mask=None, drop_mask=None, drop_sc
 
 
 def attention_bwd(dctx, q, k, v, ctx, lse2, B, heads, Sq, Skv, mask=None, drop_mask=None, drop_scale=1.0,
-                  dq=None, dk=None, dv=None, ctx_lo=None):
-    """dq, dk, dv from the saved q, k, v, ctx and row statistics (probabilities are recomputed)."""
-    a = _attn_args(q, k, v, B, heads, Sq, Skv, mask, drop_mask, drop_scale)
+                  dq=None, dk=None, dv=None, ctx_lo=None, causal_len=0):
+    """dq, dk, dv from the saved q, k, v, ctx and row statistics (probabilities are recomputed).  causal_len: the
+    forward's."""
+    a = _attn_args(q, k, v, B, heads, Sq, Skv, mask, drop_mask, drop_scale, causal_len)
     _req(dctx, torch.bfloat16, "dctx")
     _req(ctx, torch.bfloat16, "ctx")
     W = q.shape[-1]

@@ -55,6 +55,7 @@ class AttnArgs(ctypes.Structure):
         ("dv", ctypes.c_void_p), ("ld_dv", ctypes.c_int64),
         ("B", ctypes.c_int), ("heads", ctypes.c_int), ("Sq", ctypes.c_int), ("Skv", ctypes.c_int),
         ("head_dim", ctypes.c_int),
+        ("causal_len", ctypes.c_int),
     ]
 
 

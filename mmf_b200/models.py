@@ -6,6 +6,8 @@
   registry.register_model("lxmert")       LXMERT       <->  mmf/models/lxmert.py:647-790
   registry.register_model("uniter")       UNITER       <->  mmf/models/uniter.py:615-774   (mmf_b200/uniter_model.py)
   registry.register_model("vinvl")        VinVL        <->  mmf/models/vinvl.py:392-505    (mmf_b200/vinvl_model.py)
+  registry.register_model("m4c")          M4C          <->  mmf/models/m4c.py:34-347       (mmf_b200/m4c_model.py)
+  registry.register_model("m4c_captioner") M4CCaptioner <->  mmf/models/m4c_captioner.py:6-24
 
 Each is a `BaseModel` (mmf/models/base_model.py:67-337 contract: ctor(config) -> build() -> forward(SampleList) -> dict
 with "scores" and/or "losses"; `config_path()` names the model's default YAML; `__call__` fills "losses" from the
@@ -1033,3 +1035,4 @@ class LXMERT(BaseModel):
 
 from . import uniter_model  # noqa: E402,F401  (registers "uniter"; it needs the names defined above)
 from . import vinvl_model  # noqa: E402,F401  (registers "vinvl"; it needs the names defined above)
+from . import m4c_model  # noqa: E402,F401  (registers "m4c" and "m4c_captioner"; it needs the names defined above)

@@ -289,8 +289,13 @@ class _BertEncoderFn(torch.autograd.Function):
         return (None, None, None, None, None, dx.view(B, S, H).to(ctx.in_dtype)) + tuple(runner.pack.autograd_grads(aliased))
 
 
-def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hidden_states=False, output_attentions=False):
+def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hidden_states=False, output_attentions=False,
+                     causal_len=0):
     """hidden_states [B,S,H] (fp32 or bf16), attention_mask additive [B,1,1,S] / [B,S] / None.
+    causal_len = T > 0 makes the last T positions a causal tail (engine.CausalTail, M4C's prefix-LM mask): every query
+    attends to the keys before the tail that attention_mask keeps, the first S - T queries to no tail key, and tail query t
+    to tail keys 0..t; attention_mask is not read for the tail keys.  Such a call runs the dense path even with skip_padding
+    set, and cannot return probabilities.
     Returns (last,), then the L layer inputs if output_hidden_states, then the L layers' attention probabilities
     [B, heads, S, S] (hidden-state dtype, post-dropout in training) if output_attentions.  The hidden states and
     probabilities are outputs for inspection: they carry no gradient, so a loss that reads them back-propagates nothing
@@ -304,7 +309,12 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
     if H != runner.weights[0].hidden:
         raise ValueError("hidden size %d does not match the encoder's %d" % (H, runner.weights[0].hidden))
     mask = E.additive_mask_2d(attention_mask, B, S)
-    if runner.skip_padding and mask is not None and not output_attentions:
+    causal_len = int(causal_len)
+    if causal_len:
+        if not 0 < causal_len <= S:
+            raise ValueError("causal_len must be in [0, S=%d], got %d" % (S, causal_len))
+        mask = E.CausalTail(mask, causal_len)
+    elif runner.skip_padding and mask is not None and not output_attentions:
         packing = _plan_packing(mask, B, S)
         if packing is not None and packing.varlen.total == 0:
             # every token is padding: nothing to compute, every output row (and every input-gradient row) is zero
