@@ -65,9 +65,23 @@ typedef struct {
   int splits;                    /* split-K factor, MMFB_EPI_ATOMIC_F32 only (0/1 = none) */
   int block_n;                   /* 0 = auto, else 128 or 256 */
   int cluster;                   /* 0, 1 or 2; kept for ABI compatibility: every GEMM runs as single-CTA tiles */
+  void* workspace;               /* MMFB_EPI_ATOMIC_F32 only: NULL and 0 = fp32 vector reductions (see below) */
+  int64_t workspace_bytes;
 } mmfb_gemm_args;
 
 int mmfb_gemm(const mmfb_gemm_args* args, mmfb_stream stream);
+
+/* Ordered split-K (MMFB_EPI_ATOMIC_F32 with a workspace).  By default the S = splits units of an output tile add their
+ * fp32 partial tiles into C with vector reductions, in whatever order they finish, so the low bits of C vary from run to
+ * run whenever the GEMM actually runs S > 1 splits.  With `workspace` set, unit (tile, s) instead STORES its partial P_s
+ * (the product over split s's k-blocks, accumulated from zero) into slice s of the fp32 workspace [S, M, N], and a second
+ * kernel computes  C = ((C + P_0) + P_1) + ... + P_{S-1}  in fp32, split by split: the same bits on every run.
+ * mmfb_gemm_workspace_bytes(M, N, K, splits) (host only, no device needed) gives the bytes this takes: S * M * N * 4 for the
+ * split factor the GEMM will run (splits is lowered until every split owns a k-block of 64), or 0 when that factor is 1 -
+ * a single unit per tile adds C + acc once, which is already deterministic, and the workspace is not touched.
+ * An ordered call (workspace or workspace_bytes non-zero) whose workspace is NULL, smaller than that size or not 16-byte
+ * aligned is MMFB_ERR_ARG before any launch.  The workspace is the caller's; nothing in it is kept between calls. */
+int64_t mmfb_gemm_workspace_bytes(int M, int N, int K, int splits);
 
 /* Fused multi-head attention core (everything between the Q/K/V projections and the output projection):
  *   ctx = dropout(softmax(Q K^T / sqrt(d) + mask)) V        BertSelfAttentionJit.forward hf_layers.py:182-210,
@@ -182,16 +196,35 @@ typedef struct {
   void* dz; int64_t lddz;            /* bf16 [M,H] gradient wrt the dropped dense output */
   float* dgamma; float* dbeta; float* dbias;
   int M, H;
+  float* workspace;                  /* backward: NULL and 0 = fp32 atomics for dgamma/dbeta/dbias (see below) */
+  int64_t workspace_bytes;
 } mmfb_ln_args;
 
 int mmfb_layernorm_fwd(const mmfb_ln_args* args, mmfb_stream stream);
 int mmfb_layernorm_bwd(const mmfb_ln_args* args, mmfb_stream stream);
+
+/* Ordered reductions over rows.  The rows are cut into chunks of 128 (chunk k = rows [128k, 128k + 128)), a number that
+ * depends on M alone.  Each chunk sums its rows in a fixed order (8 warps, warp w taking rows w, w + 8, ... of the chunk,
+ * the warps' sums added in warp order) and STORES that partial into the workspace; a second kernel then adds the partials
+ * to the destination in chunk order:  out[n] += ((part_0[n] + part_1[n]) + ...) + part_{K-1}[n].
+ * The result has the same bits on every run and does not depend on the number of SMs.
+ *   mmfb_layernorm_bwd with workspace set: dgamma / dbeta / dbias are accumulated this way; dy and dz are computed row by
+ *   row exactly as without it (the same bits).  Size: mmfb_layernorm_bwd_workspace_bytes(M, H) = ceil(M/128) * 3 * H * 4.
+ *   mmfb_colsum_ordered: the column sum of mmfb_colsum.  Size: mmfb_colsum_workspace_bytes(M, N) = ceil(M/128) * N * 4.
+ * The size queries are host only (no device needed) and return 0 for an empty shape.  A layernorm_bwd with workspace or
+ * workspace_bytes non-zero is an ordered call; an ordered call whose workspace is NULL, smaller than the size above or not
+ * 16-byte aligned is MMFB_ERR_ARG before any launch. */
+int64_t mmfb_layernorm_bwd_workspace_bytes(int M, int H);
+int64_t mmfb_colsum_workspace_bytes(int M, int N);
 
 /* out[n] += sum_m X[m,n]   (bias gradients), X bf16 [M,N], out fp32 [N].
  * Like the LayerNorm calls, the column sums, embed_compose / embed_scatter / embed_scatter_sorted and dropout_apply read
  * and write bf16 rows as 16-byte vectors: every row tensor they use starts 16-byte aligned and, when M > 1, has a leading
  * dimension that is a multiple of 8 (the gathered src / dsrc rows whatever M is); MMFB_ERR_ARG otherwise. */
 int mmfb_colsum(const void* X, int64_t ldx, float* out, int M, int N, mmfb_stream stream);
+/* mmfb_colsum with the chunk-ordered sum described above; workspace fp32, mmfb_colsum_workspace_bytes(M, N) bytes */
+int mmfb_colsum_ordered(const void* X, int64_t ldx, float* out, int M, int N, float* workspace, int64_t workspace_bytes,
+                        mmfb_stream stream);
 
 /* Philox keep-bits for nn.Dropout(p): word w bit j <-> element 32*w+j, P(bit=1) = 1-p (16-bit resolution) */
 int mmfb_dropout_bits(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t offset, float p, mmfb_stream stream);
@@ -227,6 +260,16 @@ int mmfb_embed_scatter(const mmfb_scatter_args* args, mmfb_stream stream);
  * Equal indices are summed in registers first (one atomic per run of <= 32 rows instead of one per row). */
 int mmfb_embed_scatter_sorted(const void* dy, int64_t lddy, const int32_t* order, const int32_t* sorted_idx, float* dtab,
                               int M, int H, mmfb_stream stream);
+/* The same sum in an order fixed by the index vector alone.  Sorted positions are cut into chunks of 32 (one warp each);
+ * a chunk sums each of its runs of equal indices in position order.  A run that lies inside one chunk has no other
+ * contributor and is added to its table row directly.  A run that crosses chunk boundaries leaves one partial per chunk
+ * in the workspace, and a second kernel adds  ((piece_first + piece_next) + ...) + piece_last  to the row, chunks in
+ * position order.  Same bits on every run.  workspace: fp32, mmfb_embed_scatter_sorted_workspace_bytes(M, H) =
+ * ceil(M/32) * 2 * H * 4 bytes (host only); NULL, smaller or not 16-byte aligned is MMFB_ERR_ARG before any launch. */
+int64_t mmfb_embed_scatter_sorted_workspace_bytes(int M, int H);
+int mmfb_embed_scatter_sorted_ordered(const void* dy, int64_t lddy, const int32_t* order, const int32_t* sorted_idx,
+                                      float* dtab, int M, int H, float* workspace, int64_t workspace_bytes,
+                                      mmfb_stream stream);
 
 /* dz = dy where y > 0 else 0 (backward of the ReLU epilogue); contiguous bf16 buffers of n elements */
 int mmfb_relu_bwd(const void* dy, const void* y, void* dz, int64_t n, mmfb_stream stream);
@@ -241,6 +284,8 @@ int mmfb_gelu_bwd(const void* dh, const void* u, void* du, int64_t n, mmfb_strea
  * *loss_sum (and stored in row_loss[m] when given) and the row is OVERWRITTEN by
  * d(logits) = (softmax(z_m) - onehot(label[m])) * grad_scale;  ignored rows are overwritten by zeros.  A label outside
  * [0, V) that is not ignore_index is treated like ignore_index: zero gradient, row_loss 0, nothing added to *loss_sum.
+ * *loss_sum takes one fp32 atomic per row, so its low bits depend on the order the rows finish; loss_sum may be NULL, and a
+ * caller that needs the same bits on every run sums row_loss in a fixed order instead (d(logits) is per row and exact).
  * Replaces CrossEntropyLoss(ignore_index=-1) over prediction_scores.view(-1, vocab_size) of the masked-LM heads
  * (mmf/models/visual_bert.py:215,269-277; mmf/models/transformers/heads/mlm.py:46-97) inside the chunked
  * linear + cross-entropy head: the full [tokens, 30522] logits tensor never exists in HBM. */

@@ -183,6 +183,16 @@ int mmfb_colsum(const void* X, int64_t ldx, float* out, int M, int N, mmfb_strea
   MMFB_REQUIRE_DEVICE();
   return colsum(X, ldx, out, M, N, reinterpret_cast<cudaStream_t>(stream));
 }
+int mmfb_colsum_ordered(const void* X, int64_t ldx, float* out, int M, int N, float* workspace, int64_t workspace_bytes,
+                        mmfb_stream stream) {
+  if (!X || !out) return set_error(MMFB_ERR_ARG, "mmfb_colsum_ordered: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return colsum_ordered(X, ldx, out, M, N, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+int64_t mmfb_gemm_workspace_bytes(int M, int N, int K, int splits) { return gemm_workspace_bytes(M, N, K, splits); }
+int64_t mmfb_layernorm_bwd_workspace_bytes(int M, int H) { return ln_bwd_workspace_bytes(M, H); }
+int64_t mmfb_colsum_workspace_bytes(int M, int N) { return colsum_workspace_bytes(M, N); }
+int64_t mmfb_embed_scatter_sorted_workspace_bytes(int M, int H) { return scatter_sorted_workspace_bytes(M, H); }
 int mmfb_dropout_bits(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t offset, float p, mmfb_stream stream) {
   if (!out) return set_error(MMFB_ERR_ARG, "mmfb_dropout_bits: null pointer");
   MMFB_REQUIRE_DEVICE();
@@ -209,6 +219,15 @@ int mmfb_embed_scatter_sorted(const void* dy, int64_t lddy, const int32_t* order
   if (!dy || !order || !sorted_idx || !dtab) return set_error(MMFB_ERR_ARG, "mmfb_embed_scatter_sorted: null pointer");
   MMFB_REQUIRE_DEVICE();
   return scatter_sorted(dy, lddy, order, sorted_idx, dtab, M, H, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_embed_scatter_sorted_ordered(const void* dy, int64_t lddy, const int32_t* order, const int32_t* sorted_idx,
+                                      float* dtab, int M, int H, float* workspace, int64_t workspace_bytes,
+                                      mmfb_stream stream) {
+  if (!dy || !order || !sorted_idx || !dtab)
+    return set_error(MMFB_ERR_ARG, "mmfb_embed_scatter_sorted_ordered: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return scatter_sorted_ordered(dy, lddy, order, sorted_idx, dtab, M, H, workspace, workspace_bytes,
+                                reinterpret_cast<cudaStream_t>(stream));
 }
 int mmfb_relu_bwd(const void* dy, const void* y, void* dz, int64_t n, mmfb_stream stream) {
   if (!dy || !y || !dz) return set_error(MMFB_ERR_ARG, "mmfb_relu_bwd: null pointer");

@@ -40,7 +40,7 @@ struct GemmDev {
   int splits;
   bf16* c;               // bf16 destination [M, ldc]
   bf16* c2;              // second bf16 destination (EPI_BIAS_GELU)
-  float* c32;            // EPI_ATOMIC_F32 destination
+  float* c32;            // EPI_ATOMIC_F32 destination; EPI_PARTIAL_F32: the workspace [splits, M, N]
   int64_t ldc;
   const bf16* bias;      // [N] or null
   const bf16* aux;       // residual / pre-activation, [M, ldaux], or null; read through the aux tensor map
@@ -53,6 +53,8 @@ struct GemmDev {
 __host__ __device__ constexpr bool epi_reads_aux(int epi) {
   return epi == EPI_BIAS_DROP_RESID || epi == EPI_GELU_BWD || epi == EPI_ADD_AUX;
 }
+// epilogues that write fp32 pairs straight from the accumulators (split-K weight gradient)
+__host__ __device__ constexpr bool epi_f32(int epi) { return epi == EPI_ATOMIC_F32 || epi == EPI_PARTIAL_F32; }
 
 template <int BN>
 struct Cfg {
@@ -121,7 +123,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (EPI != EPI_ATOMIC_F32) tma_prefetch_desc(&tmC);
+    if (!epi_f32(EPI)) tma_prefetch_desc(&tmC);
     if (EPI == EPI_BIAS_GELU) tma_prefetch_desc(&tmC2);
     if (has_aux) tma_prefetch_desc(&tmX);
     for (int s = 0; s < STAGES; ++s) {
@@ -221,8 +223,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       mbar_arrive(&empty[prev]);           // every unit owns at least one k-block
     }
 
-    if (EPI == EPI_ATOMIC_F32) {
-      // ---------------------------- split-K epilogue: fp32 vector reductions ----------------------------
+    if (epi_f32(EPI)) {
+      // ------------- split-K epilogue: fp32 vector reductions into C, or plain stores of the split's partial -------------
+      float* dst = p.c32;
+      if (EPI == EPI_PARTIAL_F32) dst += static_cast<int64_t>(u % p.splits) * p.M * p.N;   // ldc = N
 #pragma unroll
       for (int rh = 0; rh < 2; ++rh) {
         const int m = w.m0 + half * 64 + warp * 16 + (lane >> 2) + rh * 8;
@@ -231,9 +235,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         for (int j = 0; j < BN / 8; ++j) {
           const int n = w.n0 + j * 8 + (lane & 3) * 2;
           if (n >= p.N) continue;                // N % 8 == 0: n < N implies n + 1 < N
-          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p.c32 + static_cast<int64_t>(m) * p.ldc + n),
-                       "f"(acc[j * 4 + rh * 2]), "f"(acc[j * 4 + rh * 2 + 1])
-                       : "memory");
+          if (EPI == EPI_ATOMIC_F32) {
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + static_cast<int64_t>(m) * p.ldc + n),
+                         "f"(acc[j * 4 + rh * 2]), "f"(acc[j * 4 + rh * 2 + 1])
+                         : "memory");
+          } else {
+            *reinterpret_cast<float2*>(dst + static_cast<int64_t>(m) * p.ldc + n) =
+                make_float2(acc[j * 4 + rh * 2], acc[j * 4 + rh * 2 + 1]);
+          }
         }
       }
       continue;
@@ -337,12 +346,47 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       }
     }
   }
-  if (EPI != EPI_ATOMIC_F32 && issuer) tma_store_wait_all();   // the staging smem must outlive the reads of the stores
+  if (!epi_f32(EPI) && issuer) tma_store_wait_all();   // the staging smem must outlive the reads of the stores
+}
+
+// Second kernel of the ordered split-K GEMM:  C = ((C + P_0) + P_1) + ... + P_{S-1}  for the partials P_s = ws[s] [M, N].
+// Four consecutive columns per thread (N % 8 == 0: they lie in one row).
+__global__ void __launch_bounds__(256)
+splitk_reduce_kernel(const float* __restrict__ ws, int S, int M, int N, float* __restrict__ c, int64_t ldc) {
+  griddep_launch();
+  griddep_wait();
+  const int64_t mn = static_cast<int64_t>(M) * N;
+  const int64_t i = (static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x) * 4;
+  if (i >= mn) return;
+  float2* dst = reinterpret_cast<float2*>(c + (i / N) * ldc + (i % N));
+  const float2 c0 = dst[0], c1 = dst[1];
+  float4 r = make_float4(c0.x, c0.y, c1.x, c1.y);
+  for (int s = 0; s < S; ++s) {
+    const float4 v = *reinterpret_cast<const float4*>(ws + s * mn + i);
+    r.x += v.x; r.y += v.y; r.z += v.z; r.w += v.w;
+  }
+  dst[0] = make_float2(r.x, r.y);
+  dst[1] = make_float2(r.z, r.w);
 }
 
 // ----------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------
+int gemm_effective_splits(int K, int splits) {
+  int s = splits > 0 ? splits : 1;
+  const int kb_total = (K + BK - 1) / BK;
+  if (s > kb_total) s = kb_total;
+  // every split must own at least one k-block
+  while (s > 1 && ((kb_total + s - 1) / s) * (s - 1) >= kb_total) --s;
+  return s;
+}
+
+int64_t gemm_workspace_bytes(int M, int N, int K, int splits) {
+  if (M <= 0 || N <= 0 || K <= 0) return 0;
+  const int s = gemm_effective_splits(K, splits);
+  return s > 1 ? static_cast<int64_t>(s) * M * N * 4 : 0;
+}
+
 template <int BN, bool A_MN, bool B_MN, int EPI>
 static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
   using C = Cfg<BN>;
@@ -372,20 +416,16 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
   memset(&tmC, 0, sizeof(tmC));
   memset(&tmC2, 0, sizeof(tmC2));
   memset(&tmX, 0, sizeof(tmX));
-  if (EPI != EPI_ATOMIC_F32 && (rc = make_tmap_2d(&tmC, a.C, a.N, a.M, a.ldc, 64, 64))) return rc;
+  if (!epi_f32(EPI) && (rc = make_tmap_2d(&tmC, a.C, a.N, a.M, a.ldc, 64, 64))) return rc;
   if (EPI == EPI_BIAS_GELU && (rc = make_tmap_2d(&tmC2, a.C2, a.N, a.M, a.ldc, 64, 64))) return rc;
   if (AUX && a.aux != nullptr && (rc = make_tmap_2d(&tmX, a.aux, a.N, a.M, a.ldaux, 64, 64))) return rc;
   GemmDev p;
   p.M = a.M; p.N = a.N; p.K = a.K;
-  p.splits = (EPI == EPI_ATOMIC_F32 && a.splits > 0) ? a.splits : 1;
-  const int kb_total = (a.K + BK - 1) / BK;
-  if (p.splits > kb_total) p.splits = kb_total;
-  // every split must own at least one k-block
-  while (p.splits > 1 && ((kb_total + p.splits - 1) / p.splits) * (p.splits - 1) >= kb_total) --p.splits;
+  p.splits = epi_f32(EPI) ? gemm_effective_splits(a.K, a.splits) : 1;
   p.c = reinterpret_cast<bf16*>(a.C);
   p.c2 = reinterpret_cast<bf16*>(a.C2);
-  p.c32 = reinterpret_cast<float*>(a.C);
-  p.ldc = a.ldc;
+  p.c32 = reinterpret_cast<float*>(EPI == EPI_PARTIAL_F32 ? a.workspace : a.C);
+  p.ldc = EPI == EPI_PARTIAL_F32 ? a.N : a.ldc;
   p.bias = reinterpret_cast<const bf16*>(a.bias);
   p.aux = reinterpret_cast<const bf16*>(a.aux);
   p.dmask = a.drop_mask;
@@ -429,6 +469,21 @@ static int dispatch(const mmfb_gemm_args& a, cudaStream_t s) {
   }
 }
 
+// Ordered split-K: every (tile, split) unit stores its partial into the workspace, then one more kernel adds the
+// partials into C in split order.  No unit waits for another, so this is safe whatever number of CTAs is resident.
+template <int BN>
+static int gemm_ordered(const mmfb_gemm_args& a, int splits, cudaStream_t stream) {
+  int rc = launch<BN, true, true, EPI_PARTIAL_F32>(a, stream);
+  if (rc) return rc;
+  const int64_t quads = static_cast<int64_t>(a.M) * a.N / 4;
+  MMFB_LAUNCH(splitk_reduce_kernel, static_cast<unsigned>((quads + 255) / 256), 256, 0, stream,
+              reinterpret_cast<const float*>(a.workspace), splits, a.M, a.N, reinterpret_cast<float*>(a.C), a.ldc);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "gemm split-K reduce launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return MMFB_OK;
+}
+
 int gemm(const mmfb_gemm_args& a, cudaStream_t stream) {
   if (a.M <= 0 || a.N <= 0 || a.K <= 0) return set_error(MMFB_ERR_ARG, "gemm: empty problem %dx%dx%d", a.M, a.N, a.K);
   // only CONTIGUOUS extents need 16-byte granularity (TMA row pitch / vector epilogue); K of an MN-major operand
@@ -440,6 +495,17 @@ int gemm(const mmfb_gemm_args& a, cudaStream_t stream) {
   if ((a.lda % 8) || (a.ldb % 8) || (a.epi != EPI_ATOMIC_F32 && (a.ldc % 8)))
     return set_error(MMFB_ERR_ARG, "gemm: leading dimensions must be multiples of 8 elements");
   const int bn = a.block_n > 0 ? a.block_n : (a.N >= 256 ? 256 : 128);
+  const bool ordered = a.epi == EPI_ATOMIC_F32 && (a.workspace != nullptr || a.workspace_bytes != 0);
+  const int splits = gemm_effective_splits(a.K, a.splits);
+  if (ordered && splits > 1 && (bn == 128 || bn == 256) && a.a_mn && a.b_mn) {
+    const int64_t need = gemm_workspace_bytes(a.M, a.N, a.K, a.splits);
+    if (a.workspace == nullptr || a.workspace_bytes < need || (reinterpret_cast<uintptr_t>(a.workspace) & 15))
+      return set_error(MMFB_ERR_ARG, "gemm: ordered split-K needs a 16-byte aligned workspace of %lld bytes (got %p, %lld)",
+                       (long long)need, a.workspace, (long long)a.workspace_bytes);
+    if ((reinterpret_cast<uintptr_t>(a.C) & 7) || (a.ldc % 2))
+      return set_error(MMFB_ERR_ARG, "gemm: ordered split-K needs an 8-byte aligned C with an even ldc");
+    return bn == 256 ? gemm_ordered<256>(a, splits, stream) : gemm_ordered<128>(a, splits, stream);
+  }
   if (bn == 256) return dispatch<256>(a, stream);
   if (bn == 128) return dispatch<128>(a, stream);
   return set_error(MMFB_ERR_ARG, "gemm: block_n must be 128 or 256");

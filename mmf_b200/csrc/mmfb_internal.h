@@ -15,8 +15,25 @@ enum {
   EPI_GELU_BWD = MMFB_EPI_GELU_BWD,
   EPI_ADD_AUX = MMFB_EPI_ADD_AUX,
   EPI_ATOMIC_F32 = MMFB_EPI_ATOMIC_F32,
-  EPI_BIAS_RELU = MMFB_EPI_BIAS_RELU
+  EPI_BIAS_RELU = MMFB_EPI_BIAS_RELU,
+  // internal: the ordered split-K weight gradient - unit (tile, split s) stores its fp32 partial into slice s of the
+  // caller's workspace [S, M, N] (plain stores), and a second kernel adds the slices into C in split order
+  EPI_PARTIAL_F32 = 100
 };
+
+// Rows per chunk of the ordered column sums (colsum, LayerNorm parameter gradients): chunk k holds rows
+// [k * ORDER_ROWS, (k + 1) * ORDER_ROWS), so the number of chunks and every partial depend on M alone.
+constexpr int ORDER_ROWS = 128;
+// Sorted positions per chunk of the ordered embedding-table scatter (the run-aggregation window of one warp).
+constexpr int SCATTER_CHUNK = 32;
+inline int order_chunks(int M) { return (M + ORDER_ROWS - 1) / ORDER_ROWS; }
+
+// split-K factor the GEMM actually runs for K and the requested `splits`: every split owns at least one k-block
+int gemm_effective_splits(int K, int splits);
+int64_t gemm_workspace_bytes(int M, int N, int K, int splits);
+int64_t ln_bwd_workspace_bytes(int M, int H);
+int64_t colsum_workspace_bytes(int M, int N);
+int64_t scatter_sorted_workspace_bytes(int M, int H);
 
 // records a thread-local error message and returns `code`
 int set_error(int code, const char* fmt, ...);
@@ -65,6 +82,7 @@ int attn_causal_bwd(const mmfb_attn_args& a, cudaStream_t stream);
 int ln_fwd(const mmfb_ln_args& a, cudaStream_t s);
 int ln_bwd(const mmfb_ln_args& a, cudaStream_t s);
 int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s);
+int colsum_ordered(const void* X, int64_t ldx, float* out, int M, int N, float* ws, int64_t ws_bytes, cudaStream_t s);
 int dropout_bits(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t offset, float p, const uint64_t* epoch, cudaStream_t s);
 int compose(const mmfb_compose_args& a, cudaStream_t s);
 int scatter(const mmfb_scatter_args& a, cudaStream_t s);
@@ -79,6 +97,8 @@ int dropout_apply(const void* x, int64_t ldx, const uint32_t* bits, int64_t ldm,
 int gelu_bwd(const void* dh, const void* u, void* du, int64_t n, cudaStream_t s);
 int scatter_sorted(const void* dy, int64_t lddy, const int32_t* order, const int32_t* sorted_idx, float* dtab, int M,
                    int H, cudaStream_t s);
+int scatter_sorted_ordered(const void* dy, int64_t lddy, const int32_t* order, const int32_t* sorted_idx, float* dtab, int M,
+                           int H, float* ws, int64_t ws_bytes, cudaStream_t s);
 int ot_fwd(const mmfb_ot_args& a, cudaStream_t s);
 int ot_bwd(const mmfb_ot_args& a, cudaStream_t s);
 

@@ -102,14 +102,19 @@ ln_fwd_kernel(const bf16* __restrict__ y, int64_t ldy, const bf16* __restrict__ 
 // A persistent grid (grid-stride over row groups) keeps the number of fp32 atomics at 3*H per block.
 // Two kernels, chosen by H: ln_bwd_stream_kernel for H <= 1024, ln_bwd_kernel for 1024 < H <= 2048.
 // ----------------------------------------------------------------------------------------------
+// ORDERED (both kernels): block b owns the rows of chunk b (ORDER_ROWS rows, warp w taking rows w, w + ROW_WARPS, ...) and
+// stores its three column-sum sets to ws[b][which][H] instead of adding them to dgamma / dbeta / dbias; chunk_reduce_kernel
+// adds them up in chunk order.  The row outputs dy / dz do not depend on which block computes a row.
 // Rows of up to MAXV * 256 columns: a warp loads, computes and stores a row held in registers, and only the other warps
 // of the SM cover its load latency.
+template <bool ORDERED>
 __global__ void __launch_bounds__(ROW_WARPS * 32)
 ln_bwd_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict__ dx2, int64_t lddx2,
               const bf16* __restrict__ y, int64_t ldy, const float* __restrict__ mean,
               const float* __restrict__ rstd, const bf16* __restrict__ gamma, bf16* __restrict__ dy, int64_t lddy,
               bf16* __restrict__ dz, int64_t lddz, const uint32_t* __restrict__ dmask, int64_t ldmask, float dscale,
-              float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M, int H) {
+              float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M, int H,
+              float* __restrict__ ws) {
   griddep_launch();
   griddep_wait();
   __shared__ float red[ROW_WARPS][256];
@@ -120,8 +125,10 @@ ln_bwd_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict_
 #pragma unroll
     for (int e = 0; e < 8; ++e) { ag[i][e] = 0.0f; ab[i][e] = 0.0f; az[i][e] = 0.0f; }
 
-  for (int64_t row = static_cast<int64_t>(blockIdx.x) * ROW_WARPS + warp; row < M;
-       row += static_cast<int64_t>(gridDim.x) * ROW_WARPS) {
+  const int64_t row_end = ORDERED ? min(static_cast<int64_t>(M), (static_cast<int64_t>(blockIdx.x) + 1) * ORDER_ROWS) : M;
+  const int64_t stride = ORDERED ? ROW_WARPS : static_cast<int64_t>(gridDim.x) * ROW_WARPS;
+  for (int64_t row = static_cast<int64_t>(blockIdx.x) * (ORDERED ? ORDER_ROWS : ROW_WARPS) + warp; row < row_end;
+       row += stride) {
     const float mu = mean[row], rs = rstd[row];
     float g[MAXV][8], d[MAXV][8], xh[MAXV][8];
     float s1 = 0.0f, s2 = 0.0f;
@@ -190,7 +197,10 @@ ln_bwd_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict_
       float t = 0.0f;
 #pragma unroll
       for (int w = 0; w < ROW_WARPS; ++w) t += red[w][c];
-      if (i * 256 + c < H) atomicAdd(dst + i * 256 + c, t);
+      if (i * 256 + c < H) {
+        if (ORDERED) ws[(static_cast<int64_t>(blockIdx.x) * 3 + which) * H + i * 256 + c] = t;
+        else atomicAdd(dst + i * 256 + c, t);
+      }
     }
   }
 }
@@ -219,15 +229,18 @@ __device__ __forceinline__ void bulk_load_1d(void* dst_smem, const void* src, ui
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(dst_smem)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-template <int NV, bool HAS_DX2, int ST>
+template <int NV, bool HAS_DX2, int ST, bool ORDERED>
 __global__ void __launch_bounds__(ROW_WARPS * 32, 2)
 ln_bwd_stream_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict__ dx2, int64_t lddx2,
                      const bf16* __restrict__ y, int64_t ldy, const float* __restrict__ mean,
                      const float* __restrict__ rstd, const bf16* __restrict__ gamma, bf16* __restrict__ dy, int64_t lddy,
                      bf16* __restrict__ dz, int64_t lddz, const uint32_t* __restrict__ dmask, int64_t ldmask, float dscale,
-                     float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M, int H) {
+                     float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M_rows, int H,
+                     float* __restrict__ ws) {
   griddep_launch();
   griddep_wait();
+  // the bound of the rows this block visits: its chunk's end when ORDERED
+  const int M = ORDERED ? min(M_rows, static_cast<int>(blockIdx.x + 1) * ORDER_ROWS) : M_rows;
   constexpr int NT = HAS_DX2 ? 3 : 2;                 // tensors per slot: dx, y (, dx2)
   constexpr int ROWB = NV * 512;                      // bytes reserved per tensor row in a slot
   extern __shared__ __align__(128) uint8_t ln_smem[];
@@ -250,8 +263,8 @@ ln_bwd_stream_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __re
   uint8_t* my = ring + warp * (ST * NT * ROWB);
   uint64_t* my_full = full + warp * ST;
   const uint32_t row_bytes = static_cast<uint32_t>(H) * 2u;
-  const int64_t stride = static_cast<int64_t>(gridDim.x) * ROW_WARPS;
-  const int64_t row_first = static_cast<int64_t>(blockIdx.x) * ROW_WARPS + warp;
+  const int64_t stride = ORDERED ? ROW_WARPS : static_cast<int64_t>(gridDim.x) * ROW_WARPS;
+  const int64_t row_first = static_cast<int64_t>(blockIdx.x) * (ORDERED ? ORDER_ROWS : ROW_WARPS) + warp;
   auto fill = [&](int slot, int64_t row) {            // lane 0
     uint8_t* d = my + slot * (NT * ROWB);
     mbar_expect_tx(&my_full[slot], NT * row_bytes);
@@ -393,16 +406,21 @@ ln_bwd_stream_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __re
       float t = 0.0f;
 #pragma unroll
       for (int w = 0; w < ROW_WARPS; ++w) t += red[w * 256 + c];
-      if (i * 256 + c < H) atomicAdd(dst + i * 256 + c, t);
+      if (i * 256 + c < H) {
+        if (ORDERED) ws[(static_cast<int64_t>(blockIdx.x) * 3 + which) * H + i * 256 + c] = t;
+        else atomicAdd(dst + i * 256 + c, t);
+      }
     }
   }
 }
 
 // ----------------------------------------------------------------------------------------------
 // column sums (bias gradients):  out[n] += sum_m X[m, n]
+// ORDERED: block (x, k) sums the rows of chunk k and stores the partial to ws[k][N]; chunk_reduce_kernel adds them up.
 // ----------------------------------------------------------------------------------------------
+template <bool ORDERED>
 __global__ void __launch_bounds__(256)
-colsum_kernel(const bf16* __restrict__ X, int64_t ldx, float* __restrict__ out, int M, int N) {
+colsum_kernel(const bf16* __restrict__ X, int64_t ldx, float* __restrict__ out, int M, int N, float* __restrict__ ws) {
   griddep_launch();
   griddep_wait();
   __shared__ float red[8][256];
@@ -415,13 +433,15 @@ colsum_kernel(const bf16* __restrict__ X, int64_t ldx, float* __restrict__ out, 
     // four independent 16-byte loads in flight per lane (the one-load-per-iteration loop reached 0.57 of the HBM peak),
     // packed fp32 adds
     uint64_t a2[4] = {0ull, 0ull, 0ull, 0ull};
-    const int64_t stride = static_cast<int64_t>(gridDim.y) * 8;
-    for (int64_t row = static_cast<int64_t>(blockIdx.y) * 8 + warp; row < M; row += 4 * stride) {
+    const int64_t stride = ORDERED ? 8 : static_cast<int64_t>(gridDim.y) * 8;
+    const int64_t row_end = ORDERED ? min(static_cast<int64_t>(M), (static_cast<int64_t>(blockIdx.y) + 1) * ORDER_ROWS) : M;
+    for (int64_t row = static_cast<int64_t>(blockIdx.y) * (ORDERED ? ORDER_ROWS : 8) + warp; row < row_end;
+         row += 4 * stride) {
       uint4 u[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         const int64_t r = row + k * stride;
-        u[k] = r < M ? *reinterpret_cast<const uint4*>(X + r * ldx + col) : make_uint4(0u, 0u, 0u, 0u);
+        u[k] = r < row_end ? *reinterpret_cast<const uint4*>(X + r * ldx + col) : make_uint4(0u, 0u, 0u, 0u);
       }
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
@@ -441,7 +461,37 @@ colsum_kernel(const bf16* __restrict__ X, int64_t ldx, float* __restrict__ out, 
 #pragma unroll
   for (int w = 0; w < 8; ++w) t += red[w][threadIdx.x];
   const int c = blockIdx.x * 256 + threadIdx.x;
-  if (c < N) atomicAdd(out + c, t);
+  if (c < N) {
+    if (ORDERED) ws[static_cast<int64_t>(blockIdx.y) * N + c] = t;
+    else atomicAdd(out + c, t);
+  }
+}
+
+// Second kernel of the ordered column sums: ws holds `chunks` partial rows of width segs * n, segment j of which belongs to
+// out.p[j] (skipped when null).  out[c] += ((part_0[c] + part_1[c]) + ...) + part_{chunks-1}[c], one thread per column.
+struct ChunkOuts {
+  float* p[3];
+};
+__global__ void __launch_bounds__(256)
+chunk_reduce_kernel(const float* __restrict__ ws, int chunks, int n, int segs, ChunkOuts out) {
+  griddep_launch();
+  griddep_wait();
+  const int c = blockIdx.x * 256 + threadIdx.x;
+  const int width = segs * n;
+  if (c >= width) return;
+  float* dst = out.p[c / n];
+  if (dst == nullptr) return;
+  float t = 0.0f;
+  int k = 0;
+  for (; k + 16 <= chunks; k += 16) {     // sixteen loads in flight, added in chunk order
+    float v[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = ws[static_cast<int64_t>(k + j) * width + c];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) t += v[j];
+  }
+  for (; k < chunks; ++k) t += ws[static_cast<int64_t>(k) * width + c];
+  dst[c % n] += t;
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -569,10 +619,15 @@ scatter_kernel(ScatterDev c, const bf16* __restrict__ dy, int64_t lddy, int M, i
 // Table-gradient scatter over SORTED indices: warp w owns sorted positions [32w, 32w+32); rows with equal index are
 // summed in registers and flushed with one atomic per column per run, so an index shared by thousands of rows (type /
 // position embeddings) costs M/32 atomics per address instead of M.
-template <int NV>
+// ORDERED: a run piece that is the whole run (nothing before or after it in other chunks) is added to its table row with
+// a plain read-modify-write - no other warp touches that row.  A piece of a run that crosses a chunk boundary is stored to
+// the workspace instead: slot ws[w][0] when the run began before this chunk, ws[w][1] when it begins here and goes on
+// past it; scatter_runs_kernel adds the pieces of each crossing run in chunk order.
+template <int NV, bool ORDERED>
 __global__ void __launch_bounds__(ROW_WARPS * 32)
 scatter_sorted_kernel(const bf16* __restrict__ dy, int64_t lddy, const int32_t* __restrict__ order,
-                      const int32_t* __restrict__ sorted_idx, float* __restrict__ dtab, int M, int H) {
+                      const int32_t* __restrict__ sorted_idx, float* __restrict__ dtab, int M, int H,
+                      float* __restrict__ ws) {
   griddep_launch();
   griddep_wait();
   const int lane = threadIdx.x & 31;
@@ -585,22 +640,39 @@ scatter_sorted_kernel(const bf16* __restrict__ dy, int64_t lddy, const int32_t* 
 #pragma unroll
     for (int e = 0; e < 8; ++e) acc[i][e] = 0.0f;
   int cur = -1;
+  int run_start = 0;
   const int n = (M - p0) < 32 ? static_cast<int>(M - p0) : 32;
   for (int k = 0; k <= n; ++k) {
     const int id = (k < n) ? sorted_idx[p0 + k] : -2;
     if (id != cur) {
       if (cur >= 0) {
+        float* piece = nullptr;       // ORDERED: the workspace slot of a crossing run's piece
+        if (ORDERED) {
+          if (run_start == 0 && p0 > 0 && sorted_idx[p0 - 1] == cur) piece = ws + (w * 2) * H;
+          else if (k == n && p0 + n < M && sorted_idx[p0 + n] == cur) piece = ws + (w * 2 + 1) * H;
+        }
 #pragma unroll
         for (int i = 0; i < NV; ++i) {
           const int col = i * 256 + lane * 8;
           if (col < H) {
             float* d = dtab + static_cast<int64_t>(cur) * H + col;
+            if (!ORDERED) {
 #pragma unroll
-            for (int e = 0; e < 8; ++e) { atomicAdd(d + e, acc[i][e]); acc[i][e] = 0.0f; }
+              for (int e = 0; e < 8; ++e) atomicAdd(d + e, acc[i][e]);
+            } else if (piece != nullptr) {
+              *reinterpret_cast<float4*>(piece + col) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+              *reinterpret_cast<float4*>(piece + col + 4) = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
+            } else {
+#pragma unroll
+              for (int e = 0; e < 8; ++e) d[e] += acc[i][e];
+            }
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[i][e] = 0.0f;
           }
         }
       }
       cur = id;
+      run_start = k;
     }
     if (k < n && id >= 0) {
       const int64_t r = order[p0 + k];
@@ -615,6 +687,48 @@ scatter_sorted_kernel(const bf16* __restrict__ dy, int64_t lddy, const int32_t* 
         }
       }
     }
+  }
+}
+
+// Second kernel of the ordered scatter: block w adds up the run that begins in chunk w and crosses into chunk w + 1, if
+// there is one: its piece ws[w][1], then ws[c][0] of every later chunk c the run reaches, in chunk order, and adds the sum
+// to the run's table row.  The run's end is found by a binary search of the sorted indices, so the pieces' loads do not
+// wait on each other.
+__global__ void __launch_bounds__(256)
+scatter_runs_kernel(const int32_t* __restrict__ sorted_idx, const float* __restrict__ ws, float* __restrict__ dtab, int M,
+                    int H) {
+  griddep_launch();
+  griddep_wait();
+  const int64_t w = blockIdx.x;
+  const int64_t p0 = w * SCATTER_CHUNK;
+  const int64_t last = min(static_cast<int64_t>(M), p0 + SCATTER_CHUNK) - 1;
+  if (last + 1 >= M) return;
+  const int id = sorted_idx[last];
+  if (id < 0 || sorted_idx[last + 1] != id) return;                          // nothing crosses out of this chunk
+  if (sorted_idx[p0] == id && p0 > 0 && sorted_idx[p0 - 1] == id) return;    // the run began in an earlier chunk
+  int64_t lo = last + 1, hi = M;                                              // first position past the run
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (sorted_idx[mid] == id) lo = mid + 1;
+    else hi = mid;
+  }
+  const int64_t c_last = (lo - 1) / SCATTER_CHUNK;                            // chunk of the run's last position
+  for (int col = threadIdx.x * 4; col < H; col += 256 * 4) {
+    float4 t = *reinterpret_cast<const float4*>(ws + (w * 2 + 1) * H + col);
+    int64_t c = w + 1;
+    for (; c + 8 <= c_last + 1; c += 8) {       // eight loads in flight, added in chunk order
+      float4 v[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = *reinterpret_cast<const float4*>(ws + ((c + j) * 2) * H + col);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { t.x += v[j].x; t.y += v[j].y; t.z += v[j].z; t.w += v[j].w; }
+    }
+    for (; c <= c_last; ++c) {
+      const float4 v = *reinterpret_cast<const float4*>(ws + (c * 2) * H + col);
+      t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
+    }
+    float* d = dtab + static_cast<int64_t>(id) * H + col;
+    d[0] += t.x; d[1] += t.y; d[2] += t.z; d[3] += t.w;
   }
 }
 
@@ -746,21 +860,68 @@ static int ln_bwd_grid(int M) {
   return grid < cap ? grid : cap;
 }
 
-template <int NV, bool HAS_DX2, int ST>
+int64_t ln_bwd_workspace_bytes(int M, int H) {
+  return (M > 0 && H > 0) ? static_cast<int64_t>(order_chunks(M)) * 3 * H * 4 : 0;
+}
+int64_t colsum_workspace_bytes(int M, int N) {
+  return (M > 0 && N > 0) ? static_cast<int64_t>(order_chunks(M)) * N * 4 : 0;
+}
+int64_t scatter_sorted_workspace_bytes(int M, int H) {
+  return (M > 0 && H > 0) ? static_cast<int64_t>((M + SCATTER_CHUNK - 1) / SCATTER_CHUNK) * 2 * H * 4 : 0;
+}
+static int check_workspace(const char* who, const float* ws, int64_t ws_bytes, int64_t need) {
+  if (ws == nullptr || ws_bytes < need || (reinterpret_cast<uintptr_t>(ws) & 15))
+    return set_error(MMFB_ERR_ARG, "%s: the ordered reduction needs a 16-byte aligned workspace of %lld bytes (got %p, %lld)",
+                     who, static_cast<long long>(need), static_cast<const void*>(ws), static_cast<long long>(ws_bytes));
+  return MMFB_OK;
+}
+// adds the `chunks` partial rows of ws (segments of n columns, segment j for out[j]) to their destinations
+static int chunk_reduce(const float* ws, int chunks, int n, float* out0, float* out1, float* out2, int segs, cudaStream_t s,
+                        const char* who) {
+  ChunkOuts o;
+  o.p[0] = out0; o.p[1] = out1; o.p[2] = out2;
+  MMFB_LAUNCH(chunk_reduce_kernel, (segs * n + 255) / 256, 256, 0, s, ws, chunks, n, segs, o);
+  return launch_ok(who);
+}
+
+template <int NV, bool HAS_DX2, int ST, bool ORDERED>
 static int ln_bwd_stream(const mmfb_ln_args& a, cudaStream_t s) {
   constexpr size_t smem = static_cast<size_t>(ROW_WARPS) * ST * (HAS_DX2 ? 3 : 2) * NV * 512 + ROW_WARPS * 256 * 4 +
                           NV * 256 * 4 + 4096 + ROW_WARPS * ST * 8;
-  auto kern = ln_bwd_stream_kernel<NV, HAS_DX2, ST>;
+  auto kern = ln_bwd_stream_kernel<NV, HAS_DX2, ST, ORDERED>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "cudaFuncSetAttribute(layernorm_bwd): %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  MMFB_LAUNCH(kern, ln_bwd_grid(a.M), ROW_WARPS * 32, smem, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2, a.lddx2,
-              (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy, a.lddy, (bf16*)a.dz, a.lddz,
-              a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H);
+  MMFB_LAUNCH(kern, ORDERED ? order_chunks(a.M) : ln_bwd_grid(a.M), ROW_WARPS * 32, smem, s, (const bf16*)a.dx, a.lddx,
+              (const bf16*)a.dx2, a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy, a.lddy,
+              (bf16*)a.dz, a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H, a.workspace);
   return launch_ok("layernorm_bwd");
+}
+
+// The ordered LayerNorm backward: the kernels above with one block per chunk of rows, then the chunk partials of dgamma,
+// dbeta and dbias added in chunk order.  Same ring depths as the atomic path.
+static int ln_bwd_ordered(const mmfb_ln_args& a, bool wide, cudaStream_t s) {
+  const int chunks = order_chunks(a.M);
+  if (wide) {
+    MMFB_LAUNCH(ln_bwd_kernel<true>, chunks, ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2,
+                a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy, a.lddy, (bf16*)a.dz,
+                a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H, a.workspace);
+    int rc = launch_ok("layernorm_bwd");
+    if (rc) return rc;
+  } else {
+    static int (*const stream[2][4])(const mmfb_ln_args&, cudaStream_t) = {
+        {ln_bwd_stream<1, false, 4, true>, ln_bwd_stream<2, false, 4, true>, ln_bwd_stream<3, false, 3, true>,
+         ln_bwd_stream<4, false, 2, true>},
+        {ln_bwd_stream<1, true, 3, true>, ln_bwd_stream<2, true, 3, true>, ln_bwd_stream<3, true, 2, true>,
+         ln_bwd_stream<4, true, 2, true>}};
+    int rc = stream[a.dx2 != nullptr][(a.H + 255) / 256 - 1](a, s);
+    if (rc) return rc;
+  }
+  if (!a.dgamma && !a.dbeta && !a.dbias) return MMFB_OK;
+  return chunk_reduce(a.workspace, chunks, a.H, a.dgamma, a.dbeta, a.dbias, 3, s, "layernorm_bwd reduce");
 }
 
 int ln_bwd(const mmfb_ln_args& a, cudaStream_t s) {
@@ -774,16 +935,23 @@ int ln_bwd(const mmfb_ln_args& a, cudaStream_t s) {
   rc = check_aligned("layernorm_bwd", a.M, {{a.dx, a.lddx, "dx"}, {a.dx2, a.lddx2, "dx2"}, {a.y, a.ldy, "y"},
                                             {a.dy, a.lddy, "dy"}, {dz, a.lddz, "dz"}, {wide ? a.gamma : nullptr, 0, "gamma"}});
   if (rc) return rc;
+  if (a.workspace != nullptr || a.workspace_bytes != 0) {
+    rc = check_workspace("layernorm_bwd", a.workspace, a.workspace_bytes, ln_bwd_workspace_bytes(a.M, a.H));
+    if (rc) return rc;
+    return ln_bwd_ordered(a, wide, s);
+  }
   if (wide) {
-    MMFB_LAUNCH(ln_bwd_kernel, ln_bwd_grid(a.M), ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2,
+    MMFB_LAUNCH(ln_bwd_kernel<false>, ln_bwd_grid(a.M), ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2,
                 a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy, a.lddy, (bf16*)a.dz,
-                a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H);
+                a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H, nullptr);
     return launch_ok("layernorm_bwd");
   }
   // ln_bwd_stream<NV, HAS_DX2, ST> indexed by [dx2 given][NV - 1]; NV = 256-column slabs per row, ST = ring depth
   static int (*const stream[2][4])(const mmfb_ln_args&, cudaStream_t) = {
-      {ln_bwd_stream<1, false, 4>, ln_bwd_stream<2, false, 4>, ln_bwd_stream<3, false, 3>, ln_bwd_stream<4, false, 2>},
-      {ln_bwd_stream<1, true, 3>, ln_bwd_stream<2, true, 3>, ln_bwd_stream<3, true, 2>, ln_bwd_stream<4, true, 2>}};
+      {ln_bwd_stream<1, false, 4, false>, ln_bwd_stream<2, false, 4, false>, ln_bwd_stream<3, false, 3, false>,
+       ln_bwd_stream<4, false, 2, false>},
+      {ln_bwd_stream<1, true, 3, false>, ln_bwd_stream<2, true, 3, false>, ln_bwd_stream<3, true, 2, false>,
+       ln_bwd_stream<4, true, 2, false>}};
   return stream[a.dx2 != nullptr][(a.H + 255) / 256 - 1](a, s);
 }
 
@@ -796,8 +964,19 @@ int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s)
   const int cap = (num_sms() * 4 + grid.x - 1) / grid.x;
   grid.y = rows_blocks < cap ? rows_blocks : cap;
   if (grid.y < 1) grid.y = 1;
-  MMFB_LAUNCH(colsum_kernel, grid, 256, 0, s, (const bf16*)X, ldx, out, M, N);
+  MMFB_LAUNCH(colsum_kernel<false>, grid, 256, 0, s, (const bf16*)X, ldx, out, M, N, nullptr);
   return launch_ok("colsum");
+}
+
+int colsum_ordered(const void* X, int64_t ldx, float* out, int M, int N, float* ws, int64_t ws_bytes, cudaStream_t s) {
+  if (M <= 0 || N <= 0 || N % 8) return set_error(MMFB_ERR_ARG, "colsum_ordered: bad shape %dx%d", M, N);
+  int rc = check_aligned("colsum_ordered", M, {{X, ldx, "x"}});
+  if (rc) return rc;
+  if ((rc = check_workspace("colsum_ordered", ws, ws_bytes, colsum_workspace_bytes(M, N)))) return rc;
+  const int chunks = order_chunks(M);
+  MMFB_LAUNCH(colsum_kernel<true>, dim3((N + 255) / 256, chunks), 256, 0, s, (const bf16*)X, ldx, out, M, N, ws);
+  if ((rc = launch_ok("colsum_ordered"))) return rc;
+  return chunk_reduce(ws, chunks, N, out, nullptr, nullptr, 1, s, "colsum_ordered reduce");
 }
 
 int dropout_bits(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t offset, float p, const uint64_t* epoch, cudaStream_t s) {
@@ -858,10 +1037,28 @@ int scatter_sorted(const void* dy, int64_t lddy, const int32_t* order, const int
   const int warps = (M + 31) / 32;
   const int grid = (warps + ROW_WARPS - 1) / ROW_WARPS;
   const int nv = (H + 255) / 256;
-#define SS(NV) MMFB_LAUNCH(scatter_sorted_kernel<NV>, grid, ROW_WARPS * 32, 0, s, (const bf16*)dy, lddy, order, sorted_idx, dtab, M, H)
+#define SS(NV) MMFB_LAUNCH((scatter_sorted_kernel<NV, false>), grid, ROW_WARPS * 32, 0, s, (const bf16*)dy, lddy, order, sorted_idx, dtab, M, H, nullptr)
   if (nv <= 1) SS(1); else if (nv == 2) SS(2); else if (nv == 3) SS(3); else SS(4);
 #undef SS
   return launch_ok("embed_scatter_sorted");
+}
+
+int scatter_sorted_ordered(const void* dy, int64_t lddy, const int32_t* order, const int32_t* sorted_idx, float* dtab, int M,
+                           int H, float* ws, int64_t ws_bytes, cudaStream_t s) {
+  int rc = check_rows(M, H, "embed_scatter_sorted_ordered");
+  if (rc) return rc;
+  if (H > 1024) return set_error(MMFB_ERR_ARG, "embed_scatter_sorted_ordered: hidden size %d > 1024", H);
+  if ((rc = check_aligned("embed_scatter_sorted_ordered", M, {{dy, lddy, "dy"}}))) return rc;
+  if ((rc = check_workspace("embed_scatter_sorted_ordered", ws, ws_bytes, scatter_sorted_workspace_bytes(M, H)))) return rc;
+  const int chunks = (M + SCATTER_CHUNK - 1) / SCATTER_CHUNK;
+  const int grid = (chunks + ROW_WARPS - 1) / ROW_WARPS;
+  const int nv = (H + 255) / 256;
+#define SS(NV) MMFB_LAUNCH((scatter_sorted_kernel<NV, true>), grid, ROW_WARPS * 32, 0, s, (const bf16*)dy, lddy, order, sorted_idx, dtab, M, H, ws)
+  if (nv <= 1) SS(1); else if (nv == 2) SS(2); else if (nv == 3) SS(3); else SS(4);
+#undef SS
+  if ((rc = launch_ok("embed_scatter_sorted_ordered"))) return rc;
+  MMFB_LAUNCH(scatter_runs_kernel, chunks, 256, 0, s, sorted_idx, (const float*)ws, dtab, M, H);
+  return launch_ok("embed_scatter_sorted_ordered runs");
 }
 
 int relu_bwd(const void* dy, const void* y, void* dz, int64_t n, cudaStream_t s) {

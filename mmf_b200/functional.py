@@ -3,8 +3,16 @@
 Each wrapper validates dtypes/devices, allocates outputs with torch (so the caching allocator and
 autograd own every buffer) and enqueues the kernel on the current CUDA stream.  Nothing here
 computes on the CPU.
+
+Deterministic mode: while torch.use_deterministic_algorithms(True) is in effect, every wrapper whose kernel would add
+fp32 values with atomics in arrival order - gemm with EPI_ATOMIC_F32 and splits > 1, colsum, layernorm_bwd's parameter
+gradients, embed_scatter_sorted and ce_rows' loss sum - runs the ordered variant instead, whose summation order depends
+only on the call's shapes and indices, so repeated steps give the same bits.  The flag is read on every call; this module
+is the only one that knows about it.  A path that has no ordered variant (embed_scatter with table gradients) raises
+RuntimeError, or warns under warn_only=True, as PyTorch's own non-deterministic ops do.
 """
 import ctypes
+import warnings
 
 import torch
 
@@ -23,6 +31,25 @@ def _req(t, dtype, name):
         raise ValueError("%s must be contiguous in its last dimension" % name)
 
 
+def _ordered():
+    return torch.are_deterministic_algorithms_enabled()
+
+
+def _workspace(nbytes, device):
+    """fp32 scratch of an ordered reduction, from torch's caching allocator (capture-safe).  Dropping it right after the
+    launch is safe: the allocator only hands the block to work enqueued later on the same stream."""
+    return torch.empty((int(nbytes) + 3) // 4, dtype=torch.float32, device=device)
+
+
+def _no_ordered_path(what):
+    msg = ("%s does not have a deterministic implementation, but you set 'torch.use_deterministic_algorithms(True)'. "
+           "You can turn off determinism just for this operation, or you can use the 'warn_only=True' option" % what)
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg)
+    else:
+        raise RuntimeError(msg)
+
+
 def _idx_len(idx, M, name):
     """the kernels read one index per output row and never check: a short index buffer is an out-of-bounds device read"""
     if idx.numel() != M or not idx.is_contiguous():
@@ -34,7 +61,8 @@ def gemm(a, b, *, a_mn=False, b_mn=False, epi=lib.EPI_BIAS, bias=None, aux=None,
     """C[M,N] = epi(A[M,K] @ B[N,K]^T) on the wgmma GEMM.
 
     a: [M,K] (a_mn=False) or [K,M] (a_mn=True); b: [N,K] (b_mn=False) or [K,N] (b_mn=True); bf16.
-    Returns C (and C2 for EPI_BIAS_GELU).  For EPI_ATOMIC_F32 `out` (fp32 [M,N]) is accumulated into.
+    Returns C (and C2 for EPI_BIAS_GELU).  For EPI_ATOMIC_F32 `out` (fp32 [M,N]) is accumulated into; in deterministic
+    mode with splits > 1 the split partials go through a workspace and are added in split order.
     """
     _req(a, torch.bfloat16, "a")
     _req(b, torch.bfloat16, "b")
@@ -69,6 +97,12 @@ def gemm(a, b, *, a_mn=False, b_mn=False, epi=lib.EPI_BIAS, bias=None, aux=None,
     args.drop_scale = float(drop_scale)
     args.M, args.N, args.K = M, N, K
     args.epi, args.splits, args.block_n, args.cluster = int(epi), int(splits), int(block_n), int(cluster)
+    ws = None
+    if epi == lib.EPI_ATOMIC_F32 and splits > 1 and _ordered():
+        nbytes = LIB.mmfb_gemm_workspace_bytes(M, N, K, int(splits))
+        if nbytes > 0:
+            ws = _workspace(nbytes, a.device)
+            args.workspace, args.workspace_bytes = ws.data_ptr(), nbytes
     check(LIB.mmfb_gemm(ctypes.byref(args), _stream_ptr()))
     if epi == lib.EPI_BIAS_GELU:
         return out, out2
@@ -437,6 +471,11 @@ def layernorm_bwd(dx, y, mean, rstd, gamma, dgamma, dbeta, dbias=None, dx2=None,
             _req(t, torch.float32, name)
             setattr(a, name, t.data_ptr())
     a.M, a.H = M, H
+    ws = None
+    if (dgamma is not None or dbeta is not None or dbias is not None) and _ordered():
+        nbytes = LIB.mmfb_layernorm_bwd_workspace_bytes(M, H)
+        ws = _workspace(nbytes, y.device)
+        a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
     check(LIB.mmfb_layernorm_bwd(ctypes.byref(a), _stream_ptr()))
     return dy, dz
 
@@ -444,6 +483,12 @@ def layernorm_bwd(dx, y, mean, rstd, gamma, dgamma, dbeta, dbias=None, dx2=None,
 def colsum(x, out):
     """out[n] += sum_m x[m,n] (x bf16 [M,N], out fp32 [N])."""
     _req(x, torch.bfloat16, "x"); _req(out, torch.float32, "out")
+    if _ordered():
+        nbytes = LIB.mmfb_colsum_workspace_bytes(x.shape[0], x.shape[1])
+        ws = _workspace(nbytes, x.device)
+        check(LIB.mmfb_colsum_ordered(x.data_ptr(), x.stride(0), out.data_ptr(), x.shape[0], x.shape[1], ws.data_ptr(),
+                                      nbytes, _stream_ptr()))
+        return out
     check(LIB.mmfb_colsum(x.data_ptr(), x.stride(0), out.data_ptr(), x.shape[0], x.shape[1], _stream_ptr()))
     return out
 
@@ -500,6 +545,13 @@ def ce_rows(logits, labels, ignore_index, grad_scale, loss_sum, row_loss=None):
     if row_loss is not None:
         _req(row_loss, torch.float32, "row_loss")
         rl = row_loss.data_ptr()
+    if _ordered():
+        # the kernel's loss_sum takes one atomic per row; here the loss is a fixed-order sum of the per-row losses instead
+        rows = row_loss if row_loss is not None else torch.empty(M, dtype=torch.float32, device=logits.device)
+        check(LIB.mmfb_ce_rows(logits.data_ptr(), logits.stride(0), labels.data_ptr(), int(ignore_index), M, V,
+                               float(grad_scale), None, rows.data_ptr(), _stream_ptr()))
+        loss_sum.add_(rows.sum())
+        return logits
     check(LIB.mmfb_ce_rows(logits.data_ptr(), logits.stride(0), labels.data_ptr(), int(ignore_index), M, V, float(grad_scale),
                            loss_sum.data_ptr(), rl, _stream_ptr()))
     return logits
@@ -596,8 +648,10 @@ def embed_compose(M, H, srcs=(), tabs=(), device=None):
 
 def embed_scatter(dy, dsrcs=(), dtabs=()):
     """Backward of embed_compose: dsrcs (bf16 tensor, rows) get plain row stores, dtabs (fp32 table grad, idx) get
-    atomic accumulation."""
+    atomic accumulation (no ordered variant: refused in deterministic mode; embed_scatter_sorted has one)."""
     _req(dy, torch.bfloat16, "dy")
+    if len(dtabs) and _ordered():
+        _no_ordered_path("mmf_b200.functional.embed_scatter with table gradients (dtabs)")
     M, H = dy.shape
     a = ScatterArgs()
     for k, (t, rows) in enumerate(dsrcs):
@@ -624,6 +678,12 @@ def embed_scatter_sorted(dy, dtab, sorted_idx, order):
     _req(sorted_idx, torch.int32, "sorted_idx"); _req(order, torch.int32, "order")
     M, H = dy.shape
     _idx_len(sorted_idx, M, "sorted_idx"); _idx_len(order, M, "order")
+    if _ordered():
+        nbytes = LIB.mmfb_embed_scatter_sorted_workspace_bytes(M, H)
+        ws = _workspace(nbytes, dy.device)
+        check(LIB.mmfb_embed_scatter_sorted_ordered(dy.data_ptr(), dy.stride(0), order.data_ptr(), sorted_idx.data_ptr(),
+                                                    dtab.data_ptr(), M, H, ws.data_ptr(), nbytes, _stream_ptr()))
+        return
     check(LIB.mmfb_embed_scatter_sorted(dy.data_ptr(), dy.stride(0), order.data_ptr(), sorted_idx.data_ptr(),
                                         dtab.data_ptr(), M, H, _stream_ptr()))
 

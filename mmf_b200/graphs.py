@@ -10,7 +10,10 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
     counter that the generator mixes into its Philox counter (functional.dropout_epoch): every replay draws fresh masks;
   * gradients: captured with `.grad` unset, so the flat gradient buffers are zeroed inside the graph and the parameters'
     `.grad` are views of them afterwards - an optimizer sees fresh gradients after every replay;
-  * inputs: static device tensors, refreshed by `copy_` on the replay stream (shapes are fixed at capture).
+  * inputs: static device tensors, refreshed by `copy_` on the replay stream (shapes are fixed at capture);
+  * deterministic mode: the graph records the reductions that torch.use_deterministic_algorithms selected AT CAPTURE
+    (mmf_b200.functional reads the flag per call): a step captured under the flag replays the ordered kernels, and one
+    captured without it replays the atomic ones, whatever the flag says at replay.  Capture under the mode you want.
 The reference has no counterpart (its trainer launches eagerly, mmf/trainers/core/training_loop.py:185-213); this is the
 answer to SURVEY.md 8a's "at T = R = 36 everything is launch-bound"."""
 import torch

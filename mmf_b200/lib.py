@@ -35,6 +35,7 @@ class GemmArgs(ctypes.Structure):
         ("splits", ctypes.c_int),
         ("block_n", ctypes.c_int),
         ("cluster", ctypes.c_int),
+        ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_int64),
     ]
 
 
@@ -73,6 +74,7 @@ class LnArgs(ctypes.Structure):
         ("dz", ctypes.c_void_p), ("lddz", ctypes.c_int64),
         ("dgamma", ctypes.c_void_p), ("dbeta", ctypes.c_void_p), ("dbias", ctypes.c_void_p),
         ("M", ctypes.c_int), ("H", ctypes.c_int),
+        ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_int64),
     ]
 
 
@@ -134,6 +136,18 @@ def _load():
     lib.mmfb_launch_count.restype = ctypes.c_int64
     lib.mmfb_colsum.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                                 ctypes.c_void_p]
+    lib.mmfb_colsum_ordered.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                        ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
+    lib.mmfb_embed_scatter_sorted_ordered.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
+                                                      ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                                      ctypes.c_int64, ctypes.c_void_p]
+    lib.mmfb_gemm_workspace_bytes.argtypes = [ctypes.c_int] * 4
+    for name in ("mmfb_layernorm_bwd_workspace_bytes", "mmfb_colsum_workspace_bytes",
+                 "mmfb_embed_scatter_sorted_workspace_bytes"):
+        getattr(lib, name).argtypes = [ctypes.c_int, ctypes.c_int]
+    for name in ("mmfb_gemm_workspace_bytes", "mmfb_layernorm_bwd_workspace_bytes", "mmfb_colsum_workspace_bytes",
+                 "mmfb_embed_scatter_sorted_workspace_bytes"):
+        getattr(lib, name).restype = ctypes.c_int64
     lib.mmfb_dropout_bits.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint64, ctypes.c_uint64,
                                       ctypes.c_float, ctypes.c_void_p]
     lib.mmfb_dropout_bits_epoch.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_void_p,
