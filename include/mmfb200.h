@@ -314,7 +314,9 @@ int mmfb_cast_f32_bf16(const float* in, void* out, int64_t n, mmfb_stream stream
  *           p *= 1 - lr wd;  m += (g-m)(1-b1);  v = b2 v + (1-b2) g^2;  p -= step_size * m / (sqrt(v)/bc2_sqrt + eps)
  *           with step_size = lr/(1-b1^t), bc2_sqrt = sqrt(1-b2^t)
  * `group` (nullable) gives the hyper-parameter group of every 8-element block (parameters are padded to multiples of
- * 8 in the flat buffer); grad_scale multiplies the gradient first (1/loss_scale, clipping coefficient). */
+ * 8 in the flat buffer); grad_scale multiplies the gradient first (1/loss_scale, clipping coefficient).  When
+ * grad_scale_dev is set, the factor is grad_scale * *grad_scale_dev, the fp32 read from DEVICE memory when the kernel
+ * runs (the clip coefficient mmfb_grad_norm writes), so a clipped step needs no device-to-host read. */
 #define MMFB_ADAMW_MAX_GROUPS 8
 typedef struct {
   float* param;
@@ -331,8 +333,41 @@ typedef struct {
   float bc2_sqrt[MMFB_ADAMW_MAX_GROUPS];
   float beta1, beta2, eps, grad_scale;
   int mode;
+  const float* grad_scale_dev;   /* nullable: DEVICE fp32 factor applied on top of grad_scale */
 } mmfb_adamw_args;
 int mmfb_adamw(const mmfb_adamw_args* args, mmfb_stream stream);
+
+/* Global L2 norm of a list of gradient segments and torch's clip coefficient, on the device, in two launches:
+ *   total_norm = sqrt(sum over every element x of every segment of x^2)
+ *   clip_coef  = min(max_norm / (total_norm + 1e-6), 1)   (fp32, as torch.nn.utils.clip_grad_norm_; NaN stays NaN)
+ * out[0] = total_norm, out[1] = clip_coef (DEVICE fp32 [2]); clip_coef is what mmfb_adamw's grad_scale_dev reads.
+ * `segments` is a DEVICE array: segment s covers n elements (fp32 or bf16, contiguous) at ptr and owns the partial-sum
+ * blocks [first_block, first_block + ceil(n / MMFB_GRAD_NORM_BLOCK)); first_block is the running sum of the blocks of the
+ * segments before it and n_blocks the total (the table is not checked on the device).  `partials` is DEVICE fp64
+ * workspace [n_blocks].  Block b sums the squares of its MMFB_GRAD_NORM_BLOCK elements in fp64 in a fixed order into
+ * partials[b]; the second launch adds the partials in a fixed order: no atomics, and the result depends only on the
+ * segment lengths and dtypes, so repeated calls give the same bits in every mode.  The fp32 norm is within one fp32 ulp of
+ * the exact norm.  Non-finite gradients give an inf / NaN norm, as torch's with error_if_nonfinite=False.
+ * norm_type must be 2 (MMFB_ERR_ARG otherwise). */
+#define MMFB_GRAD_NORM_BLOCK 16384
+#define MMFB_GRAD_F32 0
+#define MMFB_GRAD_BF16 1
+typedef struct {
+  const void* ptr;
+  int64_t n;
+  int dtype;                 /* MMFB_GRAD_F32 or MMFB_GRAD_BF16 */
+  int first_block;
+} mmfb_grad_segment;
+typedef struct {
+  const mmfb_grad_segment* segments;   /* DEVICE [n_segments] */
+  int n_segments;
+  int n_blocks;
+  double* partials;                    /* DEVICE fp64 [n_blocks] */
+  float* out;                          /* DEVICE fp32 [2] */
+  float max_norm;
+  float norm_type;
+} mmfb_grad_norm_args;
+int mmfb_grad_norm(const mmfb_grad_norm_args* args, mmfb_stream stream);
 
 /* Optimal-transport distance of word-region alignment (UNITER's WRA loss): cosine cost, the IPOT transport plan and
  * trace(C T) in ONE kernel, one CTA per sample; the gradient through the cosine cost in a second one.  Replaces

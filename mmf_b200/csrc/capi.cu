@@ -261,6 +261,13 @@ int mmfb_adamw(const mmfb_adamw_args* args, mmfb_stream stream) {
   MMFB_REQUIRE_DEVICE();
   return adamw(*args, reinterpret_cast<cudaStream_t>(stream));
 }
+int mmfb_grad_norm(const mmfb_grad_norm_args* args, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_grad_norm: null args");
+  if (args->norm_type != 2.0f)
+    return set_error(MMFB_ERR_ARG, "mmfb_grad_norm: only norm_type 2 is supported (got %g)", args->norm_type);
+  MMFB_REQUIRE_DEVICE();
+  return grad_norm(*args, reinterpret_cast<cudaStream_t>(stream));
+}
 int mmfb_cast_f32_bf16(const float* in, void* out, int64_t n, mmfb_stream stream) {
   if (!in || !out) return set_error(MMFB_ERR_ARG, "mmfb_cast_f32_bf16: null pointer");
   MMFB_REQUIRE_DEVICE();

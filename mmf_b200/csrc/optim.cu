@@ -11,9 +11,12 @@ struct AdamWDev {
   float* p; const float* g; float* m; float* v; bf16* pb; const uint8_t* grp; int64_t n;
   float lr[MMFB_ADAMW_MAX_GROUPS], wd[MMFB_ADAMW_MAX_GROUPS], step[MMFB_ADAMW_MAX_GROUPS], bc2s[MMFB_ADAMW_MAX_GROUPS];
   float b1, b2, eps, gscale;
+  const float* gscale_dev;   // read only by the SCALE_DEV instantiations (a device-side clipping coefficient)
 };
 
-template <int MODE>
+// SCALE_DEV: the gradient factor is gscale * *gscale_dev, read once per thread after the previous kernel has completed.
+// The instantiations without it are the kernels this file always had.
+template <int MODE, bool SCALE_DEV>
 __global__ void __launch_bounds__(256)
 adamw_kernel(const __grid_constant__ AdamWDev a) {
   griddep_launch();
@@ -23,6 +26,7 @@ adamw_kernel(const __grid_constant__ AdamWDev a) {
   if (i >= a.n) return;
   const int gi = a.grp != nullptr ? a.grp[blk] : 0;
   const float lr = a.lr[gi], wd = a.wd[gi], step = a.step[gi], bc2s = a.bc2s[gi];
+  const float gsdev = SCALE_DEV ? a.gscale * *a.gscale_dev : 0.0f;
   float p[8], g[8], m[8], v[8];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -37,7 +41,7 @@ adamw_kernel(const __grid_constant__ AdamWDev a) {
   }
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
-    const float gr = g[e] * a.gscale;
+    const float gr = g[e] * (SCALE_DEV ? gsdev : a.gscale);
     if (MODE == 0) {
       // exp_avg.mul_(b1).add_(g, alpha=1-b1); exp_avg_sq.mul_(b2).addcmul_(g, g, value=1-b2)
       m[e] = __fmaf_rn(gr, 1.0f - a.b1, m[e] * a.b1);
@@ -83,14 +87,158 @@ int adamw(const mmfb_adamw_args& a, cudaStream_t s) {
     const int j = i < a.n_groups ? i : 0;
     d.lr[i] = a.lr[j]; d.wd[i] = a.weight_decay[j]; d.step[i] = a.step_size[j]; d.bc2s[i] = a.bc2_sqrt[j];
   }
-  d.b1 = a.beta1; d.b2 = a.beta2; d.eps = a.eps; d.gscale = a.grad_scale;
+  d.b1 = a.beta1; d.b2 = a.beta2; d.eps = a.eps; d.gscale = a.grad_scale; d.gscale_dev = a.grad_scale_dev;
   const int64_t blocks8 = a.n / 8;
   const unsigned grid = static_cast<unsigned>((blocks8 + 255) / 256);
-  if (a.mode == 0) MMFB_LAUNCH(adamw_kernel<0>, grid, 256, 0, s, d);
-  else MMFB_LAUNCH(adamw_kernel<1>, grid, 256, 0, s, d);
+  if (a.grad_scale_dev != nullptr) {
+    if (a.mode == 0) MMFB_LAUNCH((adamw_kernel<0, true>), grid, 256, 0, s, d);
+    else MMFB_LAUNCH((adamw_kernel<1, true>), grid, 256, 0, s, d);
+  } else {
+    if (a.mode == 0) MMFB_LAUNCH((adamw_kernel<0, false>), grid, 256, 0, s, d);
+    else MMFB_LAUNCH((adamw_kernel<1, false>), grid, 256, 0, s, d);
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw launch: %s", cudaGetErrorString(e));
   count_launch();
+  return MMFB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Global L2 norm of a list of gradient segments (include/mmfb200.h: mmfb_grad_norm), two launches, no atomics.
+// grad_norm_partial_kernel: block b owns elements [c * BLOCK, (c + 1) * BLOCK) (BLOCK = MMFB_GRAD_NORM_BLOCK) of the segment whose first_block <= b
+// is largest, c = b - first_block.  Thread t owns the 8-element groups t, t + 256, ... of that chunk (GN_GROUPS of them)
+// and adds x^2 element by element in fp64; the 256 thread sums are added by a fixed shuffle tree, and the 8 warp sums in
+// warp order, into partial[b].  The element-to-thread map does not depend on alignment (an unaligned or short group is
+// read element by element in the same order), so the order depends on the segment lengths and dtypes alone.
+// grad_norm_final_kernel: one block of 1024 threads; thread t adds partials t, t + 1024, ... in index order, then the same
+// fixed tree.  Squares of fp32 / bf16 values are exact in fp64, so the fp64 sum has a relative error below ~1e-14 for any
+// realistic length, and the fp32 result is a faithful rounding of the exact norm (within one fp32 ulp).
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int GN_THREADS = 256;
+constexpr int GN_GROUPS = MMFB_GRAD_NORM_BLOCK / (GN_THREADS * 8);
+static_assert(GN_GROUPS * GN_THREADS * 8 == MMFB_GRAD_NORM_BLOCK, "grad-norm chunk must be whole 8-element groups");
+constexpr int GN_FINAL_THREADS = 1024;
+
+__device__ __forceinline__ double gn_block_sum(double acc, double* red) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (lane == 0) red[warp] = acc;
+  __syncthreads();
+  double tot = 0.0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) tot += red[w];
+  return tot;
+}
+
+__device__ __forceinline__ double gn_load(const void* p, int dtype, int64_t i) {
+  return dtype == MMFB_GRAD_BF16 ? static_cast<double>(__bfloat162float(static_cast<const bf16*>(p)[i]))
+                                 : static_cast<double>(static_cast<const float*>(p)[i]);
+}
+
+__global__ void __launch_bounds__(GN_THREADS)
+grad_norm_partial_kernel(const mmfb_grad_segment* __restrict__ segs, int n_segs, double* __restrict__ partial) {
+  __shared__ int s_seg;
+  __shared__ double red[GN_THREADS / 32];
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x;
+  if (threadIdx.x == 0) {                         // largest s with first_block <= b (empty segments are skipped over)
+    int lo = 0, hi = n_segs - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (segs[mid].first_block <= b) lo = mid; else hi = mid - 1;
+    }
+    s_seg = lo;
+  }
+  __syncthreads();
+  const mmfb_grad_segment sg = segs[s_seg];
+  const int64_t start = static_cast<int64_t>(b - sg.first_block) * MMFB_GRAD_NORM_BLOCK;
+  const int64_t len = min(static_cast<int64_t>(MMFB_GRAD_NORM_BLOCK), sg.n - start);
+  double acc = 0.0;
+  if (sg.dtype == MMFB_GRAD_BF16) {
+    const bf16* p = static_cast<const bf16*>(sg.ptr) + start;
+    const bool vec = (reinterpret_cast<uintptr_t>(p) & 15) == 0;
+#pragma unroll 4
+    for (int k = 0; k < GN_GROUPS; ++k) {
+      const int64_t j = (static_cast<int64_t>(k) * GN_THREADS + threadIdx.x) * 8;
+      if (j >= len) break;
+      if (vec && j + 8 <= len) {
+        const uint4 u = __ldcs(reinterpret_cast<const uint4*>(p + j));
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float2 f = unpack_bf16x2(w[q]);
+          acc = fma(static_cast<double>(f.x), static_cast<double>(f.x), acc);
+          acc = fma(static_cast<double>(f.y), static_cast<double>(f.y), acc);
+        }
+      } else {
+        for (int64_t e = j; e < min(j + 8, len); ++e) {
+          const double x = gn_load(p, MMFB_GRAD_BF16, e);
+          acc = fma(x, x, acc);
+        }
+      }
+    }
+  } else {
+    const float* p = static_cast<const float*>(sg.ptr) + start;
+    const bool vec = (reinterpret_cast<uintptr_t>(p) & 15) == 0;
+#pragma unroll 4
+    for (int k = 0; k < GN_GROUPS; ++k) {
+      const int64_t j = (static_cast<int64_t>(k) * GN_THREADS + threadIdx.x) * 8;
+      if (j >= len) break;
+      if (vec && j + 8 <= len) {
+        const float4 u = __ldcs(reinterpret_cast<const float4*>(p + j));
+        const float4 v = __ldcs(reinterpret_cast<const float4*>(p + j + 4));
+        const float f[8] = {u.x, u.y, u.z, u.w, v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc = fma(static_cast<double>(f[q]), static_cast<double>(f[q]), acc);
+      } else {
+        for (int64_t e = j; e < min(j + 8, len); ++e) {
+          const double x = gn_load(p, MMFB_GRAD_F32, e);
+          acc = fma(x, x, acc);
+        }
+      }
+    }
+  }
+  const double tot = gn_block_sum(acc, red);
+  if (threadIdx.x == 0) partial[b] = tot;
+}
+
+__global__ void __launch_bounds__(GN_FINAL_THREADS)
+grad_norm_final_kernel(const double* __restrict__ partial, int n_blocks, float max_norm, float* __restrict__ out) {
+  __shared__ double red[GN_FINAL_THREADS / 32];
+  griddep_launch();
+  griddep_wait();
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < n_blocks; i += GN_FINAL_THREADS) acc += partial[i];
+  const double tot = gn_block_sum(acc, red);
+  if (threadIdx.x == 0) {
+    // torch.nn.utils.clip_grad_norm_: clip_coef = max_norm / (total_norm + 1e-6), clamped to at most 1, in fp32; torch
+    // evaluates `float / Tensor` as reciprocal(Tensor) * float, and so does this.  The comparison form keeps a NaN
+    // coefficient NaN (fminf would return 1).
+    const float norm = static_cast<float>(sqrt(tot));
+    const float c = __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), max_norm);
+    out[0] = norm;
+    out[1] = c > 1.0f ? 1.0f : c;
+  }
+}
+
+int grad_norm(const mmfb_grad_norm_args& a, cudaStream_t s) {
+  if (!a.segments || !a.partials || !a.out) return set_error(MMFB_ERR_ARG, "grad_norm: null pointer");
+  if (a.norm_type != 2.0f) return set_error(MMFB_ERR_ARG, "grad_norm: only norm_type 2 is supported (got %g)", a.norm_type);
+  if (a.n_segments < 1 || a.n_blocks < 1)
+    return set_error(MMFB_ERR_ARG, "grad_norm: need at least one segment and one block (got %d, %d)", a.n_segments, a.n_blocks);
+  if (reinterpret_cast<uintptr_t>(a.segments) & 7 || reinterpret_cast<uintptr_t>(a.partials) & 7 ||
+      reinterpret_cast<uintptr_t>(a.out) & 3)
+    return set_error(MMFB_ERR_ARG, "grad_norm: segments / partials must be 8-byte aligned, out 4-byte aligned");
+  MMFB_LAUNCH(grad_norm_partial_kernel, a.n_blocks, GN_THREADS, 0, s, a.segments, a.n_segments, a.partials);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "grad_norm launch: %s", cudaGetErrorString(e));
+  MMFB_LAUNCH(grad_norm_final_kernel, 1, GN_FINAL_THREADS, 0, s, static_cast<const double*>(a.partials), a.n_blocks,
+              a.max_norm, a.out);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "grad_norm launch: %s", cudaGetErrorString(e));
+  count_launch(2);
   return MMFB_OK;
 }
 

@@ -17,7 +17,8 @@ import warnings
 import torch
 
 from . import lib
-from .lib import LIB, AdamWArgs, AttnArgs, ComposeArgs, GemmArgs, LnArgs, OtArgs, ScatterArgs, _ptr, _stream_ptr, check
+from .lib import (LIB, AdamWArgs, AttnArgs, ComposeArgs, GemmArgs, GradNormArgs, LnArgs, OtArgs, ScatterArgs, _ptr, _stream_ptr,
+                  check)
 
 
 def _req(t, dtype, name):
@@ -588,9 +589,11 @@ def gelu_bwd(dh, u):
 
 
 def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, grad_scale=1.0, group_of_block=None,
-          param_bf16=None):
+          param_bf16=None, grad_scale_dev=None):
     """One fused AdamW step over flat fp32 buffers (staged, include/mmfb200.h: mmfb_adamw).
-    groups: list (<= 8) of dicts {lr, weight_decay, step_size, bc2_sqrt}; group_of_block: uint8 [n/8] or None."""
+    groups: list (<= 8) of dicts {lr, weight_decay, step_size, bc2_sqrt}; group_of_block: uint8 [n/8] or None;
+    grad_scale_dev: None or a one-element fp32 CUDA tensor (grad_norm's clip coefficient) multiplied into grad_scale when
+    the kernel runs."""
     for t, n in ((param, "param"), (grad, "grad"), (exp_avg, "exp_avg"), (exp_avg_sq, "exp_avg_sq")):
         _req(t, torch.float32, n)
         if not t.is_contiguous() or t.numel() != param.numel():
@@ -611,7 +614,63 @@ def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, 
     for i, g in enumerate(groups):
         a.lr[i], a.weight_decay[i], a.step_size[i], a.bc2_sqrt[i] = g["lr"], g["weight_decay"], g["step_size"], g["bc2_sqrt"]
     a.beta1, a.beta2, a.eps, a.grad_scale, a.mode = float(beta1), float(beta2), float(eps), float(grad_scale), int(mode)
+    if grad_scale_dev is not None:
+        if not grad_scale_dev.is_cuda or grad_scale_dev.dtype != torch.float32 or grad_scale_dev.numel() != 1:
+            raise ValueError("adamw: grad_scale_dev must be a one-element fp32 CUDA tensor")
+        a.grad_scale_dev = grad_scale_dev.data_ptr()
     check(LIB.mmfb_adamw(ctypes.byref(a), _stream_ptr()))
+
+
+class GradNormTable:
+    """The DEVICE segment table of mmfb_grad_norm over a fixed list of gradient buffers (see grad_norm_table)."""
+
+    def __init__(self, segments, n_segments, n_blocks, device):
+        self.segments, self.n_segments, self.n_blocks, self.device = segments, n_segments, n_blocks, device
+
+
+def grad_norm_table(grads):
+    """Segment table for grad_norm over `grads`: contiguous fp32 or bf16 CUDA tensors, one segment each (empty ones are
+    skipped).  One host-to-device copy from pinned memory, without a stream synchronisation; the table stays valid while
+    the tensors keep their storage, so callers build it once and reuse it."""
+    segs, first = [], 0
+    device = None
+    for g in grads:
+        if not g.is_cuda:
+            raise RuntimeError("grad_norm: gradients must be CUDA tensors: the B200 path has no CPU fallback")
+        if g.dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError("grad_norm: gradients must be fp32 or bf16, got %s" % g.dtype)
+        if not g.is_contiguous():
+            raise ValueError("grad_norm: gradients must be contiguous")
+        if device is not None and g.device != device:
+            raise ValueError("grad_norm: all gradients must be on one device")
+        device = g.device
+        if g.numel() == 0:
+            continue
+        segs.append((g.data_ptr(), g.numel(), lib.MMFB_GRAD_BF16 if g.dtype == torch.bfloat16 else lib.MMFB_GRAD_F32, first))
+        first += (g.numel() + lib.MMFB_GRAD_NORM_BLOCK - 1) // lib.MMFB_GRAD_NORM_BLOCK
+    if not segs:
+        raise ValueError("grad_norm: no non-empty gradient")
+    if first >= 2 ** 31:
+        raise ValueError("grad_norm: too many elements (%d partial-sum blocks)" % first)
+    arr = (lib.GradSegment * len(segs))(*[lib.GradSegment(*s) for s in segs])
+    host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).pin_memory()
+    return GradNormTable(host.to(device, non_blocking=True), len(segs), first, device)
+
+
+def grad_norm(table, max_norm, norm_type=2.0):
+    """Global L2 norm of the gradients of `table` and torch's clip coefficient min(max_norm / (norm + 1e-6), 1), both
+    computed on the device (include/mmfb200.h: mmfb_grad_norm).  Returns fp32 [2] = (total_norm, clip_coef) without a host
+    synchronisation; the summation order is fixed, so the bits repeat in every mode.  Only norm_type 2 is supported."""
+    if float(norm_type) != 2.0:
+        raise ValueError("grad_norm: only norm_type 2 is supported, got %s" % (norm_type,))
+    out = torch.empty(2, dtype=torch.float32, device=table.device)
+    partials = torch.empty(table.n_blocks, dtype=torch.float64, device=table.device)
+    a = GradNormArgs()
+    a.segments, a.n_segments, a.n_blocks = table.segments.data_ptr(), table.n_segments, table.n_blocks
+    a.partials, a.out = partials.data_ptr(), out.data_ptr()
+    a.max_norm, a.norm_type = float(max_norm), float(norm_type)
+    check(LIB.mmfb_grad_norm(ctypes.byref(a), _stream_ptr()))
+    return out
 
 
 def cast_f32_bf16(src, dst):

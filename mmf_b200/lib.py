@@ -96,6 +96,23 @@ class AdamWArgs(ctypes.Structure):
         ("bc2_sqrt", ctypes.c_float * 8),
         ("beta1", ctypes.c_float), ("beta2", ctypes.c_float), ("eps", ctypes.c_float), ("grad_scale", ctypes.c_float),
         ("mode", ctypes.c_int),
+        ("grad_scale_dev", ctypes.c_void_p),
+    ]
+
+
+MMFB_GRAD_NORM_BLOCK = 16384
+MMFB_GRAD_F32, MMFB_GRAD_BF16 = 0, 1
+
+
+class GradSegment(ctypes.Structure):
+    _fields_ = [("ptr", ctypes.c_void_p), ("n", ctypes.c_int64), ("dtype", ctypes.c_int), ("first_block", ctypes.c_int)]
+
+
+class GradNormArgs(ctypes.Structure):
+    _fields_ = [
+        ("segments", ctypes.c_void_p), ("n_segments", ctypes.c_int), ("n_blocks", ctypes.c_int),
+        ("partials", ctypes.c_void_p), ("out", ctypes.c_void_p),
+        ("max_norm", ctypes.c_float), ("norm_type", ctypes.c_float),
     ]
 
 

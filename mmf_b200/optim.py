@@ -8,6 +8,17 @@ that live in an engine ParamPack are updated by ONE kernel over the pack's flat 
 (`mmfb_adamw`: 4 streams read, 3 written, hyper-parameter group looked up per 8-element block); the per-parameter
 `state[p]["exp_avg"]` / `["exp_avg_sq"]` tensors are views of flat state buffers, so `state_dict()` keeps torch's layout.
 Parameters outside any pack (task heads, poolers) fall back to the same arithmetic in torch ops.
+
+Gradient clipping: `clip_grad_norm(max_norm)` is the hook MMF's trainer calls when the optimizer has one
+(mmf/utils/general.py `clip_gradients`, `clip_norm_mode: all`).  The global L2 norm and torch's clip coefficient are
+computed on the device (`mmfb_grad_norm`, one read of the gradients, fixed summation order); the next `step()` multiplies
+every gradient by the coefficient it reads from device memory - inside the AdamW kernel for the packs, as a tensor factor
+on the torch-op path - so nothing waits for the host and the clipped step can be captured in a CUDA graph.
+
+torch.optim.Adam: with arithmetic="torch" and weight_decay=0 the step is torch.optim.Adam's (amsgrad and maximize off):
+AdamW's decoupled decay multiplies the parameter by exactly 1, and the remaining operations - m.lerp_(g, 1-b1),
+v.mul_(b2).addcmul_(g, g, 1-b2), p.addcdiv_(m, sqrt(v)/sqrt(1-b2^t) + eps, -lr/(1-b1^t)) - are Adam's.  Pass Adam's
+eps (1e-8) explicitly: this class defaults to the reference's 1e-6.  That is how M4C's `optimizer.type: Adam` runs here.
 """
 import math
 import weakref
@@ -40,6 +51,8 @@ class B200AdamW(torch.optim.Optimizer):
         super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay,
                                       correct_bias=correct_bias))
         self._flat = {}        # id(pack) -> {"pack": weakref, "m", "v", "groups": uint8 [total/8], "gids": {...}}
+        self._clip_table = None   # (key of the gradient buffers, F.GradNormTable) of clip_grad_norm
+        self._clip_coef = None    # 0-d fp32 CUDA tensor: the coefficient the next step() applies, then drops
 
     # ---------------------------------------------------------------------------------------------------------
     def _group_hp(self, group, step):
@@ -52,11 +65,14 @@ class B200AdamW(torch.optim.Optimizer):
             return {"lr": lr, "weight_decay": wd, "step_size": ss, "bc2_sqrt": 1.0}
         return {"lr": lr, "weight_decay": wd, "step_size": lr / (1.0 - b1 ** step), "bc2_sqrt": math.sqrt(1.0 - b2 ** step)}
 
-    def _torch_update(self, p, g, st, group, grad_scale):
+    def _torch_update(self, p, g, st, group, grad_scale, coef=None):
         """same arithmetic, operation by operation, on one tensor (parameters outside the packs)"""
         b1, b2 = group["betas"]
         hp = self._group_hp(group, st["step"])
-        g = g.float() * grad_scale if grad_scale != 1.0 else g.float()
+        if coef is not None:                           # the kernel's factor: grad_scale * coef in fp32, then g * factor
+            g = g.float() * (coef * grad_scale)
+        else:
+            g = g.float() * grad_scale if grad_scale != 1.0 else g.float()
         m, v, x = st["exp_avg"], st["exp_avg_sq"], p.data
         if self.arithmetic == "transformers":
             m.mul_(b1).add_(g, alpha=1.0 - b1)
@@ -102,13 +118,66 @@ class B200AdamW(torch.optim.Optimizer):
         self._flat[id(pack)] = ent
         return ent
 
+    def _clip_grads(self):
+        """The gradient buffers clip_grad_norm covers, in parameter-group order: a pack's whole flat gradient buffer where
+        the optimizer owns every parameter of the pack and each .grad is its slice (the padding between slices is zero),
+        each other parameter's .grad on its own."""
+        pack_of = {}
+        for pack in list(E.ParamPack._live or ()):
+            for p in pack.params:
+                pack_of[id(p)] = pack
+        owned = {id(p) for g in self.param_groups for p in g["params"]}
+        grads, seen = [], set()
+        for group in self.param_groups:
+            for p in group["params"]:
+                if p.grad is None or id(p) in seen:
+                    continue
+                pack = pack_of.get(id(p))
+                if (pack is not None and pack.dtype == torch.float32 and pack.intact() and
+                        all(id(q) in owned and q.grad is not None and q.grad.dtype == torch.float32 and
+                            q.grad.data_ptr() == gp for q, gp in zip(pack.params, pack._gptrs))):
+                    grads.append(pack.grad)
+                    seen.update(id(q) for q in pack.params)
+                else:
+                    grads.append(p.grad)
+                    seen.add(id(p))
+        return grads
+
+    @torch.no_grad()
+    def clip_grad_norm(self, max_norm, norm_type=2.0):
+        """Clips the gradients of every parameter of the optimizer's groups to a global L2 norm of at most max_norm, as
+        torch.nn.utils.clip_grad_norm_(params, max_norm) does, and returns the norm before clipping as a 0-d fp32 CUDA
+        tensor - without a host synchronisation.  The gradients are not rewritten: the next step() (and only that one)
+        multiplies them by min(max_norm / (norm + 1e-6), 1), so read .grad before the step to see unclipped values.
+        Non-finite gradients give an inf / NaN norm and the same parameters as torch with error_if_nonfinite=False.
+        Only norm_type 2 is supported.  The device table of gradient buffers is rebuilt only when a gradient moves; a
+        step captured in a CUDA graph needs one eager call with the same gradients before the capture."""
+        if float(norm_type) != 2.0:
+            raise ValueError("B200AdamW.clip_grad_norm supports norm_type 2 only, got %s" % (norm_type,))
+        self._clip_coef = None
+        grads = self._clip_grads()
+        if not grads:
+            return torch.tensor(0.0)
+        key = tuple((g.data_ptr(), g.numel(), g.dtype) for g in grads)
+        if self._clip_table is None or self._clip_table[0] != key:
+            if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("B200AdamW.clip_grad_norm: the gradient buffers changed during CUDA-graph capture; "
+                                   "call clip_grad_norm once eagerly with the same gradients before capturing")
+            self._clip_table = (key, F.grad_norm_table(grads))
+        out = F.grad_norm(self._clip_table[1], max_norm, norm_type)
+        self._clip_coef = out[1]
+        return out[0]
+
     @torch.no_grad()
     def step(self, closure=None, grad_scale=1.0):
-        """grad_scale multiplies every gradient first (1 / loss scale, gradient-clipping coefficient)."""
+        """grad_scale multiplies every gradient first (1 / loss scale, gradient-clipping coefficient).  After
+        clip_grad_norm, the gradients are multiplied by grad_scale * (its device-side coefficient) in this step only."""
         loss = None
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
+        coef, self._clip_coef = self._clip_coef, None
+        clip = {} if coef is None else {"grad_scale_dev": coef}
         group_of = {id(p): gi for gi, g in enumerate(self.param_groups) for p in g["params"]}
         done = set()
         mode = 0 if self.arithmetic == "transformers" else 1
@@ -135,7 +204,7 @@ class B200AdamW(torch.optim.Optimizer):
             if ent["frozen"]:
                 hps.append({"lr": 0.0, "weight_decay": 0.0, "step_size": 0.0, "bc2_sqrt": 1.0})
             F.adamw(pack.master, pack.grad, ent["m"], ent["v"], hps, beta1=betas[0], beta2=betas[1], eps=eps, mode=mode,
-                    grad_scale=grad_scale, group_of_block=ent["groups"])
+                    grad_scale=grad_scale, group_of_block=ent["groups"], **clip)
             for p in mine:
                 self.state[p]["step"] += 1
                 done.add(id(p))
@@ -149,9 +218,10 @@ class B200AdamW(torch.optim.Optimizer):
                     st["exp_avg"] = torch.zeros_like(p.data, dtype=torch.float32)
                     st["exp_avg_sq"] = torch.zeros_like(p.data, dtype=torch.float32)
                 st["step"] += 1
-                self._torch_update(p, p.grad, st, group, grad_scale)
+                self._torch_update(p, p.grad, st, group, grad_scale, coef)
         return loss
 
     def load_state_dict(self, state_dict):
         super().load_state_dict(state_dict)
+        self._clip_coef = None
         self._flat = {}                                # re-adopt the loaded per-parameter tensors into flat buffers
