@@ -195,21 +195,29 @@ def vilbert_schedule(v_biattention_id, t_biattention_id, num_t_layers, num_v_lay
     return steps
 
 
-def vilbert_encoder(txt, img, txt_mask, img_mask, sd, prefix, cfg):
-    """ViLBERT BertEncoder.forward, mmf/models/vilbert.py:590-796 (eval-mode dropout; dynamic_attention,
-    in_batch_pairs and FAST_MODE off as in mmf/configs/models/vilbert/defaults.yaml).
+def vilbert_encoder(txt, img, txt_mask, img_mask, sd, prefix, cfg, masks=None, p_t_attn=0.0, p_t_hidden=0.0,
+                    p_v_attn=0.0, p_v_hidden=0.0):
+    """ViLBERT BertEncoder.forward, mmf/models/vilbert.py:590-796 (dynamic_attention, in_batch_pairs and FAST_MODE off
+    as in mmf/configs/models/vilbert/defaults.yaml).
     cfg: dict with num_hidden_layers, v_num_hidden_layers, num_attention_heads, v_num_attention_heads,
-    bi_num_attention_heads, v_biattention_id, t_biattention_id."""
+    bi_num_attention_heads, v_biattention_id, t_biattention_id.
+    masks: optional list of keep-mask dicts, one per step of vilbert_schedule (bert_layer's keys for a text / image layer,
+    connection_layer's for a co-attention layer); p_t_* are the text stream's probabilities (attention_probs_dropout_prob,
+    hidden_dropout_prob), p_v_* the image stream's (v_*)."""
     pre = prefix + "." if prefix else ""
-    for kind, i in vilbert_schedule(cfg["v_biattention_id"], cfg["t_biattention_id"], cfg["num_hidden_layers"],
-                                    cfg["v_num_hidden_layers"]):
+    steps = vilbert_schedule(cfg["v_biattention_id"], cfg["t_biattention_id"], cfg["num_hidden_layers"],
+                             cfg["v_num_hidden_layers"])
+    for j, (kind, i) in enumerate(steps):
+        m = masks[j] if masks else None
         if kind == "t":
-            txt, _ = bert_layer(txt, txt_mask, sd, "%slayer.%d" % (pre, i), cfg["num_attention_heads"])
+            txt, _ = bert_layer(txt, txt_mask, sd, "%slayer.%d" % (pre, i), cfg["num_attention_heads"], m, p_t_attn,
+                                p_t_hidden)
         elif kind == "v":
-            img, _ = bert_layer(img, img_mask, sd, "%sv_layer.%d" % (pre, i), cfg["v_num_attention_heads"])
+            img, _ = bert_layer(img, img_mask, sd, "%sv_layer.%d" % (pre, i), cfg["v_num_attention_heads"], m, p_v_attn,
+                                p_v_hidden)
         else:
             img, txt = connection_layer(img, img_mask, txt, txt_mask, sd, "%sc_layer.%d" % (pre, i),
-                                        cfg["bi_num_attention_heads"])
+                                        cfg["bi_num_attention_heads"], m, p_v_attn, p_t_attn, p_v_hidden, p_t_hidden)
     return txt, img
 
 
@@ -487,34 +495,47 @@ def visual_feat_encoder(feats, boxes, sd, prefix):
     return (x + y) / 2
 
 
-def lxmert_xlayer(lang, lang_mask, visn, visn_mask, sd, prefix, heads):
+def lxmert_xlayer(lang, lang_mask, visn, visn_mask, sd, prefix, heads, masks=None, p_attn=0.0, p_hidden=0.0):
     """LXMERTXLayer.forward, mmf/models/lxmert.py:244-283: ONE cross-attention block (BertCrossattLayer :68-82) used in
-    both directions from the layer inputs, then per-stream self-attention (BertAttention) and FFN."""
+    both directions from the layer inputs, then per-stream self-attention (BertAttention) and FFN.
+    masks: optional dict of keep-masks.  'x_attn_lang' [B,h,T,R] / 'x_attn_visn' [B,h,R,T] on the cross-attention
+    probabilities and 'x_out_lang' [B,T,H] / 'x_out_visn' [B,R,H] in BertAttOutput, per direction (language queries first);
+    'lang' / 'visn': bert_layer's dict ('attn', 'self_out', 'out') for each stream's self-attention and FFN."""
+    m = masks or {}
     ca = prefix + ".visual_attention"
 
-    def cross(x, ctx, ctx_mask):
-        out, _ = bert_self_attention(x, None, sd, ca + ".att", heads, kv=ctx, kv_mask=ctx_mask)
-        return bert_self_output(out, x, sd, ca + ".output")
-    la, va = cross(lang, visn, visn_mask), cross(visn, lang, lang_mask)
+    def cross(x, ctx, ctx_mask, name):
+        out, _ = bert_self_attention(x, None, sd, ca + ".att", heads, m.get("x_attn_" + name), p_attn, kv=ctx,
+                                     kv_mask=ctx_mask)
+        return bert_self_output(out, x, sd, ca + ".output", m.get("x_out_" + name), p_hidden)
+    la, va = cross(lang, visn, visn_mask, "lang"), cross(visn, lang, lang_mask, "visn")
     outs = []
     for x, mask, name in ((la, lang_mask, "lang"), (va, visn_mask, "visn")):
-        ctx, _ = bert_self_attention(x, mask, sd, "%s.%s_self_att.self" % (prefix, name), heads)
-        att = bert_self_output(ctx, x, sd, "%s.%s_self_att.output" % (prefix, name))
+        sm = m.get(name) or {}
+        ctx, _ = bert_self_attention(x, mask, sd, "%s.%s_self_att.self" % (prefix, name), heads, sm.get("attn"), p_attn)
+        att = bert_self_output(ctx, x, sd, "%s.%s_self_att.output" % (prefix, name), sm.get("self_out"), p_hidden)
         inter = bert_intermediate(att, sd, "%s.%s_inter" % (prefix, name))
-        outs.append(bert_self_output(inter, att, sd, "%s.%s_output" % (prefix, name)))
+        outs.append(bert_self_output(inter, att, sd, "%s.%s_output" % (prefix, name), sm.get("out"), p_hidden))
     return outs[0], outs[1]
 
 
-def lxmert_encoder(lang, lang_mask, feats, boxes, visn_mask, sd, prefix, l_layers, x_layers, r_layers, heads):
-    """LXMERTEncoder.forward, mmf/models/lxmert.py:309-336; masks are the additive [B,1,1,S] tensors."""
+def lxmert_encoder(lang, lang_mask, feats, boxes, visn_mask, sd, prefix, l_layers, x_layers, r_layers, heads, masks=None,
+                   p_attn=0.0, p_hidden=0.0):
+    """LXMERTEncoder.forward, mmf/models/lxmert.py:309-336; masks are the additive [B,1,1,S] tensors.
+    masks (keep-masks): optional dict with per-layer lists 'l' and 'r' (bert_layer's dicts) and 'x' (lxmert_xlayer's).
+    The visual feature encoder's own dropout is not modelled (p = 0 there)."""
     pre = prefix + "." if prefix else ""
+    km = masks or {}
     visn = visual_feat_encoder(feats, boxes, sd, pre + "visn_fc")
     for i in range(l_layers):
-        lang, _ = bert_layer(lang, lang_mask, sd, "%slayer.%d" % (pre, i), heads)
+        lang, _ = bert_layer(lang, lang_mask, sd, "%slayer.%d" % (pre, i), heads, km["l"][i] if km else None, p_attn,
+                             p_hidden)
     for i in range(r_layers):
-        visn, _ = bert_layer(visn, visn_mask, sd, "%sr_layers.%d" % (pre, i), heads)
+        visn, _ = bert_layer(visn, visn_mask, sd, "%sr_layers.%d" % (pre, i), heads, km["r"][i] if km else None, p_attn,
+                             p_hidden)
     for i in range(x_layers):
-        lang, visn = lxmert_xlayer(lang, lang_mask, visn, visn_mask, sd, "%sx_layers.%d" % (pre, i), heads)
+        lang, visn = lxmert_xlayer(lang, lang_mask, visn, visn_mask, sd, "%sx_layers.%d" % (pre, i), heads,
+                                   km["x"][i] if km else None, p_attn, p_hidden)
     return lang, visn
 
 
@@ -533,22 +554,26 @@ def vinvl_forward(input_ids, img_feats, attention_mask, sd, num_layers, heads, t
     return bert_encoder(emb, extended_attention_mask(attention_mask, emb.dtype), sd, "encoder", num_layers, heads)
 
 
-def vit_layer(x, add_mask, sd, prefix, heads):
-    """ViTLayer.forward, mmf/modules/vit.py:79-108 (pre-LN block; eval-mode dropout).  ViTAttention = BertSelfAttention on
-    layernorm_before(x) -> ViTSelfOutput.dense (no residual inside, HF modeling_vit) ; the two residuals are added in the
-    layer: h = attn + x (:96), out = output.dense(intermediate(layernorm_after(h))) + h (:99-105)."""
+def vit_layer(x, add_mask, sd, prefix, heads, masks=None, p_attn=0.0, p_hidden=0.0):
+    """ViTLayer.forward, mmf/modules/vit.py:79-108 (pre-LN block).  ViTAttention = BertSelfAttention on
+    layernorm_before(x) -> ViTSelfOutput (dense -> dropout, no residual inside, HF modeling_vit); the two residuals are
+    added in the layer: h = attn + x (:96), out = ViTOutput(intermediate(layernorm_after(h)), h) = dropout(dense(.)) + h
+    (:99-105).  masks: optional dict with keep-masks 'attn' [B,h,S,S], 'self_out' [B,S,H] (ViTSelfOutput) and 'out'
+    [B,S,H] (ViTOutput), as bert_layer's."""
+    m = masks or {}
     a = layer_norm(x, sd, prefix + ".layernorm_before")
-    ctx, _ = bert_self_attention(a, add_mask, sd, prefix + ".attention.attention", heads)
-    h = linear(ctx, sd, prefix + ".attention.output.dense") + x
+    ctx, _ = bert_self_attention(a, add_mask, sd, prefix + ".attention.attention", heads, m.get("attn"), p_attn)
+    h = dropout(linear(ctx, sd, prefix + ".attention.output.dense"), m.get("self_out"), p_hidden) + x
     b = layer_norm(h, sd, prefix + ".layernorm_after")
-    return linear(gelu_erf(linear(b, sd, prefix + ".intermediate.dense")), sd, prefix + ".output.dense") + h
+    y = linear(gelu_erf(linear(b, sd, prefix + ".intermediate.dense")), sd, prefix + ".output.dense")
+    return dropout(y, m.get("out"), p_hidden) + h
 
 
-def vit_encoder(x, add_mask, sd, prefix, num_layers, heads):
-    """ViTEncoder.forward, vit.py:118-175"""
+def vit_encoder(x, add_mask, sd, prefix, num_layers, heads, masks=None, p_attn=0.0, p_hidden=0.0):
+    """ViTEncoder.forward, vit.py:118-175.  masks: optional list of vit_layer's dicts, one per layer."""
     pre = prefix + "." if prefix else ""
     for i in range(num_layers):
-        x = vit_layer(x, add_mask, sd, "%slayer.%d" % (pre, i), heads)
+        x = vit_layer(x, add_mask, sd, "%slayer.%d" % (pre, i), heads, masks[i] if masks else None, p_attn, p_hidden)
     return x
 
 
