@@ -97,7 +97,8 @@ int64_t mmfb_gemm_workspace_bytes(int M, int N, int K, int splits);
  * key k >= P takes 0 when k <= q and -10000 otherwise, in place of mask[b, k], which is not read for those keys.  So the
  * first P queries never see the tail, and query P + t sees tail keys P .. P + t.  0 (what a zero-initialised struct
  * holds) means no tail.  Requires Sq == Skv and T <= Skv; a negative T is MMFB_ERR_ARG, and so is any T != 0 in the
- * packed (varlen) entry points and mmfb_attention_probs.  Every refusal happens before a launch. */
+ * packed (varlen) entry points and mmfb_attention_probs: packed attention with a tail is
+ * mmfb_attention_varlen_causal_fwd / _bwd.  Every refusal happens before a launch. */
 typedef struct {
   const void* q; int64_t ldq;
   const void* k; int64_t ldk;
@@ -133,6 +134,18 @@ int mmfb_attention_bwd(const mmfb_attn_args* args, mmfb_stream stream);
  * Limits: head_dim 64 or 128; max_len <= 384 (d=64) / 256 (d=128).  total = 0 returns MMFB_OK without a launch. */
 int mmfb_attention_varlen_fwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream);
 int mmfb_attention_varlen_bwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream);
+
+/* Variable-length (packed) self-attention with a causal tail: the packing of mmfb_attention_varlen_fwd / _bwd (same
+ * arguments, buffers and keep-bit layout) with causal_len = T, the packed form of M4C's prefix-LM mask.  The tail of
+ * sample b is its last T rows: with len_b = cu_seqlens[b+1] - cu_seqlens[b] and P_b = max(len_b - T, 0), counted within
+ * the sample, key k >= P_b takes 0 for queries q >= k and -10000 for the others (the dense causal rule with len_b in
+ * place of Skv), and keys below P_b take 0.  The lengths are read on the device only, so a sample shorter than T is all
+ * tail.  Each sample computes bit for bit what mmfb_attention_fwd / _bwd compute for it alone (B = 1, Sq = Skv = len_b,
+ * mask NULL, causal_len = min(T, len_b)).
+ * Requires 0 < causal_len <= max_len, Sq == Skv == max_len, mask == NULL and a non-null cu_seqlens; any other call is
+ * MMFB_ERR_ARG before a launch.  total = 0 returns MMFB_OK without a launch.  Limits as mmfb_attention_varlen_fwd. */
+int mmfb_attention_varlen_causal_fwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream);
+int mmfb_attention_varlen_causal_bwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream);
 
 /* Variable-length (packed) cross-attention: the queries come from one packed stream and the keys / values from another
  * (ViLBERT co-attention, LXMERT cross-modality layers).  cu_q, cu_kv: int32 [B+1] on the DEVICE, each a non-decreasing

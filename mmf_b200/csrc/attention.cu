@@ -32,6 +32,11 @@
 // otherwise (the staged mask holds 0 there, mask[b, k] is not read); keys below P keep the additive mask.  No key block is
 // skipped: M4C's tails (12 / 30 keys) sit inside one 64-key block, and every value stays finite, so a query whose other
 // keys are all padding still gets the softmax of its raw scores, as in the reference.
+// VARLEN && CAUSAL instantiations (packed self-attention with causal_len = T > 0, attention_varlen_causal.cu): the tail of
+// sample b is its last T rows, from P_b = max(len_b - T, 0) on (counted within the sample; a sample shorter than T is all
+// tail), found from cu after griddep_wait.  The rule is CAUSAL's with len_b in place of Skv: a tail key k takes 0 for
+// queries q >= k and -10000 otherwise, keys below P_b take 0 (packing has removed the padded ones), and keys past the end
+// of the sample keep the packed mode's -inf.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -117,7 +122,8 @@ struct AttnFwdDev {
   int total;              // VARLEN: packed query rows
   const int* cu_kv;       // VARLEN: [B+1] first packed key row of every sample (Skv = max_kv; self-attention: cu)
   int total_kv;           // VARLEN: packed key rows
-  int P;                  // CAUSAL: first key of the causal tail (Skv - causal_len)
+  int P;                  // CAUSAL: first key of the causal tail (Skv - causal_len); VARLEN && CAUSAL: Skv = max_len, and
+                          // the kernels take causal_len = Skv - P to find each sample's own tail
 };
 
 // VARLEN: sample b owns the packed rows [cu[b], cu[b+1]) of one side's row buffers (clamped to [0, total] and to max_len
@@ -127,6 +133,10 @@ __device__ __forceinline__ int2 varlen_rows(const int* cu, int b, int total, int
   const int s0 = min(max(__ldg(cu + b), 0), total);
   return make_int2(s0, max(min(min(__ldg(cu + b + 1), total) - s0, max_len), 0));
 }
+
+// VARLEN && CAUSAL: the first key of the causal tail of a sample of `len` rows, within the sample: its last Skv - P rows
+// (the causal_len), all of them when it is shorter.
+__device__ __forceinline__ int varlen_tail(int len, int P, int Skv) { return max(len - (Skv - P), 0); }
 
 // PACKED_ROW / PACKED_KV_ROW: tile row coordinate of a query / key tile (dense: within batch b; packed: sample b starts at
 // query row seq0 and key row kv0).
@@ -169,6 +179,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   // dense: the sample's rows start at row 0 of batch b; VARLEN: at packed query row seq0 / key row kv0 of the single batch
   int seq0 = 0, len = p.Skv, nkb = NKB;
   int kv0 = 0, kvlen = p.Skv;
+  int tail0 = 0;                               // VARLEN && CAUSAL: first tail key of this sample
   if constexpr (VARLEN) {
     const int2 r = varlen_rows(p.cu, b, p.total, p.Sq);
     seq0 = r.x;
@@ -178,6 +189,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     kv0 = rk.x;
     kvlen = rk.y;
     nkb = (kvlen + AT_ROWS - 1) / AT_ROWS;     // the sample's own key blocks only (none without keys)
+    if constexpr (CAUSAL) tail0 = varlen_tail(kvlen, p.P, p.Skv);
   }
   const int tb = VARLEN ? 0 : b;
   if (threadIdx.x == 0) {
@@ -234,7 +246,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         float m = (e & 1) ? mk.y : mk.x;
-        if constexpr (CAUSAL) m = causal_mask(m, q0 + r0 + g + (e >> 1) * 8, kb * AT_ROWS + nt * 8 + 2 * t4 + (e & 1), p.P, p.Skv);
+        if constexpr (CAUSAL)
+          m = causal_mask(m, q0 + r0 + g + (e >> 1) * 8, kb * AT_ROWS + nt * 8 + 2 * t4 + (e & 1), VARLEN ? tail0 : p.P,
+                          VARLEN ? kvlen : p.Skv);
         s[nt][e] = fmaf(s[nt][e], p.scale2, m);
         bmax[e >> 1] = fmaxf(bmax[e >> 1], s[nt][e]);
       }
@@ -369,6 +383,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   griddep_wait();
   int seq0 = 0, len = p.Skv, nkb = NKB;
   int kv0 = 0, kvlen = p.Skv;
+  int tail0 = 0;
   if constexpr (VARLEN) {
     const int2 r = varlen_rows(p.cu, b, p.total, p.Sq);
     seq0 = r.x;
@@ -378,6 +393,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     kv0 = rk.x;
     kvlen = rk.y;
     nkb = (kvlen + AT_ROWS - 1) / AT_ROWS;
+    if constexpr (CAUSAL) tail0 = varlen_tail(kvlen, p.P, p.Skv);
   }
   const int tb = VARLEN ? 0 : b;
   if (threadIdx.x == 0) {
@@ -447,7 +463,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       for (int e = 0; e < 4; ++e) {
         const int hr = e >> 1;
         float m = (e & 1) ? mk.y : mk.x;
-        if constexpr (CAUSAL) m = causal_mask(m, q0 + r0 + g + hr * 8, kb * AT_ROWS + nt * 8 + 2 * t4 + (e & 1), p.P, p.Skv);
+        if constexpr (CAUSAL)
+          m = causal_mask(m, q0 + r0 + g + hr * 8, kb * AT_ROWS + nt * 8 + 2 * t4 + (e & 1), VARLEN ? tail0 : p.P,
+                          VARLEN ? kvlen : p.Skv);
         const float pe = ex2_approx(fmaf(s[nt][e], p.scale2, m) - lse[hr]);
         float dpe = dp[nt][e];
         if (DROP) {
@@ -517,6 +535,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
   griddep_wait();
   int seq0 = 0, len = p.Skv, nqb = NQB;
   int kv0 = 0, kvlen = p.Skv;
+  int tail0 = 0;
   if constexpr (VARLEN) {
     const int2 rk = varlen_rows(p.cu_kv, b, p.total_kv, p.Skv);
     kv0 = rk.x;
@@ -526,6 +545,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
     seq0 = r.x;
     len = r.y;
     nqb = (len + QB - 1) / QB;                  // the sample's own query blocks only (none without queries)
+    if constexpr (CAUSAL) tail0 = varlen_tail(kvlen, p.P, p.Skv);
   }
   const int tb = VARLEN ? 0 : b;
   if (threadIdx.x == 0) {
@@ -590,7 +610,7 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
         for (int hr = 0; hr < 2; ++hr) {
           const int e = hr * 2 + j;
           float m = mk[hr];
-          if constexpr (CAUSAL) m = causal_mask(m, q, k0 + r0 + g + hr * 8, p.P, p.Skv);
+          if constexpr (CAUSAL) m = causal_mask(m, q, k0 + r0 + g + hr * 8, VARLEN ? tail0 : p.P, VARLEN ? kvlen : p.Skv);
           const float pe = ex2_approx(fmaf(s[nt][e], p.scale2, m) - lse);
           const bool keep = !DROP || ((w >> (ksh0 + hr * 8)) & 1u);
           const float dpe = keep ? dp[nt][e] * p.dscale : 0.0f;
@@ -633,7 +653,8 @@ attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_consta
 // elements is owned by D/8 consecutive lanes and reduced with shuffles (coalesced 512 B / 1 KB per warp access).
 // Every row is a query row of some sample, so the packed layout [H, total] is this kernel's own with B = 1, Sq = total:
 // the varlen backward launches it unchanged (it is defined once, in the dense translation unit).
-#if defined(MMFB_ATTN_VARLEN_TU) || defined(MMFB_ATTN_PROBS_TU) || defined(MMFB_ATTN_CAUSAL_TU)
+#if defined(MMFB_ATTN_VARLEN_TU) || defined(MMFB_ATTN_PROBS_TU) || defined(MMFB_ATTN_CAUSAL_TU) || \
+    defined(MMFB_ATTN_VARLEN_CAUSAL_TU)
 __global__ void attn_delta_kernel(const bf16* __restrict__ dO, int64_t ld_do, const bf16* __restrict__ O,
                                   int64_t ld_o, const bf16* __restrict__ Olo, float* __restrict__ delta, int B, int H,
                                   int Sq, int D);
@@ -686,7 +707,7 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ dO, int64_t ld_do, co
   }
 }
 
-#endif  // MMFB_ATTN_VARLEN_TU || MMFB_ATTN_PROBS_TU || MMFB_ATTN_CAUSAL_TU
+#endif  // MMFB_ATTN_VARLEN_TU || MMFB_ATTN_PROBS_TU || MMFB_ATTN_CAUSAL_TU || MMFB_ATTN_VARLEN_CAUSAL_TU
 
 // ----------------------------------------------------------------------------------------------
 // host
@@ -856,10 +877,12 @@ static int attn_bwd_launch(const mmfb_attn_args& a, const int32_t* cu, int total
 }
 
 // The dense entry points instantiate the dense kernels only, attention_varlen.cu (which includes this file) the packed
-// ones and attention_causal.cu the dense ones with a causal tail: instantiated in one translation unit, they share inlined
-// helpers that the compiler then schedules differently, and the dense d = 64 forward would not keep the code it has
-// without the other modes.  attention_probs.cu includes this file for its helpers only and instantiates none.
-#if !defined(MMFB_ATTN_VARLEN_TU) && !defined(MMFB_ATTN_PROBS_TU) && !defined(MMFB_ATTN_CAUSAL_TU)
+// ones, attention_causal.cu the dense ones with a causal tail and attention_varlen_causal.cu the packed ones with a causal
+// tail: instantiated in one translation unit, they share inlined helpers that the compiler then schedules differently,
+// and the dense d = 64 forward would not keep the code it has without the other modes.  attention_probs.cu includes this
+// file for its helpers only and instantiates none.
+#if !defined(MMFB_ATTN_VARLEN_TU) && !defined(MMFB_ATTN_PROBS_TU) && !defined(MMFB_ATTN_CAUSAL_TU) && \
+    !defined(MMFB_ATTN_VARLEN_CAUSAL_TU)
 int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream) {
   int rc = check_attn_common(a, "attn_fwd");
   if (rc) return rc;
@@ -966,6 +989,39 @@ int attn_causal_bwd(const mmfb_attn_args& a, cudaStream_t stream) {
   return a.head_dim == 64 ? attn_bwd_launch<64, false, true>(a, nullptr, 0, nullptr, 0, stream)
                           : attn_bwd_launch<128, false, true>(a, nullptr, 0, nullptr, 0, stream);
 }
-#endif  // MMFB_ATTN_VARLEN_TU / MMFB_ATTN_CAUSAL_TU
+#elif defined(MMFB_ATTN_VARLEN_CAUSAL_TU)
+
+// Packed self-attention with a causal tail: the packed entry points' arguments, and 0 < causal_len <= max_len (the
+// lengths are device data, so a sample shorter than the tail is all tail, see varlen_tail).
+static int check_varlen_causal(const mmfb_attn_args& a, const int32_t* cu, int total, const char* who) {
+  int rc = check_attn_common(a, who);     // also: Sq == Skv and causal_len <= Skv when causal_len > 0
+  if (rc) return rc;
+  if (a.causal_len <= 0)
+    return set_error(MMFB_ERR_ARG, "%s: causal_len must be in [1, max_len=%d] (got %d)", who, a.Skv, a.causal_len);
+  if (a.mask != nullptr) return set_error(MMFB_ERR_ARG, "%s: mask must be NULL (packing has removed the masked keys)", who);
+  if (!cu) return set_error(MMFB_ERR_ARG, "%s: null cu_seqlens", who);
+  if (total < 0) return set_error(MMFB_ERR_ARG, "%s: negative total (%d)", who, total);
+  return MMFB_OK;
+}
+
+int attn_varlen_causal_fwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream) {
+  int rc = check_varlen_causal(a, cu, total, "attn_varlen_causal_fwd");
+  if (rc) return rc;
+  if (total == 0) return MMFB_OK;
+  if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2) return set_error(MMFB_ERR_ARG, "attn_varlen_causal_fwd: null pointer");
+  return a.head_dim == 64 ? attn_fwd_launch<64, true, true>(a, cu, total, cu, total, stream)
+                          : attn_fwd_launch<128, true, true>(a, cu, total, cu, total, stream);
+}
+
+int attn_varlen_causal_bwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream) {
+  int rc = check_varlen_causal(a, cu, total, "attn_varlen_causal_bwd");
+  if (rc) return rc;
+  if (total == 0) return MMFB_OK;
+  if (!a.q || !a.k || !a.v || !a.ctx || !a.lse2 || !a.dctx || !a.delta || !a.dq || !a.dk || !a.dv)
+    return set_error(MMFB_ERR_ARG, "attn_varlen_causal_bwd: null pointer");
+  return a.head_dim == 64 ? attn_bwd_launch<64, true, true>(a, cu, total, cu, total, stream)
+                          : attn_bwd_launch<128, true, true>(a, cu, total, cu, total, stream);
+}
+#endif  // MMFB_ATTN_VARLEN_TU / MMFB_ATTN_CAUSAL_TU / MMFB_ATTN_VARLEN_CAUSAL_TU
 
 }  // namespace mmfb

@@ -148,6 +148,18 @@ int mmfb_attention_varlen_bwd(const mmfb_attn_args* args, const int32_t* cu_seql
   return attn_varlen_bwd(*args, cu_seqlens, total, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int mmfb_attention_varlen_causal_fwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_attention_varlen_causal_fwd: null args");
+  MMFB_REQUIRE_DEVICE();
+  return attn_varlen_causal_fwd(*args, cu_seqlens, total, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int mmfb_attention_varlen_causal_bwd(const mmfb_attn_args* args, const int32_t* cu_seqlens, int total, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_attention_varlen_causal_bwd: null args");
+  MMFB_REQUIRE_DEVICE();
+  return attn_varlen_causal_bwd(*args, cu_seqlens, total, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int mmfb_attention_varlen_cross_fwd(const mmfb_attn_args* args, const int32_t* cu_q, int total_q, const int32_t* cu_kv,
                                     int total_kv, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_attention_varlen_cross_fwd: null args");

@@ -79,6 +79,9 @@ int attn_probs(const mmfb_attn_args& a, void* probs, int probs_dtype, cudaStream
 // dense self-attention with a causal tail (attention_causal.cu), called by attn_fwd / attn_bwd after their checks
 int attn_causal_fwd(const mmfb_attn_args& a, cudaStream_t stream);
 int attn_causal_bwd(const mmfb_attn_args& a, cudaStream_t stream);
+// packed self-attention with a causal tail (attention_varlen_causal.cu)
+int attn_varlen_causal_fwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream);
+int attn_varlen_causal_bwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream);
 int ln_fwd(const mmfb_ln_args& a, cudaStream_t s);
 int ln_bwd(const mmfb_ln_args& a, cudaStream_t s);
 int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s);

@@ -228,7 +228,7 @@ def attention_probs(q, k, lse2, B, heads, Sq, Skv, mask=None, drop_mask=None, dr
     return out
 
 
-def _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale):
+def _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale, causal_len=0):
     """packed self-attention operands: q/k/v [total, h*d] rows of B samples delimited by cu_seqlens (int32 [B+1])"""
     if not isinstance(cu_seqlens, torch.Tensor) or cu_seqlens.dtype != torch.int32:
         raise ValueError("cu_seqlens must be an int32 tensor")
@@ -259,14 +259,19 @@ def _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale):
             raise ValueError("attention_varlen: drop_mask must be contiguous int32 [heads, total, ceil(max_len/32)]")
         a.drop_mask, a.drop_scale = drop_mask.data_ptr(), float(drop_scale)
     a.B, a.heads, a.Sq, a.Skv, a.head_dim = B, heads, max_len, max_len, W // heads
+    a.causal_len = int(causal_len)
     return a, total, W
 
 
-def attention_varlen_fwd(q, k, v, cu_seqlens, max_len, heads, drop_mask=None, drop_scale=1.0, out=None, save_lo=False):
+def attention_varlen_fwd(q, k, v, cu_seqlens, max_len, heads, drop_mask=None, drop_scale=1.0, out=None, save_lo=False,
+                         causal_len=0):
     """Packed self-attention: ctx, lse2 (, ctx_lo).  Sample b is rows [cu_seqlens[b], cu_seqlens[b+1]) of q/k/v
     [total, h*d] (views allowed) and attends to its own rows only; max_len bounds every length.  lse2 is fp32
-    [heads, total].  The lengths stay on the device: nothing here synchronises."""
-    a, total, W = _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale)
+    [heads, total].  The lengths stay on the device: nothing here synchronises.
+    causal_len = T > 0: the last T rows of every sample are a causal tail - with P_b = max(len_b - T, 0) within the
+    sample, key k >= P_b takes 0 for queries q >= k and -10000 for the others (attention_fwd's rule with len_b in place of
+    Skv; a sample shorter than T is all tail).  0 = none."""
+    a, total, W = _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale, causal_len)
     ctx = out if out is not None else torch.empty(total, W, dtype=torch.bfloat16, device=q.device)
     _req(ctx, torch.bfloat16, "out")
     lse2 = torch.empty(heads, total, dtype=torch.float32, device=q.device)
@@ -275,16 +280,18 @@ def attention_varlen_fwd(q, k, v, cu_seqlens, max_len, heads, drop_mask=None, dr
     if save_lo:
         ctx_lo = torch.empty(total, W, dtype=torch.bfloat16, device=q.device)
         a.ctx_lo = ctx_lo.data_ptr()
-    check(LIB.mmfb_attention_varlen_fwd(ctypes.byref(a), cu_seqlens.data_ptr(), total, _stream_ptr()))
+    fn = LIB.mmfb_attention_varlen_causal_fwd if a.causal_len else LIB.mmfb_attention_varlen_fwd
+    check(fn(ctypes.byref(a), cu_seqlens.data_ptr(), total, _stream_ptr()))
     if save_lo:
         return ctx, lse2, ctx_lo
     return ctx, lse2
 
 
 def attention_varlen_bwd(dctx, q, k, v, ctx, lse2, cu_seqlens, max_len, heads, drop_mask=None, drop_scale=1.0,
-                         dq=None, dk=None, dv=None, ctx_lo=None):
-    """dq, dk, dv of attention_varlen_fwd (packed rows, probabilities recomputed from the saved lse2 [heads, total])."""
-    a, total, W = _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale)
+                         dq=None, dk=None, dv=None, ctx_lo=None, causal_len=0):
+    """dq, dk, dv of attention_varlen_fwd (packed rows, probabilities recomputed from the saved lse2 [heads, total]).
+    causal_len: the forward's."""
+    a, total, W = _varlen_args(q, k, v, cu_seqlens, max_len, heads, drop_mask, drop_scale, causal_len)
     _req(dctx, torch.bfloat16, "dctx")
     _req(ctx, torch.bfloat16, "ctx")
     if dctx.shape[0] != total or ctx.shape[0] != total:
@@ -307,7 +314,8 @@ def attention_varlen_bwd(dctx, q, k, v, ctx, lse2, cu_seqlens, max_len, heads, d
     a.dq, a.ld_dq = dq.data_ptr(), dq.stride(0)
     a.dk, a.ld_dk = dk.data_ptr(), dk.stride(0)
     a.dv, a.ld_dv = dv.data_ptr(), dv.stride(0)
-    check(LIB.mmfb_attention_varlen_bwd(ctypes.byref(a), cu_seqlens.data_ptr(), total, _stream_ptr()))
+    fn = LIB.mmfb_attention_varlen_causal_bwd if a.causal_len else LIB.mmfb_attention_varlen_bwd
+    check(fn(ctypes.byref(a), cu_seqlens.data_ptr(), total, _stream_ptr()))
     return dq, dk, dv
 
 

@@ -179,7 +179,8 @@ def _load():
     lib.mmfb_dropout_apply.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_float,
                                        ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     lib.mmfb_cast_f32_bf16.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
-    for name in ("mmfb_attention_varlen_fwd", "mmfb_attention_varlen_bwd"):
+    for name in ("mmfb_attention_varlen_fwd", "mmfb_attention_varlen_bwd", "mmfb_attention_varlen_causal_fwd",
+                 "mmfb_attention_varlen_causal_bwd"):
         getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
     for name in ("mmfb_attention_varlen_cross_fwd", "mmfb_attention_varlen_cross_bwd"):
         getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,

@@ -27,6 +27,19 @@ the dropouts of the object / OCR encodings, the gather of the previous predictio
 pointer network's [B, dec, ocr] score product (a batched product, about 1.5 MFLOP per sample at TextVQA shapes: the GEMM
 ABI has no batch) and its mask, the argmax of greedy decoding and the loss `m4c_decoding_bce_with_mask`.
 
+Skip-padding (`patch.set_skip_padding(model, causal=True)`): the text BERT packs its valid question tokens, and the MMT
+call packs the valid text, object and OCR rows plus every decoding step, and runs the packed attention kernels with the
+causal tail.  The padded MMT rows then come out as exact zeros instead of the dense values.  This changes neither the loss
+nor a parameter gradient beyond rounding and the dropout masks drawn:
+  * the only padded MMT rows any consumer reads are the OCR rows, which B200OcrPtrNet scores with -10000 added (its
+    key projection of a zero row is its bias, so both paths give a score near -10000 there);
+  * m4c_decoding_bce_with_mask gives such a logit x, whose target is 0, the loss log1p(exp(x)) and the gradient
+    sigmoid(x), both exactly 0 in fp32, so nothing flows back into those rows;
+  * every valid row and every decoding step has at least one unmasked key, so the dense path gives each padded key
+    (mask -10000) a softmax weight of exactly 0 in fp32 - the keys packing removes.
+So the returned `scores` differ only at padded OCR slots, where both paths are near -10000, and greedy decoding picks the
+same tokens unless two valid scores tie within rounding.  (With `causal=False`, skip_padding packs the text BERT only.)
+
 There is no hub: `text_bert_init_from_bert_base: true` selects the bert-base hyper-parameters (BertConfig's defaults
 under `text_bert`) and puts the text BERT in its own learning-rate group, as the reference does; its weights, and the
 fc7 weights and biases the reference reads from detectron pickles, arrive through load_state_dict.

@@ -106,6 +106,8 @@ class EncoderRunner(_LayerStack):
         super().__init__(self.layers, [self.W] * len(self.layers))
         # skip padded tokens: pack the valid rows once per encoder call and run variable-length attention (run_bert_encoder)
         self.skip_padding = False
+        # with skip_padding: also pack calls with a causal tail (M4C's multimodal transformer), keeping every tail row
+        self.pack_tail = False
 
     def forward(self, x, add_mask, training, need_grad, probs=None):
         """probs: an engine.ProbsSink that receives every layer's attention probabilities, or None"""
@@ -189,6 +191,14 @@ def _plan_packing(mask, B, S, counts=None):
     rows = torch.empty(total + 1, dtype=torch.int64, device=mask.device)
     rows.scatter_(0, dest, torch.arange(B * S, device=mask.device))     # padded rows all land in the spare last slot
     return _Packing(rows[:total], E.Varlen(cu, B, total, max_len))
+
+
+def _tail_kept(mask, causal_len):
+    """the key-padding mask of a call with a causal tail, as packing reads it: the mask before the tail, and 0 (kept) on
+    the last causal_len positions, which the dense path does not read the mask at either"""
+    m = mask.clone()
+    m[:, mask.shape[1] - causal_len:] = 0.0
+    return m
 
 
 def _trivial_packing(B, S, device):
@@ -294,8 +304,10 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
     """hidden_states [B,S,H] (fp32 or bf16), attention_mask additive [B,1,1,S] / [B,S] / None.
     causal_len = T > 0 makes the last T positions a causal tail (engine.CausalTail, M4C's prefix-LM mask): every query
     attends to the keys before the tail that attention_mask keeps, the first S - T queries to no tail key, and tail query t
-    to tail keys 0..t; attention_mask is not read for the tail keys.  Such a call runs the dense path even with skip_padding
-    set, and cannot return probabilities.
+    to tail keys 0..t; attention_mask is not read for the tail keys.  Such a call cannot return probabilities.  With
+    skip_padding alone it runs the dense path; with skip_padding and runner.pack_tail it packs the rows before the tail
+    that attention_mask keeps plus every tail row (so the tail is the last T packed rows of each sample) and runs the
+    packed kernels with the tail, unless no row before the tail is padded (then it runs the dense path).
     Returns (last,), then the L layer inputs if output_hidden_states, then the L layers' attention probabilities
     [B, heads, S, S] (hidden-state dtype, post-dropout in training) if output_attentions.  The hidden states and
     probabilities are outputs for inspection: they carry no gradient, so a loss that reads them back-propagates nothing
@@ -313,7 +325,14 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
     if causal_len:
         if not 0 < causal_len <= S:
             raise ValueError("causal_len must be in [0, S=%d], got %d" % (S, causal_len))
-        mask = E.CausalTail(mask, causal_len)
+        packing = None
+        if runner.skip_padding and runner.pack_tail and mask is not None and not output_attentions:
+            packing = _plan_packing(_tail_kept(mask, causal_len), B, S)     # never empty: the tail rows stay
+        if packing is not None:
+            packing.varlen.causal_len = causal_len
+            mask = packing
+        else:
+            mask = E.CausalTail(mask, causal_len)
     elif runner.skip_padding and mask is not None and not output_attentions:
         packing = _plan_packing(mask, B, S)
         if packing is not None and packing.varlen.total == 0:

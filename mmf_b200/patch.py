@@ -7,7 +7,8 @@ re-homed into the engine's flat pack on the first CUDA forward.
 
 `set_skip_padding()` switches the single-stream encoders of a model to packed execution: padded tokens are removed once
 per encoder call and attention runs over each sample's own tokens (variable-length kernels), so padding costs nothing.
-With `two_stream=True` it also packs both streams of the ViLBERT and LXMERT encoders (variable-length cross-attention).
+With `two_stream=True` it also packs both streams of the ViLBERT and LXMERT encoders (variable-length cross-attention),
+and with `causal=True` the calls with a causal tail (M4C's multimodal transformer: variable-length attention with a tail).
 """
 import types
 
@@ -71,12 +72,14 @@ def _routed(m):
     return getattr(f, "__func__", f) is _b200_encoder_forward
 
 
-def set_skip_padding(module, enabled=True, two_stream=False):
+def set_skip_padding(module, enabled=True, two_stream=False, causal=False):
     """Sets `skip_padding` on every single-stream encoder runner under `module` (B200BertEncoder - and so VisualBERT, MMBT,
     UNITER, VinVL and the TransformerEncoder plugin -, VisualBERT's bypass `additional_layer`, encoders routed by
     attach_encoder / replace_with_b200) and returns how many it set.  ViLBERT, LXMERT and ViT runners are left alone unless
     `two_stream` is True: then `pack_streams` is set on every ViLBERT and LXMERT runner too, and they count as well.  ViT
-    runners are always left alone.
+    runners are always left alone.  With `causal` True, `pack_tail` is set as well on the single-stream runners (it counts
+    nothing extra): their calls with a causal tail (run_bert_encoder's causal_len, the multimodal transformer of `m4c` and
+    `m4c_captioner`) then pack too, keeping every tail row.  Without it such calls run the dense path.
 
     With the flag on, an encoder call with a key-padding mask runs on the valid rows only: its outputs (and the input
     gradient) are exactly zero at padded positions instead of the values the dense path computes there.  For any loss that
@@ -100,6 +103,8 @@ def set_skip_padding(module, enabled=True, two_stream=False):
             r = _runner_of(m)
         if type(r) is EncoderRunner:
             r.skip_padding = bool(enabled)
+            if causal:
+                r.pack_tail = bool(enabled)
             n += 1
         elif two_stream and isinstance(r, TwoStreamRunner):
             r.pack_streams = bool(enabled)
