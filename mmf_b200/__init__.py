@@ -37,6 +37,7 @@ _LAZY = {
     "MMFTransformer": ("mmft", "MMFTransformer"),
     "UNITER": ("uniter_model", "UNITER"),
     "VinVL": ("vinvl_model", "VinVL"),
+    "ViLT": ("vilt_model", "ViLT"),
     "M4C": ("m4c_model", "M4C"),
     "M4CCaptioner": ("m4c_model", "M4CCaptioner"),
     "build_model": ("models", "build_model"),

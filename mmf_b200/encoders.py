@@ -3,6 +3,7 @@
   B200FinetuneFasterRcnnFpnFc7  <->  FinetuneFasterRcnnFpnFc7   mmf/modules/encoders.py:116-180   relu(Linear(feat))
   B200IdentityEncoder           <->  IdentityEncoder            mmf/modules/encoders.py:183-198
   B200TransformerEncoder        <->  TransformerEncoder         mmf/modules/encoders.py:513-585   BertModelJit wrapper
+  B200ViTImageEncoder           <->  ViTEncoder                 mmf/modules/encoders.py:830-857   ViTModel wrapper (`vit`)
 
 The reference builds these through `build_encoder({type, params})` (mmf/utils/build.py:517-546); here the classes are
 registered with `registry.register_encoder(name)` in the shim and take the same config keys.
@@ -92,6 +93,21 @@ class _BertModel(nn.Module):
         return seq, self.pooler(seq), ()
 
 
+def transformer_hparams(config):
+    """the BERT hyper-parameters TransformerEncoder resolves from its config keys (AutoConfig.from_pretrained(bert_model_name,
+    **config), encoders.py:576-579): bert-base, overridden by the keys the config carries"""
+    import types
+    return types.SimpleNamespace(
+        hidden_size=_get(config, "hidden_size", 768), num_hidden_layers=_get(config, "num_hidden_layers", 12),
+        num_attention_heads=_get(config, "num_attention_heads", 12),
+        intermediate_size=_get(config, "intermediate_size", 4 * _get(config, "hidden_size", 768)),
+        vocab_size=_get(config, "vocab_size", 30522), max_position_embeddings=_get(config, "max_position_embeddings", 512),
+        type_vocab_size=_get(config, "type_vocab_size", 2), hidden_dropout_prob=_get(config, "hidden_dropout_prob", 0.1),
+        attention_probs_dropout_prob=_get(config, "attention_probs_dropout_prob", 0.1),
+        layer_norm_eps=_get(config, "layer_norm_eps", 1e-12), hidden_act="gelu",
+        initializer_range=_get(config, "initializer_range", 0.02))
+
+
 @registry.register_encoder("transformer")
 class B200TransformerEncoder(nn.Module):
     """config keys as TransformerEncoder.Config: hidden_size, num_hidden_layers, num_attention_heads, num_segments,
@@ -101,16 +117,7 @@ class B200TransformerEncoder(nn.Module):
     def __init__(self, config, *args, **kwargs):
         super().__init__()
         self.original_config = config
-        import types
-        bert = types.SimpleNamespace(
-            hidden_size=_get(config, "hidden_size", 768), num_hidden_layers=_get(config, "num_hidden_layers", 12),
-            num_attention_heads=_get(config, "num_attention_heads", 12),
-            intermediate_size=_get(config, "intermediate_size", 4 * _get(config, "hidden_size", 768)),
-            vocab_size=_get(config, "vocab_size", 30522), max_position_embeddings=_get(config, "max_position_embeddings", 512),
-            type_vocab_size=_get(config, "type_vocab_size", 2), hidden_dropout_prob=_get(config, "hidden_dropout_prob", 0.1),
-            attention_probs_dropout_prob=_get(config, "attention_probs_dropout_prob", 0.1),
-            layer_norm_eps=_get(config, "layer_norm_eps", 1e-12), hidden_act="gelu",
-            initializer_range=_get(config, "initializer_range", 0.02))
+        bert = transformer_hparams(config)
         self.module = _BertModel(bert)
         self.embeddings = self.module.embeddings
         self.config = bert
@@ -130,6 +137,57 @@ class B200TransformerEncoder(nn.Module):
     def forward(self, *args, return_sequence=False, **kwargs):
         output = self.module(*args, **kwargs)
         return output[0] if return_sequence else output[1]
+
+
+# the hub configs of the two ViT checkpoints the reference's ViLT configurations name (HF ViTConfig fields)
+_VIT_BASE = dict(hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072, hidden_act="gelu",
+                 hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0, initializer_range=0.02, layer_norm_eps=1e-12,
+                 num_channels=3, qkv_bias=True)
+VIT_PRETRAINED = {
+    "google/vit-base-patch16-224": dict(_VIT_BASE, image_size=224, patch_size=16),
+    "google/vit-base-patch32-384": dict(_VIT_BASE, image_size=384, patch_size=32),
+}
+
+# ViTModel.Config (mmf/modules/vit.py:179-186)
+VIT_MODEL_DEFAULTS = dict(name="vit", pretrained_model_name="google/vit-base-patch16-224", random_init=False,
+                          gradient_checkpointing=False, do_patch_embeddings=True)
+
+
+def vit_hf_config(config):
+    """ViTModel.from_config's hf_config (vit.py:310-323): the named checkpoint's hyper-parameters, then ViTModel.Config's
+    defaults and every key of `config` on top (`ViTConfig.from_pretrained(name, **config)`, then `hf_config.update(config)`).
+    Keys nothing reads (`hidden_dim`, `mlp_dim`, `regularize_*`, `pretrained_model`, `do_pooling`) are carried along and
+    change nothing, as in the reference."""
+    from .models import ConfigNode
+    merged = dict(VIT_MODEL_DEFAULTS, **dict(config or {}))
+    name = merged["pretrained_model_name"]
+    if name not in VIT_PRETRAINED:
+        raise ValueError("no ViT hyper-parameters for pretrained_model_name %r (there is no hub here; known: %s)"
+                         % (name, sorted(VIT_PRETRAINED)))
+    if merged.get("gradient_checkpointing"):
+        raise NotImplementedError("gradient_checkpointing is not supported on the B200 ViT path")
+    return ConfigNode(dict(VIT_PRETRAINED[name], **merged))
+
+
+@registry.register_encoder("vit")
+class B200ViTImageEncoder(nn.Module):
+    """ViTEncoder (mmf/modules/encoders.py:830-857): `.module` a ViTModel on the fused pre-LN trunk (mmf_b200.vit),
+    `.embeddings` the alias of its embeddings (state-dict keys under both names, as in the reference), `.hf_config`,
+    `.out_dim`.  There is no hub: `pretrained_model_name` selects hyper-parameters from VIT_PRETRAINED, and with
+    `random_init: False` the weights arrive through load_state_dict."""
+
+    def __init__(self, config, *args, **kwargs):
+        super().__init__()
+        from .vit import B200ViTModel
+        self.config = config
+        self.hf_config = vit_hf_config(config)
+        self.module = B200ViTModel(self.hf_config)
+        self.embeddings = self.module.embeddings
+        self.out_dim = self.hf_config.hidden_size
+
+    def forward(self, *args, output_hidden_states=False, **kwargs):
+        out = self.module(*args, output_hidden_states=output_hidden_states, **kwargs)
+        return out[0], (out[2] if output_hidden_states else None)
 
 
 # ------------------------------------------------------------------------------------------------

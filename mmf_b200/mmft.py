@@ -8,17 +8,20 @@
   heads (registry "transformer_head" table of the reference):
       "mlp"  MLPHead  <-> mmf/models/transformers/heads/mlp.py:19-96    pooler -> [dropout, transform] x n -> Linear
       "mlm"  MLMHead  <-> heads/mlm.py:20-97     labelled positions gathered FIRST, transform -> vocabulary decoder -> CE
+      "mlm_multi" MLMForMultiHeads <-> heads/mlm.py:101-113   the "mlm" head on the sample list's `hs_masked_for_mlm`
       "itm"  ITMHead  <-> heads/itm.py:19-74     pooler -> Linear(H, 2) -> CE
       "mrc"  MRCHead  <-> heads/mrc.py:15-90     masked regions -> Linear -> GELU -> LayerNorm -> Linear(1601) -> KL / CE
       "mrfr" MRFRHead <-> heads/mrfr.py:15-93    masked regions -> Linear -> GELU -> LayerNorm -> tied projection -> MSE
       "wra"  WRAHead  <-> heads/wra.py:13-83     optimal-transport distance of text rows x region rows (one kernel)
       "contrastive_three_way"  ThreeWayContrastiveHead  <-> heads/contrastive.py:14-79   MLPHead(num_labels=3) -> CE
+  build_heads_dict / HeadsDict  <-> heads/utils.py:11-166   per-task head lists, configured losses, summed losses / scores
 
 The backend is the registered "b200" transformer backend (mmf_b200.mmft_backend); a config that says `backend.type:
 huggingface` (the reference default, configs/models/mmf_transformer/defaults.yaml:4-7) is served by it as well - that is
 the drop-in.  `transformer_base` cannot be downloaded here: the BERT-base hyper-parameters are used and overridden by
 `backend.params` / `transformer_config` keys; weights arrive through load_state_dict.
 """
+import collections.abc
 import warnings
 
 import torch
@@ -138,6 +141,20 @@ class MLMHead(nn.Module):
         return {"logits": logits, "losses": {c.loss_name: loss}}
 
 
+@register_transformer_head("mlm_multi")
+class MLMForMultiHeads(nn.Module):
+    """heads/mlm.py:101-113: the `mlm` head (as `mlm_head`) run on the sample list's `hs_masked_for_mlm` - the trunk
+    output of a second pass over the masked captions (ViLT's _encode_mlm) - instead of the sequence it is handed"""
+
+    def __init__(self, config):
+        super().__init__()
+        self.config = ConfigNode(dict(config))
+        self.mlm_head = MLMHead(config)
+
+    def forward(self, _, processed_sample_list):
+        return self.mlm_head(processed_sample_list["hs_masked_for_mlm"], processed_sample_list=processed_sample_list)
+
+
 @register_transformer_head("itm")
 class ITMHead(nn.Module):
     DEFAULTS = dict(type="itm", hidden_size=768, loss_name="itm_loss", ignore_index=-1, itm_label_key="is_correct")   # itm.py:22-27
@@ -199,6 +216,76 @@ class ThreeWayContrastiveHead(nn.Module):
         scores = self.contrast_head(sequence_output)["scores"]
         loss = nn.functional.cross_entropy(scores.reshape(-1, 3).float(), labels.reshape(-1), ignore_index=c.ignore_index)
         return {"losses": {c.loss_name: loss}}
+
+
+def _head_from_config(config):
+    head_type = config.get("type", "mlp")
+    if head_type not in HEADS:
+        raise NotImplementedError("transformer head %r is not on the B200 path (have: %s)" % (head_type, sorted(HEADS)))
+    return HEADS[head_type](config)
+
+
+def build_heads_dict(head_configs, tasks, losses):
+    """heads/utils.py:11-66: a list of head configs gives one nn.ModuleList for every task; a task-keyed mapping gives an
+    nn.ModuleDict of one ModuleList per task of `tasks` (a task without a head raises ValueError).  Each head's `loss`
+    names the entry of `losses` applied to a head that returns no losses itself."""
+    if isinstance(head_configs, collections.abc.Sequence):
+        heads = nn.ModuleList([_head_from_config(c) for c in head_configs])
+        head_loss_names = [c.get("loss") for c in head_configs]
+        head_names = [c.get("type", "mlp") for c in head_configs]
+    if isinstance(head_configs, collections.abc.Mapping):
+        heads, head_names, head_loss_names = nn.ModuleDict(), {}, {}
+        for task in tasks:
+            head_config = head_configs.get(task)
+            if head_config is None:
+                raise ValueError("No head defined for %s. Dataset task %s requires a head to return dict with 'losses'"
+                                 % (task, task))
+            config_list = head_config if isinstance(head_config, collections.abc.Sequence) else [head_config]
+            heads[task] = nn.ModuleList([_head_from_config(c) for c in config_list])
+            head_loss_names[task] = [c.get("loss") for c in config_list]
+            head_names[task] = [c.get("type", "mlp") for c in config_list]
+    return HeadsDict(heads, head_names, losses, head_loss_names)
+
+
+class HeadsDict(nn.Module):
+    """heads/utils.py:69-166: runs every head of a task on the sequence; a head that returns no `losses` gets its
+    configured loss applied to its scores (flattened to [-1, n]); losses that share a key are summed, and so are the
+    scores (a head without scores counts as 0)."""
+
+    def __init__(self, heads, head_names, losses, head_loss_names):
+        super().__init__()
+        self.heads = heads
+        self.head_names = head_names
+        self.losses = losses
+        self.head_loss_names = head_loss_names
+
+    def forward(self, task, sequence, sample_list):
+        if isinstance(self.heads, nn.ModuleList):
+            modules, loss_names, names = self.heads, self.head_loss_names, self.head_names
+        else:
+            modules, loss_names, names = self.heads[task], self.head_loss_names[task], self.head_names[task]
+        outputs_list = [head(sequence, processed_sample_list=sample_list) for head in modules]
+        assert len(loss_names) == len(outputs_list)
+        processed = [self._process_head_output(o, ln, hn, sample_list)
+                     for o, ln, hn in zip(outputs_list, loss_names, names)]
+        loss_result = {}
+        for output in processed:
+            for k, v in output["losses"].items():
+                loss_result[k] = loss_result[k] + v if k in loss_result else v
+        return {"losses": loss_result, "scores": sum([output.get("scores", 0) for output in processed])}
+
+    def _process_head_output(self, outputs, loss_name, head_name, sample_list):
+        if isinstance(outputs, collections.abc.MutableMapping) and "losses" in outputs:
+            return outputs
+        if isinstance(outputs, collections.abc.MutableMapping) and "scores" in outputs:
+            logits = outputs["scores"]
+        else:
+            logits = outputs
+        logits = logits.contiguous().view(-1, logits.size(-1))
+        if loss_name is None:
+            raise ValueError("Transformer head %s must either define a 'loss' in its config or return a dict that "
+                             "contains key 'losses'." % head_name)
+        return {"losses": self.losses[loss_name](sample_list, {"scores": logits}), "scores": logits}
 
 
 def compute_masked_hidden(hidden, mask):

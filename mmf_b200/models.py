@@ -8,6 +8,7 @@
   registry.register_model("vinvl")        VinVL        <->  mmf/models/vinvl.py:392-505    (mmf_b200/vinvl_model.py)
   registry.register_model("m4c")          M4C          <->  mmf/models/m4c.py:34-347       (mmf_b200/m4c_model.py)
   registry.register_model("m4c_captioner") M4CCaptioner <->  mmf/models/m4c_captioner.py:6-24
+  registry.register_model("vilt")         ViLT         <->  mmf/models/vilt.py:118-283     (mmf_b200/vilt_model.py)
 
 Each is a `BaseModel` (mmf/models/base_model.py:67-337 contract: ctor(config) -> build() -> forward(SampleList) -> dict
 with "scores" and/or "losses"; `config_path()` names the model's default YAML; `__call__` fills "losses" from the
@@ -1036,3 +1037,4 @@ class LXMERT(BaseModel):
 from . import uniter_model  # noqa: E402,F401  (registers "uniter"; it needs the names defined above)
 from . import vinvl_model  # noqa: E402,F401  (registers "vinvl"; it needs the names defined above)
 from . import m4c_model  # noqa: E402,F401  (registers "m4c" and "m4c_captioner"; it needs the names defined above)
+from . import vilt_model  # noqa: E402,F401  (registers "vilt"; it needs the names defined above)

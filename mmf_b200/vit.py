@@ -129,6 +129,19 @@ class B200ViTEmbeddings(nn.Module):
         return self.dropout(emb)
 
 
+def extended_attention_mask(attention_mask, dtype):
+    """get_extended_attention_mask of the reference's pinned transformers (<= 4.10.1) for a 2-D mask: (1 - m) * -10000
+    as [B, 1, 1, S].  None stays None (the reference's all-ones mask adds 0 to every score).  A 3-D per-query mask is
+    not supported by the kernels."""
+    if attention_mask is None:
+        return None
+    if attention_mask.dim() == 3:
+        raise NotImplementedError("per-query [B, S, S] attention masks are not supported on the B200 ViT path")
+    if attention_mask.dim() != 2:
+        raise ValueError("Wrong shape for attention_mask (shape %s)" % (tuple(attention_mask.shape),))
+    return (1.0 - attention_mask[:, None, None, :].to(dtype)) * -10000.0
+
+
 class B200ViTModel(nn.Module):
     """ViTModel (vit.py:178-274): `do_patch_embeddings=False` (vit.py:187, ViLT feeds already-embedded tokens) skips the
     patch embedding; output (sequence_output, pooled_output[, hidden_states])."""
@@ -149,11 +162,14 @@ class B200ViTModel(nn.Module):
         self.embeddings.position_embeddings.data.normal_(0.0, std)
 
     def forward(self, input_values=None, attention_mask=None, output_hidden_states=False):
+        """attention_mask: the 0/1 key mask [B, S] (1 = attend), as ViTModel.forward takes it (vit.py:276-284); it is turned
+        into the additive (1 - m) * -10000 of get_extended_attention_mask before the encoder"""
         if input_values is None:
             raise ValueError("You have to specify input_values")
         do_patch = getattr(self.config, "do_patch_embeddings", True)
         emb = self.embeddings(input_values) if do_patch else input_values
-        enc = self.encoder(emb, attention_mask=attention_mask, output_hidden_states=output_hidden_states, return_dict=True)
+        enc = self.encoder(emb, attention_mask=extended_attention_mask(attention_mask, self.layernorm.weight.dtype),
+                           output_hidden_states=output_hidden_states, return_dict=True)
         shape = enc.last_hidden_state.shape
         seq = ops.layer_norm(enc.last_hidden_state.reshape(-1, shape[-1]), self.layernorm.weight, self.layernorm.bias,
                              self.layernorm.eps).view(shape).to(self.layernorm.weight.dtype)
