@@ -83,6 +83,22 @@ int mmfb_gemm(const mmfb_gemm_args* args, mmfb_stream stream);
  * aligned is MMFB_ERR_ARG before any launch.  The workspace is the caller's; nothing in it is kept between calls. */
 int64_t mmfb_gemm_workspace_bytes(int M, int N, int K, int splits);
 
+/* mmfb_gemm with device bounds.  m_dev: NULL, or a DEVICE int32 row bound: only the 128-row tiles that start below
+ * min(M, *m_dev) are computed and stored.  k_dev: NULL, or a DEVICE int32 bound on K: only the 64-deep k-blocks that start
+ * below min(K, *k_dev) are summed.  Both NULL is mmfb_gemm.  A masked-LM head captured in a CUDA graph runs its vocabulary GEMMs on a fixed
+ * capacity of rows of which only a prefix, counted on the device, is labelled (mmfb_select_rows).  The bounds are read
+ * when the kernel runs, after the kernel before it has finished; the grid is still sized from M, N, K and the CTAs with no
+ * work left exit at once.  With b = clamp(*m_dev, 0, M), rows [0, ceil(b/128)*128) of C are computed and stored exactly as
+ * an unbounded call computes them, and no row at or past that is read or written.  With b = clamp(*k_dev, 0, K) (the
+ * weight gradient, where K is the row count), the k-blocks [0, ceil(b/64)) are shared among the launched splits the way an
+ * unbounded call with K = b shares them; a split left without a k-block adds nothing, or with a workspace stores a zero
+ * partial.  So the operand rows between b and the rounded bound are read: the caller keeps them zero.  Supported for
+ * MMFB_EPI_BIAS with (a_mn, b_mn) = (0, 0) or (0, 1) and for MMFB_EPI_ATOMIC_F32 with (1, 1), with or without a
+ * workspace (with one, the ordered reduce also covers only the rows below the rounded M bound: the rows of C past it
+ * are not read or written, and the workspace rows past it are not read); anything else is MMFB_ERR_ARG before a launch.
+ * A bound of 0 adds nothing to C. */
+int mmfb_gemm_bounded(const mmfb_gemm_args* args, const int32_t* m_dev, const int32_t* k_dev, mmfb_stream stream);
+
 /* Fused multi-head attention core (everything between the Q/K/V projections and the output projection):
  *   ctx = dropout(softmax(Q K^T / sqrt(d) + mask)) V        BertSelfAttentionJit.forward hf_layers.py:182-210,
  *   BertBiAttention.forward vilbert.py:421-461 (cross: q from one stream, k/v from the other).
@@ -304,6 +320,33 @@ int mmfb_gelu_bwd(const void* dh, const void* u, void* du, int64_t n, mmfb_strea
  * linear + cross-entropy head: the full [tokens, 30522] logits tensor never exists in HBM. */
 int mmfb_ce_rows(void* logits, int64_t ldl, const int64_t* labels, int64_t ignore_index, int M, int V, float grad_scale,
                  float* loss_sum, float* row_loss, mmfb_stream stream);
+
+/* Static-rows masked-LM loss: the labelled rows of a batch, selected and counted on the device, so that a CUDA graph can
+ * capture the head.  The head works on a fixed capacity of M rows (every row of its labels); rows [0, count) are the
+ * labelled rows in row-major order, rows [count, M) hold zero features, ignore_index labels and zero gradients.
+ *
+ * mmfb_select_rows: labels int64 [M] (DEVICE).  One CTA, an ordered scan with no atomics (the same bits on every run).
+ * A row is selected when its label != ignore_index (a label outside [0, V) is selected too; the loss kernel ignores it).
+ *   state: DEVICE int32 [2 + 2M]: state[0] = count; state[1] = the fp32 bits of 1 / max(count, 1), the double reciprocal
+ *          rounded once to fp32; pos = state + 2: pos[i] = the source row of output row i, -1 for i >= count;
+ *          inv = state + 2 + M: inv[r] = the output row of source row r, -1 when r is not selected.
+ *   labels_out: DEVICE int64 [M]: labels[pos[i]], ignore_index for i >= count.
+ * mmfb_gather_rows: out[r] = idx[r] >= 0 ? x[idx[r]] : 0 for r < M (bf16 rows of H, H % 8 == 0, 16-byte aligned rows).
+ *   With idx = pos it gathers the selected rows [M, H] (zeros past count); with idx = inv it is the backward, the full
+ *   [M, H] input gradient (the gathered gradient at selected rows, zero elsewhere), with no atomics.
+ * mmfb_ce_rows_bounded: mmfb_ce_rows on the rows below *m_dev rounded up to 128 (the GEMM's row tile) and with
+ *   grad_scale = *scale_dev, both read from DEVICE memory when the kernel runs; rows at and past the rounded bound are
+ *   not read or written (row_loss included).  The rows between *m_dev and the rounded bound must carry ignore_index.
+ * mmfb_colsum_bounded: out[n] += sum over the rows below min(M, *m_dev) of X[m, n]; with a workspace
+ *   (mmfb_colsum_workspace_bytes(M, N) bytes) the chunk-ordered sum of mmfb_colsum_ordered, which then adds the same
+ *   partials as mmfb_colsum_ordered on the rows below the bound, followed by zero partials. */
+int mmfb_select_rows(const int64_t* labels, int64_t ignore_index, int M, int32_t* state, int64_t* labels_out,
+                     mmfb_stream stream);
+int mmfb_gather_rows(const void* x, int64_t ldx, const int32_t* idx, void* out, int64_t ldo, int M, int H, mmfb_stream stream);
+int mmfb_ce_rows_bounded(void* logits, int64_t ldl, const int64_t* labels, int64_t ignore_index, int M, int V,
+                         const int32_t* m_dev, const float* scale_dev, float* loss_sum, float* row_loss, mmfb_stream stream);
+int mmfb_colsum_bounded(const void* X, int64_t ldx, float* out, int M, int N, const int32_t* m_dev, float* workspace,
+                        int64_t workspace_bytes, mmfb_stream stream);
 
 /* out = a + b; contiguous bf16 buffers of n elements.  The residual-gradient join of a pre-LN layer (ViT: the residual
  * branches off BEFORE the LayerNorm, mmf/modules/vit.py:96-108), which a post-LN layer gets for free from the GEMM epilogue. */

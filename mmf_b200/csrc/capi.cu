@@ -124,6 +124,12 @@ int mmfb_gemm(const mmfb_gemm_args* args, mmfb_stream stream) {
   return gemm(*args, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int mmfb_gemm_bounded(const mmfb_gemm_args* args, const int32_t* m_dev, const int32_t* k_dev, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_gemm_bounded: null args");
+  MMFB_REQUIRE_DEVICE();
+  return gemm(*args, reinterpret_cast<cudaStream_t>(stream), m_dev, k_dev);
+}
+
 int mmfb_attention_fwd(const mmfb_attn_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_attention_fwd: null args");
   MMFB_REQUIRE_DEVICE();
@@ -256,6 +262,30 @@ int mmfb_ce_rows(void* logits, int64_t ldl, const int64_t* labels, int64_t ignor
   if (!logits || !labels) return set_error(MMFB_ERR_ARG, "mmfb_ce_rows: null pointer");
   MMFB_REQUIRE_DEVICE();
   return ce_rows(logits, ldl, labels, ignore_index, M, V, grad_scale, loss_sum, row_loss, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_ce_rows_bounded(void* logits, int64_t ldl, const int64_t* labels, int64_t ignore_index, int M, int V,
+                         const int32_t* m_dev, const float* scale_dev, float* loss_sum, float* row_loss, mmfb_stream stream) {
+  if (!logits || !labels || !m_dev || !scale_dev) return set_error(MMFB_ERR_ARG, "mmfb_ce_rows_bounded: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return ce_rows_bounded(logits, ldl, labels, ignore_index, M, V, m_dev, scale_dev, loss_sum, row_loss,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_colsum_bounded(const void* X, int64_t ldx, float* out, int M, int N, const int32_t* m_dev, float* workspace,
+                        int64_t workspace_bytes, mmfb_stream stream) {
+  if (!X || !out || !m_dev) return set_error(MMFB_ERR_ARG, "mmfb_colsum_bounded: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return colsum_bounded(X, ldx, out, M, N, m_dev, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_select_rows(const int64_t* labels, int64_t ignore_index, int M, int32_t* state, int64_t* labels_out,
+                     mmfb_stream stream) {
+  if (!labels || !state || !labels_out) return set_error(MMFB_ERR_ARG, "mmfb_select_rows: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return select_rows(labels, ignore_index, M, state, labels_out, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_gather_rows(const void* x, int64_t ldx, const int32_t* idx, void* out, int64_t ldo, int M, int H, mmfb_stream stream) {
+  if (!x || !idx || !out) return set_error(MMFB_ERR_ARG, "mmfb_gather_rows: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return gather_rows(x, ldx, idx, out, ldo, M, H, reinterpret_cast<cudaStream_t>(stream));
 }
 int mmfb_add_bf16(const void* a, const void* b, void* out, int64_t n, mmfb_stream stream) {
   if (!a || !b || !out) return set_error(MMFB_ERR_ARG, "mmfb_add_bf16: null pointer");

@@ -30,14 +30,24 @@ __device__ __forceinline__ float block_reduce(float v, float* red, bool is_max) 
   return r;
 }
 
+// BOUNDED: the rows come from a fixed capacity of which only a prefix, counted on the device, is labelled: rows at or
+// past *m_dev rounded up to BOUNDED_ROW_TILE are not touched (the rows between carry ignore_index and are zeroed, which
+// is what the bounded GEMMs that read them next need), and grad_scale is *scale_dev.
+template <bool BOUNDED = false>
 __global__ void __launch_bounds__(256)
 ce_rows_kernel(bf16* __restrict__ z, int64_t ldz, const int64_t* __restrict__ labels, int64_t ignore_index, int M, int V,
-               float grad_scale, float* __restrict__ loss_sum, float* __restrict__ row_loss) {
+               float grad_scale, float* __restrict__ loss_sum, float* __restrict__ row_loss,
+               const int32_t* __restrict__ m_dev = nullptr, const float* __restrict__ scale_dev = nullptr) {
   griddep_launch();
   griddep_wait();
   __shared__ float red[8];
   const int row = blockIdx.x;
   if (row >= M) return;
+  if constexpr (BOUNDED) {
+    const int b = max(*m_dev, 0);
+    if (row >= (b + BOUNDED_ROW_TILE - 1) / BOUNDED_ROW_TILE * BOUNDED_ROW_TILE) return;
+    grad_scale = *scale_dev;
+  }
   bf16* zr = z + static_cast<int64_t>(row) * ldz;
   const int64_t label = labels[row];
   const bool active = label != ignore_index && label >= 0 && label < V;
@@ -99,9 +109,24 @@ int ce_rows(void* logits, int64_t ldl, const int64_t* labels, int64_t ignore_ind
             float* loss_sum, float* row_loss, cudaStream_t s) {
   if (M <= 0 || V <= 0 || (V % 8) || (ldl % 8)) return set_error(MMFB_ERR_ARG, "ce_rows: bad shape %dx%d (ld %lld)", M, V, (long long)ldl);
   if (reinterpret_cast<uintptr_t>(logits) & 15) return set_error(MMFB_ERR_ARG, "ce_rows: logits must be 16-byte aligned");
-  MMFB_LAUNCH(ce_rows_kernel, M, 256, 0, s, reinterpret_cast<bf16*>(logits), ldl, labels, ignore_index, M, V, grad_scale, loss_sum, row_loss);
+  MMFB_LAUNCH(ce_rows_kernel<false>, M, 256, 0, s, reinterpret_cast<bf16*>(logits), ldl, labels, ignore_index, M, V, grad_scale,
+              loss_sum, row_loss, nullptr, nullptr);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "ce_rows launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return MMFB_OK;
+}
+
+int ce_rows_bounded(void* logits, int64_t ldl, const int64_t* labels, int64_t ignore_index, int M, int V,
+                    const int32_t* m_dev, const float* scale_dev, float* loss_sum, float* row_loss, cudaStream_t s) {
+  if (M <= 0 || V <= 0 || (V % 8) || (ldl % 8)) return set_error(MMFB_ERR_ARG, "ce_rows_bounded: bad shape %dx%d (ld %lld)", M, V, (long long)ldl);
+  if (reinterpret_cast<uintptr_t>(logits) & 15) return set_error(MMFB_ERR_ARG, "ce_rows_bounded: logits must be 16-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(m_dev) | reinterpret_cast<uintptr_t>(scale_dev)) & 3)
+    return set_error(MMFB_ERR_ARG, "ce_rows_bounded: m_dev / scale_dev must be 4-byte aligned");
+  MMFB_LAUNCH(ce_rows_kernel<true>, M, 256, 0, s, reinterpret_cast<bf16*>(logits), ldl, labels, ignore_index, M, V, 0.0f,
+              loss_sum, row_loss, m_dev, scale_dev);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "ce_rows_bounded launch: %s", cudaGetErrorString(e));
   count_launch();
   return MMFB_OK;
 }

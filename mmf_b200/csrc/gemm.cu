@@ -47,6 +47,8 @@ struct GemmDev {
   const uint32_t* dmask; // dropout keep-bits, [M, ldmask] words (bit n%32 of word n/32), or null
   int64_t ldmask;
   float dscale;          // 1/(1-p)
+  const int32_t* m_dev;  // BOUNDED: device row bound (tiles starting at or past min(M, *m_dev) are skipped), or null
+  const int32_t* k_dev;  // BOUNDED: device bound on K (only the k-blocks below min(K, *k_dev) are summed), or null
 };
 
 // epilogues that read a per-element bf16 operand (aux): it is loaded by TMA into the output staging boxes
@@ -98,7 +100,9 @@ __device__ __forceinline__ Unit decode_unit(int u, const GemmDev& p, int tiles_n
   return w;
 }
 
-template <int BN, bool A_MN, bool B_MN, int EPI>
+// BOUNDED: the extents come from device memory (GemmDev::m_dev / k_dev), read after griddep_wait - the masked-LM head's
+// vocabulary GEMMs run on a fixed capacity of rows of which only a device-counted prefix is labelled (DESIGN.md 4.1).
+template <int BN, bool A_MN, bool B_MN, int EPI, bool BOUNDED = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2,
@@ -116,9 +120,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   griddep_launch();
   const int wg = threadIdx.x >> 7;
   const int tiles_n = (p.N + BN - 1) / BN;
-  const int kb_total = (p.K + BK - 1) / BK;
-  const int kb_per_split = (kb_total + p.splits - 1) / p.splits;
-  const int units = ((p.M + BM - 1) / BM) * tiles_n * p.splits;
+  int kb_total = (p.K + BK - 1) / BK;
+  int kb_per_split = (kb_total + p.splits - 1) / p.splits;
+  int units = ((p.M + BM - 1) / BM) * tiles_n * p.splits;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
@@ -136,6 +140,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
   __syncthreads();
   griddep_wait();        // operands / aux / bias of this GEMM may come from the kernel that is still finishing
+  if constexpr (BOUNDED) {
+    // row tiles at or past the bound are not units at all (m is the outermost unit index); the k-blocks below the K bound
+    // are shared among the launched splits as an unbounded call with K = bound would share them, and a unit left
+    // without one adds nothing (EPI_ATOMIC_F32) or stores a zero partial (EPI_PARTIAL_F32, so the reduce is unchanged)
+    if (p.m_dev != nullptr) units = ((min(p.M, max(*p.m_dev, 0)) + BM - 1) / BM) * tiles_n * p.splits;
+    if (p.k_dev != nullptr) {
+      kb_total = (min(p.K, max(*p.k_dev, 0)) + BK - 1) / BK;
+      kb_per_split = (kb_total + p.splits - 1) / p.splits;
+    }
+  }
 
   // The ring position (slot s, phase ph) runs on over all k-blocks of all units of this CTA, in the same order in the
   // producer and in both consumers, and is never reset between units: the producer fills the next unit's first slots
@@ -220,11 +234,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
       wgmma_wait<0>();
-      mbar_arrive(&empty[prev]);           // every unit owns at least one k-block
+      if (!BOUNDED || prev >= 0) mbar_arrive(&empty[prev]);   // every unbounded unit owns at least one k-block
     }
 
     if (epi_f32(EPI)) {
       // ------------- split-K epilogue: fp32 vector reductions into C, or plain stores of the split's partial -------------
+      if (BOUNDED && EPI == EPI_ATOMIC_F32 && w.kb0 >= w.kb1) continue;   // no k-block below the bound: nothing to add
       float* dst = p.c32;
       if (EPI == EPI_PARTIAL_F32) dst += static_cast<int64_t>(u % p.splits) * p.M * p.N;   // ldc = N
 #pragma unroll
@@ -351,13 +366,20 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
 // Second kernel of the ordered split-K GEMM:  C = ((C + P_0) + P_1) + ... + P_{S-1}  for the partials P_s = ws[s] [M, N].
 // Four consecutive columns per thread (N % 8 == 0: they lie in one row).
+// BOUNDED (a device row bound m_dev on the GEMM): the partial kernel stored no partial for the row tiles at or past
+// min(M, *m_dev) rounded up to BM, so those rows of C are neither read nor written here either.
+template <bool BOUNDED = false>
 __global__ void __launch_bounds__(256)
-splitk_reduce_kernel(const float* __restrict__ ws, int S, int M, int N, float* __restrict__ c, int64_t ldc) {
+splitk_reduce_kernel(const float* __restrict__ ws, int S, int M, int N, float* __restrict__ c, int64_t ldc,
+                     const int32_t* __restrict__ m_dev = nullptr) {
   griddep_launch();
   griddep_wait();
   const int64_t mn = static_cast<int64_t>(M) * N;
   const int64_t i = (static_cast<int64_t>(blockIdx.x) * 256 + threadIdx.x) * 4;
   if (i >= mn) return;
+  if constexpr (BOUNDED) {
+    if (m_dev != nullptr && i / N >= min(M, (max(*m_dev, 0) + BM - 1) / BM * BM)) return;
+  }
   float2* dst = reinterpret_cast<float2*>(c + (i / N) * ldc + (i % N));
   const float2 c0 = dst[0], c1 = dst[1];
   float4 r = make_float4(c0.x, c0.y, c1.x, c1.y);
@@ -387,8 +409,9 @@ int64_t gemm_workspace_bytes(int M, int N, int K, int splits) {
   return s > 1 ? static_cast<int64_t>(s) * M * N * 4 : 0;
 }
 
-template <int BN, bool A_MN, bool B_MN, int EPI>
-static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
+template <int BN, bool A_MN, bool B_MN, int EPI, bool BOUNDED = false>
+static int launch(const mmfb_gemm_args& a, cudaStream_t stream, const int32_t* m_dev = nullptr,
+                  const int32_t* k_dev = nullptr) {
   using C = Cfg<BN>;
   constexpr bool AUX = epi_reads_aux(EPI);
   CUtensorMap tmA, tmB;
@@ -431,8 +454,10 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream) {
   p.dmask = a.drop_mask;
   p.ldmask = a.ldmask;
   p.dscale = a.drop_scale;
+  p.m_dev = BOUNDED ? m_dev : nullptr;
+  p.k_dev = BOUNDED ? k_dev : nullptr;
 
-  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN, EPI, BOUNDED>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
@@ -469,22 +494,40 @@ static int dispatch(const mmfb_gemm_args& a, cudaStream_t s) {
   }
 }
 
+// The device-bounded instantiations (m_dev / k_dev set): the masked-LM head's vocabulary GEMM, its dgrad and its wgrad.
+template <int BN>
+static int dispatch_bounded(const mmfb_gemm_args& a, cudaStream_t s, const int32_t* m_dev, const int32_t* k_dev) {
+  const int key = (a.a_mn ? 100 : 0) + (a.b_mn ? 10 : 0) + a.epi;
+  switch (key) {
+    case 0 + EPI_BIAS: return launch<BN, false, false, EPI_BIAS, true>(a, s, m_dev, k_dev);
+    case 10 + EPI_BIAS: return launch<BN, false, true, EPI_BIAS, true>(a, s, m_dev, k_dev);
+    case 110 + EPI_ATOMIC_F32: return launch<BN, true, true, EPI_ATOMIC_F32, true>(a, s, m_dev, k_dev);
+    default:
+      return set_error(MMFB_ERR_ARG, "gemm: a device bound (m_dev / k_dev) is not supported for (a_mn=%d, b_mn=%d, epi=%d)",
+                       a.a_mn, a.b_mn, a.epi);
+  }
+}
+
 // Ordered split-K: every (tile, split) unit stores its partial into the workspace, then one more kernel adds the
 // partials into C in split order.  No unit waits for another, so this is safe whatever number of CTAs is resident.
-template <int BN>
-static int gemm_ordered(const mmfb_gemm_args& a, int splits, cudaStream_t stream) {
-  int rc = launch<BN, true, true, EPI_PARTIAL_F32>(a, stream);
+// BOUNDED: units without a k-block below the K bound store zero partials, so the reduce adds the same partials as an
+// unbounded call with K = bound, then zeros; with an M bound the reduce skips the rows whose tiles stored no partial.
+template <int BN, bool BOUNDED>
+static int gemm_ordered(const mmfb_gemm_args& a, int splits, cudaStream_t stream, const int32_t* m_dev,
+                        const int32_t* k_dev) {
+  int rc = launch<BN, true, true, EPI_PARTIAL_F32, BOUNDED>(a, stream, m_dev, k_dev);
   if (rc) return rc;
   const int64_t quads = static_cast<int64_t>(a.M) * a.N / 4;
-  MMFB_LAUNCH(splitk_reduce_kernel, static_cast<unsigned>((quads + 255) / 256), 256, 0, stream,
-              reinterpret_cast<const float*>(a.workspace), splits, a.M, a.N, reinterpret_cast<float*>(a.C), a.ldc);
+  MMFB_LAUNCH(splitk_reduce_kernel<BOUNDED>, static_cast<unsigned>((quads + 255) / 256), 256, 0, stream,
+              reinterpret_cast<const float*>(a.workspace), splits, a.M, a.N, reinterpret_cast<float*>(a.C), a.ldc,
+              BOUNDED ? m_dev : nullptr);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "gemm split-K reduce launch: %s", cudaGetErrorString(e));
   count_launch();
   return MMFB_OK;
 }
 
-int gemm(const mmfb_gemm_args& a, cudaStream_t stream) {
+int gemm(const mmfb_gemm_args& a, cudaStream_t stream, const int32_t* m_dev, const int32_t* k_dev) {
   if (a.M <= 0 || a.N <= 0 || a.K <= 0) return set_error(MMFB_ERR_ARG, "gemm: empty problem %dx%dx%d", a.M, a.N, a.K);
   // only CONTIGUOUS extents need 16-byte granularity (TMA row pitch / vector epilogue); K of an MN-major operand
   // (= the token count in the weight-gradient GEMM) is a row count and may be anything
@@ -496,6 +539,9 @@ int gemm(const mmfb_gemm_args& a, cudaStream_t stream) {
     return set_error(MMFB_ERR_ARG, "gemm: leading dimensions must be multiples of 8 elements");
   const int bn = a.block_n > 0 ? a.block_n : (a.N >= 256 ? 256 : 128);
   const bool ordered = a.epi == EPI_ATOMIC_F32 && (a.workspace != nullptr || a.workspace_bytes != 0);
+  const bool bounded = m_dev != nullptr || k_dev != nullptr;
+  if ((reinterpret_cast<uintptr_t>(m_dev) | reinterpret_cast<uintptr_t>(k_dev)) & 3)
+    return set_error(MMFB_ERR_ARG, "gemm: m_dev / k_dev must be 4-byte aligned");
   const int splits = gemm_effective_splits(a.K, a.splits);
   if (ordered && splits > 1 && (bn == 128 || bn == 256) && a.a_mn && a.b_mn) {
     const int64_t need = gemm_workspace_bytes(a.M, a.N, a.K, a.splits);
@@ -504,7 +550,15 @@ int gemm(const mmfb_gemm_args& a, cudaStream_t stream) {
                        (long long)need, a.workspace, (long long)a.workspace_bytes);
     if ((reinterpret_cast<uintptr_t>(a.C) & 7) || (a.ldc % 2))
       return set_error(MMFB_ERR_ARG, "gemm: ordered split-K needs an 8-byte aligned C with an even ldc");
-    return bn == 256 ? gemm_ordered<256>(a, splits, stream) : gemm_ordered<128>(a, splits, stream);
+    if (bounded)
+      return bn == 256 ? gemm_ordered<256, true>(a, splits, stream, m_dev, k_dev)
+                       : gemm_ordered<128, true>(a, splits, stream, m_dev, k_dev);
+    return bn == 256 ? gemm_ordered<256, false>(a, splits, stream, nullptr, nullptr)
+                     : gemm_ordered<128, false>(a, splits, stream, nullptr, nullptr);
+  }
+  if (bounded) {
+    if (bn == 256) return dispatch_bounded<256>(a, stream, m_dev, k_dev);
+    if (bn == 128) return dispatch_bounded<128>(a, stream, m_dev, k_dev);
   }
   if (bn == 256) return dispatch<256>(a, stream);
   if (bn == 128) return dispatch<128>(a, stream);

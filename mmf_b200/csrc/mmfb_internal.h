@@ -27,6 +27,9 @@ constexpr int ORDER_ROWS = 128;
 // Sorted positions per chunk of the ordered embedding-table scatter (the run-aggregation window of one warp).
 constexpr int SCATTER_CHUNK = 32;
 inline int order_chunks(int M) { return (M + ORDER_ROWS - 1) / ORDER_ROWS; }
+// Rows a device-bounded row kernel (ce_rows_bounded) covers: the device count rounded up to this, the GEMM's row tile,
+// so that every row a bounded GEMM tile reads next has been written (include/mmfb200.h, "Device bounds").
+constexpr int BOUNDED_ROW_TILE = 128;
 
 // split-K factor the GEMM actually runs for K and the requested `splits`: every split owns at least one k-block
 int gemm_effective_splits(int K, int splits);
@@ -66,7 +69,8 @@ cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
 #define MMFB_LAUNCH(kern, grid, block, smem, stream, ...) \
   (void)::mmfb::launch_k(kern, dim3(grid), dim3(block), static_cast<size_t>(smem), stream, __VA_ARGS__)
 
-int gemm(const mmfb_gemm_args& a, cudaStream_t stream);
+// m_dev / k_dev: the device bounds of mmfb_gemm_bounded (NULL: none)
+int gemm(const mmfb_gemm_args& a, cudaStream_t stream, const int32_t* m_dev = nullptr, const int32_t* k_dev = nullptr);
 int attn_fwd(const mmfb_attn_args& a, cudaStream_t stream);
 int attn_bwd(const mmfb_attn_args& a, cudaStream_t stream);
 int attn_varlen_fwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream);
@@ -95,6 +99,12 @@ int adamw(const mmfb_adamw_args& a, cudaStream_t s);
 int grad_norm(const mmfb_grad_norm_args& a, cudaStream_t s);
 int ce_rows(void* logits, int64_t ldl, const int64_t* labels, int64_t ignore_index, int M, int V, float grad_scale,
             float* loss_sum, float* row_loss, cudaStream_t s);
+int ce_rows_bounded(void* logits, int64_t ldl, const int64_t* labels, int64_t ignore_index, int M, int V,
+                    const int32_t* m_dev, const float* scale_dev, float* loss_sum, float* row_loss, cudaStream_t s);
+int colsum_bounded(const void* X, int64_t ldx, float* out, int M, int N, const int32_t* m_dev, float* ws, int64_t ws_bytes,
+                   cudaStream_t s);
+int select_rows(const int64_t* labels, int64_t ignore_index, int M, int32_t* state, int64_t* labels_out, cudaStream_t s);
+int gather_rows(const void* x, int64_t ldx, const int32_t* idx, void* out, int64_t ldo, int M, int H, cudaStream_t s);
 int add_bf16(const void* a, const void* b, void* out, int64_t n, cudaStream_t s);
 int dropout_apply(const void* x, int64_t ldx, const uint32_t* bits, int64_t ldm, float scale, void* out, int64_t ldo, int M,
                   int H, cudaStream_t s);

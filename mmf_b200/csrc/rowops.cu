@@ -417,12 +417,20 @@ ln_bwd_stream_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __re
 // ----------------------------------------------------------------------------------------------
 // column sums (bias gradients):  out[n] += sum_m X[m, n]
 // ORDERED: block (x, k) sums the rows of chunk k and stores the partial to ws[k][N]; chunk_reduce_kernel adds them up.
+// BOUNDED: only the rows below min(M, *m_dev) are summed (the grid is sized from M): an atomic block with no row there
+// exits, an ordered chunk with no row there stores a zero partial, so the reduce adds exactly what an unbounded call on
+// the rows below the bound adds, then zeros.
 // ----------------------------------------------------------------------------------------------
-template <bool ORDERED>
+template <bool ORDERED, bool BOUNDED = false>
 __global__ void __launch_bounds__(256)
-colsum_kernel(const bf16* __restrict__ X, int64_t ldx, float* __restrict__ out, int M, int N, float* __restrict__ ws) {
+colsum_kernel(const bf16* __restrict__ X, int64_t ldx, float* __restrict__ out, int M, int N, float* __restrict__ ws,
+              const int32_t* __restrict__ m_dev = nullptr) {
   griddep_launch();
   griddep_wait();
+  if constexpr (BOUNDED) {
+    M = min(M, max(*m_dev, 0));
+    if (!ORDERED && static_cast<int64_t>(blockIdx.y) * 8 >= M) return;
+  }
   __shared__ float red[8][256];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int col = blockIdx.x * 256 + lane * 8;
@@ -964,7 +972,7 @@ int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s)
   const int cap = (num_sms() * 4 + grid.x - 1) / grid.x;
   grid.y = rows_blocks < cap ? rows_blocks : cap;
   if (grid.y < 1) grid.y = 1;
-  MMFB_LAUNCH(colsum_kernel<false>, grid, 256, 0, s, (const bf16*)X, ldx, out, M, N, nullptr);
+  MMFB_LAUNCH(colsum_kernel<false>, grid, 256, 0, s, (const bf16*)X, ldx, out, M, N, nullptr, nullptr);
   return launch_ok("colsum");
 }
 
@@ -974,9 +982,123 @@ int colsum_ordered(const void* X, int64_t ldx, float* out, int M, int N, float* 
   if (rc) return rc;
   if ((rc = check_workspace("colsum_ordered", ws, ws_bytes, colsum_workspace_bytes(M, N)))) return rc;
   const int chunks = order_chunks(M);
-  MMFB_LAUNCH(colsum_kernel<true>, dim3((N + 255) / 256, chunks), 256, 0, s, (const bf16*)X, ldx, out, M, N, ws);
+  MMFB_LAUNCH(colsum_kernel<true>, dim3((N + 255) / 256, chunks), 256, 0, s, (const bf16*)X, ldx, out, M, N, ws, nullptr);
   if ((rc = launch_ok("colsum_ordered"))) return rc;
   return chunk_reduce(ws, chunks, N, out, nullptr, nullptr, 1, s, "colsum_ordered reduce");
+}
+
+// colsum / colsum_ordered (ws non-null) of the rows below min(M, *m_dev); grid and workspace sized from M
+int colsum_bounded(const void* X, int64_t ldx, float* out, int M, int N, const int32_t* m_dev, float* ws, int64_t ws_bytes,
+                   cudaStream_t s) {
+  if (M <= 0 || N <= 0 || N % 8) return set_error(MMFB_ERR_ARG, "colsum_bounded: bad shape %dx%d", M, N);
+  int rc = check_aligned("colsum_bounded", M, {{X, ldx, "x"}});
+  if (rc) return rc;
+  if (reinterpret_cast<uintptr_t>(m_dev) & 3) return set_error(MMFB_ERR_ARG, "colsum_bounded: m_dev must be 4-byte aligned");
+  if (ws != nullptr || ws_bytes != 0) {
+    if ((rc = check_workspace("colsum_bounded", ws, ws_bytes, colsum_workspace_bytes(M, N)))) return rc;
+    const int chunks = order_chunks(M);
+    MMFB_LAUNCH((colsum_kernel<true, true>), dim3((N + 255) / 256, chunks), 256, 0, s, (const bf16*)X, ldx, out, M, N, ws,
+                m_dev);
+    if ((rc = launch_ok("colsum_bounded"))) return rc;
+    return chunk_reduce(ws, chunks, N, out, nullptr, nullptr, 1, s, "colsum_bounded reduce");
+  }
+  dim3 grid((N + 255) / 256, 1);
+  int rows_blocks = (M + 63) / 64;
+  const int cap = (num_sms() * 4 + grid.x - 1) / grid.x;
+  grid.y = rows_blocks < cap ? rows_blocks : cap;
+  if (grid.y < 1) grid.y = 1;
+  MMFB_LAUNCH((colsum_kernel<false, true>), grid, 256, 0, s, (const bf16*)X, ldx, out, M, N, nullptr, m_dev);
+  return launch_ok("colsum_bounded");
+}
+
+// Row selection of a static-rows masked-LM head (one CTA; the labels of one batch are a few ten thousand int64).  Thread t
+// owns the consecutive labels [t * per, (t + 1) * per): it counts its labelled ones, an exclusive scan over the threads in
+// thread order gives its first output slot, and a second pass writes them.  No atomics: the same bits on every run.
+// state (int32 [2 + 2M]): [0] = count, [1] = the fp32 bits of 1 / max(count, 1) (the double reciprocal rounded once, as
+// the host computes it), [2, 2 + M) = pos (output row -> source row, -1 past count), [2 + M, 2 + 2M) = inv (source row ->
+// output row, -1 for an unlabelled row).  labels_out[i] = labels[pos[i]], ignore_index past count.
+constexpr int SELECT_THREADS = 1024;
+__global__ void __launch_bounds__(SELECT_THREADS)
+select_rows_kernel(const int64_t* __restrict__ labels, int64_t ignore_index, int M, int32_t* __restrict__ state,
+                   int64_t* __restrict__ labels_out) {
+  griddep_launch();
+  griddep_wait();
+  __shared__ int warp_tot[SELECT_THREADS / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int per = (M + SELECT_THREADS - 1) / SELECT_THREADS;
+  const int b = min(M, static_cast<int>(threadIdx.x) * per), e = min(M, b + per);
+  int n = 0;
+  for (int i = b; i < e; ++i) n += labels[i] != ignore_index;
+  int incl = n;                                   // inclusive scan within the warp
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) warp_tot[warp] = incl;
+  __syncthreads();
+  int before = 0, total = 0;
+  for (int w = 0; w < SELECT_THREADS / 32; ++w) {
+    const int t = warp_tot[w];
+    if (w < warp) before += t;
+    total += t;
+  }
+  int slot = before + incl - n;
+  int32_t* pos = state + 2;
+  int32_t* inv = state + 2 + M;
+  for (int i = b; i < e; ++i) {
+    const int64_t l = labels[i];
+    if (l != ignore_index) {
+      pos[slot] = i;
+      inv[i] = slot;
+      labels_out[slot] = l;
+      ++slot;
+    } else {
+      inv[i] = -1;
+    }
+  }
+  for (int i = total + threadIdx.x; i < M; i += SELECT_THREADS) {
+    pos[i] = -1;
+    labels_out[i] = ignore_index;
+  }
+  if (threadIdx.x == 0) {
+    state[0] = total;
+    state[1] = __float_as_int(__double2float_rn(1.0 / static_cast<double>(max(total, 1))));
+  }
+}
+
+// out[r] = idx[r] >= 0 ? x[idx[r]] : 0, one warp per output row, 16-byte vectors.  With pos this is the forward gather of
+// the selected rows; with inv it is its backward (each source row takes its gathered row's gradient, or zero): no atomics.
+__global__ void __launch_bounds__(ROW_WARPS * 32)
+gather_rows_kernel(const bf16* __restrict__ x, int64_t ldx, const int32_t* __restrict__ idx, bf16* __restrict__ out,
+                   int64_t ldo, int M, int H) {
+  griddep_launch();
+  griddep_wait();
+  const int row = blockIdx.x * ROW_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= M) return;
+  const int src = idx[row];
+  uint4* dst = reinterpret_cast<uint4*>(out + static_cast<int64_t>(row) * ldo);
+  const uint4* from = reinterpret_cast<const uint4*>(x + static_cast<int64_t>(src < 0 ? 0 : src) * ldx);
+  for (int v = lane; v < H / 8; v += 32) dst[v] = src >= 0 ? from[v] : make_uint4(0u, 0u, 0u, 0u);
+}
+
+int select_rows(const int64_t* labels, int64_t ignore_index, int M, int32_t* state, int64_t* labels_out, cudaStream_t s) {
+  if (M <= 0) return set_error(MMFB_ERR_ARG, "select_rows: empty problem");
+  if ((reinterpret_cast<uintptr_t>(labels) | reinterpret_cast<uintptr_t>(labels_out)) & 7 ||
+      reinterpret_cast<uintptr_t>(state) & 3)
+    return set_error(MMFB_ERR_ARG, "select_rows: misaligned buffer");
+  MMFB_LAUNCH(select_rows_kernel, 1, SELECT_THREADS, 0, s, labels, ignore_index, M, state, labels_out);
+  return launch_ok("select_rows");
+}
+
+int gather_rows(const void* x, int64_t ldx, const int32_t* idx, void* out, int64_t ldo, int M, int H, cudaStream_t s) {
+  if (M <= 0 || H <= 0 || H % 8) return set_error(MMFB_ERR_ARG, "gather_rows: bad shape %dx%d", M, H);
+  int rc = check_aligned("gather_rows", 2, {{x, ldx, "x"}, {out, ldo, "out"}});
+  if (rc) return rc;
+  if (reinterpret_cast<uintptr_t>(idx) & 3) return set_error(MMFB_ERR_ARG, "gather_rows: idx must be 4-byte aligned");
+  MMFB_LAUNCH(gather_rows_kernel, (M + ROW_WARPS - 1) / ROW_WARPS, ROW_WARPS * 32, 0, s, (const bf16*)x, ldx, idx, (bf16*)out,
+              ldo, M, H);
+  return launch_ok("gather_rows");
 }
 
 int dropout_bits(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t offset, float p, const uint64_t* epoch, cudaStream_t s) {

@@ -57,13 +57,25 @@ def _idx_len(idx, M, name):
         raise ValueError("%s must be a contiguous vector of %d indices (one per row), got shape %s" % (name, M, tuple(idx.shape)))
 
 
+def _bound(t, name):
+    """a device bound: one int32 in CUDA memory (read by the kernel when it runs, never on the host)"""
+    if t is None:
+        return None
+    _req(t, torch.int32, name)
+    if t.numel() != 1:
+        raise ValueError("%s must be a CUDA int32 tensor with one element" % name)
+    return t.data_ptr()
+
+
 def gemm(a, b, *, a_mn=False, b_mn=False, epi=lib.EPI_BIAS, bias=None, aux=None, drop_mask=None,
-         drop_scale=1.0, out=None, out2=None, splits=1, block_n=0, cluster=0):
+         drop_scale=1.0, out=None, out2=None, splits=1, block_n=0, cluster=0, m_bound=None, k_bound=None):
     """C[M,N] = epi(A[M,K] @ B[N,K]^T) on the wgmma GEMM.
 
     a: [M,K] (a_mn=False) or [K,M] (a_mn=True); b: [N,K] (b_mn=False) or [K,N] (b_mn=True); bf16.
     Returns C (and C2 for EPI_BIAS_GELU).  For EPI_ATOMIC_F32 `out` (fp32 [M,N]) is accumulated into; in deterministic
     mode with splits > 1 the split partials go through a workspace and are added in split order.
+    m_bound / k_bound: int32 [1] CUDA tensors bounding M / K on the device (include/mmfb200.h, "Device bounds"); only the
+    row tiles below the rounded M bound are written, so `out` past it keeps what it held.
     """
     _req(a, torch.bfloat16, "a")
     _req(b, torch.bfloat16, "b")
@@ -104,7 +116,11 @@ def gemm(a, b, *, a_mn=False, b_mn=False, epi=lib.EPI_BIAS, bias=None, aux=None,
         if nbytes > 0:
             ws = _workspace(nbytes, a.device)
             args.workspace, args.workspace_bytes = ws.data_ptr(), nbytes
-    check(LIB.mmfb_gemm(ctypes.byref(args), _stream_ptr()))
+    if m_bound is not None or k_bound is not None:
+        check(LIB.mmfb_gemm_bounded(ctypes.byref(args), _bound(m_bound, "m_bound"), _bound(k_bound, "k_bound"),
+                                    _stream_ptr()))
+    else:
+        check(LIB.mmfb_gemm(ctypes.byref(args), _stream_ptr()))
     if epi == lib.EPI_BIAS_GELU:
         return out, out2
     return out
@@ -564,6 +580,81 @@ def ce_rows(logits, labels, ignore_index, grad_scale, loss_sum, row_loss=None):
     check(LIB.mmfb_ce_rows(logits.data_ptr(), logits.stride(0), labels.data_ptr(), int(ignore_index), M, V, float(grad_scale),
                            loss_sum.data_ptr(), rl, _stream_ptr()))
     return logits
+
+
+def ce_rows_bounded(logits, labels, ignore_index, scale, m_bound, loss_sum=None, row_loss=None):
+    """ce_rows on the rows below m_bound rounded up to 128, with grad_scale read from `scale` (fp32 [1]), both on the
+    device.  Rows at and past the rounded bound are untouched (row_loss included).  In deterministic mode the loss goes only
+    to row_loss (required), which the caller sums in a fixed order; otherwise it is added to loss_sum with atomics."""
+    _req(logits, torch.bfloat16, "logits"); _req(labels, torch.int64, "labels"); _req(scale, torch.float32, "scale")
+    M, V = logits.shape
+    if labels.numel() != M or not labels.is_contiguous():
+        raise ValueError("ce_rows_bounded: one contiguous int64 label per row required")
+    if row_loss is not None:
+        _req(row_loss, torch.float32, "row_loss")
+        if row_loss.numel() != M:
+            raise ValueError("ce_rows_bounded: row_loss must have one element per row")
+    if _ordered():
+        if row_loss is None:
+            raise ValueError("ce_rows_bounded: deterministic mode needs row_loss (summed by the caller in a fixed order)")
+        loss_sum = None
+    elif loss_sum is not None and (not loss_sum.is_cuda or loss_sum.dtype != torch.float32 or loss_sum.numel() != 1):
+        raise ValueError("ce_rows_bounded: loss_sum must be a CUDA fp32 tensor with one element")
+    check(LIB.mmfb_ce_rows_bounded(logits.data_ptr(), logits.stride(0), labels.data_ptr(), int(ignore_index), M, V,
+                                   _bound(m_bound, "m_bound"), scale.data_ptr(), _ptr(loss_sum), _ptr(row_loss),
+                                   _stream_ptr()))
+    return logits
+
+
+def colsum_bounded(x, out, m_bound):
+    """out[n] += sum over the rows m < m_bound (int32 [1] on the device) of x[m, n]; ordered in deterministic mode."""
+    _req(x, torch.bfloat16, "x"); _req(out, torch.float32, "out")
+    M, N = x.shape
+    ws, nbytes = None, 0
+    if _ordered():
+        nbytes = LIB.mmfb_colsum_workspace_bytes(M, N)
+        ws = _workspace(nbytes, x.device)
+    check(LIB.mmfb_colsum_bounded(x.data_ptr(), x.stride(0), out.data_ptr(), M, N, _bound(m_bound, "m_bound"), _ptr(ws),
+                                  nbytes, _stream_ptr()))
+    return out
+
+
+class SelectedRows:
+    """Device state of mmfb_select_rows over M labels: `count` (int32 [1]), `scale` (fp32 [1], 1 / max(count, 1)),
+    `pos` / `inv` (int32 [M]) and the gathered `labels` (int64 [M], ignore_index past count).  Nothing is read on the host."""
+
+    def __init__(self, state, labels):
+        M = labels.numel()
+        self.state, self.labels = state, labels
+        self.count = state[0:1]
+        self.scale = state[1:2].view(torch.float32)
+        self.pos, self.inv = state[2:2 + M], state[2 + M:]
+
+
+def select_rows(labels, ignore_index):
+    """the rows whose label != ignore_index, in row-major order, selected on the device (mmfb_select_rows)"""
+    _req(labels, torch.int64, "labels")
+    if not labels.is_contiguous():
+        raise ValueError("select_rows: labels must be contiguous")
+    M = labels.numel()
+    state = torch.empty(2 + 2 * M, dtype=torch.int32, device=labels.device)
+    out = torch.empty(M, dtype=torch.int64, device=labels.device)
+    check(LIB.mmfb_select_rows(labels.data_ptr(), int(ignore_index), M, state.data_ptr(), out.data_ptr(), _stream_ptr()))
+    return SelectedRows(state, out)
+
+
+def gather_rows(x, idx, out=None):
+    """out[r] = x[idx[r]] where idx[r] >= 0, else 0 (bf16 rows; idx int32 on the device)"""
+    _req(x, torch.bfloat16, "x"); _req(idx, torch.int32, "idx")
+    M, H = idx.numel(), x.shape[1]
+    if out is None:
+        out = torch.empty(M, H, dtype=torch.bfloat16, device=x.device)
+    _req(out, torch.bfloat16, "out")
+    if tuple(out.shape) != (M, H):
+        raise ValueError("gather_rows: out must be [%d, %d]" % (M, H))
+    check(LIB.mmfb_gather_rows(x.data_ptr(), x.stride(0), idx.data_ptr(), out.data_ptr(), out.stride(0), M, H,
+                               _stream_ptr()))
+    return out
 
 
 def add(a, b):

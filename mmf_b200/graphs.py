@@ -13,12 +13,41 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
   * inputs: static device tensors, refreshed by `copy_` on the replay stream (shapes are fixed at capture);
   * deterministic mode: the graph records the reductions that torch.use_deterministic_algorithms selected AT CAPTURE
     (mmf_b200.functional reads the flag per call): a step captured under the flag replays the ordered kernels, and one
-    captured without it replays the atomic ones, whatever the flag says at replay.  Capture under the mode you want.
+    captured without it replays the atomic ones, whatever the flag says at replay.  Capture under the mode you want;
+  * masked-LM losses: their labelled rows are a data-dependent number, found on the host in an eager step.  Inside
+    `static_rows()` the heads (mmf_b200.heads.masked_lm_loss "fused" / "masked", mmf_b200.mmft.MLMHead) select and count
+    them on the device instead and bound the vocabulary-sized kernels by that count, so the step can be captured;
+    `GraphedStep(..., static_rows=True)` captures under it.  Such a step returns no MLM logits.
 The reference has no counterpart (its trainer launches eagerly, mmf/trainers/core/training_loop.py:185-213); this is the
 answer to SURVEY.md 8a's "at T = R = 36 everything is launch-bound"."""
+import contextlib
+
 import torch
 
 from . import functional as F
+
+_STATIC_ROWS = [0]      # depth of nested static_rows() contexts
+
+
+@contextlib.contextmanager
+def static_rows():
+    """Run the masked-LM heads in static-rows mode while the context is open: the labelled rows are selected on the device
+    into a fixed capacity (every row of the labels), the vocabulary GEMM and loss are bounded by the device count, the loss
+    is the same mean cross-entropy and `logits` is None.  Nothing is read on the host, so the step can be captured.  A
+    batch with no labelled row gives a loss of exactly 0 and zero gradients."""
+    _STATIC_ROWS[0] += 1
+    try:
+        yield
+    finally:
+        _STATIC_ROWS[0] -= 1
+
+
+_static_rows_context = static_rows     # GraphedStep's `static_rows` argument shadows the name
+
+
+def static_rows_active():
+    """whether a static_rows() context is open (read by the masked-LM heads on every forward)"""
+    return _STATIC_ROWS[0] > 0
 
 
 def _map(fn, x):
@@ -41,9 +70,17 @@ def _copy_into(dst, src):
 
 
 class GraphedStep:
-    def __init__(self, model, loss_fn, example_batch, warmup=3):
+    def __init__(self, model, loss_fn, example_batch, warmup=3, static_rows=False):
         """loss_fn(batch) -> scalar loss; `example_batch`: (nested dict / list of) CUDA tensors with the shapes of every later
-        batch.  The model must be in the mode (train / eval) it will be replayed in."""
+        batch.  The model must be in the mode (train / eval) it will be replayed in.
+
+        The batch must carry every input the forward would otherwise build from a Python value: a tensor made from a
+        host value during capture is frozen into the graph or is a copy the capture refuses.  ViLT's `is_correct`, for
+        one, is made by torch.tensor when the batch lacks it.
+
+        static_rows=True: warm-up and capture run inside static_rows(), so a model whose only refusal is the masked-LM
+        row gather (it declares `static_rows_capturable = True`: VinVL, ViLT with an `mlm` head) is accepted, and LXMERT's
+        masked-LM loss is captured too.  Opt-in because the replayed step differs from an eager one: no MLM logits."""
         if any(getattr(m.__dict__.get("_runner"), "skip_padding", False) for m in model.modules()):
             raise RuntimeError("GraphedStep: the model has skip_padding encoders, which read the token count on the host and "
                                "cannot be captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)")
@@ -52,10 +89,15 @@ class GraphedStep:
                                "counts on the host and cannot be captured; turn them off with "
                                "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)")
         for m in model.modules():
-            if getattr(m, "graph_capturable", True) is False:
+            if getattr(m, "graph_capturable", True) is False and not (static_rows and getattr(m, "static_rows_capturable",
+                                                                                           False)):
                 reason = getattr(m, "graph_refusal", "does work on the host in every forward")
                 raise RuntimeError("GraphedStep: %s %s, so its step cannot be captured" % (type(m).__name__, reason))
         self.model, self.loss_fn = model, loss_fn
+        with _static_rows_context() if static_rows else contextlib.nullcontext():
+            self._capture(model, loss_fn, example_batch, warmup)
+
+    def _capture(self, model, loss_fn, example_batch, warmup):
         self.static = _map(lambda t: t.detach().clone(), example_batch)
         dev = next(t for t in _flatten(self.static) if t.is_cuda).device
         self.epoch = F.dropout_epoch(dev, create=True)

@@ -16,10 +16,14 @@ column slice of the padded product; autograd's slice / pad backward routes the g
 `positions="masked"` evaluates only the rows whose label is not ignore_index (what MMFT's MLM head does,
 mmf/models/transformers/heads/mlm.py:79-82): identical loss, ~7x less work; the default reproduces the reference's
 full `logits` output.
+Inside mmf_b200.graphs.static_rows() the "fused" and "masked" positions run `static_masked_lm_loss`: the labelled rows
+are selected and counted on the device, so the head can be captured in a CUDA graph (no logits are returned).
 """
 import torch
 from torch import nn
 
+from . import functional as F
+from . import graphs
 from . import ops
 from .modules import _init_bert_weights, _require_cuda
 
@@ -74,14 +78,30 @@ class B200BertPreTrainingHeads(nn.Module):
         return scores, self.seq_relationship(pooled_output)
 
 
+def static_masked_lm_loss(predictions, sequence_output, labels, ignore_index=-1):
+    """mean CE of the masked-LM head over the labelled rows, with no host read: the rows are selected on the device
+    (F.select_rows) into a fixed capacity of every row of `labels`, zero past the count; the transform runs on the whole
+    capacity, the vocabulary GEMM and the loss only on the labelled rows (ops.linear_cross_entropy_static).  A batch with
+    no labelled row gives a loss of exactly 0 and zero gradients.  `predictions` is a B200BertLMPredictionHead."""
+    H = sequence_output.shape[-1]
+    sel = F.select_rows(labels.reshape(-1).to(torch.int64).contiguous(), ignore_index)
+    rows = ops.gather_rows(sequence_output.reshape(-1, H), sel)
+    h = predictions.transform(rows)
+    return ops.linear_cross_entropy_static(h, predictions.decoder.weight, predictions.bias, sel.labels, sel.count,
+                                           sel.scale, ignore_index)
+
+
 def masked_lm_loss(cls, sequence_output, masked_lm_labels, ignore_index=-1, positions="all"):
     """the reference's loss (visual_bert.py:269-277).  Returns (loss, logits): logits are [B,S,V] for positions="all",
     [n_masked, V] for positions="masked" (rows in row-major order of the labelled positions).
     positions="fused": the labelled rows are gathered first (like "masked": identical loss and gradients, the ignored rows
     contribute nothing), then transform -> vocabulary GEMM -> cross-entropy run chunk by chunk with the loss kernel writing
-    d(logits) in place (ops.linear_cross_entropy): no logits tensor is returned (None) or ever materialised as a whole."""
+    d(logits) in place (ops.linear_cross_entropy): no logits tensor is returned (None) or ever materialised as a whole.
+    Inside graphs.static_rows(), "fused" and "masked" run static_masked_lm_loss and return (loss, None)."""
     labels = masked_lm_labels.reshape(-1)
     H = sequence_output.shape[-1]
+    if positions in ("fused", "masked") and graphs.static_rows_active():
+        return static_masked_lm_loss(cls.predictions, sequence_output, labels, ignore_index), None
     if positions == "fused":
         idx = torch.nonzero(labels != ignore_index, as_tuple=False).squeeze(1)
         if idx.numel() == 0:

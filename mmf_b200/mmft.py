@@ -29,7 +29,8 @@ from torch import nn
 
 from . import ops
 from .encoders import build_encoder
-from .heads import B200BertLMPredictionHead, B200BertPredictionHeadTransform
+from .graphs import static_rows_active
+from .heads import B200BertLMPredictionHead, B200BertPredictionHeadTransform, static_masked_lm_loss
 from .models import BERT_BASE, MODEL_DEFAULTS, B200Linear, BaseModel, ConfigNode
 from .modules import _init_bert_weights
 from .registry import registry
@@ -127,6 +128,10 @@ class MLMHead(nn.Module):
             assert processed_sample_list.get("mlm_labels") is not None
             assert "combined_labels" in processed_sample_list["mlm_labels"]
             labels = processed_sample_list["mlm_labels"]["combined_labels"]
+        if static_rows_active():
+            # rows selected and counted on the device (mmf_b200.graphs.static_rows): capturable, no logits, no warning
+            loss = static_masked_lm_loss(self.cls.predictions, sequence_output, labels, c.ignore_index)
+            return {"logits": None, "losses": {c.loss_name: loss}}
         sel = labels.ne(c.ignore_index)                             # gather the labelled rows first (mlm.py:79-82)
         labels = labels[sel]
         if labels.numel() == 0:

@@ -287,6 +287,91 @@ def linear_cross_entropy(h2d, weight, bias, labels, ignore_index=-1, chunk_rows=
     return _LinearCrossEntropy.apply(h2d, weight, bias, labels, int(ignore_index), int(chunk_rows))
 
 
+class _GatherRows(torch.autograd.Function):
+    """rows [M, H] = x[sel.pos] with zero rows past sel.count (mmfb_gather_rows by pos); backward: the same kernel by
+    sel.inv writes the whole input gradient, the gathered gradient at the selected rows and zero elsewhere"""
+
+    @staticmethod
+    def forward(ctx, x, sel):
+        ctx.sel, ctx.dtype = sel, x.dtype
+        return F.gather_rows(_bf16(x), sel.pos)
+
+    @staticmethod
+    def backward(ctx, g):
+        return F.gather_rows(g.to(torch.bfloat16).contiguous(), ctx.sel.inv).to(ctx.dtype), None
+
+
+def gather_rows(x2d, sel):
+    """the rows of x2d [M, H] that F.select_rows selected, as a fixed-capacity [M, H] bf16 tensor (zeros past count)"""
+    return _GatherRows.apply(x2d, sel)
+
+
+class _LinearCrossEntropyStatic(torch.autograd.Function):
+    """_LinearCrossEntropy on a fixed capacity of rows of which the first `count` (a device int32) are labelled and the
+    rest hold zero features and ignore_index labels - the static-rows mode a CUDA graph can capture (mmf_b200.graphs).
+
+    The chunk loop runs over the whole capacity; every vocabulary-sized kernel of a chunk (the GEMM, ce_rows, the dgrad,
+    the wgrad and the bias column sum) takes the chunk's share of `count` as a device bound, so a chunk that starts past
+    `count` costs launches whose CTAs exit at once, and inside a chunk only the rows below `count` rounded up to a
+    128-row tile are computed.  The loss is loss_sum * scale with `scale` = 1 / max(count, 1) in device memory: no host
+    read.  In deterministic mode the row losses are summed over the whole capacity in one fixed-shape sum."""
+
+    @staticmethod
+    def forward(ctx, h, weight, bias, labels, count, scale, ignore_index, chunk_rows):
+        hb, wb = _bf16(h), _bf16(weight)
+        V, K = wb.shape
+        pad = (-V) % 8
+        if pad:
+            wb = torch.nn.functional.pad(wb, (0, 0, 0, pad))
+        bb = _bf16(bias) if bias is not None else torch.zeros(V, dtype=torch.bfloat16, device=wb.device)
+        if pad:
+            bb = torch.cat([bb, torch.full((pad,), -30000.0, dtype=torch.bfloat16, device=bb.device)])
+        M = hb.shape[0]
+        labels = labels.reshape(-1).to(torch.int64).contiguous()
+        need_h, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        need_b = bias is not None and ctx.needs_input_grad[2]
+        # rows past count are never written by the bounded kernels: their gradients stay the zeros allocated here
+        dh = torch.zeros_like(hb) if need_h else None
+        dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device) if need_w else None
+        db = torch.zeros(wb.shape[0], dtype=torch.float32, device=wb.device) if need_b else None
+        ordered = torch.are_deterministic_algorithms_enabled()
+        loss_sum = torch.zeros((), dtype=torch.float32, device=wb.device)
+        row_loss = torch.zeros(M, dtype=torch.float32, device=wb.device) if ordered else None
+        # the labelled rows of chunk i: clamp(count - i * chunk_rows, 0, chunk_rows), one device int32 per chunk
+        starts = torch.arange(0, M, chunk_rows, dtype=torch.int32, device=wb.device)
+        bounds = (count.reshape(1) - starts).clamp_(0, chunk_rows)
+        for i, r0 in enumerate(range(0, M, chunk_rows)):
+            r1 = min(M, r0 + chunk_rows)
+            nb = bounds[i:i + 1]
+            z = F.gemm(hb[r0:r1], wb, epi=lib.EPI_BIAS, bias=bb, m_bound=nb)
+            F.ce_rows_bounded(z, labels[r0:r1], ignore_index, scale, nb, loss_sum=loss_sum,
+                              row_loss=row_loss[r0:r1] if ordered else None)
+            if need_h:
+                F.gemm(z, wb, b_mn=True, epi=lib.EPI_BIAS, out=dh[r0:r1], m_bound=nb)
+            if need_w:
+                F.gemm(z, hb[r0:r1], a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
+                       splits=best_splits(wb.shape[0], K, r1 - r0), k_bound=nb)
+            if need_b:
+                F.colsum_bounded(z, db, nb)
+        if ordered:
+            loss_sum = row_loss.sum()
+        ctx.save_for_backward(*[t for t in (dh, dw, db) if t is not None])
+        ctx.have = (need_h, need_w, need_b)
+        ctx.V = V
+        ctx.dtypes = (h.dtype, weight.dtype, bias.dtype if bias is not None else None)
+        return loss_sum * scale.reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        return _LinearCrossEntropy.backward(ctx, g) + (None, None)
+
+
+def linear_cross_entropy_static(h2d, weight, bias, labels, count, scale, ignore_index=-1, chunk_rows=2048):
+    """linear_cross_entropy over a fixed capacity of rows whose first `count` (int32 [1] on the device) are the labelled
+    ones; `scale` (fp32 [1] on the device) = 1 / max(count, 1).  Rows past count must hold ignore_index labels."""
+    return _LinearCrossEntropyStatic.apply(h2d, weight, bias, labels, count, scale, int(ignore_index), int(chunk_rows))
+
+
 class _LinearT(torch.autograd.Function):
     """y = x W + b with W stored [K, N]: the GEMM reads the weight MN-major (the layout the dgrad calls use), so a weight
     that is another layer's nn.Linear weight - MRFR's projection back to the feature space, tied to UNITER's img_linear

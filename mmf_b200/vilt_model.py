@@ -131,6 +131,7 @@ class ViLT(BaseModel):
     an `mlp` head, masked-COCO pretraining through `mlm_multi` + `itm`"""
 
     graph_refusal = "gathers a data-dependent number of rows (the labelled masked-LM positions) in every pretraining forward"
+    static_rows_capturable = True   # that gather is the only refusal: GraphedStep(..., static_rows=True) captures the step
 
     @classmethod
     def config_path(cls):

@@ -133,6 +133,7 @@ class VinVL(BaseModel):
 
     graph_capturable = False        # see mmf_b200.graphs.GraphedStep
     graph_refusal = "gathers a data-dependent number of rows (the labelled masked-LM positions) in every pretraining forward"
+    static_rows_capturable = True   # that gather is the only refusal: GraphedStep(..., static_rows=True) captures the step
 
     def __init__(self, config):
         super().__init__(config)
