@@ -93,8 +93,11 @@ int64_t mmfb_gemm_workspace_bytes(int M, int N, int K, int splits);
  * weight gradient, where K is the row count), the k-blocks [0, ceil(b/64)) are shared among the launched splits the way an
  * unbounded call with K = b shares them; a split left without a k-block adds nothing, or with a workspace stores a zero
  * partial.  So the operand rows between b and the rounded bound are read: the caller keeps them zero.  Supported for
- * MMFB_EPI_BIAS with (a_mn, b_mn) = (0, 0) or (0, 1) and for MMFB_EPI_ATOMIC_F32 with (1, 1), with or without a
- * workspace (with one, the ordered reduce also covers only the rows below the rounded M bound: the rows of C past it
+ * MMFB_EPI_BIAS with (a_mn, b_mn) = (0, 0) or (0, 1), for MMFB_EPI_ATOMIC_F32 with (1, 1), with or without a
+ * workspace, and for the encoder layer's epilogues: MMFB_EPI_BIAS_GELU and MMFB_EPI_BIAS_DROP_RESID with (0, 0),
+ * MMFB_EPI_GELU_BWD and MMFB_EPI_ADD_AUX with (0, 1).  Their per-row operands (aux, the dropout keep bits) are read only
+ * for the row tiles below the rounded bound, like A; C and C2 are written only there.  A row between b and the rounded
+ * bound is computed from whatever its operand rows hold and affects no other row (with one, the ordered reduce also covers only the rows below the rounded M bound: the rows of C past it
  * are not read or written, and the workspace rows past it are not read); anything else is MMFB_ERR_ARG before a launch.
  * A bound of 0 adds nothing to C. */
 int mmfb_gemm_bounded(const mmfb_gemm_args* args, const int32_t* m_dev, const int32_t* k_dev, mmfb_stream stream);
@@ -231,6 +234,16 @@ typedef struct {
 
 int mmfb_layernorm_fwd(const mmfb_ln_args* args, mmfb_stream stream);
 int mmfb_layernorm_bwd(const mmfb_ln_args* args, mmfb_stream stream);
+
+/* The LayerNorm calls with a DEVICE int32 row bound m_dev (non-NULL, 4-byte aligned): with b = clamp(*m_dev, 0, M), read
+ * when the kernel runs, only rows [0, b) of every row tensor (y, x, mean, rstd, dx, dx2, dy, dz, the keep bits) are read
+ * or written; the rows at and past b keep what they held.  Every shape the unbounded calls take is covered, with the
+ * same limits.  Row outputs equal those of the unbounded call with M = b, bit for bit.  dgamma / dbeta / dbias sum the
+ * rows below b only.  With a workspace (sized for M) the chunks at and past b store zero partials, so the result equals
+ * an unbounded ordered call with M = b (the same 128-row chunks) bit for bit.  An encoder layer captured in a CUDA graph
+ * runs its LayerNorms this way on a fixed capacity of packed rows, of which the first b are tokens. */
+int mmfb_layernorm_fwd_bounded(const mmfb_ln_args* args, const int32_t* m_dev, mmfb_stream stream);
+int mmfb_layernorm_bwd_bounded(const mmfb_ln_args* args, const int32_t* m_dev, mmfb_stream stream);
 
 /* Ordered reductions over rows.  The rows are cut into chunks of 128 (chunk k = rows [128k, 128k + 128)), a number that
  * depends on M alone.  Each chunk sums its rows in a fixed order (8 warps, warp w taking rows w, w + 8, ... of the chunk,

@@ -196,6 +196,16 @@ int mmfb_layernorm_bwd(const mmfb_ln_args* args, mmfb_stream stream) {
   MMFB_REQUIRE_DEVICE();
   return ln_bwd(*args, reinterpret_cast<cudaStream_t>(stream));
 }
+int mmfb_layernorm_fwd_bounded(const mmfb_ln_args* args, const int32_t* m_dev, mmfb_stream stream) {
+  if (!args || !m_dev) return set_error(MMFB_ERR_ARG, "mmfb_layernorm_fwd_bounded: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return ln_fwd(*args, reinterpret_cast<cudaStream_t>(stream), m_dev);
+}
+int mmfb_layernorm_bwd_bounded(const mmfb_ln_args* args, const int32_t* m_dev, mmfb_stream stream) {
+  if (!args || !m_dev) return set_error(MMFB_ERR_ARG, "mmfb_layernorm_bwd_bounded: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return ln_bwd(*args, reinterpret_cast<cudaStream_t>(stream), m_dev);
+}
 int mmfb_colsum(const void* X, int64_t ldx, float* out, int M, int N, mmfb_stream stream) {
   if (!X || !out) return set_error(MMFB_ERR_ARG, "mmfb_colsum: null pointer");
   MMFB_REQUIRE_DEVICE();

@@ -494,13 +494,19 @@ static int dispatch(const mmfb_gemm_args& a, cudaStream_t s) {
   }
 }
 
-// The device-bounded instantiations (m_dev / k_dev set): the masked-LM head's vocabulary GEMM, its dgrad and its wgrad.
+// The device-bounded instantiations (m_dev / k_dev set): the masked-LM head's vocabulary GEMM, its dgrad and its wgrad,
+// and the encoder layer's GEMMs on a fixed capacity of packed rows (QKV / O-proj / FFN-up / FFN-down and their dgrads).
+// A row tile at or past the rounded bound is no unit, so nothing of it is loaded (A, the aux box) or stored (C, C2).
 template <int BN>
 static int dispatch_bounded(const mmfb_gemm_args& a, cudaStream_t s, const int32_t* m_dev, const int32_t* k_dev) {
   const int key = (a.a_mn ? 100 : 0) + (a.b_mn ? 10 : 0) + a.epi;
   switch (key) {
     case 0 + EPI_BIAS: return launch<BN, false, false, EPI_BIAS, true>(a, s, m_dev, k_dev);
+    case 0 + EPI_BIAS_GELU: return launch<BN, false, false, EPI_BIAS_GELU, true>(a, s, m_dev, k_dev);
+    case 0 + EPI_BIAS_DROP_RESID: return launch<BN, false, false, EPI_BIAS_DROP_RESID, true>(a, s, m_dev, k_dev);
     case 10 + EPI_BIAS: return launch<BN, false, true, EPI_BIAS, true>(a, s, m_dev, k_dev);
+    case 10 + EPI_GELU_BWD: return launch<BN, false, true, EPI_GELU_BWD, true>(a, s, m_dev, k_dev);
+    case 10 + EPI_ADD_AUX: return launch<BN, false, true, EPI_ADD_AUX, true>(a, s, m_dev, k_dev);
     case 110 + EPI_ATOMIC_F32: return launch<BN, true, true, EPI_ATOMIC_F32, true>(a, s, m_dev, k_dev);
     default:
       return set_error(MMFB_ERR_ARG, "gemm: a device bound (m_dev / k_dev) is not supported for (a_mn=%d, b_mn=%d, epi=%d)",

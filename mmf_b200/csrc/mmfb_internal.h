@@ -86,8 +86,9 @@ int attn_causal_bwd(const mmfb_attn_args& a, cudaStream_t stream);
 // packed self-attention with a causal tail (attention_varlen_causal.cu)
 int attn_varlen_causal_fwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream);
 int attn_varlen_causal_bwd(const mmfb_attn_args& a, const int32_t* cu, int total, cudaStream_t stream);
-int ln_fwd(const mmfb_ln_args& a, cudaStream_t s);
-int ln_bwd(const mmfb_ln_args& a, cudaStream_t s);
+// m_dev: the device row bound of mmfb_layernorm_*_bounded (NULL: none)
+int ln_fwd(const mmfb_ln_args& a, cudaStream_t s, const int32_t* m_dev = nullptr);
+int ln_bwd(const mmfb_ln_args& a, cudaStream_t s, const int32_t* m_dev = nullptr);
 int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s);
 int colsum_ordered(const void* X, int64_t ldx, float* out, int M, int N, float* ws, int64_t ws_bytes, cudaStream_t s);
 int dropout_bits(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t offset, float p, const uint64_t* epoch, cudaStream_t s);

@@ -35,15 +35,18 @@ __device__ __forceinline__ void st8(bf16* p, const float (&f)[8]) {
 
 // ----------------------------------------------------------------------------------------------
 // LayerNorm forward:  x = LN(y) * gamma + beta  (+ optional dropout on the OUTPUT, used by the embeddings)
+// BOUNDED (all LayerNorm kernels): only the rows below min(M, *m_dev) are read and written - an encoder layer's rows on a
+// fixed capacity of which a device-counted prefix is valid (packed skip-padding under CUDA-graph capture).
 // ----------------------------------------------------------------------------------------------
-template <int NV>
+template <int NV, bool BOUNDED = false>
 __global__ void __launch_bounds__(ROW_WARPS * 32)
 ln_fwd_kernel(const bf16* __restrict__ y, int64_t ldy, const bf16* __restrict__ gamma,
               const bf16* __restrict__ beta, bf16* __restrict__ x, int64_t ldx, float* __restrict__ mean,
               float* __restrict__ rstd, const uint32_t* __restrict__ dmask, int64_t ldmask, float dscale, int M,
-              int H, float eps) {
+              int H, float eps, const int32_t* __restrict__ m_dev = nullptr) {
   griddep_launch();
   griddep_wait();
+  if constexpr (BOUNDED) M = min(M, max(*m_dev, 0));
   const int lane = threadIdx.x & 31;
   const int64_t row = static_cast<int64_t>(blockIdx.x) * ROW_WARPS + (threadIdx.x >> 5);
   if (row >= M) return;
@@ -105,18 +108,21 @@ ln_fwd_kernel(const bf16* __restrict__ y, int64_t ldy, const bf16* __restrict__ 
 // ORDERED (both kernels): block b owns the rows of chunk b (ORDER_ROWS rows, warp w taking rows w, w + ROW_WARPS, ...) and
 // stores its three column-sum sets to ws[b][which][H] instead of adding them to dgamma / dbeta / dbias; chunk_reduce_kernel
 // adds them up in chunk order.  The row outputs dy / dz do not depend on which block computes a row.
+// BOUNDED (both kernels): M becomes min(M, *m_dev) on the device.  The grid stays sized from M: an ordered chunk at or past
+// the bound stores zero partials, so the reduce adds what an unbounded ordered call with M = bound adds, then zeros.
 // Rows of up to MAXV * 256 columns: a warp loads, computes and stores a row held in registers, and only the other warps
 // of the SM cover its load latency.
-template <bool ORDERED>
+template <bool ORDERED, bool BOUNDED = false>
 __global__ void __launch_bounds__(ROW_WARPS * 32)
 ln_bwd_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict__ dx2, int64_t lddx2,
               const bf16* __restrict__ y, int64_t ldy, const float* __restrict__ mean,
               const float* __restrict__ rstd, const bf16* __restrict__ gamma, bf16* __restrict__ dy, int64_t lddy,
               bf16* __restrict__ dz, int64_t lddz, const uint32_t* __restrict__ dmask, int64_t ldmask, float dscale,
               float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M, int H,
-              float* __restrict__ ws) {
+              float* __restrict__ ws, const int32_t* __restrict__ m_dev = nullptr) {
   griddep_launch();
   griddep_wait();
+  if constexpr (BOUNDED) M = min(M, max(*m_dev, 0));
   __shared__ float red[ROW_WARPS][256];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   float ag[MAXV][8], ab[MAXV][8], az[MAXV][8];
@@ -229,16 +235,17 @@ __device__ __forceinline__ void bulk_load_1d(void* dst_smem, const void* src, ui
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(dst_smem)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-template <int NV, bool HAS_DX2, int ST, bool ORDERED>
+template <int NV, bool HAS_DX2, int ST, bool ORDERED, bool BOUNDED = false>
 __global__ void __launch_bounds__(ROW_WARPS * 32, 2)
 ln_bwd_stream_kernel(const bf16* __restrict__ dx, int64_t lddx, const bf16* __restrict__ dx2, int64_t lddx2,
                      const bf16* __restrict__ y, int64_t ldy, const float* __restrict__ mean,
                      const float* __restrict__ rstd, const bf16* __restrict__ gamma, bf16* __restrict__ dy, int64_t lddy,
                      bf16* __restrict__ dz, int64_t lddz, const uint32_t* __restrict__ dmask, int64_t ldmask, float dscale,
                      float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias, int M_rows, int H,
-                     float* __restrict__ ws) {
+                     float* __restrict__ ws, const int32_t* __restrict__ m_dev = nullptr) {
   griddep_launch();
   griddep_wait();
+  if constexpr (BOUNDED) M_rows = min(M_rows, max(*m_dev, 0));
   // the bound of the rows this block visits: its chunk's end when ORDERED
   const int M = ORDERED ? min(M_rows, static_cast<int>(blockIdx.x + 1) * ORDER_ROWS) : M_rows;
   constexpr int NT = HAS_DX2 ? 3 : 2;                 // tensors per slot: dx, y (, dx2)
@@ -846,18 +853,25 @@ static int check_aligned(const char* who, int M, std::initializer_list<RowTensor
   return MMFB_OK;
 }
 
-int ln_fwd(const mmfb_ln_args& a, cudaStream_t s) {
+int ln_fwd(const mmfb_ln_args& a, cudaStream_t s, const int32_t* m_dev) {
   int rc = check_rows(a.M, a.H, "layernorm_fwd");
   if (rc) return rc;
   if (!a.y || !a.gamma || !a.beta || !a.x) return set_error(MMFB_ERR_ARG, "layernorm_fwd: null pointer");
   rc = check_aligned("layernorm_fwd", a.M, {{a.y, a.ldy, "y"}, {a.x, a.ldx, "x"}, {a.gamma, 0, "gamma"}, {a.beta, 0, "beta"}});
   if (rc) return rc;
-#define LN_FWD(NV)                                                                                         \
-  MMFB_LAUNCH(ln_fwd_kernel<NV>, (a.M + ROW_WARPS - 1) / ROW_WARPS, ROW_WARPS * 32, 0, s,                           \
+  if (reinterpret_cast<uintptr_t>(m_dev) & 3) return set_error(MMFB_ERR_ARG, "layernorm_fwd: m_dev must be 4-byte aligned");
+#define LN_FWD(NV, BND)                                                                                    \
+  MMFB_LAUNCH((ln_fwd_kernel<NV, BND>), (a.M + ROW_WARPS - 1) / ROW_WARPS, ROW_WARPS * 32, 0, s,                    \
       (const bf16*)a.y, a.ldy, (const bf16*)a.gamma, (const bf16*)a.beta, (bf16*)a.x, a.ldx, a.mean, a.rstd, \
-      a.drop_mask, a.ldmask, a.drop_scale, a.M, a.H, a.eps)
+      a.drop_mask, a.ldmask, a.drop_scale, a.M, a.H, a.eps, m_dev)
   const int nv = (a.H + 255) / 256;
-  if (nv <= 1) LN_FWD(1); else if (nv == 2) LN_FWD(2); else if (nv == 3) LN_FWD(3); else if (nv == 4) LN_FWD(4); else LN_FWD(8);
+  if (m_dev != nullptr) {
+    if (nv <= 1) LN_FWD(1, true); else if (nv == 2) LN_FWD(2, true); else if (nv == 3) LN_FWD(3, true);
+    else if (nv == 4) LN_FWD(4, true); else LN_FWD(8, true);
+  } else {
+    if (nv <= 1) LN_FWD(1, false); else if (nv == 2) LN_FWD(2, false); else if (nv == 3) LN_FWD(3, false);
+    else if (nv == 4) LN_FWD(4, false); else LN_FWD(8, false);
+  }
 #undef LN_FWD
   return launch_ok("layernorm_fwd");
 }
@@ -892,11 +906,11 @@ static int chunk_reduce(const float* ws, int chunks, int n, float* out0, float* 
   return launch_ok(who);
 }
 
-template <int NV, bool HAS_DX2, int ST, bool ORDERED>
-static int ln_bwd_stream(const mmfb_ln_args& a, cudaStream_t s) {
+template <int NV, bool HAS_DX2, int ST, bool ORDERED, bool BOUNDED>
+static int ln_bwd_stream(const mmfb_ln_args& a, cudaStream_t s, const int32_t* m_dev) {
   constexpr size_t smem = static_cast<size_t>(ROW_WARPS) * ST * (HAS_DX2 ? 3 : 2) * NV * 512 + ROW_WARPS * 256 * 4 +
                           NV * 256 * 4 + 4096 + ROW_WARPS * ST * 8;
-  auto kern = ln_bwd_stream_kernel<NV, HAS_DX2, ST, ORDERED>;
+  auto kern = ln_bwd_stream_kernel<NV, HAS_DX2, ST, ORDERED, BOUNDED>;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
@@ -905,34 +919,44 @@ static int ln_bwd_stream(const mmfb_ln_args& a, cudaStream_t s) {
   }
   MMFB_LAUNCH(kern, ORDERED ? order_chunks(a.M) : ln_bwd_grid(a.M), ROW_WARPS * 32, smem, s, (const bf16*)a.dx, a.lddx,
               (const bf16*)a.dx2, a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy, a.lddy,
-              (bf16*)a.dz, a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H, a.workspace);
+              (bf16*)a.dz, a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H, a.workspace,
+              m_dev);
   return launch_ok("layernorm_bwd");
+}
+
+// ln_bwd_stream<NV, HAS_DX2, ST, ORDERED, BOUNDED> indexed by [dx2 given][NV - 1]; NV = 256-column slabs per row, ST = ring
+// depth (the same depths with and without the bound)
+template <bool ORDERED, bool BOUNDED>
+static int ln_bwd_stream_dispatch(const mmfb_ln_args& a, cudaStream_t s, const int32_t* m_dev) {
+  static int (*const stream[2][4])(const mmfb_ln_args&, cudaStream_t, const int32_t*) = {
+      {ln_bwd_stream<1, false, 4, ORDERED, BOUNDED>, ln_bwd_stream<2, false, 4, ORDERED, BOUNDED>,
+       ln_bwd_stream<3, false, 3, ORDERED, BOUNDED>, ln_bwd_stream<4, false, 2, ORDERED, BOUNDED>},
+      {ln_bwd_stream<1, true, 3, ORDERED, BOUNDED>, ln_bwd_stream<2, true, 3, ORDERED, BOUNDED>,
+       ln_bwd_stream<3, true, 2, ORDERED, BOUNDED>, ln_bwd_stream<4, true, 2, ORDERED, BOUNDED>}};
+  return stream[a.dx2 != nullptr][(a.H + 255) / 256 - 1](a, s, m_dev);
 }
 
 // The ordered LayerNorm backward: the kernels above with one block per chunk of rows, then the chunk partials of dgamma,
 // dbeta and dbias added in chunk order.  Same ring depths as the atomic path.
-static int ln_bwd_ordered(const mmfb_ln_args& a, bool wide, cudaStream_t s) {
+template <bool BOUNDED>
+static int ln_bwd_ordered(const mmfb_ln_args& a, bool wide, cudaStream_t s, const int32_t* m_dev) {
   const int chunks = order_chunks(a.M);
   if (wide) {
-    MMFB_LAUNCH(ln_bwd_kernel<true>, chunks, ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2,
-                a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy, a.lddy, (bf16*)a.dz,
-                a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H, a.workspace);
+    MMFB_LAUNCH((ln_bwd_kernel<true, BOUNDED>), chunks, ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx,
+                (const bf16*)a.dx2, a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy,
+                a.lddy, (bf16*)a.dz, a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H,
+                a.workspace, m_dev);
     int rc = launch_ok("layernorm_bwd");
     if (rc) return rc;
   } else {
-    static int (*const stream[2][4])(const mmfb_ln_args&, cudaStream_t) = {
-        {ln_bwd_stream<1, false, 4, true>, ln_bwd_stream<2, false, 4, true>, ln_bwd_stream<3, false, 3, true>,
-         ln_bwd_stream<4, false, 2, true>},
-        {ln_bwd_stream<1, true, 3, true>, ln_bwd_stream<2, true, 3, true>, ln_bwd_stream<3, true, 2, true>,
-         ln_bwd_stream<4, true, 2, true>}};
-    int rc = stream[a.dx2 != nullptr][(a.H + 255) / 256 - 1](a, s);
+    int rc = ln_bwd_stream_dispatch<true, BOUNDED>(a, s, m_dev);
     if (rc) return rc;
   }
   if (!a.dgamma && !a.dbeta && !a.dbias) return MMFB_OK;
   return chunk_reduce(a.workspace, chunks, a.H, a.dgamma, a.dbeta, a.dbias, 3, s, "layernorm_bwd reduce");
 }
 
-int ln_bwd(const mmfb_ln_args& a, cudaStream_t s) {
+int ln_bwd(const mmfb_ln_args& a, cudaStream_t s, const int32_t* m_dev) {
   int rc = check_rows(a.M, a.H, "layernorm_bwd");
   if (rc) return rc;
   if (!a.dx || !a.y || !a.mean || !a.rstd || !a.gamma) return set_error(MMFB_ERR_ARG, "layernorm_bwd: null pointer");
@@ -943,24 +967,21 @@ int ln_bwd(const mmfb_ln_args& a, cudaStream_t s) {
   rc = check_aligned("layernorm_bwd", a.M, {{a.dx, a.lddx, "dx"}, {a.dx2, a.lddx2, "dx2"}, {a.y, a.ldy, "y"},
                                             {a.dy, a.lddy, "dy"}, {dz, a.lddz, "dz"}, {wide ? a.gamma : nullptr, 0, "gamma"}});
   if (rc) return rc;
+  if (reinterpret_cast<uintptr_t>(m_dev) & 3) return set_error(MMFB_ERR_ARG, "layernorm_bwd: m_dev must be 4-byte aligned");
+  const bool bounded = m_dev != nullptr;
   if (a.workspace != nullptr || a.workspace_bytes != 0) {
     rc = check_workspace("layernorm_bwd", a.workspace, a.workspace_bytes, ln_bwd_workspace_bytes(a.M, a.H));
     if (rc) return rc;
-    return ln_bwd_ordered(a, wide, s);
+    return bounded ? ln_bwd_ordered<true>(a, wide, s, m_dev) : ln_bwd_ordered<false>(a, wide, s, nullptr);
   }
   if (wide) {
-    MMFB_LAUNCH(ln_bwd_kernel<false>, ln_bwd_grid(a.M), ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2,
+    auto kern = bounded ? ln_bwd_kernel<false, true> : ln_bwd_kernel<false, false>;
+    MMFB_LAUNCH(kern, ln_bwd_grid(a.M), ROW_WARPS * 32, 0, s, (const bf16*)a.dx, a.lddx, (const bf16*)a.dx2,
                 a.lddx2, (const bf16*)a.y, a.ldy, a.mean, a.rstd, (const bf16*)a.gamma, (bf16*)a.dy, a.lddy, (bf16*)a.dz,
-                a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H, nullptr);
+                a.lddz, a.drop_mask, a.ldmask, a.drop_scale, a.dgamma, a.dbeta, a.dbias, a.M, a.H, nullptr, m_dev);
     return launch_ok("layernorm_bwd");
   }
-  // ln_bwd_stream<NV, HAS_DX2, ST> indexed by [dx2 given][NV - 1]; NV = 256-column slabs per row, ST = ring depth
-  static int (*const stream[2][4])(const mmfb_ln_args&, cudaStream_t) = {
-      {ln_bwd_stream<1, false, 4, false>, ln_bwd_stream<2, false, 4, false>, ln_bwd_stream<3, false, 3, false>,
-       ln_bwd_stream<4, false, 2, false>},
-      {ln_bwd_stream<1, true, 3, false>, ln_bwd_stream<2, true, 3, false>, ln_bwd_stream<3, true, 2, false>,
-       ln_bwd_stream<4, true, 2, false>}};
-  return stream[a.dx2 != nullptr][(a.H + 255) / 256 - 1](a, s);
+  return bounded ? ln_bwd_stream_dispatch<false, true>(a, s, m_dev) : ln_bwd_stream_dispatch<false, false>(a, s, nullptr);
 }
 
 int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s) {

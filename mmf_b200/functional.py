@@ -452,13 +452,16 @@ def pack_keep_bits(keep):
 LN_EPS = 1e-12
 
 
-def layernorm_fwd(y, gamma, beta, eps=LN_EPS, drop_mask=None, drop_scale=1.0, out=None):
-    """x, mean, rstd = LayerNorm(y) over the last dim; y bf16 [M,H] (row stride allowed)."""
+def layernorm_fwd(y, gamma, beta, eps=LN_EPS, drop_mask=None, drop_scale=1.0, out=None, m_bound=None):
+    """x, mean, rstd = LayerNorm(y) over the last dim; y bf16 [M,H] (row stride allowed).
+    m_bound: an int32 [1] CUDA tensor; only the rows below it are read and written (mmfb_layernorm_fwd_bounded), and the
+    rows past it of the tensors this call allocates are zero."""
     _req(y, torch.bfloat16, "y"); _req(gamma, torch.bfloat16, "gamma"); _req(beta, torch.bfloat16, "beta")
     M, H = y.shape
-    x = out if out is not None else torch.empty(M, H, dtype=torch.bfloat16, device=y.device)
-    mean = torch.empty(M, dtype=torch.float32, device=y.device)
-    rstd = torch.empty(M, dtype=torch.float32, device=y.device)
+    alloc = torch.empty if m_bound is None else torch.zeros
+    x = out if out is not None else alloc(M, H, dtype=torch.bfloat16, device=y.device)
+    mean = alloc(M, dtype=torch.float32, device=y.device)
+    rstd = alloc(M, dtype=torch.float32, device=y.device)
     a = LnArgs()
     a.y, a.ldy, a.gamma, a.beta = y.data_ptr(), y.stride(0), gamma.data_ptr(), beta.data_ptr()
     a.x, a.ldx, a.mean, a.rstd = x.data_ptr(), x.stride(0), mean.data_ptr(), rstd.data_ptr()
@@ -466,18 +469,23 @@ def layernorm_fwd(y, gamma, beta, eps=LN_EPS, drop_mask=None, drop_scale=1.0, ou
         _req(drop_mask, torch.int32, "drop_mask")
         a.drop_mask, a.ldmask, a.drop_scale = drop_mask.data_ptr(), drop_mask.stride(0), float(drop_scale)
     a.eps, a.M, a.H = float(eps), M, H
-    check(LIB.mmfb_layernorm_fwd(ctypes.byref(a), _stream_ptr()))
+    if m_bound is not None:
+        check(LIB.mmfb_layernorm_fwd_bounded(ctypes.byref(a), _bound(m_bound, "m_bound"), _stream_ptr()))
+    else:
+        check(LIB.mmfb_layernorm_fwd(ctypes.byref(a), _stream_ptr()))
     return x, mean, rstd
 
 
 def layernorm_bwd(dx, y, mean, rstd, gamma, dgamma, dbeta, dbias=None, dx2=None, drop_mask=None, drop_scale=1.0,
-                  need_dz=True):
+                  need_dz=True, m_bound=None):
     """Returns (dy, dz): dy = grad wrt y (goes to the residual branch), dz = grad wrt the dense output that was
     dropped before the residual add (dz is dy when there is no dropout).  dgamma/dbeta/dbias (fp32 [H]) are
-    accumulated in place."""
+    accumulated in place.  m_bound: an int32 [1] CUDA tensor; only the rows below it are read and written and summed
+    (mmfb_layernorm_bwd_bounded), and dy / dz are zero past it."""
     _req(dx, torch.bfloat16, "dx"); _req(y, torch.bfloat16, "y"); _req(gamma, torch.bfloat16, "gamma")
     M, H = y.shape
-    dy = torch.empty(M, H, dtype=torch.bfloat16, device=y.device)
+    alloc = torch.empty if m_bound is None else torch.zeros
+    dy = alloc(M, H, dtype=torch.bfloat16, device=y.device)
     a = LnArgs()
     a.dx, a.lddx = dx.data_ptr(), dx.stride(0)
     if dx2 is not None:
@@ -488,7 +496,7 @@ def layernorm_bwd(dx, y, mean, rstd, gamma, dgamma, dbeta, dbias=None, dx2=None,
     dz = dy
     if drop_mask is not None:
         _req(drop_mask, torch.int32, "drop_mask")
-        dz = torch.empty(M, H, dtype=torch.bfloat16, device=y.device)
+        dz = alloc(M, H, dtype=torch.bfloat16, device=y.device)
         a.drop_mask, a.ldmask, a.drop_scale = drop_mask.data_ptr(), drop_mask.stride(0), float(drop_scale)
     a.dz, a.lddz = dz.data_ptr(), dz.stride(0)
     for name, t in (("dgamma", dgamma), ("dbeta", dbeta), ("dbias", dbias)):
@@ -501,7 +509,10 @@ def layernorm_bwd(dx, y, mean, rstd, gamma, dgamma, dbeta, dbias=None, dx2=None,
         nbytes = LIB.mmfb_layernorm_bwd_workspace_bytes(M, H)
         ws = _workspace(nbytes, y.device)
         a.workspace, a.workspace_bytes = ws.data_ptr(), nbytes
-    check(LIB.mmfb_layernorm_bwd(ctypes.byref(a), _stream_ptr()))
+    if m_bound is not None:
+        check(LIB.mmfb_layernorm_bwd_bounded(ctypes.byref(a), _bound(m_bound, "m_bound"), _stream_ptr()))
+    else:
+        check(LIB.mmfb_layernorm_bwd(ctypes.byref(a), _stream_ptr()))
     return dy, dz
 
 

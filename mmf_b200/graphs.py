@@ -17,7 +17,10 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
   * masked-LM losses: their labelled rows are a data-dependent number, found on the host in an eager step.  Inside
     `static_rows()` the heads (mmf_b200.heads.masked_lm_loss "fused" / "masked", mmf_b200.mmft.MLMHead) select and count
     them on the device instead and bound the vocabulary-sized kernels by that count, so the step can be captured;
-    `GraphedStep(..., static_rows=True)` captures under it.  Such a step returns no MLM logits.
+    `GraphedStep(..., static_rows=True)` captures under it.  Such a step returns no MLM logits;
+  * skip-padding: a single-stream encoder with skip_padding set plans its packing on the host in an eager step.  Inside
+    `static_rows()` it plans it on the device at the capacity B*S (mmf_b200.modules._plan_packing_static) and bounds
+    every GEMM, LayerNorm and column sum of its layers by the device token count, so that step can be captured too.
 The reference has no counterpart (its trainer launches eagerly, mmf/trainers/core/training_loop.py:185-213); this is the
 answer to SURVEY.md 8a's "at T = R = 36 everything is launch-bound"."""
 import contextlib
@@ -34,7 +37,9 @@ def static_rows():
     """Run the masked-LM heads in static-rows mode while the context is open: the labelled rows are selected on the device
     into a fixed capacity (every row of the labels), the vocabulary GEMM and loss are bounded by the device count, the loss
     is the same mean cross-entropy and `logits` is None.  Nothing is read on the host, so the step can be captured.  A
-    batch with no labelled row gives a loss of exactly 0 and zero gradients."""
+    batch with no labelled row gives a loss of exactly 0 and zero gradients.
+    Single-stream skip_padding encoders (calls without a causal tail) plan their packing on the device in the same way
+    (mmf_b200.modules.run_bert_encoder)."""
     _STATIC_ROWS[0] += 1
     try:
         yield
@@ -80,14 +85,23 @@ class GraphedStep:
 
         static_rows=True: warm-up and capture run inside static_rows(), so a model whose only refusal is the masked-LM
         row gather (it declares `static_rows_capturable = True`: VinVL, ViLT with an `mlm` head) is accepted, and LXMERT's
-        masked-LM loss is captured too.  Opt-in because the replayed step differs from an eager one: no MLM logits."""
-        if any(getattr(m.__dict__.get("_runner"), "skip_padding", False) for m in model.modules()):
+        masked-LM loss is captured too.  Single-stream skip_padding encoders (patch.set_skip_padding(model)) plan their
+        packing on the device there and are captured as well, at a fixed capacity of every row of the batch.  Those with
+        `pack_tail` (set_skip_padding(..., causal=True)) and two-stream encoders with `pack_streams` are still refused.
+        Opt-in because the replayed step differs from an eager one: no MLM logits."""
+        runners = [m.__dict__.get("_runner") for m in model.modules()]
+        if not static_rows and any(getattr(r, "skip_padding", False) for r in runners):
             raise RuntimeError("GraphedStep: the model has skip_padding encoders, which read the token count on the host and "
                                "cannot be captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)")
-        if any(getattr(m.__dict__.get("_runner"), "pack_streams", False) for m in model.modules()):
+        if static_rows and any(getattr(r, "skip_padding", False) and getattr(r, "pack_tail", False) for r in runners):
+            raise RuntimeError("GraphedStep: the model has skip_padding encoders with pack_tail set, which read the token "
+                               "count on the host for calls with a causal tail even under static_rows, so they cannot be "
+                               "captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)")
+        if any(getattr(r, "pack_streams", False) for r in runners):
             raise RuntimeError("GraphedStep: the model has two-stream encoders with pack_streams set, which read the token "
-                               "counts on the host and cannot be captured; turn them off with "
-                               "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)")
+                               "counts on the host%s and cannot be captured; turn them off with "
+                               "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)"
+                               % (" even under static_rows" if static_rows else ""))
         for m in model.modules():
             if getattr(m, "graph_capturable", True) is False and not (static_rows and getattr(m, "static_rows_capturable",
                                                                                            False)):

@@ -20,6 +20,7 @@ import torch
 from torch import nn
 
 from . import engine as E
+from . import graphs
 from . import lib
 
 
@@ -193,6 +194,41 @@ def _plan_packing(mask, B, S, counts=None):
     return _Packing(rows[:total], E.Varlen(cu, B, total, max_len))
 
 
+class _StaticPacking:
+    """The packing of a padded [B, S] batch planned on the device, at the fixed capacity C = B*S (graphs.static_rows()):
+    `pack_map` (int32 [C]) holds the flat indices of the valid rows in _plan_packing's order, then -1; `unpack_map` (int32
+    [B*S]) holds each position's packed row, or -1 at padded positions.  Packing, unpacking and both backwards are one
+    row-gather kernel each (mmfb_gather_rows), and every shape depends on B and S only, so a CUDA graph can capture it.
+    `varlen` carries the device count cu[B] as Varlen.count, which bounds the layers' kernels."""
+
+    def __init__(self, pack_map, unpack_map, varlen):
+        self.pack_map, self.unpack_map, self.varlen = pack_map, unpack_map, varlen
+
+    def pack(self, t):
+        """[B*S, H] -> [C, H]: the valid rows first, in their original order within each sample, then zero rows"""
+        return E.F.gather_rows(t, self.pack_map)
+
+    def unpack(self, t, BS):
+        """[C, H] -> [B*S, H] with exact zero rows at padded positions"""
+        return E.F.gather_rows(t, self.unpack_map)
+
+
+def _plan_packing_static(mask, B, S):
+    """_plan_packing without a host read: the packing of an additive [B, S] fp32 mask (0 = token, anything else = padding)
+    at capacity B*S.  Every row valid and every row padded are planned like any other batch, and the soft-mask check of
+    _plan_packing cannot run: a mask value that is neither 0 nor <= -10000 is taken as padding without a check."""
+    C = B * S
+    valid = (mask == 0).reshape(-1)
+    incl = torch.cumsum(valid, 0, dtype=torch.int32)                    # valid rows up to and including each position
+    cu = torch.zeros(B + 1, dtype=torch.int32, device=mask.device)
+    cu[1:] = incl.view(B, S)[:, -1]
+    unpack_map = torch.where(valid, incl - 1, torch.full_like(incl, -1))
+    # packed row i comes from the first position where `incl` reaches i + 1; past the count no position does
+    pack_map = torch.searchsorted(incl, torch.arange(1, C + 1, dtype=torch.int32, device=mask.device), out_int32=True)
+    pack_map = torch.where(pack_map < C, pack_map, torch.full_like(pack_map, -1))
+    return _StaticPacking(pack_map, unpack_map, E.Varlen(cu, B, C, S, count=cu[B:]))
+
+
 def _tail_kept(mask, causal_len):
     """the key-padding mask of a call with a causal tail, as packing reads it: the mask before the tail, and 0 (kept) on
     the last causal_len positions, which the dense path does not read the mask at either"""
@@ -261,7 +297,7 @@ class _BertEncoderFn(torch.autograd.Function):
         need_grad = any(ctx.needs_input_grad)   # (grad mode itself is always off inside Function.forward)
         runner.pack.refresh()
         xb = x.detach().to(torch.bfloat16).contiguous()
-        packing = add_mask if isinstance(add_mask, _Packing) else None
+        packing = add_mask if isinstance(add_mask, (_Packing, _StaticPacking)) else None
         probs = _probs_sink(x.dtype) if want_attn else None
         if packing is None:
             out, saved, hiddens = runner.forward(xb, add_mask, training, need_grad, probs=probs)
@@ -289,7 +325,7 @@ class _BertEncoderFn(torch.autograd.Function):
             raise RuntimeError("B200 encoder: backward called twice or activations were not saved")
         aliased = runner.pack.prepare_grads()
         d = dout.to(torch.bfloat16).contiguous().view(B * S, H)
-        if isinstance(ctx.add_mask, _Packing):
+        if isinstance(ctx.add_mask, (_Packing, _StaticPacking)):
             packing = ctx.add_mask
             dx = runner.backward(packing.pack(d), ctx.saved, packing.varlen, 1, packing.varlen.total)
             dx = packing.unpack(dx, B * S)
@@ -312,7 +348,11 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
     [B, heads, S, S] (hidden-state dtype, post-dropout in training) if output_attentions.  The hidden states and
     probabilities are outputs for inspection: they carry no gradient, so a loss that reads them back-propagates nothing
     through them.  A call that asks for probabilities runs the dense path even with skip_padding set, so they have the
-    reference's [B, heads, S, S] shape, padded rows and keys included."""
+    reference's [B, heads, S, S] shape, padded rows and keys included.
+    Inside graphs.static_rows(), a call without a causal tail on a skip_padding runner plans its packing on the device
+    (_plan_packing_static) instead: nothing is read on the host, so the call can be captured in a CUDA graph.  It runs the
+    packed path at a fixed capacity of B*S rows whatever the mask holds (every row valid, or none: then the outputs and
+    the input gradient are exact zeros), and its mask values other than 0 and <= -10000 are not checked."""
     _require_cuda(hidden_states, "hidden_states")
     if hidden_states.dim() != 3:
         raise ValueError("hidden_states must be [batch, seq, hidden], got %s" % (tuple(hidden_states.shape),))
@@ -333,6 +373,10 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
             mask = packing
         else:
             mask = E.CausalTail(mask, causal_len)
+    elif runner.skip_padding and mask is not None and not output_attentions and graphs.static_rows_active():
+        if runner.W is not E.BertLayerW:
+            raise RuntimeError("skip_padding under static_rows() covers BERT layer stacks only")
+        mask = _plan_packing_static(mask, B, S)
     elif runner.skip_padding and mask is not None and not output_attentions:
         packing = _plan_packing(mask, B, S)
         if packing is not None and packing.varlen.total == 0:

@@ -84,7 +84,10 @@ def set_skip_padding(module, enabled=True, two_stream=False, causal=False):
     With the flag on, an encoder call with a key-padding mask runs on the valid rows only: its outputs (and the input
     gradient) are exactly zero at padded positions instead of the values the dense path computes there.  For any loss that
     does not read padded positions it computes the same function and gradients as the dense path, up to rounding and the
-    dropout masks drawn.  It reads the token count on the host, so it cannot be captured in a CUDA graph.
+    dropout masks drawn.  An eager call reads the token count on the host.  Inside graphs.static_rows() a call without a
+    causal tail plans its packing on the device instead, at a fixed capacity of every row, so
+    `GraphedStep(..., static_rows=True)` captures such a model; calls with a causal tail (`causal`) and two-stream packing
+    still read the counts on the host and cannot be captured.
 
     A two-stream call falls back to the dense path when some sample has tokens in one stream and none in the other: there
     the dense outputs of those tokens depend on the other stream's padded rows.
