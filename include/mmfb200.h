@@ -385,8 +385,15 @@ int mmfb_cast_f32_bf16(const float* in, void* out, int64_t n, mmfb_stream stream
  * `group` (nullable) gives the hyper-parameter group of every 8-element block (parameters are padded to multiples of
  * 8 in the flat buffer); grad_scale multiplies the gradient first (1/loss_scale, clipping coefficient).  When
  * grad_scale_dev is set, the factor is grad_scale * *grad_scale_dev, the fp32 read from DEVICE memory when the kernel
- * runs (the clip coefficient mmfb_grad_norm writes), so a clipped step needs no device-to-host read. */
+ * runs (the clip coefficient mmfb_grad_norm writes), so a clipped step needs no device-to-host read.
+ * When hp_dev is set, group g's lr / weight_decay / step_size / bc2_sqrt and beta1 / beta2 / eps are read from the
+ * DEVICE table entry hp_dev[g] (written by mmfb_adamw_hparams) and the corresponding launch fields are ignored, so the
+ * launch can be captured in a CUDA graph and replayed at later steps and learning rates. */
 #define MMFB_ADAMW_MAX_GROUPS 8
+typedef struct {
+  float lr, weight_decay, step_size, bc2_sqrt;
+  float beta1, beta2, eps, pad_;
+} mmfb_adamw_hp;
 typedef struct {
   float* param;
   const float* grad;
@@ -403,8 +410,67 @@ typedef struct {
   float beta1, beta2, eps, grad_scale;
   int mode;
   const float* grad_scale_dev;   /* nullable: DEVICE fp32 factor applied on top of grad_scale */
+  const mmfb_adamw_hp* hp_dev;   /* nullable: DEVICE [n_groups] hyper-parameters replacing the launch fields */
 } mmfb_adamw_args;
 int mmfb_adamw(const mmfb_adamw_args* args, mmfb_stream stream);
+
+/* Device-side AdamW hyper-parameters, one CTA: for every slot s (a parameter, or a pack's parameter group) that is not
+ * MMFB_ADAMW_SLOT_FROZEN, step[s] += 1 and, with t = step[s] and g = groups[slots[s].group], in fp64 then rounded once
+ * to fp32 (the formulas of mmf_b200.optim.B200AdamW._group_hp):
+ *   mode 0: step_size = lr * sqrt(1 - b2^t) / (1 - b1^t) with MMFB_ADAMW_SLOT_CORRECT_BIAS, lr without; bc2_sqrt = 1
+ *   mode 1: step_size = lr / (1 - b1^t);  bc2_sqrt = sqrt(1 - b2^t)
+ * hp[s] = {lr, weight_decay, step_size, bc2_sqrt, b1, b2, eps}.  A frozen slot (pack parameters the optimizer does not
+ * own) keeps its step and gets lr = weight_decay = step_size = 0, bc2_sqrt = 1.  `groups` is the table the host stages
+ * before each step (the values a learning-rate scheduler writes); `slots`, `step` and `hp` stay put. */
+#define MMFB_ADAMW_SLOT_CORRECT_BIAS 1
+#define MMFB_ADAMW_SLOT_FROZEN 2
+typedef struct {
+  double lr, weight_decay, beta1, beta2, eps;
+} mmfb_adamw_group_hp;
+typedef struct {
+  int group;                 /* index into groups */
+  int flags;                 /* MMFB_ADAMW_SLOT_* */
+} mmfb_adamw_slot;
+typedef struct {
+  const mmfb_adamw_group_hp* groups;   /* DEVICE [groups used by slots] */
+  const mmfb_adamw_slot* slots;        /* DEVICE [n_slots] */
+  int64_t* step;                       /* DEVICE [n_slots] step counts */
+  mmfb_adamw_hp* hp;                   /* DEVICE [n_slots] */
+  int n_slots;
+  int mode;                            /* 0 transformers, 1 torch (as mmfb_adamw) */
+} mmfb_adamw_hparams_args;
+int mmfb_adamw_hparams(const mmfb_adamw_hparams_args* args, mmfb_stream stream);
+
+/* One AdamW launch over any number of separate fp32 tensors (parameters outside the flat packs), with the per-element
+ * arithmetic of mmfb_adamw (the same device function: bit-identical results element for element).  Segment s updates
+ * n elements at param / grad / exp_avg / exp_avg_sq (contiguous fp32, any 4-byte alignment) with hyper-parameters
+ * hp[slot].  head: 0-3 elements before the first element at which all four pointers are 16-byte aligned, or -1 when
+ * they never are together (every element is then accessed singly).  The segment owns the CTAs [first_block,
+ * first_block + ceil((n + lead) / MMFB_ADAMW_SEGMENT_BLOCK)), lead = (8 - head) % 8 for head > 0 and 0 otherwise;
+ * first_block is the running sum over the segments before it and n_blocks the total.  Gradients are multiplied by
+ * grad_scale (times *grad_scale_dev when set) first. */
+#define MMFB_ADAMW_SEGMENT_BLOCK 2048
+typedef struct {
+  float* param;
+  const float* grad;
+  float* exp_avg;
+  float* exp_avg_sq;
+  int64_t n;
+  int slot;
+  int first_block;
+  int head;
+  int pad_;
+} mmfb_adamw_segment;
+typedef struct {
+  const mmfb_adamw_segment* segments;  /* DEVICE [n_segments] */
+  int n_segments;
+  int n_blocks;
+  const mmfb_adamw_hp* hp;             /* DEVICE, indexed by the segments' slots */
+  float grad_scale;
+  int mode;
+  const float* grad_scale_dev;         /* nullable */
+} mmfb_adamw_segments_args;
+int mmfb_adamw_segments(const mmfb_adamw_segments_args* args, mmfb_stream stream);
 
 /* Global L2 norm of a list of gradient segments and torch's clip coefficient, on the device, in two launches:
  *   total_norm = sqrt(sum over every element x of every segment of x^2)

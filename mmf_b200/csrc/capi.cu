@@ -313,6 +313,16 @@ int mmfb_adamw(const mmfb_adamw_args* args, mmfb_stream stream) {
   MMFB_REQUIRE_DEVICE();
   return adamw(*args, reinterpret_cast<cudaStream_t>(stream));
 }
+int mmfb_adamw_hparams(const mmfb_adamw_hparams_args* args, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_adamw_hparams: null args");
+  MMFB_REQUIRE_DEVICE();
+  return adamw_hparams(*args, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_adamw_segments(const mmfb_adamw_segments_args* args, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_adamw_segments: null args");
+  MMFB_REQUIRE_DEVICE();
+  return adamw_segments(*args, reinterpret_cast<cudaStream_t>(stream));
+}
 int mmfb_grad_norm(const mmfb_grad_norm_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_grad_norm: null args");
   if (args->norm_type != 2.0f)

@@ -97,6 +97,8 @@ int scatter(const mmfb_scatter_args& a, cudaStream_t s);
 int cast_params(const float* in, void* out, int64_t n, cudaStream_t s);
 int relu_bwd(const void* dy, const void* y, void* dz, int64_t n, cudaStream_t s);
 int adamw(const mmfb_adamw_args& a, cudaStream_t s);
+int adamw_hparams(const mmfb_adamw_hparams_args& a, cudaStream_t s);
+int adamw_segments(const mmfb_adamw_segments_args& a, cudaStream_t s);
 int grad_norm(const mmfb_grad_norm_args& a, cudaStream_t s);
 int ce_rows(void* logits, int64_t ldl, const int64_t* labels, int64_t ignore_index, int M, int V, float grad_scale,
             float* loss_sum, float* row_loss, cudaStream_t s);

@@ -12,11 +12,35 @@ struct AdamWDev {
   float lr[MMFB_ADAMW_MAX_GROUPS], wd[MMFB_ADAMW_MAX_GROUPS], step[MMFB_ADAMW_MAX_GROUPS], bc2s[MMFB_ADAMW_MAX_GROUPS];
   float b1, b2, eps, gscale;
   const float* gscale_dev;   // read only by the SCALE_DEV instantiations (a device-side clipping coefficient)
+  const mmfb_adamw_hp* hp;   // read only by the HP_DEV instantiations (mmfb_adamw_hparams' table)
 };
 
+// One element of the AdamW step, shared by adamw_kernel and adamw_segments_kernel so that both give the same bits.
+// gr = g * gs is the scaled gradient; step = step_size, bc2s = bc2_sqrt.
+template <int MODE>
+__device__ __forceinline__ void adamw_elem(float& p, float& m, float& v, float g, float gs, float lr, float wd, float step,
+                                           float bc2s, float b1, float b2, float eps) {
+  const float gr = g * gs;
+  if (MODE == 0) {
+    // exp_avg.mul_(b1).add_(g, alpha=1-b1); exp_avg_sq.mul_(b2).addcmul_(g, g, value=1-b2)
+    m = __fmaf_rn(gr, 1.0f - b1, m * b1);
+    v = __fmaf_rn(gr * gr, 1.0f - b2, v * b2);
+    const float denom = __fsqrt_rn(v) + eps;
+    p = __fmaf_rn(-step, __fdiv_rn(m, denom), p);                          // p.addcdiv_(m, denom, value=-step_size)
+    if (wd > 0.0f) p = __fmaf_rn(p, -lr * wd, p);                          // p.add_(p, alpha=-lr*wd)
+  } else {
+    p = p * (1.0f - lr * wd);                                              // p.mul_(1 - lr*wd)
+    m = __fmaf_rn(gr - m, 1.0f - b1, m);                                   // m.lerp_(g, 1-b1)
+    v = __fmaf_rn(gr * gr, 1.0f - b2, v * b2);
+    const float denom = __fdiv_rn(__fsqrt_rn(v), bc2s) + eps;
+    p = __fmaf_rn(-step, __fdiv_rn(m, denom), p);
+  }
+}
+
 // SCALE_DEV: the gradient factor is gscale * *gscale_dev, read once per thread after the previous kernel has completed.
-// The instantiations without it are the kernels this file always had.
-template <int MODE, bool SCALE_DEV>
+// HP_DEV: the group's hyper-parameters come from the device table a.hp instead of the launch parameters.
+// The instantiations without either are the kernels this file always had.
+template <int MODE, bool SCALE_DEV, bool HP_DEV>
 __global__ void __launch_bounds__(256)
 adamw_kernel(const __grid_constant__ AdamWDev a) {
   griddep_launch();
@@ -25,8 +49,14 @@ adamw_kernel(const __grid_constant__ AdamWDev a) {
   const int64_t i = blk * 8;
   if (i >= a.n) return;
   const int gi = a.grp != nullptr ? a.grp[blk] : 0;
-  const float lr = a.lr[gi], wd = a.wd[gi], step = a.step[gi], bc2s = a.bc2s[gi];
-  const float gsdev = SCALE_DEV ? a.gscale * *a.gscale_dev : 0.0f;
+  float lr, wd, step, bc2s, b1, b2, eps;
+  if (HP_DEV) {
+    const mmfb_adamw_hp h = a.hp[gi];
+    lr = h.lr; wd = h.weight_decay; step = h.step_size; bc2s = h.bc2_sqrt; b1 = h.beta1; b2 = h.beta2; eps = h.eps;
+  } else {
+    lr = a.lr[gi]; wd = a.wd[gi]; step = a.step[gi]; bc2s = a.bc2s[gi]; b1 = a.b1; b2 = a.b2; eps = a.eps;
+  }
+  const float gs = SCALE_DEV ? a.gscale * *a.gscale_dev : a.gscale;
   float p[8], g[8], m[8], v[8];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -40,23 +70,7 @@ adamw_kernel(const __grid_constant__ AdamWDev a) {
     v[4 * h] = tv.x; v[4 * h + 1] = tv.y; v[4 * h + 2] = tv.z; v[4 * h + 3] = tv.w;
   }
 #pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const float gr = g[e] * (SCALE_DEV ? gsdev : a.gscale);
-    if (MODE == 0) {
-      // exp_avg.mul_(b1).add_(g, alpha=1-b1); exp_avg_sq.mul_(b2).addcmul_(g, g, value=1-b2)
-      m[e] = __fmaf_rn(gr, 1.0f - a.b1, m[e] * a.b1);
-      v[e] = __fmaf_rn(gr * gr, 1.0f - a.b2, v[e] * a.b2);
-      const float denom = __fsqrt_rn(v[e]) + a.eps;
-      p[e] = __fmaf_rn(-step, __fdiv_rn(m[e], denom), p[e]);              // p.addcdiv_(m, denom, value=-step_size)
-      if (wd > 0.0f) p[e] = __fmaf_rn(p[e], -lr * wd, p[e]);               // p.add_(p, alpha=-lr*wd)
-    } else {
-      p[e] = p[e] * (1.0f - lr * wd);                                      // p.mul_(1 - lr*wd)
-      m[e] = __fmaf_rn(gr - m[e], 1.0f - a.b1, m[e]);                      // m.lerp_(g, 1-b1)
-      v[e] = __fmaf_rn(gr * gr, 1.0f - a.b2, v[e] * a.b2);
-      const float denom = __fdiv_rn(__fsqrt_rn(v[e]), bc2s) + a.eps;
-      p[e] = __fmaf_rn(-step, __fdiv_rn(m[e], denom), p[e]);
-    }
-  }
+  for (int e = 0; e < 8; ++e) adamw_elem<MODE>(p[e], m[e], v[e], g[e], gs, lr, wd, step, bc2s, b1, b2, eps);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     *reinterpret_cast<float4*>(a.p + i + 4 * h) = make_float4(p[4 * h], p[4 * h + 1], p[4 * h + 2], p[4 * h + 3]);
@@ -80,6 +94,7 @@ int adamw(const mmfb_adamw_args& a, cudaStream_t s) {
   if ((reinterpret_cast<uintptr_t>(a.param) | reinterpret_cast<uintptr_t>(a.grad) | reinterpret_cast<uintptr_t>(a.exp_avg) |
        reinterpret_cast<uintptr_t>(a.exp_avg_sq) | reinterpret_cast<uintptr_t>(a.param_bf16)) & 15)
     return set_error(MMFB_ERR_ARG, "adamw: buffers must be 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(a.hp_dev) & 15) return set_error(MMFB_ERR_ARG, "adamw: hp_dev must be 16-byte aligned");
   AdamWDev d;
   d.p = a.param; d.g = a.grad; d.m = a.exp_avg; d.v = a.exp_avg_sq; d.pb = reinterpret_cast<bf16*>(a.param_bf16);
   d.grp = a.group; d.n = a.n;
@@ -88,17 +103,173 @@ int adamw(const mmfb_adamw_args& a, cudaStream_t s) {
     d.lr[i] = a.lr[j]; d.wd[i] = a.weight_decay[j]; d.step[i] = a.step_size[j]; d.bc2s[i] = a.bc2_sqrt[j];
   }
   d.b1 = a.beta1; d.b2 = a.beta2; d.eps = a.eps; d.gscale = a.grad_scale; d.gscale_dev = a.grad_scale_dev;
+  d.hp = a.hp_dev;
   const int64_t blocks8 = a.n / 8;
   const unsigned grid = static_cast<unsigned>((blocks8 + 255) / 256);
-  if (a.grad_scale_dev != nullptr) {
-    if (a.mode == 0) MMFB_LAUNCH((adamw_kernel<0, true>), grid, 256, 0, s, d);
-    else MMFB_LAUNCH((adamw_kernel<1, true>), grid, 256, 0, s, d);
-  } else {
-    if (a.mode == 0) MMFB_LAUNCH((adamw_kernel<0, false>), grid, 256, 0, s, d);
-    else MMFB_LAUNCH((adamw_kernel<1, false>), grid, 256, 0, s, d);
+  const int variant = a.mode * 4 + (a.grad_scale_dev != nullptr ? 2 : 0) + (a.hp_dev != nullptr ? 1 : 0);
+  switch (variant) {
+    case 0: MMFB_LAUNCH((adamw_kernel<0, false, false>), grid, 256, 0, s, d); break;
+    case 1: MMFB_LAUNCH((adamw_kernel<0, false, true>), grid, 256, 0, s, d); break;
+    case 2: MMFB_LAUNCH((adamw_kernel<0, true, false>), grid, 256, 0, s, d); break;
+    case 3: MMFB_LAUNCH((adamw_kernel<0, true, true>), grid, 256, 0, s, d); break;
+    case 4: MMFB_LAUNCH((adamw_kernel<1, false, false>), grid, 256, 0, s, d); break;
+    case 5: MMFB_LAUNCH((adamw_kernel<1, false, true>), grid, 256, 0, s, d); break;
+    case 6: MMFB_LAUNCH((adamw_kernel<1, true, false>), grid, 256, 0, s, d); break;
+    default: MMFB_LAUNCH((adamw_kernel<1, true, true>), grid, 256, 0, s, d); break;
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return MMFB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Device-side hyper-parameters (include/mmfb200.h: mmfb_adamw_hparams): one CTA, one slot per thread and pass.  fp64
+// operation by operation as the host's B200AdamW._group_hp evaluates it (Python float ** int is C pow), rounded once.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int HP_THREADS = 256;
+
+__global__ void __launch_bounds__(HP_THREADS)
+adamw_hparams_kernel(const mmfb_adamw_group_hp* __restrict__ groups, const mmfb_adamw_slot* __restrict__ slots,
+                     int64_t* __restrict__ steps, mmfb_adamw_hp* __restrict__ out, int n_slots, int mode) {
+  griddep_launch();
+  griddep_wait();
+  for (int s = threadIdx.x; s < n_slots; s += HP_THREADS) {
+    const mmfb_adamw_slot sl = slots[s];
+    const mmfb_adamw_group_hp g = groups[sl.group];
+    mmfb_adamw_hp h;
+    h.beta1 = __double2float_rn(g.beta1); h.beta2 = __double2float_rn(g.beta2); h.eps = __double2float_rn(g.eps);
+    h.pad_ = 0.0f;
+    if (sl.flags & MMFB_ADAMW_SLOT_FROZEN) {
+      h.lr = 0.0f; h.weight_decay = 0.0f; h.step_size = 0.0f; h.bc2_sqrt = 1.0f;
+    } else {
+      const int64_t t = steps[s] + 1;
+      steps[s] = t;
+      const double td = static_cast<double>(t);
+      const double bc1 = __dsub_rn(1.0, pow(g.beta1, td));               // 1 - b1 ** t
+      const double bc2s = __dsqrt_rn(__dsub_rn(1.0, pow(g.beta2, td)));  // math.sqrt(1 - b2 ** t)
+      double ss, b2c;
+      if (mode == 0) {
+        ss = (sl.flags & MMFB_ADAMW_SLOT_CORRECT_BIAS) ? __ddiv_rn(__dmul_rn(g.lr, bc2s), bc1) : g.lr;
+        b2c = 1.0;
+      } else {
+        ss = __ddiv_rn(g.lr, bc1);
+        b2c = bc2s;
+      }
+      h.lr = __double2float_rn(g.lr); h.weight_decay = __double2float_rn(g.weight_decay);
+      h.step_size = __double2float_rn(ss); h.bc2_sqrt = __double2float_rn(b2c);
+    }
+    out[s] = h;
+  }
+}
+
+int adamw_hparams(const mmfb_adamw_hparams_args& a, cudaStream_t s) {
+  if (!a.groups || !a.slots || !a.step || !a.hp) return set_error(MMFB_ERR_ARG, "adamw_hparams: null pointer");
+  if (a.n_slots < 1) return set_error(MMFB_ERR_ARG, "adamw_hparams: need at least one slot (got %d)", a.n_slots);
+  if (a.mode != 0 && a.mode != 1) return set_error(MMFB_ERR_ARG, "adamw_hparams: mode must be 0 (transformers) or 1 (torch)");
+  if ((reinterpret_cast<uintptr_t>(a.groups) | reinterpret_cast<uintptr_t>(a.step)) & 7 ||
+      reinterpret_cast<uintptr_t>(a.slots) & 7 || reinterpret_cast<uintptr_t>(a.hp) & 15)
+    return set_error(MMFB_ERR_ARG, "adamw_hparams: groups / slots / step must be 8-byte aligned, hp 16-byte aligned");
+  MMFB_LAUNCH(adamw_hparams_kernel, 1, HP_THREADS, 0, s, a.groups, a.slots, a.step, a.hp, a.n_slots, a.mode);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw_hparams launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return MMFB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// AdamW over a table of separate fp32 tensors (include/mmfb200.h: mmfb_adamw_segments).  CTA b finds the segment whose
+// first_block <= b is largest; thread t of its chunk c owns the 8-element group k = c * 256 + t, elements
+// [8k - lead, 8k - lead + 8) of the segment clipped to [0, n).  A group inside the segment whose four streams are
+// 16-byte aligned (head >= 0) moves as float4 pairs; the head group, the tail group and segments that are not co-aligned
+// are read and written element by element.  Elements go through adamw_elem, as in adamw_kernel.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int AS_THREADS = MMFB_ADAMW_SEGMENT_BLOCK / 8;
+static_assert(AS_THREADS == 256, "one 8-element group per thread");
+
+template <int MODE, bool SCALE_DEV>
+__global__ void __launch_bounds__(AS_THREADS)
+adamw_segments_kernel(const mmfb_adamw_segment* __restrict__ segs, int n_segs, const mmfb_adamw_hp* __restrict__ hp,
+                      float gscale, const float* __restrict__ gscale_dev) {
+  __shared__ int s_seg;
+  griddep_launch();
+  griddep_wait();
+  const int b = blockIdx.x;
+  if (threadIdx.x == 0) {
+    int lo = 0, hi = n_segs - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (segs[mid].first_block <= b) lo = mid; else hi = mid - 1;
+    }
+    s_seg = lo;
+  }
+  __syncthreads();
+  const mmfb_adamw_segment sg = segs[s_seg];
+  const int lead = sg.head > 0 ? 8 - sg.head : 0;
+  const int64_t start = (static_cast<int64_t>(b - sg.first_block) * AS_THREADS + threadIdx.x) * 8 - lead;
+  if (start >= sg.n) return;
+  const mmfb_adamw_hp h = hp[sg.slot];
+  const float gs = SCALE_DEV ? gscale * *gscale_dev : gscale;
+  const bool vec = sg.head >= 0 && start >= 0 && start + 8 <= sg.n;
+  float p[8], g[8], m[8], v[8];
+  if (vec) {
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const float4 tp = *reinterpret_cast<const float4*>(sg.param + start + 4 * q);
+      const float4 tg = *reinterpret_cast<const float4*>(sg.grad + start + 4 * q);
+      const float4 tm = *reinterpret_cast<const float4*>(sg.exp_avg + start + 4 * q);
+      const float4 tv = *reinterpret_cast<const float4*>(sg.exp_avg_sq + start + 4 * q);
+      p[4 * q] = tp.x; p[4 * q + 1] = tp.y; p[4 * q + 2] = tp.z; p[4 * q + 3] = tp.w;
+      g[4 * q] = tg.x; g[4 * q + 1] = tg.y; g[4 * q + 2] = tg.z; g[4 * q + 3] = tg.w;
+      m[4 * q] = tm.x; m[4 * q + 1] = tm.y; m[4 * q + 2] = tm.z; m[4 * q + 3] = tm.w;
+      v[4 * q] = tv.x; v[4 * q + 1] = tv.y; v[4 * q + 2] = tv.z; v[4 * q + 3] = tv.w;
+    }
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int64_t j = start + e;
+      const bool in = j >= 0 && j < sg.n;
+      p[e] = in ? sg.param[j] : 0.0f; g[e] = in ? sg.grad[j] : 0.0f;
+      m[e] = in ? sg.exp_avg[j] : 0.0f; v[e] = in ? sg.exp_avg_sq[j] : 0.0f;
+    }
+  }
+#pragma unroll
+  for (int e = 0; e < 8; ++e)
+    adamw_elem<MODE>(p[e], m[e], v[e], g[e], gs, h.lr, h.weight_decay, h.step_size, h.bc2_sqrt, h.beta1, h.beta2, h.eps);
+  if (vec) {
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      *reinterpret_cast<float4*>(sg.param + start + 4 * q) = make_float4(p[4 * q], p[4 * q + 1], p[4 * q + 2], p[4 * q + 3]);
+      *reinterpret_cast<float4*>(sg.exp_avg + start + 4 * q) = make_float4(m[4 * q], m[4 * q + 1], m[4 * q + 2], m[4 * q + 3]);
+      *reinterpret_cast<float4*>(sg.exp_avg_sq + start + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+    }
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const int64_t j = start + e;
+      if (j >= 0 && j < sg.n) { sg.param[j] = p[e]; sg.exp_avg[j] = m[e]; sg.exp_avg_sq[j] = v[e]; }
+    }
+  }
+}
+
+int adamw_segments(const mmfb_adamw_segments_args& a, cudaStream_t s) {
+  if (!a.segments || !a.hp) return set_error(MMFB_ERR_ARG, "adamw_segments: null pointer");
+  if (a.n_segments < 1 || a.n_blocks < 1)
+    return set_error(MMFB_ERR_ARG, "adamw_segments: need at least one segment and one block (got %d, %d)", a.n_segments,
+                     a.n_blocks);
+  if (a.mode != 0 && a.mode != 1) return set_error(MMFB_ERR_ARG, "adamw_segments: mode must be 0 (transformers) or 1 (torch)");
+  if (reinterpret_cast<uintptr_t>(a.segments) & 7 || reinterpret_cast<uintptr_t>(a.hp) & 15 ||
+      reinterpret_cast<uintptr_t>(a.grad_scale_dev) & 3)
+    return set_error(MMFB_ERR_ARG, "adamw_segments: segments must be 8-byte aligned, hp 16-byte, grad_scale_dev 4-byte");
+  const int variant = a.mode * 2 + (a.grad_scale_dev != nullptr ? 1 : 0);
+  switch (variant) {
+    case 0: MMFB_LAUNCH((adamw_segments_kernel<0, false>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, a.hp, a.grad_scale, a.grad_scale_dev); break;
+    case 1: MMFB_LAUNCH((adamw_segments_kernel<0, true>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, a.hp, a.grad_scale, a.grad_scale_dev); break;
+    case 2: MMFB_LAUNCH((adamw_segments_kernel<1, false>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, a.hp, a.grad_scale, a.grad_scale_dev); break;
+    default: MMFB_LAUNCH((adamw_segments_kernel<1, true>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, a.hp, a.grad_scale, a.grad_scale_dev); break;
+  }
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw_segments launch: %s", cudaGetErrorString(e));
   count_launch();
   return MMFB_OK;
 }

@@ -699,11 +699,12 @@ def gelu_bwd(dh, u):
 
 
 def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, grad_scale=1.0, group_of_block=None,
-          param_bf16=None, grad_scale_dev=None):
+          param_bf16=None, grad_scale_dev=None, hp_dev=None):
     """One fused AdamW step over flat fp32 buffers (staged, include/mmfb200.h: mmfb_adamw).
     groups: list (<= 8) of dicts {lr, weight_decay, step_size, bc2_sqrt}; group_of_block: uint8 [n/8] or None;
     grad_scale_dev: None or a one-element fp32 CUDA tensor (grad_norm's clip coefficient) multiplied into grad_scale when
-    the kernel runs."""
+    the kernel runs.  hp_dev: None or an fp32 CUDA tensor [n_groups, 8] written by adamw_hparams; the kernel then reads
+    every group's hyper-parameters and beta1 / beta2 / eps from it, and `groups` may be None."""
     for t, n in ((param, "param"), (grad, "grad"), (exp_avg, "exp_avg"), (exp_avg_sq, "exp_avg_sq")):
         _req(t, torch.float32, n)
         if not t.is_contiguous() or t.numel() != param.numel():
@@ -718,10 +719,16 @@ def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, 
         if group_of_block.numel() != param.numel() // 8:
             raise ValueError("adamw: group_of_block needs one entry per 8 elements")
         a.group = group_of_block.data_ptr()
-    a.n, a.n_groups = param.numel(), len(groups)
-    if not 1 <= len(groups) <= 8:
+    if hp_dev is not None:
+        _req_hp(hp_dev, "adamw")
+        n_groups = hp_dev.shape[0]
+        a.hp_dev = hp_dev.data_ptr()
+    else:
+        n_groups = len(groups)
+    a.n, a.n_groups = param.numel(), n_groups
+    if not 1 <= n_groups <= 8:
         raise ValueError("adamw: between 1 and 8 hyper-parameter groups per launch")
-    for i, g in enumerate(groups):
+    for i, g in enumerate(groups or ()):
         a.lr[i], a.weight_decay[i], a.step_size[i], a.bc2_sqrt[i] = g["lr"], g["weight_decay"], g["step_size"], g["bc2_sqrt"]
     a.beta1, a.beta2, a.eps, a.grad_scale, a.mode = float(beta1), float(beta2), float(eps), float(grad_scale), int(mode)
     if grad_scale_dev is not None:
@@ -729,6 +736,104 @@ def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, 
             raise ValueError("adamw: grad_scale_dev must be a one-element fp32 CUDA tensor")
         a.grad_scale_dev = grad_scale_dev.data_ptr()
     check(LIB.mmfb_adamw(ctypes.byref(a), _stream_ptr()))
+
+
+def _req_hp(hp, what):
+    if not hp.is_cuda or hp.dtype != torch.float32 or hp.dim() != 2 or hp.shape[1] != lib.ADAMW_HP_FLOATS or \
+            not hp.is_contiguous():
+        raise ValueError("%s: the hyper-parameter table must be a contiguous fp32 CUDA tensor [slots, %d]"
+                         % (what, lib.ADAMW_HP_FLOATS))
+
+
+def adamw_hparams(groups, slots, step, hp, mode):
+    """Advance the step counts and write the AdamW hyper-parameter table on the device (include/mmfb200.h:
+    mmfb_adamw_hparams).  groups: fp64 CUDA [n_groups, 5] (lr, weight_decay, beta1, beta2, eps); slots: the device
+    table of adamw_slot_table; step: int64 CUDA [n_slots], advanced by one for every slot that is not frozen; hp: fp32
+    CUDA [n_slots, 8], overwritten.  Nothing is read on the host."""
+    if groups.dtype != torch.float64 or groups.dim() != 2 or groups.shape[1] != lib.ADAMW_GROUP_HP_DOUBLES or \
+            not groups.is_contiguous():
+        raise ValueError("adamw_hparams: groups must be a contiguous fp64 tensor [n_groups, %d]" % lib.ADAMW_GROUP_HP_DOUBLES)
+    if step.dtype != torch.int64 or step.dim() != 1 or not step.is_contiguous():
+        raise ValueError("adamw_hparams: step must be a contiguous int64 tensor")
+    _req_hp(hp, "adamw_hparams")
+    if hp.shape[0] != step.numel() or slots.numel() != step.numel() * 8:
+        raise ValueError("adamw_hparams: slots, step and hp must have one entry per slot")
+    for t in (groups, slots, step):
+        if not t.is_cuda:
+            raise RuntimeError("adamw_hparams: tensors must be CUDA tensors: the B200 path has no CPU fallback")
+    a = lib.AdamWHparamsArgs()
+    a.groups, a.slots, a.step, a.hp = groups.data_ptr(), slots.data_ptr(), step.data_ptr(), hp.data_ptr()
+    a.n_slots, a.mode = step.numel(), int(mode)
+    check(LIB.mmfb_adamw_hparams(ctypes.byref(a), _stream_ptr()))
+
+
+def adamw_slot_table(slots, device):
+    """DEVICE table of mmfb_adamw_slot for adamw_hparams: `slots` is a list of (group index, flags)."""
+    arr = (lib.AdamWSlot * len(slots))(*[lib.AdamWSlot(*s) for s in slots])
+    host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).pin_memory()
+    return host.to(device, non_blocking=True)
+
+
+def adamw_segment_rows(segments):
+    """Host rows of the mmfb_adamw_segments table: `segments` is a list of (param, grad, exp_avg, exp_avg_sq, slot)
+    with contiguous fp32 tensors of equal sizes.  Returns (rows, n_blocks), a row being (param_ptr, grad_ptr,
+    exp_avg_ptr, exp_avg_sq_ptr, n, slot, first_block, head); empty tensors get no row."""
+    rows, first = [], 0
+    for p, g, m, v, slot in segments:
+        for t, name in ((p, "param"), (g, "grad"), (m, "exp_avg"), (v, "exp_avg_sq")):
+            if t.dtype != torch.float32 or not t.is_contiguous():
+                raise ValueError("adamw_segments: %s must be a contiguous fp32 tensor, got %s%s"
+                                 % (name, t.dtype, "" if t.is_contiguous() else " (not contiguous)"))
+            if t.numel() != p.numel():
+                raise ValueError("adamw_segments: %s has %d elements, param %d" % (name, t.numel(), p.numel()))
+        if p.numel() == 0:
+            continue
+        ptrs = (p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr())
+        mis = {(x >> 2) & 3 for x in ptrs}
+        head = (4 - mis.pop()) & 3 if len(mis) == 1 else -1
+        lead = 8 - head if head > 0 else 0
+        rows.append(ptrs + (p.numel(), int(slot), first, head))
+        first += (p.numel() + lead + lib.MMFB_ADAMW_SEGMENT_BLOCK - 1) // lib.MMFB_ADAMW_SEGMENT_BLOCK
+    if first >= 2 ** 31:
+        raise ValueError("adamw_segments: too many elements (%d blocks)" % first)
+    return rows, first
+
+
+class AdamWSegmentTable:
+    """The DEVICE table of mmfb_adamw_segments over a fixed list of tensors (see adamw_segment_table)."""
+
+    def __init__(self, segments, rows, n_blocks):
+        self.segments, self.rows, self.n_blocks = segments, rows, n_blocks
+
+
+def adamw_segment_table(segments):
+    """Segment table for adamw_segments (rows as adamw_segment_rows).  One host-to-device copy from pinned memory without
+    a stream synchronisation; it stays valid while the tensors keep their storage."""
+    for s in segments:
+        for t in s[:4]:
+            if not t.is_cuda:
+                raise RuntimeError("adamw_segments: tensors must be CUDA tensors: the B200 path has no CPU fallback")
+    rows, n_blocks = adamw_segment_rows(segments)
+    if not rows:
+        raise ValueError("adamw_segments: no non-empty tensor")
+    arr = (lib.AdamWSegment * len(rows))(*[lib.AdamWSegment(*r, 0) for r in rows])
+    host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).pin_memory()
+    return AdamWSegmentTable(host.to(segments[0][0].device, non_blocking=True), rows, n_blocks)
+
+
+def adamw_segments(table, hp, *, mode, grad_scale=1.0, grad_scale_dev=None):
+    """One AdamW launch over every tensor of `table` (include/mmfb200.h: mmfb_adamw_segments), each with the
+    hyper-parameters of its slot in hp (fp32 CUDA [slots, 8], written by adamw_hparams).  Element for element the
+    arithmetic of adamw; grad_scale_dev as there."""
+    _req_hp(hp, "adamw_segments")
+    a = lib.AdamWSegmentsArgs()
+    a.segments, a.n_segments, a.n_blocks = table.segments.data_ptr(), len(table.rows), table.n_blocks
+    a.hp, a.grad_scale, a.mode = hp.data_ptr(), float(grad_scale), int(mode)
+    if grad_scale_dev is not None:
+        if not grad_scale_dev.is_cuda or grad_scale_dev.dtype != torch.float32 or grad_scale_dev.numel() != 1:
+            raise ValueError("adamw_segments: grad_scale_dev must be a one-element fp32 CUDA tensor")
+        a.grad_scale_dev = grad_scale_dev.data_ptr()
+    check(LIB.mmfb_adamw_segments(ctypes.byref(a), _stream_ptr()))
 
 
 class GradNormTable:

@@ -21,6 +21,13 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
   * skip-padding: a single-stream encoder with skip_padding set plans its packing on the host in an eager step.  Inside
     `static_rows()` it plans it on the device at the capacity B*S (mmf_b200.modules._plan_packing_static) and bounds
     every GEMM, LayerNorm and column sum of its layers by the device token count, so that step can be captured too.
+  * the optimizer: `GraphedStep(..., optimizer=opt, max_grad_norm=c)` with a `B200AdamW(..., capturable=True)` captures
+    the whole step - gradients zeroed in place, forward, backward, `opt.clip_grad_norm(c)`, `opt.step()`.  The step
+    counts and bias corrections advance on the device; the groups' lr / weight_decay / betas / eps are staged from
+    `param_groups` before every replay, so a learning-rate scheduler stepped between replays takes effect.  What the
+    capture freezes: which parameters have gradients, the gradient and state buffers (they keep their storage from the
+    warm-up on), `grad_scale` 1, correct_bias and the arithmetic mode.  The warm-up steps are undone, so capturing does
+    not change the parameters or the optimizer state;
 The reference has no counterpart (its trainer launches eagerly, mmf/trainers/core/training_loop.py:185-213); this is the
 answer to SURVEY.md 8a's "at T = R = 36 everything is launch-bound"."""
 import contextlib
@@ -75,7 +82,7 @@ def _copy_into(dst, src):
 
 
 class GraphedStep:
-    def __init__(self, model, loss_fn, example_batch, warmup=3, static_rows=False):
+    def __init__(self, model, loss_fn, example_batch, warmup=3, static_rows=False, optimizer=None, max_grad_norm=None):
         """loss_fn(batch) -> scalar loss; `example_batch`: (nested dict / list of) CUDA tensors with the shapes of every later
         batch.  The model must be in the mode (train / eval) it will be replayed in.
 
@@ -88,7 +95,18 @@ class GraphedStep:
         masked-LM loss is captured too.  Single-stream skip_padding encoders (patch.set_skip_padding(model)) plan their
         packing on the device there and are captured as well, at a fixed capacity of every row of the batch.  Those with
         `pack_tail` (set_skip_padding(..., causal=True)) and two-stream encoders with `pack_streams` are still refused.
-        Opt-in because the replayed step differs from an eager one: no MLM logits."""
+        Opt-in because the replayed step differs from an eager one: no MLM logits.
+
+        optimizer: a B200AdamW(..., capturable=True) over the model's parameters; the graph then holds the whole training
+        step: gradients zeroed, forward, backward, optimizer.clip_grad_norm(max_grad_norm) when max_grad_norm is set, and
+        optimizer.step().  Each call stages the groups' current hyper-parameters, then replays; afterwards `.grad` holds
+        the step's unclipped gradients, as after an eager step."""
+        if max_grad_norm is not None and optimizer is None:
+            raise ValueError("GraphedStep: max_grad_norm clips inside the captured optimizer step; pass optimizer= as well, "
+                             "or clip and step eagerly after each replay")
+        if optimizer is not None and not getattr(optimizer, "capturable", False):
+            raise ValueError("GraphedStep: the optimizer's step reads host values at every step and cannot be captured; "
+                             "construct it as mmf_b200.optim.B200AdamW(..., capturable=True)")
         runners = [m.__dict__.get("_runner") for m in model.modules()]
         if not static_rows and any(getattr(r, "skip_padding", False) for r in runners):
             raise RuntimeError("GraphedStep: the model has skip_padding encoders, which read the token count on the host and "
@@ -108,6 +126,7 @@ class GraphedStep:
                 reason = getattr(m, "graph_refusal", "does work on the host in every forward")
                 raise RuntimeError("GraphedStep: %s %s, so its step cannot be captured" % (type(m).__name__, reason))
         self.model, self.loss_fn = model, loss_fn
+        self.optimizer, self.max_grad_norm = optimizer, max_grad_norm
         with _static_rows_context() if static_rows else contextlib.nullcontext():
             self._capture(model, loss_fn, example_batch, warmup)
 
@@ -115,30 +134,91 @@ class GraphedStep:
         self.static = _map(lambda t: t.detach().clone(), example_batch)
         dev = next(t for t in _flatten(self.static) if t.is_cuda).device
         self.epoch = F.dropout_epoch(dev, create=True)
+        opt = self.optimizer
+        saved = _save_optimizer(opt) if opt is not None else None
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             for _ in range(max(1, warmup)):              # lazy engine state, kernel attributes, library work buffers
-                model.zero_grad(set_to_none=True)
+                self._zero_grads()
                 self.epoch.add_(1)
                 loss_fn(self.static).backward()
+                if opt is not None:                      # builds the optimizer's device tables on these gradients
+                    self._optimizer_step()
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
-        model.zero_grad(set_to_none=True)
+        if opt is None:
+            model.zero_grad(set_to_none=True)
+        else:
+            _restore_optimizer(opt, saved)
+            torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
         # captured on the warm-up stream: autograd binds every parameter's gradient accumulator to the stream that was current
         # when the accumulator was created, i.e. this one, as long as no autograd graph from an earlier eager step on another
         # stream is still alive (it would keep the old accumulators - and their stream - in use)
         with torch.cuda.graph(self.graph, stream=side):
+            if opt is not None:
+                self._zero_grads()
             self.epoch.add_(1)
             self.loss = loss_fn(self.static)
             self.loss.backward()
+            if opt is not None:
+                self._optimizer_step()
+        self._plan = opt._cap if opt is not None else None
+
+    def _zero_grads(self):
+        """without an optimizer: .grad unset (the flat buffers are zeroed inside the graph); with one: zeroed in place, so
+        every gradient keeps the storage the optimizer's tables point at"""
+        if self.optimizer is None:
+            self.model.zero_grad(set_to_none=True)
+            return
+        grads = [p.grad for p in self.model.parameters() if p.grad is not None]
+        if grads:
+            torch._foreach_zero_(grads)
+
+    def _optimizer_step(self):
+        if self.max_grad_norm is not None:
+            self.optimizer.clip_grad_norm(self.max_grad_norm)
+        self.optimizer.step()
 
     def __call__(self, batch=None):
         if batch is not None:
             _copy_into(self.static, batch)
+        if self.optimizer is not None:
+            self.optimizer.stage_hparams(self._plan)
         self.graph.replay()
         return self.loss
+
+
+def _save_optimizer(opt):
+    """copies of the parameters and optimizer state that the warm-up steps change"""
+    params = [p for g in opt.param_groups for p in g["params"]]
+    return {"params": [(p, p.detach().clone()) for p in params],
+            "state": {p: {k: (v.clone() if torch.is_tensor(v) else v) for k, v in opt.state[p].items()}
+                      for p in params if p in opt.state},
+            "flat": {k: (e["m"].clone(), e["v"].clone()) for k, e in opt._flat.items()}}
+
+
+def _restore_optimizer(opt, saved):
+    """undo the warm-up steps: parameters, moments (flat buffers included) and step counts as they were before"""
+    for p, c in saved["params"]:
+        p.detach().copy_(c)
+    for k, e in opt._flat.items():
+        if k in saved["flat"]:
+            e["m"].copy_(saved["flat"][k][0])
+            e["v"].copy_(saved["flat"][k][1])
+        else:
+            e["m"].zero_()
+            e["v"].zero_()
+    for p, st in opt.state.items():
+        old = saved["state"].get(p, {})
+        for k in ("exp_avg", "exp_avg_sq"):
+            if k in st:
+                st[k].copy_(old[k]) if k in old else st[k].zero_()
+        if torch.is_tensor(st.get("step")):
+            st["step"].copy_(old["step"]) if torch.is_tensor(old.get("step")) else st["step"].fill_(int(old.get("step", 0)))
+        elif "step" in st:
+            st["step"] = old.get("step", 0)
 
 
 def _flatten(x):

@@ -97,6 +97,40 @@ class AdamWArgs(ctypes.Structure):
         ("beta1", ctypes.c_float), ("beta2", ctypes.c_float), ("eps", ctypes.c_float), ("grad_scale", ctypes.c_float),
         ("mode", ctypes.c_int),
         ("grad_scale_dev", ctypes.c_void_p),
+        ("hp_dev", ctypes.c_void_p),
+    ]
+
+
+MMFB_ADAMW_SLOT_CORRECT_BIAS, MMFB_ADAMW_SLOT_FROZEN = 1, 2
+MMFB_ADAMW_SEGMENT_BLOCK = 2048
+ADAMW_HP_FLOATS = 8          # floats per mmfb_adamw_hp entry
+ADAMW_GROUP_HP_DOUBLES = 5   # doubles per mmfb_adamw_group_hp entry
+
+
+class AdamWSlot(ctypes.Structure):
+    _fields_ = [("group", ctypes.c_int), ("flags", ctypes.c_int)]
+
+
+class AdamWHparamsArgs(ctypes.Structure):
+    _fields_ = [
+        ("groups", ctypes.c_void_p), ("slots", ctypes.c_void_p), ("step", ctypes.c_void_p), ("hp", ctypes.c_void_p),
+        ("n_slots", ctypes.c_int), ("mode", ctypes.c_int),
+    ]
+
+
+class AdamWSegment(ctypes.Structure):
+    _fields_ = [
+        ("param", ctypes.c_void_p), ("grad", ctypes.c_void_p), ("exp_avg", ctypes.c_void_p), ("exp_avg_sq", ctypes.c_void_p),
+        ("n", ctypes.c_int64), ("slot", ctypes.c_int), ("first_block", ctypes.c_int), ("head", ctypes.c_int),
+        ("pad_", ctypes.c_int),
+    ]
+
+
+class AdamWSegmentsArgs(ctypes.Structure):
+    _fields_ = [
+        ("segments", ctypes.c_void_p), ("n_segments", ctypes.c_int), ("n_blocks", ctypes.c_int),
+        ("hp", ctypes.c_void_p), ("grad_scale", ctypes.c_float), ("mode", ctypes.c_int),
+        ("grad_scale_dev", ctypes.c_void_p),
     ]
 
 

@@ -15,6 +15,14 @@ computed on the device (`mmfb_grad_norm`, one read of the gradients, fixed summa
 every gradient by the coefficient it reads from device memory - inside the AdamW kernel for the packs, as a tensor factor
 on the torch-op path - so nothing waits for the host and the clipped step can be captured in a CUDA graph.
 
+Capturable steps: `B200AdamW(..., capturable=True)` steps every parameter with library launches and reads nothing on the
+host, so clip + step can be captured in a CUDA graph (mmf_b200.graphs.GraphedStep(..., optimizer=opt)).  The step counts
+live on the device (`state[p]["step"]` is a 0-d int64 CUDA tensor, shared by the parameters of one pack and group) and
+one launch (`mmfb_adamw_hparams`) advances them and computes each slot's step size and bias corrections from the group
+values, which stay Python floats in `param_groups` (schedulers keep working) and are staged by one pinned host-to-device
+copy per step.  Packs get one `mmfb_adamw` each reading that table; every other parameter goes into one
+`mmfb_adamw_segments` launch.  `state_dict()` reports the step counts as ints (one device read).
+
 torch.optim.Adam: with arithmetic="torch" and weight_decay=0 the step is torch.optim.Adam's (amsgrad and maximize off):
 AdamW's decoupled decay multiplies the parameter by exactly 1, and the remaining operations - m.lerp_(g, 1-b1),
 v.mul_(b2).addcmul_(g, g, 1-b2), p.addcdiv_(m, sqrt(v)/sqrt(1-b2^t) + eps, -lr/(1-b1^t)) - are Adam's.  Pass Adam's
@@ -27,6 +35,47 @@ import torch
 
 from . import engine as E
 from . import functional as F
+from . import lib
+
+
+def _capturing():
+    return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
+
+
+def _read_steps(steps):
+    """ints of a list of step counts (ints or 0-d tensors), with one device read per device"""
+    out = list(steps)
+    by_dev = {}
+    for i, t in enumerate(out):
+        if torch.is_tensor(t):
+            by_dev.setdefault(t.device, []).append(i)
+    for idx in by_dev.values():
+        vals = torch.stack([out[i].reshape(()).to(torch.int64) for i in idx]).tolist()
+        for i, v in zip(idx, vals):
+            out[i] = int(v)
+    return [int(v) for v in out]
+
+
+def _h2d(t, device, out=None):
+    """a host tensor on `device` (into `out` if given): one non-blocking copy from pinned memory (the caching host
+    allocator keeps the pinned block until the copy has run)"""
+    if device.type == "cuda":
+        t = t.pin_memory()
+    if out is None:
+        return t.to(device, non_blocking=True)
+    return out.copy_(t, non_blocking=True)
+
+
+class _CapturablePlan:
+    """What a capturable step launches: the slots (a pack's parameter group, or a loose parameter) with their device
+    step counts and hyper-parameter table, the pack launches, and the segment table of the loose parameters."""
+
+    def __init__(self, layout_key, device, mode):
+        self.layout_key, self.device, self.mode = layout_key, device, mode
+        self.packs = []          # (pack, flat state entry, first slot, slots, betas, eps)
+        self.loose = []          # (param, slot)
+        self.slots = []          # (group index, flags)
+        self.table_key, self.table = None, None
 
 
 def _reference_arithmetic():
@@ -40,7 +89,7 @@ def _reference_arithmetic():
 
 class B200AdamW(torch.optim.Optimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0, correct_bias=True,
-                 arithmetic="auto"):
+                 arithmetic="auto", capturable=False):
         if lr < 0.0 or eps < 0.0 or not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
             raise ValueError("Invalid AdamW hyper-parameters: lr=%s betas=%s eps=%s" % (lr, betas, eps))
         if arithmetic == "auto":
@@ -53,6 +102,8 @@ class B200AdamW(torch.optim.Optimizer):
         self._flat = {}        # id(pack) -> {"pack": weakref, "m", "v", "groups": uint8 [total/8], "gids": {...}}
         self._clip_table = None   # (key of the gradient buffers, F.GradNormTable) of clip_grad_norm
         self._clip_coef = None    # 0-d fp32 CUDA tensor: the coefficient the next step() applies, then drops
+        self.capturable = bool(capturable)   # fixed at construction, as the arithmetic mode and correct_bias are
+        self._cap = None          # _CapturablePlan of the last capturable step
 
     # ---------------------------------------------------------------------------------------------------------
     def _group_hp(self, group, step):
@@ -178,6 +229,9 @@ class B200AdamW(torch.optim.Optimizer):
                 loss = closure()
         coef, self._clip_coef = self._clip_coef, None
         clip = {} if coef is None else {"grad_scale_dev": coef}
+        if self.capturable:
+            self._step_capturable(grad_scale, clip)
+            return loss
         group_of = {id(p): gi for gi, g in enumerate(self.param_groups) for p in g["params"]}
         done = set()
         mode = 0 if self.arithmetic == "transformers" else 1
@@ -222,6 +276,159 @@ class B200AdamW(torch.optim.Optimizer):
         return loss
 
     def load_state_dict(self, state_dict):
+        """Takes the state of a B200AdamW in either mode or of torch.optim.AdamW / Adam (tensor step counts)."""
         super().load_state_dict(state_dict)
         self._clip_coef = None
         self._flat = {}                                # re-adopt the loaded per-parameter tensors into flat buffers
+        if self.capturable:
+            self._cap = None
+            for st in self.state.values():
+                if torch.is_tensor(st.get("step")):
+                    st["step"] = int(st["step"].item())
+
+    def state_dict(self):
+        """torch's layout; in capturable mode the device step counts are read back (once) and reported as ints."""
+        sd = super().state_dict()
+        if not self.capturable:
+            return sd
+        state = {k: dict(v) for k, v in sd["state"].items()}
+        keys = [k for k, v in state.items() if "step" in v]
+        for k, v in zip(keys, _read_steps([state[k]["step"] for k in keys])):
+            state[k]["step"] = v
+        sd["state"] = state
+        return sd
+
+    # ---------------------------------------------------------------------------------------------------------
+    # capturable mode
+    def _capturable_plan(self):
+        """The plan of the next capturable step: rebuilt when the stepped parameters or the packs change (this reads the
+        step counts on the host), its segment table when a loose gradient or state tensor moves; neither may happen
+        during stream capture."""
+        group_of = {id(p): gi for gi, g in enumerate(self.param_groups) for p in g["params"]}
+        stepped, seen = [], set()
+        for group in self.param_groups:
+            for p in group["params"]:
+                if p.grad is not None and id(p) not in seen:
+                    seen.add(id(p))
+                    stepped.append(p)
+        if not stepped:
+            return None
+        order = {id(p): i for i, p in enumerate(stepped)}
+        packs = []
+        for pack in list(E.ParamPack._live or ()):
+            owned = [p for p in pack.params if id(p) in group_of]
+            mine = [p for p in owned if id(p) in seen]
+            if not mine:
+                continue
+            ok = (pack.dtype == torch.float32 and pack.intact() and len(mine) == len(owned) and
+                  all(p.grad.dtype == torch.float32 and p.grad.data_ptr() == pack._gptrs[pack._index[id(p)]]
+                      for p in mine) and
+                  len({(self.param_groups[group_of[id(p)]]["betas"], self.param_groups[group_of[id(p)]]["eps"])
+                       for p in mine}) == 1)
+            packs.append((min(order[id(p)] for p in mine), pack, mine, ok))
+        packs.sort(key=lambda t: t[0])
+        layout_key = (tuple(id(p) for p in stepped), tuple((id(pk), pk.master.data_ptr(), ok) for _, pk, _, ok in packs))
+        plan = self._cap
+        if plan is None or plan.layout_key != layout_key:
+            if _capturing():
+                raise RuntimeError("B200AdamW(capturable=True): the parameters with gradients changed during CUDA-graph "
+                                   "capture; run one eager step with the same gradients before capturing")
+            plan = self._cap = self._build_layout(layout_key, stepped, packs, group_of)
+        table_key = tuple((p.data_ptr(), p.grad.data_ptr(), self.state[p]["exp_avg"].data_ptr(),
+                           self.state[p]["exp_avg_sq"].data_ptr()) for p, _ in plan.loose)
+        if plan.loose and plan.table_key != table_key:
+            if _capturing():
+                raise RuntimeError("B200AdamW(capturable=True): a gradient or optimizer-state buffer moved during "
+                                   "CUDA-graph capture; run one eager step with the same gradients before capturing")
+            for p, _ in plan.loose:
+                if not p.grad.is_contiguous() or p.grad.dtype != torch.float32:
+                    raise ValueError("B200AdamW(capturable=True): gradients must be contiguous fp32 tensors; a parameter "
+                                     "of shape %s has a %s%s gradient" % (tuple(p.shape), p.grad.dtype,
+                                                                          "" if p.grad.is_contiguous() else
+                                                                          " non-contiguous"))
+            plan.table = F.adamw_segment_table([(p.data, p.grad, self.state[p]["exp_avg"], self.state[p]["exp_avg_sq"], s)
+                                                for p, s in plan.loose])
+            plan.table_key = table_key
+        return plan
+
+    def _build_layout(self, layout_key, stepped, packs, group_of):
+        device = stepped[0].device
+        plan = _CapturablePlan(layout_key, device, 0 if self.arithmetic == "transformers" else 1)
+        steps = dict(zip((id(p) for p in stepped), _read_steps([self.state[p].get("step", 0) if p in self.state else 0
+                                                                  for p in stepped])))
+        cb = lambda gi: lib.MMFB_ADAMW_SLOT_CORRECT_BIAS if self.param_groups[gi].get("correct_bias", True) else 0
+        counts, slot_of = [], {}
+        in_pack = set()
+        for _, pack, mine, ok in packs:
+            by_group = {}
+            for p in mine:
+                by_group.setdefault(group_of[id(p)], set()).add(steps[id(p)])
+            if not ok or any(len(v) != 1 for v in by_group.values()):
+                continue                               # mixed step counts or betas: its parameters go to the segments
+            ent = self._flat_state(pack, group_of)
+            s0, g0 = len(plan.slots), min(by_group)
+            for gi in range(len(self.param_groups)):
+                if gi in by_group:
+                    plan.slots.append((gi, cb(gi)))
+                    counts.append(next(iter(by_group[gi])))
+                else:                                  # a group without parameters here: its entry is never read
+                    plan.slots.append((g0, lib.MMFB_ADAMW_SLOT_FROZEN))
+                    counts.append(0)
+            if ent["frozen"]:                          # pack parameters the optimizer was not given
+                plan.slots.append((g0, lib.MMFB_ADAMW_SLOT_FROZEN))
+                counts.append(0)
+            g = self.param_groups[g0]
+            plan.packs.append((pack, ent, s0, len(plan.slots) - s0, g["betas"], g["eps"]))
+            for p in mine:
+                slot_of[id(p)] = s0 + group_of[id(p)]
+                in_pack.add(id(p))
+        for p in stepped:
+            if id(p) in in_pack:
+                continue
+            if p.dtype != torch.float32 or not p.is_contiguous():
+                raise ValueError("B200AdamW(capturable=True): parameters outside the engine's packs must be contiguous "
+                                 "fp32 tensors; got a %s%s parameter of shape %s"
+                                 % ("" if p.is_contiguous() else "non-contiguous ", p.dtype, tuple(p.shape)))
+            st = self.state[p]
+            for k in ("exp_avg", "exp_avg_sq"):
+                t = st.get(k)
+                if t is None or t.dtype != torch.float32 or not t.is_contiguous() or t.device != p.device:
+                    st[k] = torch.zeros_like(p.data, dtype=torch.float32) if t is None else \
+                        t.to(device=p.device, dtype=torch.float32).contiguous()
+            slot_of[id(p)] = len(plan.slots)
+            plan.loose.append((p, len(plan.slots)))
+            plan.slots.append((group_of[id(p)], cb(group_of[id(p)])))
+            counts.append(steps[id(p)])
+        plan.step = _h2d(torch.tensor(counts, dtype=torch.int64), device)
+        plan.slot_table = F.adamw_slot_table(plan.slots, device)
+        plan.hp = torch.zeros(len(plan.slots), lib.ADAMW_HP_FLOATS, dtype=torch.float32, device=device)
+        plan.groups = torch.zeros(len(self.param_groups), lib.ADAMW_GROUP_HP_DOUBLES, dtype=torch.float64, device=device)
+        for p in stepped:
+            self.state[p]["step"] = plan.step[slot_of[id(p)]]
+        return plan
+
+    def _group_values(self):
+        """the staged table: (lr, weight_decay, beta1, beta2, eps) of every group, fp64"""
+        return torch.tensor([[float(g["lr"]), float(g["weight_decay"]), float(g["betas"][0]), float(g["betas"][1]),
+                              float(g["eps"])] for g in self.param_groups], dtype=torch.float64)
+
+    def stage_hparams(self, plan=None):
+        """Copy the groups' current lr / weight_decay / betas / eps to the device table the next (eager or replayed)
+        capturable step reads: one non-blocking copy from pinned memory on the current stream.  An eager step() does
+        this itself; GraphedStep does it before every replay."""
+        plan = plan if plan is not None else self._cap
+        if plan is not None:
+            _h2d(self._group_values(), plan.device, out=plan.groups)
+
+    def _step_capturable(self, grad_scale, clip):
+        plan = self._capturable_plan()
+        if plan is None:
+            return
+        if not _capturing():
+            self.stage_hparams(plan)
+        F.adamw_hparams(plan.groups, plan.slot_table, plan.step, plan.hp, plan.mode)
+        for pack, ent, s0, n, betas, eps in plan.packs:
+            F.adamw(pack.master, pack.grad, ent["m"], ent["v"], None, beta1=betas[0], beta2=betas[1], eps=eps,
+                    mode=plan.mode, grad_scale=grad_scale, group_of_block=ent["groups"], hp_dev=plan.hp[s0:s0 + n], **clip)
+        if plan.loose:
+            F.adamw_segments(plan.table, plan.hp, mode=plan.mode, grad_scale=grad_scale, **clip)
