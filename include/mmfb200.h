@@ -361,6 +361,24 @@ int mmfb_ce_rows_bounded(void* logits, int64_t ldl, const int64_t* labels, int64
 int mmfb_colsum_bounded(const void* X, int64_t ldx, float* out, int M, int N, const int32_t* m_dev, float* workspace,
                         int64_t workspace_bytes, mmfb_stream stream);
 
+/* Static-rows region losses of masked region classification (MRC) and feature regression (MRFR): the rows of a fixed
+ * capacity M of which the first count = clamp(*m_dev, 0, M) (DEVICE int32) are the masked regions, selected on the
+ * device (mmfb_select_rows); row r < count takes its target from row tgt_idx[r] (DEVICE int32 [M]) of tgt (fp32, row
+ * stride ldt).  Both write the gradient of their bf16 input IN PLACE, scaled by *scale_dev (DEVICE fp32, read when the
+ * kernel runs), and the fp32 loss of row r to row_loss[r] (the caller sums the rows in a fixed order and multiplies by
+ * the same scale).  Rows in [count, ceil(count / 128) * 128) get a zero gradient and a zero row loss, as the bounded
+ * GEMMs that read them next require; rows at and past that are not read or written.  A count of 0 writes nothing.
+ * mmfb_kl_rows_bounded: logits [M, V] (ldl >= V rounded up to 8): with p = softmax(z) and q the target row,
+ *   row loss sum_j xlogy(q_j, q_j) - q_j log p_j, gradient (p_j sum_k q_k - q_j) * scale; columns [V, round8(V)) - the
+ *   GEMM's zero padding - get a zero gradient.  F.kl_div(F.log_softmax(z), q, reduction="batchmean") with scale =
+ *   1 / count (mmf/models/transformers/heads/mrc.py).
+ * mmfb_mse_rows_bounded: pred [M, D]: row loss sum_j (z_j - t_j)^2, gradient 2 (z_j - t_j) * scale; F.mse_loss(z, t)
+ *   with scale = 1 / (count * D) (heads/mrfr.py). */
+int mmfb_kl_rows_bounded(void* logits, int64_t ldl, int M, int V, const float* tgt, int64_t ldt, const int32_t* tgt_idx,
+                         const int32_t* m_dev, const float* scale_dev, float* row_loss, mmfb_stream stream);
+int mmfb_mse_rows_bounded(void* pred, int64_t ldp, int M, int D, const float* tgt, int64_t ldt, const int32_t* tgt_idx,
+                          const int32_t* m_dev, const float* scale_dev, float* row_loss, mmfb_stream stream);
+
 /* out = a + b; contiguous bf16 buffers of n elements.  The residual-gradient join of a pre-LN layer (ViT: the residual
  * branches off BEFORE the LayerNorm, mmf/modules/vit.py:96-108), which a post-LN layer gets for free from the GEMM epilogue. */
 int mmfb_add_bf16(const void* a, const void* b, void* out, int64_t n, mmfb_stream stream);

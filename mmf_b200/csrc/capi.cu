@@ -286,6 +286,20 @@ int mmfb_colsum_bounded(const void* X, int64_t ldx, float* out, int M, int N, co
   MMFB_REQUIRE_DEVICE();
   return colsum_bounded(X, ldx, out, M, N, m_dev, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream));
 }
+int mmfb_kl_rows_bounded(void* logits, int64_t ldl, int M, int V, const float* tgt, int64_t ldt, const int32_t* tgt_idx,
+                         const int32_t* m_dev, const float* scale_dev, float* row_loss, mmfb_stream stream) {
+  if (!logits || !tgt || !tgt_idx || !m_dev || !scale_dev || !row_loss)
+    return set_error(MMFB_ERR_ARG, "mmfb_kl_rows_bounded: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return kl_rows_bounded(logits, ldl, M, V, tgt, ldt, tgt_idx, m_dev, scale_dev, row_loss, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_mse_rows_bounded(void* pred, int64_t ldp, int M, int D, const float* tgt, int64_t ldt, const int32_t* tgt_idx,
+                          const int32_t* m_dev, const float* scale_dev, float* row_loss, mmfb_stream stream) {
+  if (!pred || !tgt || !tgt_idx || !m_dev || !scale_dev || !row_loss)
+    return set_error(MMFB_ERR_ARG, "mmfb_mse_rows_bounded: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return mse_rows_bounded(pred, ldp, M, D, tgt, ldt, tgt_idx, m_dev, scale_dev, row_loss, reinterpret_cast<cudaStream_t>(stream));
+}
 int mmfb_select_rows(const int64_t* labels, int64_t ignore_index, int M, int32_t* state, int64_t* labels_out,
                      mmfb_stream stream) {
   if (!labels || !state || !labels_out) return set_error(MMFB_ERR_ARG, "mmfb_select_rows: null pointer");

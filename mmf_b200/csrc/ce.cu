@@ -131,4 +131,125 @@ int ce_rows_bounded(void* logits, int64_t ldl, const int64_t* labels, int64_t ig
   return MMFB_OK;
 }
 
+// The region heads' losses on a fixed capacity of rows (masked region classification / feature regression of UNITER,
+// mmf/models/transformers/heads/mrc.py and mrfr.py), bounded by a device count like ce_rows_bounded: row r < count is
+// the r-th masked region, its target is row tgt_idx[r] of `tgt`; rows in [count, rounded bound) get a zero gradient and
+// a zero row loss (the bounded GEMMs after this read them); rows at and past the rounded bound are not touched.
+//
+// kl:  q = target row (soft labels), p = softmax(z):  loss_r = sum_j xlogy(q_j, q_j) - q_j log p_j
+//      dz_j = (p_j sum_k q_k - q_j) * scale                  (F.kl_div(F.log_softmax(z), q) per row)
+//      columns [V, ldz-rounded-to-8) are the GEMM's zero padding: their gradient is written as 0
+// mse: loss_r = sum_j (z_j - t_j)^2,  dz_j = 2 (z_j - t_j) * scale    (F.mse_loss per row)
+// The gradient is written in place over z (bf16); row_loss[r] gets the fp32 row loss, summed by the caller.
+__device__ __forceinline__ int bounded_rows(const int32_t* m_dev, int M, int* count) {
+  const int b = min(max(*m_dev, 0), M);
+  *count = b;
+  return min(M, (b + BOUNDED_ROW_TILE - 1) / BOUNDED_ROW_TILE * BOUNDED_ROW_TILE);
+}
+
+__global__ void __launch_bounds__(256)
+kl_rows_bounded_kernel(bf16* __restrict__ z, int64_t ldz, int M, int V, int Vp, const float* __restrict__ tgt, int64_t ldt,
+                       const int32_t* __restrict__ tgt_idx, const int32_t* __restrict__ m_dev,
+                       const float* __restrict__ scale_dev, float* __restrict__ row_loss) {
+  griddep_launch();
+  griddep_wait();
+  __shared__ float red[8];
+  const int row = blockIdx.x;
+  int count;
+  if (row >= bounded_rows(m_dev, M, &count)) return;
+  bf16* zr = z + static_cast<int64_t>(row) * ldz;
+  if (row >= count) {
+    for (int i = threadIdx.x; i < Vp; i += 256) zr[i] = __float2bfloat16(0.0f);
+    if (threadIdx.x == 0) row_loss[row] = 0.0f;
+    return;
+  }
+  const float* q = tgt + static_cast<int64_t>(tgt_idx[row]) * ldt;
+  float mx = -INFINITY, qs = 0.0f, qlq = 0.0f, qz = 0.0f;
+  for (int i = threadIdx.x; i < V; i += 256) {
+    const float zi = __bfloat162float(zr[i]), qi = q[i];
+    mx = fmaxf(mx, zi);
+    qs += qi;
+    qlq += qi == 0.0f ? 0.0f : qi * logf(qi);
+    qz += qi * zi;
+  }
+  mx = block_reduce(mx, red, true);
+  qs = block_reduce(qs, red, false);
+  qlq = block_reduce(qlq, red, false);
+  qz = block_reduce(qz, red, false);
+  const float mx2 = mx * 1.4426950408889634f;
+  float se = 0.0f;
+  for (int i = threadIdx.x; i < V; i += 256) se += exp2f(fmaf(__bfloat162float(zr[i]), 1.4426950408889634f, -mx2));
+  se = block_reduce(se, red, false);
+  const float scale = *scale_dev, f = qs / se;
+  for (int i = threadIdx.x; i < Vp; i += 256) {
+    float g = 0.0f;
+    if (i < V) g = (exp2f(fmaf(__bfloat162float(zr[i]), 1.4426950408889634f, -mx2)) * f - q[i]) * scale;
+    zr[i] = __float2bfloat16(g);
+  }
+  if (threadIdx.x == 0) row_loss[row] = qlq - qz + (mx + logf(se)) * qs;
+}
+
+__global__ void __launch_bounds__(256)
+mse_rows_bounded_kernel(bf16* __restrict__ z, int64_t ldz, int M, int D, const float* __restrict__ tgt, int64_t ldt,
+                        const int32_t* __restrict__ tgt_idx, const int32_t* __restrict__ m_dev,
+                        const float* __restrict__ scale_dev, float* __restrict__ row_loss) {
+  griddep_launch();
+  griddep_wait();
+  __shared__ float red[8];
+  const int row = blockIdx.x;
+  int count;
+  if (row >= bounded_rows(m_dev, M, &count)) return;
+  bf16* zr = z + static_cast<int64_t>(row) * ldz;
+  if (row >= count) {
+    for (int i = threadIdx.x; i < D; i += 256) zr[i] = __float2bfloat16(0.0f);
+    if (threadIdx.x == 0) row_loss[row] = 0.0f;
+    return;
+  }
+  const float* t = tgt + static_cast<int64_t>(tgt_idx[row]) * ldt;
+  const float scale2 = 2.0f * *scale_dev;
+  float s = 0.0f;
+  for (int i = threadIdx.x; i < D; i += 256) {
+    const float d = __bfloat162float(zr[i]) - t[i];
+    s += d * d;
+    zr[i] = __float2bfloat16(d * scale2);
+  }
+  s = block_reduce(s, red, false);
+  if (threadIdx.x == 0) row_loss[row] = s;
+}
+
+static int region_rows_check(const char* what, const void* z, int64_t ldz, int M, int cols, int padded_cols,
+                             const void* tgt, int64_t ldt, const void* tgt_idx, const void* m_dev, const void* scale_dev) {
+  if (M <= 0 || cols <= 0 || ldz < padded_cols || ldt < cols)
+    return set_error(MMFB_ERR_ARG, "%s: bad shape %dx%d (ldz %lld, ldt %lld)", what, M, cols, (long long)ldz, (long long)ldt);
+  if ((reinterpret_cast<uintptr_t>(z) & 1) || (reinterpret_cast<uintptr_t>(tgt) & 3) || (reinterpret_cast<uintptr_t>(tgt_idx) & 3) ||
+      ((reinterpret_cast<uintptr_t>(m_dev) | reinterpret_cast<uintptr_t>(scale_dev)) & 3))
+    return set_error(MMFB_ERR_ARG, "%s: misaligned buffer", what);
+  return MMFB_OK;
+}
+
+int kl_rows_bounded(void* logits, int64_t ldl, int M, int V, const float* tgt, int64_t ldt, const int32_t* tgt_idx,
+                    const int32_t* m_dev, const float* scale_dev, float* row_loss, cudaStream_t s) {
+  const int Vp = (V + 7) / 8 * 8;
+  int rc = region_rows_check("kl_rows_bounded", logits, ldl, M, V, Vp, tgt, ldt, tgt_idx, m_dev, scale_dev);
+  if (rc != MMFB_OK) return rc;
+  MMFB_LAUNCH(kl_rows_bounded_kernel, M, 256, 0, s, reinterpret_cast<bf16*>(logits), ldl, M, V, Vp, tgt, ldt, tgt_idx,
+              m_dev, scale_dev, row_loss);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "kl_rows_bounded launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return MMFB_OK;
+}
+
+int mse_rows_bounded(void* pred, int64_t ldp, int M, int D, const float* tgt, int64_t ldt, const int32_t* tgt_idx,
+                     const int32_t* m_dev, const float* scale_dev, float* row_loss, cudaStream_t s) {
+  int rc = region_rows_check("mse_rows_bounded", pred, ldp, M, D, D, tgt, ldt, tgt_idx, m_dev, scale_dev);
+  if (rc != MMFB_OK) return rc;
+  MMFB_LAUNCH(mse_rows_bounded_kernel, M, 256, 0, s, reinterpret_cast<bf16*>(pred), ldp, M, D, tgt, ldt, tgt_idx, m_dev,
+              scale_dev, row_loss);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "mse_rows_bounded launch: %s", cudaGetErrorString(e));
+  count_launch();
+  return MMFB_OK;
+}
+
 }  // namespace mmfb

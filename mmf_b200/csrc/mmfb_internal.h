@@ -106,6 +106,10 @@ int ce_rows_bounded(void* logits, int64_t ldl, const int64_t* labels, int64_t ig
                     const int32_t* m_dev, const float* scale_dev, float* loss_sum, float* row_loss, cudaStream_t s);
 int colsum_bounded(const void* X, int64_t ldx, float* out, int M, int N, const int32_t* m_dev, float* ws, int64_t ws_bytes,
                    cudaStream_t s);
+int kl_rows_bounded(void* logits, int64_t ldl, int M, int V, const float* tgt, int64_t ldt, const int32_t* tgt_idx,
+                    const int32_t* m_dev, const float* scale_dev, float* row_loss, cudaStream_t s);
+int mse_rows_bounded(void* pred, int64_t ldp, int M, int D, const float* tgt, int64_t ldt, const int32_t* tgt_idx,
+                     const int32_t* m_dev, const float* scale_dev, float* row_loss, cudaStream_t s);
 int select_rows(const int64_t* labels, int64_t ignore_index, int M, int32_t* state, int64_t* labels_out, cudaStream_t s);
 int gather_rows(const void* x, int64_t ldx, const int32_t* idx, void* out, int64_t ldo, int M, int H, cudaStream_t s);
 int add_bf16(const void* a, const void* b, void* out, int64_t n, cudaStream_t s);

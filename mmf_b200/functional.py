@@ -630,6 +630,44 @@ def colsum_bounded(x, out, m_bound):
     return out
 
 
+def _region_rows(what, z, cols, target, tgt_idx, m_bound, scale, row_loss):
+    _req(z, torch.bfloat16, "z"); _req(target, torch.float32, "target"); _req(tgt_idx, torch.int32, "tgt_idx")
+    _req(scale, torch.float32, "scale"); _req(row_loss, torch.float32, "row_loss")
+    if z.dim() != 2 or target.dim() != 2:
+        raise ValueError("%s: z and target must be 2-D" % what)
+    M = z.shape[0]
+    if not 0 < cols <= z.shape[1] or target.shape[1] != cols:
+        raise ValueError("%s: %d columns of z [%d, %d] against a target of %d columns"
+                         % (what, cols, M, z.shape[1], target.shape[1]))
+    _idx_len(tgt_idx, M, "tgt_idx")
+    if row_loss.numel() != M or not row_loss.is_contiguous():
+        raise ValueError("%s: row_loss must be a contiguous vector of %d" % (what, M))
+    if scale.numel() != 1:
+        raise ValueError("%s: scale must be a CUDA fp32 tensor with one element" % what)
+    return (z.data_ptr(), z.stride(0), M, cols, target.data_ptr(), target.stride(0), tgt_idx.data_ptr(),
+            _bound(m_bound, "m_bound"), scale.data_ptr(), row_loss.data_ptr(), _stream_ptr())
+
+
+def kl_rows_bounded(logits, V, target, tgt_idx, m_bound, scale, row_loss):
+    """In place: logits [M, >= round8(V)] bf16 -> d(logits) of the KL divergence of softmax(logits[:, :V]) from the target
+    rows target[tgt_idx[r]] (fp32 [*, V]), times `scale` (fp32 [1]), for the rows below m_bound (int32 [1]); row_loss[r]
+    gets the row's KL.  Rows between the bound and its 128-row tile edge are zeroed, later rows untouched
+    (mmfb_kl_rows_bounded); the padding columns [V, round8(V)) get a zero gradient."""
+    if logits.dim() == 2 and logits.shape[1] < -(-V // 8) * 8:
+        raise ValueError("kl_rows_bounded: logits need %d columns (V rounded up to 8), got %d" % (-(-V // 8) * 8,
+                                                                                                logits.shape[1]))
+    check(LIB.mmfb_kl_rows_bounded(*_region_rows("kl_rows_bounded", logits, V, target, tgt_idx, m_bound, scale, row_loss)))
+    return logits
+
+
+def mse_rows_bounded(pred, target, tgt_idx, m_bound, scale, row_loss):
+    """In place: pred [M, D] bf16 -> 2 (pred - target[tgt_idx[r]]) * scale for the rows below m_bound; row_loss[r] gets the
+    row's summed squared error (mmfb_mse_rows_bounded, the same row rules as kl_rows_bounded)."""
+    check(LIB.mmfb_mse_rows_bounded(*_region_rows("mse_rows_bounded", pred, pred.shape[-1], target, tgt_idx, m_bound,
+                                                   scale, row_loss)))
+    return pred
+
+
 class SelectedRows:
     """Device state of mmfb_select_rows over M labels: `count` (int32 [1]), `scale` (fp32 [1], 1 / max(count, 1)),
     `pos` / `inv` (int32 [M]) and the gathered `labels` (int64 [M], ignore_index past count).  Nothing is read on the host."""

@@ -28,10 +28,14 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
     capture freezes: which parameters have gradients, the gradient and state buffers (they keep their storage from the
     warm-up on), `grad_scale` 1, correct_bias and the arithmetic mode.  The warm-up steps are undone, so capturing does
     not change the parameters or the optimizer state;
+  * host draws: a model that draws its task on the host in every forward (UNITER) is captured by GraphedTaskSteps, one
+    graph per task, with the draws made on the host before each replay;
 The reference has no counterpart (its trainer launches eagerly, mmf/trainers/core/training_loop.py:185-213); this is the
 answer to SURVEY.md 8a's "at T = R = 36 everything is launch-bound"."""
 import contextlib
+import random
 
+import numpy as np
 import torch
 
 from . import functional as F
@@ -101,25 +105,8 @@ class GraphedStep:
         step: gradients zeroed, forward, backward, optimizer.clip_grad_norm(max_grad_norm) when max_grad_norm is set, and
         optimizer.step().  Each call stages the groups' current hyper-parameters, then replays; afterwards `.grad` holds
         the step's unclipped gradients, as after an eager step."""
-        if max_grad_norm is not None and optimizer is None:
-            raise ValueError("GraphedStep: max_grad_norm clips inside the captured optimizer step; pass optimizer= as well, "
-                             "or clip and step eagerly after each replay")
-        if optimizer is not None and not getattr(optimizer, "capturable", False):
-            raise ValueError("GraphedStep: the optimizer's step reads host values at every step and cannot be captured; "
-                             "construct it as mmf_b200.optim.B200AdamW(..., capturable=True)")
-        runners = [m.__dict__.get("_runner") for m in model.modules()]
-        if not static_rows and any(getattr(r, "skip_padding", False) for r in runners):
-            raise RuntimeError("GraphedStep: the model has skip_padding encoders, which read the token count on the host and "
-                               "cannot be captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)")
-        if static_rows and any(getattr(r, "skip_padding", False) and getattr(r, "pack_tail", False) for r in runners):
-            raise RuntimeError("GraphedStep: the model has skip_padding encoders with pack_tail set, which read the token "
-                               "count on the host for calls with a causal tail even under static_rows, so they cannot be "
-                               "captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)")
-        if any(getattr(r, "pack_streams", False) for r in runners):
-            raise RuntimeError("GraphedStep: the model has two-stream encoders with pack_streams set, which read the token "
-                               "counts on the host%s and cannot be captured; turn them off with "
-                               "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)"
-                               % (" even under static_rows" if static_rows else ""))
+        _check_optimizer("GraphedStep", optimizer, max_grad_norm)
+        _check_runners("GraphedStep", model, static_rows)
         for m in model.modules():
             if getattr(m, "graph_capturable", True) is False and not (static_rows and getattr(m, "static_rows_capturable",
                                                                                            False)):
@@ -188,6 +175,194 @@ class GraphedStep:
             self.optimizer.stage_hparams(self._plan)
         self.graph.replay()
         return self.loss
+
+
+def _check_optimizer(who, optimizer, max_grad_norm):
+    if max_grad_norm is not None and optimizer is None:
+        raise ValueError("%s: max_grad_norm clips inside the captured optimizer step; pass optimizer= as well, "
+                         "or clip and step eagerly after each replay" % who)
+    if optimizer is not None and not getattr(optimizer, "capturable", False):
+        raise ValueError("%s: the optimizer's step reads host values at every step and cannot be captured; "
+                         "construct it as mmf_b200.optim.B200AdamW(..., capturable=True)" % who)
+
+
+def _check_runners(who, model, static_rows):
+    """the encoders' skip-padding modes that read token counts on the host, and so cannot be captured"""
+    runners = [m.__dict__.get("_runner") for m in model.modules()]
+    if not static_rows and any(getattr(r, "skip_padding", False) for r in runners):
+        raise RuntimeError("%s: the model has skip_padding encoders, which read the token count on the host and "
+                           "cannot be captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)" % who)
+    if static_rows and any(getattr(r, "skip_padding", False) and getattr(r, "pack_tail", False) for r in runners):
+        raise RuntimeError("%s: the model has skip_padding encoders with pack_tail set, which read the token "
+                           "count on the host for calls with a causal tail even under static_rows, so they cannot be "
+                           "captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)" % who)
+    if any(getattr(r, "pack_streams", False) for r in runners):
+        raise RuntimeError("%s: the model has two-stream encoders with pack_streams set, which read the token "
+                           "counts on the host%s and cannot be captured; turn them off with "
+                           "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)"
+                           % (who, " even under static_rows" if static_rows else ""))
+
+
+class GraphedTaskSteps:
+    """One CUDA graph per task for a model whose forward draws its task on the host (UNITER: the task with torch.randint,
+    the region masks of mrc / mrfr with numpy and random).  The model defines `draw(sample_list, task=None)`, which makes
+    those draws, stores them in the sample list under `model.draws_key` and returns the task's name, and a forward that
+    finds them draws nothing.  So the draws stay on the host, where the reference makes them, and everything after them
+    is captured:
+
+        steps = GraphedTaskSteps(model, loss_fn, example_batch, optimizer=opt, max_grad_norm=1.0)
+        loss = steps(batch)      # draws on the host, copies batch and draws into the static inputs, replays that task
+
+    Every graph is captured inside static_rows() (the masked-LM and region heads select their rows on the device) with
+    its task's draws fixed; all graphs share one memory pool, so a returned loss is valid until the next call.
+    Constructing the object leaves the torch CPU, numpy and `random` generators as they were, although warm-up and
+    capture draw too; each call then draws exactly what an eager forward draws.
+
+    Gradients: each task's graph zeroes and fills the gradients of the parameters that task reaches, in buffers all
+    graphs share; after a call `.grad` is set for those and None for the others, as after an eager step from
+    zero_grad(set_to_none=True).  With a capturable B200AdamW every graph carries its own optimizer plan, so a replayed
+    step of task t updates exactly the parameters an eager step of t updates: heads t does not reach keep their values,
+    moments and step counts.  The step counts live in one device table that each graph reads before and writes after its
+    optimizer step; step the optimizer only through this object while it is in use.  The warm-up steps are undone.
+    Skip-padding and pack_streams encoders are refused as by GraphedStep without static_rows."""
+
+    def __init__(self, model, loss_fn, example_batch, warmup=3, optimizer=None, max_grad_norm=None):
+        if not callable(getattr(model, "draw", None)) or not getattr(model, "draws_key", None) or \
+                not getattr(model, "tasks", None):
+            raise TypeError("GraphedTaskSteps: the model must define draw(sample_list, task=None), draws_key and tasks; "
+                            "capture a model that draws nothing on the host with GraphedStep")
+        _check_optimizer("GraphedTaskSteps", optimizer, max_grad_norm)
+        _check_runners("GraphedTaskSteps", model, False)
+        for m in model.modules():
+            if m is not model and getattr(m, "graph_capturable", True) is False and \
+                    not getattr(m, "static_rows_capturable", False):
+                raise RuntimeError("GraphedTaskSteps: %s %s, so its step cannot be captured"
+                                   % (type(m).__name__, getattr(m, "graph_refusal", "does work on the host in every forward")))
+        self.model, self.loss_fn = model, loss_fn
+        self.optimizer, self.max_grad_norm = optimizer, max_grad_norm
+        self.tasks = list(dict.fromkeys(model.tasks))
+        self.task = None
+        state = (torch.get_rng_state(), np.random.get_state(), random.getstate())
+        try:
+            with _static_rows_context():
+                self._capture(example_batch, warmup)
+        finally:
+            torch.set_rng_state(state[0])
+            np.random.set_state(state[1])
+            random.setstate(state[2])
+
+    def _batch(self, task):
+        """a fresh top level over the static inputs (the forward adds and replaces keys) with the task's static draws"""
+        b = dict(self.static)
+        b[self.model.draws_key] = self.draws[task]
+        return b
+
+    def _capture(self, example_batch, warmup):
+        model, opt = self.model, self.optimizer
+        self.static = _map(lambda t: t.detach().clone(), example_batch)
+        self.draws = {}
+        for t in self.tasks:
+            probe = dict(self.static)
+            model.draw(probe, task=t)
+            self.draws[t] = _map(lambda x: x.detach().clone(), probe[model.draws_key])
+        dev = next(t for t in _flatten(self.static) if t.is_cuda).device
+        self.epoch = F.dropout_epoch(dev, create=True)
+        params = list(dict.fromkeys(model.parameters()))
+        saved = _save_optimizer(opt) if opt is not None else None
+        self.grads, self.used, self.graphs, self.losses, self.plans, self._keep = {}, {}, {}, {}, {}, []
+        pool = None
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        for t in self.tasks:
+            with torch.cuda.stream(side):
+                model.zero_grad(set_to_none=True)          # which parameters task t reaches: those that get a .grad
+                self._step(self._batch(t))
+                self.used[t] = [p for p in params if p.grad is not None]
+                for p in self.used[t]:
+                    self.grads.setdefault(p, p.grad)
+                for _ in range(max(1, warmup)):            # on the shared buffers: the optimizer's tables point at them
+                    self._bind_grads(t)
+                    torch._foreach_zero_([self.grads[p] for p in self.used[t]])
+                    self._step(self._batch(t))
+            torch.cuda.current_stream(dev).wait_stream(side)
+            torch.cuda.synchronize(dev)
+            plan = opt._cap if opt is not None else None
+            counts = None
+            if plan is not None:
+                # the graph reads these device buffers at every replay: they must live as long as it does
+                counts = (plan,) + self._step_slots(plan, params)
+                self._keep.append((opt._clip_table, counts))
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, pool=pool, stream=side):
+                torch._foreach_zero_([self.grads[p] for p in self.used[t]])
+                self.epoch.add_(1)
+                self.losses[t] = self._step(self._batch(t), counts)
+            pool = graph.pool()
+            self.graphs[t], self.plans[t] = graph, plan
+        if opt is not None:
+            _restore_optimizer(opt, saved)
+            steps = [saved["state"].get(p, {}).get("step", 0) for p in params]
+            from .optim import _read_steps
+            self.steps.copy_(torch.tensor(_read_steps(steps) + [0], dtype=torch.int64))
+            for i, p in enumerate(params):
+                if p in opt.state:
+                    opt.state[p]["step"] = self.steps[i]
+            torch.cuda.synchronize(dev)
+        self._bind_grads(self.tasks[-1])
+
+    def _step_slots(self, plan, params):
+        """device index tables between the plan's step-count slots and the shared per-parameter table `self.steps`
+        (one entry per parameter, then one spare for the slots no parameter reads)"""
+        if not hasattr(self, "steps"):
+            self.steps = torch.zeros(len(params) + 1, dtype=torch.int64, device=plan.device)
+        index = {id(p): i for i, p in enumerate(params)}
+        group_of = {id(p): gi for gi, g in enumerate(self.optimizer.param_groups) for p in g["params"]}
+        slot_param = [len(params)] * len(plan.slots)
+        written = []                                       # (parameter index, slot)
+        for pack, _, s0, _, _, _ in plan.packs:
+            for p in pack.params:
+                if id(p) in group_of and p.grad is not None:
+                    slot_param[s0 + group_of[id(p)]] = index[id(p)]
+                    written.append((index[id(p)], s0 + group_of[id(p)]))
+        for p, slot in plan.loose:
+            slot_param[slot] = index[id(p)]
+            written.append((index[id(p)], slot))
+        to_dev = lambda v: torch.tensor(v, dtype=torch.int64).to(plan.device)
+        return to_dev(slot_param), to_dev([s for _, s in written]), to_dev([i for i, _ in written])
+
+    def _bind_grads(self, task):
+        for p in self.grads:
+            p.grad = None
+        for p in self.used[task]:
+            p.grad = self.grads[p]
+
+    def _step(self, batch, counts=None):
+        loss = self.loss_fn(batch)
+        loss.backward()
+        opt = self.optimizer
+        if opt is not None:
+            if self.max_grad_norm is not None:
+                opt.clip_grad_norm(self.max_grad_norm)
+            if counts is not None:                         # this graph's step counts from the shared table ...
+                plan, gather, slots, idx = counts
+                plan.step.copy_(self.steps.index_select(0, gather))
+            opt.step()
+            if counts is not None:                         # ... and back
+                self.steps.index_copy_(0, idx, plan.step.index_select(0, slots))
+        return loss
+
+    def __call__(self, batch=None):
+        if batch is not None:
+            _copy_into(self.static, batch)
+        probe = dict(self.static)
+        task = self.model.draw(probe)
+        _copy_into(self.draws[task], probe[self.model.draws_key])
+        if self.optimizer is not None:
+            self.optimizer.stage_hparams(self.plans[task])
+        self.graphs[task].replay()
+        self._bind_grads(task)
+        self.task = task
+        return self.losses[task]
 
 
 def _save_optimizer(opt):

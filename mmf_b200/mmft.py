@@ -27,6 +27,7 @@ import warnings
 import torch
 from torch import nn
 
+from . import functional as F
 from . import ops
 from .encoders import build_encoder
 from .graphs import static_rows_active
@@ -311,6 +312,47 @@ def _linear_gelu_ln(seq, x):
     return ops.layer_norm(h, seq[2].weight, seq[2].bias, seq[2].eps)
 
 
+def _static_region_rows(seq, sequence_output, masks, targets):
+    """Static-rows form of compute_masked_hidden + the region transform: inside graphs.static_rows() the label / target
+    entry holds every region's target [B, R, D] and the regions are the last R rows of the sequence (UNITER's layout:
+    text, then regions).  The masked regions are selected on the device into a fixed capacity of B * R rows
+    (F.select_rows over the region mask), gathered, and run through Linear -> GELU -> LayerNorm bounded by the device
+    count.  Returns (h, selection, fp32 targets [B * R, D])."""
+    B, R, D = targets.shape
+    H = sequence_output.shape[-1]
+    region = masks[:, masks.shape[1] - R:].reshape(-1).to(torch.int64).contiguous()
+    sel = F.select_rows(region, 0)
+    rows = ops.gather_rows(sequence_output[:, sequence_output.shape[1] - R:].reshape(B * R, H), sel)
+    h = ops.linear_gelu_layer_norm_static(rows, seq[0].weight, seq[0].bias, seq[2].weight, seq[2].bias, seq[2].eps,
+                                          sel.count)
+    return h, sel, targets.reshape(B * R, D).float().contiguous()
+
+
+def _static_region_loss(seq, sequence_output, masks, targets, kind, projection=None):
+    """MRC's KL loss (kind "kl", the classifier's last Linear) or MRFR's mean squared error (kind "mse", the tied
+    projection read MN-major) over the masked regions, bounded by their device count: 0 with zero gradients when no
+    region is masked"""
+    h, sel, tgt = _static_region_rows(seq, sequence_output, masks, targets)
+    if kind == "kl":
+        last = seq[3]
+        return ops.region_loss_static(h, last.weight, last.bias, tgt, sel.pos, sel.count, sel.scale, "kl")
+    weight, bias = projection
+    return ops.region_loss_static(h, weight, bias, tgt, sel.pos, sel.count, sel.scale * (1.0 / tgt.shape[1]), "mse",
+                                  weight_t=True)
+
+
+def _static_region_ce(seq, sequence_output, masks, targets, ignore_index):
+    """MRC without KL: cross-entropy against the arg-max of each target row past the background class, found on the
+    device, through the bounded cross-entropy row kernel.  The 1601-wide projection is padded to a multiple of 8 with a
+    -30000 bias, so the padding columns vanish from the softmax."""
+    h, sel, tgt = _static_region_rows(seq, sequence_output, masks, targets)
+    labels = torch.max(tgt[:, 1:], dim=-1)[1] + 1
+    labels = torch.where(sel.pos >= 0, labels.index_select(0, sel.pos.clamp_min(0)).to(torch.int64),
+                         torch.full_like(labels, ignore_index))
+    last = seq[3]
+    return ops.linear_cross_entropy_static(h, last.weight, last.bias, labels, sel.count, sel.scale, ignore_index)
+
+
 @register_transformer_head("mrc")
 class MRCHead(nn.Module):
     """Masked region classification (heads/mrc.py:15-90); parameters `region_classifier.{0,2,3}.*`"""
@@ -326,6 +368,13 @@ class MRCHead(nn.Module):
     def forward(self, sequence_output, encoded_layers=None, processed_sample_list=None):
         region_labels = _required(processed_sample_list, self.mrc_label_key, "MRC")
         masks = _required(processed_sample_list, self.mrc_mask_key, "MRC")
+        if static_rows_active():
+            if self.use_kl:
+                loss = _static_region_loss(self.region_classifier, sequence_output, masks, region_labels, "kl")
+            else:
+                loss = _static_region_ce(self.region_classifier, sequence_output, masks, region_labels,
+                                         self.ignore_index)
+            return {"losses": {self.loss_name: loss}}
         h = _linear_gelu_ln(self.region_classifier, compute_masked_hidden(sequence_output, masks))
         last = self.region_classifier[3]
         logits = ops.linear_any(h, last.weight, last.bias).float()       # label_dim = 1601 is not a multiple of 8
@@ -357,6 +406,10 @@ class MRFRHead(nn.Module):
     def forward(self, sequence_output, encoded_layers=None, processed_sample_list=None):
         feat_targets = _required(processed_sample_list, self.mrfr_target_key, "MRFR")
         masks = _required(processed_sample_list, self.mrfr_mask_key, "MRFR")
+        if static_rows_active():
+            loss = _static_region_loss(self.feat_regress, sequence_output, masks, feat_targets, "mse",
+                                       (self.linear_proj_weight, self.linear_proj_bias))
+            return {"losses": {self.loss_name: loss}}
         h = _linear_gelu_ln(self.feat_regress, compute_masked_hidden(sequence_output, masks))
         prediction = ops.linear_t(h, self.linear_proj_weight, self.linear_proj_bias)
         loss = nn.functional.mse_loss(prediction.float(), feat_targets.float(), reduction="mean")
@@ -399,6 +452,12 @@ class WRAHead(nn.Module):
         y_len = self._lengths(ot_inputs["img_pad"], ot_inputs.get("img_lens"), il, "img_pad")
         itm_labels = processed_sample_list[self.wra_label_key]
         ot_dist = ops.optimal_transport_dist(sequence_output, tl, il, x_len, y_len).to(sequence_output.dtype)
+        if static_rows_active():
+            # the same loss from masked sums and a device count: nothing is read on the host
+            pos, neg = itm_labels == 1, itm_labels == 0
+            zero = ot_dist.new_zeros(())
+            total = torch.where(pos, ot_dist, zero).sum() - torch.where(neg, ot_dist, zero).sum()
+            return {"losses": {self.loss_name: total / (pos.sum() + neg.sum()).to(ot_dist.dtype)}}
         ot_pos = ot_dist.masked_select(itm_labels == 1)
         ot_neg = ot_dist.masked_select(itm_labels == 0)
         loss = (ot_pos.sum() - ot_neg.sum()) / (ot_pos.size(0) + ot_neg.size(0))

@@ -409,6 +409,102 @@ def linear_t(x2d, weight_kn, bias):
     return _LinearT.apply(x2d, weight_kn, bias)
 
 
+class _LinearGELULayerNormStatic(torch.autograd.Function):
+    """LayerNorm(gelu(x W^T + b)) - the region heads' transform - on a fixed capacity of rows of which the first `count`
+    (int32 [1] on the device) are live and the rest zero: the GELU GEMM, the LayerNorm and their backward (LayerNorm,
+    GELU', dgrad, weight gradient, bias column sum) are all bounded by the device count, so nothing is read on the host.
+    Output rows past the count are zero."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, ln_weight, ln_bias, eps, count):
+        xb, wb, bb, g, be = _bf16(x), _bf16(weight), _bf16(bias), _bf16(ln_weight), _bf16(ln_bias)
+        u, h = F.gemm(xb, wb, epi=lib.EPI_BIAS_GELU, bias=bb, m_bound=count)
+        y, mean, rstd = F.layernorm_fwd(h, g, be, eps, m_bound=count)
+        ctx.save_for_backward(xb, wb, u, h, mean, rstd, g, count)
+        ctx.dtypes = (x.dtype, weight.dtype, bias.dtype, ln_weight.dtype, ln_bias.dtype)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        xb, wb, u, h, mean, rstd, g, count = ctx.saved_tensors
+        dg = torch.zeros(g.shape, dtype=torch.float32, device=g.device)
+        dbeta = torch.zeros_like(dg)
+        # rows at and past the count come back zero; u is finite up to the 128-row tile edge, which is as far as the
+        # dgrad reads du (the weight gradient reads it to the 64-row k-block edge)
+        dh, _ = F.layernorm_bwd(dy.to(torch.bfloat16).contiguous(), h, mean, rstd, g, dg, dbeta, m_bound=count)
+        du = F.gelu_bwd(dh, u)
+        dx = F.gemm(du, wb, b_mn=True, epi=lib.EPI_BIAS, m_bound=count)
+        dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)
+        F.gemm(du, xb, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
+               splits=best_splits(wb.shape[0], wb.shape[1], xb.shape[0]), k_bound=count)
+        db = torch.zeros(wb.shape[0], dtype=torch.float32, device=wb.device)
+        F.colsum_bounded(du, db, count)
+        t = ctx.dtypes
+        return dx.to(t[0]), dw.to(t[1]), db.to(t[2]), dg.to(t[3]), dbeta.to(t[4]), None, None
+
+
+def linear_gelu_layer_norm_static(x2d, weight, bias, ln_weight, ln_bias, eps, count):
+    """LayerNorm(gelu(x2d W^T + b)) on the rows below `count` (int32 [1] on the device) of a fixed capacity whose later rows
+    are zero; bf16 [M, N], zero past the count"""
+    return _LinearGELULayerNormStatic.apply(x2d, weight, bias, ln_weight, ln_bias, float(eps), count)
+
+
+class _RegionLossStatic(torch.autograd.Function):
+    """The region heads' output projection and loss on a fixed capacity of rows whose first `count` are the masked regions:
+    z = h W^T + b (weight [N, K]) or h W + b (weight_t: W stored [K, N], MRFR's tied image projection, read MN-major), then
+    mmfb_kl_rows_bounded (MRC) or mmfb_mse_rows_bounded (MRFR) against target[tgt_idx[r]], which write d(z) in place; the
+    dgrad, weight gradient and bias column sum run in the forward too, every kernel bounded by the device count.  The loss
+    is the fixed-order sum of the row losses times `scale` (fp32 [1] on the device), so the same bits on every run; the
+    backward multiplies the saved gradients by the incoming scalar.  N need not be a multiple of 8: the weight and bias are
+    zero-padded and the loss kernel zeroes the padding columns' gradient."""
+
+    @staticmethod
+    def forward(ctx, h, weight, bias, target, tgt_idx, count, scale, kind, weight_t):
+        hb, wb, bb = _bf16(h), _bf16(weight), _bf16(bias)
+        K, N = wb.shape if weight_t else wb.shape[::-1]
+        pad = (-N) % 8
+        if pad:
+            if weight_t:
+                raise ValueError("region loss: a transposed weight needs N %% 8 == 0, got %d" % N)
+            wb = torch.nn.functional.pad(wb, (0, 0, 0, pad))
+            bb = torch.nn.functional.pad(bb, (0, pad))
+        M = hb.shape[0]
+        z = F.gemm(hb, wb, b_mn=weight_t, epi=lib.EPI_BIAS, bias=bb, m_bound=count)
+        row_loss = torch.zeros(M, dtype=torch.float32, device=hb.device)
+        if kind == "kl":
+            F.kl_rows_bounded(z, N, target, tgt_idx, count, scale, row_loss)
+        else:
+            F.mse_rows_bounded(z, target, tgt_idx, count, scale, row_loss)
+        dh = F.gemm(z, wb, b_mn=not weight_t, epi=lib.EPI_BIAS, out=torch.zeros_like(hb), m_bound=count)
+        dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)
+        if weight_t:                                  # [K, N] = h^T z
+            F.gemm(hb, z, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw, splits=best_splits(K, N + pad, M),
+                   k_bound=count)
+        else:                                         # [N, K] = z^T h
+            F.gemm(z, hb, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw, splits=best_splits(N + pad, K, M),
+                   k_bound=count)
+        db = torch.zeros(N + pad, dtype=torch.float32, device=wb.device)
+        F.colsum_bounded(z, db, count)
+        ctx.save_for_backward(dh, dw[:N] if not weight_t else dw, db[:N])
+        ctx.dtypes = (h.dtype, weight.dtype, bias.dtype)
+        return row_loss.sum() * scale.reshape(())
+
+    @staticmethod
+    def backward(ctx, g):
+        dh, dw, db = ctx.saved_tensors
+        t = ctx.dtypes
+        return ((dh.float() * g).to(t[0]), (dw * g).to(t[1]), (db * g).to(t[2])) + (None,) * 6
+
+
+def region_loss_static(h2d, weight, bias, target, tgt_idx, count, scale, kind, weight_t=False):
+    """kind "kl": scale * sum_r KL(target[tgt_idx[r]] || softmax(h_r W^T + b)); kind "mse": scale * sum_r
+    ||h_r W + b - target[tgt_idx[r]]||^2 (weight_t=True, weight [K, N]) - over the rows r below `count` (int32 [1] on the
+    device) of a fixed capacity whose later rows are zero.  target: fp32 [*, N]; tgt_idx: int32, one per row."""
+    if kind not in ("kl", "mse"):
+        raise ValueError("region_loss_static: kind must be 'kl' or 'mse', got %r" % (kind,))
+    return _RegionLossStatic.apply(h2d, weight, bias, target, tgt_idx, count, scale, kind, bool(weight_t))
+
+
 class _OptimalTransport(torch.autograd.Function):
     """dist [B] of mmfb_ot_fwd over two row ranges of one sequence buffer; the backward (mmfb_ot_bwd) writes both ranges of
     the sequence gradient in place.  The plan is a constant of the backward, as in the reference (ot.py:98-101)."""

@@ -17,8 +17,13 @@ What the reference does, and so what is done here:
   * `encoder` / `text_embeddings` are keyword overrides of the bert-base BertConfig (`type`, `params` and other nested
     entries of the default YAML are carried by that config and read by nobody).
 There is no hub here: `random_init` / `bert_model_name` only select the bert-base hyper-parameters and weights arrive
-through load_state_dict.  The step draws on the host and gathers a data-dependent number of rows, so GraphedStep refuses
-this model.
+through load_state_dict.
+
+CUDA graphs: `UNITER.draw(sample_list)` makes a forward's host draws (the task, and for mrc / mrfr the region masks) up
+front and stores them in the sample list under DRAWS_KEY; a forward that finds them there draws nothing and, inside
+graphs.static_rows(), reads nothing on the host (device-side position-feature normalisation, WRA pads built on the device,
+region heads bounded by a device count).  mmf_b200.graphs.GraphedTaskSteps captures one graph per task on that basis;
+GraphedStep refuses the model, whose every step draws on the host.
 """
 import collections.abc
 import copy
@@ -30,6 +35,7 @@ import torch
 from torch import nn
 
 from .models import BERT_BASE, MODEL_DEFAULTS, BaseModel, ConfigNode, Losses, _sl_get
+from .graphs import static_rows_active
 from .registry import registry
 from .uniter import B200UNITERModelBase
 
@@ -51,6 +57,8 @@ CONFIG_DEFAULTS = dict(random_init=False, bert_model_name="bert-base-uncased", i
 DEFAULT_PRETRAINING_HEAD_CONFIGS = {"mlm": {"type": "mlm"}, "itm": {"type": "itm"}, "mrc": {"type": "mrc"},
                                     "mrfr": {"type": "mrfr"}, "wra": {"type": "wra"}}
 DEFAULT_PRETRAINING_TASKS = "mlm,itm,mrc,mrfr,wra"
+
+DRAWS_KEY = "uniter_draws"       # {"task": name, "image_mask": bool [B, R] (mrc / mrfr)}: see UNITER.draw
 
 _UNSUPPORTED = ("output_attentions", "output_hidden_states", "is_decoder", "add_cross_attention")
 
@@ -178,11 +186,21 @@ class B200UNITERForPretraining(nn.Module):
         if task not in ("wra", "itm"):
             self._remove_mismatched_captions(sl)
 
+    def draw_image_masks(self, image_feat):
+        """one region mask per sample (uniter.py:476-481), as a bool [B, R] tensor on image_feat's device"""
+        img_masks = torch.tensor([self._get_img_mask(self.mask_probability, image_feat.size(1))
+                                  for _ in range(image_feat.size(0))]).bool()
+        if image_feat.is_cuda:           # from pinned memory: the copy does not wait for the work queued before it
+            return img_masks.pin_memory().to(image_feat.device, non_blocking=True)
+        return img_masks
+
     def _add_image_feat_masked(self, sl):
         img_feat_masked = torch.clone(sl["image_feat"])
-        num_feat = img_feat_masked.size(1)
-        img_masks = [self._get_img_mask(self.mask_probability, num_feat) for _ in range(img_feat_masked.size(0))]
-        img_masks = torch.tensor(img_masks).bool().to(img_feat_masked.device)
+        drawn = sl.get(DRAWS_KEY)
+        if drawn is not None and drawn.get("image_mask") is not None:
+            img_masks = drawn["image_mask"]
+        else:
+            img_masks = self.draw_image_masks(img_feat_masked)
         sl["image_feat_masked"] = img_feat_masked.data.masked_fill(img_masks.unsqueeze(-1).expand_as(img_feat_masked), 0)
         sl["image_mask"] = img_masks
 
@@ -208,7 +226,7 @@ class B200UNITERForPretraining(nn.Module):
         sl["itm_labels"] = {"is_correct": sl["is_correct"]}
 
     def _get_feature_mask(self, image_mask, sentence_len):
-        padding_for_txt = torch.zeros((image_mask.size(0), sentence_len)).to(image_mask)
+        padding_for_txt = torch.zeros((image_mask.size(0), sentence_len), dtype=image_mask.dtype, device=image_mask.device)
         return torch.cat([padding_for_txt, image_mask], dim=-1)
 
     def _mask_inputs_in_sample_list(self, sl, mask_key):
@@ -222,16 +240,22 @@ class B200UNITERForPretraining(nn.Module):
         assert "image_feat_masked" in sl
         image_mask = sl["image_mask"]
         cls_prob = sl["cls_prob"].to(image_mask.device)
-        img_masks_ext = image_mask.unsqueeze(-1).expand_as(cls_prob)
-        sl[self.heads["mrc"].mrc_label_key] = cls_prob[img_masks_ext].contiguous().view(-1, cls_prob.size(2))
+        if static_rows_active():         # every region's target: the head selects the masked ones on the device
+            sl[self.heads["mrc"].mrc_label_key] = cls_prob
+        else:
+            img_masks_ext = image_mask.unsqueeze(-1).expand_as(cls_prob)
+            sl[self.heads["mrc"].mrc_label_key] = cls_prob[img_masks_ext].contiguous().view(-1, cls_prob.size(2))
         self._mask_inputs_in_sample_list(sl, self.heads["mrc"].mrc_mask_key)
 
     def _preprocess_mrfr(self, sl):
         assert "image_mask" in sl
         assert "image_feat_masked" in sl
         image_mask, image_feat = sl["image_mask"], sl["image_feat"]
-        img_masks_ext = image_mask.unsqueeze(-1).expand_as(image_feat)
-        sl[self.heads["mrfr"].mrfr_target_key] = image_feat[img_masks_ext].contiguous().view(-1, image_feat.size(2))
+        if static_rows_active():
+            sl[self.heads["mrfr"].mrfr_target_key] = image_feat
+        else:
+            img_masks_ext = image_mask.unsqueeze(-1).expand_as(image_feat)
+            sl[self.heads["mrfr"].mrfr_target_key] = image_feat[img_masks_ext].contiguous().view(-1, image_feat.size(2))
         self._mask_inputs_in_sample_list(sl, self.heads["mrfr"].mrfr_mask_key)
 
     def _preprocess_wra(self, sl):
@@ -239,16 +263,19 @@ class B200UNITERForPretraining(nn.Module):
         txt_lens = [i.size(0) for i in sl["input_ids"]]
         num_bbs = [f.size(0) for f in sl["image_feat"]]
 
+        device = sl["input_ids"].device
+
         def _compute_pad(lens):
-            pad = torch.zeros(len(lens), max(lens))
+            # uniter.py:565-570, built on the device: row i is padding from lens[i] on
+            pad = torch.zeros(len(lens), max(lens), dtype=torch.bool, device=device)
             for i, n in enumerate(lens):
-                pad.data[i, n:].fill_(1)
+                if n < pad.size(1):
+                    pad[i, n:] = True
             return pad
 
-        device = sl["input_ids"].device
-        # the lengths ride along on the host: the kernel takes them as launch parameters
-        sl[self.heads["wra"].ot_inputs_key] = {"txt_pad": _compute_pad(txt_lens).to(device).bool(),
-                                               "img_pad": _compute_pad(num_bbs).to(device).bool(),
+        # the lengths are the padded sizes, so they depend only on shapes; they ride along on the host, where the kernel
+        # takes them as launch parameters
+        sl[self.heads["wra"].ot_inputs_key] = {"txt_pad": _compute_pad(txt_lens), "img_pad": _compute_pad(num_bbs),
                                                "txt_lens": txt_lens, "img_lens": num_bbs}
         sl[self.heads["wra"].wra_label_key] = sl["is_correct"]
 
@@ -269,9 +296,11 @@ class B200UNITERForPretraining(nn.Module):
 class UNITER(BaseModel):
     """Modification for Joint Vision-Language Encoding (uniter.py:615-774)"""
 
-    graph_capturable = False        # host-side task / mask draws and masked gathers: see mmf_b200.graphs.GraphedStep
+    graph_capturable = False        # host-side task / mask draws: see mmf_b200.graphs.GraphedTaskSteps
     graph_refusal = ("draws its task and region masks on the host in every forward and gathers a data-dependent number of "
-                     "rows")
+                     "rows; capture one graph per task with mmf_b200.graphs.GraphedTaskSteps")
+
+    draws_key = DRAWS_KEY
 
     def __init__(self, config):
         super().__init__(config)
@@ -299,6 +328,22 @@ class UNITER(BaseModel):
     def init_losses(self):
         """Defer loss management to submodels, do nothing when called by build_model."""
 
+    def draw(self, sample_list, task=None):
+        """Make the host draws of a forward, in the reference's order, and store them in the sample list under DRAWS_KEY:
+        the task with torch.randint over `tasks` (classification too), then for mrc / mrfr one region mask per sample
+        with np.random.binomial + random.choice, as a bool [B, R] tensor on the features' device.  A forward that finds
+        them draws nothing, so `draw` followed by a forward makes the same choices from the same seeds as a forward
+        alone.  `task` fixes the task instead of drawing it (the masks are still drawn).  Returns the task's name."""
+        if task is None:
+            task = self.tasks[torch.randint(len(self.tasks), (1,)).item()]
+        elif task not in self.tasks:
+            raise ValueError("UNITER.draw: task %r is not one of %s" % (task, self.tasks))
+        draws = {"task": task}
+        if self.do_pretraining and task in ("mrc", "mrfr"):
+            draws["image_mask"] = self.uniter.draw_image_masks(sample_list["image_feature_0"])
+        sample_list[DRAWS_KEY] = draws
+        return task
+
     def add_pos_feat(self, sample_list):
         info = _sl_get(sample_list, "image_info_0", None)
         assert info is not None
@@ -306,11 +351,17 @@ class UNITER(BaseModel):
         # (x1, y1, x2, y2), dim = (bs, num_feats, 4)
         bboxs = torch.as_tensor(_sl_get(info, "bbox"))[:, :, :4]
         norm_xy = torch.clone(bboxs)
-        if norm_xy[0, 0, 0] < 1:          # the reference's rule, kept as written (uniter.py:686-700)
+
+        def max_image_size():
             img_h = torch.as_tensor(_sl_get(info, "image_height")).unsqueeze(1).unsqueeze(1)
             img_w = torch.as_tensor(_sl_get(info, "image_width")).unsqueeze(1).unsqueeze(1)
-            max_image_size = torch.cat([img_w, img_h, img_w, img_h], dim=-1).to(norm_xy.device)
-            norm_xy /= max_image_size
+            return torch.cat([img_w, img_h, img_w, img_h], dim=-1).to(norm_xy.device)
+
+        if DRAWS_KEY in sample_list and _sl_get(info, "image_height", None) is not None:
+            # the same rule selected on the device, so a captured step reads nothing on the host
+            norm_xy = torch.where(norm_xy[0, 0, 0] < 1, norm_xy / max_image_size(), norm_xy)
+        elif norm_xy[0, 0, 0] < 1:        # the reference's rule, kept as written (uniter.py:686-700)
+            norm_xy /= max_image_size()
         bbox_w = (norm_xy[:, :, 2] - norm_xy[:, :, 0]).unsqueeze(-1)
         bbox_h = (norm_xy[:, :, 3] - norm_xy[:, :, 1]).unsqueeze(-1)
         area = bbox_w * bbox_h
@@ -327,8 +378,11 @@ class UNITER(BaseModel):
             assert len(image_dim.size()) == len(image_mask.size())
         sample_list["image_mask"] = (image_mask < image_dim).long()
         sample_list["attention_mask"] = torch.cat((sample_list["input_mask"], sample_list["image_mask"]), dim=-1)
-        task_index = torch.randint(len(self.tasks), (1,)).item()
-        sample_list["task"] = self.tasks[task_index]
+        if DRAWS_KEY in sample_list:
+            sample_list["task"] = sample_list[DRAWS_KEY]["task"]
+        else:
+            task_index = torch.randint(len(self.tasks), (1,)).item()
+            sample_list["task"] = self.tasks[task_index]
         sample_list["position_ids"] = torch.arange(0, sample_list["input_ids"].size(1), dtype=torch.long,
                                                    device=image_feat.device).unsqueeze(0)
         self.add_pos_feat(sample_list)
