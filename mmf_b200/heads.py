@@ -81,14 +81,15 @@ class B200BertPreTrainingHeads(nn.Module):
 def static_masked_lm_loss(predictions, sequence_output, labels, ignore_index=-1):
     """mean CE of the masked-LM head over the labelled rows, with no host read: the rows are selected on the device
     (F.select_rows) into a fixed capacity of every row of `labels`, zero past the count; the transform runs on the whole
-    capacity, the vocabulary GEMM and the loss only on the labelled rows (ops.linear_cross_entropy_static).  A batch with
-    no labelled row gives a loss of exactly 0 and zero gradients.  `predictions` is a B200BertLMPredictionHead."""
+    capacity, the vocabulary GEMM and the loss only on the labelled rows (ops.linear_cross_entropy with a count).  A
+    batch with no labelled row gives a loss of exactly 0 and zero gradients.  `predictions` is a
+    B200BertLMPredictionHead."""
     H = sequence_output.shape[-1]
     sel = F.select_rows(labels.reshape(-1).to(torch.int64).contiguous(), ignore_index)
     rows = ops.gather_rows(sequence_output.reshape(-1, H), sel)
     h = predictions.transform(rows)
-    return ops.linear_cross_entropy_static(h, predictions.decoder.weight, predictions.bias, sel.labels, sel.count,
-                                           sel.scale, ignore_index)
+    return ops.linear_cross_entropy(h, predictions.decoder.weight, predictions.bias, sel.labels, ignore_index,
+                                    count=sel.count, scale=sel.scale)
 
 
 def masked_lm_loss(cls, sequence_output, masked_lm_labels, ignore_index=-1, positions="all"):

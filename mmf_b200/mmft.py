@@ -306,10 +306,11 @@ def _required(processed_sample_list, key, head):
     return processed_sample_list[key]
 
 
-def _linear_gelu_ln(seq, x):
-    """nn.Sequential(Linear, GELU, LayerNorm) of the region heads: GEMM with the GELU epilogue, then the row LayerNorm"""
-    h = ops.linear_gelu(x, seq[0].weight, seq[0].bias)
-    return ops.layer_norm(h, seq[2].weight, seq[2].bias, seq[2].eps)
+def _linear_gelu_ln(seq, x, count=None):
+    """nn.Sequential(Linear, GELU, LayerNorm) of the region heads: GEMM with the GELU epilogue, then the row LayerNorm;
+    with `count` (int32 [1] on the device) both and their backward are bounded by it, and rows past it are zero"""
+    h = ops.linear_gelu(x, seq[0].weight, seq[0].bias, count)
+    return ops.layer_norm(h, seq[2].weight, seq[2].bias, seq[2].eps, count)
 
 
 def _static_region_rows(seq, sequence_output, masks, targets):
@@ -323,9 +324,7 @@ def _static_region_rows(seq, sequence_output, masks, targets):
     region = masks[:, masks.shape[1] - R:].reshape(-1).to(torch.int64).contiguous()
     sel = F.select_rows(region, 0)
     rows = ops.gather_rows(sequence_output[:, sequence_output.shape[1] - R:].reshape(B * R, H), sel)
-    h = ops.linear_gelu_layer_norm_static(rows, seq[0].weight, seq[0].bias, seq[2].weight, seq[2].bias, seq[2].eps,
-                                          sel.count)
-    return h, sel, targets.reshape(B * R, D).float().contiguous()
+    return _linear_gelu_ln(seq, rows, sel.count), sel, targets.reshape(B * R, D).float().contiguous()
 
 
 def _static_region_loss(seq, sequence_output, masks, targets, kind, projection=None):
@@ -350,7 +349,7 @@ def _static_region_ce(seq, sequence_output, masks, targets, ignore_index):
     labels = torch.where(sel.pos >= 0, labels.index_select(0, sel.pos.clamp_min(0)).to(torch.int64),
                          torch.full_like(labels, ignore_index))
     last = seq[3]
-    return ops.linear_cross_entropy_static(h, last.weight, last.bias, labels, sel.count, sel.scale, ignore_index)
+    return ops.linear_cross_entropy(h, last.weight, last.bias, labels, ignore_index, count=sel.count, scale=sel.scale)
 
 
 @register_transformer_head("mrc")

@@ -9,138 +9,119 @@ import torch
 
 from . import functional as F
 from . import lib
-from .engine import best_splits
+from .engine import _bnd, best_splits
 
 
 def _bf16(t):
     return t.detach().to(torch.bfloat16).contiguous()
 
 
+_EPI = {None: lib.EPI_BIAS, "relu": lib.EPI_BIAS_RELU, "gelu": lib.EPI_BIAS_GELU}
+
+
+def _linear_grads(need, dz, xb, wb, weight_t=False, count=None, dx=None, dw=None, db=None):
+    """The gradients of z = x W^T + b (W [N, K]), or of z = x W + b with W stored [K, N] (weight_t), from dz = dL/dz (bf16),
+    for the inputs (x, W, b) that `need` flags: dx = the dgrad GEMM, written into `dx` (allocated by the GEMM when None);
+    dW = the split-K weight-gradient GEMM and db = the column sum of dz, accumulated in fp32 into `dw` / `db` (allocated
+    zero when None).  With `count` (int32 [1] on the device) every kernel reads only the rows of dz below it.  Returns
+    (dx, dw, db), None where not needed."""
+    if need[0]:
+        dx = F.gemm(dz, wb, b_mn=not weight_t, epi=lib.EPI_BIAS, out=dx, **_bnd("m_bound", count))
+    if need[1]:
+        if dw is None:
+            dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)
+        a, b = (xb, dz) if weight_t else (dz, xb)           # weight_t: [K, N] = x^T dz, otherwise [N, K] = dz^T x
+        F.gemm(a, b, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw, splits=best_splits(*wb.shape, xb.shape[0]),
+               **_bnd("k_bound", count))
+    if need[2]:
+        if db is None:
+            db = torch.zeros(dz.shape[1], dtype=torch.float32, device=dz.device)
+        if count is None:
+            F.colsum(dz, db)
+        else:
+            F.colsum_bounded(dz, db, count)
+    return dx, dw, db
+
+
 class _Linear(torch.autograd.Function):
-    """y = x W^T + b on the wgmma GEMM; backward: dgrad (MN-major W), split-K wgrad, column-sum bias gradient."""
+    """y = act(x W^T + b) on the wgmma GEMM with the bias (+ ReLU / GELU) epilogue; the GELU epilogue also writes the
+    pre-activation u, saved for the backward.  weight_t: W is stored [K, N] and read MN-major (the layout the dgrad calls
+    use), so a weight that is another layer's nn.Linear weight - MRFR's projection back to the feature space, tied to
+    UNITER's img_linear (heads/mrfr.py:48-49, 86-88) - is consumed as it lies and autograd sums both uses' gradients into
+    the one parameter.  count: int32 [1] on the device, the live rows of a fixed capacity whose later rows are zero; the
+    GEMM and the dgrad, weight gradient and bias column sum of the backward are bounded by it, so nothing is read on the
+    host.  Backward: dy masked by (y > 0) (relu_bwd) or times GELU'(u) (gelu_bwd), then _linear_grads."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias):
+    def forward(ctx, x, weight, bias, act, weight_t, count):
         xb, wb = _bf16(x), _bf16(weight)
         bb = _bf16(bias) if bias is not None else None
-        y = F.gemm(xb, wb, epi=lib.EPI_BIAS, bias=bb)
-        ctx.save_for_backward(xb, wb)
+        y = F.gemm(xb, wb, b_mn=weight_t, epi=_EPI[act], bias=bb, **_bnd("m_bound", count))
+        aux = None
+        if act == "gelu":
+            aux, y = y
+        elif act == "relu":
+            aux = y
+        ctx.save_for_backward(xb, wb, aux, count)
+        ctx.act, ctx.weight_t = act, weight_t
         ctx.dtypes = (x.dtype, weight.dtype, bias.dtype if bias is not None else None)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        xb, wb = ctx.saved_tensors
-        dyb = dy.to(torch.bfloat16).contiguous()
-        dx = dw = db = None
-        if ctx.needs_input_grad[0]:
-            dx = F.gemm(dyb, wb, b_mn=True, epi=lib.EPI_BIAS).to(ctx.dtypes[0])
-        if ctx.needs_input_grad[1]:
-            dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)
-            F.gemm(dyb, xb, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
-                   splits=best_splits(wb.shape[0], wb.shape[1], xb.shape[0]))
-            dw = dw.to(ctx.dtypes[1])
-        if ctx.dtypes[2] is not None and ctx.needs_input_grad[2]:
-            db = torch.zeros(wb.shape[0], dtype=torch.float32, device=wb.device)
-            F.colsum(dyb, db)
-            db = db.to(ctx.dtypes[2])
-        return dx, dw, db
+        xb, wb, aux, count = ctx.saved_tensors
+        dz = dy.to(torch.bfloat16).contiguous()
+        if ctx.act == "relu":
+            dz = F.relu_bwd(dz, aux)
+        elif ctx.act == "gelu":
+            # with a count: u is finite up to the 128-row tile edge, which is as far as the dgrad reads dz (the weight
+            # gradient reads it to the 64-row k-block edge); dy is zero at and past the count
+            dz = F.gelu_bwd(dz, aux)
+        grads = _linear_grads(ctx.needs_input_grad, dz, xb, wb, ctx.weight_t, count)
+        return tuple([g if g is None else g.to(t) for g, t in zip(grads, ctx.dtypes)]) + (None, None, None)
 
 
 def linear(x2d, weight, bias=None):
     """x2d [M, K] (any float dtype) -> bf16 [M, N].  K and N must be multiples of 8 (TMA row pitch)."""
-    return _Linear.apply(x2d, weight, bias)
-
-
-class _LinearReLU(torch.autograd.Function):
-    """y = relu(x W^T + b): GEMM with the ReLU epilogue; backward masks dy with (y > 0) and reuses the Linear backward."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias):
-        xb, wb, bb = _bf16(x), _bf16(weight), _bf16(bias)
-        y = F.gemm(xb, wb, epi=lib.EPI_BIAS_RELU, bias=bb)
-        ctx.save_for_backward(xb, wb, y)
-        ctx.dtypes = (x.dtype, weight.dtype, bias.dtype)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        xb, wb, y = ctx.saved_tensors
-        dz = F.relu_bwd(dy.to(torch.bfloat16).contiguous(), y)
-        dx = dw = db = None
-        if ctx.needs_input_grad[0]:
-            dx = F.gemm(dz, wb, b_mn=True, epi=lib.EPI_BIAS).to(ctx.dtypes[0])
-        if ctx.needs_input_grad[1]:
-            dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)
-            F.gemm(dz, xb, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
-                   splits=best_splits(wb.shape[0], wb.shape[1], xb.shape[0]))
-            dw = dw.to(ctx.dtypes[1])
-        if ctx.needs_input_grad[2]:
-            db = torch.zeros(wb.shape[0], dtype=torch.float32, device=wb.device)
-            F.colsum(dz, db)
-            db = db.to(ctx.dtypes[2])
-        return dx, dw, db
+    return _Linear.apply(x2d, weight, bias, None, False, None)
 
 
 def linear_relu(x2d, weight, bias):
-    return _LinearReLU.apply(x2d, weight, bias)
+    return _Linear.apply(x2d, weight, bias, "relu", False, None)
 
 
-class _LinearGELU(torch.autograd.Function):
-    """h = gelu(x W^T + b): GEMM with the bias + GELU epilogue (it also writes the pre-activation u, saved for the
-    backward); backward: du = dh * GELU'(u) (row kernel), then the Linear backward."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias):
-        xb, wb, bb = _bf16(x), _bf16(weight), _bf16(bias)
-        u, h = F.gemm(xb, wb, epi=lib.EPI_BIAS_GELU, bias=bb)
-        ctx.save_for_backward(xb, wb, u)
-        ctx.dtypes = (x.dtype, weight.dtype, bias.dtype)
-        return h
-
-    @staticmethod
-    def backward(ctx, dh):
-        xb, wb, u = ctx.saved_tensors
-        du = F.gelu_bwd(dh.to(torch.bfloat16).contiguous(), u)
-        dx = dw = db = None
-        if ctx.needs_input_grad[0]:
-            dx = F.gemm(du, wb, b_mn=True, epi=lib.EPI_BIAS).to(ctx.dtypes[0])
-        if ctx.needs_input_grad[1]:
-            dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)
-            F.gemm(du, xb, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
-                   splits=best_splits(wb.shape[0], wb.shape[1], xb.shape[0]))
-            dw = dw.to(ctx.dtypes[1])
-        if ctx.needs_input_grad[2]:
-            db = torch.zeros(wb.shape[0], dtype=torch.float32, device=wb.device)
-            F.colsum(du, db)
-            db = db.to(ctx.dtypes[2])
-        return dx, dw, db
+def linear_gelu(x2d, weight, bias, count=None):
+    """gelu(x2d W^T + b); with `count` (int32 [1] on the device) only the rows below it are computed, later rows are zero"""
+    return _Linear.apply(x2d, weight, bias, "gelu", False, count)
 
 
-def linear_gelu(x2d, weight, bias):
-    return _LinearGELU.apply(x2d, weight, bias)
+def linear_t(x2d, weight_kn, bias):
+    """F.linear(x, weight_kn.t(), bias): x2d [M, K], weight_kn [K, N] -> bf16 [M, N]; K and N multiples of 8."""
+    return _Linear.apply(x2d, weight_kn, bias, None, True, None)
 
 
 class _LayerNorm(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, weight, bias, eps):
+    def forward(ctx, x, weight, bias, eps, count):
         xb, g, b = _bf16(x), _bf16(weight), _bf16(bias)
-        y, mean, rstd = F.layernorm_fwd(xb, g, b, eps)
-        ctx.save_for_backward(xb, mean, rstd, g)
+        y, mean, rstd = F.layernorm_fwd(xb, g, b, eps, **_bnd("m_bound", count))
+        ctx.save_for_backward(xb, mean, rstd, g, count)
         ctx.dtypes = (x.dtype, weight.dtype, bias.dtype)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        xb, mean, rstd, g = ctx.saved_tensors
+        xb, mean, rstd, g, count = ctx.saved_tensors
         dg = torch.zeros(g.shape, dtype=torch.float32, device=g.device)
         db = torch.zeros_like(dg)
-        dx, _ = F.layernorm_bwd(dy.to(torch.bfloat16).contiguous(), xb, mean, rstd, g, dg, db)
-        return dx.to(ctx.dtypes[0]), dg.to(ctx.dtypes[1]), db.to(ctx.dtypes[2]), None
+        dx, _ = F.layernorm_bwd(dy.to(torch.bfloat16).contiguous(), xb, mean, rstd, g, dg, db, **_bnd("m_bound", count))
+        return dx.to(ctx.dtypes[0]), dg.to(ctx.dtypes[1]), db.to(ctx.dtypes[2]), None, None
 
 
-def layer_norm(x2d, weight, bias, eps=1e-12):
-    return _LayerNorm.apply(x2d, weight, bias, eps)
+def layer_norm(x2d, weight, bias, eps=1e-12, count=None):
+    """row LayerNorm; with `count` (int32 [1] on the device) only the rows below it are read and written, later output rows
+    and their gradients are zero"""
+    return _LayerNorm.apply(x2d, weight, bias, eps, count)
 
 
 class _ComposeLN(torch.autograd.Function):
@@ -224,67 +205,89 @@ def linear_any(x2d, weight, bias=None):
     return y[:, :N] if pn else y
 
 
-class _LinearCrossEntropy(torch.autograd.Function):
-    """mean cross-entropy of (h W^T + b) against integer labels WITHOUT the [rows, V] logits tensor: the rows are processed
-    in chunks - vocabulary GEMM -> mmfb_ce_rows (loss + d(logits) in place) -> dgrad and split-K wgrad of the chunk - so at
-    most `chunk_rows` x V logits exist at a time (sized to stay L2-resident between the three kernels that touch them).
-    Gradients are therefore computed in the FORWARD (scaled by 1 / n_active); the backward multiplies them by the incoming
-    scalar.  Reference: prediction scores + CrossEntropyLoss(ignore_index) of mmf/models/visual_bert.py:269-277 and
-    mmf/models/transformers/heads/mlm.py:83-88."""
+class _LinearLoss(torch.autograd.Function):
+    """A loss of the projection z = h W^T + b (W [N, K]), or z = h W + b with W stored [K, N] (weight_t, read MN-major),
+    WITHOUT the [rows, N] tensor z: the rows are processed in chunks - GEMM -> row-loss kernel (loss + d(z) in place) ->
+    dgrad, split-K weight gradient and bias column sum of the chunk (_linear_grads) - so at most `chunk_rows` x N values of
+    z exist at a time (sized to stay L2-resident between the kernels that touch them).  Gradients are therefore computed
+    in the FORWARD, already scaled; the backward multiplies them by the incoming scalar.  N need not be a multiple of 8:
+    the weight and bias are padded, and the row kernels give the padding columns a zero gradient.
+
+    kind "ce": mean cross-entropy against integer `target` labels (mmfb_ce_rows), rows labelled ignore_index excluded.
+    Reference: prediction scores + CrossEntropyLoss(ignore_index) of mmf/models/visual_bert.py:269-277 and
+    mmf/models/transformers/heads/mlm.py:83-88.  kind "kl" / "mse": the region heads' KL divergence from / squared error
+    against the fp32 rows target[tgt_idx[r]] (mmfb_kl_rows_bounded, mmfb_mse_rows_bounded).
+
+    count None (cross-entropy only): the scale 1 / n_active is read on the host, the loss goes to one fp32 sum.
+    count (int32 [1] on the device): static-rows mode, the rows are a fixed capacity of which the first `count` are live
+    and the rest hold zero features (and ignore_index labels), as a CUDA graph can capture it (mmf_b200.graphs).  Every
+    kernel of a chunk takes the chunk's share of `count` as a device bound, so a chunk that starts past `count` costs
+    launches whose CTAs exit at once, and inside a chunk only the rows below `count` rounded up to a 128-row tile are
+    computed; chunk_rows None runs one chunk bounded by `count` itself.  The loss is scaled by `scale` (fp32 [1] on the
+    device): no host read.  The row losses are summed over the whole capacity in one fixed-order sum, for the
+    cross-entropy only in deterministic mode."""
 
     @staticmethod
-    def forward(ctx, h, weight, bias, labels, ignore_index, chunk_rows):
+    def forward(ctx, h, weight, bias, target, tgt_idx, count, scale, kind, ignore_index, weight_t, chunk_rows):
         hb, wb = _bf16(h), _bf16(weight)
-        V, K = wb.shape
-        pad = (-V) % 8
-        if pad:                                # V = 30522 is not a multiple of 8: zero rows, and a -inf-like bias so that
-            wb = torch.nn.functional.pad(wb, (0, 0, 0, pad))      # the padded logits vanish from the softmax
-        bb = _bf16(bias) if bias is not None else torch.zeros(V, dtype=torch.bfloat16, device=wb.device)
+        M, N = hb.shape[0], wb.shape[1 if weight_t else 0]
+        pad = (-N) % 8
+        if pad:                     # zero weight rows; for the softmax of the cross-entropy a -inf-like bias as well, so
+            wb = torch.nn.functional.pad(wb, (0, 0, 0, pad))                 # that the padded logits vanish
+        bb = _bf16(bias) if bias is not None else torch.zeros(N, dtype=torch.bfloat16, device=wb.device)
         if pad:
-            bb = torch.cat([bb, torch.full((pad,), -30000.0, dtype=torch.bfloat16, device=bb.device)])
-        M = hb.shape[0]
-        labels = labels.reshape(-1).to(torch.int64).contiguous()
-        n_active = (labels != ignore_index).sum()
-        scale = 1.0 / float(max(int(n_active), 1))      # the one host read of the head (the reference's mean reduction)
-        loss_sum = torch.zeros((), dtype=torch.float32, device=wb.device)
-        need_h, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        need_b = bias is not None and ctx.needs_input_grad[2]
-        dh = torch.empty_like(hb) if need_h else None
+            fill = -30000.0 if kind == "ce" else 0.0
+            bb = torch.cat([bb, torch.full((pad,), fill, dtype=torch.bfloat16, device=bb.device)])
+        if count is None:
+            scale = 1.0 / float(max(int((target != ignore_index).sum()), 1))    # the one host read (the mean reduction)
+        need = need_h, need_w, need_b = ctx.needs_input_grad[:3]
+        # in static-rows mode rows past count are never written by the bounded kernels: their gradients stay zero
+        dh = (torch.empty_like if count is None else torch.zeros_like)(hb) if need_h else None
         dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device) if need_w else None
-        db = torch.zeros(wb.shape[0], dtype=torch.float32, device=wb.device) if need_b else None
-        for r0 in range(0, M, chunk_rows):
+        db = torch.zeros(N + pad, dtype=torch.float32, device=wb.device) if need_b else None
+        ordered = kind != "ce" or (count is not None and torch.are_deterministic_algorithms_enabled())
+        loss_sum = torch.zeros((), dtype=torch.float32, device=wb.device)
+        row_loss = torch.zeros(M, dtype=torch.float32, device=wb.device) if ordered else None
+        if chunk_rows is None:
+            chunk_rows, bounds = M, count
+        elif count is not None:     # the live rows of chunk i: clamp(count - i * chunk_rows, 0, chunk_rows), one int32 each
+            starts = torch.arange(0, M, chunk_rows, dtype=torch.int32, device=wb.device)
+            bounds = (count.reshape(1) - starts).clamp_(0, chunk_rows)
+        for i, r0 in enumerate(range(0, M, chunk_rows)):
             r1 = min(M, r0 + chunk_rows)
-            z = F.gemm(hb[r0:r1], wb, epi=lib.EPI_BIAS, bias=bb)
-            F.ce_rows(z, labels[r0:r1], ignore_index, scale, loss_sum)      # z now holds d(logits)
-            if need_h:
-                F.gemm(z, wb, b_mn=True, epi=lib.EPI_BIAS, out=dh[r0:r1])
-            if need_w:
-                F.gemm(z, hb[r0:r1], a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
-                       splits=best_splits(wb.shape[0], K, r1 - r0))
-            if need_b:
-                F.colsum(z, db)
-        ctx.save_for_backward(*[t for t in (dh, dw, db) if t is not None])
-        ctx.have = (need_h, need_w, need_b)
-        ctx.V = V
+            nb = None if count is None else bounds[i:i + 1]
+            z = F.gemm(hb[r0:r1], wb, b_mn=weight_t, epi=lib.EPI_BIAS, bias=bb, **_bnd("m_bound", nb))
+            if kind == "kl":
+                F.kl_rows_bounded(z, N, target, tgt_idx[r0:r1], nb, scale, row_loss[r0:r1])
+            elif kind == "mse":
+                F.mse_rows_bounded(z, target, tgt_idx[r0:r1], nb, scale, row_loss[r0:r1])
+            elif count is None:
+                F.ce_rows(z, target[r0:r1], ignore_index, scale, loss_sum)
+            else:
+                F.ce_rows_bounded(z, target[r0:r1], ignore_index, scale, nb, loss_sum=loss_sum,
+                                  row_loss=row_loss[r0:r1] if ordered else None)
+            _linear_grads(need, z, hb[r0:r1], wb, weight_t, nb, dh[r0:r1] if need_h else None, dw, db)
+        if ordered:
+            loss_sum = row_loss.sum()
+        ctx.save_for_backward(dh, dw if dw is None or weight_t else dw[:N], db if db is None else db[:N])
         ctx.dtypes = (h.dtype, weight.dtype, bias.dtype if bias is not None else None)
-        return loss_sum * scale
+        return loss_sum * (scale if count is None else scale.reshape(()))
 
     @staticmethod
     def backward(ctx, g):
-        saved = list(ctx.saved_tensors)
-        need_h, need_w, need_b = ctx.have
-        dh = saved.pop(0) if need_h else None
-        dw = saved.pop(0) if need_w else None
-        db = saved.pop(0) if need_b else None
-        gh = (dh.float() * g).to(ctx.dtypes[0]) if need_h else None
-        gw = (dw[:ctx.V] * g).to(ctx.dtypes[1]) if need_w else None
-        gb = (db[:ctx.V] * g).to(ctx.dtypes[2]) if need_b else None
-        return gh, gw, gb, None, None, None
+        grads = [t if t is None else (t.float() * g).to(dt) for t, dt in zip(ctx.saved_tensors, ctx.dtypes)]
+        return tuple(grads) + (None,) * 8
 
 
-def linear_cross_entropy(h2d, weight, bias, labels, ignore_index=-1, chunk_rows=2048):
-    """mean_i CE((h W^T + b)_i, labels_i) over the rows with labels_i != ignore_index (0 when there is none), fp32 scalar."""
-    return _LinearCrossEntropy.apply(h2d, weight, bias, labels, int(ignore_index), int(chunk_rows))
+def linear_cross_entropy(h2d, weight, bias, labels, ignore_index=-1, chunk_rows=2048, count=None, scale=None):
+    """mean_i CE((h W^T + b)_i, labels_i) over the rows with labels_i != ignore_index (0 when there is none), fp32 scalar.
+    Static-rows mode: `count` (int32 [1] on the device) is the number of labelled rows, which come first, and `scale`
+    (fp32 [1] on the device) = 1 / max(count, 1); later rows must hold ignore_index labels."""
+    if (count is None) != (scale is None):
+        raise ValueError("linear_cross_entropy: count and scale go together")
+    labels = labels.reshape(-1).to(torch.int64).contiguous()
+    return _LinearLoss.apply(h2d, weight, bias, labels, None, count, scale, "ce", int(ignore_index), False,
+                             int(chunk_rows))
 
 
 class _GatherRows(torch.autograd.Function):
@@ -306,203 +309,16 @@ def gather_rows(x2d, sel):
     return _GatherRows.apply(x2d, sel)
 
 
-class _LinearCrossEntropyStatic(torch.autograd.Function):
-    """_LinearCrossEntropy on a fixed capacity of rows of which the first `count` (a device int32) are labelled and the
-    rest hold zero features and ignore_index labels - the static-rows mode a CUDA graph can capture (mmf_b200.graphs).
-
-    The chunk loop runs over the whole capacity; every vocabulary-sized kernel of a chunk (the GEMM, ce_rows, the dgrad,
-    the wgrad and the bias column sum) takes the chunk's share of `count` as a device bound, so a chunk that starts past
-    `count` costs launches whose CTAs exit at once, and inside a chunk only the rows below `count` rounded up to a
-    128-row tile are computed.  The loss is loss_sum * scale with `scale` = 1 / max(count, 1) in device memory: no host
-    read.  In deterministic mode the row losses are summed over the whole capacity in one fixed-shape sum."""
-
-    @staticmethod
-    def forward(ctx, h, weight, bias, labels, count, scale, ignore_index, chunk_rows):
-        hb, wb = _bf16(h), _bf16(weight)
-        V, K = wb.shape
-        pad = (-V) % 8
-        if pad:
-            wb = torch.nn.functional.pad(wb, (0, 0, 0, pad))
-        bb = _bf16(bias) if bias is not None else torch.zeros(V, dtype=torch.bfloat16, device=wb.device)
-        if pad:
-            bb = torch.cat([bb, torch.full((pad,), -30000.0, dtype=torch.bfloat16, device=bb.device)])
-        M = hb.shape[0]
-        labels = labels.reshape(-1).to(torch.int64).contiguous()
-        need_h, need_w = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        need_b = bias is not None and ctx.needs_input_grad[2]
-        # rows past count are never written by the bounded kernels: their gradients stay the zeros allocated here
-        dh = torch.zeros_like(hb) if need_h else None
-        dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device) if need_w else None
-        db = torch.zeros(wb.shape[0], dtype=torch.float32, device=wb.device) if need_b else None
-        ordered = torch.are_deterministic_algorithms_enabled()
-        loss_sum = torch.zeros((), dtype=torch.float32, device=wb.device)
-        row_loss = torch.zeros(M, dtype=torch.float32, device=wb.device) if ordered else None
-        # the labelled rows of chunk i: clamp(count - i * chunk_rows, 0, chunk_rows), one device int32 per chunk
-        starts = torch.arange(0, M, chunk_rows, dtype=torch.int32, device=wb.device)
-        bounds = (count.reshape(1) - starts).clamp_(0, chunk_rows)
-        for i, r0 in enumerate(range(0, M, chunk_rows)):
-            r1 = min(M, r0 + chunk_rows)
-            nb = bounds[i:i + 1]
-            z = F.gemm(hb[r0:r1], wb, epi=lib.EPI_BIAS, bias=bb, m_bound=nb)
-            F.ce_rows_bounded(z, labels[r0:r1], ignore_index, scale, nb, loss_sum=loss_sum,
-                              row_loss=row_loss[r0:r1] if ordered else None)
-            if need_h:
-                F.gemm(z, wb, b_mn=True, epi=lib.EPI_BIAS, out=dh[r0:r1], m_bound=nb)
-            if need_w:
-                F.gemm(z, hb[r0:r1], a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
-                       splits=best_splits(wb.shape[0], K, r1 - r0), k_bound=nb)
-            if need_b:
-                F.colsum_bounded(z, db, nb)
-        if ordered:
-            loss_sum = row_loss.sum()
-        ctx.save_for_backward(*[t for t in (dh, dw, db) if t is not None])
-        ctx.have = (need_h, need_w, need_b)
-        ctx.V = V
-        ctx.dtypes = (h.dtype, weight.dtype, bias.dtype if bias is not None else None)
-        return loss_sum * scale.reshape(())
-
-    @staticmethod
-    def backward(ctx, g):
-        return _LinearCrossEntropy.backward(ctx, g) + (None, None)
-
-
-def linear_cross_entropy_static(h2d, weight, bias, labels, count, scale, ignore_index=-1, chunk_rows=2048):
-    """linear_cross_entropy over a fixed capacity of rows whose first `count` (int32 [1] on the device) are the labelled
-    ones; `scale` (fp32 [1] on the device) = 1 / max(count, 1).  Rows past count must hold ignore_index labels."""
-    return _LinearCrossEntropyStatic.apply(h2d, weight, bias, labels, count, scale, int(ignore_index), int(chunk_rows))
-
-
-class _LinearT(torch.autograd.Function):
-    """y = x W + b with W stored [K, N]: the GEMM reads the weight MN-major (the layout the dgrad calls use), so a weight
-    that is another layer's nn.Linear weight - MRFR's projection back to the feature space, tied to UNITER's img_linear
-    (heads/mrfr.py:48-49, 86-88) - is consumed as it lies and autograd sums both uses' gradients into the one parameter."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias):
-        xb, wb, bb = _bf16(x), _bf16(weight), _bf16(bias)
-        y = F.gemm(xb, wb, b_mn=True, epi=lib.EPI_BIAS, bias=bb)
-        ctx.save_for_backward(xb, wb)
-        ctx.dtypes = (x.dtype, weight.dtype, bias.dtype)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        xb, wb = ctx.saved_tensors
-        dyb = dy.to(torch.bfloat16).contiguous()
-        dx = dw = db = None
-        if ctx.needs_input_grad[0]:
-            dx = F.gemm(dyb, wb, epi=lib.EPI_BIAS).to(ctx.dtypes[0])              # dy [M, N] @ W[K, N]^T
-        if ctx.needs_input_grad[1]:
-            dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)       # x^T dy: [K, N]
-            F.gemm(xb, dyb, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
-                   splits=best_splits(wb.shape[0], wb.shape[1], xb.shape[0]))
-            dw = dw.to(ctx.dtypes[1])
-        if ctx.needs_input_grad[2]:
-            db = torch.zeros(wb.shape[1], dtype=torch.float32, device=wb.device)
-            F.colsum(dyb, db)
-            db = db.to(ctx.dtypes[2])
-        return dx, dw, db
-
-
-def linear_t(x2d, weight_kn, bias):
-    """F.linear(x, weight_kn.t(), bias): x2d [M, K], weight_kn [K, N] -> bf16 [M, N]; K and N multiples of 8."""
-    return _LinearT.apply(x2d, weight_kn, bias)
-
-
-class _LinearGELULayerNormStatic(torch.autograd.Function):
-    """LayerNorm(gelu(x W^T + b)) - the region heads' transform - on a fixed capacity of rows of which the first `count`
-    (int32 [1] on the device) are live and the rest zero: the GELU GEMM, the LayerNorm and their backward (LayerNorm,
-    GELU', dgrad, weight gradient, bias column sum) are all bounded by the device count, so nothing is read on the host.
-    Output rows past the count are zero."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias, ln_weight, ln_bias, eps, count):
-        xb, wb, bb, g, be = _bf16(x), _bf16(weight), _bf16(bias), _bf16(ln_weight), _bf16(ln_bias)
-        u, h = F.gemm(xb, wb, epi=lib.EPI_BIAS_GELU, bias=bb, m_bound=count)
-        y, mean, rstd = F.layernorm_fwd(h, g, be, eps, m_bound=count)
-        ctx.save_for_backward(xb, wb, u, h, mean, rstd, g, count)
-        ctx.dtypes = (x.dtype, weight.dtype, bias.dtype, ln_weight.dtype, ln_bias.dtype)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        xb, wb, u, h, mean, rstd, g, count = ctx.saved_tensors
-        dg = torch.zeros(g.shape, dtype=torch.float32, device=g.device)
-        dbeta = torch.zeros_like(dg)
-        # rows at and past the count come back zero; u is finite up to the 128-row tile edge, which is as far as the
-        # dgrad reads du (the weight gradient reads it to the 64-row k-block edge)
-        dh, _ = F.layernorm_bwd(dy.to(torch.bfloat16).contiguous(), h, mean, rstd, g, dg, dbeta, m_bound=count)
-        du = F.gelu_bwd(dh, u)
-        dx = F.gemm(du, wb, b_mn=True, epi=lib.EPI_BIAS, m_bound=count)
-        dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)
-        F.gemm(du, xb, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw,
-               splits=best_splits(wb.shape[0], wb.shape[1], xb.shape[0]), k_bound=count)
-        db = torch.zeros(wb.shape[0], dtype=torch.float32, device=wb.device)
-        F.colsum_bounded(du, db, count)
-        t = ctx.dtypes
-        return dx.to(t[0]), dw.to(t[1]), db.to(t[2]), dg.to(t[3]), dbeta.to(t[4]), None, None
-
-
-def linear_gelu_layer_norm_static(x2d, weight, bias, ln_weight, ln_bias, eps, count):
-    """LayerNorm(gelu(x2d W^T + b)) on the rows below `count` (int32 [1] on the device) of a fixed capacity whose later rows
-    are zero; bf16 [M, N], zero past the count"""
-    return _LinearGELULayerNormStatic.apply(x2d, weight, bias, ln_weight, ln_bias, float(eps), count)
-
-
-class _RegionLossStatic(torch.autograd.Function):
-    """The region heads' output projection and loss on a fixed capacity of rows whose first `count` are the masked regions:
-    z = h W^T + b (weight [N, K]) or h W + b (weight_t: W stored [K, N], MRFR's tied image projection, read MN-major), then
-    mmfb_kl_rows_bounded (MRC) or mmfb_mse_rows_bounded (MRFR) against target[tgt_idx[r]], which write d(z) in place; the
-    dgrad, weight gradient and bias column sum run in the forward too, every kernel bounded by the device count.  The loss
-    is the fixed-order sum of the row losses times `scale` (fp32 [1] on the device), so the same bits on every run; the
-    backward multiplies the saved gradients by the incoming scalar.  N need not be a multiple of 8: the weight and bias are
-    zero-padded and the loss kernel zeroes the padding columns' gradient."""
-
-    @staticmethod
-    def forward(ctx, h, weight, bias, target, tgt_idx, count, scale, kind, weight_t):
-        hb, wb, bb = _bf16(h), _bf16(weight), _bf16(bias)
-        K, N = wb.shape if weight_t else wb.shape[::-1]
-        pad = (-N) % 8
-        if pad:
-            if weight_t:
-                raise ValueError("region loss: a transposed weight needs N %% 8 == 0, got %d" % N)
-            wb = torch.nn.functional.pad(wb, (0, 0, 0, pad))
-            bb = torch.nn.functional.pad(bb, (0, pad))
-        M = hb.shape[0]
-        z = F.gemm(hb, wb, b_mn=weight_t, epi=lib.EPI_BIAS, bias=bb, m_bound=count)
-        row_loss = torch.zeros(M, dtype=torch.float32, device=hb.device)
-        if kind == "kl":
-            F.kl_rows_bounded(z, N, target, tgt_idx, count, scale, row_loss)
-        else:
-            F.mse_rows_bounded(z, target, tgt_idx, count, scale, row_loss)
-        dh = F.gemm(z, wb, b_mn=not weight_t, epi=lib.EPI_BIAS, out=torch.zeros_like(hb), m_bound=count)
-        dw = torch.zeros(wb.shape, dtype=torch.float32, device=wb.device)
-        if weight_t:                                  # [K, N] = h^T z
-            F.gemm(hb, z, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw, splits=best_splits(K, N + pad, M),
-                   k_bound=count)
-        else:                                         # [N, K] = z^T h
-            F.gemm(z, hb, a_mn=True, b_mn=True, epi=lib.EPI_ATOMIC_F32, out=dw, splits=best_splits(N + pad, K, M),
-                   k_bound=count)
-        db = torch.zeros(N + pad, dtype=torch.float32, device=wb.device)
-        F.colsum_bounded(z, db, count)
-        ctx.save_for_backward(dh, dw[:N] if not weight_t else dw, db[:N])
-        ctx.dtypes = (h.dtype, weight.dtype, bias.dtype)
-        return row_loss.sum() * scale.reshape(())
-
-    @staticmethod
-    def backward(ctx, g):
-        dh, dw, db = ctx.saved_tensors
-        t = ctx.dtypes
-        return ((dh.float() * g).to(t[0]), (dw * g).to(t[1]), (db * g).to(t[2])) + (None,) * 6
-
-
 def region_loss_static(h2d, weight, bias, target, tgt_idx, count, scale, kind, weight_t=False):
     """kind "kl": scale * sum_r KL(target[tgt_idx[r]] || softmax(h_r W^T + b)); kind "mse": scale * sum_r
     ||h_r W + b - target[tgt_idx[r]]||^2 (weight_t=True, weight [K, N]) - over the rows r below `count` (int32 [1] on the
-    device) of a fixed capacity whose later rows are zero.  target: fp32 [*, N]; tgt_idx: int32, one per row."""
+    device) of a fixed capacity whose later rows are zero, in one chunk (_LinearLoss).  target: fp32 [*, N]; tgt_idx:
+    int32, one per row."""
     if kind not in ("kl", "mse"):
         raise ValueError("region_loss_static: kind must be 'kl' or 'mse', got %r" % (kind,))
-    return _RegionLossStatic.apply(h2d, weight, bias, target, tgt_idx, count, scale, kind, bool(weight_t))
+    if weight_t and weight.shape[1] % 8:
+        raise ValueError("region loss: a transposed weight needs N %% 8 == 0, got %d" % weight.shape[1])
+    return _LinearLoss.apply(h2d, weight, bias, target, tgt_idx, count, scale, kind, None, bool(weight_t), None)
 
 
 class _OptimalTransport(torch.autograd.Function):

@@ -1,5 +1,5 @@
-"""Static-rows masked-LM loss on the CPU, over the kernel test double: the chunk loop of
-ops.linear_cross_entropy_static hands every vocabulary-sized call its chunk's device bound, the head's loss and gradients
+"""Static-rows masked-LM loss on the CPU, over the kernel test double: the chunk loop of ops.linear_cross_entropy with a
+device count hands every vocabulary-sized call its chunk's device bound, the head's loss and gradients
 equal today's gathered path, GraphedStep refuses exactly what it refused without `static_rows` and accepts VinVL and
 ViLT with it, and the C header declares the new entry points.  The kernels themselves run on the H100
 (tests/test_static_rows_gpu.py).  Doubles for the new entry points live here, not in tests/fake_kernels.py."""
@@ -99,7 +99,8 @@ def double(monkeypatch):
     return d
 
 
-@pytest.mark.parametrize("capacity,count", [(5000, 2100), (5000, 0), (300, 300), (4096, 2048)])
+@pytest.mark.parametrize("capacity,count", [(5000, 2100), (5000, 0), (300, 300), (4096, 2048), (4097, 4097),
+                                            (4097, 2048), (2049, 1), (129, 128)])
 def test_chunk_loop_hands_every_vocabulary_call_its_device_bound(double, capacity, count):
     from mmf_b200 import lib, ops
     g = torch.Generator().manual_seed(capacity + count)
@@ -113,7 +114,7 @@ def test_chunk_loop_hands_every_vocabulary_call_its_device_bound(double, capacit
     b = (torch.randn(V, generator=g) * 0.1).requires_grad_(True)
     cnt = torch.tensor([count], dtype=torch.int32)
     scale = torch.tensor([1.0 / max(count, 1)], dtype=torch.float32)
-    loss = ops.linear_cross_entropy_static(h, w, b, labels, cnt, scale, -1, chunk)
+    loss = ops.linear_cross_entropy(h, w, b, labels, -1, chunk, count=cnt, scale=scale)
     chunks = math.ceil(capacity / chunk)
     kinds = [(c[0], c[1]) for c in double.calls]
     per_chunk = [("gemm", lib.EPI_BIAS), ("ce_rows", None), ("gemm", lib.EPI_BIAS), ("gemm", lib.EPI_ATOMIC_F32),

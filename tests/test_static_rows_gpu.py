@@ -200,7 +200,8 @@ def test_bounded_ce_rows_and_colsum(cap):
                     assert torch.equal(out, ref)
 
 
-@pytest.mark.parametrize("cap,c", [(5000, 2100), (5000, 4999), (700, 1), (700, 0)])
+@pytest.mark.parametrize("cap,c", [(5000, 2100), (5000, 4999), (700, 1), (700, 0), (4097, 4097), (4096, 2048),
+                                   (2049, 2049), (300, 129)])
 def test_static_linear_cross_entropy_matches_todays(cap, c):
     from mmf_b200 import ops
     g = torch.Generator().manual_seed(cap + c)
@@ -213,8 +214,8 @@ def test_static_linear_cross_entropy_matches_todays(cap, c):
     labels[:c] = torch.randint(0, V, (c,), generator=g)
     h, labels = hf.to(DEV).to(torch.bfloat16).requires_grad_(True), labels.to(DEV)
     with _deterministic():
-        loss = ops.linear_cross_entropy_static(h, w, b, labels, _bound(c),
-                                               torch.tensor([1.0 / max(c, 1)], dtype=torch.float32, device=DEV))
+        loss = ops.linear_cross_entropy(h, w, b, labels, count=_bound(c),
+                                        scale=torch.tensor([1.0 / max(c, 1)], dtype=torch.float32, device=DEV))
         loss.backward()
         if not c:
             assert loss.item() == 0.0 and not h.grad.any() and not w.grad.any() and not b.grad.any()
