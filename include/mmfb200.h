@@ -46,8 +46,14 @@ enum {
   MMFB_EPI_GELU_BWD = 3,        /* C = acc * gelu_erf'(aux)            dgrad through BertIntermediate */
   MMFB_EPI_ADD_AUX = 4,         /* C = acc + aux                       dgrad + residual gradient     */
   MMFB_EPI_ATOMIC_F32 = 5,      /* C(fp32) += acc                      split-K weight gradient       */
-  MMFB_EPI_BIAS_RELU = 6        /* C = relu(acc + bias)                FinetuneFasterRcnnFpnFc7, encoders.py:176-179 */
+  MMFB_EPI_BIAS_RELU = 6,       /* C = relu(acc + bias)                FinetuneFasterRcnnFpnFc7, encoders.py:176-179 */
+  MMFB_EPI_BIAS_GELU_DROP = 7,  /* C = u = acc + bias ; C2 = keep * scale * gelu_erf(u)   timm Mlp fc1 -> GELU -> Dropout */
+  MMFB_EPI_GELU_DROP_BWD = 8    /* C = acc * keep * scale * gelu_erf'(aux)               its dgrad (aux = u)           */
 };
+/* MMFB_EPI_BIAS_GELU_DROP runs with (a_mn, b_mn) = (0, 0) and MMFB_EPI_GELU_DROP_BWD with (0, 1).  Both read the keep bits
+ * drop_mask (bit n % 32 of word n / 32 of row m keeps element (m, n); mmfb_dropout_bits) and scale kept values by drop_scale:
+ * drop_mask NULL or not 4-byte aligned, ldmask < ceil(N/32), drop_scale not positive and finite, C2 NULL (_GELU_DROP) or aux
+ * NULL (_GELU_DROP_BWD) is MMFB_ERR_ARG before any launch.  Dropped elements of C2 / C are exact zeros. */
 
 /* C[M,N] = epi( A[M,K] * B[N,K]^T ).  a_mn/b_mn = 0: operand stored [rows,K] (K contiguous);
  * = 1: operand stored [K,rows] (rows contiguous), i.e. the transposed view of a row-major tensor. */
@@ -274,6 +280,18 @@ int mmfb_dropout_bits(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t off
  * captured training step draws fresh masks as long as the graph increments *epoch (mmf_b200/graphs.py) */
 int mmfb_dropout_bits_epoch(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t offset, const uint64_t* epoch, float p,
                             mmfb_stream stream);
+/* Keep bits for dropout(p) followed by stochastic depth (timm DropPath(p_path)) on an activation of M rows of H columns,
+ * M = batch * rows_per_sample: out [M, ceil(H/32)] words.  Element (m, n) is kept when its element draw keeps it - the
+ * draws of mmfb_dropout_bits(out, M * ceil(H/32), seed, offset, p) - AND sample m / rows_per_sample is kept, with
+ * probability 1 - p_path from one draw per sample at Philox counter offset + 4 * M * ceil(H/32) + sample (16-bit
+ * resolution), shared by the sample's rows.  Kept values are scaled by 1 / ((1 - p)(1 - p_path)).  The call uses the
+ * counters [offset, offset + 4 * M * ceil(H/32) + batch).  M, H or rows_per_sample <= 0, M % rows_per_sample != 0, p or
+ * p_path outside [0, 1) is MMFB_ERR_ARG. */
+int mmfb_dropout_path_bits(uint32_t* out, int M, int H, int rows_per_sample, uint64_t seed, uint64_t offset, float p,
+                           float p_path, mmfb_stream stream);
+/* the same with the device step counter of mmfb_dropout_bits_epoch mixed into every counter it uses */
+int mmfb_dropout_path_bits_epoch(uint32_t* out, int M, int H, int rows_per_sample, uint64_t seed, uint64_t offset,
+                                 const uint64_t* epoch, float p, float p_path, mmfb_stream stream);
 
 /* Embedding row composer (K1): y[r] = src0[src_row0[r]] + src1[src_row1[r]] + tab0[idx0[r]] + tab1[idx1[r]] +
  * tab2[idx2[r]]; a NULL pointer or a negative index drops the term.  src*: bf16 [*, ldsrc] dense rows (e.g. the

@@ -232,6 +232,20 @@ int mmfb_dropout_bits_epoch(uint32_t* out, int64_t nwords, uint64_t seed, uint64
   MMFB_REQUIRE_DEVICE();
   return dropout_bits(out, nwords, seed, offset, p, epoch, reinterpret_cast<cudaStream_t>(stream));
 }
+int mmfb_dropout_path_bits(uint32_t* out, int M, int H, int rows_per_sample, uint64_t seed, uint64_t offset, float p,
+                           float p_path, mmfb_stream stream) {
+  if (!out) return set_error(MMFB_ERR_ARG, "mmfb_dropout_path_bits: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return dropout_path_bits(out, M, H, rows_per_sample, seed, offset, p, p_path, nullptr,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_dropout_path_bits_epoch(uint32_t* out, int M, int H, int rows_per_sample, uint64_t seed, uint64_t offset,
+                                 const uint64_t* epoch, float p, float p_path, mmfb_stream stream) {
+  if (!out || !epoch) return set_error(MMFB_ERR_ARG, "mmfb_dropout_path_bits_epoch: null pointer");
+  MMFB_REQUIRE_DEVICE();
+  return dropout_path_bits(out, M, H, rows_per_sample, seed, offset, p, p_path, epoch,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
 int mmfb_embed_compose(const mmfb_compose_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_embed_compose: null args");
   MMFB_REQUIRE_DEVICE();

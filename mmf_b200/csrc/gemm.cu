@@ -23,6 +23,7 @@
 // HF BertSelfOutput/BertIntermediate/BertOutput invoked at hf_layers.py:248,289-290,
 // mmf/models/vilbert.py:77-79,127,144-145,396-412,504-509 and their autograd backward
 // (mmf/trainers/core/training_loop.py:211-213).
+#include <float.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -39,21 +40,27 @@ struct GemmDev {
   int M, N, K;
   int splits;
   bf16* c;               // bf16 destination [M, ldc]
-  bf16* c2;              // second bf16 destination (EPI_BIAS_GELU)
+  bf16* c2;              // second bf16 destination (EPI_BIAS_GELU, EPI_BIAS_GELU_DROP)
   float* c32;            // EPI_ATOMIC_F32 destination; EPI_PARTIAL_F32: the workspace [splits, M, N]
   int64_t ldc;
   const bf16* bias;      // [N] or null
   const bf16* aux;       // residual / pre-activation, [M, ldaux], or null; read through the aux tensor map
   const uint32_t* dmask; // dropout keep-bits, [M, ldmask] words (bit n%32 of word n/32), or null
   int64_t ldmask;
-  float dscale;          // 1/(1-p)
+  float dscale;          // 1/(1-p), or whatever scale the caller's keep bits stand for
   const int32_t* m_dev;  // BOUNDED: device row bound (tiles starting at or past min(M, *m_dev) are skipped), or null
   const int32_t* k_dev;  // BOUNDED: device bound on K (only the k-blocks below min(K, *k_dev) are summed), or null
 };
 
 // epilogues that read a per-element bf16 operand (aux): it is loaded by TMA into the output staging boxes
 __host__ __device__ constexpr bool epi_reads_aux(int epi) {
-  return epi == EPI_BIAS_DROP_RESID || epi == EPI_GELU_BWD || epi == EPI_ADD_AUX;
+  return epi == EPI_BIAS_DROP_RESID || epi == EPI_GELU_BWD || epi == EPI_ADD_AUX || epi == EPI_GELU_DROP_BWD;
+}
+// epilogues that write gelu(u) (times the keep bits) as a second output C2
+__host__ __device__ constexpr bool epi_writes_c2(int epi) { return epi == EPI_BIAS_GELU || epi == EPI_BIAS_GELU_DROP; }
+// epilogues that read dropout keep bits
+__host__ __device__ constexpr bool epi_reads_mask(int epi) {
+  return epi == EPI_BIAS_DROP_RESID || epi == EPI_BIAS_GELU_DROP || epi == EPI_GELU_DROP_BWD;
 }
 // epilogues that write fp32 pairs straight from the accumulators (split-K weight gradient)
 __host__ __device__ constexpr bool epi_f32(int epi) { return epi == EPI_ATOMIC_F32 || epi == EPI_PARTIAL_F32; }
@@ -128,7 +135,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (!epi_f32(EPI)) tma_prefetch_desc(&tmC);
-    if (EPI == EPI_BIAS_GELU) tma_prefetch_desc(&tmC2);
+    if (epi_writes_c2(EPI)) tma_prefetch_desc(&tmC2);
     if (has_aux) tma_prefetch_desc(&tmX);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
@@ -269,7 +276,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     // map.  With aux, each box's buffer already holds the chunk's aux box, which the results overwrite in place.
     // Box i goes to buffer i % STG_BOXES, which box i - STG_BOXES used last: before the barrier of box i - 1 the issuer
     // waited until that store had read its source out.  C's box of a chunk is written as it is computed; C2's values
-    // (EPI_BIAS_GELU) wait in registers until C's box has been handed to the TMA unit.
+    // (EPI_BIAS_GELU, EPI_BIAS_GELU_DROP) wait in registers until C's box has been handed to the TMA unit.
     const auto store_box = [&](const CUtensorMap* tm, uint8_t* bx, int c0, int c1) {
       fence_proxy_async();
       if (issuer) tma_store_wait_read<C::STG_BOXES - 2>();   // frees the buffer of the box after this one
@@ -280,17 +287,29 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       }
       ++box;
     };
+    // The hidden-dropout epilogues read the two keep words of a row's 64-column chunk starting at c0 once (a word at or
+    // past N, or of a row past M - mrow null -, keeps everything: those results are clipped); pair jj's two bits then sit
+    // at bit (jj % 4) * 8 + (lane % 4) * 2 of word jj / 4.
+    const auto chunk_keep_words = [&](uint32_t (&kw)[2], const uint32_t* mrow, int c0) {
+      kw[0] = kw[1] = 0xFFFFFFFFu;
+      if (mrow == nullptr) return;
+      kw[0] = __ldg(mrow + (c0 >> 5));
+      if (c0 + 32 < p.N) kw[1] = __ldg(mrow + (c0 >> 5) + 1);
+    };
+    const auto pair_keep = [&](const uint32_t (&kw)[2], int jj) {
+      return kw[jj >> 2] >> ((jj & 3) * 8 + (lane & 3) * 2);       // bit 0: column n, bit 1: column n + 1
+    };
     // SWIZZLE_128B: 16-byte chunk jj of row r sits at chunk jj ^ (r % 8); the 32 lanes of a warp hit 32 banks
     const uint32_t st_row0 = (warp * 16 + (lane >> 2)) * 128 + (lane & 3) * 4;
     // Epilogues that read aux / mask store with a plain C++ store, which the compiler may move below the loads of later
-    // pairs so that their latencies overlap.  EPI_BIAS_GELU reads no per-element operand; there the ordered asm store
-    // keeps the compiler from holding many u and gelu(u) values at once (it would spill).
+    // pairs so that their latencies overlap.  The epilogues with a C2 output keep the ordered asm store: it keeps the
+    // compiler from holding many u and gelu(u) values at once (it would spill).
     const auto pair_at = [&](uint8_t* bx, int rh, int jj) {
       return reinterpret_cast<uint32_t*>(bx + st_row0 + rh * 8 * 128 + ((jj ^ (lane >> 2)) << 4));
     };
     const auto st_pair = [&](uint8_t* bx, int rh, int jj, uint32_t v) {
       uint32_t* dst = pair_at(bx, rh, jj);
-      if (EPI == EPI_BIAS_GELU) asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(dst)), "r"(v) : "memory");
+      if (epi_writes_c2(EPI)) asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(dst)), "r"(v) : "memory");
       else *dst = v;
     };
 #pragma unroll
@@ -307,20 +326,23 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       }
       // every box of a kernel with aux has had exactly one aux load: box / STG_BOXES loads used this buffer before
       if (has_aux) mbar_wait(&auxb[half * C::STG_BOXES + box % C::STG_BOXES], (box / C::STG_BOXES) & 1);
-      uint32_t h[2][8];                          // gelu(u) of EPI_BIAS_GELU
+      uint32_t h[2][8];                          // the C2 values: gelu(u), times keep * scale with EPI_BIAS_GELU_DROP
 #pragma unroll
       for (int rh = 0; rh < 2; ++rh) {
         const int m = w.m0 + half * 64 + warp * 16 + (lane >> 2) + rh * 8;
         const bool row_in = m < p.M;
-        const uint32_t* mrow = (EPI == EPI_BIAS_DROP_RESID && p.dmask != nullptr && row_in)
+        const uint32_t* mrow = (epi_reads_mask(EPI) && p.dmask != nullptr && row_in)
                                    ? p.dmask + static_cast<int64_t>(m) * p.ldmask
                                    : nullptr;
+        uint32_t kw[2];
+        if (EPI == EPI_GELU_DROP_BWD) chunk_keep_words(kw, mrow, w.n0 + cb * 64);
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int j = cb * 8 + jj;
           const int n = w.n0 + j * 8 + (lane & 3) * 2;
           float v0 = acc[j * 4 + rh * 2], v1 = acc[j * 4 + rh * 2 + 1];
-          if (EPI == EPI_BIAS || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_DROP_RESID || EPI == EPI_BIAS_RELU) {
+          if (EPI == EPI_BIAS || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_DROP_RESID || EPI == EPI_BIAS_RELU ||
+              EPI == EPI_BIAS_GELU_DROP) {
             if (p.bias != nullptr && n < p.N) {
               const float2 b = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n)));
               v0 += b.x;
@@ -336,11 +358,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             v0 = (bits & 1u) ? v0 * p.dscale : 0.0f;
             v1 = (bits & 2u) ? v1 * p.dscale : 0.0f;
           }
+          const uint32_t keep = EPI == EPI_GELU_DROP_BWD ? pair_keep(kw, jj) : 3u;
           if (has_aux) {
             const float2 x = unpack_bf16x2(*pair_at(bx, rh, jj));
             if (EPI == EPI_GELU_BWD) {
               v0 *= gelu_erf_grad(x.x);
               v1 *= gelu_erf_grad(x.y);
+            } else if (EPI == EPI_GELU_DROP_BWD) {
+              // the backward of h = keep * scale * gelu(u): acc * keep * scale * gelu'(u)
+              v0 = (keep & 1u) ? v0 * p.dscale * gelu_erf_grad(x.x) : 0.0f;
+              v1 = (keep & 2u) ? v1 * p.dscale * gelu_erf_grad(x.y) : 0.0f;
             } else {
               v0 += x.x;
               v1 += x.y;
@@ -348,15 +375,32 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           }
           st_pair(bx, rh, jj, pack_bf16x2(v0, v1));
           if (EPI == EPI_BIAS_GELU) h[rh][jj] = pack_bf16x2(gelu_erf(v0), gelu_erf(v1));
+          // scaled here, dropped below by clearing the bf16 halves (an exact 0): the keep words are read only once C's box
+          // is out, which keeps the register count within the 168 of three warpgroups (no spill at BN = 256)
+          if (EPI == EPI_BIAS_GELU_DROP) h[rh][jj] = pack_bf16x2(gelu_erf(v0) * p.dscale, gelu_erf(v1) * p.dscale);
         }
       }
       store_box(&tmC, bx, w.n0 + cb * 64, w.m0 + half * 64);
-      if (EPI == EPI_BIAS_GELU) {
+      if (epi_writes_c2(EPI)) {
         bx = stg + (box % C::STG_BOXES) * C::BOX_BYTES;
 #pragma unroll
-        for (int rh = 0; rh < 2; ++rh)
+        for (int rh = 0; rh < 2; ++rh) {
+          uint32_t kw[2];
+          if (EPI == EPI_BIAS_GELU_DROP) {
+            const int m = w.m0 + half * 64 + warp * 16 + (lane >> 2) + rh * 8;
+            chunk_keep_words(kw, (p.dmask != nullptr && m < p.M) ? p.dmask + static_cast<int64_t>(m) * p.ldmask : nullptr,
+                             w.n0 + cb * 64);
+          }
 #pragma unroll
-          for (int jj = 0; jj < 8; ++jj) st_pair(bx, rh, jj, h[rh][jj]);
+          for (int jj = 0; jj < 8; ++jj) {
+            uint32_t v = h[rh][jj];
+            if (EPI == EPI_BIAS_GELU_DROP) {
+              const uint32_t keep = pair_keep(kw, jj);
+              v &= ((keep & 1u) ? 0x0000FFFFu : 0u) | ((keep & 2u) ? 0xFFFF0000u : 0u);
+            }
+            st_pair(bx, rh, jj, v);
+          }
+        }
         store_box(&tmC2, bx, w.n0 + cb * 64, w.m0 + half * 64);
       }
     }
@@ -424,7 +468,17 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream, const int32_t* m
   if (!B_MN) rc = make_tmap_2d(&tmB, a.B, a.K, a.N, a.ldb, 64, BN);
   else rc = make_tmap_2d(&tmB, a.B, a.N, a.K, a.ldb, 64, 64);
   if (rc) return rc;
-  if (EPI == EPI_BIAS_GELU && a.C2 == nullptr) return set_error(MMFB_ERR_ARG, "gemm: this epilogue needs the C2 output");
+  if (epi_writes_c2(EPI) && a.C2 == nullptr) return set_error(MMFB_ERR_ARG, "gemm: this epilogue needs the C2 output");
+  if (EPI == EPI_BIAS_GELU_DROP || EPI == EPI_GELU_DROP_BWD) {
+    // the hidden-dropout epilogues exist for their keep bits: a call without them is a caller's error, not "no dropout"
+    if (a.drop_mask == nullptr || (reinterpret_cast<uintptr_t>(a.drop_mask) & 3) || a.ldmask < (a.N + 31) / 32)
+      return set_error(MMFB_ERR_ARG, "gemm: this epilogue needs 4-byte aligned keep bits with ldmask >= ceil(N/32) = %d "
+                       "(drop_mask=%p ldmask=%lld)", (a.N + 31) / 32, (const void*)a.drop_mask, (long long)a.ldmask);
+    if (!(a.drop_scale > 0.0f && a.drop_scale <= FLT_MAX))
+      return set_error(MMFB_ERR_ARG, "gemm: drop_scale must be positive and finite, got %f", a.drop_scale);
+    if (EPI == EPI_GELU_DROP_BWD && a.aux == nullptr)
+      return set_error(MMFB_ERR_ARG, "gemm: this epilogue needs the pre-activation u as aux");
+  }
   if (((reinterpret_cast<uintptr_t>(a.C) | reinterpret_cast<uintptr_t>(a.C2) | reinterpret_cast<uintptr_t>(a.bias) |
         reinterpret_cast<uintptr_t>(a.aux)) & 3) ||
       (a.aux != nullptr && (a.ldaux % 2)))
@@ -440,7 +494,7 @@ static int launch(const mmfb_gemm_args& a, cudaStream_t stream, const int32_t* m
   memset(&tmC2, 0, sizeof(tmC2));
   memset(&tmX, 0, sizeof(tmX));
   if (!epi_f32(EPI) && (rc = make_tmap_2d(&tmC, a.C, a.N, a.M, a.ldc, 64, 64))) return rc;
-  if (EPI == EPI_BIAS_GELU && (rc = make_tmap_2d(&tmC2, a.C2, a.N, a.M, a.ldc, 64, 64))) return rc;
+  if (epi_writes_c2(EPI) && (rc = make_tmap_2d(&tmC2, a.C2, a.N, a.M, a.ldc, 64, 64))) return rc;
   if (AUX && a.aux != nullptr && (rc = make_tmap_2d(&tmX, a.aux, a.N, a.M, a.ldaux, 64, 64))) return rc;
   GemmDev p;
   p.M = a.M; p.N = a.N; p.K = a.K;
@@ -482,9 +536,11 @@ static int dispatch(const mmfb_gemm_args& a, cudaStream_t s) {
     case 0 + EPI_BIAS_GELU: return launch<BN, false, false, EPI_BIAS_GELU>(a, s);
     case 0 + EPI_BIAS_DROP_RESID: return launch<BN, false, false, EPI_BIAS_DROP_RESID>(a, s);
     case 0 + EPI_BIAS_RELU: return launch<BN, false, false, EPI_BIAS_RELU>(a, s);
+    case 0 + EPI_BIAS_GELU_DROP: return launch<BN, false, false, EPI_BIAS_GELU_DROP>(a, s);
     case 10 + EPI_BIAS: return launch<BN, false, true, EPI_BIAS>(a, s);
     case 10 + EPI_GELU_BWD: return launch<BN, false, true, EPI_GELU_BWD>(a, s);
     case 10 + EPI_ADD_AUX: return launch<BN, false, true, EPI_ADD_AUX>(a, s);
+    case 10 + EPI_GELU_DROP_BWD: return launch<BN, false, true, EPI_GELU_DROP_BWD>(a, s);
     case 110 + EPI_ATOMIC_F32: return launch<BN, true, true, EPI_ATOMIC_F32>(a, s);
     // test-only layout combinations (kept small: plain store epilogue)
     case 100 + EPI_BIAS: return launch<BN, true, false, EPI_BIAS>(a, s);

@@ -16,6 +16,8 @@ enum {
   EPI_ADD_AUX = MMFB_EPI_ADD_AUX,
   EPI_ATOMIC_F32 = MMFB_EPI_ATOMIC_F32,
   EPI_BIAS_RELU = MMFB_EPI_BIAS_RELU,
+  EPI_BIAS_GELU_DROP = MMFB_EPI_BIAS_GELU_DROP,
+  EPI_GELU_DROP_BWD = MMFB_EPI_GELU_DROP_BWD,
   // internal: the ordered split-K weight gradient - unit (tile, split s) stores its fp32 partial into slice s of the
   // caller's workspace [S, M, N] (plain stores), and a second kernel adds the slices into C in split order
   EPI_PARTIAL_F32 = 100
@@ -92,6 +94,8 @@ int ln_bwd(const mmfb_ln_args& a, cudaStream_t s, const int32_t* m_dev = nullptr
 int colsum(const void* X, int64_t ldx, float* out, int M, int N, cudaStream_t s);
 int colsum_ordered(const void* X, int64_t ldx, float* out, int M, int N, float* ws, int64_t ws_bytes, cudaStream_t s);
 int dropout_bits(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t offset, float p, const uint64_t* epoch, cudaStream_t s);
+int dropout_path_bits(uint32_t* out, int M, int H, int rows_per_sample, uint64_t seed, uint64_t offset, float p, float p_path,
+                      const uint64_t* epoch, cudaStream_t s);
 int compose(const mmfb_compose_args& a, cudaStream_t s);
 int scatter(const mmfb_scatter_args& a, cudaStream_t s);
 int cast_params(const float* in, void* out, int64_t n, cudaStream_t s);

@@ -544,6 +544,46 @@ __global__ void dropout_bits_kernel(uint32_t* __restrict__ out, int64_t nwords, 
   out[w] = gt | eq;                                // keep where r >= thresh16
 }
 
+// word w of dropout_bits_kernel at the same (seed, offset), for the stochastic-depth kernel below
+__device__ __forceinline__ uint32_t keep_word(uint64_t seed, uint64_t offset, int64_t w, uint32_t thresh16) {
+  uint32_t gt = 0u, eq = 0xFFFFFFFFu;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const uint4 r = philox4x32(seed, offset + static_cast<uint64_t>(w) * 4 + i);
+    const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int b = 15 - (i * 4 + k);              // plane of bit b, most significant first
+      if ((thresh16 >> b) & 1u) {
+        eq &= rr[k];                               // threshold bit 1: equal so far only where the uniform's bit is 1 too
+      } else {
+        gt |= eq & rr[k];                          // threshold bit 0, uniform bit 1: greater from here on
+        eq &= ~rr[k];
+      }
+    }
+  }
+  return gt | eq;                                  // keep where r >= thresh16
+}
+
+
+// Dropout AND stochastic depth (timm DropPath): word w of row m = w / words is the element keep word of dropout_bits_kernel
+// at the same counter, cleared unless sample m / rows_per_sample survives its own draw - the high 16 bits of the first
+// Philox word at counter offset + 4 * nwords + sample against thresh_path16.  Every thread of a sample repeats that draw,
+// so no thread waits for another.
+__global__ void dropout_path_bits_kernel(uint32_t* __restrict__ out, int64_t nwords, int words, int rows_per_sample,
+                                         uint64_t seed, uint64_t offset, uint32_t thresh16, uint32_t thresh_path16,
+                                         const unsigned long long* __restrict__ epoch) {
+  griddep_launch();
+  griddep_wait();
+  const int64_t w = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (w >= nwords) return;
+  if (epoch != nullptr) offset += static_cast<uint64_t>(*epoch) << 40;
+  const int64_t sample = w / words / rows_per_sample;
+  const uint4 r = philox4x32(seed, offset + static_cast<uint64_t>(nwords) * 4 + static_cast<uint64_t>(sample));
+  const bool sample_kept = (r.x >> 16) >= thresh_path16;
+  out[w] = sample_kept ? keep_word(seed, offset, w, thresh16) : 0u;
+}
+
 // ----------------------------------------------------------------------------------------------
 // embedding compose:  y[r] = src0[s0[r]] + src1[s1[r]] + tab0[i0[r]] + tab1[i1[r]] + tab2[i2[r]]   (absent terms: index < 0)
 // followed by LayerNorm (+dropout) -> x[r]; y (pre-LN) is saved for the backward.
@@ -1130,6 +1170,24 @@ int dropout_bits(uint32_t* out, int64_t nwords, uint64_t seed, uint64_t offset, 
   MMFB_LAUNCH(dropout_bits_kernel, static_cast<unsigned>((nwords + 255) / 256), 256, 0, s, out, nwords, seed, offset, thresh,
               reinterpret_cast<const unsigned long long*>(epoch));
   return launch_ok("dropout_bits");
+}
+
+int dropout_path_bits(uint32_t* out, int M, int H, int rows_per_sample, uint64_t seed, uint64_t offset, float p, float p_path,
+                      const uint64_t* epoch, cudaStream_t s) {
+  if (M <= 0 || H <= 0 || rows_per_sample <= 0 || M % rows_per_sample)
+    return set_error(MMFB_ERR_ARG, "dropout_path_bits: bad shape M=%d H=%d rows_per_sample=%d (M must be a multiple of it)",
+                     M, H, rows_per_sample);
+  if (!(p >= 0.0f && p < 1.0f) || !(p_path >= 0.0f && p_path < 1.0f))
+    return set_error(MMFB_ERR_ARG, "dropout_path_bits: p and p_path must be in [0,1), got %f, %f", p, p_path);
+  const auto thresh = [](float q) {
+    const uint32_t t = static_cast<uint32_t>(q * 65536.0f + 0.5f);
+    return t > 65535u ? 65535u : t;
+  };
+  const int words = (H + 31) / 32;
+  const int64_t nwords = static_cast<int64_t>(M) * words;
+  MMFB_LAUNCH(dropout_path_bits_kernel, static_cast<unsigned>((nwords + 255) / 256), 256, 0, s, out, nwords, words,
+              rows_per_sample, seed, offset, thresh(p), thresh(p_path), reinterpret_cast<const unsigned long long*>(epoch));
+  return launch_ok("dropout_path_bits");
 }
 
 int compose(const mmfb_compose_args& a, cudaStream_t s) {

@@ -4,6 +4,7 @@
   B200IdentityEncoder           <->  IdentityEncoder            mmf/modules/encoders.py:183-198
   B200TransformerEncoder        <->  TransformerEncoder         mmf/modules/encoders.py:513-585   BertModelJit wrapper
   B200ViTImageEncoder           <->  ViTEncoder                 mmf/modules/encoders.py:830-857   ViTModel wrapper (`vit`)
+  B200AlbefVitEncoder           <->  AlbefVitEncoder            mmf/models/albef/vit.py:21-42     VisionTransformer wrapper
 
 The reference builds these through `build_encoder({type, params})` (mmf/utils/build.py:517-546); here the classes are
 registered with `registry.register_encoder(name)` in the shim and take the same config keys.
@@ -188,6 +189,33 @@ class B200ViTImageEncoder(nn.Module):
     def forward(self, *args, output_hidden_states=False, **kwargs):
         out = self.module(*args, output_hidden_states=output_hidden_states, **kwargs)
         return out[0], (out[2] if output_hidden_states else None)
+
+
+# AlbefVitEncoder.Config (mmf/models/albef/vit.py:23-27); the VisionTransformer's keys sit under `params`
+ALBEF_VIT_ENCODER_DEFAULTS = dict(name="albef_vit_encoder", pretrained=False, out_dim=768)
+
+
+@registry.register_encoder("albef_vit_encoder")
+class B200AlbefVitEncoder(nn.Module):
+    """AlbefVitEncoder (mmf/models/albef/vit.py:21-42): `.vit` a VisionTransformer on the fused pre-LN trunk
+    (mmf_b200.albef_vit) built from `config.params` (img_size, patch_size, in_chans, embed_dim, depth, num_heads, mlp_ratio,
+    qkv_bias, drop_rate, attn_drop_rate, drop_path_rate; the reference's defaults).  `pretrained: true` loads the state
+    dict at `pretrained_path` into `.vit` and puts it in eval mode, as the reference does."""
+
+    def __init__(self, config, *args, **kwargs):
+        super().__init__()
+        from .albef_vit import B200AlbefVisionTransformer
+        self.config = _get(config, "params", None) or {}
+        pretrained = _get(config, "pretrained", ALBEF_VIT_ENCODER_DEFAULTS["pretrained"])
+        pretrained_path = _get(config, "pretrained_path", None)
+        self.vit = B200AlbefVisionTransformer(self.config)
+        if pretrained:
+            state_dict = torch.load(pretrained_path, map_location="cpu")
+            self.vit.load_state_dict(state_dict)
+            self.vit.eval()
+
+    def forward(self, x):
+        return self.vit(x)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -72,7 +72,7 @@ def gemm(a, b, *, a_mn=False, b_mn=False, epi=lib.EPI_BIAS, bias=None, aux=None,
     """C[M,N] = epi(A[M,K] @ B[N,K]^T) on the wgmma GEMM.
 
     a: [M,K] (a_mn=False) or [K,M] (a_mn=True); b: [N,K] (b_mn=False) or [K,N] (b_mn=True); bf16.
-    Returns C (and C2 for EPI_BIAS_GELU).  For EPI_ATOMIC_F32 `out` (fp32 [M,N]) is accumulated into; in deterministic
+    Returns C (and C2 for EPI_BIAS_GELU and EPI_BIAS_GELU_DROP).  For EPI_ATOMIC_F32 `out` (fp32 [M,N]) is accumulated into; in deterministic
     mode with splits > 1 the split partials go through a workspace and are added in split order.
     m_bound / k_bound: int32 [1] CUDA tensors bounding M / K on the device (include/mmfb200.h, "Device bounds"); only the
     row tiles below the rounded M bound are written, so `out` past it keeps what it held.
@@ -95,7 +95,7 @@ def gemm(a, b, *, a_mn=False, b_mn=False, epi=lib.EPI_BIAS, bias=None, aux=None,
         if out is None:
             out = torch.empty(M, N, dtype=torch.bfloat16, device=a.device)
         _req(out, torch.bfloat16, "out")
-        if epi == lib.EPI_BIAS_GELU and out2 is None:
+        if epi in (lib.EPI_BIAS_GELU, lib.EPI_BIAS_GELU_DROP) and out2 is None:
             out2 = torch.empty(M, N, dtype=torch.bfloat16, device=a.device)
     args = GemmArgs()
     args.A, args.lda, args.a_mn = a.data_ptr(), a.stride(0), int(a_mn)
@@ -121,7 +121,7 @@ def gemm(a, b, *, a_mn=False, b_mn=False, epi=lib.EPI_BIAS, bias=None, aux=None,
                                     _stream_ptr()))
     else:
         check(LIB.mmfb_gemm(ctypes.byref(args), _stream_ptr()))
-    if epi == lib.EPI_BIAS_GELU:
+    if epi in (lib.EPI_BIAS_GELU, lib.EPI_BIAS_GELU_DROP):
         return out, out2
     return out
 
@@ -555,6 +555,21 @@ def dropout_bits(shape_rows, ncols, p, seed, offset, device):
     else:
         check(LIB.mmfb_dropout_bits_epoch(out.data_ptr(), out.numel(), int(seed) & (2 ** 64 - 1), int(offset),
                                           epoch.data_ptr(), float(p), _stream_ptr()))
+    return out
+
+
+def dropout_path_bits(batch, rows_per_sample, ncols, p, p_path, seed, offset, device):
+    """int32 keep-bit words [batch * rows_per_sample, ceil(ncols/32)] for nn.Dropout(p) followed by timm's DropPath(p_path)
+    over the batch's samples: the draws of dropout_bits at (seed, offset), with every row of a dropped sample cleared.  Kept
+    values scale by 1 / ((1 - p)(1 - p_path)).  Uses the Philox counters [offset, offset + 4 * words + batch)."""
+    M = int(batch) * int(rows_per_sample)
+    out = torch.empty(M, (ncols + 31) // 32, dtype=torch.int32, device=device)
+    epoch = dropout_epoch(out.device)
+    args = (out.data_ptr(), M, int(ncols), int(rows_per_sample), int(seed) & (2 ** 64 - 1), int(offset))
+    if epoch is None:
+        check(LIB.mmfb_dropout_path_bits(*args, float(p), float(p_path), _stream_ptr()))
+    else:
+        check(LIB.mmfb_dropout_path_bits_epoch(*args, epoch.data_ptr(), float(p), float(p_path), _stream_ptr()))
     return out
 
 

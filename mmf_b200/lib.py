@@ -19,6 +19,8 @@ EPI_GELU_BWD = 3
 EPI_ADD_AUX = 4
 EPI_ATOMIC_F32 = 5
 EPI_BIAS_RELU = 6
+EPI_BIAS_GELU_DROP = 7
+EPI_GELU_DROP_BWD = 8
 
 
 class GemmArgs(ctypes.Structure):
@@ -203,6 +205,11 @@ def _load():
                                       ctypes.c_float, ctypes.c_void_p]
     lib.mmfb_dropout_bits_epoch.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_void_p,
                                             ctypes.c_float, ctypes.c_void_p]
+    lib.mmfb_dropout_path_bits.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_uint64,
+                                           ctypes.c_uint64, ctypes.c_float, ctypes.c_float, ctypes.c_void_p]
+    lib.mmfb_dropout_path_bits_epoch.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_uint64,
+                                                 ctypes.c_uint64, ctypes.c_void_p, ctypes.c_float, ctypes.c_float,
+                                                 ctypes.c_void_p]
     lib.mmfb_embed_scatter_sorted.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
                                               ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     lib.mmfb_gelu_bwd.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]

@@ -119,9 +119,9 @@ class EncoderRunner(_LayerStack):
         hiddens = []
         extra = {} if probs is None else {"probs": probs}
         for m, w in zip(self.layers, self.weights):
-            pa, ph = self.W.dropout_p(m) if training else (0.0, 0.0)
+            ps = [p if training else 0.0 for p in self.W.dropout_p(m)]
             hiddens.append(h)
-            h, s = self.W.fwd(h, add_mask, w, B, S, pa, ph, ds, **extra)
+            h, s = self.W.fwd(h, add_mask, w, B, S, *ps, ds, **extra)
             saved.append(s if need_grad else None)
         return h, saved, hiddens
 
