@@ -43,6 +43,7 @@ _LAZY = {
     "build_model": ("models", "build_model"),
     "load_model_config": ("models", "load_model_config"),
     "GraphedStep": ("graphs", "GraphedStep"),
+    "GraphedForward": ("graphs", "GraphedForward"),
 }
 
 

@@ -30,6 +30,9 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
     not change the parameters or the optimizer state;
   * host draws: a model that draws its task on the host in every forward (UNITER) is captured by GraphedTaskSteps, one
     graph per task, with the draws made on the host before each replay;
+  * evaluation: GraphedForward(model.eval(), batch) captures the eval forward `model(batch)` under torch.no_grad() -
+    scores and losses, for M4C and the M4C captioner every greedy decoding step - and returns the captured output,
+    overwritten by the next call.  It refuses what GraphedStep refuses, and a model in training mode;
 The reference has no counterpart (its trainer launches eagerly, mmf/trainers/core/training_loop.py:185-213); this is the
 answer to SURVEY.md 8a's "at T = R = 36 everything is launch-bound"."""
 import contextlib
@@ -106,12 +109,7 @@ class GraphedStep:
         optimizer.step().  Each call stages the groups' current hyper-parameters, then replays; afterwards `.grad` holds
         the step's unclipped gradients, as after an eager step."""
         _check_optimizer("GraphedStep", optimizer, max_grad_norm)
-        _check_runners("GraphedStep", model, static_rows)
-        for m in model.modules():
-            if getattr(m, "graph_capturable", True) is False and not (static_rows and getattr(m, "static_rows_capturable",
-                                                                                           False)):
-                reason = getattr(m, "graph_refusal", "does work on the host in every forward")
-                raise RuntimeError("GraphedStep: %s %s, so its step cannot be captured" % (type(m).__name__, reason))
+        _check_capturable("GraphedStep", model, static_rows)
         self.model, self.loss_fn = model, loss_fn
         self.optimizer, self.max_grad_norm = optimizer, max_grad_norm
         with _static_rows_context() if static_rows else contextlib.nullcontext():
@@ -186,6 +184,17 @@ def _check_optimizer(who, optimizer, max_grad_norm):
                          "construct it as mmf_b200.optim.B200AdamW(..., capturable=True)" % who)
 
 
+def _check_capturable(who, model, static_rows):
+    """the refusals GraphedStep and GraphedForward share: skip-padding encoders that read token counts on the host, and
+    modules that declare `graph_capturable = False` (unless static_rows covers their only refusal)"""
+    _check_runners(who, model, static_rows)
+    for m in model.modules():
+        if getattr(m, "graph_capturable", True) is False and not (static_rows and getattr(m, "static_rows_capturable",
+                                                                                       False)):
+            reason = getattr(m, "graph_refusal", "does work on the host in every forward")
+            raise RuntimeError("%s: %s %s, so its step cannot be captured" % (who, type(m).__name__, reason))
+
+
 def _check_runners(who, model, static_rows):
     """the encoders' skip-padding modes that read token counts on the host, and so cannot be captured"""
     runners = [m.__dict__.get("_runner") for m in model.modules()]
@@ -201,6 +210,87 @@ def _check_runners(who, model, static_rows):
                            "counts on the host%s and cannot be captured; turn them off with "
                            "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)"
                            % (who, " even under static_rows" if static_rows else ""))
+
+
+class GraphedForward:
+    """An evaluation forward replayed as one CUDA graph:
+
+        fwd = GraphedForward(model.eval(), example_batch)     # warm-up, then capture of model(batch) under no_grad
+        out = fwd(batch)                                      # copies `batch` into the static inputs, replays the graph
+
+    The graph records `model(static_batch)` - for a registered model BaseModel.__call__, so `scores` and, when the batch
+    carries targets, `losses` are in it - as an eager `model.eval()` forward under torch.no_grad() launches it.  M4C and
+    the M4C captioner run all their greedy decoding steps in that forward (a fixed trip count, nothing read on the host),
+    so the whole decode is one graph.
+
+    The returned output is the captured structure of static tensors: every call overwrites it, so it is valid until the
+    next call; clone what must outlive it.  `example_batch` is a (nested dict / SampleList / list of) CUDA tensors with the
+    shapes of every later batch; its mapping types are kept, so a SampleList stays one.  Non-tensor values (dataset
+    names) are fixed at capture.  As for GraphedStep, the batch must carry every input the forward would otherwise build
+    from a host value.  Every forward gets fresh containers over the static tensors, so a forward that replaces keys of
+    its sample list (MMBT's token shift, VisualBERT's masks) does not replace the static inputs.  As for GraphedStep,
+    the reductions are those torch.use_deterministic_algorithms selected at capture: the static-rows masked-LM loss adds
+    its row losses with atomics unless captured under the flag.
+
+    The model must be in eval mode: nothing is drawn, and the dropout step counter of GraphedStep is neither created nor
+    advanced.  Refused before any warm-up, as GraphedStep refuses them: skip-padding encoders without static_rows,
+    pack_tail and pack_streams encoders, and modules that declare `graph_capturable = False` (UNITER, whose forward draws
+    its task on the host; VinVL and ViLT pretraining without static_rows).  Also refused: a model that returns attention
+    probabilities or hidden states (output_attentions / output_hidden_states / visualization), and a model or batch off
+    the GPU.
+
+    static_rows=True: warm-up and capture run inside static_rows(), so pretraining validation losses (the masked-LM
+    heads select their rows on the device, and return no MLM logits) and single-stream skip-padding encoders (packed at a
+    fixed capacity of every row of the batch) are captured."""
+
+    def __init__(self, model, example_batch, warmup=3, static_rows=False):
+        if model.training:
+            raise ValueError("GraphedForward: the model is in training mode; capture an evaluation forward after "
+                             "model.eval(), and a training step with GraphedStep")
+        _check_capturable("GraphedForward", model, static_rows)
+        for m in model.modules():
+            if getattr(m, "output_attentions", False) or getattr(m, "output_hidden_states", False) or \
+                    getattr(getattr(m, "config", None), "visualization", False) is True:
+                raise RuntimeError("GraphedForward: %s returns attention probabilities or hidden states, which are not "
+                                   "captured; turn off output_attentions / output_hidden_states / visualization"
+                                   % type(m).__name__)
+        off = sorted({str(t.device) for t in list(model.parameters()) + list(_flatten(example_batch))
+                      if not t.is_cuda})
+        if off or not any(True for _ in _flatten(example_batch)):
+            raise RuntimeError("GraphedForward: the model and every tensor of the batch must be on a CUDA device (found "
+                               "%s); a CUDA graph replays device work only" % (", ".join(off) or "no tensor in the batch"))
+        self.model = model
+        with _static_rows_context() if static_rows else contextlib.nullcontext():
+            self._capture(model, example_batch, warmup)
+
+    def _capture(self, model, example_batch, warmup):
+        self.static = _map_keep(lambda t: t.detach().clone(), example_batch)
+        dev = next(t for t in _flatten(self.static) if t.is_cuda).device
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.no_grad(), torch.cuda.stream(side):
+            for _ in range(max(1, warmup)):              # lazy engine state, kernel attributes, library work buffers
+                model(_map_keep(lambda t: t, self.static))
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.no_grad(), torch.cuda.graph(self.graph, stream=side):
+            self.output = model(_map_keep(lambda t: t, self.static))
+
+    def __call__(self, batch=None):
+        if batch is not None:
+            _copy_into(self.static, batch)
+        self.graph.replay()
+        return self.output
+
+
+def _map_keep(fn, x):
+    """_map that keeps each container's type (the models read a SampleList's fields as attributes)"""
+    if isinstance(x, dict):
+        return type(x)((k, _map_keep(fn, v)) for k, v in x.items())
+    if isinstance(x, (list, tuple)):
+        return type(x)(_map_keep(fn, v) for v in x)
+    return fn(x) if torch.is_tensor(x) else x
 
 
 class GraphedTaskSteps:
