@@ -10,9 +10,11 @@ import kernel_check as kc
 
 pytestmark = pytest.mark.gpu
 
-EPI_NAMES = {0: "bias", 1: "bias_gelu", 2: "bias_drop_resid", 3: "gelu_bwd", 4: "add_aux", 5: "atomic_f32", 6: "bias_relu"}
+EPI_NAMES = {0: "bias", 1: "bias_gelu", 2: "bias_drop_resid", 3: "gelu_bwd", 4: "add_aux", 5: "atomic_f32", 6: "bias_relu",
+             7: "bias_gelu_drop", 8: "gelu_drop_bwd"}
 # every (a_mn, b_mn, epi) that dispatch() accepts
-COMBOS = [(0, 0, 0), (0, 0, 1), (0, 0, 2), (0, 0, 6), (0, 1, 0), (0, 1, 3), (0, 1, 4), (1, 1, 5), (1, 0, 0), (1, 1, 0)]
+COMBOS = [(0, 0, 0), (0, 0, 1), (0, 0, 2), (0, 0, 6), (0, 1, 0), (0, 1, 3), (0, 1, 4), (1, 1, 5), (1, 0, 0), (1, 1, 0),
+          (0, 0, 7), (0, 1, 8)]
 # curated (M, N, K) lists: every M, N and K of the sweep appears, not their product
 M_ANY = [1, 8, 63, 64, 65, 127, 129, 1000]
 M_MN = [8, 64, 72, 120, 136, 1000, 8, 256]                # MN-major A needs M % 8 == 0
@@ -48,29 +50,40 @@ def _effective_splits(splits, K):
     return s
 
 
-def run_and_check(a_mn, b_mn, epi, M, N, K, bn, seed, with_bias=True, with_aux=True, splits=1):
-    """one launch through functional.gemm and the per-element check of each output; returns the worst |err|/bound"""
+def run_and_check(a_mn, b_mn, epi, M, N, K, bn, seed, with_bias=True, with_aux=True, splits=1, guard=None):
+    """one launch through functional.gemm and the per-element check of each output; returns the worst |err|/bound.
+    guard (tests/test_poison_guard_gpu.py): places every operand inside a poisoned allocation (guard.inp) and every
+    output inside a sentinel-filled one (guard.out), to be checked by the caller afterwards"""
     from mmf_b200 import functional as F, lib
     g = _gen(seed)
     a_st, a = _operand(M, K, a_mn, g)
     b_st, b = _operand(N, K, b_mn, g)
     acc, absab = kc.gemm_ref(a, b)
-    bias = _bf16(N, g=g) if with_bias and epi in (0, 1, 2, 6) else None
-    aux = _bf16(M, N, g=g, scale=1.0) if with_aux and epi in (2, 3, 4) else None
+    bias = _bf16(N, g=g) if with_bias and epi in (0, 1, 2, 6, 7) else None
+    aux = _bf16(M, N, g=g, scale=1.0) if (with_aux or epi == 8) and epi in (2, 3, 4, 8) else None
     bias64 = bias.double() if bias is not None else torch.zeros(N, dtype=torch.float64, device="cuda")
     aux64 = aux.double() if aux is not None else None
     words, keep, dsc = None, None, 1.0
-    if epi == 2:
-        wpr = (N + 31) // 32 + 3                                          # ldmask > ceil(N/32)
+    if epi in (2, 7, 8):
+        wpr = (N + 31) // 32 + (3 if epi == 2 else 0)                     # ldmask > ceil(N/32) for epi 2
         words = torch.randint(-2 ** 31, 2 ** 31, (M, wpr), generator=g, device="cuda", dtype=torch.int64).to(torch.int32)
         keep = F.unpack_keep_bits(words, N).double()
         dsc = 1.0 / 0.9
+    out = out2 = None
+    if guard is not None:
+        a_st, b_st = guard.inp(a_st), guard.inp(b_st)
+        bias = guard.inp(bias) if bias is not None else None
+        aux = guard.inp(aux) if aux is not None else None
+        words = guard.inp(words, fill=-1) if words is not None else None
+        if epi != 5:
+            out = guard.out((M, N), torch.bfloat16)
+            out2 = guard.out((M, N), torch.bfloat16) if epi in (1, 7) else None
     lay = kc.gemm_layout(bn, _effective_splits(splits, K) if epi == 5 else 1)
     tag = "a_mn=%d b_mn=%d epi=%s M=%d N=%d K=%d bn=%d" % (a_mn, b_mn, EPI_NAMES[epi], M, N, K, bn)
     worst = 0.0
     if epi == 5:
         c0 = torch.randn(M, N, generator=g, device="cuda")
-        out = c0.clone()
+        out = c0.clone() if guard is None else guard.out((M, N), torch.float32, init=c0)
         F.gemm(a_st, b_st, a_mn=True, b_mn=True, epi=epi, out=out, splits=splits, block_n=bn)
         ref = c0.double() + acc
         s_eff = _effective_splits(splits, K)
@@ -78,7 +91,7 @@ def run_and_check(a_mn, b_mn, epi, M, N, K, bn, seed, with_bias=True, with_aux=T
         bound = kc.gemm_bound(ref, absab, c0.double().abs(), bf16_out=False) + kc.U_F32 * s_eff * (absab + ref.abs())
         return kc.assert_within(out, ref, bound, lay, tag)
     res = F.gemm(a_st, b_st, a_mn=bool(a_mn), b_mn=bool(b_mn), epi=epi, bias=bias, aux=aux, drop_mask=words,
-                 drop_scale=dsc, block_n=bn)
+                 drop_scale=dsc, block_n=bn, out=out, out2=out2)
     if epi in (0, 6):
         ref = acc + bias64
         bound = kc.gemm_bound(ref, absab, bias64.abs())
@@ -113,6 +126,26 @@ def run_and_check(a_mn, b_mn, epi, M, N, K, bn, seed, with_bias=True, with_aux=T
     elif epi == 4:
         ref = acc + (aux64 if aux64 is not None else 0.0)
         worst = kc.assert_within(res, ref, kc.gemm_bound(ref, absab, aux64.abs() if aux64 is not None else 0.0), lay, tag)
+    elif epi == 7:
+        # the bounds of tests/test_albef_vit_kernels_gpu.py::test_bias_gelu_drop_vs_fp64
+        u, h = res
+        uref = acc + bias64
+        worst = kc.assert_within(u, uref, kc.gemm_bound(uref, absab, bias64.abs()), lay, tag + " (u)")
+        kept = keep.bool()
+        href = torch.where(kept, kc.gelu64(uref) * dsc, torch.zeros_like(uref))
+        hb = kc.U_BF16 * href.abs() + dsc * (kc.gelu_grad64(uref).abs() * kc.U_ACC * (absab + bias64.abs())
+                                             + 2.0 ** -22 * uref.abs() + kc.U_F32 * href.abs())
+        worst = max(worst, kc.assert_within(h, href, torch.where(kept, hb, torch.zeros_like(hb)), lay, tag + " (h)"))
+        assert torch.equal(h[~kept], torch.zeros_like(h[~kept])), tag
+    elif epi == 8:
+        # the bound of tests/test_albef_vit_kernels_gpu.py::test_gelu_drop_bwd_vs_fp64
+        kept = keep.bool()
+        gg = kc.gelu_grad64(aux64)
+        ref = torch.where(kept, acc * dsc * gg, torch.zeros_like(acc))
+        bound = kc.U_BF16 * ref.abs() + dsc * (gg.abs() * kc.U_ACC * absab + acc.abs() * 2.0 ** -21 * (1 + aux64.abs())
+                                               + 2 * kc.U_F32 * (acc * gg).abs())
+        worst = kc.assert_within(res, ref, torch.where(kept, bound, torch.zeros_like(bound)), lay, tag)
+        assert torch.equal(res[~kept], torch.zeros_like(res[~kept])), tag
     return worst
 
 
