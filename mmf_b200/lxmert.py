@@ -52,11 +52,18 @@ class B200VisualFeatEncoder(nn.Module):
         return self.dropout(x).view(B, R, H)
 
 
+def _layer_norm_eps(config):
+    """the eps of HF's BertAttention / BertOutput / BertSelfOutput, which every LXMERT layer is built from
+    (lxmert.py:69-80, 233-248, 305-311): config.layer_norm_eps.  Only the visual feature encoder and the answer head
+    fix 1e-12."""
+    return float(getattr(config, "layer_norm_eps", 1e-12))
+
+
 class _CrossAtt(_Holder):
-    def __init__(self, hidden, heads, p_attn, p_hidden):
+    def __init__(self, hidden, heads, p_attn, p_hidden, eps):
         super().__init__()
         self.att = B200BertSelfAttention(hidden, heads, p_attn)
-        self.output = B200BertSelfOutput(hidden, hidden, p_hidden, 1e-12)
+        self.output = B200BertSelfOutput(hidden, hidden, p_hidden, eps)
 
 
 class B200LXMERTXLayer(_Holder):
@@ -64,13 +71,14 @@ class B200LXMERTXLayer(_Holder):
         super().__init__()
         h, nh, it = config.hidden_size, config.num_attention_heads, config.intermediate_size
         pa, ph = float(config.attention_probs_dropout_prob), float(config.hidden_dropout_prob)
-        self.visual_attention = _CrossAtt(h, nh, pa, ph)
-        self.lang_self_att = B200BertAttention(h, nh, pa, ph, 1e-12)
-        self.visn_self_att = B200BertAttention(h, nh, pa, ph, 1e-12)
+        eps = _layer_norm_eps(config)
+        self.visual_attention = _CrossAtt(h, nh, pa, ph, eps)
+        self.lang_self_att = B200BertAttention(h, nh, pa, ph, eps)
+        self.visn_self_att = B200BertAttention(h, nh, pa, ph, eps)
         self.lang_inter = B200BertIntermediate(h, it)
-        self.lang_output = B200BertSelfOutput(it, h, ph, 1e-12)
+        self.lang_output = B200BertSelfOutput(it, h, ph, eps)
         self.visn_inter = B200BertIntermediate(h, it)
-        self.visn_output = B200BertSelfOutput(it, h, ph, 1e-12)
+        self.visn_output = B200BertSelfOutput(it, h, ph, eps)
 
 
 class B200LXMERTEncoder(nn.Module):
@@ -83,7 +91,8 @@ class B200LXMERTEncoder(nn.Module):
         self.visn_fc = B200VisualFeatEncoder(config)
         self.num_l_layers, self.num_x_layers, self.num_r_layers = config.l_layers, config.x_layers, config.r_layers
         mk = lambda: B200BertLayer(config.hidden_size, config.num_attention_heads, config.intermediate_size,
-                                   float(config.attention_probs_dropout_prob), float(config.hidden_dropout_prob), 1e-12)
+                                   float(config.attention_probs_dropout_prob), float(config.hidden_dropout_prob),
+                                   _layer_norm_eps(config))
         self.layer = nn.ModuleList([mk() for _ in range(self.num_l_layers)])
         self.x_layers = nn.ModuleList([B200LXMERTXLayer(config) for _ in range(self.num_x_layers)])
         self.r_layers = nn.ModuleList([mk() for _ in range(self.num_r_layers)])

@@ -653,7 +653,10 @@ class B200ConnectionLayer(_Holder):
         self.v_intermediate = B200BertIntermediate(cfg.v_hidden_size, cfg.v_intermediate_size)
         self.v_output = B200BertSelfOutput(cfg.v_intermediate_size, cfg.v_hidden_size, cfg.v_hidden_dropout_prob, 1e-12)
         self.t_intermediate = B200BertIntermediate(cfg.hidden_size, cfg.intermediate_size)
-        self.t_output = B200BertSelfOutput(cfg.intermediate_size, cfg.hidden_size, cfg.hidden_dropout_prob, 1e-12)
+        # the text side is HF's BertOutput (config.layer_norm_eps); the image side and biOutput fix 1e-12
+        # (vilbert.py:303, 483-490, 520-526)
+        self.t_output = B200BertSelfOutput(cfg.intermediate_size, cfg.hidden_size, cfg.hidden_dropout_prob,
+                                           float(getattr(cfg, "layer_norm_eps", 1e-12)))
 
 
 def vilbert_schedule(v_ids, t_ids, n_t, n_v):
@@ -686,9 +689,12 @@ class B200ViLBertEncoder(nn.Module):
         self.config = config
         self.v_biattention_id = list(config.v_biattention_id)
         self.t_biattention_id = list(config.t_biattention_id)
+        # text layers: vilbert.BertLayer over HF's BertSelfOutput / BertOutput (config.layer_norm_eps); image layers:
+        # BertImageSelfOutput / BertImageOutput, which fix 1e-12 (vilbert.py:131-170, 254, 303)
         self.layer = nn.ModuleList([
             B200BertLayer(config.hidden_size, config.num_attention_heads, config.intermediate_size,
-                          float(config.attention_probs_dropout_prob), float(config.hidden_dropout_prob), 1e-12)
+                          float(config.attention_probs_dropout_prob), float(config.hidden_dropout_prob),
+                          float(getattr(config, "layer_norm_eps", 1e-12)))
             for _ in range(config.num_hidden_layers)])
         self.v_layer = nn.ModuleList([
             B200BertLayer(config.v_hidden_size, config.v_num_attention_heads, config.v_intermediate_size,

@@ -79,9 +79,10 @@ def _drop(t, site):
     return torch.where(keep.to(t.device), t * scale, torch.zeros_like(t))
 
 
-def vit_ref(images, sd, cfg, keeps=None, pos=None, dtype=torch.float64):
+def vit_ref(images, sd, cfg, keeps=None, pos=None, dtype=torch.float64, eps=1e-6):
     """VisionTransformer.forward in `dtype`.  sd: the reference's parameter names (no `vit.` prefix), tensors that may
-    require grad; keeps: per block the dict of Draws.blocks, or None (eval); pos: (keep, scale) of pos_drop, or None."""
+    require grad; keeps: per block the dict of Draws.blocks, or None (eval); pos: (keep, scale) of pos_drop, or None;
+    eps: of every LayerNorm (the reference's 1e-6; another value only to show that a test can tell them apart)."""
     p = {k: v.to(dtype) for k, v in sd.items()}
     patch = cfg.get("patch_size", 16)
     H, heads = cfg["embed_dim"], cfg["num_heads"]
@@ -94,14 +95,14 @@ def vit_ref(images, sd, cfg, keeps=None, pos=None, dtype=torch.float64):
     for i in range(cfg["depth"]):
         k = keeps[i] if keeps is not None else {}
         pre = "blocks.%d." % i
-        a = TF.layer_norm(x, (H,), p[pre + "norm1.weight"], p[pre + "norm1.bias"], 1e-6)
+        a = TF.layer_norm(x, (H,), p[pre + "norm1.weight"], p[pre + "norm1.bias"], eps)
         qkv = TF.linear(a, p[pre + "attn.qkv.weight"], p.get(pre + "attn.qkv.bias"))
         q, kk, v = qkv.reshape(B, S, 3, heads, d).permute(2, 0, 3, 1, 4)
         att = torch.softmax(q @ kk.transpose(-2, -1) / math.sqrt(d), dim=-1)
         att = _drop(att, k.get("attn"))
         ctx = (att @ v).transpose(1, 2).reshape(B, S, H)
         x = x + _drop(TF.linear(ctx, p[pre + "attn.proj.weight"], p[pre + "attn.proj.bias"]), k.get("proj"))
-        b = TF.layer_norm(x, (H,), p[pre + "norm2.weight"], p[pre + "norm2.bias"], 1e-6)
+        b = TF.layer_norm(x, (H,), p[pre + "norm2.weight"], p[pre + "norm2.bias"], eps)
         g = _drop(TF.gelu(TF.linear(b, p[pre + "mlp.fc1.weight"], p[pre + "mlp.fc1.bias"])), k.get("mlp"))
         x = x + _drop(TF.linear(g, p[pre + "mlp.fc2.weight"], p[pre + "mlp.fc2.bias"]), k.get("fc2"))
-    return TF.layer_norm(x, (H,), p["norm.weight"], p["norm.bias"], 1e-6)
+    return TF.layer_norm(x, (H,), p["norm.weight"], p["norm.bias"], eps)

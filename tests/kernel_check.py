@@ -36,6 +36,10 @@ U_F32 = 2.0 ** -24      # fp32 round-to-nearest
 # operands those errors add up like a random walk, so 16 steps' worth of worst-case rounding (2^-20 of sum |a||b|)
 # covers sqrt(K/16) <= 16, i.e. K <= 4096, with room to spare
 U_ACC = 2.0 ** -20
+# ex2.approx.ftz returns 0 for results below fp32's normal range: every probability the attention kernels compute carries,
+# besides its relative error, an absolute error of at most 2^-126 (a p of 2^-150 is stored as 0).  Rows whose max lies
+# more than 126 log2 units above other keys (one-hot rows of trained models) are where this term is the whole error.
+U_FTZ = 2.0 ** -126
 LOG2E = 1.0 / math.log(2.0)
 LN2 = math.log(2.0)
 
@@ -277,6 +281,8 @@ def attention_ref(q, k, v, B, heads, Sq, Skv, mask=None, keep=None, p_drop=0.0, 
     # fp32 O = sum_j p_j v_j / l:  P packed to bf16 before the PV product (2^-8 P|V|), its fp32 accumulation (2^-20 P|V|),
     # p errors r_j in the numerator ((P r)|V|) and in the normaliser l ((P r) 1 |O|)
     b_O = ((0.0 if p_exact else U_BF16) + U_ACC) * PaV + (Pd * r_f) @ aV + (P * r_f).sum(-1, keepdim=True) * O.abs()
+    # + the flush of p below 2^-126 (U_FTZ per key, in the numerator and in l)
+    b_O = b_O + U_FTZ * (Kp @ aV + Skv * O.abs())
     res = {"ctx": _merge(O), "lse2": lse2.squeeze(-1),
            "b_ctx": _merge(b_O + U_BF16 * O.abs()),                                # + bf16 output rounding
            "b_lo": _merge(b_O + 2.0 ** -16 * O.abs())}                             # ctx + ctx_lo: hi + lo of the fp32 O
@@ -299,6 +305,8 @@ def attention_ref(q, k, v, B, heads, Sq, Skv, mask=None, keep=None, p_drop=0.0, 
     e_delta = (adO * b_Oused).sum(-1, keepdim=True) + U_ACC * (adO * O.abs()).sum(-1, keepdim=True)
     # dS = p (dPd - delta): dP accumulated in fp32 (2^-20 |dO||V|^T), delta error, p error; dS is then packed to bf16
     e_dS = P * (U_ACC * Kp * (adO @ aV.transpose(-1, -2)) + e_delta) + P * r_b * (dPd - delta).abs()
+    # the recomputed p flushed below 2^-126 (U_FTZ |dPd - delta|), and the bf16 dS operand below the normal range (U_FTZ)
+    e_dS = e_dS + U_FTZ * ((dPd - delta).abs() + 1.0)
     adS = dS.abs()
     w_dS = e_dS + (U_BF16 + U_ACC) * adS                                           # error of the bf16 dS operand
     sc = 1.0 / math.sqrt(d)
@@ -308,8 +316,9 @@ def attention_ref(q, k, v, B, heads, Sq, Skv, mask=None, keep=None, p_drop=0.0, 
     res["dq"], res["dk"], res["dv"] = _merge(dQ), _merge(dK), _merge(dV)
     res["b_dq"] = _merge(sc * (w_dS @ K.abs()) + U_BF16 * dQ.abs())
     res["b_dk"] = _merge(sc * (w_dS.transpose(-1, -2) @ Q.abs()) + U_BF16 * dK.abs())
-    # dV = (P keep dscale)^T dO with P packed to bf16 and recomputed with error r_b
-    res["b_dv"] = _merge(((U_BF16 + U_ACC) * Pd + Pd * r_b).transpose(-1, -2) @ adO + U_BF16 * dV.abs())
+    # dV = (P keep dscale)^T dO with P packed to bf16 and recomputed with error r_b (+ its flush below 2^-126, twice: the
+    # fp32 p and the bf16 operand)
+    res["b_dv"] = _merge(((U_BF16 + U_ACC) * Pd + Pd * r_b + 2 * U_FTZ * Kp).transpose(-1, -2) @ adO + U_BF16 * dV.abs())
     return res
 
 

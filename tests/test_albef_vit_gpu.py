@@ -6,6 +6,9 @@
     restatement's own error, at that element or as its row's rms) + 8 bf16 ulps + 3e-2 x rms(fp64 row), so one misrouted
     mask row or sample
     shows, and per tensor in relative L2 within 1.5 x the bf16 restatement's + 2e-3;
+  * the same step with the position table and patch bias zeroed and two samples' images scaled down, so that their rows
+    enter the first block with a variance of about eps / 10 (eps = 1e-6), per tensor in relative L2; LayerNorm's eps is
+    observable there: the fp64 restatement with eps = 1e-12 misses those samples' image gradient by more than 5x;
   * every sample a DropPath draw drops leaves its residual input unchanged, bit for bit;
   * one step under GraphedStep equals the eager step bit for bit under torch.use_deterministic_algorithms(True), and two
     replays draw different DropPath samples."""
@@ -73,6 +76,22 @@ def _close(what, got, ref64, ref16):
         what, int(bad.sum()), i, got.reshape(-1)[i].item(), ref64.reshape(-1)[i].item(), bound.reshape(-1)[i].item())
 
 
+QUIET = (1, 5)          # samples whose patch rows enter the first LayerNorm with a variance of about eps / 10 = 1e-7
+
+
+def _quiet(vit, images, samples, std=5.8e-4):
+    """zeroes pos_embed and the patch projection's bias and scales the images of `samples` to N(0, std^2): their patch
+    rows reach the first block's norm1 with a variance of about 768 x 0.02^2 x std^2 ~ 1e-7, with no cancellation behind
+    them (so bf16 holds them to its relative precision).  The [CLS] token stays: an all-zero row would hide pos_drop's
+    keep bits from the test, which reads them off the rows that pos_drop zeroed."""
+    with torch.no_grad():
+        for t in (vit.pos_embed, vit.patch_embed.proj.bias):
+            t.zero_()
+        images = images.clone()
+        images[list(samples)] = torch.randn_like(images[list(samples)]) * std
+    return images
+
+
 def test_training_step_vs_fp64_with_the_kernels_keep_bits(monkeypatch):
     torch.manual_seed(21)
     enc = _encoder(TRAIN_CFG).train()
@@ -106,6 +125,50 @@ def test_training_step_vs_fp64_with_the_kernels_keep_bits(monkeypatch):
     assert rel(images.grad, dx64) <= 1.5 * rel(dx16, dx64) + 2e-3
     for n, p in enc.vit.named_parameters():
         assert rel(p.grad, g64[n]) <= 1.5 * rel(g16[n], g64[n]) + 2e-3 or g64[n].norm() < 1e-6, n
+
+
+def test_training_step_with_rows_at_the_layernorm_eps(monkeypatch):
+    """the training step of the test above with pos_embed and the patch bias zeroed and two samples' images scaled down
+    (_quiet): their rows enter the first block with a variance of about eps / 10, where LayerNorm's eps = 1e-6 matters.
+    Output, image gradient and every parameter gradient against fp64 in relative L2 (within 1.5 x the bf16
+    restatement's + 2e-3); the fp64 restatement with eps = 1e-12 must miss the quiet samples' image gradient by more
+    than 5x that bound"""
+    torch.manual_seed(21)
+    enc = _encoder(TRAIN_CFG).train()
+    draws = AV.Draws().install(monkeypatch)
+    pos = {}
+    enc.vit.pos_drop.register_forward_hook(lambda m, i, o: pos.update(x=i[0].detach(), y=o.detach()))
+    B, S = 8, 197
+    images = _quiet(enc.vit, torch.randn(B, 3, 224, 224, device=DEV), QUIET).requires_grad_(True)
+    out = enc(images)
+    w = torch.randn_like(out)
+    (out * w).sum().backward()
+    torch.cuda.synchronize()
+    keeps = draws.blocks(TRAIN_CFG, B, S)
+    pos_keep = ((pos["y"] != 0) | (pos["x"] == 0), 1.0 / (1.0 - TRAIN_CFG["drop_rate"]))
+    var = pos["x"].double().var(-1, unbiased=False)                                 # [B, S]: the rows norm1 reads
+    quiet = var[list(QUIET), 1:]
+    assert bool((quiet > 2e-8).all() and (quiet < 1e-6).all()), (quiet.min().item(), quiet.max().item())
+    res = {}
+    for dt, eps in ((torch.float64, 1e-6), (torch.bfloat16, 1e-6), (torch.float64, 1e-12)):
+        sd = {k: v.detach().to(torch.bfloat16).to(dt).requires_grad_(True) for k, v in enc.vit.state_dict().items()}
+        x = images.detach().to(torch.bfloat16).to(dt).requires_grad_(True)
+        ref = AV.vit_ref(x, sd, TRAIN_CFG, keeps, pos_keep, dtype=dt, eps=eps)
+        (ref * w.to(dt)).sum().backward()
+        res[dt, eps] = (ref, x.grad, {k: v.grad for k, v in sd.items()})
+    (r64, dx64, g64), (r16, dx16, g16) = res[torch.float64, 1e-6], res[torch.bfloat16, 1e-6]
+    assert rel(out, r64) <= 1.5 * rel(r16, r64) + 2e-3
+    assert rel(images.grad, dx64) <= 1.5 * rel(dx16, dx64) + 2e-3
+    for n, p in enc.vit.named_parameters():
+        assert rel(p.grad, g64[n]) <= 1.5 * rel(g16[n], g64[n]) + 2e-3 or g64[n].norm() < 1e-6, n
+    # eps shows in the gradient of the quiet samples' images: norm1's backward scales it by rstd = 1 / sqrt(var + eps)
+    # (in the forward, the later LayerNorms normalise the scale of the first block's branch away)
+    q = list(QUIET)
+    # the quiet samples on their own (their gradients are far larger than the others' and would carry the whole tensor)
+    assert rel(images.grad[q], dx64[q]) <= 1.5 * rel(dx16[q], dx64[q]) + 2e-3
+    miss = rel(images.grad[q], res[torch.float64, 1e-12][1][q]) / (1.5 * rel(dx16[q], dx64[q]) + 2e-3)
+    print("albef quiet rows: d images misses fp64 with eps = 1e-12 by %.1f x the bound" % miss)
+    assert miss >= 5.0, "d images is as close to LayerNorms with eps = 1e-12 as to eps = 1e-6: %.2f x the bound" % miss
 
 
 def test_dropped_samples_pass_their_residual_bit_for_bit(monkeypatch):

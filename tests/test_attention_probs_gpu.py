@@ -3,12 +3,13 @@
 Kernel, element by element against fp64 (tests/kernel_check.py): P[b,h,q,k] = 2^(z - lse2) (* keep * dscale), computed
 from the z the kernel stages (fp32 q.k accumulation, fmaf with the clamped mask) and the lse2 the forward saved.  Its
 per-element bound (probs_ref below) is the backward's recomputed-p bound of kernel_check.attention_ref:
-    |P - P64| <= Kp P ln2 (E + e_lse)  +  u_out Kp P
+    |P - P64| <= Kp P ln2 (E + e_lse)  +  u_out Kp P  +  2^-126 Kp
 E: exponent error of the staged score (fmaf and mask product 2^-23 (|z| + |m|), fp32 accumulation 2^-20 scale2 |q||k|,
 ex2.approx 2^-22); e_lse: error of the forward's lse2 (kernel_check's b_lse2); u_out: output rounding, 2^-24 (fp32) or
-2^-8 (bf16).  Sweeps sequence edges, far-from-square cross shapes, odd head counts, mask kinds and keep bits, with output
-buffers prefilled with NaN between guard regions.  Then consistency with the forward (row sums, P V against ctx + ctx_lo of
-the same call) and the encoders at full size against the fp32 oracle."""
+2^-8 (bf16); 2^-126: the flush of p below fp32's normal range.  Sweeps sequence edges, far-from-square cross shapes, odd
+head counts, mask kinds and keep bits, with output buffers prefilled with NaN between guard regions.  Then consistency
+with the forward (row sums, P V against ctx + ctx_lo of the same call) and the encoders at full size against the fp32
+oracle."""
 import math
 
 import pytest
@@ -55,7 +56,8 @@ def probs_ref(q, k, B, heads, Sq, Skv, mask=None, keep=None, p_drop=0.0, out_dty
     e_lse = (P * E).sum(-1, keepdim=True) + E_max + 1.5 * (Skv / 4 + 2) * kc.U_F32 + 2.0 ** -20 + 2.0 ** -23 * lse2.abs()
     u_out = kc.U_F32 if out_dtype == torch.float32 else kc.U_BF16
     Pd = P * Kp
-    bound = Pd * kc.LN2 * (E + e_lse) + u_out * Pd
+    # + kc.U_FTZ: ex2.approx.ftz stores a p below 2^-126 as 0
+    bound = Pd * kc.LN2 * (E + e_lse) + u_out * Pd + kc.U_FTZ * Kp
     return Pd, bound, P, kc.LN2 * (E + e_lse) + u_out
 
 
