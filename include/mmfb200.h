@@ -424,7 +424,11 @@ int mmfb_cast_f32_bf16(const float* in, void* out, int64_t n, mmfb_stream stream
  * runs (the clip coefficient mmfb_grad_norm writes), so a clipped step needs no device-to-host read.
  * When hp_dev is set, group g's lr / weight_decay / step_size / bc2_sqrt and beta1 / beta2 / eps are read from the
  * DEVICE table entry hp_dev[g] (written by mmfb_adamw_hparams) and the corresponding launch fields are ignored, so the
- * launch can be captured in a CUDA graph and replayed at later steps and learning rates. */
+ * launch can be captured in a CUDA graph and replayed at later steps and learning rates.
+ * Loss scaling (torch.amp.GradScaler), both nullable: when found_inf is set and *found_inf is non-zero, the launch writes
+ * nothing (param, param_bf16, exp_avg, exp_avg_sq keep their bits).  When loss_scale_dev is set, every gradient is first
+ * multiplied by inv = (float)(1.0 / (double)*loss_scale_dev) - GradScaler.unscale_'s factor - and then by the factor
+ * above, as a second fp32 multiply: the bits of unscale_ followed by a step, for any scale. */
 #define MMFB_ADAMW_MAX_GROUPS 8
 typedef struct {
   float lr, weight_decay, step_size, bc2_sqrt;
@@ -445,8 +449,10 @@ typedef struct {
   float bc2_sqrt[MMFB_ADAMW_MAX_GROUPS];
   float beta1, beta2, eps, grad_scale;
   int mode;
+  const float* loss_scale_dev;   /* nullable: DEVICE fp32 loss scale S; gradients are multiplied by 1/S first */
+  const float* found_inf;        /* nullable: DEVICE fp32; non-zero makes the launch a no-op */
   const float* grad_scale_dev;   /* nullable: DEVICE fp32 factor applied on top of grad_scale */
-  const mmfb_adamw_hp* hp_dev;   /* nullable: DEVICE [n_groups] hyper-parameters replacing the launch fields */
+  const mmfb_adamw_hp* hp_dev;   /* nullable: DEVICE [n_groups] hyper-parameters replacing the launch fields (last) */
 } mmfb_adamw_args;
 int mmfb_adamw(const mmfb_adamw_args* args, mmfb_stream stream);
 
@@ -457,7 +463,9 @@ int mmfb_adamw(const mmfb_adamw_args* args, mmfb_stream stream);
  *   mode 1: step_size = lr / (1 - b1^t);  bc2_sqrt = sqrt(1 - b2^t)
  * hp[s] = {lr, weight_decay, step_size, bc2_sqrt, b1, b2, eps}.  A frozen slot (pack parameters the optimizer does not
  * own) keeps its step and gets lr = weight_decay = step_size = 0, bc2_sqrt = 1.  `groups` is the table the host stages
- * before each step (the values a learning-rate scheduler writes); `slots`, `step` and `hp` stay put. */
+ * before each step (the values a learning-rate scheduler writes); `slots`, `step` and `hp` stay put.
+ * found_inf (nullable, DEVICE fp32): when *found_inf is non-zero the launch writes nothing - no step count advances, as a
+ * step that GradScaler skips does not count in torch's fused Adam. */
 #define MMFB_ADAMW_SLOT_CORRECT_BIAS 1
 #define MMFB_ADAMW_SLOT_FROZEN 2
 typedef struct {
@@ -474,6 +482,7 @@ typedef struct {
   mmfb_adamw_hp* hp;                   /* DEVICE [n_slots] */
   int n_slots;
   int mode;                            /* 0 transformers, 1 torch (as mmfb_adamw) */
+  const float* found_inf;              /* nullable: DEVICE fp32; non-zero makes the launch a no-op */
 } mmfb_adamw_hparams_args;
 int mmfb_adamw_hparams(const mmfb_adamw_hparams_args* args, mmfb_stream stream);
 
@@ -484,7 +493,7 @@ int mmfb_adamw_hparams(const mmfb_adamw_hparams_args* args, mmfb_stream stream);
  * they never are together (every element is then accessed singly).  The segment owns the CTAs [first_block,
  * first_block + ceil((n + lead) / MMFB_ADAMW_SEGMENT_BLOCK)), lead = (8 - head) % 8 for head > 0 and 0 otherwise;
  * first_block is the running sum over the segments before it and n_blocks the total.  Gradients are multiplied by
- * grad_scale (times *grad_scale_dev when set) first. */
+ * grad_scale (times *grad_scale_dev when set) first; loss_scale_dev and found_inf act as in mmfb_adamw. */
 #define MMFB_ADAMW_SEGMENT_BLOCK 2048
 typedef struct {
   float* param;
@@ -505,6 +514,8 @@ typedef struct {
   float grad_scale;
   int mode;
   const float* grad_scale_dev;         /* nullable */
+  const float* loss_scale_dev;         /* nullable: DEVICE fp32 loss scale, as in mmfb_adamw */
+  const float* found_inf;              /* nullable: DEVICE fp32 skip flag, as in mmfb_adamw */
 } mmfb_adamw_segments_args;
 int mmfb_adamw_segments(const mmfb_adamw_segments_args* args, mmfb_stream stream);
 
@@ -519,7 +530,9 @@ int mmfb_adamw_segments(const mmfb_adamw_segments_args* args, mmfb_stream stream
  * partials[b]; the second launch adds the partials in a fixed order: no atomics, and the result depends only on the
  * segment lengths and dtypes, so repeated calls give the same bits in every mode.  The fp32 norm is within one fp32 ulp of
  * the exact norm.  Non-finite gradients give an inf / NaN norm, as torch's with error_if_nonfinite=False.
- * norm_type must be 2 (MMFB_ERR_ARG otherwise). */
+ * norm_type must be 2 (MMFB_ERR_ARG otherwise).  max_norm_scale_dev (nullable, DEVICE fp32 S) makes the threshold
+ * max_norm * S, one fp32 multiply when the kernel runs: the clip of loss-scaled gradients at max_norm times the loss
+ * scale, without reading S on the host. */
 #define MMFB_GRAD_NORM_BLOCK 16384
 #define MMFB_GRAD_F32 0
 #define MMFB_GRAD_BF16 1
@@ -537,6 +550,7 @@ typedef struct {
   float* out;                          /* DEVICE fp32 [2] */
   float max_norm;
   float norm_type;
+  const float* max_norm_scale_dev;     /* nullable: DEVICE fp32 factor on max_norm */
 } mmfb_grad_norm_args;
 int mmfb_grad_norm(const mmfb_grad_norm_args* args, mmfb_stream stream);
 

@@ -336,18 +336,26 @@ int mmfb_dropout_apply(const void* x, int64_t ldx, const uint32_t* bits, int64_t
   MMFB_REQUIRE_DEVICE();
   return dropout_apply(x, ldx, bits, ldm, scale, out, ldo, M, H, reinterpret_cast<cudaStream_t>(stream));
 }
+// the loss-scaling fields of the optimizer launches: nullable DEVICE fp32 scalars
+static bool misaligned_f32(const float* p) { return (reinterpret_cast<uintptr_t>(p) & 3) != 0; }
+
 int mmfb_adamw(const mmfb_adamw_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_adamw: null args");
+  if (misaligned_f32(args->loss_scale_dev) || misaligned_f32(args->found_inf))
+    return set_error(MMFB_ERR_ARG, "mmfb_adamw: loss_scale_dev and found_inf must be 4-byte aligned");
   MMFB_REQUIRE_DEVICE();
   return adamw(*args, reinterpret_cast<cudaStream_t>(stream));
 }
 int mmfb_adamw_hparams(const mmfb_adamw_hparams_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_adamw_hparams: null args");
+  if (misaligned_f32(args->found_inf)) return set_error(MMFB_ERR_ARG, "mmfb_adamw_hparams: found_inf must be 4-byte aligned");
   MMFB_REQUIRE_DEVICE();
   return adamw_hparams(*args, reinterpret_cast<cudaStream_t>(stream));
 }
 int mmfb_adamw_segments(const mmfb_adamw_segments_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_adamw_segments: null args");
+  if (misaligned_f32(args->loss_scale_dev) || misaligned_f32(args->found_inf))
+    return set_error(MMFB_ERR_ARG, "mmfb_adamw_segments: loss_scale_dev and found_inf must be 4-byte aligned");
   MMFB_REQUIRE_DEVICE();
   return adamw_segments(*args, reinterpret_cast<cudaStream_t>(stream));
 }
@@ -355,6 +363,8 @@ int mmfb_grad_norm(const mmfb_grad_norm_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_grad_norm: null args");
   if (args->norm_type != 2.0f)
     return set_error(MMFB_ERR_ARG, "mmfb_grad_norm: only norm_type 2 is supported (got %g)", args->norm_type);
+  if (misaligned_f32(args->max_norm_scale_dev))
+    return set_error(MMFB_ERR_ARG, "mmfb_grad_norm: max_norm_scale_dev must be 4-byte aligned");
   MMFB_REQUIRE_DEVICE();
   return grad_norm(*args, reinterpret_cast<cudaStream_t>(stream));
 }

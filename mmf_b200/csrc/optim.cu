@@ -13,7 +13,17 @@ struct AdamWDev {
   float b1, b2, eps, gscale;
   const float* gscale_dev;   // read only by the SCALE_DEV instantiations (a device-side clipping coefficient)
   const mmfb_adamw_hp* hp;   // read only by the HP_DEV instantiations (mmfb_adamw_hparams' table)
+  const float* loss_scale_dev;   // read only by the AMP instantiations (nullable there too)
+  const float* found_inf;        // read only by the AMP instantiations (nullable there too)
 };
+
+// GradScaler's unscale factor of a loss scale S: (float)(1.0 / (double)S), as torch's _scale.double().reciprocal().float().
+__device__ __forceinline__ float amp_inv_scale(const float* s) {
+  return __double2float_rn(__ddiv_rn(1.0, static_cast<double>(*s)));
+}
+
+// A non-zero found_inf (GradScaler's flag of non-finite gradients) makes the whole update a no-op.
+__device__ __forceinline__ bool amp_skip(const float* found_inf) { return found_inf != nullptr && *found_inf != 0.0f; }
 
 // One element of the AdamW step, shared by adamw_kernel and adamw_segments_kernel so that both give the same bits.
 // gr = g * gs is the scaled gradient; step = step_size, bc2s = bc2_sqrt.
@@ -39,12 +49,15 @@ __device__ __forceinline__ void adamw_elem(float& p, float& m, float& v, float g
 
 // SCALE_DEV: the gradient factor is gscale * *gscale_dev, read once per thread after the previous kernel has completed.
 // HP_DEV: the group's hyper-parameters come from the device table a.hp instead of the launch parameters.
-// The instantiations without either are the kernels this file always had.
-template <int MODE, bool SCALE_DEV, bool HP_DEV>
+// AMP: loss scaling on the device - nothing is written when *found_inf is non-zero, and every gradient is first multiplied
+// by amp_inv_scale(loss_scale_dev) (each pointer nullable), then by the factor above: GradScaler.unscale_, then step().
+// The instantiations without any of the three are the kernels this file always had.
+template <int MODE, bool SCALE_DEV, bool HP_DEV, bool AMP>
 __global__ void __launch_bounds__(256)
 adamw_kernel(const __grid_constant__ AdamWDev a) {
   griddep_launch();
   griddep_wait();
+  if (AMP && amp_skip(a.found_inf)) return;
   const int64_t blk = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;     // 8-element block
   const int64_t i = blk * 8;
   if (i >= a.n) return;
@@ -68,6 +81,11 @@ adamw_kernel(const __grid_constant__ AdamWDev a) {
     g[4 * h] = tg.x; g[4 * h + 1] = tg.y; g[4 * h + 2] = tg.z; g[4 * h + 3] = tg.w;
     m[4 * h] = tm.x; m[4 * h + 1] = tm.y; m[4 * h + 2] = tm.z; m[4 * h + 3] = tm.w;
     v[4 * h] = tv.x; v[4 * h + 1] = tv.y; v[4 * h + 2] = tv.z; v[4 * h + 3] = tv.w;
+  }
+  if (AMP && a.loss_scale_dev != nullptr) {
+    const float inv = amp_inv_scale(a.loss_scale_dev);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) g[e] = g[e] * inv;
   }
 #pragma unroll
   for (int e = 0; e < 8; ++e) adamw_elem<MODE>(p[e], m[e], v[e], g[e], gs, lr, wd, step, bc2s, b1, b2, eps);
@@ -104,18 +122,28 @@ int adamw(const mmfb_adamw_args& a, cudaStream_t s) {
   }
   d.b1 = a.beta1; d.b2 = a.beta2; d.eps = a.eps; d.gscale = a.grad_scale; d.gscale_dev = a.grad_scale_dev;
   d.hp = a.hp_dev;
+  d.loss_scale_dev = a.loss_scale_dev; d.found_inf = a.found_inf;
   const int64_t blocks8 = a.n / 8;
   const unsigned grid = static_cast<unsigned>((blocks8 + 255) / 256);
-  const int variant = a.mode * 4 + (a.grad_scale_dev != nullptr ? 2 : 0) + (a.hp_dev != nullptr ? 1 : 0);
+  const bool amp = a.loss_scale_dev != nullptr || a.found_inf != nullptr;
+  const int variant = (amp ? 8 : 0) + a.mode * 4 + (a.grad_scale_dev != nullptr ? 2 : 0) + (a.hp_dev != nullptr ? 1 : 0);
   switch (variant) {
-    case 0: MMFB_LAUNCH((adamw_kernel<0, false, false>), grid, 256, 0, s, d); break;
-    case 1: MMFB_LAUNCH((adamw_kernel<0, false, true>), grid, 256, 0, s, d); break;
-    case 2: MMFB_LAUNCH((adamw_kernel<0, true, false>), grid, 256, 0, s, d); break;
-    case 3: MMFB_LAUNCH((adamw_kernel<0, true, true>), grid, 256, 0, s, d); break;
-    case 4: MMFB_LAUNCH((adamw_kernel<1, false, false>), grid, 256, 0, s, d); break;
-    case 5: MMFB_LAUNCH((adamw_kernel<1, false, true>), grid, 256, 0, s, d); break;
-    case 6: MMFB_LAUNCH((adamw_kernel<1, true, false>), grid, 256, 0, s, d); break;
-    default: MMFB_LAUNCH((adamw_kernel<1, true, true>), grid, 256, 0, s, d); break;
+    case 0: MMFB_LAUNCH((adamw_kernel<0, false, false, false>), grid, 256, 0, s, d); break;
+    case 1: MMFB_LAUNCH((adamw_kernel<0, false, true, false>), grid, 256, 0, s, d); break;
+    case 2: MMFB_LAUNCH((adamw_kernel<0, true, false, false>), grid, 256, 0, s, d); break;
+    case 3: MMFB_LAUNCH((adamw_kernel<0, true, true, false>), grid, 256, 0, s, d); break;
+    case 4: MMFB_LAUNCH((adamw_kernel<1, false, false, false>), grid, 256, 0, s, d); break;
+    case 5: MMFB_LAUNCH((adamw_kernel<1, false, true, false>), grid, 256, 0, s, d); break;
+    case 6: MMFB_LAUNCH((adamw_kernel<1, true, false, false>), grid, 256, 0, s, d); break;
+    case 7: MMFB_LAUNCH((adamw_kernel<1, true, true, false>), grid, 256, 0, s, d); break;
+    case 8: MMFB_LAUNCH((adamw_kernel<0, false, false, true>), grid, 256, 0, s, d); break;
+    case 9: MMFB_LAUNCH((adamw_kernel<0, false, true, true>), grid, 256, 0, s, d); break;
+    case 10: MMFB_LAUNCH((adamw_kernel<0, true, false, true>), grid, 256, 0, s, d); break;
+    case 11: MMFB_LAUNCH((adamw_kernel<0, true, true, true>), grid, 256, 0, s, d); break;
+    case 12: MMFB_LAUNCH((adamw_kernel<1, false, false, true>), grid, 256, 0, s, d); break;
+    case 13: MMFB_LAUNCH((adamw_kernel<1, false, true, true>), grid, 256, 0, s, d); break;
+    case 14: MMFB_LAUNCH((adamw_kernel<1, true, false, true>), grid, 256, 0, s, d); break;
+    default: MMFB_LAUNCH((adamw_kernel<1, true, true, true>), grid, 256, 0, s, d); break;
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw launch: %s", cudaGetErrorString(e));
@@ -127,13 +155,18 @@ int adamw(const mmfb_adamw_args& a, cudaStream_t s) {
 // Device-side hyper-parameters (include/mmfb200.h: mmfb_adamw_hparams): one CTA, one slot per thread and pass.  fp64
 // operation by operation as the host's B200AdamW._group_hp evaluates it (Python float ** int is C pow), rounded once.
 // ---------------------------------------------------------------------------------------------------------------------
+// SKIP: a non-zero *found_inf makes the launch a no-op (no step count advances, the table keeps its values), as a
+// step that GradScaler skips does not count in torch's fused Adam.
 constexpr int HP_THREADS = 256;
 
+template <bool SKIP>
 __global__ void __launch_bounds__(HP_THREADS)
 adamw_hparams_kernel(const mmfb_adamw_group_hp* __restrict__ groups, const mmfb_adamw_slot* __restrict__ slots,
-                     int64_t* __restrict__ steps, mmfb_adamw_hp* __restrict__ out, int n_slots, int mode) {
+                     int64_t* __restrict__ steps, mmfb_adamw_hp* __restrict__ out, int n_slots, int mode,
+                     const float* __restrict__ found_inf) {
   griddep_launch();
   griddep_wait();
+  if (SKIP && *found_inf != 0.0f) return;
   for (int s = threadIdx.x; s < n_slots; s += HP_THREADS) {
     const mmfb_adamw_slot sl = slots[s];
     const mmfb_adamw_group_hp g = groups[sl.group];
@@ -170,7 +203,12 @@ int adamw_hparams(const mmfb_adamw_hparams_args& a, cudaStream_t s) {
   if ((reinterpret_cast<uintptr_t>(a.groups) | reinterpret_cast<uintptr_t>(a.step)) & 7 ||
       reinterpret_cast<uintptr_t>(a.slots) & 7 || reinterpret_cast<uintptr_t>(a.hp) & 15)
     return set_error(MMFB_ERR_ARG, "adamw_hparams: groups / slots / step must be 8-byte aligned, hp 16-byte aligned");
-  MMFB_LAUNCH(adamw_hparams_kernel, 1, HP_THREADS, 0, s, a.groups, a.slots, a.step, a.hp, a.n_slots, a.mode);
+  if (a.found_inf != nullptr)
+    MMFB_LAUNCH(adamw_hparams_kernel<true>, 1, HP_THREADS, 0, s, a.groups, a.slots, a.step, a.hp, a.n_slots, a.mode,
+                a.found_inf);
+  else
+    MMFB_LAUNCH(adamw_hparams_kernel<false>, 1, HP_THREADS, 0, s, a.groups, a.slots, a.step, a.hp, a.n_slots, a.mode,
+                a.found_inf);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw_hparams launch: %s", cudaGetErrorString(e));
   count_launch();
@@ -182,18 +220,20 @@ int adamw_hparams(const mmfb_adamw_hparams_args& a, cudaStream_t s) {
 // first_block <= b is largest; thread t of its chunk c owns the 8-element group k = c * 256 + t, elements
 // [8k - lead, 8k - lead + 8) of the segment clipped to [0, n).  A group inside the segment whose four streams are
 // 16-byte aligned (head >= 0) moves as float4 pairs; the head group, the tail group and segments that are not co-aligned
-// are read and written element by element.  Elements go through adamw_elem, as in adamw_kernel.
+// are read and written element by element.  Elements go through adamw_elem, as in adamw_kernel; AMP as there.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int AS_THREADS = MMFB_ADAMW_SEGMENT_BLOCK / 8;
 static_assert(AS_THREADS == 256, "one 8-element group per thread");
 
-template <int MODE, bool SCALE_DEV>
+template <int MODE, bool SCALE_DEV, bool AMP>
 __global__ void __launch_bounds__(AS_THREADS)
 adamw_segments_kernel(const mmfb_adamw_segment* __restrict__ segs, int n_segs, const mmfb_adamw_hp* __restrict__ hp,
-                      float gscale, const float* __restrict__ gscale_dev) {
+                      float gscale, const float* __restrict__ gscale_dev, const float* __restrict__ loss_scale_dev,
+                      const float* __restrict__ found_inf) {
   __shared__ int s_seg;
   griddep_launch();
   griddep_wait();
+  if (AMP && amp_skip(found_inf)) return;
   const int b = blockIdx.x;
   if (threadIdx.x == 0) {
     int lo = 0, hi = n_segs - 1;
@@ -233,6 +273,11 @@ adamw_segments_kernel(const mmfb_adamw_segment* __restrict__ segs, int n_segs, c
       m[e] = in ? sg.exp_avg[j] : 0.0f; v[e] = in ? sg.exp_avg_sq[j] : 0.0f;
     }
   }
+  if (AMP && loss_scale_dev != nullptr) {
+    const float inv = amp_inv_scale(loss_scale_dev);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) g[e] = g[e] * inv;
+  }
 #pragma unroll
   for (int e = 0; e < 8; ++e)
     adamw_elem<MODE>(p[e], m[e], v[e], g[e], gs, h.lr, h.weight_decay, h.step_size, h.bc2_sqrt, h.beta1, h.beta2, h.eps);
@@ -261,13 +306,22 @@ int adamw_segments(const mmfb_adamw_segments_args& a, cudaStream_t s) {
   if (reinterpret_cast<uintptr_t>(a.segments) & 7 || reinterpret_cast<uintptr_t>(a.hp) & 15 ||
       reinterpret_cast<uintptr_t>(a.grad_scale_dev) & 3)
     return set_error(MMFB_ERR_ARG, "adamw_segments: segments must be 8-byte aligned, hp 16-byte, grad_scale_dev 4-byte");
-  const int variant = a.mode * 2 + (a.grad_scale_dev != nullptr ? 1 : 0);
+  const bool amp = a.loss_scale_dev != nullptr || a.found_inf != nullptr;
+  const int variant = (amp ? 4 : 0) + a.mode * 2 + (a.grad_scale_dev != nullptr ? 1 : 0);
+#define MMFB_AS_LAUNCH(MODE, SCALE_DEV, AMP)                                                                       \
+  MMFB_LAUNCH((adamw_segments_kernel<MODE, SCALE_DEV, AMP>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, \
+              a.hp, a.grad_scale, a.grad_scale_dev, a.loss_scale_dev, a.found_inf)
   switch (variant) {
-    case 0: MMFB_LAUNCH((adamw_segments_kernel<0, false>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, a.hp, a.grad_scale, a.grad_scale_dev); break;
-    case 1: MMFB_LAUNCH((adamw_segments_kernel<0, true>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, a.hp, a.grad_scale, a.grad_scale_dev); break;
-    case 2: MMFB_LAUNCH((adamw_segments_kernel<1, false>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, a.hp, a.grad_scale, a.grad_scale_dev); break;
-    default: MMFB_LAUNCH((adamw_segments_kernel<1, true>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, a.hp, a.grad_scale, a.grad_scale_dev); break;
+    case 0: MMFB_AS_LAUNCH(0, false, false); break;
+    case 1: MMFB_AS_LAUNCH(0, true, false); break;
+    case 2: MMFB_AS_LAUNCH(1, false, false); break;
+    case 3: MMFB_AS_LAUNCH(1, true, false); break;
+    case 4: MMFB_AS_LAUNCH(0, false, true); break;
+    case 5: MMFB_AS_LAUNCH(0, true, true); break;
+    case 6: MMFB_AS_LAUNCH(1, false, true); break;
+    default: MMFB_AS_LAUNCH(1, true, true); break;
   }
+#undef MMFB_AS_LAUNCH
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw_segments launch: %s", cudaGetErrorString(e));
   count_launch();
@@ -375,8 +429,11 @@ grad_norm_partial_kernel(const mmfb_grad_segment* __restrict__ segs, int n_segs,
   if (threadIdx.x == 0) partial[b] = tot;
 }
 
+// SCALE_DEV: the threshold is max_norm * *max_norm_scale in fp32 (MMF's clip of loss-scaled gradients at max_norm * S).
+template <bool SCALE_DEV>
 __global__ void __launch_bounds__(GN_FINAL_THREADS)
-grad_norm_final_kernel(const double* __restrict__ partial, int n_blocks, float max_norm, float* __restrict__ out) {
+grad_norm_final_kernel(const double* __restrict__ partial, int n_blocks, float max_norm, float* __restrict__ out,
+                       const float* __restrict__ max_norm_scale) {
   __shared__ double red[GN_FINAL_THREADS / 32];
   griddep_launch();
   griddep_wait();
@@ -388,7 +445,8 @@ grad_norm_final_kernel(const double* __restrict__ partial, int n_blocks, float m
     // evaluates `float / Tensor` as reciprocal(Tensor) * float, and so does this.  The comparison form keeps a NaN
     // coefficient NaN (fminf would return 1).
     const float norm = static_cast<float>(sqrt(tot));
-    const float c = __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), max_norm);
+    const float mn = SCALE_DEV ? __fmul_rn(max_norm, *max_norm_scale) : max_norm;
+    const float c = __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), mn);
     out[0] = norm;
     out[1] = c > 1.0f ? 1.0f : c;
   }
@@ -405,8 +463,12 @@ int grad_norm(const mmfb_grad_norm_args& a, cudaStream_t s) {
   MMFB_LAUNCH(grad_norm_partial_kernel, a.n_blocks, GN_THREADS, 0, s, a.segments, a.n_segments, a.partials);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "grad_norm launch: %s", cudaGetErrorString(e));
-  MMFB_LAUNCH(grad_norm_final_kernel, 1, GN_FINAL_THREADS, 0, s, static_cast<const double*>(a.partials), a.n_blocks,
-              a.max_norm, a.out);
+  if (a.max_norm_scale_dev != nullptr)
+    MMFB_LAUNCH(grad_norm_final_kernel<true>, 1, GN_FINAL_THREADS, 0, s, static_cast<const double*>(a.partials),
+                a.n_blocks, a.max_norm, a.out, a.max_norm_scale_dev);
+  else
+    MMFB_LAUNCH(grad_norm_final_kernel<false>, 1, GN_FINAL_THREADS, 0, s, static_cast<const double*>(a.partials),
+                a.n_blocks, a.max_norm, a.out, a.max_norm_scale_dev);
   e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "grad_norm launch: %s", cudaGetErrorString(e));
   count_launch(2);

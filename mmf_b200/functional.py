@@ -751,13 +751,25 @@ def gelu_bwd(dh, u):
     return du
 
 
+def _req_scalar(t, what, name):
+    """the device scalars of the optimizer launches: None or a one-element fp32 CUDA tensor; returns its pointer"""
+    if t is None:
+        return None
+    if not torch.is_tensor(t) or not t.is_cuda or t.dtype != torch.float32 or t.numel() != 1:
+        raise ValueError("%s: %s must be a one-element fp32 CUDA tensor" % (what, name))
+    return t.data_ptr()
+
+
 def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, grad_scale=1.0, group_of_block=None,
-          param_bf16=None, grad_scale_dev=None, hp_dev=None):
+          param_bf16=None, grad_scale_dev=None, hp_dev=None, loss_scale_dev=None, found_inf=None):
     """One fused AdamW step over flat fp32 buffers (staged, include/mmfb200.h: mmfb_adamw).
     groups: list (<= 8) of dicts {lr, weight_decay, step_size, bc2_sqrt}; group_of_block: uint8 [n/8] or None;
     grad_scale_dev: None or a one-element fp32 CUDA tensor (grad_norm's clip coefficient) multiplied into grad_scale when
     the kernel runs.  hp_dev: None or an fp32 CUDA tensor [n_groups, 8] written by adamw_hparams; the kernel then reads
-    every group's hyper-parameters and beta1 / beta2 / eps from it, and `groups` may be None."""
+    every group's hyper-parameters and beta1 / beta2 / eps from it, and `groups` may be None.
+    loss_scale_dev, found_inf: None or one-element fp32 CUDA tensors (GradScaler's scale and non-finite flag): the
+    gradients are first multiplied by fp32(1 / fp64(scale)), as GradScaler.unscale_ does, and a non-zero found_inf makes
+    the launch write nothing."""
     for t, n in ((param, "param"), (grad, "grad"), (exp_avg, "exp_avg"), (exp_avg_sq, "exp_avg_sq")):
         _req(t, torch.float32, n)
         if not t.is_contiguous() or t.numel() != param.numel():
@@ -788,6 +800,8 @@ def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, 
         if not grad_scale_dev.is_cuda or grad_scale_dev.dtype != torch.float32 or grad_scale_dev.numel() != 1:
             raise ValueError("adamw: grad_scale_dev must be a one-element fp32 CUDA tensor")
         a.grad_scale_dev = grad_scale_dev.data_ptr()
+    a.loss_scale_dev = _req_scalar(loss_scale_dev, "adamw", "loss_scale_dev")
+    a.found_inf = _req_scalar(found_inf, "adamw", "found_inf")
     check(LIB.mmfb_adamw(ctypes.byref(a), _stream_ptr()))
 
 
@@ -798,11 +812,12 @@ def _req_hp(hp, what):
                          % (what, lib.ADAMW_HP_FLOATS))
 
 
-def adamw_hparams(groups, slots, step, hp, mode):
+def adamw_hparams(groups, slots, step, hp, mode, found_inf=None):
     """Advance the step counts and write the AdamW hyper-parameter table on the device (include/mmfb200.h:
     mmfb_adamw_hparams).  groups: fp64 CUDA [n_groups, 5] (lr, weight_decay, beta1, beta2, eps); slots: the device
     table of adamw_slot_table; step: int64 CUDA [n_slots], advanced by one for every slot that is not frozen; hp: fp32
-    CUDA [n_slots, 8], overwritten.  Nothing is read on the host."""
+    CUDA [n_slots, 8], overwritten.  found_inf: None or a one-element fp32 CUDA tensor; when it is non-zero the launch
+    changes nothing (a step GradScaler skips does not count).  Nothing is read on the host."""
     if groups.dtype != torch.float64 or groups.dim() != 2 or groups.shape[1] != lib.ADAMW_GROUP_HP_DOUBLES or \
             not groups.is_contiguous():
         raise ValueError("adamw_hparams: groups must be a contiguous fp64 tensor [n_groups, %d]" % lib.ADAMW_GROUP_HP_DOUBLES)
@@ -817,6 +832,7 @@ def adamw_hparams(groups, slots, step, hp, mode):
     a = lib.AdamWHparamsArgs()
     a.groups, a.slots, a.step, a.hp = groups.data_ptr(), slots.data_ptr(), step.data_ptr(), hp.data_ptr()
     a.n_slots, a.mode = step.numel(), int(mode)
+    a.found_inf = _req_scalar(found_inf, "adamw_hparams", "found_inf")
     check(LIB.mmfb_adamw_hparams(ctypes.byref(a), _stream_ptr()))
 
 
@@ -874,10 +890,10 @@ def adamw_segment_table(segments):
     return AdamWSegmentTable(host.to(segments[0][0].device, non_blocking=True), rows, n_blocks)
 
 
-def adamw_segments(table, hp, *, mode, grad_scale=1.0, grad_scale_dev=None):
+def adamw_segments(table, hp, *, mode, grad_scale=1.0, grad_scale_dev=None, loss_scale_dev=None, found_inf=None):
     """One AdamW launch over every tensor of `table` (include/mmfb200.h: mmfb_adamw_segments), each with the
     hyper-parameters of its slot in hp (fp32 CUDA [slots, 8], written by adamw_hparams).  Element for element the
-    arithmetic of adamw; grad_scale_dev as there."""
+    arithmetic of adamw; grad_scale_dev, loss_scale_dev and found_inf as there."""
     _req_hp(hp, "adamw_segments")
     a = lib.AdamWSegmentsArgs()
     a.segments, a.n_segments, a.n_blocks = table.segments.data_ptr(), len(table.rows), table.n_blocks
@@ -886,6 +902,8 @@ def adamw_segments(table, hp, *, mode, grad_scale=1.0, grad_scale_dev=None):
         if not grad_scale_dev.is_cuda or grad_scale_dev.dtype != torch.float32 or grad_scale_dev.numel() != 1:
             raise ValueError("adamw_segments: grad_scale_dev must be a one-element fp32 CUDA tensor")
         a.grad_scale_dev = grad_scale_dev.data_ptr()
+    a.loss_scale_dev = _req_scalar(loss_scale_dev, "adamw_segments", "loss_scale_dev")
+    a.found_inf = _req_scalar(found_inf, "adamw_segments", "found_inf")
     check(LIB.mmfb_adamw_segments(ctypes.byref(a), _stream_ptr()))
 
 
@@ -925,10 +943,12 @@ def grad_norm_table(grads):
     return GradNormTable(host.to(device, non_blocking=True), len(segs), first, device)
 
 
-def grad_norm(table, max_norm, norm_type=2.0):
+def grad_norm(table, max_norm, norm_type=2.0, max_norm_scale_dev=None):
     """Global L2 norm of the gradients of `table` and torch's clip coefficient min(max_norm / (norm + 1e-6), 1), both
     computed on the device (include/mmfb200.h: mmfb_grad_norm).  Returns fp32 [2] = (total_norm, clip_coef) without a host
-    synchronisation; the summation order is fixed, so the bits repeat in every mode.  Only norm_type 2 is supported."""
+    synchronisation; the summation order is fixed, so the bits repeat in every mode.  Only norm_type 2 is supported.
+    max_norm_scale_dev: None or a one-element fp32 CUDA tensor S; the threshold is then fp32(max_norm) * S in fp32, read
+    when the kernel runs (the clip of loss-scaled gradients)."""
     if float(norm_type) != 2.0:
         raise ValueError("grad_norm: only norm_type 2 is supported, got %s" % (norm_type,))
     out = torch.empty(2, dtype=torch.float32, device=table.device)
@@ -937,6 +957,7 @@ def grad_norm(table, max_norm, norm_type=2.0):
     a.segments, a.n_segments, a.n_blocks = table.segments.data_ptr(), table.n_segments, table.n_blocks
     a.partials, a.out = partials.data_ptr(), out.data_ptr()
     a.max_norm, a.norm_type = float(max_norm), float(norm_type)
+    a.max_norm_scale_dev = _req_scalar(max_norm_scale_dev, "grad_norm", "max_norm_scale_dev")
     check(LIB.mmfb_grad_norm(ctypes.byref(a), _stream_ptr()))
     return out
 

@@ -28,6 +28,12 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
     capture freezes: which parameters have gradients, the gradient and state buffers (they keep their storage from the
     warm-up on), `grad_scale` 1, correct_bias and the arithmetic mode.  The warm-up steps are undone, so capturing does
     not change the parameters or the optimizer state;
+  * loss scaling: `GraphedStep(..., optimizer=opt, scaler=torch.amp.GradScaler("cuda"))` captures MMF's fp16 update -
+    `scaler.scale(loss).backward()`, `opt.clip_grad_norm(c, scale=scaler._get_scale_async())`, `scaler.step(opt)`,
+    `scaler.update()`.  The capturable optimizer reads the scale and found_inf on the device, and GradScaler's
+    non-finite check and scale update are device ops, so a step with non-finite gradients is skipped and the scale
+    backs off or grows inside the replay.  What the capture freezes: the scaler's scale and growth-tracker tensors and
+    its factors and interval.  Its warm-up updates are undone too;
   * host draws: a model that draws its task on the host in every forward (UNITER) is captured by GraphedTaskSteps, one
     graph per task, with the draws made on the host before each replay;
   * evaluation: GraphedForward(model.eval(), batch) captures the eval forward `model(batch)` under torch.no_grad() -
@@ -89,7 +95,8 @@ def _copy_into(dst, src):
 
 
 class GraphedStep:
-    def __init__(self, model, loss_fn, example_batch, warmup=3, static_rows=False, optimizer=None, max_grad_norm=None):
+    def __init__(self, model, loss_fn, example_batch, warmup=3, static_rows=False, optimizer=None, max_grad_norm=None,
+                 scaler=None):
         """loss_fn(batch) -> scalar loss; `example_batch`: (nested dict / list of) CUDA tensors with the shapes of every later
         batch.  The model must be in the mode (train / eval) it will be replayed in.
 
@@ -107,11 +114,22 @@ class GraphedStep:
         optimizer: a B200AdamW(..., capturable=True) over the model's parameters; the graph then holds the whole training
         step: gradients zeroed, forward, backward, optimizer.clip_grad_norm(max_grad_norm) when max_grad_norm is set, and
         optimizer.step().  Each call stages the groups' current hyper-parameters, then replays; afterwards `.grad` holds
-        the step's unclipped gradients, as after an eager step."""
+        the step's unclipped gradients, as after an eager step.
+
+        scaler: a torch.amp.GradScaler (needs optimizer=); the graph then runs MMF's fp16 update: zero the gradients,
+        loss_fn (put the autocast inside it, with cache_enabled=False as torch requires under capture),
+        scaler.scale(loss).backward(), optimizer.clip_grad_norm(max_grad_norm, scale=<the device scale>) when
+        max_grad_norm is set, scaler.step(optimizer), scaler.update().  A call returns the unscaled loss; afterwards
+        `.grad` holds the scaled gradients (the optimizer unscales inside its kernels), and the scaler's scale and growth
+        tracker are those of the replayed update."""
         _check_optimizer("GraphedStep", optimizer, max_grad_norm)
+        if scaler is not None and optimizer is None:
+            raise ValueError("GraphedStep: scaler= unscales and skips inside the captured optimizer step; pass "
+                             "optimizer=B200AdamW(..., capturable=True) as well, or scale and step eagerly after each "
+                             "replay")
         _check_capturable("GraphedStep", model, static_rows)
         self.model, self.loss_fn = model, loss_fn
-        self.optimizer, self.max_grad_norm = optimizer, max_grad_norm
+        self.optimizer, self.max_grad_norm, self.scaler = optimizer, max_grad_norm, scaler
         with _static_rows_context() if static_rows else contextlib.nullcontext():
             self._capture(model, loss_fn, example_batch, warmup)
 
@@ -121,13 +139,14 @@ class GraphedStep:
         self.epoch = F.dropout_epoch(dev, create=True)
         opt = self.optimizer
         saved = _save_optimizer(opt) if opt is not None else None
+        saved_scaler = _save_scaler(self.scaler) if self.scaler is not None else None
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
             for _ in range(max(1, warmup)):              # lazy engine state, kernel attributes, library work buffers
                 self._zero_grads()
                 self.epoch.add_(1)
-                loss_fn(self.static).backward()
+                self._backward(loss_fn(self.static))
                 if opt is not None:                      # builds the optimizer's device tables on these gradients
                     self._optimizer_step()
         torch.cuda.current_stream(dev).wait_stream(side)
@@ -136,6 +155,8 @@ class GraphedStep:
             model.zero_grad(set_to_none=True)
         else:
             _restore_optimizer(opt, saved)
+            if self.scaler is not None:
+                _restore_scaler(self.scaler, saved_scaler)
             torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
         # captured on the warm-up stream: autograd binds every parameter's gradient accumulator to the stream that was current
@@ -146,7 +167,7 @@ class GraphedStep:
                 self._zero_grads()
             self.epoch.add_(1)
             self.loss = loss_fn(self.static)
-            self.loss.backward()
+            self._backward(self.loss)
             if opt is not None:
                 self._optimizer_step()
         self._plan = opt._cap if opt is not None else None
@@ -161,10 +182,20 @@ class GraphedStep:
         if grads:
             torch._foreach_zero_(grads)
 
+    def _backward(self, loss):
+        (loss if self.scaler is None else self.scaler.scale(loss)).backward()
+
     def _optimizer_step(self):
+        scaler = self.scaler
+        if scaler is None:
+            if self.max_grad_norm is not None:
+                self.optimizer.clip_grad_norm(self.max_grad_norm)
+            self.optimizer.step()
+            return
         if self.max_grad_norm is not None:
-            self.optimizer.clip_grad_norm(self.max_grad_norm)
-        self.optimizer.step()
+            self.optimizer.clip_grad_norm(self.max_grad_norm, scale=scaler._get_scale_async())
+        scaler.step(self.optimizer)
+        scaler.update()
 
     def __call__(self, batch=None):
         if batch is not None:
@@ -484,6 +515,22 @@ def _restore_optimizer(opt, saved):
             st["step"].copy_(old["step"]) if torch.is_tensor(old.get("step")) else st["step"].fill_(int(old.get("step", 0)))
         elif "step" in st:
             st["step"] = old.get("step", 0)
+
+
+def _save_scaler(scaler):
+    """copies of the GradScaler state the warm-up updates change (None before its first scale())"""
+    scale, tracker = scaler._scale, scaler._growth_tracker
+    return (scale.clone() if scale is not None else None, tracker.clone() if tracker is not None else None)
+
+
+def _restore_scaler(scaler, saved):
+    """undo the warm-up updates in place: the graph reads and writes these tensors at every replay.  A scaler whose
+    tensors the warm-up created gets its initial scale and a zero growth tracker, the state it stands for."""
+    scale, tracker = saved
+    if scaler._scale is not None:
+        scaler._scale.copy_(scale) if scale is not None else scaler._scale.fill_(scaler._init_scale)
+    if scaler._growth_tracker is not None:
+        scaler._growth_tracker.copy_(tracker) if tracker is not None else scaler._growth_tracker.zero_()
 
 
 def _flatten(x):

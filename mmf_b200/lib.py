@@ -98,6 +98,7 @@ class AdamWArgs(ctypes.Structure):
         ("bc2_sqrt", ctypes.c_float * 8),
         ("beta1", ctypes.c_float), ("beta2", ctypes.c_float), ("eps", ctypes.c_float), ("grad_scale", ctypes.c_float),
         ("mode", ctypes.c_int),
+        ("loss_scale_dev", ctypes.c_void_p), ("found_inf", ctypes.c_void_p),
         ("grad_scale_dev", ctypes.c_void_p),
         ("hp_dev", ctypes.c_void_p),
     ]
@@ -117,6 +118,7 @@ class AdamWHparamsArgs(ctypes.Structure):
     _fields_ = [
         ("groups", ctypes.c_void_p), ("slots", ctypes.c_void_p), ("step", ctypes.c_void_p), ("hp", ctypes.c_void_p),
         ("n_slots", ctypes.c_int), ("mode", ctypes.c_int),
+        ("found_inf", ctypes.c_void_p),
     ]
 
 
@@ -133,6 +135,7 @@ class AdamWSegmentsArgs(ctypes.Structure):
         ("segments", ctypes.c_void_p), ("n_segments", ctypes.c_int), ("n_blocks", ctypes.c_int),
         ("hp", ctypes.c_void_p), ("grad_scale", ctypes.c_float), ("mode", ctypes.c_int),
         ("grad_scale_dev", ctypes.c_void_p),
+        ("loss_scale_dev", ctypes.c_void_p), ("found_inf", ctypes.c_void_p),
     ]
 
 
@@ -149,6 +152,7 @@ class GradNormArgs(ctypes.Structure):
         ("segments", ctypes.c_void_p), ("n_segments", ctypes.c_int), ("n_blocks", ctypes.c_int),
         ("partials", ctypes.c_void_p), ("out", ctypes.c_void_p),
         ("max_norm", ctypes.c_float), ("norm_type", ctypes.c_float),
+        ("max_norm_scale_dev", ctypes.c_void_p),
     ]
 
 

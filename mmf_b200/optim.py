@@ -23,6 +23,15 @@ values, which stay Python floats in `param_groups` (schedulers keep working) and
 copy per step.  Packs get one `mmfb_adamw` each reading that table; every other parameter goes into one
 `mmfb_adamw_segments` launch.  `state_dict()` reports the step counts as ints (one device read).
 
+Loss scaling: a capturable B200AdamW implements torch's fused-optimizer protocol (`_step_supports_amp_scaling`), the path
+MMF's trainer takes with `training.fp16` (mmf/trainers/core/training_loop.py: `scaler.step(optimizer)`).  GradScaler then
+neither unscales the gradients nor reads `found_inf` on the host: it hands `step()` its scale and found_inf tensors, and
+every launch of the step reads them on the device - the kernels multiply each gradient by fp32(1 / fp64(scale)) before
+the clip factor, GradScaler.unscale_'s arithmetic, and a non-zero found_inf makes the launches write nothing, step counts
+included.  So `.grad` keeps the scaled gradients after `scaler.step`, as with torch's fused optimizers.
+`clip_grad_norm(max_norm, scale=scaler._get_scale_async())` clips the scaled gradients at max_norm times the device scale.
+The default mode keeps its step counts on the host and keeps GradScaler's unscale_ path.
+
 torch.optim.Adam: with arithmetic="torch" and weight_decay=0 the step is torch.optim.Adam's (amsgrad and maximize off):
 AdamW's decoupled decay multiplies the parameter by exactly 1, and the remaining operations - m.lerp_(g, 1-b1),
 v.mul_(b2).addcmul_(g, g, 1-b2), p.addcdiv_(m, sqrt(v)/sqrt(1-b2^t) + eps, -lr/(1-b1^t)) - are Adam's.  Pass Adam's
@@ -104,6 +113,10 @@ class B200AdamW(torch.optim.Optimizer):
         self._clip_coef = None    # 0-d fp32 CUDA tensor: the coefficient the next step() applies, then drops
         self.capturable = bool(capturable)   # fixed at construction, as the arithmetic mode and correct_bias are
         self._cap = None          # _CapturablePlan of the last capturable step
+        if self.capturable:
+            # torch.amp.GradScaler.step then passes its scale and found_inf tensors (attributes `grad_scale` and
+            # `found_inf` during the call) instead of unscaling on the device and reading found_inf on the host
+            self._step_supports_amp_scaling = True
 
     # ---------------------------------------------------------------------------------------------------------
     def _group_hp(self, group, step):
@@ -195,14 +208,17 @@ class B200AdamW(torch.optim.Optimizer):
         return grads
 
     @torch.no_grad()
-    def clip_grad_norm(self, max_norm, norm_type=2.0):
+    def clip_grad_norm(self, max_norm, norm_type=2.0, scale=None):
         """Clips the gradients of every parameter of the optimizer's groups to a global L2 norm of at most max_norm, as
         torch.nn.utils.clip_grad_norm_(params, max_norm) does, and returns the norm before clipping as a 0-d fp32 CUDA
         tensor - without a host synchronisation.  The gradients are not rewritten: the next step() (and only that one)
         multiplies them by min(max_norm / (norm + 1e-6), 1), so read .grad before the step to see unclipped values.
         Non-finite gradients give an inf / NaN norm and the same parameters as torch with error_if_nonfinite=False.
         Only norm_type 2 is supported.  The device table of gradient buffers is rebuilt only when a gradient moves; a
-        step captured in a CUDA graph needs one eager call with the same gradients before the capture."""
+        step captured in a CUDA graph needs one eager call with the same gradients before the capture.
+        scale: None or a 0-d fp32 CUDA tensor S (GradScaler's `_get_scale_async()`); the threshold is then max_norm * S,
+        computed in fp32 when the kernel runs - MMF's clip of loss-scaled gradients, `max_norm * scaler.get_scale()`,
+        without the host read."""
         if float(norm_type) != 2.0:
             raise ValueError("B200AdamW.clip_grad_norm supports norm_type 2 only, got %s" % (norm_type,))
         self._clip_coef = None
@@ -215,14 +231,17 @@ class B200AdamW(torch.optim.Optimizer):
                 raise RuntimeError("B200AdamW.clip_grad_norm: the gradient buffers changed during CUDA-graph capture; "
                                    "call clip_grad_norm once eagerly with the same gradients before capturing")
             self._clip_table = (key, F.grad_norm_table(grads))
-        out = F.grad_norm(self._clip_table[1], max_norm, norm_type)
+        out = F.grad_norm(self._clip_table[1], max_norm, norm_type,
+                          **({} if scale is None else {"max_norm_scale_dev": scale}))
         self._clip_coef = out[1]
         return out[0]
 
     @torch.no_grad()
     def step(self, closure=None, grad_scale=1.0):
         """grad_scale multiplies every gradient first (1 / loss scale, gradient-clipping coefficient).  After
-        clip_grad_norm, the gradients are multiplied by grad_scale * (its device-side coefficient) in this step only."""
+        clip_grad_norm, the gradients are multiplied by grad_scale * (its device-side coefficient) in this step only.
+        In capturable mode under GradScaler.step, the scaler's `grad_scale` and `found_inf` tensors (set on the
+        optimizer for the call) are read by every launch on the device; see the module docstring."""
         loss = None
         if closure is not None:
             with torch.enable_grad():
@@ -230,7 +249,11 @@ class B200AdamW(torch.optim.Optimizer):
         coef, self._clip_coef = self._clip_coef, None
         clip = {} if coef is None else {"grad_scale_dev": coef}
         if self.capturable:
-            self._step_capturable(grad_scale, clip)
+            amp = {}                               # set by GradScaler.step for this call only
+            for key, attr in (("loss_scale_dev", "grad_scale"), ("found_inf", "found_inf")):
+                if getattr(self, attr, None) is not None:
+                    amp[key] = getattr(self, attr)
+            self._step_capturable(grad_scale, clip, amp)
             return loss
         group_of = {id(p): gi for gi, g in enumerate(self.param_groups) for p in g["params"]}
         done = set()
@@ -420,15 +443,17 @@ class B200AdamW(torch.optim.Optimizer):
         if plan is not None:
             _h2d(self._group_values(), plan.device, out=plan.groups)
 
-    def _step_capturable(self, grad_scale, clip):
+    def _step_capturable(self, grad_scale, clip, amp):
         plan = self._capturable_plan()
         if plan is None:
             return
         if not _capturing():
             self.stage_hparams(plan)
-        F.adamw_hparams(plan.groups, plan.slot_table, plan.step, plan.hp, plan.mode)
+        F.adamw_hparams(plan.groups, plan.slot_table, plan.step, plan.hp, plan.mode,
+                        **({"found_inf": amp["found_inf"]} if "found_inf" in amp else {}))
         for pack, ent, s0, n, betas, eps in plan.packs:
             F.adamw(pack.master, pack.grad, ent["m"], ent["v"], None, beta1=betas[0], beta2=betas[1], eps=eps,
-                    mode=plan.mode, grad_scale=grad_scale, group_of_block=ent["groups"], hp_dev=plan.hp[s0:s0 + n], **clip)
+                    mode=plan.mode, grad_scale=grad_scale, group_of_block=ent["groups"], hp_dev=plan.hp[s0:s0 + n],
+                    **clip, **amp)
         if plan.loose:
-            F.adamw_segments(plan.table, plan.hp, mode=plan.mode, grad_scale=grad_scale, **clip)
+            F.adamw_segments(plan.table, plan.hp, mode=plan.mode, grad_scale=grad_scale, **clip, **amp)
