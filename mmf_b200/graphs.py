@@ -34,6 +34,14 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
     non-finite check and scale update are device ops, so a step with non-finite gradients is skipped and the scale
     backs off or grows inside the replay.  What the capture freezes: the scaler's scale and growth-tracker tensors and
     its factors and interval.  Its warm-up updates are undone too;
+  * gradient accumulation: `GraphedStep(..., optimizer=opt, update_frequency=K)` runs MMF's `training.update_frequency`
+    (mmf/trainers/core/training_loop.py: zero_grad, K backwards of losses not divided by K, clip, step).  It
+    captures a micro-batch graph (dropout epoch, forward, backward, no zeroing: every gradient adds in place) and an
+    update graph (clip, step, or scaler.step and scaler.update) in one memory pool; each call replays the micro graph,
+    the K-th of a group replays the update too, and `finish_update()` updates after a partial group.  The gradients are
+    zeroed in place (a graph of one `_foreach_zero_`) before the first micro-batch of a group, never set to None: the
+    optimizer's device tables point at them.  After an update `.grad` holds the group's sum, as after MMF's eager update.  It freezes what the one-graph step
+    freezes, and every micro-batch draws fresh dropout masks and counts its own static rows;
   * host draws: a model that draws its task on the host in every forward (UNITER) is captured by GraphedTaskSteps, one
     graph per task, with the draws made on the host before each replay;
   * evaluation: GraphedForward(model.eval(), batch) captures the eval forward `model(batch)` under torch.no_grad() -
@@ -42,6 +50,7 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
 The reference has no counterpart (its trainer launches eagerly, mmf/trainers/core/training_loop.py:185-213); this is the
 answer to SURVEY.md 8a's "at T = R = 36 everything is launch-bound"."""
 import contextlib
+import numbers
 import random
 
 import numpy as np
@@ -96,7 +105,7 @@ def _copy_into(dst, src):
 
 class GraphedStep:
     def __init__(self, model, loss_fn, example_batch, warmup=3, static_rows=False, optimizer=None, max_grad_norm=None,
-                 scaler=None):
+                 scaler=None, update_frequency=1):
         """loss_fn(batch) -> scalar loss; `example_batch`: (nested dict / list of) CUDA tensors with the shapes of every later
         batch.  The model must be in the mode (train / eval) it will be replayed in.
 
@@ -121,15 +130,37 @@ class GraphedStep:
         scaler.scale(loss).backward(), optimizer.clip_grad_norm(max_grad_norm, scale=<the device scale>) when
         max_grad_norm is set, scaler.step(optimizer), scaler.update().  A call returns the unscaled loss; afterwards
         `.grad` holds the scaled gradients (the optimizer unscales inside its kernels), and the scaler's scale and growth
-        tracker are those of the replayed update."""
+        tracker are those of the replayed update.
+
+        update_frequency: K > 1 (needs optimizer=) accumulates the gradients of K calls and updates once, as MMF's
+        `training.update_frequency: K` does; the loss is not divided by K.  Two graphs are captured in one memory pool:
+        a micro-batch graph (advance the dropout epoch, loss_fn, the backward - scaled with a scaler - adding into the
+        gradients in place) and an update graph (the clip and optimizer or scaler calls above), with a small graph
+        that zeroes the gradients in place.  Each call copies the batch, replays the micro graph and returns that
+        micro-batch's loss, valid until the next call; the first call of a group first replays the zeroing, and the
+        K-th stages the hyper-parameters and replays the update.  `pending` counts the
+        micro-batches since the last update, and finish_update() updates after a partial group (MMF's last update of a
+        run).  After an update `.grad` holds the group's summed gradients, unclipped and, with a scaler, scaled.
+        Construction leaves the gradients zeroed.  K = 1 is the one-graph step above."""
         _check_optimizer("GraphedStep", optimizer, max_grad_norm)
         if scaler is not None and optimizer is None:
             raise ValueError("GraphedStep: scaler= unscales and skips inside the captured optimizer step; pass "
                              "optimizer=B200AdamW(..., capturable=True) as well, or scale and step eagerly after each "
                              "replay")
+        if not isinstance(update_frequency, numbers.Integral) or isinstance(update_frequency, bool) or \
+                update_frequency < 1:
+            raise ValueError("GraphedStep: update_frequency must be a positive int (MMF's training.update_frequency), "
+                             "got %r" % (update_frequency,))
+        if update_frequency > 1 and optimizer is None:
+            raise ValueError("GraphedStep: update_frequency=%d accumulates gradients over %d calls and updates inside "
+                             "the captured optimizer step; pass optimizer=B200AdamW(..., capturable=True) as well "
+                             "(without one, every replay starts from fresh gradients)"
+                             % (update_frequency, update_frequency))
         _check_capturable("GraphedStep", model, static_rows)
         self.model, self.loss_fn = model, loss_fn
         self.optimizer, self.max_grad_norm, self.scaler = optimizer, max_grad_norm, scaler
+        self.update_frequency = int(update_frequency)
+        self.pending = 0          # micro-batches accumulated since the last update (update_frequency > 1)
         with _static_rows_context() if static_rows else contextlib.nullcontext():
             self._capture(model, loss_fn, example_batch, warmup)
 
@@ -157,8 +188,13 @@ class GraphedStep:
             _restore_optimizer(opt, saved)
             if self.scaler is not None:
                 _restore_scaler(self.scaler, saved_scaler)
+            if self.update_frequency > 1:
+                self._zero_grads()
             torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
+        if self.update_frequency > 1:
+            self._capture_accumulating(loss_fn, side)
+            return
         # captured on the warm-up stream: autograd binds every parameter's gradient accumulator to the stream that was current
         # when the accumulator was created, i.e. this one, as long as no autograd graph from an earlier eager step on another
         # stream is still alive (it would keep the old accumulators - and their stream - in use)
@@ -171,6 +207,23 @@ class GraphedStep:
             if opt is not None:
                 self._optimizer_step()
         self._plan = opt._cap if opt is not None else None
+
+    def _capture_accumulating(self, loss_fn, side):
+        """update_frequency > 1: the micro-batch graph, then in its memory pool the in-place zeroing and the update.  Every
+        .grad is bound to its final buffer here, so the packs' prepare_grads records no zeroing and loose gradients are
+        added to in place by AccumulateGrad: both accumulate across replays.  The zeroing allocates nothing; the update
+        may reuse pool blocks the micro graph freed, which holds because it replays after micro-batches and leaves nothing
+        in the pool that a later replay reads."""
+        with torch.cuda.graph(self.graph, stream=side):
+            self.epoch.add_(1)
+            self.loss = loss_fn(self.static)
+            self._backward(self.loss)
+        self.zero_graph, self.update_graph = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.zero_graph, pool=self.graph.pool(), stream=side):
+            self._zero_grads()
+        with torch.cuda.graph(self.update_graph, pool=self.graph.pool(), stream=side):
+            self._optimizer_step()
+        self._plan = self.optimizer._cap
 
     def _zero_grads(self):
         """without an optimizer: .grad unset (the flat buffers are zeroed inside the graph); with one: zeroed in place, so
@@ -200,10 +253,32 @@ class GraphedStep:
     def __call__(self, batch=None):
         if batch is not None:
             _copy_into(self.static, batch)
+        if self.update_frequency > 1:
+            return self._micro_batch()
         if self.optimizer is not None:
             self.optimizer.stage_hparams(self._plan)
         self.graph.replay()
         return self.loss
+
+    def _micro_batch(self):
+        if not self.pending:
+            self.zero_graph.replay()
+        self.graph.replay()
+        self.pending += 1
+        if self.pending == self.update_frequency:
+            self.finish_update()
+        return self.loss
+
+    def finish_update(self):
+        """Replay the update for the micro-batches accumulated since the last one: clip, step (or scaler.step and
+        scaler.update) with the groups' current hyper-parameters.  A call updates on its own on the update_frequency-th
+        micro-batch of a group, so this is for a partial group, MMF's last update of a run.  Nothing happens when no
+        micro-batch is pending."""
+        if not self.pending:
+            return
+        self.optimizer.stage_hparams(self._plan)
+        self.update_graph.replay()
+        self.pending = 0
 
 
 def _check_optimizer(who, optimizer, max_grad_norm):
