@@ -601,4 +601,8 @@ int64_t mmfb_launch_count(void);   /* number of kernels this library has launche
 #ifdef __cplusplus
 }
 #endif
+
+/* the device planner of skip-padding packings (mmfb_plan_packing) */
+#include "mmfb200_plan.h"
+
 #endif /* MMFB200_H_ */

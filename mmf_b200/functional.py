@@ -721,6 +721,35 @@ def gather_rows(x, idx, out=None):
     return out
 
 
+def plan_packing(masks, B, lens, causal_len=0):
+    """The packing of one or two streams planned on the device (mmfb_plan_packing): `masks` holds each stream's additive
+    fp32 [B, S_k] CUDA mask, or None for an unpadded stream, and `lens` their S_k.  Returns one (cu int32 [B+1], pack_map
+    int32 [B*S_k], unpack_map int32 [B*S_k]) per stream, None for a stream without a mask.  A position is kept where its
+    mask is exactly 0, or inside the causal tail (the last causal_len positions, one stream only); with two streams a
+    sample empty in one stream and not in the other keeps every position of the empty one.  Nothing is read on the host."""
+    masks, lens = list(masks), [int(s) for s in lens]
+    if len(masks) not in (1, 2) or len(lens) != len(masks):
+        raise ValueError("plan_packing: one or two streams, each with its length")
+    out, args = [], []
+    for m, S in zip(masks, lens):
+        if m is None:
+            out.append(None)
+            args += [None, S, None, None, None]
+            continue
+        _req(m, torch.float32, "mask")
+        if tuple(m.shape) != (B, S) or not m.is_contiguous():
+            raise ValueError("plan_packing: a mask must be contiguous fp32 [B=%d, S=%d], got %s" % (B, S, tuple(m.shape)))
+        cu = torch.empty(B + 1, dtype=torch.int32, device=m.device)
+        pack_map = torch.empty(B * S, dtype=torch.int32, device=m.device)
+        unpack_map = torch.empty(B * S, dtype=torch.int32, device=m.device)
+        out.append((cu, pack_map, unpack_map))
+        args += [m.data_ptr(), S, cu.data_ptr(), pack_map.data_ptr(), unpack_map.data_ptr()]
+    if len(masks) == 1:
+        args += [None, 0, None, None, None]
+    check(LIB.mmfb_plan_packing(*args, int(B), int(causal_len), _stream_ptr()))
+    return out
+
+
 def add(a, b):
     """a + b (bf16, contiguous, same size)."""
     _req(a, torch.bfloat16, "a"); _req(b, torch.bfloat16, "b")

@@ -21,6 +21,8 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
   * skip-padding: a single-stream encoder with skip_padding set plans its packing on the host in an eager step.  Inside
     `static_rows()` it plans it on the device at the capacity B*S (mmf_b200.modules._plan_packing_static) and bounds
     every GEMM, LayerNorm and column sum of its layers by the device token count, so that step can be captured too.
+    Runners switched on with set_skip_padding(..., device_plan=True) do the same for M4C's causal tail (pack_tail) and
+    the ViLBERT / LXMERT streams (pack_streams): one kernel (functional.plan_packing) plans every stream of the call.
   * the optimizer: `GraphedStep(..., optimizer=opt, max_grad_norm=c)` with a `B200AdamW(..., capturable=True)` captures
     the whole step - gradients zeroed in place, forward, backward, `opt.clip_grad_norm(c)`, `opt.step()`.  The step
     counts and bias corrections advance on the device; the groups' lr / weight_decay / betas / eps are staged from
@@ -68,7 +70,8 @@ def static_rows():
     is the same mean cross-entropy and `logits` is None.  Nothing is read on the host, so the step can be captured.  A
     batch with no labelled row gives a loss of exactly 0 and zero gradients.
     Single-stream skip_padding encoders (calls without a causal tail) plan their packing on the device in the same way
-    (mmf_b200.modules.run_bert_encoder)."""
+    (mmf_b200.modules.run_bert_encoder), and so do causal-tail and two-stream encoders whose runner has `device_plan`
+    set (patch.set_skip_padding(..., device_plan=True))."""
     _STATIC_ROWS[0] += 1
     try:
         yield
@@ -117,7 +120,8 @@ class GraphedStep:
         row gather (it declares `static_rows_capturable = True`: VinVL, ViLT with an `mlm` head) is accepted, and LXMERT's
         masked-LM loss is captured too.  Single-stream skip_padding encoders (patch.set_skip_padding(model)) plan their
         packing on the device there and are captured as well, at a fixed capacity of every row of the batch.  Those with
-        `pack_tail` (set_skip_padding(..., causal=True)) and two-stream encoders with `pack_streams` are still refused.
+        `pack_tail` (set_skip_padding(..., causal=True)) and two-stream encoders with `pack_streams` are captured too
+        when they were switched on with set_skip_padding(..., device_plan=True), and refused otherwise.
         Opt-in because the replayed step differs from an eager one: no MLM logits.
 
         optimizer: a B200AdamW(..., capturable=True) over the model's parameters; the graph then holds the whole training
@@ -302,16 +306,19 @@ def _check_capturable(who, model, static_rows):
 
 
 def _check_runners(who, model, static_rows):
-    """the encoders' skip-padding modes that read token counts on the host, and so cannot be captured"""
+    """the encoders' skip-padding modes that read token counts on the host, and so cannot be captured: under static_rows,
+    pack_tail and pack_streams runners with `device_plan` set plan on the device and are accepted"""
     runners = [m.__dict__.get("_runner") for m in model.modules()]
     if not static_rows and any(getattr(r, "skip_padding", False) for r in runners):
         raise RuntimeError("%s: the model has skip_padding encoders, which read the token count on the host and "
                            "cannot be captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)" % who)
-    if static_rows and any(getattr(r, "skip_padding", False) and getattr(r, "pack_tail", False) for r in runners):
+    planned = lambda r: static_rows and getattr(r, "device_plan", False)      # counts planned on the device instead
+    if static_rows and any(getattr(r, "skip_padding", False) and getattr(r, "pack_tail", False) and not planned(r)
+                           for r in runners):
         raise RuntimeError("%s: the model has skip_padding encoders with pack_tail set, which read the token "
                            "count on the host for calls with a causal tail even under static_rows, so they cannot be "
                            "captured; turn them off with mmf_b200.patch.set_skip_padding(model, False)" % who)
-    if any(getattr(r, "pack_streams", False) for r in runners):
+    if any(getattr(r, "pack_streams", False) and not planned(r) for r in runners):
         raise RuntimeError("%s: the model has two-stream encoders with pack_streams set, which read the token "
                            "counts on the host%s and cannot be captured; turn them off with "
                            "mmf_b200.patch.set_skip_padding(model, False, two_stream=True)"
@@ -341,7 +348,8 @@ class GraphedForward:
     The model must be in eval mode: nothing is drawn, and the dropout step counter of GraphedStep is neither created nor
     advanced.  Refused before any warm-up, as GraphedStep refuses them: skip-padding encoders without static_rows,
     pack_tail and pack_streams encoders, and modules that declare `graph_capturable = False` (UNITER, whose forward draws
-    its task on the host; VinVL and ViLT pretraining without static_rows).  Also refused: a model that returns attention
+    its task on the host; VinVL and ViLT pretraining without static_rows); under static_rows pack_tail and pack_streams
+    encoders switched on with device_plan=True are accepted.  Also refused: a model that returns attention
     probabilities or hidden states (output_attentions / output_hidden_states / visualization), and a model or batch off
     the GPU.
 

@@ -236,7 +236,9 @@ def _load():
                                      ctypes.c_void_p]
     lib.mmfb_gather_rows.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
                                      ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
-    lib.mmfb_add_bf16.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
+    lib.mmfb_plan_packing.argtypes = ([ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 3) * 2 + \
+        [ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
+    lib.mmfb_add_bf16.argtypes =[ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]
     lib.mmfb_dropout_apply.argtypes = [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_float,
                                        ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]
     lib.mmfb_cast_f32_bf16.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]

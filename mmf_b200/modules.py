@@ -109,6 +109,9 @@ class EncoderRunner(_LayerStack):
         self.skip_padding = False
         # with skip_padding: also pack calls with a causal tail (M4C's multimodal transformer), keeping every tail row
         self.pack_tail = False
+        # with pack_tail: inside graphs.static_rows() plan those calls on the device (_static_packings) so they can be
+        # captured
+        self.device_plan = False
 
     def forward(self, x, add_mask, training, need_grad, probs=None):
         """probs: an engine.ProbsSink that receives every layer's attention probabilities, or None"""
@@ -227,6 +230,26 @@ def _plan_packing_static(mask, B, S):
     pack_map = torch.searchsorted(incl, torch.arange(1, C + 1, dtype=torch.int32, device=mask.device), out_int32=True)
     pack_map = torch.where(pack_map < C, pack_map, torch.full_like(pack_map, -1))
     return _StaticPacking(pack_map, unpack_map, E.Varlen(cu, B, C, S, count=cu[B:]))
+
+
+def _static_packings(masks, B, lens, causal_len=0):
+    """The packings of one or two streams planned on the device by one kernel (functional.plan_packing), at the capacity
+    B*S of each stream: a _StaticPacking per stream with a mask, whose Varlen carries the device count cu[B]; a stream
+    without a mask keeps the trivial packing, unbounded.  With causal_len = T > 0 (one stream) the last T positions of
+    every sample are kept whatever the mask holds there, as _tail_kept does.  Two streams: a sample with tokens in one
+    stream and none in the other keeps every row of the empty one, so the other's queries attend over all of them - the
+    dense path gives those keys one common mask value, so the function is the dense one up to rounding, where
+    plan_two_stream falls back to the dense path.  A sample without tokens in either stream keeps no row (zero outputs
+    and input gradients).  Nothing is read on the host, and a mask value that is neither 0 nor <= -10000 is padding."""
+    device = next(m.device for m in masks if m is not None)
+    out = []
+    for S, plan in zip(lens, E.F.plan_packing(masks, B, lens, causal_len)):
+        if plan is None:
+            out.append(_trivial_packing(B, S, device))
+            continue
+        cu, pack_map, unpack_map = plan
+        out.append(_StaticPacking(pack_map, unpack_map, E.Varlen(cu, B, B * S, S, causal_len, count=cu[B:])))
+    return out
 
 
 def _tail_kept(mask, causal_len):
@@ -352,7 +375,9 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
     Inside graphs.static_rows(), a call without a causal tail on a skip_padding runner plans its packing on the device
     (_plan_packing_static) instead: nothing is read on the host, so the call can be captured in a CUDA graph.  It runs the
     packed path at a fixed capacity of B*S rows whatever the mask holds (every row valid, or none: then the outputs and
-    the input gradient are exact zeros), and its mask values other than 0 and <= -10000 are not checked."""
+    the input gradient are exact zeros), and its mask values other than 0 and <= -10000 are not checked.  A call with a
+    causal tail on a pack_tail runner with `device_plan` set does the same there (_static_packings): it packs the same
+    rows as the eager call, every tail row included, and runs the packed path even when no row is padded."""
     _require_cuda(hidden_states, "hidden_states")
     if hidden_states.dim() != 3:
         raise ValueError("hidden_states must be [batch, seq, hidden], got %s" % (tuple(hidden_states.shape),))
@@ -367,7 +392,12 @@ def run_bert_encoder(runner, hidden_states, attention_mask, training, output_hid
             raise ValueError("causal_len must be in [0, S=%d], got %d" % (S, causal_len))
         packing = None
         if runner.skip_padding and runner.pack_tail and mask is not None and not output_attentions:
-            packing = _plan_packing(_tail_kept(mask, causal_len), B, S)     # never empty: the tail rows stay
+            if graphs.static_rows_active() and runner.device_plan:
+                if runner.W is not E.BertLayerW:
+                    raise RuntimeError("skip_padding under static_rows() covers BERT layer stacks only")
+                packing = _static_packings([mask], B, [S], causal_len)[0]
+            else:
+                packing = _plan_packing(_tail_kept(mask, causal_len), B, S)     # never empty: the tail rows stay
         if packing is not None:
             packing.varlen.causal_len = causal_len
             mask = packing
@@ -403,6 +433,9 @@ class TwoStreamRunner(_LayerStack):
         # skip padded tokens in both streams: pack each stream's valid rows once per encoder call and run variable-length
         # self- and cross-attention (plan_two_stream)
         self.pack_streams = False
+        # with pack_streams: inside graphs.static_rows() plan the packing on the device (_static_packings) so the call can
+        # be captured
+        self.device_plan = False
 
     def forward(self, xs, masks, lens, B, training, need_grad, block_states=None, probs=None):
         """xs: the two streams' [rows, H] activations, replaced by the outputs; masks: their additive masks, None or Varlen
@@ -444,7 +477,7 @@ class _TwoStreamEncoderFn(torch.autograd.Function):
         need_grad = any(ctx.needs_input_grad)
         runner.pack.refresh()
         xs = [x.detach().to(torch.bfloat16).contiguous().view(B * S, H) for x, S, H in zip((x0, x1), lens, Hs)]
-        packings = masks if isinstance(masks[0], _Packing) else None
+        packings = masks if isinstance(masks[0], (_Packing, _StaticPacking)) else None
         if packings is not None:                  # both streams run on their valid rows only
             xs, masks = [pk.pack(x) for pk, x in zip(packings, xs)], [pk.varlen for pk in packings]
         blocks = [] if want_blocks else None
@@ -488,12 +521,18 @@ def run_two_stream_encoder(runner, x0, x1, mask0, mask1, training, want_blocks=F
     Returns the two outputs, then (stream 0, stream 1) after every step that joins the streams if want_blocks, then the
     attention probabilities in step order if want_attn; the block states and probabilities carry no gradient.  With
     `runner.pack_streams` set the layers run on the valid rows (a call that asks for probabilities runs the dense path);
-    returns None when every token of both streams is padding, where every output and input-gradient row is zero."""
+    returns None when every token of both streams is padding, where every output and input-gradient row is zero.
+    Inside graphs.static_rows() a runner with `device_plan` set plans the packing on the device instead
+    (_static_packings), so the call can be captured: it always runs the packed path at the capacity of every row (never
+    returns None), and a sample with tokens in one stream only keeps every row of the other."""
     B, S0, _ = x0.shape
     S1 = x1.shape[1]
     runner.ensure(x0.device)
     masks = (E.additive_mask_2d(mask0, B, S0), E.additive_mask_2d(mask1, B, S1))
-    if runner.pack_streams and not want_attn:
+    if runner.pack_streams and not want_attn and runner.device_plan and graphs.static_rows_active() and \
+            any(m is not None for m in masks):
+        masks = tuple(_static_packings(masks, B, (S0, S1)))
+    elif runner.pack_streams and not want_attn:
         plan = plan_two_stream(*masks, B, S0, S1, x0.device)
         if plan == "empty":
             return None

@@ -72,7 +72,7 @@ def _routed(m):
     return getattr(f, "__func__", f) is _b200_encoder_forward
 
 
-def set_skip_padding(module, enabled=True, two_stream=False, causal=False):
+def set_skip_padding(module, enabled=True, two_stream=False, causal=False, device_plan=False):
     """Sets `skip_padding` on every single-stream encoder runner under `module` (B200BertEncoder - and so VisualBERT, MMBT,
     UNITER, VinVL and the TransformerEncoder plugin -, VisualBERT's bypass `additional_layer`, encoders routed by
     attach_encoder / replace_with_b200) and returns how many it set.  ViLBERT, LXMERT and ViT runners are left alone unless
@@ -86,11 +86,17 @@ def set_skip_padding(module, enabled=True, two_stream=False, causal=False):
     does not read padded positions it computes the same function and gradients as the dense path, up to rounding and the
     dropout masks drawn.  An eager call reads the token count on the host.  Inside graphs.static_rows() a call without a
     causal tail plans its packing on the device instead, at a fixed capacity of every row, so
-    `GraphedStep(..., static_rows=True)` captures such a model; calls with a causal tail (`causal`) and two-stream packing
-    still read the counts on the host and cannot be captured.
+    `GraphedStep(..., static_rows=True)` captures such a model.  Calls with a causal tail (`causal`) and two-stream packing
+    read the counts on the host there too, and cannot be captured, unless `device_plan` is True: it sets `device_plan` on
+    every runner this call touches, and inside static_rows() those plan every stream of a call with one device kernel,
+    at the capacity of every row (mmf_b200.modules._static_packings), so that GraphedStep and GraphedForward capture
+    them.  Opt-in, because that plan costs the capacity (the packed layers run B*S rows' worth of grid whatever the mask)
+    and because of the two-stream rule below.  Outside static_rows() it changes nothing.
 
     A two-stream call falls back to the dense path when some sample has tokens in one stream and none in the other: there
-    the dense outputs of those tokens depend on the other stream's padded rows.
+    the dense outputs of those tokens depend on the other stream's padded rows.  With `device_plan` inside static_rows()
+    such a sample instead keeps every row of its empty stream, which the dense path masks uniformly, so its valid outputs
+    are the dense ones up to rounding.
 
     The registered `lxmert` model refuses packed streams (ValueError): like the reference, it passes segment ids as the text
     attention mask, so its text "padding" includes [CLS] and the masked-LM positions.  B200LXMERTBase and
@@ -108,8 +114,10 @@ def set_skip_padding(module, enabled=True, two_stream=False, causal=False):
             r.skip_padding = bool(enabled)
             if causal:
                 r.pack_tail = bool(enabled)
+            r.device_plan = bool(device_plan)
             n += 1
         elif two_stream and isinstance(r, TwoStreamRunner):
             r.pack_streams = bool(enabled)
+            r.device_plan = bool(device_plan)
             n += 1
     return n
