@@ -604,5 +604,7 @@ int64_t mmfb_launch_count(void);   /* number of kernels this library has launche
 
 /* the device planner of skip-padding packings (mmfb_plan_packing) */
 #include "mmfb200_plan.h"
+/* the device update: learning-rate schedules and the fused non-finite check (mmfb_lr_schedule, mmfb_grad_*check) */
+#include "mmfb200_update.h"
 
 #endif /* MMFB200_H_ */

@@ -13,7 +13,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SOURCES = ["capi.cu", "gemm.cu", "attention.cu", "attention_varlen.cu", "attention_causal.cu", "attention_varlen_causal.cu",
            "attention_probs.cu", "rowops.cu", "optim.cu", "ce.cu", "ot.cu", "plan.cu"]
-HEADERS = ["common.cuh", "mmfb_internal.h", "../../include/mmfb200.h", "../../include/mmfb200_plan.h"]
+HEADERS = ["common.cuh", "mmfb_internal.h", "../../include/mmfb200.h", "../../include/mmfb200_plan.h",
+           "../../include/mmfb200_update.h"]
 LIB = os.path.join(HERE, "libmmfb200.so")
 STAMP = os.path.join(HERE, ".build_stamp")
 

@@ -366,7 +366,34 @@ int mmfb_grad_norm(const mmfb_grad_norm_args* args, mmfb_stream stream) {
   if (misaligned_f32(args->max_norm_scale_dev))
     return set_error(MMFB_ERR_ARG, "mmfb_grad_norm: max_norm_scale_dev must be 4-byte aligned");
   MMFB_REQUIRE_DEVICE();
-  return grad_norm(*args, reinterpret_cast<cudaStream_t>(stream));
+  return grad_norm(*args, nullptr, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_grad_norm_check(const mmfb_grad_norm_args* args, float* found_inf, mmfb_stream stream) {
+  if (!args || !found_inf) return set_error(MMFB_ERR_ARG, "mmfb_grad_norm_check: null pointer");
+  if (args->norm_type != 2.0f)
+    return set_error(MMFB_ERR_ARG, "mmfb_grad_norm_check: only norm_type 2 is supported (got %g)", args->norm_type);
+  if (misaligned_f32(args->max_norm_scale_dev) || misaligned_f32(found_inf))
+    return set_error(MMFB_ERR_ARG, "mmfb_grad_norm_check: max_norm_scale_dev and found_inf must be 4-byte aligned");
+  MMFB_REQUIRE_DEVICE();
+  return grad_norm(*args, found_inf, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_grad_check(const mmfb_grad_segment* segments, int n_segments, int n_blocks, double* flags, float* found_inf,
+                    mmfb_stream stream) {
+  if (!segments || !flags || !found_inf) return set_error(MMFB_ERR_ARG, "mmfb_grad_check: null pointer");
+  if (n_segments < 1 || n_blocks < 1)
+    return set_error(MMFB_ERR_ARG, "mmfb_grad_check: need at least one segment and one block (got %d, %d)", n_segments,
+                     n_blocks);
+  if (misaligned_f32(found_inf)) return set_error(MMFB_ERR_ARG, "mmfb_grad_check: found_inf must be 4-byte aligned");
+  MMFB_REQUIRE_DEVICE();
+  return grad_check(segments, n_segments, n_blocks, flags, found_inf, reinterpret_cast<cudaStream_t>(stream));
+}
+int mmfb_lr_schedule(const mmfb_lr_schedule_args* args, mmfb_stream stream) {
+  if (!args) return set_error(MMFB_ERR_ARG, "mmfb_lr_schedule: null args");
+  if (!args->counter || !args->base_lr || !args->lr) return set_error(MMFB_ERR_ARG, "mmfb_lr_schedule: null pointer");
+  if (args->desc.kind < MMFB_LR_WARMUP_LINEAR || args->desc.kind > MMFB_LR_PYTHIA)
+    return set_error(MMFB_ERR_ARG, "mmfb_lr_schedule: unknown schedule kind %d", args->desc.kind);
+  MMFB_REQUIRE_DEVICE();
+  return lr_schedule(*args, reinterpret_cast<cudaStream_t>(stream));
 }
 int mmfb_cast_f32_bf16(const float* in, void* out, int64_t n, mmfb_stream stream) {
   if (!in || !out) return set_error(MMFB_ERR_ARG, "mmfb_cast_f32_bf16: null pointer");

@@ -361,8 +361,17 @@ __device__ __forceinline__ double gn_load(const void* p, int dtype, int64_t i) {
                                  : static_cast<double>(static_cast<const float*>(p)[i]);
 }
 
+// Non-finite test of one fp32 value (a bf16 value widens to the same exponent): all exponent bits set is inf or NaN.
+__device__ __forceinline__ bool gn_nonfinite(float x) { return (__float_as_uint(x) & 0x7f800000u) == 0x7f800000u; }
+
+// KIND: GN_NORM sums the squares (the kernel this file always had); GN_NORM_CHECK also tests every element for
+// inf / NaN and writes the block's flag (1.0 or 0.0) to flags[b]; GN_CHECK only tests and writes flags[b].
+enum { GN_NORM = 0, GN_NORM_CHECK = 1, GN_CHECK = 2 };
+
+template <int KIND>
 __global__ void __launch_bounds__(GN_THREADS)
-grad_norm_partial_kernel(const mmfb_grad_segment* __restrict__ segs, int n_segs, double* __restrict__ partial) {
+grad_norm_partial_kernel(const mmfb_grad_segment* __restrict__ segs, int n_segs, double* __restrict__ partial,
+                         double* __restrict__ flags) {
   __shared__ int s_seg;
   __shared__ double red[GN_THREADS / 32];
   griddep_launch();
@@ -381,6 +390,7 @@ grad_norm_partial_kernel(const mmfb_grad_segment* __restrict__ segs, int n_segs,
   const int64_t start = static_cast<int64_t>(b - sg.first_block) * MMFB_GRAD_NORM_BLOCK;
   const int64_t len = min(static_cast<int64_t>(MMFB_GRAD_NORM_BLOCK), sg.n - start);
   double acc = 0.0;
+  bool bad = false;
   if (sg.dtype == MMFB_GRAD_BF16) {
     const bf16* p = static_cast<const bf16*>(sg.ptr) + start;
     const bool vec = (reinterpret_cast<uintptr_t>(p) & 15) == 0;
@@ -394,13 +404,17 @@ grad_norm_partial_kernel(const mmfb_grad_segment* __restrict__ segs, int n_segs,
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const float2 f = unpack_bf16x2(w[q]);
-          acc = fma(static_cast<double>(f.x), static_cast<double>(f.x), acc);
-          acc = fma(static_cast<double>(f.y), static_cast<double>(f.y), acc);
+          if (KIND != GN_CHECK) {
+            acc = fma(static_cast<double>(f.x), static_cast<double>(f.x), acc);
+            acc = fma(static_cast<double>(f.y), static_cast<double>(f.y), acc);
+          }
+          if (KIND != GN_NORM) bad |= gn_nonfinite(f.x) | gn_nonfinite(f.y);
         }
       } else {
         for (int64_t e = j; e < min(j + 8, len); ++e) {
           const double x = gn_load(p, MMFB_GRAD_BF16, e);
-          acc = fma(x, x, acc);
+          if (KIND != GN_CHECK) acc = fma(x, x, acc);
+          if (KIND != GN_NORM) bad |= gn_nonfinite(static_cast<float>(x));
         }
       }
     }
@@ -416,24 +430,44 @@ grad_norm_partial_kernel(const mmfb_grad_segment* __restrict__ segs, int n_segs,
         const float4 v = __ldcs(reinterpret_cast<const float4*>(p + j + 4));
         const float f[8] = {u.x, u.y, u.z, u.w, v.x, v.y, v.z, v.w};
 #pragma unroll
-        for (int q = 0; q < 8; ++q) acc = fma(static_cast<double>(f[q]), static_cast<double>(f[q]), acc);
+        for (int q = 0; q < 8; ++q) {
+          if (KIND != GN_CHECK) acc = fma(static_cast<double>(f[q]), static_cast<double>(f[q]), acc);
+          if (KIND != GN_NORM) bad |= gn_nonfinite(f[q]);
+        }
       } else {
         for (int64_t e = j; e < min(j + 8, len); ++e) {
           const double x = gn_load(p, MMFB_GRAD_F32, e);
-          acc = fma(x, x, acc);
+          if (KIND != GN_CHECK) acc = fma(x, x, acc);
+          if (KIND != GN_NORM) bad |= gn_nonfinite(static_cast<float>(x));
         }
       }
     }
   }
-  const double tot = gn_block_sum(acc, red);
-  if (threadIdx.x == 0) partial[b] = tot;
+  if (KIND != GN_NORM) {
+    bad = __syncthreads_or(bad);                  // an OR: the flag does not depend on which element or thread found it
+    if (threadIdx.x == 0) flags[b] = bad ? 1.0 : 0.0;
+  }
+  if (KIND != GN_CHECK) {
+    const double tot = gn_block_sum(acc, red);
+    if (threadIdx.x == 0) partial[b] = tot;
+  }
+}
+
+// Writes *found_inf = 1.0f when any of flags[0, n) is non-zero and 0.0f otherwise (one block of GN_FINAL_THREADS): an
+// OR over the blocks' flags, so the value does not depend on the order in which they were written.
+__device__ __forceinline__ void gn_found_inf(const double* __restrict__ flags, int n, float* __restrict__ found_inf) {
+  bool any = false;
+  for (int i = threadIdx.x; i < n; i += GN_FINAL_THREADS) any |= flags[i] != 0.0;
+  any = __syncthreads_or(any);
+  if (threadIdx.x == 0) *found_inf = any ? 1.0f : 0.0f;
 }
 
 // SCALE_DEV: the threshold is max_norm * *max_norm_scale in fp32 (MMF's clip of loss-scaled gradients at max_norm * S).
-template <bool SCALE_DEV>
+// CHECK: also writes *found_inf from the blocks' non-finite flags at partial + n_blocks.
+template <bool SCALE_DEV, bool CHECK>
 __global__ void __launch_bounds__(GN_FINAL_THREADS)
 grad_norm_final_kernel(const double* __restrict__ partial, int n_blocks, float max_norm, float* __restrict__ out,
-                       const float* __restrict__ max_norm_scale) {
+                       const float* __restrict__ max_norm_scale, float* __restrict__ found_inf) {
   __shared__ double red[GN_FINAL_THREADS / 32];
   griddep_launch();
   griddep_wait();
@@ -450,28 +484,145 @@ grad_norm_final_kernel(const double* __restrict__ partial, int n_blocks, float m
     out[0] = norm;
     out[1] = c > 1.0f ? 1.0f : c;
   }
+  if (CHECK) gn_found_inf(partial + n_blocks, n_blocks, found_inf);
 }
 
-int grad_norm(const mmfb_grad_norm_args& a, cudaStream_t s) {
-  if (!a.segments || !a.partials || !a.out) return set_error(MMFB_ERR_ARG, "grad_norm: null pointer");
-  if (a.norm_type != 2.0f) return set_error(MMFB_ERR_ARG, "grad_norm: only norm_type 2 is supported (got %g)", a.norm_type);
+__global__ void __launch_bounds__(GN_FINAL_THREADS)
+grad_check_final_kernel(const double* __restrict__ flags, int n_blocks, float* __restrict__ found_inf) {
+  griddep_launch();
+  griddep_wait();
+  gn_found_inf(flags, n_blocks, found_inf);
+}
+
+static int grad_table_args(const mmfb_grad_segment* segs, int n_segs, int n_blocks, const void* partials, const char* who) {
+  if (!segs || !partials) return set_error(MMFB_ERR_ARG, "%s: null pointer", who);
+  if (n_segs < 1 || n_blocks < 1)
+    return set_error(MMFB_ERR_ARG, "%s: need at least one segment and one block (got %d, %d)", who, n_segs, n_blocks);
+  if (reinterpret_cast<uintptr_t>(segs) & 7 || reinterpret_cast<uintptr_t>(partials) & 7)
+    return set_error(MMFB_ERR_ARG, "%s: segments / partials must be 8-byte aligned", who);
+  return MMFB_OK;
+}
+
+int grad_norm(const mmfb_grad_norm_args& a, float* found_inf, cudaStream_t s) {
+  const char* who = found_inf ? "grad_norm_check" : "grad_norm";
+  if (!a.segments || !a.partials || !a.out) return set_error(MMFB_ERR_ARG, "%s: null pointer", who);
+  if (a.norm_type != 2.0f) return set_error(MMFB_ERR_ARG, "%s: only norm_type 2 is supported (got %g)", who, a.norm_type);
   if (a.n_segments < 1 || a.n_blocks < 1)
-    return set_error(MMFB_ERR_ARG, "grad_norm: need at least one segment and one block (got %d, %d)", a.n_segments, a.n_blocks);
+    return set_error(MMFB_ERR_ARG, "%s: need at least one segment and one block (got %d, %d)", who, a.n_segments, a.n_blocks);
   if (reinterpret_cast<uintptr_t>(a.segments) & 7 || reinterpret_cast<uintptr_t>(a.partials) & 7 ||
-      reinterpret_cast<uintptr_t>(a.out) & 3)
-    return set_error(MMFB_ERR_ARG, "grad_norm: segments / partials must be 8-byte aligned, out 4-byte aligned");
-  MMFB_LAUNCH(grad_norm_partial_kernel, a.n_blocks, GN_THREADS, 0, s, a.segments, a.n_segments, a.partials);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "grad_norm launch: %s", cudaGetErrorString(e));
-  if (a.max_norm_scale_dev != nullptr)
-    MMFB_LAUNCH(grad_norm_final_kernel<true>, 1, GN_FINAL_THREADS, 0, s, static_cast<const double*>(a.partials),
-                a.n_blocks, a.max_norm, a.out, a.max_norm_scale_dev);
+      reinterpret_cast<uintptr_t>(a.out) & 3 || reinterpret_cast<uintptr_t>(found_inf) & 3)
+    return set_error(MMFB_ERR_ARG, "%s: segments / partials must be 8-byte aligned, out and found_inf 4-byte aligned", who);
+  if (found_inf)
+    MMFB_LAUNCH(grad_norm_partial_kernel<GN_NORM_CHECK>, a.n_blocks, GN_THREADS, 0, s, a.segments, a.n_segments,
+                a.partials, a.partials + a.n_blocks);
   else
-    MMFB_LAUNCH(grad_norm_final_kernel<false>, 1, GN_FINAL_THREADS, 0, s, static_cast<const double*>(a.partials),
-                a.n_blocks, a.max_norm, a.out, a.max_norm_scale_dev);
+    MMFB_LAUNCH(grad_norm_partial_kernel<GN_NORM>, a.n_blocks, GN_THREADS, 0, s, a.segments, a.n_segments, a.partials,
+                static_cast<double*>(nullptr));
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "%s launch: %s", who, cudaGetErrorString(e));
+#define MMFB_GN_FINAL(SCALE_DEV, CHECK)                                                                                 \
+  MMFB_LAUNCH((grad_norm_final_kernel<SCALE_DEV, CHECK>), 1, GN_FINAL_THREADS, 0, s, static_cast<const double*>(a.partials), \
+              a.n_blocks, a.max_norm, a.out, a.max_norm_scale_dev, found_inf)
+  if (a.max_norm_scale_dev != nullptr) {
+    if (found_inf) MMFB_GN_FINAL(true, true); else MMFB_GN_FINAL(true, false);
+  } else {
+    if (found_inf) MMFB_GN_FINAL(false, true); else MMFB_GN_FINAL(false, false);
+  }
+#undef MMFB_GN_FINAL
   e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "grad_norm launch: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "%s launch: %s", who, cudaGetErrorString(e));
   count_launch(2);
+  return MMFB_OK;
+}
+
+int grad_check(const mmfb_grad_segment* segs, int n_segs, int n_blocks, double* flags, float* found_inf, cudaStream_t s) {
+  int st = grad_table_args(segs, n_segs, n_blocks, flags, "grad_check");
+  if (st != MMFB_OK) return st;
+  if (!found_inf) return set_error(MMFB_ERR_ARG, "grad_check: null pointer");
+  if (reinterpret_cast<uintptr_t>(found_inf) & 3) return set_error(MMFB_ERR_ARG, "grad_check: found_inf must be 4-byte aligned");
+  MMFB_LAUNCH(grad_norm_partial_kernel<GN_CHECK>, n_blocks, GN_THREADS, 0, s, segs, n_segs, static_cast<double*>(nullptr),
+              flags);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "grad_check launch: %s", cudaGetErrorString(e));
+  MMFB_LAUNCH(grad_check_final_kernel, 1, GN_FINAL_THREADS, 0, s, static_cast<const double*>(flags), n_blocks, found_inf);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "grad_check launch: %s", cudaGetErrorString(e));
+  count_launch(2);
+  return MMFB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Learning-rate schedules (include/mmfb200.h: mmfb_lr_schedule): one warp.  Every thread reads the counter t (plus one
+// when advancing), evaluates MMF's schedule at t in fp64 with explicitly rounded operations (no contraction into fma,
+// so each line is the host's Python expression), and writes base_lr[g] * lambda(t) for its groups; thread 0 then
+// stores the advanced counter.  The powers lr_ratio ** i come from the descriptor, computed on the host.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int LR_THREADS = 32;
+
+// bisect.bisect_right(lr_steps, t), the binary search itself (so an unsorted list gives the host's index as well)
+__device__ __forceinline__ int lr_bisect_right(const mmfb_lr_schedule_desc& d, int64_t t) {
+  int lo = 0, hi = d.n_lr_steps;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (t < d.lr_steps[mid]) hi = mid; else lo = mid + 1;
+  }
+  return lo;
+}
+
+// The factor on base_lr.  The multi-step kinds return it as warmup_factor * (1 - alpha) + alpha or lr_ratio ** idx;
+// base_lr * factor is then the reference's `base_lr * lr_ratio` (MultiStepScheduler.get_lr) and `base_lr * lmbda(t)`
+// (LambdaLR over lr_lambda_update) alike.
+__device__ __forceinline__ double lr_factor(const mmfb_lr_schedule_desc& d, int64_t t) {
+  if (d.kind == MMFB_LR_WARMUP_LINEAR || d.kind == MMFB_LR_WARMUP_COSINE) {
+    const int64_t w = d.warmup_iterations, n = d.total_steps;
+    if (t < w) return __ddiv_rn(static_cast<double>(t), static_cast<double>(w > 1 ? w : 1));
+    const int64_t span = n - w > 1 ? n - w : 1;
+    if (d.kind == MMFB_LR_WARMUP_LINEAR) {
+      const double x = __ddiv_rn(static_cast<double>(n - t), static_cast<double>(span));
+      return x > 0.0 ? x : 0.0;                                                    // max(0.0, x)
+    }
+    const double progress = __ddiv_rn(static_cast<double>(t - w), static_cast<double>(span));
+    const double arg = __dmul_rn(__dmul_rn(__dmul_rn(3.141592653589793, d.num_cycles), 2.0), progress);  // math.pi
+    const double y = __dmul_rn(0.5, __dadd_rn(1.0, cos(arg)));
+    return y > 0.0 ? y : 0.0;
+  }
+  if (d.use_warmup && t <= d.warmup_iterations) {
+    const double alpha = __ddiv_rn(static_cast<double>(t), static_cast<double>(d.warmup_iterations));
+    return __dadd_rn(__dmul_rn(d.warmup_factor, __dsub_rn(1.0, alpha)), alpha);
+  }
+  return d.ratio_pow[lr_bisect_right(d, t)];
+}
+
+__global__ void __launch_bounds__(LR_THREADS)
+lr_schedule_kernel(const __grid_constant__ mmfb_lr_schedule_args a) {
+  griddep_launch();
+  griddep_wait();
+  const int64_t t = *a.counter + (a.advance ? 1 : 0);
+  const double f = lr_factor(a.desc, t);
+  for (int g = threadIdx.x; g < a.n_groups; g += LR_THREADS)
+    a.lr[static_cast<int64_t>(g) * a.lr_stride] = __dmul_rn(a.base_lr[g], f);
+  __syncwarp();                                   // every lane has read the counter
+  if (a.advance && threadIdx.x == 0) *a.counter = t;
+}
+
+int lr_schedule(const mmfb_lr_schedule_args& a, cudaStream_t s) {
+  const mmfb_lr_schedule_desc& d = a.desc;
+  if (!a.counter || !a.base_lr || !a.lr) return set_error(MMFB_ERR_ARG, "lr_schedule: null pointer");
+  if ((reinterpret_cast<uintptr_t>(a.counter) | reinterpret_cast<uintptr_t>(a.base_lr) | reinterpret_cast<uintptr_t>(a.lr)) & 7)
+    return set_error(MMFB_ERR_ARG, "lr_schedule: counter, base_lr and lr must be 8-byte aligned");
+  if (a.n_groups < 1 || a.lr_stride < 1)
+    return set_error(MMFB_ERR_ARG, "lr_schedule: need n_groups >= 1 and lr_stride >= 1 (got %d, %d)", a.n_groups, a.lr_stride);
+  if (d.kind < MMFB_LR_WARMUP_LINEAR || d.kind > MMFB_LR_PYTHIA)
+    return set_error(MMFB_ERR_ARG, "lr_schedule: unknown schedule kind %d", d.kind);
+  if (d.n_lr_steps < 0 || d.n_lr_steps > MMFB_LR_MAX_MILESTONES)
+    return set_error(MMFB_ERR_ARG, "lr_schedule: n_lr_steps must be in [0, %d] (got %d)", MMFB_LR_MAX_MILESTONES, d.n_lr_steps);
+  if ((d.kind == MMFB_LR_MULTI_STEP || d.kind == MMFB_LR_PYTHIA) && d.use_warmup && d.warmup_iterations < 1)
+    return set_error(MMFB_ERR_ARG, "lr_schedule: warmup needs warmup_iterations >= 1 (got %lld)",
+                     static_cast<long long>(d.warmup_iterations));
+  MMFB_LAUNCH(lr_schedule_kernel, 1, LR_THREADS, 0, s, a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "lr_schedule launch: %s", cudaGetErrorString(e));
+  count_launch();
   return MMFB_OK;
 }
 

@@ -991,6 +991,57 @@ def grad_norm(table, max_norm, norm_type=2.0, max_norm_scale_dev=None):
     return out
 
 
+def grad_norm_check(table, max_norm, found_inf, norm_type=2.0, max_norm_scale_dev=None):
+    """grad_norm, and GradScaler's non-finite check of the same gradients in the same read (include/mmfb200.h:
+    mmfb_grad_norm_check): found_inf, a one-element fp32 CUDA tensor, is overwritten with 1.0 when any element is inf or
+    NaN and 0.0 otherwise.  The test is per element, not on the norm.  Returns fp32 [2] as grad_norm."""
+    if float(norm_type) != 2.0:
+        raise ValueError("grad_norm_check: only norm_type 2 is supported, got %s" % (norm_type,))
+    out = torch.empty(2, dtype=torch.float32, device=table.device)
+    partials = torch.empty(2 * table.n_blocks, dtype=torch.float64, device=table.device)
+    a = GradNormArgs()
+    a.segments, a.n_segments, a.n_blocks = table.segments.data_ptr(), table.n_segments, table.n_blocks
+    a.partials, a.out = partials.data_ptr(), out.data_ptr()
+    a.max_norm, a.norm_type = float(max_norm), float(norm_type)
+    a.max_norm_scale_dev = _req_scalar(max_norm_scale_dev, "grad_norm_check", "max_norm_scale_dev")
+    fi = _req_scalar(found_inf, "grad_norm_check", "found_inf")
+    if fi is None:
+        raise ValueError("grad_norm_check: found_inf must be a one-element fp32 CUDA tensor")
+    check(LIB.mmfb_grad_norm_check(ctypes.byref(a), fi, _stream_ptr()))
+    return out
+
+
+def grad_check(table, found_inf):
+    """GradScaler's non-finite check alone over the gradients of a grad_norm table (include/mmfb200.h: mmfb_grad_check):
+    found_inf is overwritten with 1.0 when any element is inf or NaN and 0.0 otherwise, nothing read on the host."""
+    fi = _req_scalar(found_inf, "grad_check", "found_inf")
+    if fi is None:
+        raise ValueError("grad_check: found_inf must be a one-element fp32 CUDA tensor")
+    flags = torch.empty(table.n_blocks, dtype=torch.float64, device=table.device)
+    check(LIB.mmfb_grad_check(table.segments.data_ptr(), table.n_segments, table.n_blocks, flags.data_ptr(), fi,
+                              _stream_ptr()))
+
+
+def lr_schedule(counter, base_lr, lr, desc, advance, lr_stride=1):
+    """One launch of MMF's learning-rate schedule on the device (include/mmfb200.h: mmfb_lr_schedule): with t = counter
+    (+ 1 when advancing), lr[g * lr_stride] = base_lr[g] * f(t) in fp64, and the counter is stored advanced.
+    counter: int64 CUDA [1]; base_lr: fp64 CUDA [n_groups]; lr: fp64 CUDA, typically the optimizer's group table;
+    desc: a lib.LrScheduleDesc."""
+    if counter.dtype != torch.int64 or counter.numel() != 1 or not counter.is_cuda:
+        raise ValueError("lr_schedule: counter must be a one-element int64 CUDA tensor")
+    if base_lr.dtype != torch.float64 or base_lr.dim() != 1 or not base_lr.is_contiguous() or not base_lr.is_cuda:
+        raise ValueError("lr_schedule: base_lr must be a contiguous fp64 CUDA tensor [n_groups]")
+    if lr.dtype != torch.float64 or not lr.is_contiguous() or not lr.is_cuda or \
+            lr.numel() < (base_lr.numel() - 1) * lr_stride + 1:
+        raise ValueError("lr_schedule: lr must be a contiguous fp64 CUDA tensor holding n_groups entries %d apart"
+                         % lr_stride)
+    a = lib.LrScheduleArgs()
+    a.counter, a.base_lr, a.lr = counter.data_ptr(), base_lr.data_ptr(), lr.data_ptr()
+    a.n_groups, a.lr_stride, a.advance = base_lr.numel(), int(lr_stride), 1 if advance else 0
+    a.desc = desc
+    check(LIB.mmfb_lr_schedule(ctypes.byref(a), _stream_ptr()))
+
+
 def cast_f32_bf16(src, dst):
     _req(src, torch.float32, "src"); _req(dst, torch.bfloat16, "dst")
     if src.numel() != dst.numel() or not src.is_contiguous() or not dst.is_contiguous():

@@ -36,6 +36,9 @@ nothing is traced or compiled.  What a capture freezes and how it is kept correc
     non-finite check and scale update are device ops, so a step with non-finite gradients is skipped and the scale
     backs off or grows inside the replay.  What the capture freezes: the scaler's scale and growth-tracker tensors and
     its factors and interval.  Its warm-up updates are undone too;
+  * learning-rate schedules: `GraphedStep(..., optimizer=opt, lr_scheduler=mmf_b200.optim.DeviceLRScheduler(opt, ...))`
+    ends every captured update with the scheduler's device step, so the lr needs no host work between replays; the
+    schedule descriptor (kind, warm-up, milestones, the powers of lr_ratio) and the base lrs' buffer are frozen;
   * gradient accumulation: `GraphedStep(..., optimizer=opt, update_frequency=K)` runs MMF's `training.update_frequency`
     (mmf/trainers/core/training_loop.py: zero_grad, K backwards of losses not divided by K, clip, step).  It
     captures a micro-batch graph (dropout epoch, forward, backward, no zeroing: every gradient adds in place) and an
@@ -108,7 +111,7 @@ def _copy_into(dst, src):
 
 class GraphedStep:
     def __init__(self, model, loss_fn, example_batch, warmup=3, static_rows=False, optimizer=None, max_grad_norm=None,
-                 scaler=None, update_frequency=1):
+                 scaler=None, update_frequency=1, lr_scheduler=None):
         """loss_fn(batch) -> scalar loss; `example_batch`: (nested dict / list of) CUDA tensors with the shapes of every later
         batch.  The model must be in the mode (train / eval) it will be replayed in.
 
@@ -145,8 +148,18 @@ class GraphedStep:
         K-th stages the hyper-parameters and replays the update.  `pending` counts the
         micro-batches since the last update, and finish_update() updates after a partial group (MMF's last update of a
         run).  After an update `.grad` holds the group's summed gradients, unclipped and, with a scaler, scaled.
-        Construction leaves the gradients zeroed.  K = 1 is the one-graph step above."""
+        Construction leaves the gradients zeroed.  K = 1 is the one-graph step above.
+
+        lr_scheduler: a mmf_b200.optim.DeviceLRScheduler attached to `optimizer`; the update then ends with
+        lr_scheduler.step() (after scaler.update() with a scaler), MMF's scheduler step, inside the graph: the next
+        update's lr is computed on the device and the replay needs no host work for it.  It advances once per update
+        (once per K calls), skipped fp16 updates included.  Warm-up and capture leave its counter as they found it.
+
+        With a scaler and B200AdamW(..., fused_inf_check=True) the update checks the gradients for inf / NaN in the
+        library's clip launch (optimizer.clip_grad_norm(max_grad_norm, scaler=scaler)), or in its check-only launch
+        (optimizer.check_finite(scaler)) without max_grad_norm, instead of GradScaler's foreach pass."""
         _check_optimizer("GraphedStep", optimizer, max_grad_norm)
+        _check_scheduler("GraphedStep", optimizer, lr_scheduler)
         if scaler is not None and optimizer is None:
             raise ValueError("GraphedStep: scaler= unscales and skips inside the captured optimizer step; pass "
                              "optimizer=B200AdamW(..., capturable=True) as well, or scale and step eagerly after each "
@@ -163,6 +176,7 @@ class GraphedStep:
         _check_capturable("GraphedStep", model, static_rows)
         self.model, self.loss_fn = model, loss_fn
         self.optimizer, self.max_grad_norm, self.scaler = optimizer, max_grad_norm, scaler
+        self.lr_scheduler = lr_scheduler
         self.update_frequency = int(update_frequency)
         self.pending = 0          # micro-batches accumulated since the last update (update_frequency > 1)
         with _static_rows_context() if static_rows else contextlib.nullcontext():
@@ -175,6 +189,7 @@ class GraphedStep:
         opt = self.optimizer
         saved = _save_optimizer(opt) if opt is not None else None
         saved_scaler = _save_scaler(self.scaler) if self.scaler is not None else None
+        saved_counter = self.lr_scheduler.counter.clone() if self.lr_scheduler is not None else None
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
@@ -192,6 +207,8 @@ class GraphedStep:
             _restore_optimizer(opt, saved)
             if self.scaler is not None:
                 _restore_scaler(self.scaler, saved_scaler)
+            if self.lr_scheduler is not None:
+                _restore_scheduler(self.lr_scheduler, saved_counter)
             if self.update_frequency > 1:
                 self._zero_grads()
             torch.cuda.synchronize(dev)
@@ -243,16 +260,24 @@ class GraphedStep:
         (loss if self.scaler is None else self.scaler.scale(loss)).backward()
 
     def _optimizer_step(self):
-        scaler = self.scaler
+        scaler, opt = self.scaler, self.optimizer
         if scaler is None:
             if self.max_grad_norm is not None:
-                self.optimizer.clip_grad_norm(self.max_grad_norm)
-            self.optimizer.step()
-            return
-        if self.max_grad_norm is not None:
-            self.optimizer.clip_grad_norm(self.max_grad_norm, scale=scaler._get_scale_async())
-        scaler.step(self.optimizer)
-        scaler.update()
+                opt.clip_grad_norm(self.max_grad_norm)
+            opt.step()
+        else:
+            fused = getattr(opt, "fused_inf_check", False)
+            if self.max_grad_norm is not None:
+                if fused:
+                    opt.clip_grad_norm(self.max_grad_norm, scaler=scaler)
+                else:
+                    opt.clip_grad_norm(self.max_grad_norm, scale=scaler._get_scale_async())
+            elif fused:
+                opt.check_finite(scaler)
+            scaler.step(opt)
+            scaler.update()
+        if self.lr_scheduler is not None:
+            self.lr_scheduler.step()
 
     def __call__(self, batch=None):
         if batch is not None:
@@ -292,6 +317,17 @@ def _check_optimizer(who, optimizer, max_grad_norm):
     if optimizer is not None and not getattr(optimizer, "capturable", False):
         raise ValueError("%s: the optimizer's step reads host values at every step and cannot be captured; "
                          "construct it as mmf_b200.optim.B200AdamW(..., capturable=True)" % who)
+
+
+def _check_scheduler(who, optimizer, lr_scheduler):
+    if lr_scheduler is None:
+        return
+    if optimizer is None:
+        raise ValueError("%s: lr_scheduler= steps inside the captured update; pass optimizer=B200AdamW(..., "
+                         "capturable=True) as well" % who)
+    if getattr(lr_scheduler, "optimizer", None) is not optimizer or not callable(getattr(lr_scheduler, "refresh", None)):
+        raise ValueError("%s: lr_scheduler must be a mmf_b200.optim.DeviceLRScheduler built on this optimizer (a host "
+                         "LambdaLR is stepped between replays instead)" % who)
 
 
 def _check_capturable(who, model, static_rows):
@@ -428,14 +464,17 @@ class GraphedTaskSteps:
     step of task t updates exactly the parameters an eager step of t updates: heads t does not reach keep their values,
     moments and step counts.  The step counts live in one device table that each graph reads before and writes after its
     optimizer step; step the optimizer only through this object while it is in use.  The warm-up steps are undone.
+    lr_scheduler: a DeviceLRScheduler on the optimizer, stepped inside every task's graph after its optimizer step, as
+    in GraphedStep; all graphs advance its one device counter, which warm-up and capture leave as they found it.
     Skip-padding and pack_streams encoders are refused as by GraphedStep without static_rows."""
 
-    def __init__(self, model, loss_fn, example_batch, warmup=3, optimizer=None, max_grad_norm=None):
+    def __init__(self, model, loss_fn, example_batch, warmup=3, optimizer=None, max_grad_norm=None, lr_scheduler=None):
         if not callable(getattr(model, "draw", None)) or not getattr(model, "draws_key", None) or \
                 not getattr(model, "tasks", None):
             raise TypeError("GraphedTaskSteps: the model must define draw(sample_list, task=None), draws_key and tasks; "
                             "capture a model that draws nothing on the host with GraphedStep")
         _check_optimizer("GraphedTaskSteps", optimizer, max_grad_norm)
+        _check_scheduler("GraphedTaskSteps", optimizer, lr_scheduler)
         _check_runners("GraphedTaskSteps", model, False)
         for m in model.modules():
             if m is not model and getattr(m, "graph_capturable", True) is False and \
@@ -443,7 +482,7 @@ class GraphedTaskSteps:
                 raise RuntimeError("GraphedTaskSteps: %s %s, so its step cannot be captured"
                                    % (type(m).__name__, getattr(m, "graph_refusal", "does work on the host in every forward")))
         self.model, self.loss_fn = model, loss_fn
-        self.optimizer, self.max_grad_norm = optimizer, max_grad_norm
+        self.optimizer, self.max_grad_norm, self.lr_scheduler = optimizer, max_grad_norm, lr_scheduler
         self.tasks = list(dict.fromkeys(model.tasks))
         self.task = None
         state = (torch.get_rng_state(), np.random.get_state(), random.getstate())
@@ -473,6 +512,7 @@ class GraphedTaskSteps:
         self.epoch = F.dropout_epoch(dev, create=True)
         params = list(dict.fromkeys(model.parameters()))
         saved = _save_optimizer(opt) if opt is not None else None
+        saved_counter = self.lr_scheduler.counter.clone() if self.lr_scheduler is not None else None
         self.grads, self.used, self.graphs, self.losses, self.plans, self._keep = {}, {}, {}, {}, {}, []
         pool = None
         side = torch.cuda.Stream(device=dev)
@@ -511,6 +551,8 @@ class GraphedTaskSteps:
             for i, p in enumerate(params):
                 if p in opt.state:
                     opt.state[p]["step"] = self.steps[i]
+            if self.lr_scheduler is not None:
+                _restore_scheduler(self.lr_scheduler, saved_counter)
             torch.cuda.synchronize(dev)
         self._bind_grads(self.tasks[-1])
 
@@ -553,6 +595,8 @@ class GraphedTaskSteps:
             opt.step()
             if counts is not None:                         # ... and back
                 self.steps.index_copy_(0, idx, plan.step.index_select(0, slots))
+            if self.lr_scheduler is not None:
+                self.lr_scheduler.step()
         return loss
 
     def __call__(self, batch=None):
@@ -614,6 +658,12 @@ def _restore_scaler(scaler, saved):
         scaler._scale.copy_(scale) if scale is not None else scaler._scale.fill_(scaler._init_scale)
     if scaler._growth_tracker is not None:
         scaler._growth_tracker.copy_(tracker) if tracker is not None else scaler._growth_tracker.zero_()
+
+
+def _restore_scheduler(sched, counter):
+    """undo the warm-up's scheduler steps in place (the graphs read the counter and the lr table at every replay)"""
+    sched.counter.copy_(counter)
+    sched.refresh()
 
 
 def _flatten(x):

@@ -156,6 +156,29 @@ class GradNormArgs(ctypes.Structure):
     ]
 
 
+MMFB_LR_WARMUP_LINEAR, MMFB_LR_WARMUP_COSINE, MMFB_LR_MULTI_STEP, MMFB_LR_PYTHIA = 0, 1, 2, 3
+MMFB_LR_MAX_MILESTONES = 32
+
+
+class LrScheduleDesc(ctypes.Structure):
+    _fields_ = [
+        ("kind", ctypes.c_int), ("use_warmup", ctypes.c_int),
+        ("warmup_iterations", ctypes.c_int64), ("total_steps", ctypes.c_int64),
+        ("warmup_factor", ctypes.c_double), ("num_cycles", ctypes.c_double),
+        ("n_lr_steps", ctypes.c_int), ("pad_", ctypes.c_int),
+        ("lr_steps", ctypes.c_int64 * MMFB_LR_MAX_MILESTONES),
+        ("ratio_pow", ctypes.c_double * (MMFB_LR_MAX_MILESTONES + 1)),
+    ]
+
+
+class LrScheduleArgs(ctypes.Structure):
+    _fields_ = [
+        ("counter", ctypes.c_void_p), ("base_lr", ctypes.c_void_p), ("lr", ctypes.c_void_p),
+        ("n_groups", ctypes.c_int), ("lr_stride", ctypes.c_int), ("advance", ctypes.c_int), ("pad_", ctypes.c_int),
+        ("desc", LrScheduleDesc),
+    ]
+
+
 class ScatterArgs(ctypes.Structure):
     _fields_ = [
         ("dsrc", ctypes.c_void_p * 2), ("ldsrc", ctypes.c_int64 * 2), ("src_row", ctypes.c_void_p * 2),
@@ -249,6 +272,10 @@ def _load():
         getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int,
                                        ctypes.c_void_p]
     lib.mmfb_attention_probs.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
+    lib.mmfb_grad_norm_check.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
+    lib.mmfb_grad_check.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
+                                    ctypes.c_void_p]
+    lib.mmfb_lr_schedule.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
     for name in ("mmfb_ot_fwd", "mmfb_ot_bwd"):
         getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p]
     return lib

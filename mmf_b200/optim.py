@@ -32,12 +32,27 @@ included.  So `.grad` keeps the scaled gradients after `scaler.step`, as with to
 `clip_grad_norm(max_norm, scale=scaler._get_scale_async())` clips the scaled gradients at max_norm times the device scale.
 The default mode keeps its step counts on the host and keeps GradScaler's unscale_ path.
 
+Learning-rate schedules on the device: `DeviceLRScheduler(opt, kind, **params)` (registered under MMF's scheduler names
+warmup_linear, warmup_cosine, multi_step and pythia) keeps LambdaLR's counter on the device and writes each group's
+scheduled lr into the fp64 group table the capturable step reads (`mmfb_lr_schedule`), so `sched.step()` is one launch
+that a CUDA graph can hold.  While it is attached, stage_hparams copies weight decay, betas and eps but not lr.
+
+Fused non-finite check: `B200AdamW(..., capturable=True, fused_inf_check=True)` with
+`clip_grad_norm(c, scaler=scaler)` (or `check_finite(scaler)` without clipping) tests every gradient for inf / NaN in
+the library's own launch and hands the flag to GradScaler as the result of an unscale, so `scaler.step` does not run
+its foreach check and unscale pass.  It relies on GradScaler internals, as `_get_scale_async` does: the per-optimizer
+state `_per_optimizer_states[id(opt)]` with its "stage" (torch.amp.grad_scaler.OptState) and "found_inf_per_device"
+entries, and step()'s handling of an optimizer with `_step_supports_amp_scaling` in stage UNSCALED: it reads
+found_inf_per_device instead of calling `_check_inf_per_device`, and sets `grad_scale` to None, so the optimizer keeps
+the scale tensor itself to unscale inside its kernels.
+
 torch.optim.Adam: with arithmetic="torch" and weight_decay=0 the step is torch.optim.Adam's (amsgrad and maximize off):
 AdamW's decoupled decay multiplies the parameter by exactly 1, and the remaining operations - m.lerp_(g, 1-b1),
 v.mul_(b2).addcmul_(g, g, 1-b2), p.addcdiv_(m, sqrt(v)/sqrt(1-b2^t) + eps, -lr/(1-b1^t)) - are Adam's.  Pass Adam's
 eps (1e-8) explicitly: this class defaults to the reference's 1e-6.  That is how M4C's `optimizer.type: Adam` runs here.
 """
 import math
+import numbers
 import weakref
 
 import torch
@@ -45,6 +60,7 @@ import torch
 from . import engine as E
 from . import functional as F
 from . import lib
+from .registry import registry
 
 
 def _capturing():
@@ -98,7 +114,7 @@ def _reference_arithmetic():
 
 class B200AdamW(torch.optim.Optimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0, correct_bias=True,
-                 arithmetic="auto", capturable=False):
+                 arithmetic="auto", capturable=False, fused_inf_check=False):
         if lr < 0.0 or eps < 0.0 or not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
             raise ValueError("Invalid AdamW hyper-parameters: lr=%s betas=%s eps=%s" % (lr, betas, eps))
         if arithmetic == "auto":
@@ -113,6 +129,13 @@ class B200AdamW(torch.optim.Optimizer):
         self._clip_coef = None    # 0-d fp32 CUDA tensor: the coefficient the next step() applies, then drops
         self.capturable = bool(capturable)   # fixed at construction, as the arithmetic mode and correct_bias are
         self._cap = None          # _CapturablePlan of the last capturable step
+        if fused_inf_check and not self.capturable:
+            raise ValueError("B200AdamW: fused_inf_check=True needs capturable=True (the steps that read GradScaler's "
+                             "scale and found_inf on the device)")
+        self.fused_inf_check = bool(fused_inf_check)
+        self._found_inf = None    # fp32 [1] CUDA: the flag the fused check writes and hands to GradScaler
+        self._amp_scale = None    # GradScaler's scale tensor registered by the fused check, read by the next step
+        self._lr_sched = None     # the DeviceLRScheduler writing the groups' lr on the device, if one is attached
         if self.capturable:
             # torch.amp.GradScaler.step then passes its scale and found_inf tensors (attributes `grad_scale` and
             # `found_inf` during the call) instead of unscaling on the device and reading found_inf on the host
@@ -207,8 +230,62 @@ class B200AdamW(torch.optim.Optimizer):
                     seen.add(id(p))
         return grads
 
+    def _grad_table(self):
+        """the F.GradNormTable over _clip_grads(), rebuilt (never during capture) when a gradient buffer moves"""
+        grads = self._clip_grads()
+        if not grads:
+            return None
+        key = tuple((g.data_ptr(), g.numel(), g.dtype) for g in grads)
+        if self._clip_table is None or self._clip_table[0] != key:
+            if _capturing():
+                raise RuntimeError("B200AdamW.clip_grad_norm: the gradient buffers changed during CUDA-graph capture; "
+                                   "call clip_grad_norm once eagerly with the same gradients before capturing")
+            self._clip_table = (key, F.grad_norm_table(grads))
+            if self.fused_inf_check and (self._found_inf is None or self._found_inf.device != grads[0].device):
+                self._found_inf = torch.zeros(1, dtype=torch.float32, device=grads[0].device)
+        return self._clip_table[1]
+
+    def _fused_scaler(self, scaler, who):
+        """the GradScaler whose non-finite check this call replaces (None when it is disabled); refuses one whose
+        optimizer state is past READY, as GradScaler.unscale_ does"""
+        if not self.fused_inf_check:
+            raise ValueError("B200AdamW.%s: scaler= needs B200AdamW(..., capturable=True, fused_inf_check=True)" % who)
+        if not scaler.is_enabled():
+            return None
+        from torch.amp.grad_scaler import OptState
+        if scaler._scale is None:
+            raise RuntimeError("B200AdamW.%s: the scaler has no scale yet; call scaler.scale(loss) first" % who)
+        if scaler._per_optimizer_states[id(self)]["stage"] is not OptState.READY:
+            raise RuntimeError("B200AdamW.%s: the scaler already unscaled or stepped this optimizer since the last "
+                               "update()" % who)
+        return scaler
+
+    def _register_found_inf(self, scaler):
+        """GradScaler's per-optimizer state as after unscale_: found_inf on its device, stage UNSCALED, so that
+        scaler.step passes it to step() and scaler.update() reads it, and neither checks the gradients again"""
+        from torch.amp.grad_scaler import OptState
+        st = scaler._per_optimizer_states[id(self)]
+        st["found_inf_per_device"] = {self._found_inf.device: self._found_inf}
+        st["stage"] = OptState.UNSCALED
+        self._amp_scale = scaler._get_scale_async()
+
     @torch.no_grad()
-    def clip_grad_norm(self, max_norm, norm_type=2.0, scale=None):
+    def check_finite(self, scaler):
+        """GradScaler's non-finite check of this optimizer's gradients in one library launch pair, for an fp16 update
+        without clipping (MMF's clip_gradients false): the flag goes to the scaler as clip_grad_norm(..., scaler=)
+        hands it over.  Needs fused_inf_check=True.  Returns the fp32 [1] flag (None when the scaler is disabled)."""
+        scaler = self._fused_scaler(scaler, "check_finite")
+        if scaler is None:
+            return None
+        table = self._grad_table()
+        if table is None:
+            raise RuntimeError("B200AdamW.check_finite: no parameter of the optimizer has a gradient")
+        F.grad_check(table, self._found_inf)
+        self._register_found_inf(scaler)
+        return self._found_inf
+
+    @torch.no_grad()
+    def clip_grad_norm(self, max_norm, norm_type=2.0, scale=None, scaler=None):
         """Clips the gradients of every parameter of the optimizer's groups to a global L2 norm of at most max_norm, as
         torch.nn.utils.clip_grad_norm_(params, max_norm) does, and returns the norm before clipping as a 0-d fp32 CUDA
         tensor - without a host synchronisation.  The gradients are not rewritten: the next step() (and only that one)
@@ -218,21 +295,26 @@ class B200AdamW(torch.optim.Optimizer):
         step captured in a CUDA graph needs one eager call with the same gradients before the capture.
         scale: None or a 0-d fp32 CUDA tensor S (GradScaler's `_get_scale_async()`); the threshold is then max_norm * S,
         computed in fp32 when the kernel runs - MMF's clip of loss-scaled gradients, `max_norm * scaler.get_scale()`,
-        without the host read."""
+        without the host read.
+        scaler: a torch.amp.GradScaler (needs fused_inf_check=True): the same read of the gradients also tests every
+        element for inf / NaN, and the flag is handed to the scaler as unscale_ would (see the module docstring), so
+        scaler.step runs no check of its own; scale defaults to the scaler's device scale."""
         if float(norm_type) != 2.0:
             raise ValueError("B200AdamW.clip_grad_norm supports norm_type 2 only, got %s" % (norm_type,))
+        if scaler is not None:
+            scaler = self._fused_scaler(scaler, "clip_grad_norm")
+            if scaler is not None and scale is None:
+                scale = scaler._get_scale_async()
         self._clip_coef = None
-        grads = self._clip_grads()
-        if not grads:
+        table = self._grad_table()
+        if table is None:
             return torch.tensor(0.0)
-        key = tuple((g.data_ptr(), g.numel(), g.dtype) for g in grads)
-        if self._clip_table is None or self._clip_table[0] != key:
-            if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
-                raise RuntimeError("B200AdamW.clip_grad_norm: the gradient buffers changed during CUDA-graph capture; "
-                                   "call clip_grad_norm once eagerly with the same gradients before capturing")
-            self._clip_table = (key, F.grad_norm_table(grads))
-        out = F.grad_norm(self._clip_table[1], max_norm, norm_type,
-                          **({} if scale is None else {"max_norm_scale_dev": scale}))
+        kw = {} if scale is None else {"max_norm_scale_dev": scale}
+        if scaler is None:
+            out = F.grad_norm(table, max_norm, norm_type, **kw)
+        else:
+            out = F.grad_norm_check(table, max_norm, self._found_inf, norm_type, **kw)
+            self._register_found_inf(scaler)
         self._clip_coef = out[1]
         return out[0]
 
@@ -253,6 +335,9 @@ class B200AdamW(torch.optim.Optimizer):
             for key, attr in (("loss_scale_dev", "grad_scale"), ("found_inf", "found_inf")):
                 if getattr(self, attr, None) is not None:
                     amp[key] = getattr(self, attr)
+            fused_scale, self._amp_scale = self._amp_scale, None
+            if fused_scale is not None and "loss_scale_dev" not in amp:
+                amp["loss_scale_dev"] = fused_scale  # GradScaler passes grad_scale=None after the fused check
             self._step_capturable(grad_scale, clip, amp)
             return loss
         group_of = {id(p): gi for gi, g in enumerate(self.param_groups) for p in g["params"]}
@@ -425,7 +510,11 @@ class B200AdamW(torch.optim.Optimizer):
         plan.step = _h2d(torch.tensor(counts, dtype=torch.int64), device)
         plan.slot_table = F.adamw_slot_table(plan.slots, device)
         plan.hp = torch.zeros(len(plan.slots), lib.ADAMW_HP_FLOATS, dtype=torch.float32, device=device)
-        plan.groups = torch.zeros(len(self.param_groups), lib.ADAMW_GROUP_HP_DOUBLES, dtype=torch.float64, device=device)
+        if self._lr_sched is not None:                 # the scheduler's table: its lr column is written on the device
+            plan.groups = self._lr_sched._table_for(self, device)
+        else:
+            plan.groups = torch.zeros(len(self.param_groups), lib.ADAMW_GROUP_HP_DOUBLES, dtype=torch.float64,
+                                      device=device)
         for p in stepped:
             self.state[p]["step"] = plan.step[slot_of[id(p)]]
         return plan
@@ -438,10 +527,20 @@ class B200AdamW(torch.optim.Optimizer):
     def stage_hparams(self, plan=None):
         """Copy the groups' current lr / weight_decay / betas / eps to the device table the next (eager or replayed)
         capturable step reads: one non-blocking copy from pinned memory on the current stream.  An eager step() does
-        this itself; GraphedStep does it before every replay."""
+        this itself; GraphedStep does it before every replay.  With a DeviceLRScheduler attached the lr is the one
+        the scheduler wrote on the device and is not copied (one copy per group of the other four values)."""
         plan = plan if plan is not None else self._cap
-        if plan is not None:
+        if plan is None:
+            return
+        if self._lr_sched is None:
             _h2d(self._group_values(), plan.device, out=plan.groups)
+            return
+        # a DeviceLRScheduler owns the lr column: one copy per group of its weight_decay, beta1, beta2, eps
+        host = self._group_values()[:, 1:].contiguous()
+        if plan.device.type == "cuda":
+            host = host.pin_memory()
+        for g in range(host.shape[0]):
+            plan.groups[g, 1:].copy_(host[g], non_blocking=True)
 
     def _step_capturable(self, grad_scale, clip, amp):
         plan = self._capturable_plan()
@@ -457,3 +556,181 @@ class B200AdamW(torch.optim.Optimizer):
                     **clip, **amp)
         if plan.loose:
             F.adamw_segments(plan.table, plan.hp, mode=plan.mode, grad_scale=grad_scale, **clip, **amp)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# learning-rate schedules on the device
+_SCHEDULE_KINDS = {"warmup_linear": lib.MMFB_LR_WARMUP_LINEAR, "warmup_cosine": lib.MMFB_LR_WARMUP_COSINE,
+                   "multi_step": lib.MMFB_LR_MULTI_STEP, "pythia": lib.MMFB_LR_PYTHIA}
+
+
+def _cfg(obj, key):
+    """obj.key or obj[key] (an omegaconf / namespace config or a dict); KeyError when it has neither"""
+    if isinstance(obj, dict):
+        return obj[key]
+    try:
+        return getattr(obj, key)
+    except AttributeError:
+        raise KeyError(key)
+
+
+def _milestones(lr_steps, who):
+    steps = list(lr_steps)
+    if len(steps) > lib.MMFB_LR_MAX_MILESTONES:
+        raise ValueError("%s: at most %d lr_steps (got %d)" % (who, lib.MMFB_LR_MAX_MILESTONES, len(steps)))
+    out = []
+    for x in steps:
+        if isinstance(x, bool) or not (isinstance(x, numbers.Integral) or (isinstance(x, float) and x.is_integer())):
+            raise ValueError("%s: lr_steps must be whole update counts, got %r" % (who, x))
+        out.append(int(x))
+    return out
+
+
+def schedule_desc(kind, num_warmup_steps=None, num_training_steps=None, num_cycles=0.5, use_warmup=False, lr_steps=(),
+                  lr_ratio=0.1, warmup_iterations=0, warmup_factor=1.0):
+    """The lib.LrScheduleDesc of one of MMF's schedules (mmf/modules/schedulers.py), with the host's powers
+    lr_ratio ** i.  use_warmup counts only when it `is True`, as in the reference's tests."""
+    if kind not in _SCHEDULE_KINDS:
+        raise ValueError("DeviceLRScheduler: unknown schedule %r (MMF's are %s)" % (kind, ", ".join(_SCHEDULE_KINDS)))
+    d = lib.LrScheduleDesc()
+    d.kind = _SCHEDULE_KINDS[kind]
+    if kind in ("warmup_linear", "warmup_cosine"):
+        if num_warmup_steps is None or num_training_steps is None:
+            raise TypeError("DeviceLRScheduler(%r) needs num_warmup_steps and num_training_steps" % kind)
+        d.warmup_iterations, d.total_steps = int(num_warmup_steps), int(num_training_steps)
+        d.num_cycles = float(num_cycles)
+        return d
+    steps = _milestones(lr_steps, "DeviceLRScheduler(%r)" % kind)
+    d.use_warmup = 1 if use_warmup is True else 0
+    d.warmup_iterations = int(warmup_iterations) if use_warmup else 0
+    if d.use_warmup and d.warmup_iterations < 1:
+        raise ValueError("DeviceLRScheduler(%r): use_warmup needs warmup_iterations >= 1 (the reference divides by it)"
+                         % kind)
+    d.warmup_factor = float(warmup_factor)
+    d.n_lr_steps = len(steps)
+    for i, x in enumerate(steps):
+        d.lr_steps[i] = x
+    for i in range(len(steps) + 1):
+        d.ratio_pow[i] = float(lr_ratio ** i)          # pow(lr_ratio, idx) of the reference, on the host
+    return d
+
+
+class DeviceLRScheduler:
+    """MMF's learning-rate schedulers with LambdaLR's counter and arithmetic on the device, for a capturable B200AdamW:
+
+        sched = DeviceLRScheduler(opt, "warmup_linear", num_warmup_steps=2000, num_training_steps=88000)
+        ... opt.step(); sched.step()        # or GraphedStep(..., optimizer=opt, lr_scheduler=sched)
+
+    kind and the keyword arguments are those of the reference's schedulers (mmf/modules/schedulers.py): warmup_linear
+    and warmup_cosine (transformers' get_*_schedule_with_warmup: num_warmup_steps, num_training_steps, num_cycles),
+    multi_step (use_warmup, lr_steps, lr_ratio, warmup_iterations, warmup_factor) and pythia (lr_lambda_update over
+    the registered config's training.* values).  The counter is LambdaLR's last_epoch, an int64 on the device; step()
+    is one launch that advances it and writes every group's base_lr * f(last_epoch) into the fp64 group table the
+    optimizer's next step reads, so it can be captured.  As LambdaLR does on construction, the lr is the schedule at
+    step 0 before the first step().  The counter is separate from the AdamW step counts: it advances on updates that
+    GradScaler skips, as MMF's trainer steps its scheduler on every update.
+
+    LambdaLR's surface: step(), get_last_lr() (one device read), last_epoch (one device read), state_dict() and
+    load_state_dict(), which resumes at the saved counter in place (graphs captured with this scheduler stay valid).
+    The groups' "lr" in param_groups stays the base lr ("initial_lr"): the scheduled lr lives on the device.  One
+    schedule for all groups, as LambdaLR with one lambda."""
+
+    def __init__(self, optimizer, kind, **params):
+        if not isinstance(optimizer, B200AdamW) or not optimizer.capturable:
+            raise TypeError("DeviceLRScheduler: the optimizer must be mmf_b200.optim.B200AdamW(..., capturable=True), "
+                            "whose steps read the lr from the device table this scheduler writes; use torch's "
+                            "LambdaLR schedulers with other optimizers")
+        if optimizer._lr_sched is not None:
+            raise RuntimeError("DeviceLRScheduler: the optimizer already has a device scheduler attached")
+        if kind == "pythia":
+            if params:
+                raise TypeError("DeviceLRScheduler('pythia') reads training.* from the registered config, as the "
+                                "reference does; got arguments %s" % sorted(params))
+            cfg = registry.get("config")
+            if cfg is None:
+                raise RuntimeError("DeviceLRScheduler('pythia'): no config registered (registry.register('config', ...))")
+            tr = _cfg(cfg, "training")
+            params = {k: _cfg(tr, k) for k in ("use_warmup", "lr_steps", "lr_ratio", "warmup_iterations",
+                                                "warmup_factor")}
+        elif kind == "multi_step":
+            for k in ("use_warmup", "lr_steps", "lr_ratio", "warmup_factor") + \
+                    (("warmup_iterations",) if params.get("use_warmup") else ()):
+                if k not in params:
+                    raise TypeError("DeviceLRScheduler('multi_step') needs %s" % k)
+            w = params["warmup_iterations"] if params["use_warmup"] else 0
+            if not params["lr_steps"] or not w < params["lr_steps"][0]:
+                raise ValueError("DeviceLRScheduler('multi_step'): warmup_iterations must be below the first of lr_steps")
+        self.kind, self.params = kind, dict(params)
+        self.desc = schedule_desc(kind, **params)
+        self.optimizer = optimizer
+        dev = next((p.device for g in optimizer.param_groups for p in g["params"]), None)
+        if dev is None or dev.type != "cuda":
+            raise RuntimeError("DeviceLRScheduler: the optimizer's parameters must be on a CUDA device")
+        self.device = dev
+        self.base_lrs = [float(g.setdefault("initial_lr", g["lr"])) for g in optimizer.param_groups]
+        self.base_lr = _h2d(torch.tensor(self.base_lrs, dtype=torch.float64), dev)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=dev)
+        plan = optimizer._cap
+        if plan is not None and plan.groups.shape[0] == len(self.base_lrs):
+            self.table = plan.groups                   # graphs captured before this read this table: keep it
+        else:
+            self.table = torch.zeros(len(self.base_lrs), lib.ADAMW_GROUP_HP_DOUBLES, dtype=torch.float64, device=dev)
+        optimizer._lr_sched = self
+        self._launch(advance=False)
+
+    def _table_for(self, optimizer, device):
+        if self.table.shape[0] != len(optimizer.param_groups) or self.table.device != device:
+            raise RuntimeError("DeviceLRScheduler: the optimizer's parameter groups changed since the scheduler was "
+                               "built; build a new scheduler")
+        return self.table
+
+    def _launch(self, advance):
+        F.lr_schedule(self.counter, self.base_lr, self.table, self.desc, advance, lr_stride=lib.ADAMW_GROUP_HP_DOUBLES)
+
+    def step(self):
+        """advance the counter and write the next lr of every group, on the device (capturable)"""
+        self._launch(advance=True)
+
+    def refresh(self):
+        """rewrite the groups' lr from the current counter (after the counter was set in place)"""
+        self._launch(advance=False)
+
+    @property
+    def last_epoch(self):
+        return int(self.counter.item())
+
+    def get_last_lr(self):
+        """the lr of every group that the next optimizer step uses, read from the device"""
+        return self.table[:, 0].tolist()
+
+    def state_dict(self):
+        return {"kind": self.kind, "params": dict(self.params), "base_lrs": list(self.base_lrs),
+                "last_epoch": self.last_epoch}
+
+    def load_state_dict(self, state_dict):
+        if state_dict["kind"] != self.kind:
+            raise ValueError("DeviceLRScheduler.load_state_dict: a %r state for a %r scheduler"
+                             % (state_dict["kind"], self.kind))
+        if len(state_dict["base_lrs"]) != len(self.base_lrs):
+            raise ValueError("DeviceLRScheduler.load_state_dict: %d base lrs for %d groups"
+                             % (len(state_dict["base_lrs"]), len(self.base_lrs)))
+        self.base_lrs = [float(x) for x in state_dict["base_lrs"]]
+        _h2d(torch.tensor(self.base_lrs, dtype=torch.float64), self.device, out=self.base_lr)
+        _h2d(torch.tensor([int(state_dict["last_epoch"])], dtype=torch.int64), self.device, out=self.counter)
+        self.refresh()
+
+
+def _registered(kind, name):
+    def __init__(self, optimizer, *args, **kwargs):
+        if args:
+            raise TypeError("%s takes keyword arguments only (MMF's scheduler.params)" % name)
+        DeviceLRScheduler.__init__(self, optimizer, kind, **kwargs)
+    cls = type(name, (DeviceLRScheduler,), {"__init__": __init__, "__doc__": "DeviceLRScheduler(optimizer, %r, ...)"
+                                                                           % kind})
+    return registry.register_scheduler(kind)(cls)
+
+
+DeviceWarmupLinearScheduler = _registered("warmup_linear", "DeviceWarmupLinearScheduler")
+DeviceWarmupCosineScheduler = _registered("warmup_cosine", "DeviceWarmupCosineScheduler")
+DeviceMultiStepScheduler = _registered("multi_step", "DeviceMultiStepScheduler")
+DevicePythiaScheduler = _registered("pythia", "DevicePythiaScheduler")
