@@ -606,5 +606,7 @@ int64_t mmfb_launch_count(void);   /* number of kernels this library has launche
 #include "mmfb200_plan.h"
 /* the device update: learning-rate schedules and the fused non-finite check (mmfb_lr_schedule, mmfb_grad_*check) */
 #include "mmfb200_update.h"
+/* the capturable AdamW step gated per slot (mmfb_adamw_active, mmfb_adamw_hparams_active, mmfb_adamw_segments_active) */
+#include "mmfb200_active.h"
 
 #endif /* MMFB200_H_ */

@@ -359,6 +359,28 @@ int mmfb_adamw_segments(const mmfb_adamw_segments_args* args, mmfb_stream stream
   MMFB_REQUIRE_DEVICE();
   return adamw_segments(*args, reinterpret_cast<cudaStream_t>(stream));
 }
+int mmfb_adamw_active(const mmfb_adamw_args* args, const uint8_t* active, mmfb_stream stream) {
+  if (!args || !active) return set_error(MMFB_ERR_ARG, "mmfb_adamw_active: null pointer");
+  if (!args->hp_dev) return set_error(MMFB_ERR_ARG, "mmfb_adamw_active: active needs hp_dev (one byte per hp entry)");
+  if (misaligned_f32(args->loss_scale_dev) || misaligned_f32(args->found_inf))
+    return set_error(MMFB_ERR_ARG, "mmfb_adamw_active: loss_scale_dev and found_inf must be 4-byte aligned");
+  MMFB_REQUIRE_DEVICE();
+  return adamw(*args, reinterpret_cast<cudaStream_t>(stream), active);
+}
+int mmfb_adamw_hparams_active(const mmfb_adamw_hparams_args* args, const uint8_t* active, mmfb_stream stream) {
+  if (!args || !active) return set_error(MMFB_ERR_ARG, "mmfb_adamw_hparams_active: null pointer");
+  if (misaligned_f32(args->found_inf))
+    return set_error(MMFB_ERR_ARG, "mmfb_adamw_hparams_active: found_inf must be 4-byte aligned");
+  MMFB_REQUIRE_DEVICE();
+  return adamw_hparams(*args, reinterpret_cast<cudaStream_t>(stream), active);
+}
+int mmfb_adamw_segments_active(const mmfb_adamw_segments_args* args, const uint8_t* active, mmfb_stream stream) {
+  if (!args || !active) return set_error(MMFB_ERR_ARG, "mmfb_adamw_segments_active: null pointer");
+  if (misaligned_f32(args->loss_scale_dev) || misaligned_f32(args->found_inf))
+    return set_error(MMFB_ERR_ARG, "mmfb_adamw_segments_active: loss_scale_dev and found_inf must be 4-byte aligned");
+  MMFB_REQUIRE_DEVICE();
+  return adamw_segments(*args, reinterpret_cast<cudaStream_t>(stream), active);
+}
 int mmfb_grad_norm(const mmfb_grad_norm_args* args, mmfb_stream stream) {
   if (!args) return set_error(MMFB_ERR_ARG, "mmfb_grad_norm: null args");
   if (args->norm_type != 2.0f)

@@ -100,9 +100,10 @@ int compose(const mmfb_compose_args& a, cudaStream_t s);
 int scatter(const mmfb_scatter_args& a, cudaStream_t s);
 int cast_params(const float* in, void* out, int64_t n, cudaStream_t s);
 int relu_bwd(const void* dy, const void* y, void* dz, int64_t n, cudaStream_t s);
-int adamw(const mmfb_adamw_args& a, cudaStream_t s);
-int adamw_hparams(const mmfb_adamw_hparams_args& a, cudaStream_t s);
-int adamw_segments(const mmfb_adamw_segments_args& a, cudaStream_t s);
+// active: the per-slot gate of include/mmfb200_active.h (NULL: none, the ungated kernels)
+int adamw(const mmfb_adamw_args& a, cudaStream_t s, const uint8_t* active = nullptr);
+int adamw_hparams(const mmfb_adamw_hparams_args& a, cudaStream_t s, const uint8_t* active = nullptr);
+int adamw_segments(const mmfb_adamw_segments_args& a, cudaStream_t s, const uint8_t* active = nullptr);
 int grad_norm(const mmfb_grad_norm_args& a, float* found_inf, cudaStream_t s);
 int grad_check(const mmfb_grad_segment* segs, int n_segs, int n_blocks, double* flags, float* found_inf, cudaStream_t s);
 int lr_schedule(const mmfb_lr_schedule_args& a, cudaStream_t s);

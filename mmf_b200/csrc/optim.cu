@@ -15,6 +15,7 @@ struct AdamWDev {
   const mmfb_adamw_hp* hp;   // read only by the HP_DEV instantiations (mmfb_adamw_hparams' table)
   const float* loss_scale_dev;   // read only by the AMP instantiations (nullable there too)
   const float* found_inf;        // read only by the AMP instantiations (nullable there too)
+  const uint8_t* active;         // read only by the GATE instantiations: one byte per hp entry
 };
 
 // GradScaler's unscale factor of a loss scale S: (float)(1.0 / (double)S), as torch's _scale.double().reciprocal().float().
@@ -51,8 +52,10 @@ __device__ __forceinline__ void adamw_elem(float& p, float& m, float& v, float g
 // HP_DEV: the group's hyper-parameters come from the device table a.hp instead of the launch parameters.
 // AMP: loss scaling on the device - nothing is written when *found_inf is non-zero, and every gradient is first multiplied
 // by amp_inv_scale(loss_scale_dev) (each pointer nullable), then by the factor above: GradScaler.unscale_, then step().
-// The instantiations without any of the three are the kernels this file always had.
-template <int MODE, bool SCALE_DEV, bool HP_DEV, bool AMP>
+// GATE (with HP_DEV only): a block whose group g has active[g] == 0 reads and writes nothing, as torch.optim.AdamW skips
+// a parameter whose grad is None (include/mmfb200_active.h).
+// The instantiations without any of the four are the kernels this file always had.
+template <int MODE, bool SCALE_DEV, bool HP_DEV, bool AMP, bool GATE = false>
 __global__ void __launch_bounds__(256)
 adamw_kernel(const __grid_constant__ AdamWDev a) {
   griddep_launch();
@@ -62,6 +65,7 @@ adamw_kernel(const __grid_constant__ AdamWDev a) {
   const int64_t i = blk * 8;
   if (i >= a.n) return;
   const int gi = a.grp != nullptr ? a.grp[blk] : 0;
+  if (GATE && a.active[gi] == 0) return;
   float lr, wd, step, bc2s, b1, b2, eps;
   if (HP_DEV) {
     const mmfb_adamw_hp h = a.hp[gi];
@@ -103,7 +107,7 @@ adamw_kernel(const __grid_constant__ AdamWDev a) {
   }
 }
 
-int adamw(const mmfb_adamw_args& a, cudaStream_t s) {
+int adamw(const mmfb_adamw_args& a, cudaStream_t s, const uint8_t* active) {
   if (!a.param || !a.grad || !a.exp_avg || !a.exp_avg_sq) return set_error(MMFB_ERR_ARG, "adamw: null pointer");
   if (a.n <= 0 || (a.n % 8)) return set_error(MMFB_ERR_ARG, "adamw: n must be a positive multiple of 8 (got %lld)", (long long)a.n);
   if (a.n_groups < 1 || a.n_groups > MMFB_ADAMW_MAX_GROUPS)
@@ -122,10 +126,27 @@ int adamw(const mmfb_adamw_args& a, cudaStream_t s) {
   }
   d.b1 = a.beta1; d.b2 = a.beta2; d.eps = a.eps; d.gscale = a.grad_scale; d.gscale_dev = a.grad_scale_dev;
   d.hp = a.hp_dev;
-  d.loss_scale_dev = a.loss_scale_dev; d.found_inf = a.found_inf;
+  d.loss_scale_dev = a.loss_scale_dev; d.found_inf = a.found_inf; d.active = active;
   const int64_t blocks8 = a.n / 8;
   const unsigned grid = static_cast<unsigned>((blocks8 + 255) / 256);
   const bool amp = a.loss_scale_dev != nullptr || a.found_inf != nullptr;
+  if (active != nullptr) {
+    if (a.hp_dev == nullptr) return set_error(MMFB_ERR_ARG, "adamw_active: active needs hp_dev (one byte per hp entry)");
+    switch ((amp ? 4 : 0) + a.mode * 2 + (a.grad_scale_dev != nullptr ? 1 : 0)) {
+      case 0: MMFB_LAUNCH((adamw_kernel<0, false, true, false, true>), grid, 256, 0, s, d); break;
+      case 1: MMFB_LAUNCH((adamw_kernel<0, true, true, false, true>), grid, 256, 0, s, d); break;
+      case 2: MMFB_LAUNCH((adamw_kernel<1, false, true, false, true>), grid, 256, 0, s, d); break;
+      case 3: MMFB_LAUNCH((adamw_kernel<1, true, true, false, true>), grid, 256, 0, s, d); break;
+      case 4: MMFB_LAUNCH((adamw_kernel<0, false, true, true, true>), grid, 256, 0, s, d); break;
+      case 5: MMFB_LAUNCH((adamw_kernel<0, true, true, true, true>), grid, 256, 0, s, d); break;
+      case 6: MMFB_LAUNCH((adamw_kernel<1, false, true, true, true>), grid, 256, 0, s, d); break;
+      default: MMFB_LAUNCH((adamw_kernel<1, true, true, true, true>), grid, 256, 0, s, d); break;
+    }
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw_active launch: %s", cudaGetErrorString(e));
+    count_launch();
+    return MMFB_OK;
+  }
   const int variant = (amp ? 8 : 0) + a.mode * 4 + (a.grad_scale_dev != nullptr ? 2 : 0) + (a.hp_dev != nullptr ? 1 : 0);
   switch (variant) {
     case 0: MMFB_LAUNCH((adamw_kernel<0, false, false, false>), grid, 256, 0, s, d); break;
@@ -157,13 +178,15 @@ int adamw(const mmfb_adamw_args& a, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------------------------------
 // SKIP: a non-zero *found_inf makes the launch a no-op (no step count advances, the table keeps its values), as a
 // step that GradScaler skips does not count in torch's fused Adam.
+// GATE: a slot with active[s] == 0 is treated as a frozen one - its step count is neither read nor advanced and its
+// row gets step_size 0 - as torch.optim.AdamW leaves a parameter whose grad is None.
 constexpr int HP_THREADS = 256;
 
-template <bool SKIP>
+template <bool SKIP, bool GATE = false>
 __global__ void __launch_bounds__(HP_THREADS)
 adamw_hparams_kernel(const mmfb_adamw_group_hp* __restrict__ groups, const mmfb_adamw_slot* __restrict__ slots,
                      int64_t* __restrict__ steps, mmfb_adamw_hp* __restrict__ out, int n_slots, int mode,
-                     const float* __restrict__ found_inf) {
+                     const float* __restrict__ found_inf, const uint8_t* __restrict__ active) {
   griddep_launch();
   griddep_wait();
   if (SKIP && *found_inf != 0.0f) return;
@@ -173,7 +196,7 @@ adamw_hparams_kernel(const mmfb_adamw_group_hp* __restrict__ groups, const mmfb_
     mmfb_adamw_hp h;
     h.beta1 = __double2float_rn(g.beta1); h.beta2 = __double2float_rn(g.beta2); h.eps = __double2float_rn(g.eps);
     h.pad_ = 0.0f;
-    if (sl.flags & MMFB_ADAMW_SLOT_FROZEN) {
+    if ((sl.flags & MMFB_ADAMW_SLOT_FROZEN) || (GATE && active[s] == 0)) {
       h.lr = 0.0f; h.weight_decay = 0.0f; h.step_size = 0.0f; h.bc2_sqrt = 1.0f;
     } else {
       const int64_t t = steps[s] + 1;
@@ -196,19 +219,26 @@ adamw_hparams_kernel(const mmfb_adamw_group_hp* __restrict__ groups, const mmfb_
   }
 }
 
-int adamw_hparams(const mmfb_adamw_hparams_args& a, cudaStream_t s) {
+int adamw_hparams(const mmfb_adamw_hparams_args& a, cudaStream_t s, const uint8_t* active) {
   if (!a.groups || !a.slots || !a.step || !a.hp) return set_error(MMFB_ERR_ARG, "adamw_hparams: null pointer");
   if (a.n_slots < 1) return set_error(MMFB_ERR_ARG, "adamw_hparams: need at least one slot (got %d)", a.n_slots);
   if (a.mode != 0 && a.mode != 1) return set_error(MMFB_ERR_ARG, "adamw_hparams: mode must be 0 (transformers) or 1 (torch)");
   if ((reinterpret_cast<uintptr_t>(a.groups) | reinterpret_cast<uintptr_t>(a.step)) & 7 ||
       reinterpret_cast<uintptr_t>(a.slots) & 7 || reinterpret_cast<uintptr_t>(a.hp) & 15)
     return set_error(MMFB_ERR_ARG, "adamw_hparams: groups / slots / step must be 8-byte aligned, hp 16-byte aligned");
-  if (a.found_inf != nullptr)
+  if (active != nullptr) {
+    if (a.found_inf != nullptr)
+      MMFB_LAUNCH((adamw_hparams_kernel<true, true>), 1, HP_THREADS, 0, s, a.groups, a.slots, a.step, a.hp, a.n_slots,
+                  a.mode, a.found_inf, active);
+    else
+      MMFB_LAUNCH((adamw_hparams_kernel<false, true>), 1, HP_THREADS, 0, s, a.groups, a.slots, a.step, a.hp, a.n_slots,
+                  a.mode, a.found_inf, active);
+  } else if (a.found_inf != nullptr)
     MMFB_LAUNCH(adamw_hparams_kernel<true>, 1, HP_THREADS, 0, s, a.groups, a.slots, a.step, a.hp, a.n_slots, a.mode,
-                a.found_inf);
+                a.found_inf, active);
   else
     MMFB_LAUNCH(adamw_hparams_kernel<false>, 1, HP_THREADS, 0, s, a.groups, a.slots, a.step, a.hp, a.n_slots, a.mode,
-                a.found_inf);
+                a.found_inf, active);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw_hparams launch: %s", cudaGetErrorString(e));
   count_launch();
@@ -225,11 +255,12 @@ int adamw_hparams(const mmfb_adamw_hparams_args& a, cudaStream_t s) {
 constexpr int AS_THREADS = MMFB_ADAMW_SEGMENT_BLOCK / 8;
 static_assert(AS_THREADS == 256, "one 8-element group per thread");
 
-template <int MODE, bool SCALE_DEV, bool AMP>
+// GATE: a segment whose slot has active[slot] == 0 reads and writes nothing (include/mmfb200_active.h).
+template <int MODE, bool SCALE_DEV, bool AMP, bool GATE = false>
 __global__ void __launch_bounds__(AS_THREADS)
 adamw_segments_kernel(const mmfb_adamw_segment* __restrict__ segs, int n_segs, const mmfb_adamw_hp* __restrict__ hp,
                       float gscale, const float* __restrict__ gscale_dev, const float* __restrict__ loss_scale_dev,
-                      const float* __restrict__ found_inf) {
+                      const float* __restrict__ found_inf, const uint8_t* __restrict__ active) {
   __shared__ int s_seg;
   griddep_launch();
   griddep_wait();
@@ -245,6 +276,7 @@ adamw_segments_kernel(const mmfb_adamw_segment* __restrict__ segs, int n_segs, c
   }
   __syncthreads();
   const mmfb_adamw_segment sg = segs[s_seg];
+  if (GATE && active[sg.slot] == 0) return;
   const int lead = sg.head > 0 ? 8 - sg.head : 0;
   const int64_t start = (static_cast<int64_t>(b - sg.first_block) * AS_THREADS + threadIdx.x) * 8 - lead;
   if (start >= sg.n) return;
@@ -297,7 +329,7 @@ adamw_segments_kernel(const mmfb_adamw_segment* __restrict__ segs, int n_segs, c
   }
 }
 
-int adamw_segments(const mmfb_adamw_segments_args& a, cudaStream_t s) {
+int adamw_segments(const mmfb_adamw_segments_args& a, cudaStream_t s, const uint8_t* active) {
   if (!a.segments || !a.hp) return set_error(MMFB_ERR_ARG, "adamw_segments: null pointer");
   if (a.n_segments < 1 || a.n_blocks < 1)
     return set_error(MMFB_ERR_ARG, "adamw_segments: need at least one segment and one block (got %d, %d)", a.n_segments,
@@ -310,8 +342,20 @@ int adamw_segments(const mmfb_adamw_segments_args& a, cudaStream_t s) {
   const int variant = (amp ? 4 : 0) + a.mode * 2 + (a.grad_scale_dev != nullptr ? 1 : 0);
 #define MMFB_AS_LAUNCH(MODE, SCALE_DEV, AMP)                                                                       \
   MMFB_LAUNCH((adamw_segments_kernel<MODE, SCALE_DEV, AMP>), a.n_blocks, AS_THREADS, 0, s, a.segments, a.n_segments, \
-              a.hp, a.grad_scale, a.grad_scale_dev, a.loss_scale_dev, a.found_inf)
-  switch (variant) {
+              a.hp, a.grad_scale, a.grad_scale_dev, a.loss_scale_dev, a.found_inf, active)
+#define MMFB_AS_GATED(MODE, SCALE_DEV, AMP)                                                                          \
+  MMFB_LAUNCH((adamw_segments_kernel<MODE, SCALE_DEV, AMP, true>), a.n_blocks, AS_THREADS, 0, s, a.segments,          \
+              a.n_segments, a.hp, a.grad_scale, a.grad_scale_dev, a.loss_scale_dev, a.found_inf, active)
+  if (active != nullptr) switch (variant) {
+    case 0: MMFB_AS_GATED(0, false, false); break;
+    case 1: MMFB_AS_GATED(0, true, false); break;
+    case 2: MMFB_AS_GATED(1, false, false); break;
+    case 3: MMFB_AS_GATED(1, true, false); break;
+    case 4: MMFB_AS_GATED(0, false, true); break;
+    case 5: MMFB_AS_GATED(0, true, true); break;
+    case 6: MMFB_AS_GATED(1, false, true); break;
+    default: MMFB_AS_GATED(1, true, true); break;
+  } else switch (variant) {
     case 0: MMFB_AS_LAUNCH(0, false, false); break;
     case 1: MMFB_AS_LAUNCH(0, true, false); break;
     case 2: MMFB_AS_LAUNCH(1, false, false); break;
@@ -322,6 +366,7 @@ int adamw_segments(const mmfb_adamw_segments_args& a, cudaStream_t s) {
     default: MMFB_AS_LAUNCH(1, true, true); break;
   }
 #undef MMFB_AS_LAUNCH
+#undef MMFB_AS_GATED
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MMFB_ERR_CUDA, "adamw_segments launch: %s", cudaGetErrorString(e));
   count_launch();

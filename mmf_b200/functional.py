@@ -789,8 +789,18 @@ def _req_scalar(t, what, name):
     return t.data_ptr()
 
 
+def _req_active(active, n_slots, what):
+    """the per-slot gate of include/mmfb200_active.h: None or a contiguous uint8 CUDA tensor [n_slots]"""
+    if active is None:
+        return None
+    if not torch.is_tensor(active) or not active.is_cuda or active.dtype != torch.uint8 or active.dim() != 1 or \
+            not active.is_contiguous() or active.numel() != n_slots:
+        raise ValueError("%s: active must be a contiguous uint8 CUDA tensor with one entry per slot (%d)" % (what, n_slots))
+    return ctypes.c_void_p(active.data_ptr())
+
+
 def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, grad_scale=1.0, group_of_block=None,
-          param_bf16=None, grad_scale_dev=None, hp_dev=None, loss_scale_dev=None, found_inf=None):
+          param_bf16=None, grad_scale_dev=None, hp_dev=None, loss_scale_dev=None, found_inf=None, active=None):
     """One fused AdamW step over flat fp32 buffers (staged, include/mmfb200.h: mmfb_adamw).
     groups: list (<= 8) of dicts {lr, weight_decay, step_size, bc2_sqrt}; group_of_block: uint8 [n/8] or None;
     grad_scale_dev: None or a one-element fp32 CUDA tensor (grad_norm's clip coefficient) multiplied into grad_scale when
@@ -798,7 +808,11 @@ def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, 
     every group's hyper-parameters and beta1 / beta2 / eps from it, and `groups` may be None.
     loss_scale_dev, found_inf: None or one-element fp32 CUDA tensors (GradScaler's scale and non-finite flag): the
     gradients are first multiplied by fp32(1 / fp64(scale)), as GradScaler.unscale_ does, and a non-zero found_inf makes
-    the launch write nothing."""
+    the launch write nothing.
+    active: None or a uint8 CUDA tensor with one entry per row of hp_dev (include/mmfb200_active.h: mmfb_adamw_active);
+    the blocks of a group whose entry is 0 read and write nothing."""
+    if active is not None and hp_dev is None:
+        raise ValueError("adamw: active gates the rows of hp_dev; pass hp_dev as well")
     for t, n in ((param, "param"), (grad, "grad"), (exp_avg, "exp_avg"), (exp_avg_sq, "exp_avg_sq")):
         _req(t, torch.float32, n)
         if not t.is_contiguous() or t.numel() != param.numel():
@@ -831,7 +845,11 @@ def adamw(param, grad, exp_avg, exp_avg_sq, groups, *, beta1, beta2, eps, mode, 
         a.grad_scale_dev = grad_scale_dev.data_ptr()
     a.loss_scale_dev = _req_scalar(loss_scale_dev, "adamw", "loss_scale_dev")
     a.found_inf = _req_scalar(found_inf, "adamw", "found_inf")
-    check(LIB.mmfb_adamw(ctypes.byref(a), _stream_ptr()))
+    gate = _req_active(active, n_groups, "adamw")
+    if gate is None:
+        check(LIB.mmfb_adamw(ctypes.byref(a), _stream_ptr()))
+    else:
+        check(LIB.mmfb_adamw_active(ctypes.byref(a), gate, _stream_ptr()))
 
 
 def _req_hp(hp, what):
@@ -841,12 +859,14 @@ def _req_hp(hp, what):
                          % (what, lib.ADAMW_HP_FLOATS))
 
 
-def adamw_hparams(groups, slots, step, hp, mode, found_inf=None):
+def adamw_hparams(groups, slots, step, hp, mode, found_inf=None, active=None):
     """Advance the step counts and write the AdamW hyper-parameter table on the device (include/mmfb200.h:
     mmfb_adamw_hparams).  groups: fp64 CUDA [n_groups, 5] (lr, weight_decay, beta1, beta2, eps); slots: the device
     table of adamw_slot_table; step: int64 CUDA [n_slots], advanced by one for every slot that is not frozen; hp: fp32
     CUDA [n_slots, 8], overwritten.  found_inf: None or a one-element fp32 CUDA tensor; when it is non-zero the launch
-    changes nothing (a step GradScaler skips does not count).  Nothing is read on the host."""
+    changes nothing (a step GradScaler skips does not count).  Nothing is read on the host.
+    active: None or a uint8 CUDA tensor [n_slots] (include/mmfb200_active.h: mmfb_adamw_hparams_active); a slot whose
+    entry is 0 keeps its step count and gets a frozen slot's row."""
     if groups.dtype != torch.float64 or groups.dim() != 2 or groups.shape[1] != lib.ADAMW_GROUP_HP_DOUBLES or \
             not groups.is_contiguous():
         raise ValueError("adamw_hparams: groups must be a contiguous fp64 tensor [n_groups, %d]" % lib.ADAMW_GROUP_HP_DOUBLES)
@@ -862,7 +882,11 @@ def adamw_hparams(groups, slots, step, hp, mode, found_inf=None):
     a.groups, a.slots, a.step, a.hp = groups.data_ptr(), slots.data_ptr(), step.data_ptr(), hp.data_ptr()
     a.n_slots, a.mode = step.numel(), int(mode)
     a.found_inf = _req_scalar(found_inf, "adamw_hparams", "found_inf")
-    check(LIB.mmfb_adamw_hparams(ctypes.byref(a), _stream_ptr()))
+    gate = _req_active(active, step.numel(), "adamw_hparams")
+    if gate is None:
+        check(LIB.mmfb_adamw_hparams(ctypes.byref(a), _stream_ptr()))
+    else:
+        check(LIB.mmfb_adamw_hparams_active(ctypes.byref(a), gate, _stream_ptr()))
 
 
 def adamw_slot_table(slots, device):
@@ -919,10 +943,12 @@ def adamw_segment_table(segments):
     return AdamWSegmentTable(host.to(segments[0][0].device, non_blocking=True), rows, n_blocks)
 
 
-def adamw_segments(table, hp, *, mode, grad_scale=1.0, grad_scale_dev=None, loss_scale_dev=None, found_inf=None):
+def adamw_segments(table, hp, *, mode, grad_scale=1.0, grad_scale_dev=None, loss_scale_dev=None, found_inf=None,
+                   active=None):
     """One AdamW launch over every tensor of `table` (include/mmfb200.h: mmfb_adamw_segments), each with the
     hyper-parameters of its slot in hp (fp32 CUDA [slots, 8], written by adamw_hparams).  Element for element the
-    arithmetic of adamw; grad_scale_dev, loss_scale_dev and found_inf as there."""
+    arithmetic of adamw; grad_scale_dev, loss_scale_dev and found_inf as there.  active: None or a uint8 CUDA tensor
+    with one entry per row of hp (mmfb_adamw_segments_active); a segment whose slot's entry is 0 is left alone."""
     _req_hp(hp, "adamw_segments")
     a = lib.AdamWSegmentsArgs()
     a.segments, a.n_segments, a.n_blocks = table.segments.data_ptr(), len(table.rows), table.n_blocks
@@ -933,7 +959,11 @@ def adamw_segments(table, hp, *, mode, grad_scale=1.0, grad_scale_dev=None, loss
         a.grad_scale_dev = grad_scale_dev.data_ptr()
     a.loss_scale_dev = _req_scalar(loss_scale_dev, "adamw_segments", "loss_scale_dev")
     a.found_inf = _req_scalar(found_inf, "adamw_segments", "found_inf")
-    check(LIB.mmfb_adamw_segments(ctypes.byref(a), _stream_ptr()))
+    gate = _req_active(active, hp.shape[0], "adamw_segments")
+    if gate is None:
+        check(LIB.mmfb_adamw_segments(ctypes.byref(a), _stream_ptr()))
+    else:
+        check(LIB.mmfb_adamw_segments_active(ctypes.byref(a), gate, _stream_ptr()))
 
 
 class GradNormTable:

@@ -466,15 +466,46 @@ class GraphedTaskSteps:
     optimizer step; step the optimizer only through this object while it is in use.  The warm-up steps are undone.
     lr_scheduler: a DeviceLRScheduler on the optimizer, stepped inside every task's graph after its optimizer step, as
     in GraphedStep; all graphs advance its one device counter, which warm-up and capture leave as they found it.
+    scaler: a torch.amp.GradScaler (needs optimizer=), MMF's fp16 update as in GraphedStep: each task's graph runs
+    scaler.scale(loss).backward(), the clip at max_grad_norm times the device scale (or the fused check with
+    B200AdamW(..., fused_inf_check=True)), scaler.step, scaler.update and the scheduler.  Warm-up and capture leave the
+    scaler's scale and growth tracker as they found them.
+    update_frequency: K > 1 (needs optimizer=) accumulates K calls and updates once, as MMF's
+    training.update_frequency does; the loss is not divided by K.  The micro-batches of a group draw their tasks
+    independently, so the update cannot know on the host at capture which heads they reach: one micro-batch graph per
+    task (dropout epoch, forward, the - scaled - backward adding into the shared gradient buffers, and its task's
+    slots marked in the optimizer's per-slot gate) and one update graph over the union of what the tasks reach
+    (optimizer.gated_plan(): clip, step or scaler.step and scaler.update, the scheduler, then the gradients and the
+    gate zeroed) are captured in the shared pool.  A slot no micro-batch of the group marked is left as torch's AdamW
+    leaves a parameter whose grad is None: values, moments and step count.  Each call draws on the host, replays its
+    task's micro graph and returns that micro-batch's loss; the K-th call, or finish_update() after a partial group,
+    replays the update.  `pending` counts the micro-batches since the last update.  `.grad` is bound for the
+    parameters the group's tasks reached so far (after an update, those of the group just applied; the update graph
+    has zeroed them for the next group) and None for the others.  A pack parameter group that one task reaches only
+    in part cannot be gated as one slot and is refused at capture.
     Skip-padding and pack_streams encoders are refused as by GraphedStep without static_rows."""
 
-    def __init__(self, model, loss_fn, example_batch, warmup=3, optimizer=None, max_grad_norm=None, lr_scheduler=None):
+    def __init__(self, model, loss_fn, example_batch, warmup=3, optimizer=None, max_grad_norm=None, lr_scheduler=None,
+                 scaler=None, update_frequency=1):
         if not callable(getattr(model, "draw", None)) or not getattr(model, "draws_key", None) or \
                 not getattr(model, "tasks", None):
             raise TypeError("GraphedTaskSteps: the model must define draw(sample_list, task=None), draws_key and tasks; "
                             "capture a model that draws nothing on the host with GraphedStep")
         _check_optimizer("GraphedTaskSteps", optimizer, max_grad_norm)
         _check_scheduler("GraphedTaskSteps", optimizer, lr_scheduler)
+        if scaler is not None and optimizer is None:
+            raise ValueError("GraphedTaskSteps: scaler= unscales and skips inside the captured optimizer step; pass "
+                             "optimizer=B200AdamW(..., capturable=True) as well, or scale and step eagerly after each "
+                             "replay")
+        if not isinstance(update_frequency, numbers.Integral) or isinstance(update_frequency, bool) or \
+                update_frequency < 1:
+            raise ValueError("GraphedTaskSteps: update_frequency must be a positive int (MMF's "
+                             "training.update_frequency), got %r" % (update_frequency,))
+        if update_frequency > 1 and optimizer is None:
+            raise ValueError("GraphedTaskSteps: update_frequency=%d accumulates gradients over %d calls and updates "
+                             "inside the captured optimizer step; pass optimizer=B200AdamW(..., capturable=True) as "
+                             "well (without one, every replay starts from fresh gradients)"
+                             % (update_frequency, update_frequency))
         _check_runners("GraphedTaskSteps", model, False)
         for m in model.modules():
             if m is not model and getattr(m, "graph_capturable", True) is False and \
@@ -483,9 +514,13 @@ class GraphedTaskSteps:
                                    % (type(m).__name__, getattr(m, "graph_refusal", "does work on the host in every forward")))
         self.model, self.loss_fn = model, loss_fn
         self.optimizer, self.max_grad_norm, self.lr_scheduler = optimizer, max_grad_norm, lr_scheduler
+        self.scaler, self.update_frequency = scaler, int(update_frequency)
+        self.pending = 0          # micro-batches accumulated since the last update (update_frequency > 1)
         self.tasks = list(dict.fromkeys(model.tasks))
         self.task = None
         state = (torch.get_rng_state(), np.random.get_state(), random.getstate())
+        saved_scaler = _save_scaler(scaler) if scaler is not None else None
+        saved_counter = lr_scheduler.counter.clone() if lr_scheduler is not None else None
         try:
             with _static_rows_context():
                 self._capture(example_batch, warmup)
@@ -493,6 +528,10 @@ class GraphedTaskSteps:
             torch.set_rng_state(state[0])
             np.random.set_state(state[1])
             random.setstate(state[2])
+        if scaler is not None:                              # undo the warm-up updates (the graphs read these in place)
+            _restore_scaler(scaler, saved_scaler)
+        if lr_scheduler is not None:
+            _restore_scheduler(lr_scheduler, saved_counter)
 
     def _batch(self, task):
         """a fresh top level over the static inputs (the forward adds and replaces keys) with the task's static draws"""
@@ -512,11 +551,13 @@ class GraphedTaskSteps:
         self.epoch = F.dropout_epoch(dev, create=True)
         params = list(dict.fromkeys(model.parameters()))
         saved = _save_optimizer(opt) if opt is not None else None
-        saved_counter = self.lr_scheduler.counter.clone() if self.lr_scheduler is not None else None
         self.grads, self.used, self.graphs, self.losses, self.plans, self._keep = {}, {}, {}, {}, {}, []
         pool = None
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
+        if self.update_frequency > 1:
+            self._capture_accumulating(params, saved, dev, side, warmup)
+            return
         for t in self.tasks:
             with torch.cuda.stream(side):
                 model.zero_grad(set_to_none=True)          # which parameters task t reaches: those that get a .grad
@@ -551,8 +592,6 @@ class GraphedTaskSteps:
             for i, p in enumerate(params):
                 if p in opt.state:
                     opt.state[p]["step"] = self.steps[i]
-            if self.lr_scheduler is not None:
-                _restore_scheduler(self.lr_scheduler, saved_counter)
             torch.cuda.synchronize(dev)
         self._bind_grads(self.tasks[-1])
 
@@ -576,27 +615,94 @@ class GraphedTaskSteps:
         to_dev = lambda v: torch.tensor(v, dtype=torch.int64).to(plan.device)
         return to_dev(slot_param), to_dev([s for _, s in written]), to_dev([i for i, _ in written])
 
-    def _bind_grads(self, task):
+    def _capture_accumulating(self, params, saved, dev, side, warmup):
+        """update_frequency > 1: find what each task reaches, bind the union's gradients to shared buffers, build the
+        optimizer's gated plan over them, warm up, then capture one micro-batch graph per task and the update graph in
+        one pool.  Every .grad stays bound to its buffer during capture, so each backward adds in place."""
+        model, opt = self.model, self.optimizer
+        with torch.cuda.stream(side):
+            for t in self.tasks:                           # which parameters task t reaches: those that get a .grad
+                model.zero_grad(set_to_none=True)
+                self._step(self._batch(t), update=False)
+                self.used[t] = [p for p in params if p.grad is not None]
+                for p in self.used[t]:
+                    self.grads.setdefault(p, p.grad)
+            self._bind_grads(self.grads)
+            torch._foreach_zero_(list(self.grads.values()))
+            self._plan = plan = opt.gated_plan()
+            self._marks = {t: self._task_slots(plan, t) for t in self.tasks}
+            for _ in range(max(1, warmup)):            # lazy state, the clip table, the gated launches
+                for t in self.tasks:
+                    self._micro(t)
+                self._update()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        _restore_optimizer(opt, saved)
+        torch._foreach_zero_(list(self.grads.values()))
+        plan.active.zero_()
+        torch.cuda.synchronize(dev)
+        pool = None
+        for t in self.tasks:
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, pool=pool, stream=side):
+                self.losses[t] = self._micro(t)
+            pool = graph.pool()
+            self.graphs[t] = graph
+        self.update_graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.update_graph, pool=pool, stream=side):
+            self._update()
+        self._keep.append(opt._clip_table)                 # the update graph reads its device table
+        self._reached = set()
+        self._bind_grads(())
+
+    def _task_slots(self, plan, task):
+        """the gated plan's slots task reaches, as a device index tensor; a pack slot must be reached whole"""
+        used = {id(p) for p in self.used[task]}
+        members = {}
+        for p in self.grads:
+            members.setdefault(plan.slot_of[id(p)], []).append(id(p))
+        slots = sorted({plan.slot_of[i] for i in used})
+        for s in slots:
+            if not all(i in used for i in members[s]):
+                raise RuntimeError("GraphedTaskSteps: task %r reaches only part of a parameter group of an engine pack, "
+                                   "which update_frequency > 1 gates as one slot; use update_frequency=1" % task)
+        return torch.tensor(slots, dtype=torch.int64).to(plan.device)
+
+    def _micro(self, task):
+        """one micro-batch of task: dropout epoch, forward, (scaled) backward into the bound gradients, its slots
+        marked in the gate"""
+        self.epoch.add_(1)
+        loss = self._step(self._batch(task), update=False)
+        self._plan.active.index_fill_(0, self._marks[task], 1)
+        return loss
+
+    def _update(self):
+        """clip, step (or scaler.step and scaler.update), the scheduler, then the gradients and the gate zeroed"""
+        self._optimizer_step()
+        torch._foreach_zero_(list(self.grads.values()))
+        self._plan.active.zero_()
+
+    def _bind_grads(self, reached):
+        """reached: a task (its parameters get their shared gradient) or a collection of parameters"""
         for p in self.grads:
             p.grad = None
-        for p in self.used[task]:
+        for p in (self.used[reached] if isinstance(reached, str) else reached):
             p.grad = self.grads[p]
 
-    def _step(self, batch, counts=None):
+    # GraphedStep's backward and update sequence (they read scaler, optimizer, max_grad_norm and lr_scheduler)
+    _backward = GraphedStep._backward
+    _optimizer_step = GraphedStep._optimizer_step
+
+    def _step(self, batch, counts=None, update=True):
         loss = self.loss_fn(batch)
-        loss.backward()
-        opt = self.optimizer
-        if opt is not None:
-            if self.max_grad_norm is not None:
-                opt.clip_grad_norm(self.max_grad_norm)
+        self._backward(loss)
+        if self.optimizer is not None and update:
             if counts is not None:                         # this graph's step counts from the shared table ...
                 plan, gather, slots, idx = counts
                 plan.step.copy_(self.steps.index_select(0, gather))
-            opt.step()
+            self._optimizer_step()
             if counts is not None:                         # ... and back
                 self.steps.index_copy_(0, idx, plan.step.index_select(0, slots))
-            if self.lr_scheduler is not None:
-                self.lr_scheduler.step()
         return loss
 
     def __call__(self, batch=None):
@@ -605,12 +711,33 @@ class GraphedTaskSteps:
         probe = dict(self.static)
         task = self.model.draw(probe)
         _copy_into(self.draws[task], probe[self.model.draws_key])
+        self.task = task
+        if self.update_frequency > 1:
+            self.graphs[task].replay()
+            self._reached.update(self.used[task])
+            self.pending += 1
+            if self.pending == self.update_frequency:
+                self.finish_update()
+            else:
+                self._bind_grads(self._reached)
+            return self.losses[task]
         if self.optimizer is not None:
             self.optimizer.stage_hparams(self.plans[task])
         self.graphs[task].replay()
         self._bind_grads(task)
-        self.task = task
         return self.losses[task]
+
+    def finish_update(self):
+        """update_frequency > 1: replay the update for the micro-batches accumulated since the last one, with the groups'
+        current hyper-parameters; a call does this on its own on the update_frequency-th micro-batch, so this is for a
+        partial group, MMF's last update of a run.  Nothing happens when no micro-batch is pending."""
+        if not self.pending:
+            return
+        self.optimizer.stage_hparams(self._plan)
+        self.update_graph.replay()
+        self._bind_grads(self._reached)
+        self._reached = set()
+        self.pending = 0
 
 
 def _save_optimizer(opt):

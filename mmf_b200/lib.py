@@ -276,6 +276,8 @@ def _load():
     lib.mmfb_grad_check.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
                                     ctypes.c_void_p]
     lib.mmfb_lr_schedule.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+    for name in ("mmfb_adamw_active", "mmfb_adamw_hparams_active", "mmfb_adamw_segments_active"):
+        getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
     for name in ("mmfb_ot_fwd", "mmfb_ot_bwd"):
         getattr(lib, name).argtypes = [ctypes.c_void_p, ctypes.c_void_p]
     return lib

@@ -93,14 +93,19 @@ def _h2d(t, device, out=None):
 
 class _CapturablePlan:
     """What a capturable step launches: the slots (a pack's parameter group, or a loose parameter) with their device
-    step counts and hyper-parameter table, the pack launches, and the segment table of the loose parameters."""
+    step counts and hyper-parameter table, the pack launches, and the segment table of the loose parameters.
+    `active` (set by B200AdamW.gated_plan) is the per-slot gate of include/mmfb200_active.h: a uint8 CUDA tensor with
+    one entry per slot, read by every launch of the step; a slot whose entry is 0 is stepped as a parameter whose grad is
+    None.  Without it the step launches the ungated kernels."""
 
     def __init__(self, layout_key, device, mode):
         self.layout_key, self.device, self.mode = layout_key, device, mode
         self.packs = []          # (pack, flat state entry, first slot, slots, betas, eps)
         self.loose = []          # (param, slot)
         self.slots = []          # (group index, flags)
+        self.slot_of = {}        # id(param) -> its slot
         self.table_key, self.table = None, None
+        self.active = None
 
 
 def _reference_arithmetic():
@@ -507,6 +512,7 @@ class B200AdamW(torch.optim.Optimizer):
             plan.loose.append((p, len(plan.slots)))
             plan.slots.append((group_of[id(p)], cb(group_of[id(p)])))
             counts.append(steps[id(p)])
+        plan.slot_of = slot_of
         plan.step = _h2d(torch.tensor(counts, dtype=torch.int64), device)
         plan.slot_table = F.adamw_slot_table(plan.slots, device)
         plan.hp = torch.zeros(len(plan.slots), lib.ADAMW_HP_FLOATS, dtype=torch.float32, device=device)
@@ -517,6 +523,20 @@ class B200AdamW(torch.optim.Optimizer):
                                       device=device)
         for p in stepped:
             self.state[p]["step"] = plan.step[slot_of[id(p)]]
+        return plan
+
+    def gated_plan(self):
+        """The plan of the next capturable step, over every parameter that has a gradient now, with a per-slot gate
+        `plan.active` (zeroed, uint8 [slots]) that every launch of its steps reads: only the slots whose entry is
+        non-zero are stepped.  Bind the gradients of every parameter a later step may update (the union of what the
+        micro-batches reach) before calling this; each step then updates the slots that were marked, e.g. by
+        `plan.active.index_fill_(0, slots, 1)` inside a captured micro-batch, and `plan.slot_of[id(p)]` gives a
+        parameter's slot.  Not during capture."""
+        plan = self._capturable_plan()
+        if plan is None:
+            raise RuntimeError("B200AdamW.gated_plan: no parameter of the optimizer has a gradient")
+        if plan.active is None:
+            plan.active = torch.zeros(len(plan.slots), dtype=torch.uint8, device=plan.device)
         return plan
 
     def _group_values(self):
@@ -548,14 +568,16 @@ class B200AdamW(torch.optim.Optimizer):
             return
         if not _capturing():
             self.stage_hparams(plan)
+        gate = (lambda s0, n: {}) if plan.active is None else (lambda s0, n: {"active": plan.active[s0:s0 + n]})
         F.adamw_hparams(plan.groups, plan.slot_table, plan.step, plan.hp, plan.mode,
-                        **({"found_inf": amp["found_inf"]} if "found_inf" in amp else {}))
+                        **({"found_inf": amp["found_inf"]} if "found_inf" in amp else {}), **gate(0, len(plan.slots)))
         for pack, ent, s0, n, betas, eps in plan.packs:
             F.adamw(pack.master, pack.grad, ent["m"], ent["v"], None, beta1=betas[0], beta2=betas[1], eps=eps,
                     mode=plan.mode, grad_scale=grad_scale, group_of_block=ent["groups"], hp_dev=plan.hp[s0:s0 + n],
-                    **clip, **amp)
+                    **clip, **amp, **gate(s0, n))
         if plan.loose:
-            F.adamw_segments(plan.table, plan.hp, mode=plan.mode, grad_scale=grad_scale, **clip, **amp)
+            F.adamw_segments(plan.table, plan.hp, mode=plan.mode, grad_scale=grad_scale, **clip, **amp,
+                             **gate(0, len(plan.slots)))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
